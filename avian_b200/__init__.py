@@ -1,4 +1,4 @@
-"""avian_b200 — B200-native (sm_100a) replacement for the avian3d substep hot path.
+"""avian_b200 — H100-native (sm_90a) replacement for the avian3d substep hot path.
 
 Hot path = semi-implicit integration (IntegratorPlugin), sweep-and-prune broad phase (BroadPhasePlugin) and
 the TGS-soft contact + XPBD joint solve (SolverPlugin / XpbdSolverPlugin) of avianphysics/avian, behind the

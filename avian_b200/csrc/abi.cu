@@ -70,8 +70,8 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
         if ((e = cudaSetDevice(config->device)) != cudaSuccess) return create_fail(AVN_ERR_CUDA, cudaGetErrorString(e));
         cudaDeviceProp prop;
         if ((e = cudaGetDeviceProperties(&prop, config->device)) != cudaSuccess) return create_fail(AVN_ERR_CUDA, cudaGetErrorString(e));
-        if (prop.major != 10)
-            return create_fail(AVN_ERR_UNSUPPORTED, std::string("kernels are built for sm_100a only; device is ") + prop.name + " (sm_" +
+        if (prop.major != 9 || prop.minor != 0)
+            return create_fail(AVN_ERR_UNSUPPORTED, std::string("kernels are built for sm_90a only; device is ") + prop.name + " (sm_" +
                                                         std::to_string(prop.major) + std::to_string(prop.minor) + ")");
         auto ctx = std::make_unique<AvnContext>();
         ctx->device = config->device;

@@ -1,4 +1,4 @@
-// Device math for the avian_b200 kernels (sm_100a).
+// Device math for the avian_b200 kernels (sm_90a).
 //
 // Every routine evaluates the same floating-point expression tree as the glam / glam_matrix_extras routine
 // the reference calls at that point (the call sites are cited next to each function), because the parity bar

@@ -338,7 +338,7 @@ class Broadphase final : public BroadphaseBase {
     AvnStatus finish_download();        // persistent order + timings to the host
     const uint64_t* ext_existing_ = nullptr; uint64_t ext_existing_mask_ = 0;   // the contact store's pair set (device)
 
-    // The front part of a run is a fixed sequence of ~25 small launches (3-15 us each): captured once into a CUDA graph and replayed as long
+    // The front part of a run is a fixed sequence of ~25 small launches: captured once into a CUDA graph and replayed as long
     // as the interval count and every buffer address stay the same (buffers are grow-only, so a steady scene replays forever).
     struct GraphKey {
         int n = -1;
@@ -361,7 +361,7 @@ class Broadphase final : public BroadphaseBase {
 
     cudaStream_t stream_;
     ErrorSink* err_;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     cudaEvent_t ev0_, ev1_;
     uint64_t* h_total_ = nullptr;
     AvnTimings tm_{};

@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(256) colour_rounds_kernel(GraphRows g, const u
 // The same rounds for a SMALL number of changed edges (the steady state: a few thousand contacts start or stop touching per step) inside ONE
 // thread-block cluster: 8 CTAs x 1024 threads, every thread keeps its (at most 4) edges in registers, the two barriers of a round are hardware
 // cluster barriers instead of grid-wide ones, and "is anything left" is an OR through distributed shared memory.  A round costs the L2 round
-// trips of its atomics and loads (~2.5 us) instead of two cooperative grid barriers on top of them.
+// trips of its atomics and loads instead of two cooperative grid barriers on top of them.
 constexpr int CL_BLOCKS = 8, CL_THREADS = 1024, CL_ITEMS = 4;
 constexpr uint32_t CL_MAX = uint32_t(CL_BLOCKS) * CL_THREADS * CL_ITEMS;
 __global__ void __launch_bounds__(CL_THREADS) colour_rounds_cluster_kernel(GraphRows g, const uint32_t* __restrict__ list) {
@@ -1094,7 +1094,7 @@ class Contacts final : public ContactsBase {
     ResidentGraph graph_{};
     uint64_t table_mask_ = 0;
     uint32_t hw_ = 0, live_n_ = 0, n_bodies_ = 0, n_colliders_ = 0;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     bool configured_ = false, have_fr_ = false, have_re_ = false, table_dirty_ = true, use_cluster_ = true;
 };
 

@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(1024) rs_scan(uint32_t* data, int len) {
 // 32 consecutive keys, so (warp, round, lane) order == input order; ranks come from match_any + popc.
 // FUSED = the (digit, block) offsets are computed here from the raw per-block histograms instead of by a separate rs_scan launch:
 // offset(d, blk) = sum of all counters of the digits below d + the counters of digit d in the blocks before blk.  Every block redoes the
-// 256 x nblocks row sums (L2-resident, 49 KB at 100k keys), which is cheaper than a 12 us single-block scan kernel and its launch gap as
+// 256 x nblocks row sums (L2-resident, 49 KB at 100k keys), which is cheaper than a single-block scan kernel and its launch gap as
 // long as nblocks is small; the host keeps the scan kernel above RS_FUSE_MAX_BLOCKS.
 constexpr int RS_FUSE_MAX_BLOCKS = 128;
 template <class K, bool FUSED>

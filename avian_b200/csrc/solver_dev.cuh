@@ -13,6 +13,7 @@
 //            4+3k {anchor1.xyz, initial_separation} 5+3k {anchor2.xyz, normal effective_mass}
 //            6+3k {K1, K2, K3 (tangent effective inverse mass), normal_speed}
 //            pcr[4][Mpad] records {normal impulse, total normal impulse, tangent impulse.x, .y} of point k  <- the only constraint data written in the loop
+//            (the spare lanes of vel, dlt and the f32 impulse records carry the wavefront schedule's sequence tags, wave32_dev.cuh)
 //   joints   jnt[14][Jpad] planes in level-schedule order (see JP_* below).
 #pragma once
 #include <cuda_pipeline.h>
@@ -27,9 +28,9 @@ enum { CP_N = 0, CP_T1 = 1, CP_TV = 2, CP_IDX = 3, CP_PT0 = 4, CP_PLANES = CP_PT
 // immutable rows of point k in CP_PT0 + 3k + {0: A, 1: B, 2: D}
 #define CP_ROW(k, r) (CP_PT0 + 3 * (k) + (r))
 // The MUTABLE impulses {lambda_n, sum lambda_n, lambda_t.x, lambda_t.y} of point k live in their own array of RECORDS, pcr, point-major
-// like a plane: record (k, slot) at pcr[(k * Mpad + slot) * PCW].  f32: PCW = 2 — a record is one 32-byte L2 sector
-// {lambda_n, sum, lt.x, lt.y | tag, -, -, -} so that the wavefront schedule can read and write it with ONE 256-bit access that carries its own
-// sequence tag (wave32_dev.cuh); f64: PCW = 1 (the 32-byte Vec4<double>, no tag).  Together with the body state that precedes it in the same
+// like a plane: record (k, slot) at pcr[(k * Mpad + slot) * PCW].  f32: PCW = 2 — a record is one 32-byte L2 sector of two quads
+// {lambda_n, sum, tag, - | lt.x, lt.y, tag, -}, each of which the wavefront schedule reads and writes with ONE 128-bit access that carries the
+// record's sequence tag (wave32_dev.cuh); f64: PCW = 1 (the 32-byte Vec4<double>, no tag).  Together with the body state that precedes it in the same
 // allocation (vel | dlt | counters | pcr) it is the "hot" range pinned in L2 by the access-policy window.
 template <class S> struct PcRec { static constexpr int W = sizeof(S) == 4 ? 2 : 1; };
 // info lane of plane CP_IDX
@@ -135,6 +136,15 @@ template <class S> __device__ __forceinline__ void stv3(S* p, int i, V3<S> v) { 
 template <class S> __device__ __forceinline__ Vec4<S>* pc_ptr(const DevSolver<S>& d, int k, int slot) {
     return d.pcr + (size_t(k) * size_t(d.Mpad) + size_t(slot)) * PcRec<S>::W;
 }
+// store the value {lambda_n, sum, lt.x, lt.y} of an impulse record (f32: sequence tag 0)
+template <class S> __device__ __forceinline__ void pc_store(Vec4<S>* p, Vec4<S> v) {
+    if constexpr (PcRec<S>::W == 1) {
+        st4(p, v);
+    } else {
+        st4(p, mk4<S>(v.x, v.y, S(0), S(0)));
+        st4(p + 1, mk4<S>(v.z, v.w, S(0), S(0)));
+    }
+}
 
 template <class S> struct BodyInertia {
     V3<S> inv_mass;  // effective (locked axes applied)
@@ -192,14 +202,14 @@ __device__ void prepare_body_item(const DevSolver<S>& d, int i) {
                    avn_abs(il.m02) < eps && avn_abs(il.m12) < eps;
         if (!rot_locked && !iso) flags |= BF_GYRO;
         const bool clamped = (d.max_lin && avn_finite(d.max_lin[i])) || (d.max_ang && avn_finite(d.max_ang[i]));
-        // (measured: fusing even the 12-flop velocity step into the contact item costs more than the dependency level it saves,
-        //  1.66 -> 1.77 ms — the contact item's own latency is the critical resource; kept behind AVN_FUSE_IV for reference)
+        // (fusing even the 12-flop velocity step into the contact item lengthens the contact item, whose own latency is the critical
+        //  resource, by more than the dependency level it saves; kept behind AVN_FUSE_IV for reference)
 #ifdef AVN_FUSE_IV
         if (kind == AVN_BODY_DYNAMIC && !(flags & (BF_CUSTOM_VEL | BF_GYRO)) && !clamped) flags |= BF_FUSE_IV;
 #else
         (void)clamped;
 #endif
-        // (fusing integrate_positions the same way was measured SLOWER, 1.66 -> 1.85 ms: its double-precision sincos diverges the
+        // (fusing integrate_positions the same way is off as well: its double-precision sincos diverges the
         //  warps of every late colour of the solve pass instead of costing one cheap level; kept behind AVN_FUSE_IP for reference)
 #ifdef AVN_FUSE_IP
         if (!(flags & BF_CUSTOM_POS)) flags |= BF_FUSE_IP;
@@ -314,9 +324,7 @@ __device__ void prepare_constraint_item(const DevSolver<S>& d, int m) {
         }
         st4(&c[size_t(CP_ROW(k, 0)) * MP], mk4<S>(r1.x, r1.y, r1.z, sep0));
         st4(&c[size_t(CP_ROW(k, 1)) * MP], mk4<S>(r2.x, r2.y, r2.z, meff));
-        Vec4<S>* pc = pc_ptr(d, k, slot);
-        st4(pc, mk4<S>(imp_n, S(0), itx, ity));
-        if (PcRec<S>::W == 2) st4(pc + 1, mk4<S>(S(0), S(0), S(0), S(0)));   // sequence tag 0
+        pc_store(pc_ptr(d, k, slot), mk4<S>(imp_n, S(0), itx, ity));
         st4(&c[size_t(CP_ROW(k, 2)) * MP], mk4<S>(K1, K2, K3, d.p_normal_speed[p]));
     }
 }
@@ -376,7 +384,7 @@ __device__ __forceinline__ unsigned wave_event(int kind, int it, int s, int iter
     }
 }
 // counters: relaxed gpu-scope accesses bracketed by __threadfence() (message passing).  ld.acquire.gpu / st.release.gpu on the
-// counters instead of the fences was measured and is not faster (1.69 vs 1.66 ms per 100k-cube step).
+// counters instead of the fences is the alternative; the fences are kept.
 __device__ __forceinline__ unsigned ld_relaxed(const unsigned* p) {
     unsigned v;
     asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -393,6 +401,15 @@ __device__ __forceinline__ Vec4<double> ld4_cg(const Vec4<double>* p) {
     return mk4<double>(a.x, a.y, b.x, b.y);
 }
 template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> ldm(const Vec4<S>* p) { return WAVE ? ld4_cg(p) : ld4(p); }
+// the value {lambda_n, sum, lt.x, lt.y} of an impulse record
+template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> pc_load(const Vec4<S>* p) {
+    if constexpr (PcRec<S>::W == 1) {
+        return ldm<WAVE>(p);
+    } else {
+        const Vec4<S> a = ldm<WAVE>(p), b = ldm<WAVE>(p + 1);
+        return mk4<S>(a.x, a.y, b.x, b.y);
+    }
+}
 
 // warp-synchronous wait: all 32 lanes of the warp wait until every lane's two counters have reached their targets
 // A watchdog bounds the spin (a schedule bug must not hang the device): after ~4M polls the warp gives up and raises
@@ -515,7 +532,7 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
     }
 #pragma unroll
     for (int k = 0; k < MAXP; ++k)
-        if (k < np) PC[k] = ldm<WAVE>(pc_ptr(d, k, slot));
+        if (k < np) PC[k] = pc_load<WAVE>(pc_ptr(d, k, slot));
     __pipeline_wait_prior(0);  // this thread's staged rows have landed (only the issuing thread reads them)
 #ifdef AVN_WAVE_TRACE
     if (WAVE) {  // force the loads to complete here so the segments separate cleanly
@@ -645,7 +662,7 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
     if (PASS != PASS_WARM) {
 #pragma unroll
         for (int k = 0; k < MAXP; ++k)
-            if (k < np) st4(pc_ptr(d, k, slot), PC[k]);
+            if (k < np) pc_store(pc_ptr(d, k, slot), PC[k]);
     }
     if (WAVE && SOLVE) {
         // integrate_positions of a body whose last solve event this is (integrator/mod.rs:503-535): dp += v h, dq = exp(w h) dq
@@ -894,7 +911,7 @@ __device__ __forceinline__ void store_impulse_item(const DevSolver<S>& d, int m)
         return;
     }
     for (int k = 0; k < np; ++k) {
-        Vec4<S> pc = ld4(pc_ptr(d, k, slot));
+        Vec4<S> pc = pc_load<false>(pc_ptr(d, k, slot));
         d.p_out_ws_normal[p0 + k] = pc.x;
         d.p_out_ws_tangent[2 * (p0 + k)] = (info & CI_TANGENT) ? pc.z : S(0);
         d.p_out_ws_tangent[2 * (p0 + k) + 1] = (info & CI_TANGENT) ? pc.w : S(0);

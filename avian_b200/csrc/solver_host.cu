@@ -196,7 +196,7 @@ class Solver final : public SolverBase {
     cudaStream_t stream_;
     ErrorSink* err_;
     uint32_t cfg_flags_;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     bool coop_ok_ = false, use_mega_ = true, use_wave_ = true, l2_persist_ = false;
     size_t l2_persist_bytes_ = 0, l2_window_max_ = 0;
     int mega_grid_ = 0, mega_bps_ = 3, mega_maxp_ = 0, mega_sel_bps_ = 0;
@@ -217,8 +217,7 @@ class Solver final : public SolverBase {
         }
     }
     // blocks per SM of a step: the f32 wavefront routines fit 128 registers without spills (the delta records die before the main loop), so a
-    // wavefront-scheduled f32 step runs 4 blocks = 16 warps per SM (1.618 -> 1.562 ms at 100k cubes); the barrier schedule keeps the
-    // measured best of round 1 (3 for f32, 2 for f64).  AVN_MEGA_BPS overrides both.
+    // wavefront-scheduled f32 step runs 4 blocks = 16 warps per SM; the barrier schedule runs 3 for f32, 2 for f64 (register budget).  AVN_MEGA_BPS overrides both.
     // dynamic shared memory of the persistent kernel: the per-thread cp.async tile of the contact routines
     static size_t mega_smem_bytes(int maxp) { return stage_bytes<S>(MEGA_BLOCK, maxp); }
     int bps_for(bool wave_candidate) const { return bps_forced_ ? mega_bps_ : ((sizeof(S) == 4 && wave_candidate) ? 4 : mega_bps_); }
@@ -292,13 +291,13 @@ class Solver final : public SolverBase {
     bool sm_order_ = false;
     IslandLists isl_;
     std::vector<int> isl_jb1_, isl_jb2_;
-    // island-group schedule (solver_kernels.cuh island_substep_loop): bit-identical, but measured SLOWER than the barrier schedule on the scene it
-    // was built for (5 000 ragdolls: 2.24 ms vs 1.47 ms; one warp per island: 15.7 ms) — every block is in a different phase, so the SM's
+    // island-group schedule (solver_kernels.cuh island_substep_loop): bit-identical, but slower than the barrier schedule on the scene it
+    // was built for (5 000 ragdolls) when it was introduced — every block is in a different phase, so the SM's
     // instruction stream thrashes, and an island's few joints per level keep one warp busy.  Off by default; AVN_ISLAND_MODE=1 enables it.
     bool island_mode_ = false;
-    // body-centric warm start (wave32_dev.cuh w32_ivw_item): bit-identical, 26 -> 18 dependency levels per substep, but measured SLOWER where
-    // it matters (100k cubes 1.62 -> 1.98 ms: the item is a chain of dependent gathers, 4x more chunks than integrate_velocities had) and
-    // only 4 % faster on the chain-bound 10k scene (0.739 -> 0.708 ms).  Off by default; AVN_WARM_BY_BODY=1 enables it.
+    // body-centric warm start (wave32_dev.cuh w32_ivw_item): bit-identical, 26 -> 18 dependency levels per substep, but slower where
+    // it matters when it was introduced (100k cubes: the item is a chain of dependent gathers, 4x more chunks than integrate_velocities had)
+    // and only slightly faster on the chain-bound 10k scene.  Off by default; AVN_WARM_BY_BODY=1 enables it.
     bool warm_by_body_ = false;
     size_t hot_bytes_ = 0;
     DevBuf j_type_, j_index_, j_level_, j_planes_;
@@ -798,8 +797,8 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
         mega = mega && mega_step_;   // a step keeps the launch mode its prepare launch chose
     }
     if (l2_persist_ && dev_.isl_count > 0) {
-        // island-per-warp schedule: the state of an island lives in its SM's L1; no L2 window (an access-policy window was measured to turn
-        // the island loop's L1 hits into L2 round trips: 0.93 ms under ncu, which does not apply the stream attribute, 14.7 ms with it)
+        // island-per-warp schedule: the state of an island lives in its SM's L1; no L2 window (an access-policy window turns
+        // the island loop's L1 hits into L2 round trips)
         cudaStreamAttrValue attr{};
         attr.accessPolicyWindow.base_ptr = nullptr;
         attr.accessPolicyWindow.num_bytes = 0;
@@ -921,7 +920,7 @@ __global__ void boundary_apply_kernel(DevSolver<S> d, const int* __restrict__ bo
     }
     // the spare lanes of the velocity / delta rows carry the wavefront schedule's sequence tags (wave32_dev.cuh): kept as they are
     st4(&d.vel[2 * b], mk4<S>(l.x, l.y, l.z, ld4(&d.vel[2 * b]).w));
-    st4(&d.vel[2 * b + 1], mk4<S>(a.x, a.y, a.z, S(0)));
+    st4(&d.vel[2 * b + 1], mk4<S>(a.x, a.y, a.z, ld4(&d.vel[2 * b + 1]).w));
     const Vec4<S>* own = gathered + (size_t(owner_rank[k]) * records + size_t(source[size_t(k) * world + owner_rank[k]])) * 4;
     Vec4<S> odp = ld4(&own[2]);
     odp.w = ld4(&d.dlt[2 * b]).w;

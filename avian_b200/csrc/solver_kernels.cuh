@@ -2,12 +2,12 @@
 //
 // Two launch strategies over the SAME per-item device routines (solver_dev.cuh / joints_dev.cuh):
 //   * step_megakernel: ONE persistent cooperative kernel per physics step.  The grid is sized to exactly fill
-//     the 148 SMs (occupancy x SM count); every phase of the step (prepare, each graph colour of each pass of each
+//     the 132 SMs (occupancy x SM count); every phase of the step (prepare, each graph colour of each pass of each
 //     substep, each joint level, finalize) is a grid-stride loop followed by a grid-wide barrier.  A 100k-cube
 //     step has ~300-600 dependent phases of only 10^4..10^5 independent items each, so the step is bound by
-//     phase latency; removing ~500 kernel launches and keeping the working set hot in the 126 MB L2 between phases
-//     is what the B200 wants.
-//   * phase kernels: one launch per phase; the same arithmetic, used for profiling single phases under ncu, for
+//     phase latency; removing ~500 kernel launches and keeping the mutable working set hot in the 50 MB L2 between phases
+//     is what the GPU wants.
+//   * phase kernels: one launch per phase; the same arithmetic, used for timing single phases, for
 //     the roofline measurement of the solver-iteration kernel, and as the fallback when a cooperative launch is
 //     refused.
 #pragma once
@@ -98,7 +98,7 @@ __device__ __forceinline__ void grid_contact_pass(const DevSolver<S>& d, cg::gri
 #define AVN_WAVE_CHUNK 32
 #endif
 constexpr int WAVE_CHUNK = AVN_WAVE_CHUNK;
-// f32 runs the sector-record protocol (wave32_dev.cuh), f64 the counter protocol (solver_dev.cuh)
+// the counter protocol (solver_dev.cuh); f32 can run the tagged-record protocol instead (wave32_dev.cuh, below)
 template <class S, int PASS, int MAXP>
 __device__ __noinline__ void wave_contact_chunk(const DevSolver<S>& d, int slot, int s, int it, bool active) {
     contact_item<S, PASS, true, MAXP>(d, slot, s, it, active);
@@ -107,9 +107,10 @@ template <class S>
 __device__ __noinline__ void wave_iv_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_velocity_item<S, true>(d, i, s, active); }
 template <class S>
 __device__ __noinline__ void wave_ip_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_position_item<S, true>(d, i, s, active); }
-// f32: the sector-record protocol.  (-DAVN_WAVE_COUNTERS_F32 builds the round-1 counter protocol for f32 as well, for A/B timing.)
-// (BPS and MAXP are template parameters of all of them only so that every megakernel variant owns its copies: ptxas 12.9 segfaults when two
-//  kernels share a __noinline__ function that contains the 256-bit accesses)
+// f32 runs the counter protocol by default.  -DAVN_WAVE_RECORDS_F32 builds the tagged-record protocol (wave32_dev.cuh) instead, which
+// relies on 16-byte accesses not tearing: the PTX memory model does not promise that, and on sm_90 the records gave reads that were
+// close to the right values but not bit-identical (stale halves), so the records stay an experiment.
+// (BPS and MAXP are template parameters of all of them so that every megakernel variant owns its copies)
 template <int PASS, int MAXP, int BPS>
 __device__ __noinline__ void wave32_contact_chunk(const DevSolver<float>& d, int slot, int s, int it, bool active, int wf, int pass) {
     w32_contact_item<PASS, MAXP>(d, slot, s, it, active, wf, pass);
@@ -122,10 +123,10 @@ template <int BPS, int MAXP> __device__ __noinline__ void wave32_iv_chunk(const 
 template <int BPS, int MAXP> __device__ __noinline__ void wave32_ip_chunk(const DevSolver<float>& d, int i, int s, bool active, int wf) { w32_integrate_position_item(d, i, s, active, wf); }
 // integrate_velocities + the body's warm starts (8 bodies per warp, wave32_dev.cuh)
 template <int BPS, int MAXP> __device__ __noinline__ void wave32_ivw_chunk(const DevSolver<float>& d, int chunk, int s) { w32_ivw_item<MAXP>(d, chunk, s); }
-#ifdef AVN_WAVE_COUNTERS_F32
-constexpr bool WAVE_RECORDS_F32 = false;
-#else
+#ifdef AVN_WAVE_RECORDS_F32
 constexpr bool WAVE_RECORDS_F32 = true;
+#else
+constexpr bool WAVE_RECORDS_F32 = false;
 #endif
 template <class S> struct UseRecords { static constexpr bool value = false; };
 template <> struct UseRecords<float> { static constexpr bool value = WAVE_RECORDS_F32; };
@@ -155,7 +156,7 @@ template <class S, int BPS, int MAXP> __device__ __forceinline__ void wave_ivw(c
 // says the 16 extra CCTL per item cost more than the latency they hide.
 template <class S, int MAXP>
 __device__ __forceinline__ void wave_prefetch_slot(const DevSolver<S>& d, int slot) {
-#ifdef AVN_WAVE_PREFETCH   // measured SLOWER (1.618 -> 1.671 ms at 100k cubes, 1.562 -> 1.774 at 4 blocks/SM): kept as an experiment
+#ifdef AVN_WAVE_PREFETCH   // slower when it was introduced: kept as an experiment
     const char* base = reinterpret_cast<const char*>(d.cst + slot);
     const size_t stride = size_t(d.Mpad) * sizeof(Vec4<S>);
 #pragma unroll
@@ -171,7 +172,7 @@ __device__ __forceinline__ void wave_substep_loop(const DevSolver<S>& d) {
     long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (d.sm_slots) {
         // SM-major numbering of the warps: the BPS blocks of one SM take 4 * BPS CONSECUTIVE chunks of the schedule — the same pass, the same
-        // colour, neighbouring plane rows — instead of chunks 148 blocks apart, so the warps of an SM run the same routine on adjacent memory.
+        // colour, neighbouring plane rows — instead of chunks one SM count of blocks apart, so the warps of an SM run the same routine on adjacent memory.
         // Exactly BPS blocks are resident per SM (cooperative launch of BPS x SM-count blocks under a BPS-blocks register limit), every block
         // draws one ticket of its SM; the counters only ever grow by BPS per launch, so they stay multiples of BPS without a reset.
         // %smid values need not be dense (disabled SMs leave gaps): the first block that arrives on an SM claims the next dense index for it,

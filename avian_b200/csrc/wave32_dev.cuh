@@ -1,45 +1,73 @@
-// Wavefront schedule, f32: SECTOR-ATOMIC SEQUENCE-TAGGED RECORDS (sm_100a).
+// Wavefront schedule, f32: SEQUENCE-TAGGED RECORDS (sm_90a).  EXPERIMENT, built only with -DAVN_WAVE_RECORDS_F32: the 16-byte
+// no-tearing property below is not promised by the PTX memory model, and on the H100 the records gave stale reads (solver_kernels.cuh).
 //
 // The wavefront substep loop (solver_dev.cuh "wavefront mode") replaces grid barriers by per-body event numbers: an item may run when the
 // event counters of its bodies equal its position in their event sequences.  Round 1 kept the counters in their own array and passed the
-// data by message passing: stores -> __threadfence -> counter store | counter poll -> __threadfence -> data loads.  ncu: stall_membar 1.57 per
-// issue, and every dependency hop paid  store ack + counter hop + poll + fence + a second L2 round trip for the data  (~2 600-3 100 cycles next
-// to ~5 300 cycles of arithmetic).
+// data by message passing: stores -> __threadfence -> counter store | counter poll -> __threadfence -> data loads, and every dependency hop
+// paid  store ack + counter hop + poll + fence + a second L2 round trip for the data.
 //
-// Here every MUTABLE datum an item consumes is a 32-byte record — one L2 sector — that carries its own sequence tag, and is read and written
-// with ONE 256-bit strong access (ld/st.relaxed.gpu.global.v8.f32 = LDG/STG.E.ENL2.256.STRONG.GPU, new with sm_100):
-//     velocity record  vel[2b..2b+1]  = {lin.xyz, EVENTS | ang.xyz, -}     EVENTS = number of schedule events completed on body b
-//     delta record     dlt[2b..2b+1]  = {dp.xyz,  IPS    | dq.xyzw}        IPS    = integrate_positions steps completed on body b
-//     impulse record   pcr[(k,slot)]  = {ln, sum, lt.x, lt.y | WRITES,-,-,-}  WRITES = passes that have written the point's impulses
+// Here every MUTABLE datum an item consumes sits in a 32-byte record that carries its own sequence tag, read and written with 128-bit
+// strong accesses (ld/st.relaxed.gpu.global.v4.f32), the widest single access Hopper has:
+//     velocity record  vel[2b..2b+1]  = {lin.xyz, EVENTS | ang.xyz, EVENTS}   EVENTS = number of schedule events completed on body b
+//     impulse record   pcr[(k,slot)]  = {ln, sum, WRITES, - | lt.x, lt.y, WRITES, -}   WRITES = passes that have written the point's impulses
+//     delta record     dlt[2b..2b+1]  = {dp.xyz, IPS | dq.xyzw}          IPS    = integrate_positions steps completed on body b
 // A consumer knows the tag every record must carry when all its predecessors are done (the same arithmetic the event numbers came from),
 // loads the records and simply repeats the loads until every tag matches.  A successful poll IS the data: no counter array, no fence, no
-// second round trip; a producer publishes by storing its records, in any order.  The only hardware property relied on is that a naturally
-// aligned 32-byte vector access is performed as one sector transaction (no tearing inside a record); nothing is assumed about the order in
-// which different records become visible, because each record validates itself.
-// The separation terms of a solve pass depend only on the delta records, which change once per substep: they are computed BEFORE the wait on
-// the velocity records (the delta records are usually valid at the first look), so ~20 % of an item's arithmetic leaves the critical path.
+// second round trip; a producer publishes by storing its records, in any order.  The hardware property relied on is that a naturally
+// aligned 16-byte vector access is performed as one transaction (no tearing inside a quad).  The velocity and impulse records carry the
+// tag in BOTH quads, and a tag value is written once per record, so two quads with the expected tag come from the same store.
+// The delta record has no lane left for a second tag (the rotation fills its quad): its producer stores the rotation quad, then the tagged
+// quad with release semantics, and the consumer polls the tagged quad with acquire semantics before it reads the rotation.  It changes
+// once per substep, so the fence this costs stays off the per-item chain of the velocity records.
+// The separation terms of a solve pass depend only on the delta records: they are computed BEFORE the wait on the velocity records (the
+// delta records are usually valid at the first look), so ~20 % of an item's arithmetic leaves the critical path.
 //
-// f64 keeps the counter protocol: a Vec4<double> fills a whole sector, so delta_rotation has no lane left for a tag.
+// f64 keeps the counter protocol: a Vec4<double> fills a whole quad pair, so there is no lane left for a tag.
 #pragma once
 
 namespace avn {
 
 struct Rec32 { Vec4<float> a, b; };
-__device__ __forceinline__ Rec32 ld_rec(const Vec4<float>* p) {
-    Rec32 r;
-    asm volatile("ld.relaxed.gpu.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(r.a.x), "=f"(r.a.y), "=f"(r.a.z), "=f"(r.a.w), "=f"(r.b.x), "=f"(r.b.y), "=f"(r.b.z), "=f"(r.b.w)
-                 : "l"(p)
-                 : "memory");
+__device__ __forceinline__ Vec4<float> ld_q(const Vec4<float>* p) {
+    Vec4<float> r;
+    asm volatile("ld.relaxed.gpu.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
     return r;
 }
-__device__ __forceinline__ void st_rec(Vec4<float>* p, float a0, float a1, float a2, float a3, float b0, float b1, float b2, float b3) {
-    asm volatile("st.relaxed.gpu.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(b0), "f"(b1), "f"(b2),
-                 "f"(b3)
-                 : "memory");
+__device__ __forceinline__ Vec4<float> ld_q_acquire(const Vec4<float>* p) {
+    Vec4<float> r;
+    asm volatile("ld.acquire.gpu.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
+    return r;
+}
+__device__ __forceinline__ void st_q(Vec4<float>* p, float a0, float a1, float a2, float a3) {
+    asm volatile("st.relaxed.gpu.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a0), "f"(a1), "f"(a2), "f"(a3) : "memory");
+}
+__device__ __forceinline__ void st_q_release(Vec4<float>* p, float a0, float a1, float a2, float a3) {
+    asm volatile("st.release.gpu.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a0), "f"(a1), "f"(a2), "f"(a3) : "memory");
 }
 __device__ __forceinline__ unsigned tag_of(float lane) { return __float_as_uint(lane); }
 __device__ __forceinline__ float tag_lane(unsigned t) { return __uint_as_float(t); }
+
+// velocity record {lin.xyz, T | ang.xyz, T}
+__device__ __forceinline__ Rec32 ld_vel(const Vec4<float>* p) { Rec32 r; r.a = ld_q(p); r.b = ld_q(p + 1); return r; }
+__device__ __forceinline__ bool vel_is(const Rec32& r, unsigned t) { return tag_of(r.a.w) == t && tag_of(r.b.w) == t; }
+__device__ __forceinline__ void st_vel(Vec4<float>* p, V3<float> v, V3<float> w, unsigned t) {
+    st_q(p, v.x, v.y, v.z, tag_lane(t));
+    st_q(p + 1, w.x, w.y, w.z, tag_lane(t));
+}
+// impulse record {ln, sum, T, - | lt.x, lt.y, T, -}; its value as {ln, sum, lt.x, lt.y}
+__device__ __forceinline__ Rec32 ld_pc(const Vec4<float>* p) { Rec32 r; r.a = ld_q(p); r.b = ld_q(p + 1); return r; }
+__device__ __forceinline__ bool pc_is(const Rec32& r, unsigned t) { return tag_of(r.a.z) == t && tag_of(r.b.z) == t; }
+__device__ __forceinline__ Vec4<float> pc_val(const Rec32& r) { return mk4<float>(r.a.x, r.a.y, r.b.x, r.b.y); }
+__device__ __forceinline__ void st_pc(Vec4<float>* p, Vec4<float> v, unsigned t) {
+    st_q(p, v.x, v.y, tag_lane(t), 0.f);
+    st_q(p + 1, v.z, v.w, tag_lane(t), 0.f);
+}
+// delta record {dp.xyz, T | dq.xyzw}: rotation first, then the tag with release semantics; read back in the opposite order
+__device__ __forceinline__ Rec32 ld_dlt(const Vec4<float>* p) { Rec32 r; r.a = ld_q_acquire(p); r.b = ld_q(p + 1); return r; }
+__device__ __forceinline__ void st_dlt(Vec4<float>* p, V3<float> dp, unsigned t, Vec4<float> dq) {
+    st_q(p + 1, dq.x, dq.y, dq.z, dq.w);
+    st_q_release(p, dp.x, dp.y, dp.z, tag_lane(t));
+}
 
 constexpr unsigned W32_SPIN_LIMIT = 1u << 22;
 
@@ -74,7 +102,7 @@ __device__ __forceinline__ void w32_contact_item(const DevSolver<float>& d, int 
     // the item's own scratch rows behind the staged ones: the impulses of its points and their separations.  They live in shared memory so
     // that the loops over the points can stay ROLLED (dynamic index, no local memory): the solve and relax routines shrink from 42 KB of
     // SASS to a quarter, which matters because the SM's instruction cache (32 KB L1.5) serves warps that are in five different routines
-    // at once in the wavefront schedule (ncu: stall_no_instruction 1.18 per issue with the unrolled routines)
+    // at once in the wavefront schedule
 #define ROW_PC(k) stage[(3 * MAXP + (k)) * T]
     float* const sepv = reinterpret_cast<float*>(&stage[(4 * MAXP) * T]);
     // ---- immutable part: issued before any wait
@@ -112,8 +140,8 @@ __device__ __forceinline__ void w32_contact_item(const DevSolver<float>& d, int 
         if (np != 0 && !ver1) { D1.a = ld4(&d.dlt[2 * b1]); D1.b = ld4(&d.dlt[2 * b1 + 1]); }   // no SolverBody: constant (0, identity)
         if (np != 0 && !ver2) { D2.a = ld4(&d.dlt[2 * b2]); D2.b = ld4(&d.dlt[2 * b2 + 1]); }
         for (unsigned spins = 0;; ++spins) {
-            if (n1) D1 = ld_rec(&d.dlt[2 * b1]);
-            if (n2) D2 = ld_rec(&d.dlt[2 * b2]);
+            if (n1) D1 = ld_dlt(&d.dlt[2 * b1]);
+            if (n2) D2 = ld_dlt(&d.dlt[2 * b2]);
             if (n1) n1 = tag_of(D1.a.w) != dtag;
             if (n2) n2 = tag_of(D2.a.w) != dtag;
             if (__all_sync(0xffffffffu, !(n1 || n2))) break;
@@ -150,18 +178,18 @@ __device__ __forceinline__ void w32_contact_item(const DevSolver<float>& d, int 
         if (np != 0 && !ver2) { R2.a = ld4(&d.vel[2 * b2]); R2.b = ld4(&d.vel[2 * b2 + 1]); }
         AVN_TRACE_T(t_w1);
         for (unsigned spins = 0;; ++spins) {
-            if (n1) R1 = ld_rec(&d.vel[2 * b1]);
-            if (n2) R2 = ld_rec(&d.vel[2 * b2]);
+            if (n1) R1 = ld_vel(&d.vel[2 * b1]);
+            if (n2) R2 = ld_vel(&d.vel[2 * b2]);
 #pragma unroll 1
             for (int k = 0; k < np; ++k) {
                 if (pend & (1u << k)) {
-                    const Rec32 p = ld_rec(pc_ptr(d, k, slot));
-                    ROW_PC(k) = p.a;
-                    if (tag_of(p.b.x) == ptag) pend &= ~(1u << k);
+                    const Rec32 p = ld_pc(pc_ptr(d, k, slot));
+                    ROW_PC(k) = pc_val(p);
+                    if (pc_is(p, ptag)) pend &= ~(1u << k);
                 }
             }
-            if (n1) n1 = tag_of(R1.a.w) != e1;
-            if (n2) n2 = tag_of(R2.a.w) != e2;
+            if (n1) n1 = !vel_is(R1, e1);
+            if (n2) n2 = !vel_is(R2, e2);
             if (__all_sync(0xffffffffu, !(n1 || n2 || pend != 0u))) break;
             if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
             if (d.poll_ns) __nanosleep(unsigned(d.poll_ns));   // (experiment: back off between polls, AVN_WAVE_POLL_NS)
@@ -264,20 +292,16 @@ __device__ __forceinline__ void w32_contact_item(const DevSolver<float>& d, int 
     AVN_TRACE_ADD(d, 2, t_s0 - t_c0);
 #endif
     if (PASS != PASS_WARM) {
-        const float nt = tag_lane(ptag + 1u);
 #pragma unroll 1
-        for (int k = 0; k < np; ++k) {
-            const Vec4<S> pck = ROW_PC(k);
-            st_rec(pc_ptr(d, k, slot), pck.x, pck.y, pck.z, pck.w, nt, 0.f, 0.f, 0.f);
-        }
+        for (int k = 0; k < np; ++k) st_pc(pc_ptr(d, k, slot), ROW_PC(k), ptag + 1u);
     }
     if (ver1) {
-        if (info & CI_ZERO1) st_rec(&d.vel[2 * b1], R1.a.x, R1.a.y, R1.a.z, tag_lane(e1 + 1u), R1.b.x, R1.b.y, R1.b.z, 0.f);
-        else st_rec(&d.vel[2 * b1], v1.x, v1.y, v1.z, tag_lane(e1 + 1u), w1.x, w1.y, w1.z, 0.f);
+        if (info & CI_ZERO1) st_vel(&d.vel[2 * b1], xyz(R1.a), xyz(R1.b), e1 + 1u);
+        else st_vel(&d.vel[2 * b1], v1, w1, e1 + 1u);
     }
     if (ver2) {
-        if (info & CI_ZERO2) st_rec(&d.vel[2 * b2], R2.a.x, R2.a.y, R2.a.z, tag_lane(e2 + 1u), R2.b.x, R2.b.y, R2.b.z, 0.f);
-        else st_rec(&d.vel[2 * b2], v2.x, v2.y, v2.z, tag_lane(e2 + 1u), w2.x, w2.y, w2.z, 0.f);
+        if (info & CI_ZERO2) st_vel(&d.vel[2 * b2], xyz(R2.a), xyz(R2.b), e2 + 1u);
+        else st_vel(&d.vel[2 * b2], v2, w2, e2 + 1u);
     }
 #ifdef AVN_WAVE_TRACE
     AVN_TRACE_ADD(d, 3, clock64() - t_s0);
@@ -292,8 +316,8 @@ __device__ __forceinline__ void w32_contact_item(const DevSolver<float>& d, int 
 // ---------------------------------------------------------------------------------------------------------
 // The same routine with the loops over the points UNROLLED and the impulses / separations in registers (round 2's first version): 42 KB of
 // SASS per pass instead of 17 KB, but no shared-memory round trip inside the dependent chain of an item.  The rolled routine wins when the
-// step is throughput-bound (100k cubes: 1.61 -> 1.42 ms, the warps of an SM are in five routines at once and the 32 KB instruction cache
-// holds the rolled ones), the unrolled one when it is bound by the per-body chain (10k cubes: 0.74 ms vs 0.90 ms rolled).  The host picks
+// step is throughput-bound (100k cubes: the warps of an SM are in five routines at once and the instruction cache
+// holds the rolled ones), the unrolled one when it is bound by the per-body chain (10k cubes).  The host picks
 // per step (DevSolver::wave_rolled).
 // ---------------------------------------------------------------------------------------------------------
 template <int PASS, int MAXP>
@@ -351,8 +375,8 @@ __device__ __forceinline__ void w32_contact_item_unrolled(const DevSolver<float>
         if (np != 0 && !ver1) { D1.a = ld4(&d.dlt[2 * b1]); D1.b = ld4(&d.dlt[2 * b1 + 1]); }   // no SolverBody: constant (0, identity)
         if (np != 0 && !ver2) { D2.a = ld4(&d.dlt[2 * b2]); D2.b = ld4(&d.dlt[2 * b2 + 1]); }
         for (unsigned spins = 0;; ++spins) {
-            if (n1) D1 = ld_rec(&d.dlt[2 * b1]);
-            if (n2) D2 = ld_rec(&d.dlt[2 * b2]);
+            if (n1) D1 = ld_dlt(&d.dlt[2 * b1]);
+            if (n2) D2 = ld_dlt(&d.dlt[2 * b2]);
             if (n1) n1 = tag_of(D1.a.w) != dtag;
             if (n2) n2 = tag_of(D2.a.w) != dtag;
             if (__all_sync(0xffffffffu, !(n1 || n2))) break;
@@ -394,18 +418,18 @@ __device__ __forceinline__ void w32_contact_item_unrolled(const DevSolver<float>
         if (np != 0 && !ver2) { R2.a = ld4(&d.vel[2 * b2]); R2.b = ld4(&d.vel[2 * b2 + 1]); }
         AVN_TRACE_T(t_w1);
         for (unsigned spins = 0;; ++spins) {
-            if (n1) R1 = ld_rec(&d.vel[2 * b1]);
-            if (n2) R2 = ld_rec(&d.vel[2 * b2]);
+            if (n1) R1 = ld_vel(&d.vel[2 * b1]);
+            if (n2) R2 = ld_vel(&d.vel[2 * b2]);
 #pragma unroll
             for (int k = 0; k < MAXP; ++k) {
                 if (pend & (1u << k)) {
-                    const Rec32 p = ld_rec(pc_ptr(d, k, slot));
-                    PC[k] = p.a;
-                    if (tag_of(p.b.x) == ptag) pend &= ~(1u << k);
+                    const Rec32 p = ld_pc(pc_ptr(d, k, slot));
+                    PC[k] = pc_val(p);
+                    if (pc_is(p, ptag)) pend &= ~(1u << k);
                 }
             }
-            if (n1) n1 = tag_of(R1.a.w) != e1;
-            if (n2) n2 = tag_of(R2.a.w) != e2;
+            if (n1) n1 = !vel_is(R1, e1);
+            if (n2) n2 = !vel_is(R2, e2);
             if (__all_sync(0xffffffffu, !(n1 || n2 || pend != 0u))) break;
             if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
             if (d.poll_ns) __nanosleep(unsigned(d.poll_ns));   // (experiment: back off between polls, AVN_WAVE_POLL_NS)
@@ -506,18 +530,17 @@ __device__ __forceinline__ void w32_contact_item_unrolled(const DevSolver<float>
     AVN_TRACE_ADD(d, 2, t_s0 - t_c0);
 #endif
     if (PASS != PASS_WARM) {
-        const float nt = tag_lane(ptag + 1u);
 #pragma unroll
         for (int k = 0; k < MAXP; ++k)
-            if (k < np) st_rec(pc_ptr(d, k, slot), PC[k].x, PC[k].y, PC[k].z, PC[k].w, nt, 0.f, 0.f, 0.f);
+            if (k < np) st_pc(pc_ptr(d, k, slot), PC[k], ptag + 1u);
     }
     if (ver1) {
-        if (info & CI_ZERO1) st_rec(&d.vel[2 * b1], R1.a.x, R1.a.y, R1.a.z, tag_lane(e1 + 1u), R1.b.x, R1.b.y, R1.b.z, 0.f);
-        else st_rec(&d.vel[2 * b1], v1.x, v1.y, v1.z, tag_lane(e1 + 1u), w1.x, w1.y, w1.z, 0.f);
+        if (info & CI_ZERO1) st_vel(&d.vel[2 * b1], xyz(R1.a), xyz(R1.b), e1 + 1u);
+        else st_vel(&d.vel[2 * b1], v1, w1, e1 + 1u);
     }
     if (ver2) {
-        if (info & CI_ZERO2) st_rec(&d.vel[2 * b2], R2.a.x, R2.a.y, R2.a.z, tag_lane(e2 + 1u), R2.b.x, R2.b.y, R2.b.z, 0.f);
-        else st_rec(&d.vel[2 * b2], v2.x, v2.y, v2.z, tag_lane(e2 + 1u), w2.x, w2.y, w2.z, 0.f);
+        if (info & CI_ZERO2) st_vel(&d.vel[2 * b2], xyz(R2.a), xyz(R2.b), e2 + 1u);
+        else st_vel(&d.vel[2 * b2], v2, w2, e2 + 1u);
     }
 #ifdef AVN_WAVE_TRACE
     AVN_TRACE_ADD(d, 3, clock64() - t_s0);
@@ -592,9 +615,9 @@ __device__ __forceinline__ void w32_integrate_velocity_item(const DevSolver<floa
     {
         bool nr = live, nd = gyro;
         for (unsigned spins = 0;; ++spins) {
-            if (nr) R = ld_rec(&d.vel[2 * i]);
-            if (nd) D = ld_rec(&d.dlt[2 * i]);
-            if (nr) nr = tag_of(R.a.w) != e;
+            if (nr) R = ld_vel(&d.vel[2 * i]);
+            if (nd) D = ld_dlt(&d.dlt[2 * i]);
+            if (nr) nr = !vel_is(R, e);
             if (nd) nd = tag_of(D.a.w) != unsigned(s);
             if (__all_sync(0xffffffffu, !(nr || nd))) break;
             if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
@@ -604,7 +627,7 @@ __device__ __forceinline__ void w32_integrate_velocity_item(const DevSolver<floa
     if (!live) return;
     V3<S> v = xyz(R.a), w = xyz(R.b);
     w32_integrate_velocity_math(d, i, f, D, v, w);
-    st_rec(&d.vel[2 * i], v.x, v.y, v.z, tag_lane(e + 1u), w.x, w.y, w.z, 0.f);
+    st_vel(&d.vel[2 * i], v, w, e + 1u);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -681,9 +704,9 @@ __device__ __forceinline__ void w32_ivw_item(const DevSolver<float>& d, int chun
 #pragma unroll
             for (int k = 0; k < MAXP; ++k) {
                 if (pend & (1u << k)) {
-                    const Rec32 p = ld_rec(pc_ptr(d, k, slot));
-                    PC[k] = p.a;
-                    if (tag_of(p.b.x) == ptag) pend &= ~(1u << k);
+                    const Rec32 p = ld_pc(pc_ptr(d, k, slot));
+                    PC[k] = pc_val(p);
+                    if (pc_is(p, ptag)) pend &= ~(1u << k);
                 }
             }
             if (__all_sync(0xffffffffu, pend == 0u)) break;
@@ -710,9 +733,9 @@ __device__ __forceinline__ void w32_ivw_item(const DevSolver<float>& d, int chun
     {
         bool nr = lead, nd = gyro;
         for (unsigned spins = 0;; ++spins) {
-            if (nr) R = ld_rec(&d.vel[2 * i]);
-            if (nd) D = ld_rec(&d.dlt[2 * i]);
-            if (nr) nr = tag_of(R.a.w) != e;
+            if (nr) R = ld_vel(&d.vel[2 * i]);
+            if (nd) D = ld_dlt(&d.dlt[2 * i]);
+            if (nr) nr = !vel_is(R, e);
             if (nd) nd = tag_of(D.a.w) != unsigned(s);
             if (__all_sync(0xffffffffu, !(nr || nd))) break;
             if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
@@ -739,19 +762,19 @@ __device__ __forceinline__ void w32_ivw_item(const DevSolver<float>& d, int chun
                 for (int k = 0; k < np; ++k) {
                     if (q0 + k < CAPQ) continue;
                     const V3<S> r = xyz(ld4(&c[size_t(CP_ROW(k, side2 ? 1 : 0)) * MP]));
-                    Rec32 p = ld_rec(pc_ptr(d, k, slot));
-                    for (unsigned spins = 0; tag_of(p.b.x) != ptag; ++spins) {
+                    Rec32 p = ld_pc(pc_ptr(d, k, slot));
+                    for (unsigned spins = 0; !pc_is(p, ptag); ++spins) {
                         if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
             if (d.poll_ns) __nanosleep(unsigned(d.poll_ns));   // (experiment: back off between polls, AVN_WAVE_POLL_NS)
-                        p = ld_rec(pc_ptr(d, k, slot));
+                        p = ld_pc(pc_ptr(d, k, slot));
                     }
-                    const W32WarmDelta o = w32_warm_delta(d, in, n, t1, t2, r, p.a, tangent, side2);
+                    const W32WarmDelta o = w32_warm_delta(d, in, n, t1, t2, r, pc_val(p), tangent, side2);
                     v = v + o.a;
                     w = w + o.bw;
                 }
             }
         }
-        st_rec(&d.vel[2 * i], v.x, v.y, v.z, tag_lane(e + 1u), w.x, w.y, w.z, 0.f);
+        st_vel(&d.vel[2 * i], v, w, e + 1u);
     }
     __syncwarp();   // the slice is free again (the next item stages its rows into it)
 }
@@ -769,9 +792,9 @@ __device__ __forceinline__ void w32_integrate_position_item(const DevSolver<floa
     {
         bool nr = live, nd = live;
         for (unsigned spins = 0;; ++spins) {
-            if (nr) R = ld_rec(&d.vel[2 * i]);
-            if (nd) D = ld_rec(&d.dlt[2 * i]);
-            if (nr) nr = tag_of(R.a.w) != e;
+            if (nr) R = ld_vel(&d.vel[2 * i]);
+            if (nd) D = ld_dlt(&d.dlt[2 * i]);
+            if (nr) nr = !vel_is(R, e);
             if (nd) nd = tag_of(D.a.w) != unsigned(s);
             if (__all_sync(0xffffffffu, !(nr || nd))) break;
             if (spins > W32_SPIN_LIMIT) { d.any_restitution[1] = WAVE_WATCHDOG; break; }
@@ -779,16 +802,16 @@ __device__ __forceinline__ void w32_integrate_position_item(const DevSolver<floa
         }
     }
     if (!live) return;
-    const float nt = tag_lane(unsigned(s) + 1u);
+    const unsigned nt = unsigned(s) + 1u;
     if (f & BF_CUSTOM_POS) {
-        st_rec(&d.dlt[2 * i], D.a.x, D.a.y, D.a.z, nt, D.b.x, D.b.y, D.b.z, D.b.w);
+        st_dlt(&d.dlt[2 * i], xyz(D.a), nt, D.b);
     } else {
         V3<S> ndp = xyz(D.a) + xyz(R.a) * d.h;
         Q4<S> dq; dq.x = D.b.x; dq.y = D.b.y; dq.z = D.b.z; dq.w = D.b.w;
         Q4<S> nq = qmul(q_from_scaled_axis(xyz(R.b) * d.h, d.fast_trig != 0), dq);
-        st_rec(&d.dlt[2 * i], ndp.x, ndp.y, ndp.z, nt, nq.x, nq.y, nq.z, nq.w);
+        st_dlt(&d.dlt[2 * i], ndp, nt, mk4<float>(nq.x, nq.y, nq.z, nq.w));
     }
-    st_rec(&d.vel[2 * i], R.a.x, R.a.y, R.a.z, tag_lane(e + 1u), R.b.x, R.b.y, R.b.z, 0.f);
+    st_vel(&d.vel[2 * i], xyz(R.a), xyz(R.b), e + 1u);
 }
 
 }  // namespace avn

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — physics steps/s of the avian3d substep hot path on B200 (BASELINE.json metric).
+"""bench.py — physics steps/s of the avian3d substep hot path on H100 (BASELINE.json metric).
 
 A "step" is ONE pass of the hot path over one frozen snapshot of the headline scene (100 000-cube coupled stack, f32, 8 substeps):
 sweep-and-prune broad phase over the 100 001 collider AABBs + the whole solver stage (prepare, 8 x [integrate velocities, warm start,
@@ -29,6 +29,8 @@ The narrow phase is NOT in the step (outside the hot path, SURVEY.md 8f #1); its
                (N = 1 is the baseline of the curve).
   cpu_baseline the CPU oracle (C++ restatement of the reference path, colour-parallel, all host cores) on the same snapshot.
   --impl reference   times only that CPU arm (the reference itself is Rust and cannot be built in this image).
+  --dump-outputs DIR after the timed steps, what the last resident step computed (bodies, contact impulses, broad-phase order, new pairs) as
+               DIR/<name>.npy (float32 / float64), so that two builds can be compared output for output on the same seeded scene.
 """
 from __future__ import annotations
 
@@ -59,7 +61,7 @@ SCENES = {
 }
 LABEL = {"stack100k": "100k-cube stack", "stack10k": "10k-cube stack", "stack1k": "1k-cube stack", "ragdolls5k": "5k-ragdoll field",
          "ragdolls500": "500-ragdoll field", "spheres1m": "1M falling spheres (f64)", "spheres100k": "100k falling spheres (f64)"}
-MODES = {0: "phases", 1: "megakernel, grid barriers", 2: "megakernel, wavefront records", 3: "megakernel, one warp per island"}
+MODES = {0: "phases", 1: "megakernel, grid barriers", 2: "megakernel, wavefront schedule", 3: "megakernel, one warp per island"}
 
 
 def metric_name(scene: str) -> str:
@@ -86,7 +88,7 @@ def algorithmic_bytes(B: int, M: int, P: int, substeps: int, scalar_bytes: int =
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe); rank 0 only."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (read-only queries); rank 0 only."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -209,6 +211,10 @@ def run_gpu(args, info):
     span_ms = timer.stop_ms()
     barrier()
     wall_resident = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        ctx.broadphase_download(pairs_out)
+        ctx.solver_download()
+        dump_outputs(Path(args.dump_outputs), bodies, man, pairs_out, aabbs)
     # ---- the same loop with the per-call device times read back (stage breakdown, launch count); results are downloaded here
     mega_ms, bp_ms, launches, mode = 0.0, 0.0, 0, None
     n_break = min(K, 10)
@@ -296,7 +302,7 @@ def run_gpu(args, info):
     if peaks_path.exists():
         peak, peak_src = float(json.loads(peaks_path.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
     achieved = alg["step"] / (mega_ms / 1e3) / 1e9
     traffic = None
     tfile = ROOT / "profiles" / "traffic.json"
@@ -309,7 +315,7 @@ def run_gpu(args, info):
     cfg = workload_config(sc, prm, B, M, P, J, args.settle, sname, int(prm.solver_iterations))
     cfg.update({"colliders": n_colliders, "existing_pairs": n_existing,
                 "new_pairs_per_step": new_pairs, "parallelism": "1 pile per GPU (island sharding of independent scenes), no data-path collective",
-                "l2": "inputs larger than L2: constraint planes + columns > 126 MB per step",
+                "l2": "inputs larger than the 50 MB L2: constraint planes + columns > 100 MB per step",
                 "timing": "value: one CUDA-event span over K back-to-back steps on the library stream; e2e: wall clock between barriers; max over ranks",
                 "launch_mode": MODES.get(mode, mode)})
     roof = {"bound": "hbm", "kernel": f"step_megakernel<{'double' if sb == 8 else 'float'}> (whole solver stage, one launch per step)", "achieved": achieved,
@@ -344,6 +350,34 @@ def run_gpu(args, info):
         result["cpu_baseline"] = cpu_arm(args, prm, b0, m0, aabbs, sample_steps=args.cpu_steps, joints=joints, keep=keep)
         result["parity"] = parity_block(gpu_out, keep)
     return result
+
+
+DUMP_BUDGET = 64 << 20   # bytes over all dumped arrays
+
+
+def dump_outputs(out_dir: Path, bodies, man, pairs, aabbs) -> None:
+    """What the caller of the timed path receives after its last step, as float32 / float64 .npy files (integer ids as float64, exact):
+    the bodies, the contact impulses, the broad phase's persistent interval order and its new pairs.  The frozen snapshot usually brings
+    no new pair, and an empty list is not written.  An array whose share of DUMP_BUDGET is too small for it keeps a fixed, seeded sample
+    of its rows (sorted row indices in `<name>_rows`)."""
+    n = int(pairs.count)
+    arrays = {f"bodies_{k}": getattr(bodies, k) for k in ("position", "rotation", "linear_velocity", "angular_velocity")}
+    arrays.update({f"contacts_{k}": getattr(man, k) for k in ("warm_start_normal_impulse", "warm_start_tangent_impulse", "normal_impulse")})
+    if aabbs.order_out is not None:
+        arrays["broadphase_order"] = aabbs.order_out[:int(aabbs.retained_count)]
+    if n > 0:
+        arrays.update({f"pairs_{k}": getattr(pairs, k)[:n] for k in ("collider1", "collider2", "body1", "body2")})
+    share = DUMP_BUDGET // (2 * len(arrays))     # room for the row indices of a sampled array as well
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64) if a.dtype.kind in "iub" or a.dtype == np.float64 else a.astype(np.float32)
+        row_bytes = a.itemsize * (int(np.prod(a.shape[1:])) if a.ndim > 1 else 1)
+        if a.nbytes > share:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], share // row_bytes, replace=False))
+            np.save(out_dir / f"{name}_rows.npy", rows.astype(np.float64))
+            a = a[rows]
+        np.save(out_dir / f"{name}.npy", np.ascontiguousarray(a))
 
 
 def _resident_world(args, ctx):
@@ -644,6 +678,7 @@ def main():
     ap.add_argument("--partition-steps", type=int, default=10)
     ap.add_argument("--partition-slab-scene", default="spheres1m", choices=sorted(SCENES))
     ap.add_argument("--partition-island-scene", default="ragdolls5k", choices=sorted(SCENES))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.settle is None:

@@ -64,7 +64,7 @@ int main(void) {
     cfg.abi_version = AVN_ABI_VERSION;
     cfg.scalar_bits = 32;
     AvnContext* ctx = NULL;
-    if (avn_create(&cfg, &ctx) != AVN_OK) {          /* no CPU fallback: fails without a B200 */
+    if (avn_create(&cfg, &ctx) != AVN_OK) {          /* no CPU fallback: fails without an H100 */
         fprintf(stderr, "avn_create: %s\n", avn_last_error(NULL));
         return 1;
     }

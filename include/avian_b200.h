@@ -1,5 +1,5 @@
 /*
- * avian_b200.h — C ABI of libavian_b200.so, the B200-native replacement for the avian3d substep hot path.
+ * avian_b200.h — C ABI of libavian_b200.so, the H100-native replacement for the avian3d substep hot path.
  *
  * The reference (avianphysics/avian @ 5bef382) has no FFI: its hot path is three Bevy plugins
  * (`IntegratorPlugin`, `BroadPhasePlugin`, `SolverPlugin` + `XpbdSolverPlugin`).  A thin Rust shim

@@ -7,21 +7,22 @@ set -eu
 TAG=${1:-r02}
 LIB=$(pwd)/avian_b200/lib/libavian_b200.so
 OUT=$(pwd)/profiles
+mkdir -p $OUT
 cuobjdump -res-usage $LIB 2>/dev/null | grep -A1 "Function" | grep -v "^--" | paste - - | sed 's/^ *Function //' | c++filt | sort > $OUT/${TAG}_res_usage.txt
 TMP=$(mktemp -d); cd $TMP
 cuobjdump -xelf all $LIB >/dev/null 2>&1
 hist() { grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed -E 's/^\s+\/\*[0-9a-f]+\*\/\s+(@!?U?P[0-9T]+ )?//' | awk '{print $1}' | sed 's/;$//' | sort | uniq -c | sort -rn | awk '{printf "%8d %s\n", $1, $2}'; }
 {
-  echo "# SASS opcode histograms of avian_b200/lib/libavian_b200.so (nvdisasm -c of every cubin in the fat binary).  Blackwell-specific opcodes:"
-  echo "#   LDG.E.ENL2.256.STRONG.GPU / STG.E.ENL2.256.STRONG.GPU  the 256-bit sector accesses of the wavefront records (csrc/wave32_dev.cuh)"
+  echo "# SASS opcode histograms of avian_b200/lib/libavian_b200.so (nvdisasm -c of every cubin in the fat binary).  Opcodes to look for:"
+  echo "#   LDG.E.128.STRONG.GPU / STG.E.128.STRONG.GPU  the tagged 128-bit record accesses of the wavefront schedule (csrc/wave32_dev.cuh)"
   echo "#   LDGSTS.E.BYPASS.128                                    cp.async staging of the constraint rows into shared memory"
   echo "#   CCTL.E.PF2                                             prefetch.global.L2 of the next chunk's rows"
   for f in solver_host broadphase contacts narrow aabb; do
     echo "== $f.cu: memory / synchronisation opcodes"
-    nvdisasm -c $f.sm_100a.cubin 2>/dev/null | hist | grep -E "LDG|STG|LDGSTS|MEMBAR|CCTL|LDS|STS|ATOM|RED|BAR|ERRBAR|LDL|STL|UBLKCP|UTMA|SYNCS|MATCH|VOTE|SHFL" || true
+    nvdisasm -c $f.sm_90a.cubin 2>/dev/null | hist | grep -E "LDG|STG|LDGSTS|MEMBAR|CCTL|LDS|STS|ATOM|RED|BAR|ERRBAR|LDL|STL|UBLKCP|UTMA|SYNCS|MATCH|VOTE|SHFL" || true
   done
   echo "== solver_host.cu: all opcodes, top 60"
-  nvdisasm -c solver_host.sm_100a.cubin 2>/dev/null | hist | head -60
+  nvdisasm -c solver_host.sm_90a.cubin 2>/dev/null | hist | head -60
 } > $OUT/${TAG}_sass_histogram.txt
 cd /; rm -rf $TMP
-grep -c "ENL2.256.STRONG" $OUT/${TAG}_sass_histogram.txt || true
+grep -c "E.128.STRONG.GPU" $OUT/${TAG}_sass_histogram.txt || true

@@ -10,7 +10,7 @@ sys.path.insert(0, str(ROOT / "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu on a machine that has one")
 
 
 def _has_gpu() -> bool:
