@@ -13,7 +13,6 @@
 //            4+3k {anchor1.xyz, initial_separation} 5+3k {anchor2.xyz, normal effective_mass}
 //            6+3k {K1, K2, K3 (tangent effective inverse mass), normal_speed}
 //            pcr[4][Mpad] records {normal impulse, total normal impulse, tangent impulse.x, .y} of point k  <- the only constraint data written in the loop
-//            (the spare lanes of vel, dlt and the f32 impulse records carry the wavefront schedule's sequence tags, wave32_dev.cuh)
 //   joints   jnt[14][Jpad] planes in level-schedule order (see JP_* below).
 #pragma once
 #include <cuda_pipeline.h>
@@ -28,11 +27,8 @@ enum { CP_N = 0, CP_T1 = 1, CP_TV = 2, CP_IDX = 3, CP_PT0 = 4, CP_PLANES = CP_PT
 // immutable rows of point k in CP_PT0 + 3k + {0: A, 1: B, 2: D}
 #define CP_ROW(k, r) (CP_PT0 + 3 * (k) + (r))
 // The MUTABLE impulses {lambda_n, sum lambda_n, lambda_t.x, lambda_t.y} of point k live in their own array of RECORDS, pcr, point-major
-// like a plane: record (k, slot) at pcr[(k * Mpad + slot) * PCW].  f32: PCW = 2 — a record is one 32-byte L2 sector of two quads
-// {lambda_n, sum, tag, - | lt.x, lt.y, tag, -}, each of which the wavefront schedule reads and writes with ONE 128-bit access that carries the
-// record's sequence tag (wave32_dev.cuh); f64: PCW = 1 (the 32-byte Vec4<double>, no tag).  Together with the body state that precedes it in the same
-// allocation (vel | dlt | counters | pcr) it is the "hot" range pinned in L2 by the access-policy window.
-template <class S> struct PcRec { static constexpr int W = sizeof(S) == 4 ? 2 : 1; };
+// like a plane: record (k, slot) at pcr[k * Mpad + slot], one Vec4<S> (16 bytes in f32, 32 in f64).  Together with the body state that
+// precedes it in the same allocation (vel | dlt | counters | pcr) it is the "hot" range pinned in L2 by the access-policy window.
 // info lane of plane CP_IDX
 enum { CI_NP_MASK = 0x7, CI_ZERO1 = 1 << 4, CI_ZERO2 = 1 << 5, CI_NONDYN = 1 << 6, CI_TANGENT = 1 << 7,
        CI_VER1 = 1 << 8, CI_VER2 = 1 << 9,     // VERx: side x is a versioned body (has a SolverBody) in wavefront mode
@@ -69,16 +65,9 @@ struct DevSolver {
     int color_len[AVN_GRAPH_COLOR_COUNT];        // manifolds in the colour
     int wave;                                    // 1: wavefront (dependency-counter) substep loop, 0: grid barriers
     int* sm_slots;                               // [SMs] block tickets for the SM-major warp numbering of the wavefront loop (NULL = block-major)
-    int poll_ns;                                 // f32 wavefront: nanoseconds a warp sleeps after a failed poll (0 = spin)
-    int wave_rolled;                             // f32 wavefront: 1 = the rolled contact routines (throughput-bound steps), 0 = the unrolled ones
     unsigned int* ver;                           // [B+1] per-body event counter (wavefront mode)
     int* deg;                                    // [B+1] contact constraints touching the body (wavefront mode)
     int* stamp;                                  // [B+1] 1 + last colour that ranked the body: detects a body listed twice in one colour
-    // body-centric warm start (f32 wavefront schedule, wave32_dev.cuh "w32_ivw_item"): per body the constraints that move it, in colour order
-    int* wdeg;                                   // [B+1] adjacency entries of the body (sides whose inertia is not zeroed)
-    int* wpts;                                   // [B+1] contact points over those entries
-    uint2* adj;                                  // [ADJ_MAX][adj_stride] rank-major: {slot, WA_* | first point << 8}; NULL = slot-centric warm start
-    int adj_stride;
     int substeps, iters, rest_iters, fast_trig, match_contacts;
     S h, dt, max_overlap_speed, warm_coeff, rest_threshold, joint_force_rhs;
     S gx, gy, gz;
@@ -134,17 +123,10 @@ template <class S> __device__ __forceinline__ void stv3(S* p, int i, V3<S> v) { 
 
 // impulse record of point k of the manifold in `slot`
 template <class S> __device__ __forceinline__ Vec4<S>* pc_ptr(const DevSolver<S>& d, int k, int slot) {
-    return d.pcr + (size_t(k) * size_t(d.Mpad) + size_t(slot)) * PcRec<S>::W;
+    return d.pcr + size_t(k) * size_t(d.Mpad) + size_t(slot);
 }
-// store the value {lambda_n, sum, lt.x, lt.y} of an impulse record (f32: sequence tag 0)
-template <class S> __device__ __forceinline__ void pc_store(Vec4<S>* p, Vec4<S> v) {
-    if constexpr (PcRec<S>::W == 1) {
-        st4(p, v);
-    } else {
-        st4(p, mk4<S>(v.x, v.y, S(0), S(0)));
-        st4(p + 1, mk4<S>(v.z, v.w, S(0), S(0)));
-    }
-}
+// store the value {lambda_n, sum, lt.x, lt.y} of an impulse record
+template <class S> __device__ __forceinline__ void pc_store(Vec4<S>* p, Vec4<S> v) { st4(p, v); }
 
 template <class S> struct BodyInertia {
     V3<S> inv_mass;  // effective (locked axes applied)
@@ -351,16 +333,13 @@ __device__ __forceinline__ void apply_impulse(V3<S>& v1, V3<S>& w1, V3<S>& v2, V
 // An item may run when the counters of its bodies equal its position in their sequences, and bumps them when done.
 // Items are handed to warps in the global schedule order, all warps are co-resident (cooperative launch), and an item
 // only ever waits for items that precede it in that order, so the earliest unfinished item can always run: no deadlock.
-struct WaveStep { int substep, iters; };
-// flag words behind any_restitution: [0] some restitution coefficient != 0, [1] WAVE_* event, [2] a body has more than ADJ_MAX adjacency
-// entries (the step keeps the slot-centric warm start), [3] spare, then (8-byte aligned) the optional trace counters
-enum { FLAG_RESTITUTION = 0, FLAG_WAVE = 1, FLAG_ADJ_OVERFLOW = 2, FLAG_WORDS = 4 };
-// adjacency of the body-centric warm start: at most ADJ_MAX constraints per body (a cube in a brick stack has 8-10)
-constexpr int ADJ_MAX = 32;
-enum { WA_NP_MASK = 0x7, WA_TANGENT = 1 << 3, WA_SIDE2 = 1 << 4, WA_Q0_SHIFT = 8 };
+// flag words behind any_restitution: [0] some restitution coefficient != 0, [1] WAVE_* event, [2..3] spare, then (8-byte aligned) the
+// optional trace counters
+enum { FLAG_RESTITUTION = 0, FLAG_WAVE = 1, FLAG_WORDS = 4 };
 // Optional latency trace of the wavefront items (build with -DAVN_WAVE_TRACE; scripts/wave_trace.py): per-warp SM-cycle sums of
-// [0] dependency wait  [1] acquire fence + mutable loads + staged rows  [2] arithmetic  [3] stores + release fence + publish,
-// [4] item count.  The buffer is 8 unsigned long long counters behind the FLAG_WORDS int flags of any_restitution.
+// [0] wait for the exact event  [1] mutable loads (velocities, impulses) + staged rows  [2] arithmetic  [3] stores + release fence + publish,
+// [4] item count, [5] stage 1 of a solve item (wait for the deltas + the separations).  The buffer is 8 unsigned long long counters behind
+// the FLAG_WORDS int flags of any_restitution.
 #ifdef AVN_WAVE_TRACE
 #define AVN_TRACE_T(var) const long long var = clock64()
 #define AVN_TRACE_ADD(d, i, v) do { if ((threadIdx.x & 31) == 0) atomicAdd(reinterpret_cast<unsigned long long*>((d).any_restitution + FLAG_WORDS) + (i), (unsigned long long)(v)); } while (0)
@@ -368,29 +347,29 @@ enum { WA_NP_MASK = 0x7, WA_TANGENT = 1 << 3, WA_SIDE2 = 1 << 4, WA_Q0_SHIFT = 8
 #define AVN_TRACE_T(var)
 #define AVN_TRACE_ADD(d, i, v)
 #endif
-// wf = 1: the warm start is k events of the body (one per constraint, slot-centric warm items); wf = 0: it is part of the body's
-// integrate_velocities event (body-centric warm start, wave32_dev.cuh)
-__device__ __forceinline__ unsigned events_per_substep(int k, int iters, int wf = 1) { return 2u + unsigned(1 + wf + iters) * unsigned(k); }
+__device__ __forceinline__ unsigned events_per_substep(int k, int iters) { return 2u + unsigned(2 + iters) * unsigned(k); }
 enum { WV_IV = 0, WV_WARM = 1, WV_SOLVE = 2, WV_IP = 3, WV_RELAX = 4 };
 // position of an item in its body's event sequence
-__device__ __forceinline__ unsigned wave_event(int kind, int it, int s, int iters, int k, int r, int wf = 1) {
-    unsigned base = unsigned(s) * events_per_substep(k, iters, wf);
+__device__ __forceinline__ unsigned wave_event(int kind, int it, int s, int iters, int k, int r) {
+    unsigned base = unsigned(s) * events_per_substep(k, iters);
     switch (kind) {
         case WV_IV: return base;
         case WV_WARM: return base + 1u + r;
-        case WV_SOLVE: return base + 1u + unsigned(wf + it) * k + r;
-        case WV_IP: return base + 1u + unsigned(wf + iters) * k;
-        default: return base + 2u + unsigned(wf + iters) * k + r;
+        case WV_SOLVE: return base + 1u + unsigned(1 + it) * k + r;
+        case WV_IP: return base + 1u + unsigned(1 + iters) * k;
+        default: return base + 2u + unsigned(1 + iters) * k + r;
     }
 }
-// counters: relaxed gpu-scope accesses bracketed by __threadfence() (message passing).  ld.acquire.gpu / st.release.gpu on the
-// counters instead of the fences is the alternative; the fences are kept.
-__device__ __forceinline__ unsigned ld_relaxed(const unsigned* p) {
+// counters: message passing with acquire / release.  The consumer polls with ld.acquire.gpu (no membar: on sm_90 a strong load plus an
+// L1 invalidation) — each lane only reads data that its own counters guard, so the acquire of the poll that succeeds is all it needs.
+// The producer issues ONE fence.acq_rel.gpu after its data stores and then stores its counters relaxed (fence + strong store = release).
+__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
     unsigned v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
 __device__ __forceinline__ void st_relaxed(unsigned* p, unsigned v) { asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ void fence_acq_rel() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
 // mutable body / impulse data is read through L2 only in wavefront mode (other SMs write it while this kernel runs)
 __device__ __forceinline__ Vec4<float> ld4_cg(const Vec4<float>* p) {
     float4 v = __ldcg(reinterpret_cast<const float4*>(p));
@@ -402,30 +381,26 @@ __device__ __forceinline__ Vec4<double> ld4_cg(const Vec4<double>* p) {
 }
 template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> ldm(const Vec4<S>* p) { return WAVE ? ld4_cg(p) : ld4(p); }
 // the value {lambda_n, sum, lt.x, lt.y} of an impulse record
-template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> pc_load(const Vec4<S>* p) {
-    if constexpr (PcRec<S>::W == 1) {
-        return ldm<WAVE>(p);
-    } else {
-        const Vec4<S> a = ldm<WAVE>(p), b = ldm<WAVE>(p + 1);
-        return mk4<S>(a.x, a.y, b.x, b.y);
-    }
-}
+template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> pc_load(const Vec4<S>* p) { return ldm<WAVE>(p); }
 
-// warp-synchronous wait: all 32 lanes of the warp wait until every lane's two counters have reached their targets
+// warp-synchronous wait: all 32 lanes of the warp wait until every lane's two counters have reached their targets — exactly (EXACT) or
+// at least (counters only grow).  A lane stops polling a counter once it has seen its target: with EXACT the counter cannot move on
+// before this item publishes, and either way the acquire of that poll orders the loads that follow it.
 // A watchdog bounds the spin (a schedule bug must not hang the device): after ~4M polls the warp gives up and raises
 // *watchdog, which the host turns into an error.
+template <bool EXACT = true>
 __device__ __forceinline__ void wave_wait(const unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2, int* watchdog) {
     for (unsigned spins = 0;; ++spins) {
-        bool ok = (!need1 || ld_relaxed(ver + b1) == e1) && (!need2 || ld_relaxed(ver + b2) == e2);
-        if (__all_sync(0xffffffffu, ok)) break;
+        if (need1) { const unsigned v = ld_acquire(ver + b1); need1 = EXACT ? v != e1 : v < e1; }
+        if (need2) { const unsigned v = ld_acquire(ver + b2); need2 = EXACT ? v != e2 : v < e2; }
+        if (__all_sync(0xffffffffu, !(need1 || need2))) break;
         if (spins > (1u << 22)) { *watchdog = 1; break; }
     }
-    __threadfence();  // acquire: the loads below must observe what the publishers wrote before bumping the counters
 }
 // n1 / n2 = events this item consumed on each body (2 when it also ran the body's integrate step)
 __device__ __forceinline__ void wave_publish(unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2, unsigned n1 = 1u,
                                              unsigned n2 = 1u) {
-    __threadfence();  // release: this item's stores are visible before the counters move
+    fence_acq_rel();  // release: this item's stores are visible before the counters move
     if (need1) st_relaxed(ver + b1, e1 + n1);
     if (need2) st_relaxed(ver + b2, e2 + n2);
 }
@@ -448,25 +423,24 @@ __device__ __forceinline__ void stage_copy(Vec4<double>* dst, const Vec4<double>
 }
 // the tile only needs the rows of the widest manifold of the upload (single-point sphere contacts: a quarter of the tile, the rest
 // of the SM's shared-memory / L1 array stays L1)
-// (3 staged rows per point + 1 scratch row per point for its impulses + 1 row of separations: wave32_dev.cuh)
+// (3 staged rows per point + 1 scratch row per point for its impulses + 1 row of separations: wave_contact_item)
 template <class S> __host__ __device__ constexpr size_t stage_bytes(int threads, int max_points = AVN_MAX_MANIFOLD_POINTS) {
     return size_t(4 * max_points + 1) * threads * sizeof(Vec4<S>);
 }
 
-// `slot` indexes the padded colour-major planes.  WAVE = false: barrier mode (a padding slot returns at once).
-// WAVE = true: every lane of the warp must call this (warp-collective wait); `ws` carries the position in the schedule.
+// Barrier schedules (grid-wide phases, island groups, phase kernels); the wavefront schedule runs wave_contact_item below.
+// `slot` indexes the padded colour-major planes (a padding slot returns at once).
 // MAXP: compile-time bound on the points of a manifold (1 for sphere-only scenes: a quarter of the registers and no dead unrolled code)
-template <class S, int PASS, bool WAVE = false, int MAXP = AVN_MAX_MANIFOLD_POINTS>
-__device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, int wave_substep = 0, int wave_it = 0, bool lane_active = true) {
+template <class S, int PASS, int MAXP = AVN_MAX_MANIFOLD_POINTS>
+__device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot) {
     const size_t MP = size_t(d.Mpad);
-    Vec4<S>* c = d.cst + (lane_active ? slot : 0);
+    Vec4<S>* c = d.cst + slot;
     Vec4<S> hidx = ld4(&c[CP_IDX * MP]);
-    const int info = lane_active ? as_int(hidx.z) : 0;   // an inactive lane of a partial chunk behaves like a padding slot
+    const int info = as_int(hidx.z);
     const int np = info & CI_NP_MASK;
-    if (!WAVE && np == 0) return;
+    if (np == 0) return;
     const int b1 = as_int(hidx.x), b2 = as_int(hidx.y);
-    // ---- issue every load up front (independent 128-bit loads -> memory-level parallelism).  In wavefront mode the
-    //      immutable part (planes written by prepare only, inertia) is fetched BEFORE waiting on the counters.
+    // ---- issue every load up front (independent 128-bit loads -> memory-level parallelism)
     Vec4<S> hn = mk4<S>(0, 0, 0, 0), ht1 = hn, htv = hn;
     BodyInertia<S> in1 = zero_inertia<S>(), in2 = zero_inertia<S>();
     Vec4<S> PC[MAXP];
@@ -476,7 +450,7 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
 #define ROW_A(k) stage[(3 * (k) + 0) * T]
 #define ROW_B(k) stage[(3 * (k) + 1) * T]
 #define ROW_D(k) stage[(3 * (k) + 2) * T]
-    if (np != 0) {
+    {
         hn = ld4(&c[CP_N * MP]);
         ht1 = ld4(&c[CP_T1 * MP]);
         if (SOLVE) htv = ld4(&c[CP_TV * MP]);
@@ -492,57 +466,18 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
         }
     }
     __pipeline_commit();
-    unsigned e1 = 0, e2 = 0;
-    const bool ver1 = WAVE && np != 0 && (info & CI_VER1), ver2 = WAVE && np != 0 && (info & CI_VER2);
-    // fused integrate steps (wavefront mode): the last relax event of a body also runs its next integrate_velocities, the last
-    // biased-solve event also runs its integrate_positions — same arithmetic on the same registers, one dependency level less each
-#ifdef AVN_FUSE_IV
-    const bool fiv1 = WAVE && PASS == PASS_RELAX && (info & CI_FIV1) && wave_substep + 1 < d.substeps;
-    const bool fiv2 = WAVE && PASS == PASS_RELAX && (info & CI_FIV2) && wave_substep + 1 < d.substeps;
-#else
-    constexpr bool fiv1 = false, fiv2 = false;
-#endif
-#ifdef AVN_FUSE_IP
-    const bool fip1 = WAVE && PASS == PASS_SOLVE_BIAS && (info & CI_FIP1) && wave_it + 1 == d.iters;
-    const bool fip2 = WAVE && PASS == PASS_SOLVE_BIAS && (info & CI_FIP2) && wave_it + 1 == d.iters;
-#else
-    constexpr bool fip1 = false, fip2 = false;
-#endif
-    Vec4<S> il1, ia1, il2, ia2;   // VelocityIntegrationData rows (immutable): fetched before the wait
-    if (fiv1) { il1 = ld4(&d.itg[2 * b1]); ia1 = ld4(&d.itg[2 * b1 + 1]); }
-    if (fiv2) { il2 = ld4(&d.itg[2 * b2]); ia2 = ld4(&d.itg[2 * b2 + 1]); }
-    if (WAVE) {
-        const int rk = as_int(hidx.w);
-        const int kind = PASS == PASS_WARM ? WV_WARM : (PASS == PASS_SOLVE_BIAS ? WV_SOLVE : WV_RELAX);
-        e1 = wave_event(kind, wave_it, wave_substep, d.iters, (rk >> 8) & 0xff, rk & 0xff);
-        e2 = wave_event(kind, wave_it, wave_substep, d.iters, (rk >> 24) & 0xff, (rk >> 16) & 0xff);
-        AVN_TRACE_T(t_w0);
-        wave_wait(d.ver, ver1, b1, e1, ver2, b2, e2, d.any_restitution + 1);
-        AVN_TRACE_ADD(d, 0, clock64() - t_w0);
-        if (np == 0) return;  // padding slot: nothing to do (after the warp-collective wait)
-    }
     // ---- mutable state: body velocities / deltas and the accumulated impulses
-    AVN_TRACE_T(t_l0);
-    Vec4<S> l1 = ldm<WAVE>(&d.vel[2 * b1]), a1 = ldm<WAVE>(&d.vel[2 * b1 + 1]);
-    Vec4<S> l2 = ldm<WAVE>(&d.vel[2 * b2]), a2 = ldm<WAVE>(&d.vel[2 * b2 + 1]);
+    Vec4<S> l1 = ld4(&d.vel[2 * b1]), a1 = ld4(&d.vel[2 * b1 + 1]);
+    Vec4<S> l2 = ld4(&d.vel[2 * b2]), a2 = ld4(&d.vel[2 * b2 + 1]);
     Vec4<S> dp1, dq1, dp2, dq2;
     if (SOLVE) {
-        dp1 = ldm<WAVE>(&d.dlt[2 * b1]); dq1 = ldm<WAVE>(&d.dlt[2 * b1 + 1]);
-        dp2 = ldm<WAVE>(&d.dlt[2 * b2]); dq2 = ldm<WAVE>(&d.dlt[2 * b2 + 1]);
+        dp1 = ld4(&d.dlt[2 * b1]); dq1 = ld4(&d.dlt[2 * b1 + 1]);
+        dp2 = ld4(&d.dlt[2 * b2]); dq2 = ld4(&d.dlt[2 * b2 + 1]);
     }
 #pragma unroll
     for (int k = 0; k < MAXP; ++k)
-        if (k < np) PC[k] = pc_load<WAVE>(pc_ptr(d, k, slot));
+        if (k < np) PC[k] = pc_load<false>(pc_ptr(d, k, slot));
     __pipeline_wait_prior(0);  // this thread's staged rows have landed (only the issuing thread reads them)
-#ifdef AVN_WAVE_TRACE
-    if (WAVE) {  // force the loads to complete here so the segments separate cleanly
-        S sink = l1.x + a1.x + l2.x + a2.x + PC[0].x;
-        if (SOLVE) sink += dq1.x + dq2.x;
-        if (sink == S(1.2345e33)) d.any_restitution[1] = 2;
-    }
-    AVN_TRACE_T(t_c0);
-    if (WAVE) AVN_TRACE_ADD(d, 1, t_c0 - t_l0);
-#endif
     V3<S> v1 = xyz(l1), w1 = xyz(a1), v2 = xyz(l2), w2 = xyz(a2);
     const V3<S> n = xyz(hn), t1 = xyz(ht1);
     const V3<S> t2 = cross(t1, n);  // tangent_directions(): [tangent1, tangent1 x normal] (contact/mod.rs:411-421)
@@ -653,37 +588,256 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
             }
         }
     }
-    // ---- write back: impulses (plane 6+4k) and the velocities of the non-dominant sides
-#ifdef AVN_WAVE_TRACE
-    if (WAVE && (v1.x + v2.x + w1.x + w2.x) == S(1.2345e33)) d.any_restitution[1] = 2;
-    AVN_TRACE_T(t_s0);
-    if (WAVE) AVN_TRACE_ADD(d, 2, t_s0 - t_c0);
-#endif
+    // ---- write back: impulses and the velocities of the non-dominant sides
     if (PASS != PASS_WARM) {
 #pragma unroll
         for (int k = 0; k < MAXP; ++k)
             if (k < np) pc_store(pc_ptr(d, k, slot), PC[k]);
     }
-    if (WAVE && SOLVE) {
-        // integrate_positions of a body whose last solve event this is (integrator/mod.rs:503-535): dp += v h, dq = exp(w h) dq
-        if (fip1) {
-            V3<S> ndp = xyz(dp1) + v1 * d.h;
-            Q4<S> q; q.x = dq1.x; q.y = dq1.y; q.z = dq1.z; q.w = dq1.w;
-            Q4<S> nq = qmul(q_from_scaled_axis(w1 * d.h, d.fast_trig != 0), q);
-            st4(&d.dlt[2 * b1], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
-            st4(&d.dlt[2 * b1 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
-        }
-        if (fip2) {
-            V3<S> ndp = xyz(dp2) + v2 * d.h;
-            Q4<S> q; q.x = dq2.x; q.y = dq2.y; q.z = dq2.z; q.w = dq2.w;
-            Q4<S> nq = qmul(q_from_scaled_axis(w2 * d.h, d.fast_trig != 0), q);
-            st4(&d.dlt[2 * b2], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
-            st4(&d.dlt[2 * b2 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
-        }
-        // integrate_velocities of the NEXT substep for a body whose last relax event this is (integrator/mod.rs:362-368)
-        if (fiv1) { v1 = v1 * il1.w; w1 = w1 * ia1.w; v1 = v1 + xyz(il1); w1 = w1 + xyz(ia1); }
-        if (fiv2) { v2 = v2 * il2.w; w2 = w2 * ia2.w; v2 = v2 + xyz(il2); w2 = w2 + xyz(ia2); }
+    if (!(info & CI_ZERO1)) {
+        st4(&d.vel[2 * b1], mk4<S>(v1.x, v1.y, v1.z, S(0)));
+        st4(&d.vel[2 * b1 + 1], mk4<S>(w1.x, w1.y, w1.z, S(0)));
     }
+    if (!(info & CI_ZERO2)) {
+        st4(&d.vel[2 * b2], mk4<S>(v2.x, v2.y, v2.z, S(0)));
+        st4(&d.vel[2 * b2 + 1], mk4<S>(w2.x, w2.y, w2.z, S(0)));
+    }
+#undef ROW_A
+#undef ROW_B
+#undef ROW_D
+}
+
+// ---- wavefront mode: warm_start / solve_contacts<BIAS> / relax of ONE manifold --------------------------------------------------------
+// The same arithmetic in the same order as contact_item (bit-identical); what differs is where the operands live and when the item waits.
+//   * Rolled point loops.  Each point's impulses and separation live in this thread's scratch rows of the staging tile (rows 3*MAXP + k and
+//     4*MAXP), so no register array is indexed dynamically and nothing goes to local memory.  One routine serves the biased and the relax
+//     pass (`relax`): fewer routines compete for the SM's instruction cache, whose warps are in several routines at once.
+//   * Two-stage wait (solve passes).  A body's deltas change only at its integrate_positions, so stage 1 waits until each body's counter has
+//     passed the integrate_positions event that wrote the deltas this pass reads — nearly always true at the first look — then loads them and
+//     computes every point's separation.  Stage 2 waits for the exact event and loads the velocities and impulses.  The two quaternion
+//     rotations per point are off the dependent chain.
+//   * Acquire / release counters (wave_wait / wave_publish): no membar after a successful poll, one fence before the counter stores.
+// PASS = PASS_WARM or PASS_SOLVE_BIAS.  Every lane of the warp must call this (warp-collective waits); an inactive lane of a partial chunk
+// behaves like a padding slot.  Counters count from the prepare launch on, so `s` is the absolute substep index in every launch of a step.
+template <class S, int PASS, int MAXP>
+__device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slot, int s, int it, bool lane_active, bool relax) {
+    constexpr bool SOLVE = PASS == PASS_SOLVE_BIAS;
+    relax = SOLVE && relax;
+    const size_t MP = size_t(d.Mpad);
+    const Vec4<S>* c = d.cst + (lane_active ? slot : 0);
+    const Vec4<S> hidx = ld4(&c[CP_IDX * MP]);
+    const int info = lane_active ? as_int(hidx.z) : 0;
+    const int np = info & CI_NP_MASK;
+    const int b1 = as_int(hidx.x), b2 = as_int(hidx.y);
+    Vec4<S>* const stage = stage_base<S>() + threadIdx.x;   // this thread's column; row r at stage[r * T]
+    const int T = blockDim.x;
+#define ROW_A(k) stage[(3 * (k) + 0) * T]
+#define ROW_B(k) stage[(3 * (k) + 1) * T]
+#define ROW_D(k) stage[(3 * (k) + 2) * T]
+#define ROW_PC(k) stage[(3 * MAXP + (k)) * T]
+    S* const sepv = reinterpret_cast<S*>(&stage[(4 * MAXP) * T]);
+    // ---- immutable part (planes written by prepare, inertia): issued before any wait
+    Vec4<S> hn = mk4<S>(0, 0, 0, 0), ht1 = hn, htv = hn;
+    BodyInertia<S> in1 = zero_inertia<S>(), in2 = zero_inertia<S>();
+    if (np != 0) {
+        hn = ld4(&c[CP_N * MP]);
+        ht1 = ld4(&c[CP_T1 * MP]);
+        if (SOLVE) htv = ld4(&c[CP_TV * MP]);
+        if (!(info & CI_ZERO1)) in1 = unpack_inertia(ld4(&d.inr[2 * b1]), ld4(&d.inr[2 * b1 + 1]));
+        if (!(info & CI_ZERO2)) in2 = unpack_inertia(ld4(&d.inr[2 * b2]), ld4(&d.inr[2 * b2 + 1]));
+#pragma unroll 1
+        for (int k = 0; k < np; ++k) {
+            stage_copy(&ROW_A(k), &c[size_t(CP_ROW(k, 0)) * MP]);
+            stage_copy(&ROW_B(k), &c[size_t(CP_ROW(k, 1)) * MP]);
+            if (SOLVE && (info & CI_TANGENT)) stage_copy(&ROW_D(k), &c[size_t(CP_ROW(k, 2)) * MP]);
+        }
+    }
+    __pipeline_commit();
+    const bool ver1 = np != 0 && (info & CI_VER1), ver2 = np != 0 && (info & CI_VER2);
+    const int rk = as_int(hidx.w);
+    const int k1 = (rk >> 8) & 0xff, k2 = (rk >> 24) & 0xff;
+    const int kind = SOLVE ? (relax ? WV_RELAX : WV_SOLVE) : WV_WARM;
+    const unsigned e1 = wave_event(kind, it, s, d.iters, k1, rk & 0xff);
+    const unsigned e2 = wave_event(kind, it, s, d.iters, k2, (rk >> 16) & 0xff);
+    // fused integrate steps (experiments, off by default: prepare_body_item): the last relax event of a body also runs its next
+    // integrate_velocities, the last biased-solve event its integrate_positions
+#ifdef AVN_FUSE_IV
+    const bool fiv1 = relax && (info & CI_FIV1) && s + 1 < d.substeps, fiv2 = relax && (info & CI_FIV2) && s + 1 < d.substeps;
+#else
+    constexpr bool fiv1 = false, fiv2 = false;
+#endif
+#ifdef AVN_FUSE_IP
+    const bool fip1 = SOLVE && !relax && (info & CI_FIP1) && it + 1 == d.iters, fip2 = SOLVE && !relax && (info & CI_FIP2) && it + 1 == d.iters;
+#else
+    constexpr bool fip1 = false, fip2 = false;
+#endif
+    Vec4<S> il1, ia1, il2, ia2;   // VelocityIntegrationData rows (immutable): fetched before the wait
+    if (fiv1) { il1 = ld4(&d.itg[2 * b1]); ia1 = ld4(&d.itg[2 * b1 + 1]); }
+    if (fiv2) { il2 = ld4(&d.itg[2 * b2]); ia2 = ld4(&d.itg[2 * b2 + 1]); }
+    int* const watchdog = d.any_restitution + FLAG_WAVE;
+    const V3<S> n = xyz(hn), t1 = xyz(ht1);
+
+    // ---- stage 1 (solve passes): the deltas -> the separation of every point, before the velocities are waited for
+    if (SOLVE) {
+        AVN_TRACE_T(t_d0);
+        const int sd = relax ? s : s - 1;   // the substep whose integrate_positions wrote the deltas this pass reads (-1: prepare did)
+        if (sd >= 0)
+            wave_wait<false>(d.ver, ver1, b1, wave_event(WV_IP, 0, sd, d.iters, k1, 0) + 1u, ver2, b2, wave_event(WV_IP, 0, sd, d.iters, k2, 0) + 1u,
+                             watchdog);
+        __pipeline_wait_prior(0);   // this thread's staged rows have landed (only the issuing thread reads them)
+        if (np != 0) {
+            const Vec4<S> dp1 = ld4_cg(&d.dlt[2 * b1]), dq1 = ld4_cg(&d.dlt[2 * b1 + 1]);
+            const Vec4<S> dp2 = ld4_cg(&d.dlt[2 * b2]), dq2 = ld4_cg(&d.dlt[2 * b2 + 1]);
+            Q4<S> q1; q1.x = dq1.x; q1.y = dq1.y; q1.z = dq1.z; q1.w = dq1.w;
+            Q4<S> q2; q2.x = dq2.x; q2.y = dq2.y; q2.z = dq2.z; q2.w = dq2.w;
+            const V3<S> delta_translation = xyz(dp2) - xyz(dp1);
+#pragma unroll 1
+            for (int k = 0; k < np; ++k) {
+                const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k);
+                V3<S> rr1 = qrot(q1, xyz(PAk)), rr2 = qrot(q2, xyz(PBk));
+                V3<S> dsep = delta_translation + (rr2 - rr1);
+                sepv[k] = dot(dsep, n) + PAk.w;
+            }
+        }
+#ifdef AVN_WAVE_TRACE
+        if (np != 0 && sepv[0] == S(1.2345e33)) d.any_restitution[1] = 2;   // the separations are done here
+        AVN_TRACE_ADD(d, 5, clock64() - t_d0);
+#endif
+    }
+
+    // ---- stage 2: the exact event, then the velocities of the two bodies and the impulses of the points
+    AVN_TRACE_T(t_w0);
+    wave_wait(d.ver, ver1, b1, e1, ver2, b2, e2, watchdog);
+    AVN_TRACE_ADD(d, 0, clock64() - t_w0);
+    if (np == 0) return;   // padding slot / inactive lane (after the warp-collective waits)
+    AVN_TRACE_T(t_l0);
+    const Vec4<S> l1 = ld4_cg(&d.vel[2 * b1]), a1 = ld4_cg(&d.vel[2 * b1 + 1]);
+    const Vec4<S> l2 = ld4_cg(&d.vel[2 * b2]), a2 = ld4_cg(&d.vel[2 * b2 + 1]);
+    {   // all impulse loads in flight at once, then parked in the scratch rows
+        Vec4<S> pc[MAXP];
+#pragma unroll
+        for (int k = 0; k < MAXP; ++k)
+            if (k < np) pc[k] = pc_load<true>(pc_ptr(d, k, slot));
+#pragma unroll
+        for (int k = 0; k < MAXP; ++k)
+            if (k < np) ROW_PC(k) = pc[k];
+    }
+    if (!SOLVE) __pipeline_wait_prior(0);
+#ifdef AVN_WAVE_TRACE
+    if ((l1.x + a1.x + l2.x + a2.x) == S(1.2345e33)) d.any_restitution[1] = 2;   // force the loads to complete here
+    AVN_TRACE_T(t_c0);
+    AVN_TRACE_ADD(d, 1, t_c0 - t_l0);
+#endif
+    V3<S> v1 = xyz(l1), w1 = xyz(a1), v2 = xyz(l2), w2 = xyz(a2);
+    const V3<S> t2 = cross(t1, n);  // tangent_directions(): [tangent1, tangent1 x normal] (contact/mod.rs:411-421)
+
+    if (!SOLVE) {
+        // ContactConstraint::warm_start (contact/mod.rs:223-264)
+#pragma unroll 1
+        for (int k = 0; k < np; ++k) {
+            const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k), pck = ROW_PC(k);
+            V3<S> r1 = xyz(PAk), r2 = xyz(PBk);
+            S tx = (info & CI_TANGENT) ? pck.z : S(0), ty = (info & CI_TANGENT) ? pck.w : S(0);
+            V3<S> p = d.warm_coeff * ((pck.x * n + tx * t1) + ty * t2);
+            apply_impulse(v1, w1, v2, w2, in1, in2, r1, r2, p);
+        }
+    } else {
+        // ContactConstraint::solve (contact/mod.rs:267-354)
+        const Soft<S> soft = (info & CI_NONDYN) ? d.soft_nondyn : d.soft_dyn;
+#pragma unroll 1
+        for (int k = 0; k < np; ++k) {
+            const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k);
+            Vec4<S> pck = ROW_PC(k);
+            V3<S> r1 = xyz(PAk), r2 = xyz(PBk);
+            const S separation = sepv[k];
+            V3<S> relv = (v2 + cross(w2, r2)) - (v1 + cross(w1, r1));
+            // ContactNormalPart::solve_impulse (normal_part.rs:116-166)
+            S vn = dot(relv, n);
+            S meff = PBk.w, acc = pck.x;
+            S impulse;
+            if (separation > S(0)) {
+                impulse = -meff * (vn + separation / d.h);
+            } else if (!relax) {
+                S bias = avn_max(soft.bias * separation, -d.max_overlap_speed);
+                S scaled_mass = soft.mass_scale * meff;
+                S scaled_impulse = soft.impulse_scale * acc;
+                impulse = -scaled_mass * (vn + bias) - scaled_impulse;
+            } else {
+                impulse = -meff * vn;
+            }
+            S new_impulse = avn_max(acc + impulse, S(0));
+            impulse = new_impulse - acc;
+            pck.x = new_impulse;
+            pck.y = pck.y + new_impulse;
+            ROW_PC(k) = pck;
+            apply_impulse(v1, w1, v2, w2, in1, in2, r1, r2, impulse * n);
+        }
+        if (info & CI_TANGENT) {
+            const S friction = hn.w;
+            const V3<S> surf = xyz(htv);
+#pragma unroll 1
+            for (int k = 0; k < np; ++k) {
+                const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k), PDk = ROW_D(k);
+                Vec4<S> pck = ROW_PC(k);
+                V3<S> r1 = xyz(PAk), r2 = xyz(PBk);
+                V3<S> relv = (v2 + cross(w2, r2)) - (v1 + cross(w1, r1));
+                // ContactTangentPart::solve_impulse (tangent_part.rs:155-244)
+                S limit = friction * pck.x;
+                relv = relv + surf;
+                S ts1 = dot(relv, t1), ts2 = dot(relv, t2);
+                S t11 = ts1 * ts1, t22 = ts2 * ts2, t12 = ts1 * ts2;
+                S inv = (t11 * PDk.x + t22 * PDk.y) + t12 * PDk.z;
+                S em = (t11 + t22) * (S(1) / inv);
+                V3<S> imp = zero3<S>();
+                if (avn_finite(em)) {
+                    S nx = pck.z - em * ts1, ny = pck.w - em * ts2;
+                    S l2 = nx * nx + ny * ny;
+                    if (l2 > limit * limit) {  // Vec2::clamp_length_max
+                        S l = avn_sqrt(l2);
+                        nx = limit * (nx / l);
+                        ny = limit * (ny / l);
+                    }
+                    S dx = nx - pck.z, dy = ny - pck.w;
+                    pck.z = nx;
+                    pck.w = ny;
+                    ROW_PC(k) = pck;
+                    imp = dx * t1 + dy * t2;
+                }
+                apply_impulse(v1, w1, v2, w2, in1, in2, r1, r2, imp);
+            }
+        }
+    }
+    // ---- write back: impulses, the velocities of the non-dominant sides, then the counters
+#ifdef AVN_WAVE_TRACE
+    if ((v1.x + v2.x + w1.x + w2.x) == S(1.2345e33)) d.any_restitution[1] = 2;
+    AVN_TRACE_T(t_s0);
+    AVN_TRACE_ADD(d, 2, t_s0 - t_c0);
+#endif
+    if (SOLVE) {
+#pragma unroll 1
+        for (int k = 0; k < np; ++k) pc_store(pc_ptr(d, k, slot), ROW_PC(k));
+    }
+    // integrate_positions of a body whose last biased-solve event this is (integrator/mod.rs:503-535): dp += v h, dq = exp(w h) dq.  Its
+    // deltas are the ones stage 1 read (nothing else writes them before this item publishes).
+    if (fip1) {
+        const Vec4<S> dp = ld4_cg(&d.dlt[2 * b1]), dq4 = ld4_cg(&d.dlt[2 * b1 + 1]);
+        V3<S> ndp = xyz(dp) + v1 * d.h;
+        Q4<S> q; q.x = dq4.x; q.y = dq4.y; q.z = dq4.z; q.w = dq4.w;
+        Q4<S> nq = qmul(q_from_scaled_axis(w1 * d.h, d.fast_trig != 0), q);
+        st4(&d.dlt[2 * b1], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
+        st4(&d.dlt[2 * b1 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
+    }
+    if (fip2) {
+        const Vec4<S> dp = ld4_cg(&d.dlt[2 * b2]), dq4 = ld4_cg(&d.dlt[2 * b2 + 1]);
+        V3<S> ndp = xyz(dp) + v2 * d.h;
+        Q4<S> q; q.x = dq4.x; q.y = dq4.y; q.z = dq4.z; q.w = dq4.w;
+        Q4<S> nq = qmul(q_from_scaled_axis(w2 * d.h, d.fast_trig != 0), q);
+        st4(&d.dlt[2 * b2], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
+        st4(&d.dlt[2 * b2 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
+    }
+    // integrate_velocities of the NEXT substep for a body whose last relax event this is (integrator/mod.rs:362-368)
+    if (fiv1) { v1 = v1 * il1.w; w1 = w1 * ia1.w; v1 = v1 + xyz(il1); w1 = w1 + xyz(ia1); }
+    if (fiv2) { v2 = v2 * il2.w; w2 = w2 * ia2.w; v2 = v2 + xyz(il2); w2 = w2 + xyz(ia2); }
     if (!(info & CI_ZERO1) || fiv1) {
         st4(&d.vel[2 * b1], mk4<S>(v1.x, v1.y, v1.z, S(0)));
         st4(&d.vel[2 * b1 + 1], mk4<S>(w1.x, w1.y, w1.z, S(0)));
@@ -692,13 +846,15 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot, in
         st4(&d.vel[2 * b2], mk4<S>(v2.x, v2.y, v2.z, S(0)));
         st4(&d.vel[2 * b2 + 1], mk4<S>(w2.x, w2.y, w2.z, S(0)));
     }
-    if (WAVE) wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2, (fiv1 || fip1) ? 2u : 1u, (fiv2 || fip2) ? 2u : 1u);
+    wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2, (fiv1 || fip1) ? 2u : 1u, (fiv2 || fip2) ? 2u : 1u);
 #ifdef AVN_WAVE_TRACE
-    if (WAVE) { AVN_TRACE_ADD(d, 3, clock64() - t_s0); AVN_TRACE_ADD(d, 4, 1); }
+    AVN_TRACE_ADD(d, 3, clock64() - t_s0);
+    AVN_TRACE_ADD(d, 4, 1);
 #endif
 #undef ROW_A
 #undef ROW_B
 #undef ROW_D
+#undef ROW_PC
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -824,22 +980,6 @@ __device__ __forceinline__ void wave_rank_item(const DevSolver<S>& d, int slot) 
     if (info & CI_VER1) { bad |= atomicExch(&d.stamp[b1], colour + 1) == colour + 1; r1 = atomicAdd(&d.deg[b1], 1); }
     if (info & CI_VER2) { bad |= atomicExch(&d.stamp[b2], colour + 1) == colour + 1; r2 = atomicAdd(&d.deg[b2], 1); }
     if (bad || r1 > 0xfe || r2 > 0xfe) d.any_restitution[1] = WAVE_BAD_COLOURING;
-    if (d.adj) {
-        // adjacency of the body-centric warm start: one entry per side this constraint moves (a side with zeroed inertia keeps its
-        // velocity bit for bit).  The colours are ranked one after the other, so entry order = colour order = the reference's order.
-        const unsigned meta = unsigned(info & CI_NP_MASK) | ((info & CI_TANGENT) ? WA_TANGENT : 0u);
-        const int np = info & CI_NP_MASK;
-        if ((info & CI_VER1) && !(info & CI_ZERO1)) {
-            const int j = atomicAdd(&d.wdeg[b1], 1), q0 = atomicAdd(&d.wpts[b1], np);
-            if (j < ADJ_MAX) d.adj[size_t(j) * d.adj_stride + b1] = make_uint2(unsigned(slot), meta | (unsigned(q0) << WA_Q0_SHIFT));
-            else d.any_restitution[FLAG_ADJ_OVERFLOW] = 1;
-        }
-        if ((info & CI_VER2) && !(info & CI_ZERO2)) {
-            const int j = atomicAdd(&d.wdeg[b2], 1), q0 = atomicAdd(&d.wpts[b2], np);
-            if (j < ADJ_MAX) d.adj[size_t(j) * d.adj_stride + b2] = make_uint2(unsigned(slot), meta | WA_SIDE2 | (unsigned(q0) << WA_Q0_SHIFT));
-            else d.any_restitution[FLAG_ADJ_OVERFLOW] = 1;
-        }
-    }
     hidx.w = int_as(S(0), (r1 & 0xff) | ((r2 & 0xff) << 16));
     st4(&c[CP_IDX * MP], hidx);
 }

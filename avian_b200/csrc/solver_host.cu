@@ -55,11 +55,9 @@ class Solver final : public SolverBase {
         // latency, fewer registers spill more.  Measured best (scripts/solver_timing.py): 3 blocks/SM for f32, 2 for f64 (whose
         // state is twice as wide).  AVN_MEGA_BPS = 2|3|4 overrides the default for experiments.
         const char* bps = getenv("AVN_MEGA_BPS");
-        bps_forced_ = bps != nullptr;
         mega_bps_ = bps ? atoi(bps) : (sizeof(S) == 8 ? 2 : 3);
         if (mega_bps_ < 2 || mega_bps_ > 6) mega_bps_ = 3;
         if (mode && !strcmp(mode, "wave")) force_wave_ = true;
-        if (const char* w = getenv("AVN_WARM_BY_BODY")) warm_by_body_ = atoi(w) != 0;
         if (const char* w = getenv("AVN_ISLAND_MODE")) island_mode_ = atoi(w) != 0;
         if (const char* w = getenv("AVN_WAVE_SM_ORDER")) sm_order_ = atoi(w) != 0;
         coop_ok_ = coop_ok_ && select_megakernel(AVN_MAX_MANIFOLD_POINTS);
@@ -200,7 +198,6 @@ class Solver final : public SolverBase {
     bool coop_ok_ = false, use_mega_ = true, use_wave_ = true, l2_persist_ = false;
     size_t l2_persist_bytes_ = 0, l2_window_max_ = 0;
     int mega_grid_ = 0, mega_bps_ = 3, mega_maxp_ = 0, mega_sel_bps_ = 0;
-    bool bps_forced_ = false;
     bool force_wave_ = false;
 
     // The persistent kernel is compiled per (blocks/SM, widest manifold): MAXP = 1 (sphere-only scenes) drops the unrolled code and the
@@ -216,11 +213,8 @@ class Solver final : public SolverBase {
             default: return (const void*)step_megakernel<S, 3, MAXP>;
         }
     }
-    // blocks per SM of a step: the f32 wavefront routines fit 128 registers without spills (the delta records die before the main loop), so a
-    // wavefront-scheduled f32 step runs 4 blocks = 16 warps per SM; the barrier schedule runs 3 for f32, 2 for f64 (register budget).  AVN_MEGA_BPS overrides both.
     // dynamic shared memory of the persistent kernel: the per-thread cp.async tile of the contact routines
     static size_t mega_smem_bytes(int maxp) { return stage_bytes<S>(MEGA_BLOCK, maxp); }
-    int bps_for(bool wave_candidate) const { return bps_forced_ ? mega_bps_ : ((sizeof(S) == 4 && wave_candidate) ? 4 : mega_bps_); }
     bool select_megakernel(int max_points, int bps = 0) {
         const int maxp = max_points <= 1 ? 1 : AVN_MAX_MANIFOLD_POINTS;
         if (bps == 0) bps = mega_bps_;
@@ -287,7 +281,7 @@ class Solver final : public SolverBase {
     DevBuf o_pos_, o_rot_, o_lv_, o_av_;
     DevBuf s_inr_, s_itg_, s_pre_;
     DevBuf m_b1_, m_b2_, m_n_, m_f_, m_r_, m_tv_, m_po_, p_a1_, p_a2_, p_pen_, p_ns_, p_wn_, p_wt_, p_ni_, p_nin_, p_own_, p_owt_;
-    DevBuf hot_, c_flag_, adj_, isl_buf_, sm_slots_;
+    DevBuf hot_, c_flag_, isl_buf_, sm_slots_;
     bool sm_order_ = false;
     IslandLists isl_;
     std::vector<int> isl_jb1_, isl_jb2_;
@@ -295,10 +289,6 @@ class Solver final : public SolverBase {
     // was built for (5 000 ragdolls) when it was introduced — every block is in a different phase, so the SM's
     // instruction stream thrashes, and an island's few joints per level keep one warp busy.  Off by default; AVN_ISLAND_MODE=1 enables it.
     bool island_mode_ = false;
-    // body-centric warm start (wave32_dev.cuh w32_ivw_item): bit-identical, 26 -> 18 dependency levels per substep, but slower where
-    // it matters when it was introduced (100k cubes: the item is a chain of dependent gathers, 4x more chunks than integrate_velocities had)
-    // and only slightly faster on the chain-bound 10k scene.  Off by default; AVN_WARM_BY_BODY=1 enables it.
-    bool warm_by_body_ = false;
     size_t hot_bytes_ = 0;
     DevBuf j_type_, j_index_, j_level_, j_planes_;
     DevBuf jcol_[AVN_JOINT_TYPE_COUNT][12], jb1_[AVN_JOINT_TYPE_COUNT], jb2_[AVN_JOINT_TYPE_COUNT], jle_[AVN_JOINT_TYPE_COUNT],
@@ -629,7 +619,7 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
         auto up256 = [](size_t x) { return (x + 255) & ~size_t(255); };
         const size_t vel_b = up256(state_bytes), dlt_b = up256(state_bytes), ver_b = up256((B + 1) * sizeof(unsigned)), deg_b = up256(2 * (B + 1) * sizeof(int));
         const size_t planes_b = have_m_ ? size_t(CP_PLANES) * d.Mpad * sizeof(Vec4<S>) : 0;
-        const size_t pcr_b = have_m_ ? up256(size_t(AVN_MAX_MANIFOLD_POINTS) * d.Mpad * PcRec<S>::W * sizeof(Vec4<S>)) : 0;
+        const size_t pcr_b = have_m_ ? up256(size_t(AVN_MAX_MANIFOLD_POINTS) * d.Mpad * sizeof(Vec4<S>)) : 0;
         AVN_CUDA(hot_.ensure(vel_b + dlt_b + ver_b + deg_b + pcr_b + planes_b + 256));
         char* base = hot_.as<char>();
         d.vel = reinterpret_cast<Vec4<S>*>(base); base += vel_b;
@@ -639,16 +629,6 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
         d.pcr = have_m_ ? reinterpret_cast<Vec4<S>*>(base) : nullptr; base += pcr_b;
         d.cst = have_m_ ? reinterpret_cast<Vec4<S>*>(base) : nullptr;
         hot_bytes_ = vel_b + dlt_b + ver_b + deg_b + pcr_b;
-        // adjacency of the body-centric warm start (f32 wavefront schedule; experiment, AVN_WARM_BY_BODY=1)
-        d.adj = nullptr; d.wdeg = nullptr; d.wpts = nullptr; d.adj_stride = 0;
-        if (sizeof(S) == 4 && have_m_ && warm_by_body_) {
-            const size_t stride = (B + 1 + 31) & ~size_t(31);
-            AVN_CUDA(adj_.ensure(size_t(ADJ_MAX) * stride * sizeof(uint2) + 2 * (B + 1) * sizeof(int)));
-            d.adj = adj_.as<uint2>();
-            d.wdeg = reinterpret_cast<int*>(d.adj + size_t(ADJ_MAX) * stride);
-            d.wpts = d.wdeg + (B + 1);
-            d.adj_stride = int(stride);
-        }
     }
     // ---- joints
     have_j_ = false;
@@ -749,11 +729,9 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
     dev_.do_restitution = (flags & AVN_RUN_RESTITUTION) ? 1 : 0;
     dev_.do_finalize = (flags & AVN_RUN_FINALIZE) ? 1 : 0;
     bool mega = use_mega_ && coop_ok_;
-    if (prepare) {
-        // the schedule is decided before the kernel variant: a step that can run the wavefront schedule gets the 4-blocks-per-SM build
-        const bool wave_candidate = use_wave_ && dev_.M > 0 && dev_.J == 0 && dev_.color_len[AVN_COLOR_OVERFLOW] == 0;
-        step_bps_ = bps_for(wave_candidate);
-    }
+    // blocks per SM, the same for both schedules: at 3 (170 registers) the f32 wavefront routines run without local-memory spills; at 4
+    // (128 registers) the warm-start routine and the megakernel spill (DESIGN.md 3.1)
+    if (prepare) step_bps_ = mega_bps_;
     mega = mega && select_megakernel(max_np_, step_bps_);
     if (prepare) {
         launches_ = 0;
@@ -766,12 +744,7 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
         for (int c = 0; c < AVN_COLOR_OVERFLOW; ++c) widest_colour = std::max(widest_colour, dev_.color_len[c]);
         const bool chain_bound = force_wave_ || widest_colour <= 2 * mega_grid_ * MEGA_BLOCK;
         dev_.wave = (mega && use_wave_ && chain_bound && dev_.M > 0 && dev_.J == 0 && dev_.color_len[AVN_COLOR_OVERFLOW] == 0) ? 1 : 0;
-        // which build of the f32 wavefront contact routines: rolled (17 KB per pass, instruction-cache friendly) when a colour keeps a good part
-        // of the resident warps busy, unrolled (42 KB, shorter dependent chain per item) when the step is bound by the per-body chain
         {
-            const int resident_warps = mega_grid_ * (MEGA_BLOCK / 32);
-            dev_.wave_rolled = (widest_colour / 32 >= resident_warps / 4) ? 1 : 0;
-            if (const char* r = getenv("AVN_WAVE_ROLLED")) dev_.wave_rolled = atoi(r) != 0;
             dev_.sm_slots = nullptr;
             if (sm_order_ && mega_grid_ == step_bps_ * sm_count_) {
                 if (!sm_slots_.p) {
@@ -780,8 +753,6 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
                 }
                 dev_.sm_slots = sm_slots_.as<int>();
             }
-            dev_.poll_ns = 0;
-            if (const char* r = getenv("AVN_WAVE_POLL_NS")) dev_.poll_ns = std::max(0, atoi(r));
         }
         if (dev_.M > 0) {
             // padding slots must read as "no points": clear the index plane before prepare fills the live slots
@@ -790,7 +761,6 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
         if (dev_.wave) {
             AVN_CUDA(cudaMemsetAsync(dev_.ver, 0, (size_t(dev_.B) + 1) * sizeof(unsigned), stream_));
             AVN_CUDA(cudaMemsetAsync(dev_.deg, 0, 2 * (size_t(dev_.B) + 1) * sizeof(int), stream_));   // deg + stamp
-            if (dev_.adj) AVN_CUDA(cudaMemsetAsync(dev_.wdeg, 0, 2 * (size_t(dev_.B) + 1) * sizeof(int), stream_));   // wdeg + wpts
         }
         mega_step_ = mega;
     } else {
@@ -918,7 +888,7 @@ __global__ void boundary_apply_kernel(DevSolver<S> d, const int* __restrict__ bo
         l.x = l.x + dl.x; l.y = l.y + dl.y; l.z = l.z + dl.z;
         a.x = a.x + da.x; a.y = a.y + da.y; a.z = a.z + da.z;
     }
-    // the spare lanes of the velocity / delta rows carry the wavefront schedule's sequence tags (wave32_dev.cuh): kept as they are
+    // the spare lanes of the velocity / delta rows are kept as they are
     st4(&d.vel[2 * b], mk4<S>(l.x, l.y, l.z, ld4(&d.vel[2 * b]).w));
     st4(&d.vel[2 * b + 1], mk4<S>(a.x, a.y, a.z, ld4(&d.vel[2 * b + 1]).w));
     const Vec4<S>* own = gathered + (size_t(owner_rank[k]) * records + size_t(source[size_t(k) * world + owner_rank[k]])) * 4;
@@ -1106,8 +1076,8 @@ AvnStatus Solver<S>::download() {
     {
         unsigned long long tr[8];
         cudaMemcpy(tr, dev_.any_restitution + FLAG_WORDS, sizeof tr, cudaMemcpyDeviceToHost);
-        if (tr[4]) fprintf(stderr, "[avn wave trace] item-warps %llu  avg cycles: wait(records) %.0f  wait(delta)+staging %.0f  separations/load %.0f  compute %.0f  store+publish %.0f\n", tr[4],
-                           double(tr[0]) / tr[4], double(tr[5]) / tr[4], double(tr[1]) / tr[4], double(tr[2]) / tr[4], double(tr[3]) / tr[4]);
+        if (tr[4]) fprintf(stderr, "[avn wave trace] contact item-warps %llu  avg cycles: stage 1 (wait deltas + separations) %.0f  wait %.0f  loads %.0f  compute %.0f  "
+                           "store+publish %.0f\n", tr[4], double(tr[5]) / tr[4], double(tr[0]) / tr[4], double(tr[1]) / tr[4], double(tr[2]) / tr[4], double(tr[3]) / tr[4]);
     }
 #endif
     if (flags_host[1] == WAVE_BAD_COLOURING)

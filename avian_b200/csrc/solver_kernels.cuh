@@ -14,7 +14,6 @@
 #include <cooperative_groups.h>
 
 #include "joints_dev.cuh"
-#include "wave32_dev.cuh"
 
 namespace avn {
 namespace cg = cooperative_groups;
@@ -34,10 +33,10 @@ __device__ __forceinline__ void run_item(const DevSolver<S>& d, int i) {
     else if (OP == OP_PREPARE_JOINT) prepare_joint_item(d, i);
     else if (OP == OP_INTEGRATE_VEL) integrate_velocity_item(d, i);
     else if (OP == OP_INTEGRATE_POS) { integrate_position_item(d, i); if (d.J > 0) store_pre_solve_item(d, i); }
-    else if (OP == OP_WARM) contact_item<S, PASS_WARM, false, MAXP>(d, i);
-    else if (OP == OP_SOLVE_BIAS) contact_item<S, PASS_SOLVE_BIAS, false, MAXP>(d, i);
-    else if (OP == OP_RELAX) contact_item<S, PASS_RELAX, false, MAXP>(d, i);
-    else if (OP == OP_RESTITUTION) contact_item<S, PASS_RESTITUTION, false, MAXP>(d, i);
+    else if (OP == OP_WARM) contact_item<S, PASS_WARM, MAXP>(d, i);
+    else if (OP == OP_SOLVE_BIAS) contact_item<S, PASS_SOLVE_BIAS, MAXP>(d, i);
+    else if (OP == OP_RELAX) contact_item<S, PASS_RELAX, MAXP>(d, i);
+    else if (OP == OP_RESTITUTION) contact_item<S, PASS_RESTITUTION, MAXP>(d, i);
     else if (OP == OP_SOLVE_JOINT) solve_joint_item(d, i);
     else if (OP == OP_PROJECT_VEL) project_velocity_item(d, i);
     else if (OP == OP_DAMP_JOINT) damp_joint_item(d, i);
@@ -98,58 +97,17 @@ __device__ __forceinline__ void grid_contact_pass(const DevSolver<S>& d, cg::gri
 #define AVN_WAVE_CHUNK 32
 #endif
 constexpr int WAVE_CHUNK = AVN_WAVE_CHUNK;
-// the counter protocol (solver_dev.cuh); f32 can run the tagged-record protocol instead (wave32_dev.cuh, below)
-template <class S, int PASS, int MAXP>
-__device__ __noinline__ void wave_contact_chunk(const DevSolver<S>& d, int slot, int s, int it, bool active) {
-    contact_item<S, PASS, true, MAXP>(d, slot, s, it, active);
-}
-template <class S>
-__device__ __noinline__ void wave_iv_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_velocity_item<S, true>(d, i, s, active); }
-template <class S>
-__device__ __noinline__ void wave_ip_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_position_item<S, true>(d, i, s, active); }
-// f32 runs the counter protocol by default.  -DAVN_WAVE_RECORDS_F32 builds the tagged-record protocol (wave32_dev.cuh) instead, which
-// relies on 16-byte accesses not tearing: the PTX memory model does not promise that, and on sm_90 the records gave reads that were
-// close to the right values but not bit-identical (stale halves), so the records stay an experiment.
-// (BPS and MAXP are template parameters of all of them so that every megakernel variant owns its copies)
-template <int PASS, int MAXP, int BPS>
-__device__ __noinline__ void wave32_contact_chunk(const DevSolver<float>& d, int slot, int s, int it, bool active, int wf, int pass) {
-    w32_contact_item<PASS, MAXP>(d, slot, s, it, active, wf, pass);
-}
-template <int PASS, int MAXP, int BPS>
-__device__ __noinline__ void wave32_contact_chunk_unrolled(const DevSolver<float>& d, int slot, int s, int it, bool active, int wf) {
-    w32_contact_item_unrolled<PASS, MAXP>(d, slot, s, it, active, wf);
-}
-template <int BPS, int MAXP> __device__ __noinline__ void wave32_iv_chunk(const DevSolver<float>& d, int i, int s, bool active) { w32_integrate_velocity_item(d, i, s, active); }
-template <int BPS, int MAXP> __device__ __noinline__ void wave32_ip_chunk(const DevSolver<float>& d, int i, int s, bool active, int wf) { w32_integrate_position_item(d, i, s, active, wf); }
-// integrate_velocities + the body's warm starts (8 bodies per warp, wave32_dev.cuh)
-template <int BPS, int MAXP> __device__ __noinline__ void wave32_ivw_chunk(const DevSolver<float>& d, int chunk, int s) { w32_ivw_item<MAXP>(d, chunk, s); }
-#ifdef AVN_WAVE_RECORDS_F32
-constexpr bool WAVE_RECORDS_F32 = true;
-#else
-constexpr bool WAVE_RECORDS_F32 = false;
-#endif
-template <class S> struct UseRecords { static constexpr bool value = false; };
-template <> struct UseRecords<float> { static constexpr bool value = WAVE_RECORDS_F32; };
+// The wavefront routines are __noinline__ (each keeps its own register allocation) and take BPS and MAXP as template parameters so that
+// every megakernel variant owns its copies, compiled under that variant's register budget.  The solve routine serves the biased and the
+// relax pass.
 template <class S, int PASS, int MAXP, int BPS>
-__device__ __forceinline__ void wave_contact(const DevSolver<S>& d, int slot, int s, int it, bool active, int wf) {
-    if constexpr (UseRecords<S>::value) {
-        if (d.wave_rolled) wave32_contact_chunk<(PASS == PASS_WARM ? PASS_WARM : PASS_SOLVE_BIAS), MAXP, BPS>(d, slot, s, it, active, wf, PASS);
-        else wave32_contact_chunk_unrolled<PASS, MAXP, BPS>(d, slot, s, it, active, wf);
-    } else {
-        wave_contact_chunk<S, PASS, MAXP>(d, slot, s, it, active);
-    }
+__device__ __noinline__ void wave_contact_chunk(const DevSolver<S>& d, int slot, int s, int it, bool active, bool relax) {
+    wave_contact_item<S, PASS, MAXP>(d, slot, s, it, active, relax);
 }
-template <class S, int BPS, int MAXP> __device__ __forceinline__ void wave_iv(const DevSolver<S>& d, int i, int s, bool active) {
-    if constexpr (UseRecords<S>::value) wave32_iv_chunk<BPS, MAXP>(d, i, s, active);
-    else wave_iv_chunk<S>(d, i, s, active);
-}
-template <class S, int BPS, int MAXP> __device__ __forceinline__ void wave_ip(const DevSolver<S>& d, int i, int s, bool active, int wf) {
-    if constexpr (UseRecords<S>::value) wave32_ip_chunk<BPS, MAXP>(d, i, s, active, wf);
-    else wave_ip_chunk<S>(d, i, s, active);
-}
-template <class S, int BPS, int MAXP> __device__ __forceinline__ void wave_ivw(const DevSolver<S>& d, int chunk, int s) {
-    if constexpr (UseRecords<S>::value) wave32_ivw_chunk<BPS, MAXP>(d, chunk, s);
-}
+template <class S, int BPS, int MAXP>
+__device__ __noinline__ void wave_iv_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_velocity_item<S, true>(d, i, s, active); }
+template <class S, int BPS, int MAXP>
+__device__ __noinline__ void wave_ip_chunk(const DevSolver<S>& d, int i, int s, bool active) { integrate_position_item<S, true>(d, i, s, active); }
 
 // EXPERIMENT (off): L2 prefetch of the immutable constraint rows of the chunk this warp processes one iteration from now.  The idea: at
 // 100k bodies the planes (>100 MB) stream from HBM every pass and an item can do nothing before its index row has arrived.  The measurement
@@ -193,14 +151,8 @@ __device__ __forceinline__ void wave_substep_loop(const DevSolver<S>& d) {
         warp_id = ((long long)dense * BPS + ticket) * (blockDim.x >> 5) + (threadIdx.x >> 5);
     }
     const int body_chunks = (d.B + WAVE_CHUNK - 1) / WAVE_CHUNK, slot_chunks = d.Mpad / WAVE_CHUNK;
-    // body-centric warm start (f32 records): the first phase of a substep is integrate_velocities + warm start, 8 bodies per warp, and the
-    // slot-centric warm pass disappears.  The adjacency it needs was built by the rank pass; a body with too many constraints (flag, read
-    // after a grid barrier: uniform over the grid) keeps the slot-centric schedule.
-    const bool wbb = UseRecords<S>::value && WAVE_CHUNK == 32 && d.adj != nullptr &&
-                     *reinterpret_cast<volatile int*>(d.any_restitution + FLAG_ADJ_OVERFLOW) == 0;
-    const int wf = wbb ? 0 : 1;
-    const int first_chunks = wbb ? (d.B + 7) / 8 : body_chunks;
-    const int front_passes = wf + d.iters;                          // (warm,) iters x solve: the slot passes before integrate_positions
+    const int first_chunks = body_chunks;                           // integrate_velocities
+    const int front_passes = 1 + d.iters;                           // warm, iters x solve: the slot passes before integrate_positions
     const long long per_substep = (long long)first_chunks + body_chunks + (long long)(front_passes + 1) * slot_chunks;
     const long long total = per_substep * d.sub_end;
     // position of a chunk inside its substep -> slot of its first item, or -1 for a body chunk (prefetch experiment)
@@ -225,21 +177,20 @@ __device__ __forceinline__ void wave_substep_loop(const DevSolver<S>& d) {
         }
 #endif
         if (r < first_chunks) {
-            if (wbb) wave_ivw<S, BPS, MAXP>(d, int(r), s);
-            else wave_iv<S, BPS, MAXP>(d, int(r) * WAVE_CHUNK + lane, s, active);
+            wave_iv_chunk<S, BPS, MAXP>(d, int(r) * WAVE_CHUNK + lane, s, active);
             continue;
         }
         r -= first_chunks;
         if (r < (long long)front_passes * slot_chunks) {
             const int pass = int(r / slot_chunks), slot = int(r - (long long)pass * slot_chunks) * WAVE_CHUNK + lane;
-            if (pass < wf) wave_contact<S, PASS_WARM, MAXP, BPS>(d, slot, s, 0, active, wf);
-            else wave_contact<S, PASS_SOLVE_BIAS, MAXP, BPS>(d, slot, s, pass - wf, active, wf);
+            if (pass == 0) wave_contact_chunk<S, PASS_WARM, MAXP, BPS>(d, slot, s, 0, active, false);
+            else wave_contact_chunk<S, PASS_SOLVE_BIAS, MAXP, BPS>(d, slot, s, pass - 1, active, false);
             continue;
         }
         r -= (long long)front_passes * slot_chunks;
-        if (r < body_chunks) { wave_ip<S, BPS, MAXP>(d, int(r) * WAVE_CHUNK + lane, s, active, wf); continue; }
+        if (r < body_chunks) { wave_ip_chunk<S, BPS, MAXP>(d, int(r) * WAVE_CHUNK + lane, s, active); continue; }
         r -= body_chunks;
-        wave_contact<S, PASS_RELAX, MAXP, BPS>(d, int(r) * WAVE_CHUNK + lane, s, 0, active, wf);
+        wave_contact_chunk<S, PASS_SOLVE_BIAS, MAXP, BPS>(d, int(r) * WAVE_CHUNK + lane, s, 0, active, true);
     }
 }
 

@@ -14,7 +14,10 @@ cuobjdump -xelf all $LIB >/dev/null 2>&1
 hist() { grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed -E 's/^\s+\/\*[0-9a-f]+\*\/\s+(@!?U?P[0-9T]+ )?//' | awk '{print $1}' | sed 's/;$//' | sort | uniq -c | sort -rn | awk '{printf "%8d %s\n", $1, $2}'; }
 {
   echo "# SASS opcode histograms of avian_b200/lib/libavian_b200.so (nvdisasm -c of every cubin in the fat binary).  Opcodes to look for:"
-  echo "#   LDG.E.128.STRONG.GPU / STG.E.128.STRONG.GPU  the tagged 128-bit record accesses of the wavefront schedule (csrc/wave32_dev.cuh)"
+  echo "#   LDG.E.STRONG.GPU + CCTL.IVALL                          ld.acquire.gpu polls of the wavefront event counters (no membar after a poll)"
+  echo "#   MEMBAR.ALL.GPU                                         fence.acq_rel.gpu before a wavefront item stores its counters"
+  echo "#   MEMBAR.SC.GPU                                          __threadfence() (grid barriers); none in the wavefront routines"
+  echo "#   LDL / STL                                              local memory (spills); none in the f32 wavefront routines"
   echo "#   LDGSTS.E.BYPASS.128                                    cp.async staging of the constraint rows into shared memory"
   echo "#   CCTL.E.PF2                                             prefetch.global.L2 of the next chunk's rows"
   for f in solver_host broadphase contacts narrow aabb; do
@@ -25,4 +28,4 @@ hist() { grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed -E 's/^\s+\/\*[0-9a-f]+\*\/\s+(@
   nvdisasm -c solver_host.sm_90a.cubin 2>/dev/null | hist | head -60
 } > $OUT/${TAG}_sass_histogram.txt
 cd /; rm -rf $TMP
-grep -c "E.128.STRONG.GPU" $OUT/${TAG}_sass_histogram.txt || true
+grep -E "MEMBAR|LDL|STL" $OUT/${TAG}_sass_histogram.txt || true

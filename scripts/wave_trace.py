@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Latency breakdown of the wavefront items (GPU box).  Loads the -DAVN_WAVE_TRACE build of the library
 (avian_b200/lib/libavian_b200_trace.so; build: see DESIGN.md §3.1) and runs a few solver stages; the library prints the
-per-item average SM cycles of wait / load / compute / store+publish to stderr."""
+average SM cycles per contact item-warp of stage 1 (delta wait + separations) / wait / loads / compute / store+publish to stderr."""
 import ctypes as C
 import sys
 from pathlib import Path
