@@ -360,6 +360,27 @@ class AvnBoundary(C.Structure):
                 ("body", _vp), ("source", _vp), ("owner_rank", _vp)]
 
 
+class AvnQueryColliders(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("shape", "dims", "position", "rotation", "memberships")]
+
+
+class AvnRayBatch(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("exclude_count", C.c_uint32)] + [
+        (n, _vp) for n in ("origin", "direction", "max_distance", "solid", "max_hits", "mask", "exclude_offsets", "exclude")]
+
+
+class AvnRayClosest(C.Structure):
+    _fields_ = [(n, _vp) for n in ("collider", "distance", "normal")]
+
+
+class AvnHitList(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [(n, _vp) for n in ("offsets", "collider", "distance", "normal")]
+
+
+QUERY_SHAPES_UNCHANGED = 1
+MAX_HITS_ALL = 0xFFFFFFFF
+
+
 def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
     """Declare argument/return types of every entry point of include/avian_b200.h on `lib`."""
     P = C.POINTER
@@ -409,6 +430,10 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "solver_prefetch_bodies": ([_vp, P(AvnBodyColumns), C.c_uint32], C.c_int),
         "islands_configure": ([_vp, P(AvnIslandsConfig)], C.c_int),
         "islands_step": ([_vp, P(AvnIslandsStep)], C.c_int),
+        "query_update": ([_vp, P(AvnQueryColliders), C.c_uint32], C.c_int),
+        "query_cast_ray": ([_vp, P(AvnRayBatch), P(AvnRayClosest)], C.c_int),
+        "query_ray_hits": ([_vp, P(AvnRayBatch), P(AvnHitList)], C.c_int),
+        "query_aabb_intersections": ([_vp, C.c_uint32, _vp, _vp, P(AvnHitList)], C.c_int),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(lib, f"{prefix}_{name}")
@@ -424,7 +449,8 @@ ABI_SYMBOLS = [
     "avn_solver_step_partitioned", "avn_comm_unique_id", "avn_comm_init", "avn_comm_destroy", "avn_comm_all_gather", "avn_narrow_phase", "avn_solver_upload_edges", "avn_solver_upload_graph",
     "avn_contacts_reserve", "avn_contacts_add", "avn_contacts_remove", "avn_contacts_narrow_phase", "avn_contacts_download_impulses",
     "avn_contacts_configure", "avn_contacts_step", "avn_solver_upload_resident", "avn_broadphase_download_order", "avn_contacts_download_graph",
-    "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step"]
+    "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
+    "avn_query_aabb_intersections"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -455,6 +481,76 @@ class Colliders:
         for name, _ in AvnColliderColumns._fields_[2:]:
             setattr(s, name, _ptr(getattr(self, name)))
         return s
+
+
+@dataclass
+class QueryColliders:
+    """Collider columns of avn_query_update (AvnQueryColliders); collider index = row."""
+    shape: np.ndarray                    # uint8[C] SHAPE_CUBOID / SHAPE_SPHERE
+    dims: np.ndarray                     # [C,3] half extents / radius in [0]
+    position: np.ndarray                 # [C,3]
+    rotation: np.ndarray                 # [C,4] (x, y, z, w)
+    memberships: np.ndarray | None = None   # uint32[C] CollisionLayers::memberships (None = 1)
+
+    def as_struct(self, scalar) -> tuple["AvnQueryColliders", list]:
+        """The struct and the arrays it points into (keep them alive for the call)."""
+        dt = np.dtype(scalar)
+        keep = [np.ascontiguousarray(self.shape, dtype=np.uint8), np.ascontiguousarray(self.dims, dtype=dt).reshape(-1, 3),
+                np.ascontiguousarray(self.position, dtype=dt).reshape(-1, 3), np.ascontiguousarray(self.rotation, dtype=dt).reshape(-1, 4),
+                None if self.memberships is None else np.ascontiguousarray(self.memberships, dtype=np.uint32)]
+        return AvnQueryColliders(int(keep[2].shape[0]), 0, *(_ptr(a) for a in keep)), keep
+
+
+@dataclass
+class Rays:
+    """A batch of rays (AvnRayBatch).  exclude: per ray an iterable of collider indices it ignores (SpatialQueryFilter::excluded_entities,
+    RayCaster::ignore_self), or None."""
+    origin: np.ndarray                   # [n,3]
+    direction: np.ndarray                # [n,3] unit
+    max_distance: np.ndarray             # [n]
+    solid: np.ndarray | None = None      # bool/uint8[n] (None = all solid)
+    max_hits: np.ndarray | None = None   # uint32[n] (None = all; MAX_HITS_ALL = all)
+    mask: np.ndarray | None = None       # uint32[n] SpatialQueryFilter::mask (None = all layers)
+    exclude: list | None = None
+
+    @property
+    def count(self) -> int:
+        return int(np.asarray(self.origin).reshape(-1, 3).shape[0])
+
+    def as_struct(self, scalar) -> tuple["AvnRayBatch", list]:
+        dt, n = np.dtype(scalar), self.count
+        o = np.ascontiguousarray(self.origin, dtype=dt).reshape(-1, 3)
+        d = np.ascontiguousarray(self.direction, dtype=dt).reshape(-1, 3)
+        md = np.ascontiguousarray(np.broadcast_to(np.asarray(self.max_distance, dtype=dt), (n,)))
+        opt = lambda a, t: None if a is None else np.ascontiguousarray(a, dtype=t)
+        solid, mh, mask = opt(self.solid, np.uint8), opt(self.max_hits, np.uint32), opt(self.mask, np.uint32)
+        xoff = xs = None
+        if self.exclude is not None:
+            lists = [np.asarray(list(e), dtype=np.uint32) for e in self.exclude]
+            xoff = np.zeros(n + 1, dtype=np.uint32)
+            xoff[1:] = np.cumsum([len(e) for e in lists])
+            xs = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, dtype=np.uint32), dtype=np.uint32)
+        keep = [o, d, md, solid, mh, mask, xoff, xs]
+        st = AvnRayBatch(n, 0 if xs is None else int(xs.shape[0]), *(_ptr(a) if a is None or a.size else None for a in keep))
+        if xoff is not None:
+            st.exclude_offsets = xoff.ctypes.data
+            st.exclude = xs.ctypes.data if xs.size else None
+        return st, keep
+
+
+def hit_list(n: int, capacity: int, scalar, ray: bool) -> tuple["AvnHitList", dict]:
+    """An AvnHitList over fresh numpy arrays (offsets[n+1], collider, and for rays distance / normal)."""
+    cap = max(int(capacity), 0)
+    out = {"offsets": np.zeros(n + 1, dtype=np.uint64), "collider": np.zeros(max(cap, 1), dtype=np.uint32)}
+    if ray:
+        out["distance"] = np.zeros(max(cap, 1), dtype=scalar)
+        out["normal"] = np.zeros((max(cap, 1), 3), dtype=scalar)
+    return AvnHitList(cap, 0, _ptr(out["offsets"]), _ptr(out["collider"]), _ptr(out.get("distance")), _ptr(out.get("normal"))), out
+
+
+def hit_list_result(h: "AvnHitList", out: dict) -> dict:
+    total = int(h.count)
+    return {k: (v if k == "offsets" else v[:total]) for k, v in out.items()}
 
 
 def aabb_params(dt: float, contact_tolerance: float = 0.005, default_speculative_margin: float = float("inf")) -> "AvnAabbParams":
@@ -526,6 +622,14 @@ class Context:
     def _check(self, st: int) -> None:
         if st != OK:
             raise AvianError(st, self.lib.avn_last_error(self.handle).decode())
+
+    def _check_list(self, st: int, h: "AvnHitList") -> None:
+        """A CSR query's status: on AVN_ERR_CAPACITY the error carries the required count as .required"""
+        if st == ERR_CAPACITY:
+            e = AvianError(st, self.lib.avn_last_error(self.handle).decode())
+            e.required = int(h.count)
+            raise e
+        self._check(st)
 
     def pinned(self, shape, dtype) -> np.ndarray:
         """A numpy array backed by page-locked memory from avn_alloc_pinned (lives as long as the context)."""
@@ -839,3 +943,43 @@ class Context:
         t = AvnTimings()
         self._check(self.lib.avn_get_timings(self.handle, C.byref(t)))
         return {n: getattr(t, n) for n, _ in AvnTimings._fields_ if n != "_pad"}
+
+    # ---- spatial queries (include/avian_b200.h avn_query_*): SpatialQueryPipeline on the device
+    def query_update(self, colliders: "QueryColliders", shapes_unchanged: bool = False) -> None:
+        """avn_query_update: rebuild the collider tree from these poses (shape, dims and memberships stay on the device with shapes_unchanged)."""
+        c, keep = colliders.as_struct(self.scalar)
+        self._check(self.lib.avn_query_update(self.handle, C.byref(c), QUERY_SHAPES_UNCHANGED if shapes_unchanged else 0))
+
+    def cast_ray(self, rays: "Rays") -> dict:
+        """avn_query_cast_ray: per ray the closest hit — collider (-1 = none), distance, normal."""
+        r, keep = rays.as_struct(self.scalar)
+        n = rays.count
+        out = {"collider": np.zeros(n, dtype=np.int32), "distance": np.zeros(n, dtype=self.scalar), "normal": np.zeros((n, 3), dtype=self.scalar)}
+        o = AvnRayClosest(*(_ptr(out[k]) for k in ("collider", "distance", "normal")))
+        self._check(self.lib.avn_query_cast_ray(self.handle, C.byref(r), C.byref(o)))
+        return out
+
+    def ray_hits(self, rays: "Rays", capacity: int | None = None) -> dict:
+        """avn_query_ray_hits: CSR offsets[n+1], collider, distance, normal.  capacity=None sizes the output from the required count;
+        an explicit capacity that is too small raises AvianError(ERR_CAPACITY) with .required."""
+        r, keep = rays.as_struct(self.scalar)
+        h, out = hit_list(rays.count, 4 * rays.count if capacity is None else capacity, self.scalar, True)
+        st = self.lib.avn_query_ray_hits(self.handle, C.byref(r), C.byref(h))
+        if st == ERR_CAPACITY and capacity is None:
+            h, out = hit_list(rays.count, int(h.count), self.scalar, True)
+            st = self.lib.avn_query_ray_hits(self.handle, C.byref(r), C.byref(h))
+        self._check_list(st, h)
+        return hit_list_result(h, out)
+
+    def aabb_intersections(self, aabb_min, aabb_max, capacity: int | None = None) -> dict:
+        """avn_query_aabb_intersections: per query box the colliders whose tight AABB it touches (CSR offsets[n+1], collider)."""
+        mn = np.ascontiguousarray(aabb_min, dtype=self.scalar).reshape(-1, 3)
+        mx = np.ascontiguousarray(aabb_max, dtype=self.scalar).reshape(-1, 3)
+        n = int(mn.shape[0])
+        h, out = hit_list(n, 4 * n if capacity is None else capacity, self.scalar, False)
+        st = self.lib.avn_query_aabb_intersections(self.handle, n, _ptr(mn), _ptr(mx), C.byref(h))
+        if st == ERR_CAPACITY and capacity is None:
+            h, out = hit_list(n, int(h.count), self.scalar, False)
+            st = self.lib.avn_query_aabb_intersections(self.handle, n, _ptr(mn), _ptr(mx), C.byref(h))
+        self._check_list(st, h)
+        return hit_list_result(h, out)

@@ -17,6 +17,7 @@ struct AvnContext {
     std::unique_ptr<avn::AabbBase> aabbs;
     std::unique_ptr<avn::NarrowBase> narrow;
     std::unique_ptr<avn::ContactsBase> contacts;
+    std::unique_ptr<avn::QueriesBase> queries;
     std::unique_ptr<avn::CommBase> comm;
     AvnTimings last{};
 };
@@ -83,8 +84,9 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
         ctx->aabbs.reset(avn::make_aabb_updater(config->scalar_bits, ctx->stream, &ctx->err));
         ctx->narrow.reset(avn::make_narrow(config->scalar_bits, ctx->stream, &ctx->err));
         ctx->contacts.reset(avn::make_contacts(config->scalar_bits, ctx->stream, &ctx->err));
+        ctx->queries.reset(avn::make_queries(config->scalar_bits, ctx->stream, &ctx->err));
         ctx->comm.reset(avn::make_comm(ctx->stream, &ctx->err));
-        if (!ctx->solver || !ctx->broadphase || !ctx->aabbs || !ctx->narrow || !ctx->contacts) {
+        if (!ctx->solver || !ctx->broadphase || !ctx->aabbs || !ctx->narrow || !ctx->contacts || !ctx->queries) {
             ctx.reset();   // the members hold the stream: release them before it goes
             cudaStreamDestroy(stream);
             return create_fail(AVN_ERR_UNSUPPORTED, "scalar type not available");
@@ -107,6 +109,7 @@ void avn_destroy(AvnContext* ctx) {
     ctx->aabbs.reset();
     ctx->narrow.reset();
     ctx->contacts.reset();
+    ctx->queries.reset();
     cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -279,6 +282,20 @@ AvnStatus avn_islands_configure(AvnContext* ctx, const AvnIslandsConfig* config)
 AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step) { return guarded(ctx, [&] { return ctx->contacts->islands_step(step); }); }
 AvnStatus avn_contacts_download_impulses(AvnContext* ctx, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse) {
     return guarded(ctx, [&] { return ctx->contacts->download_impulses(warm_start_normal, warm_start_tangent, normal_impulse); });
+}
+
+// spatial queries (queries.cu): SpatialQueryPipeline::update / cast_ray / ray_hits / aabb_intersections_with_aabb
+AvnStatus avn_query_update(AvnContext* ctx, const AvnQueryColliders* colliders, uint32_t flags) {
+    return guarded(ctx, [&] { return ctx->queries->update(colliders, flags); });
+}
+AvnStatus avn_query_cast_ray(AvnContext* ctx, const AvnRayBatch* rays, AvnRayClosest* out) {
+    return guarded(ctx, [&] { return ctx->queries->cast_ray(rays, out); });
+}
+AvnStatus avn_query_ray_hits(AvnContext* ctx, const AvnRayBatch* rays, AvnHitList* out) {
+    return guarded(ctx, [&] { return ctx->queries->ray_hits(rays, out); });
+}
+AvnStatus avn_query_aabb_intersections(AvnContext* ctx, uint32_t count, const void* min, const void* max, AvnHitList* out) {
+    return guarded(ctx, [&] { return ctx->queries->aabb_intersections(count, min, max, out); });
 }
 
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out) {

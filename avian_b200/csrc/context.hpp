@@ -123,6 +123,16 @@ struct NarrowBase {
 };
 NarrowBase* make_narrow(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
+// the spatial-query tree and its batched queries (queries.cu)
+struct QueriesBase {
+    virtual ~QueriesBase() {}
+    virtual AvnStatus update(const AvnQueryColliders* colliders, uint32_t flags) = 0;
+    virtual AvnStatus cast_ray(const AvnRayBatch* rays, AvnRayClosest* out) = 0;
+    virtual AvnStatus ray_hits(const AvnRayBatch* rays, AvnHitList* out) = 0;
+    virtual AvnStatus aabb_intersections(uint32_t count, const void* min, const void* max, AvnHitList* out) = 0;
+};
+QueriesBase* make_queries(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
+
 struct ContactsBase {
     virtual ~ContactsBase() {}
     virtual AvnStatus reserve(uint32_t capacity) = 0;

@@ -1,5 +1,5 @@
-// Device primitives shared by the broad phase and the contact graph: the stable LSD radix-sort pass (8-bit digits, 2048 keys per block) and the
-// open-addressing u64 hash set.  Everything lives in an anonymous namespace: each translation unit that includes this gets its own copies.
+// Device primitives shared by the broad phase, the contact graph and the spatial queries: the stable LSD radix-sort pass (8-bit digits, 2048 keys
+// per block), the exclusive scan of per-item counts into CSR offsets and the open-addressing u64 hash set.  Everything lives in an anonymous namespace: each translation unit that includes this gets its own copies.
 #pragma once
 #include <cstdint>
 
@@ -156,6 +156,63 @@ __global__ void __launch_bounds__(RS_THREADS) rs_scatter(const K* __restrict__ k
             vals_out[pos] = val[r];
         }
     }
+}
+
+// exclusive scan of n 32-bit counts into 64-bit offsets (offsets[n] = total), three small launches:
+// per-block sums (1024 counts each) -> single-block scan of the <= 1024 block sums -> per-block local scan + base.
+__device__ __forceinline__ uint64_t block_exclusive_scan_1024(uint64_t v, uint64_t* warp_sums, uint64_t& block_total) {
+    uint64_t x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint64_t y = __shfl_up_sync(0xffffffffu, x, o);
+        if ((threadIdx.x & 31) >= o) x += y;
+    }
+    if ((threadIdx.x & 31) == 31) warp_sums[threadIdx.x >> 5] = x;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        uint64_t w = warp_sums[threadIdx.x], z = w;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            uint64_t y = __shfl_up_sync(0xffffffffu, z, o);
+            if (threadIdx.x >= o) z += y;
+        }
+        warp_sums[threadIdx.x] = z - w;
+        if (threadIdx.x == 31) warp_sums[32] = z;
+    }
+    __syncthreads();
+    block_total = warp_sums[32];
+    return x - v + warp_sums[threadIdx.x >> 5];
+}
+__global__ void __launch_bounds__(1024) scan_block_sums(const uint32_t* __restrict__ counts, int n, uint64_t* __restrict__ block_sums) {
+    __shared__ uint64_t ws[33];
+    int i = blockIdx.x * 1024 + threadIdx.x;
+    uint64_t total;
+    block_exclusive_scan_1024(i < n ? counts[i] : 0u, ws, total);
+    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(1024) scan_block_offsets(uint64_t* __restrict__ block_sums, int nblocks, uint64_t* __restrict__ total_out) {
+    __shared__ uint64_t ws[33];
+    __shared__ uint64_t carry;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int base = 0; base < nblocks; base += 1024) {
+        int i = base + threadIdx.x;
+        uint64_t v = i < nblocks ? block_sums[i] : 0ull, total;
+        uint64_t excl = block_exclusive_scan_1024(v, ws, total) + carry;
+        if (i < nblocks) block_sums[i] = excl;
+        __syncthreads();
+        if (threadIdx.x == 0) carry += total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *total_out = carry;
+}
+__global__ void __launch_bounds__(1024) scan_apply(const uint32_t* __restrict__ counts, int n, const uint64_t* __restrict__ block_offsets,
+                                                   uint64_t* __restrict__ offsets) {
+    __shared__ uint64_t ws[33];
+    int i = blockIdx.x * 1024 + threadIdx.x;
+    uint64_t total;
+    uint64_t excl = block_exclusive_scan_1024(i < n ? counts[i] : 0u, ws, total);
+    if (i < n) offsets[i] = excl + block_offsets[blockIdx.x];
 }
 
 __device__ __forceinline__ uint64_t hash64(uint64_t x) {

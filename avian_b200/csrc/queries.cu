@@ -1,0 +1,656 @@
+// Spatial queries on the device: the collider tree of SpatialQueryPipeline::update (spatial_query/pipeline.rs:96-133) rebuilt by every
+// update as an LBVH, and batched cast_ray / ray_hits / aabb_intersections_with_aabb against it (pipeline.rs:156-216, 690-729).
+// The per-shape arithmetic is csrc/query_math.hpp — the same header the host fixture's brute force compiles — evaluated in double and rounded
+// to the column scalar on store, so every answer equals the brute force over all colliders bit for bit (tests/test_gpu_query.py).
+//
+// Update (no host round trip):
+//   1. per collider: tight AABB in double; its f32 culling bounds (outward + one ulp, qm::culling_bounds); the centre; the scene bounds of
+//      the centres by ordered-integer atomics.  A collider with a non-finite pose or dims or a zero quaternion (qm::collider_valid) gets the
+//      key 0xFFFFFFFF and stays out of the tree.
+//   2. 30-bit Morton codes of the centres; stable radix sort of (code, index), 4 passes of device_prims.cuh's rs_histogram / rs_scatter.
+//   3. Karras' hierarchy over the m finite colliders (m is counted on the device): equal codes split on the index bits, so a node's common
+//      prefix length lies in [2, 63] and strictly grows downwards: depth <= 62, which the fixed traversal stack of Q_STACK entries holds.
+//   4. bottom-up refit: the second child to arrive at a node merges the two boxes (atom.acq_rel: the first arrival's box store is released
+//      by its increment and acquired by the second's, the counter discipline of the wavefront solver, DESIGN.md §3.1).
+// Queries: one thread per query, a stack traversal that culls against the f32 bounds (double slab test clipped to [0, max_distance]) and
+// runs the exact test at the leaves.  cast_ray keeps the lexicographic minimum (t, collider); ray_hits and aabb_intersections use the broad
+// phase's count -> exclusive scan -> emit -> per-segment sort pattern into CSR lists.
+#include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include "context.hpp"
+#include "device_prims.cuh"
+#include "query_math.hpp"
+
+namespace avn {
+namespace {
+
+constexpr int Q_STACK = 64;
+// node prefix lengths: [2, 31] for distinct 30-bit codes, 32 + [1, 31] for equal codes split on index bits -> at most 62 internal levels;
+// a pop pushes two children, so the stack holds at most (levels - 1) pending siblings + 2 entries
+static_assert(62 - 1 + 2 <= Q_STACK, "LBVH depth bound exceeds the traversal stack");
+constexpr uint32_t Q_INVALID_KEY = 0xFFFFFFFFu;
+constexpr int Q_THREADS = 128;
+
+struct __align__(16) NodeBox { float4 lo, hi; };   // .w unused
+
+template <class S>
+struct Tree {
+    int n;                                           // colliders passed to the update
+    const int* m;                                    // colliders in the tree (finite ones), on the device
+    const uint8_t* shape; const S* dims; const S* pos; const S* rot; const uint32_t* memb;
+    const S* tmn; const S* tmx;                      // tight AABBs rounded to S
+    const NodeBox* nodes;                            // [2m - 1]: internal nodes [0, m - 1), leaf k at m - 1 + k; root = 0
+    const int2* child;                               // [m - 1]
+    const uint32_t* leaf;                            // [m] sorted position -> collider
+};
+
+template <class S>
+struct Rays {
+    int n;
+    const S* o; const S* d; const S* maxd;
+    const uint8_t* solid; const uint32_t* max_hits; const uint32_t* mask; const uint32_t* xoff; const uint32_t* xs;
+};
+
+template <class S> __device__ __forceinline__ nm::V3 ld3(const S* p, size_t i) { return {double(p[3 * i]), double(p[3 * i + 1]), double(p[3 * i + 2])}; }
+template <class S> __device__ __forceinline__ nm::Q ldq(const S* p, size_t i) {
+    return {double(p[4 * i]), double(p[4 * i + 1]), double(p[4 * i + 2]), double(p[4 * i + 3])};
+}
+
+__device__ __forceinline__ uint32_t f_ord(float f) { const uint32_t u = __float_as_uint(f); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
+__device__ __forceinline__ float f_unord(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+
+__device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t* p, uint32_t v) {
+    uint32_t old;
+    asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+    return old;
+}
+
+__device__ __forceinline__ float f32_clamped(double x) { return float(fmin(fmax(x, -double(FLT_MAX)), double(FLT_MAX))); }
+
+// 1. per collider: validity, tight AABB (rounded to S), f32 culling box, centre; scene bounds of the centres
+template <class S>
+__global__ void __launch_bounds__(256) q_prepare(const __grid_constant__ Tree<S> t, S* __restrict__ tmn, S* __restrict__ tmx, NodeBox* __restrict__ cbox,
+                                                 float4* __restrict__ centre, uint8_t* __restrict__ valid, int* __restrict__ m, uint32_t* __restrict__ sb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    bool ok = false;
+    float cx = 0, cy = 0, cz = 0;
+    if (i < t.n) {
+        const nm::V3 he = ld3(t.dims, i), p = ld3(t.pos, i);
+        const nm::Q q = ldq(t.rot, i);
+        ok = qm::collider_valid(he, p, q);
+        if (ok) {
+            nm::V3 mn, mx;
+            qm::collider_aabb(t.shape[i], he, p, q, mn, mx);
+            tmn[3 * i] = S(mn.x); tmn[3 * i + 1] = S(mn.y); tmn[3 * i + 2] = S(mn.z);
+            tmx[3 * i] = S(mx.x); tmx[3 * i + 1] = S(mx.y); tmx[3 * i + 2] = S(mx.z);
+            NodeBox b;
+            qm::culling_bounds(mn.x, mx.x, b.lo.x, b.hi.x);
+            qm::culling_bounds(mn.y, mx.y, b.lo.y, b.hi.y);
+            qm::culling_bounds(mn.z, mx.z, b.lo.z, b.hi.z);
+            b.lo.w = b.hi.w = 0.f;
+            cbox[i] = b;
+            // the f32 centre only places the collider on the Morton curve: clamped, so a finite pose beyond the f32 range keeps finite
+            // scene bounds (its culling box is then infinite, which is conservative)
+            cx = f32_clamped((mn.x + mx.x) * 0.5); cy = f32_clamped((mn.y + mx.y) * 0.5); cz = f32_clamped((mn.z + mx.z) * 0.5);
+        }
+        valid[i] = ok ? 1 : 0;
+        centre[i] = make_float4(cx, cy, cz, 0.f);
+    }
+    const unsigned full = 0xffffffffu;
+    const unsigned ballot = __ballot_sync(full, ok);
+    const uint32_t mnx = __reduce_min_sync(full, ok ? f_ord(cx) : 0xffffffffu), mny = __reduce_min_sync(full, ok ? f_ord(cy) : 0xffffffffu),
+                   mnz = __reduce_min_sync(full, ok ? f_ord(cz) : 0xffffffffu);
+    const uint32_t mxx = __reduce_max_sync(full, ok ? f_ord(cx) : 0u), mxy = __reduce_max_sync(full, ok ? f_ord(cy) : 0u),
+                   mxz = __reduce_max_sync(full, ok ? f_ord(cz) : 0u);
+    if ((threadIdx.x & 31) == 0 && ballot) {
+        atomicAdd(m, __popc(ballot));
+        atomicMin(&sb[0], mnx); atomicMin(&sb[1], mny); atomicMin(&sb[2], mnz);
+        atomicMax(&sb[3], mxx); atomicMax(&sb[4], mxy); atomicMax(&sb[5], mxz);
+    }
+}
+
+__device__ __forceinline__ uint32_t expand10(uint32_t v) {
+    v &= 0x3ffu;
+    v = (v * 0x00010001u) & 0xFF0000FFu;
+    v = (v * 0x00000101u) & 0x0F00F00Fu;
+    v = (v * 0x00000011u) & 0xC30C30C3u;
+    v = (v * 0x00000005u) & 0x49249249u;
+    return v;
+}
+__device__ __forceinline__ uint32_t grid10(float c, float lo, float hi) {
+    const float ext = hi - lo;
+    const float u = ext > 0.f ? (c - lo) / ext : 0.f;
+    return uint32_t(fminf(fmaxf(u * 1024.f, 0.f), 1023.f));
+}
+
+// 2. Morton keys (finite colliders) or the key that sorts last (the rest)
+__global__ void q_codes(int n, const float4* __restrict__ centre, const uint8_t* __restrict__ valid, const uint32_t* __restrict__ sb,
+                        uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    vals[i] = uint32_t(i);
+    if (!valid[i]) { keys[i] = Q_INVALID_KEY; return; }
+    const float4 c = centre[i];
+    const uint32_t x = grid10(c.x, f_unord(sb[0]), f_unord(sb[3])), y = grid10(c.y, f_unord(sb[1]), f_unord(sb[4])),
+                   z = grid10(c.z, f_unord(sb[2]), f_unord(sb[5]));
+    keys[i] = (expand10(x) << 2) | (expand10(y) << 1) | expand10(z);
+}
+
+// 3. Karras (2012) hierarchy: internal node i covers a key range; equal keys compare on their index bits (32 + clz)
+__device__ __forceinline__ int q_delta(const uint32_t* keys, int m, int i, long long j) {
+    if (j < 0 || j >= m) return -1;
+    const uint32_t a = keys[i], b = keys[j];
+    return a == b ? 32 + __clz(uint32_t(i) ^ uint32_t(j)) : __clz(a ^ b);
+}
+__global__ void q_karras(const int* __restrict__ m_ptr, int n, const uint32_t* __restrict__ keys, int2* __restrict__ child, int* __restrict__ parent) {
+    const int m = *m_ptr;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) parent[0] = -1;
+    if (i >= m - 1 || i >= n) return;
+    const int d = q_delta(keys, m, i, i + 1) > q_delta(keys, m, i, i - 1) ? 1 : -1;
+    const int dmin = q_delta(keys, m, i, (long long)i - d);
+    long long lmax = 2;
+    while (q_delta(keys, m, i, i + lmax * d) > dmin) lmax *= 2;
+    long long l = 0;
+    for (long long s = lmax / 2; s >= 1; s /= 2)
+        if (q_delta(keys, m, i, i + (l + s) * d) > dmin) l += s;
+    const long long j = i + l * d;
+    const int dnode = q_delta(keys, m, i, j);
+    long long s = 0;
+    for (long long w = (l + 1) / 2;; w = (w + 1) / 2) {
+        if (q_delta(keys, m, i, i + (s + w) * d) > dnode) s += w;
+        if (w == 1) break;
+    }
+    const int gamma = int(i + s * d + (d < 0 ? -1 : 0));
+    const int lo = int(i < j ? i : j), hi = int(i < j ? j : i);
+    const int left = lo == gamma ? (m - 1) + gamma : gamma;
+    const int right = hi == gamma + 1 ? (m - 1) + gamma + 1 : gamma + 1;
+    child[i] = make_int2(left, right);
+    parent[left] = i;
+    parent[right] = i;
+}
+
+// 4. leaves and bottom-up refit: the second child to arrive at a node merges
+__global__ void q_refit(const int* __restrict__ m_ptr, const uint32_t* __restrict__ leaf, const NodeBox* __restrict__ cbox, const int* __restrict__ parent,
+                        const int2* __restrict__ child, uint32_t* __restrict__ arrived, NodeBox* nodes) {
+    const int m = *m_ptr;
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= m) return;
+    int node = (m - 1) + k;
+    NodeBox b = cbox[leaf[k]];
+    nodes[node] = b;
+    for (;;) {
+        const int p = parent[node];
+        if (p < 0) return;
+        if (atom_add_acq_rel(&arrived[p], 1u) == 0) return;   // first arrival: its box is published by this increment
+        const int2 c = child[p];
+        const NodeBox o = nodes[c.x == node ? c.y : c.x];       // the sibling's box, released by the other arrival
+        b.lo = make_float4(fminf(b.lo.x, o.lo.x), fminf(b.lo.y, o.lo.y), fminf(b.lo.z, o.lo.z), 0.f);
+        b.hi = make_float4(fmaxf(b.hi.x, o.hi.x), fmaxf(b.hi.y, o.hi.y), fmaxf(b.hi.z, o.hi.z), 0.f);
+        nodes[p] = b;
+        node = p;
+    }
+}
+
+// stack traversal: visit(box) decides whether to descend, leaf(collider) runs the exact test
+template <class S, class Visit, class Leaf>
+__device__ __forceinline__ void traverse(const Tree<S>& t, int m, Visit visit, Leaf leaf) {
+    if (m <= 0) return;
+    int stack[Q_STACK];
+    int sp = 0;
+    stack[sp++] = 0;
+    while (sp > 0) {
+        const int nd = stack[--sp];
+        const NodeBox b = t.nodes[nd];
+        if (!visit(b)) continue;
+        if (nd >= m - 1) {
+            leaf(t.leaf[nd - (m - 1)]);
+        } else {
+            const int2 c = t.child[nd];
+            stack[sp++] = c.y;
+            stack[sp++] = c.x;
+        }
+    }
+}
+
+template <class S>
+struct RayIn {
+    nm::V3 o, d;
+    double maxd;
+    bool solid, ok;
+    uint32_t mask;
+    const uint32_t* xs;
+    uint32_t nx;
+};
+template <class S>
+__device__ __forceinline__ RayIn<S> load_ray(const Rays<S>& r, int i) {
+    RayIn<S> q;
+    q.o = ld3(r.o, i);
+    q.d = ld3(r.d, i);
+    q.maxd = double(r.maxd[i]);
+    q.solid = r.solid ? r.solid[i] != 0 : true;
+    q.mask = r.mask ? r.mask[i] : 0xffffffffu;
+    q.xs = r.xoff ? r.xs + r.xoff[i] : nullptr;
+    q.nx = r.xoff ? r.xoff[i + 1] - r.xoff[i] : 0u;
+    q.ok = qm::ray_finite(q.o, q.d, q.maxd);
+    return q;
+}
+template <class S>
+__device__ __forceinline__ bool ray_leaf(const Tree<S>& t, const RayIn<S>& q, uint32_t c, double& th, nm::V3& nh) {
+    const uint32_t memb = t.memb ? t.memb[c] : 1u;
+    if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
+    return qm::ray_collider(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), q.o, q.d, q.maxd, q.solid, th, nh);
+}
+__device__ __forceinline__ bool ray_visit(const NodeBox& b, nm::V3 o, nm::V3 d, double tclip) {
+    return qm::ray_box_entry(&b.lo.x, &b.hi.x, o, d, tclip) != INFINITY;
+}
+
+// closest-hit traversal: a node's two children are tested when the node is popped, against the ray clipped to the best hit so far; a leaf
+// child runs the exact test at once, internal children go on the stack nearer-entry last, so the nearer subtree is searched first and the
+// best distance shrinks early.  The answer does not depend on this order (lexicographic minimum of (t, collider)).
+template <class S, class Leaf>
+__device__ __forceinline__ void traverse_closest(const Tree<S>& t, int m, nm::V3 o, nm::V3 d, double maxd, const double& best_t, Leaf leaf) {
+    if (m <= 0) return;
+    if (qm::ray_box_entry(&t.nodes[0].lo.x, &t.nodes[0].hi.x, o, d, maxd) == INFINITY) return;
+    if (m == 1) { leaf(t.leaf[0]); return; }
+    int stack[Q_STACK];
+    int sp = 0;
+    stack[sp++] = 0;
+    while (sp > 0) {
+        const int2 c = t.child[stack[--sp]];
+        const double clip = nm::smin(maxd, best_t);
+        const NodeBox ba = t.nodes[c.x], bb = t.nodes[c.y];
+        const double ta = qm::ray_box_entry(&ba.lo.x, &ba.hi.x, o, d, clip), tb = qm::ray_box_entry(&bb.lo.x, &bb.hi.x, o, d, clip);
+        const bool b_first = tb < ta;
+        const int near = b_first ? c.y : c.x, far = b_first ? c.x : c.y;
+        const double tn = b_first ? tb : ta, tf = b_first ? ta : tb;
+        if (tn == INFINITY) continue;
+        if (near >= m - 1) leaf(t.leaf[near - (m - 1)]);
+        // the far child: a leaf is tested now (against the clip the near leaf may just have tightened), an internal node waits
+        if (tf != INFINITY && tf <= best_t) {
+            if (far >= m - 1) leaf(t.leaf[far - (m - 1)]);
+            else stack[sp++] = far;
+        }
+        if (near < m - 1) stack[sp++] = near;
+    }
+}
+
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, int32_t* __restrict__ out_c,
+                                                         S* __restrict__ out_t, S* __restrict__ out_n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    const RayIn<S> q = load_ray(r, i);
+    double best_t = INFINITY;
+    uint32_t best_c = 0xffffffffu;
+    nm::V3 best_n{0, 0, 0};
+    if (q.ok)
+        traverse_closest(t, *t.m, q.o, q.d, q.maxd, best_t, [&](uint32_t c) {
+            double th;
+            nm::V3 nh;
+            if (ray_leaf(t, q, c, th, nh) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_n = nh; }
+        });
+    const bool hit = best_c != 0xffffffffu;
+    out_c[i] = hit ? int32_t(best_c) : -1;
+    out_t[i] = hit ? S(best_t) : S(0);
+    out_n[3 * i] = S(best_n.x); out_n[3 * i + 1] = S(best_n.y); out_n[3 * i + 2] = S(best_n.z);
+}
+
+// ray_hits count pass: every hit, and the part of it the ray keeps (max_hits)
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_ray_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, uint32_t* __restrict__ full,
+                                                          uint32_t* __restrict__ kept) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    const RayIn<S> q = load_ray(r, i);
+    uint32_t cnt = 0;
+    if (q.ok)
+        traverse(t, *t.m, [&](const NodeBox& b) { return ray_visit(b, q.o, q.d, q.maxd); },
+                 [&](uint32_t c) { double th; nm::V3 nh; if (ray_leaf(t, q, c, th, nh)) ++cnt; });
+    full[i] = cnt;
+    const uint32_t mh = r.max_hits ? r.max_hits[i] : 0xffffffffu;
+    kept[i] = cnt < mh ? cnt : mh;
+}
+
+// in-place sort of one segment: insertion sort when short, heap sort otherwise (the keys of a segment are distinct)
+template <class Less, class Swap>
+__device__ void sort_segment(uint32_t n, Less less, Swap swp) {
+    if (n < 2) return;
+    if (n <= 16) {
+        for (uint32_t i = 1; i < n; ++i)
+            for (uint32_t j = i; j > 0 && less(j, j - 1); --j) swp(j, j - 1);
+        return;
+    }
+    auto sift = [&](uint32_t root, uint32_t end) {
+        for (;;) {
+            uint32_t c = 2 * root + 1;
+            if (c >= end) return;
+            if (c + 1 < end && less(c, c + 1)) ++c;
+            if (!less(root, c)) return;
+            swp(root, c);
+            root = c;
+        }
+    };
+    for (uint32_t s = n / 2; s-- > 0;) sift(s, n);
+    for (uint32_t e = n - 1; e > 0; --e) { swp(0, e); sift(0, e); }
+}
+
+// ray_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their normals
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, const uint64_t* __restrict__ full_off,
+                                                         const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
+                                                         uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ out_n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    const RayIn<S> q = load_ray(r, i);
+    if (!q.ok) return;
+    const uint64_t base = full_off[i];
+    const uint32_t n = uint32_t(full_off[i + 1] - base), keep = uint32_t(kept_off[i + 1] - kept_off[i]);
+    if (keep == 0) return;
+    double* ts = tmp_t + base;
+    uint32_t* cs = tmp_c + base;
+    uint32_t w = 0;
+    traverse(t, *t.m, [&](const NodeBox& b) { return ray_visit(b, q.o, q.d, q.maxd); },
+             [&](uint32_t c) {
+                 double th;
+                 nm::V3 nh;
+                 if (ray_leaf(t, q, c, th, nh) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+             });
+    sort_segment(
+        w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
+        [&](uint32_t a, uint32_t b) { const double x = ts[a]; ts[a] = ts[b]; ts[b] = x; const uint32_t y = cs[a]; cs[a] = cs[b]; cs[b] = y; });
+    const uint64_t o = kept_off[i];
+    for (uint32_t k = 0; k < keep && k < w; ++k) {
+        const uint32_t c = cs[k];
+        double th;
+        nm::V3 nh{0, 0, 0};
+        ray_leaf(t, q, c, th, nh);    // the same exact test again: the normal of this hit
+        out_c[o + k] = c;
+        if (out_t) out_t[o + k] = S(ts[k]);
+        if (out_n) { out_n[3 * (o + k)] = S(nh.x); out_n[3 * (o + k) + 1] = S(nh.y); out_n[3 * (o + k) + 2] = S(nh.z); }
+    }
+}
+
+// aabb_intersections: count, then emit + sort ascending by collider
+template <class S, bool EMIT>
+__global__ void __launch_bounds__(Q_THREADS) q_aabb(const __grid_constant__ Tree<S> t, int n, const S* __restrict__ qmn, const S* __restrict__ qmx,
+                                                     uint32_t* __restrict__ counts, const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const S a[3] = {qmn[3 * i], qmn[3 * i + 1], qmn[3 * i + 2]}, b[3] = {qmx[3 * i], qmx[3 * i + 1], qmx[3 * i + 2]};
+    const double ad[3] = {double(a[0]), double(a[1]), double(a[2])}, bd[3] = {double(b[0]), double(b[1]), double(b[2])};
+    uint32_t w = 0;
+    uint32_t* seg = EMIT ? out_c + off[i] : nullptr;
+    traverse(t, *t.m,
+             [&](const NodeBox& nb) {
+                 const double lo[3] = {nb.lo.x, nb.lo.y, nb.lo.z}, hi[3] = {nb.hi.x, nb.hi.y, nb.hi.z};
+                 return qm::aabb_overlap(ad, bd, lo, hi);
+             },
+             [&](uint32_t c) {
+                 if (!qm::aabb_overlap(a, b, t.tmn + 3 * size_t(c), t.tmx + 3 * size_t(c))) return;
+                 if (EMIT) seg[w] = c;
+                 ++w;
+             });
+    if (!EMIT) { counts[i] = w; return; }
+    sort_segment(w, [&](uint32_t x, uint32_t y) { return seg[x] < seg[y]; }, [&](uint32_t x, uint32_t y) { const uint32_t v = seg[x]; seg[x] = seg[y]; seg[y] = v; });
+}
+
+template <class S>
+class Queries final : public QueriesBase {
+   public:
+    Queries(cudaStream_t stream, ErrorSink* err) : stream_(stream), err_(err) {}
+
+    AvnStatus update(const AvnQueryColliders* c, uint32_t flags) override {
+        const bool keep_shapes = (flags & AVN_QUERY_SHAPES_UNCHANGED) != 0;
+        if (const char* why = qm::check_colliders(c, !keep_shapes, sizeof(S) == 8)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: %s", why);
+        if (keep_shapes && (!built_ || c->count != uint32_t(n_)))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: AVN_QUERY_SHAPES_UNCHANGED needs a previous update of the same count");
+        const int n = int(c->count);
+        built_ = false;
+        n_ = n;
+        const size_t nn = size_t(std::max(n, 1));
+        AVN_CUDA(pos_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(rot_.ensure(4 * nn * sizeof(S)));
+        AVN_CUDA(shape_.ensure(nn));
+        AVN_CUDA(dims_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(memb_.ensure(nn * sizeof(uint32_t)));
+        AVN_CUDA(tmn_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(tmx_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(cbox_.ensure(nn * sizeof(NodeBox)));
+        AVN_CUDA(centre_.ensure(nn * sizeof(float4)));
+        AVN_CUDA(valid_.ensure(nn));
+        AVN_CUDA(k0_.ensure(nn * 4)); AVN_CUDA(k1_.ensure(nn * 4)); AVN_CUDA(v0_.ensure(nn * 4)); AVN_CUDA(v1_.ensure(nn * 4));
+        const int nblocks = int((nn + RS_TILE - 1) / RS_TILE);
+        AVN_CUDA(hist_.ensure(size_t(256) * nblocks * 4));
+        AVN_CUDA(nodes_.ensure((2 * nn) * sizeof(NodeBox)));
+        AVN_CUDA(child_.ensure(nn * sizeof(int2)));
+        AVN_CUDA(parent_.ensure(2 * nn * sizeof(int)));
+        AVN_CUDA(arrived_.ensure(nn * sizeof(uint32_t)));
+        AVN_CUDA(meta_.ensure(64));
+        if (n > 0) {
+            AVN_CUDA(cudaMemcpyAsync(pos_.p, c->position, 3 * size_t(n) * sizeof(S), cudaMemcpyHostToDevice, stream_));
+            AVN_CUDA(cudaMemcpyAsync(rot_.p, c->rotation, 4 * size_t(n) * sizeof(S), cudaMemcpyHostToDevice, stream_));
+            if (!keep_shapes) {
+                AVN_CUDA(cudaMemcpyAsync(shape_.p, c->shape, size_t(n), cudaMemcpyHostToDevice, stream_));
+                AVN_CUDA(cudaMemcpyAsync(dims_.p, c->dims, 3 * size_t(n) * sizeof(S), cudaMemcpyHostToDevice, stream_));
+                has_memb_ = c->memberships != nullptr;
+                if (has_memb_) AVN_CUDA(cudaMemcpyAsync(memb_.p, c->memberships, size_t(n) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream_));
+            }
+        }
+        // meta: [0] = m (colliders in the tree), [1..6] = ordered-integer scene bounds of the centres (min x y z, max x y z)
+        int* d_m = meta_.as<int>();
+        uint32_t* sb = meta_.as<uint32_t>() + 1;
+        AVN_CUDA(cudaMemsetAsync(d_m, 0, 4, stream_));
+        AVN_CUDA(cudaMemsetAsync(sb, 0xff, 12, stream_));
+        AVN_CUDA(cudaMemsetAsync(sb + 3, 0, 12, stream_));
+        const Tree<S> t = tree();
+        if (n > 0) {
+            const unsigned g = unsigned((n + 255) / 256);
+            q_prepare<S><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
+            q_codes<<<g, 256, 0, stream_>>>(n, centre_.as<float4>(), valid_.as<uint8_t>(), sb, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+            uint32_t *ka = k0_.as<uint32_t>(), *kb = k1_.as<uint32_t>(), *va = v0_.as<uint32_t>(), *vb = v1_.as<uint32_t>();
+            for (int pass = 0; pass < 4; ++pass) {
+                rs_histogram<uint32_t><<<nblocks, RS_THREADS, 0, stream_>>>(ka, n, 8 * pass, hist_.as<uint32_t>(), nblocks);
+                if (nblocks <= RS_FUSE_MAX_BLOCKS) {
+                    rs_scatter<uint32_t, true><<<nblocks, RS_THREADS, 0, stream_>>>(ka, va, n, 8 * pass, hist_.as<uint32_t>(), nblocks, kb, vb);
+                } else {
+                    rs_scan<<<1, 1024, 0, stream_>>>(hist_.as<uint32_t>(), 256 * nblocks);
+                    rs_scatter<uint32_t, false><<<nblocks, RS_THREADS, 0, stream_>>>(ka, va, n, 8 * pass, hist_.as<uint32_t>(), nblocks, kb, vb);
+                }
+                std::swap(ka, kb);
+                std::swap(va, vb);
+            }
+            // four passes: sorted keys and collider indices are back in k0_ / v0_
+            AVN_CUDA(cudaMemsetAsync(arrived_.p, 0, size_t(n) * sizeof(uint32_t), stream_));
+            q_karras<<<g, 256, 0, stream_>>>(d_m, n, k0_.as<uint32_t>(), child_.as<int2>(), parent_.as<int>());
+            q_refit<<<g, 256, 0, stream_>>>(d_m, v0_.as<uint32_t>(), cbox_.as<NodeBox>(), parent_.as<int>(), child_.as<int2>(), arrived_.as<uint32_t>(),
+                                            nodes_.as<NodeBox>());
+            AVN_CUDA(cudaGetLastError());
+        }
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        built_ = true;
+        return AVN_OK;
+    }
+
+    AvnStatus cast_ray(const AvnRayBatch* r, AvnRayClosest* out) override {
+        AvnStatus st = rays_in(r, "avn_query_cast_ray");
+        if (st != AVN_OK) return st;
+        if (!out || !out->collider || !out->distance || !out->normal)
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_cast_ray: collider, distance and normal outputs are required");
+        const int n = int(r->count);
+        if (n == 0) return AVN_OK;
+        AVN_CUDA(oc_.ensure(size_t(n) * 4));
+        AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
+        AVN_CUDA(on_.ensure(3 * size_t(n) * sizeof(S)));
+        q_cast_ray<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
+        AVN_CUDA(cudaGetLastError());
+        AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->normal, on_.p, 3 * size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    AvnStatus ray_hits(const AvnRayBatch* r, AvnHitList* out) override {
+        AvnStatus st = rays_in(r, "avn_query_ray_hits");
+        if (st != AVN_OK) return st;
+        if ((st = list_out(out, "avn_query_ray_hits")) != AVN_OK) return st;
+        const int n = int(r->count);
+        AVN_CUDA(full_.ensure(size_t(n + 1) * 4));
+        AVN_CUDA(kept_.ensure(size_t(n + 1) * 4));
+        AVN_CUDA(full_off_.ensure(size_t(n + 1) * 8));
+        AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
+        const Tree<S> t = tree();
+        const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        if (n > 0) q_ray_count<S><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        uint64_t tot[2];
+        if ((st = scan(full_.as<uint32_t>(), n, full_off_.as<uint64_t>())) != AVN_OK) return st;
+        if ((st = scan(kept_.as<uint32_t>(), n, kept_off_.as<uint64_t>())) != AVN_OK) return st;
+        AVN_CUDA(cudaMemcpyAsync(&tot[0], full_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(&tot[1], kept_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        out->count = tot[1];
+        if (tot[1] > out->capacity)
+            return err_->fail(AVN_ERR_CAPACITY, "avn_query_ray_hits: %llu hits, capacity %llu", (unsigned long long)tot[1], (unsigned long long)out->capacity);
+        const size_t nf = size_t(std::max<uint64_t>(tot[0], 1)), nk = size_t(std::max<uint64_t>(tot[1], 1));
+        AVN_CUDA(tmp_t_.ensure(nf * 8));
+        AVN_CUDA(tmp_c_.ensure(nf * 4));
+        AVN_CUDA(oc_.ensure(nk * 4));
+        AVN_CUDA(ot_.ensure(nk * sizeof(S)));
+        AVN_CUDA(on_.ensure(3 * nk * sizeof(S)));
+        if (n > 0 && tot[1] > 0) {
+            q_ray_emit<S><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
+                                                         oc_.as<uint32_t>(), ot_.as<S>(), on_.as<S>());
+            AVN_CUDA(cudaGetLastError());
+        }
+        return list_download(out, n, kept_off_.as<uint64_t>(), tot[1], true);
+    }
+
+    AvnStatus aabb_intersections(uint32_t count, const void* mn, const void* mx, AvnHitList* out) override {
+        if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_aabb_intersections before any avn_query_update");
+        if (count && (!mn || !mx)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_aabb_intersections: min and max are required");
+        AvnStatus st = list_out(out, "avn_query_aabb_intersections");
+        if (st != AVN_OK) return st;
+        const int n = int(count);
+        const size_t nn = size_t(std::max(n, 1));
+        AVN_CUDA(qmn_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(qmx_.ensure(3 * nn * sizeof(S)));
+        AVN_CUDA(full_.ensure((nn + 1) * 4));
+        AVN_CUDA(kept_off_.ensure((nn + 1) * 8));
+        if (n > 0) {
+            AVN_CUDA(cudaMemcpyAsync(qmn_.p, mn, 3 * size_t(n) * sizeof(S), cudaMemcpyHostToDevice, stream_));
+            AVN_CUDA(cudaMemcpyAsync(qmx_.p, mx, 3 * size_t(n) * sizeof(S), cudaMemcpyHostToDevice, stream_));
+        }
+        const Tree<S> t = tree();
+        const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        if (n > 0) q_aabb<S, false><<<g, Q_THREADS, 0, stream_>>>(t, n, qmn_.as<S>(), qmx_.as<S>(), full_.as<uint32_t>(), nullptr, nullptr);
+        if ((st = scan(full_.as<uint32_t>(), n, kept_off_.as<uint64_t>())) != AVN_OK) return st;
+        uint64_t total = 0;
+        AVN_CUDA(cudaMemcpyAsync(&total, kept_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        out->count = total;
+        if (total > out->capacity)
+            return err_->fail(AVN_ERR_CAPACITY, "avn_query_aabb_intersections: %llu hits, capacity %llu", (unsigned long long)total, (unsigned long long)out->capacity);
+        AVN_CUDA(oc_.ensure(size_t(std::max<uint64_t>(total, 1)) * 4));
+        if (n > 0 && total > 0) {
+            q_aabb<S, true><<<g, Q_THREADS, 0, stream_>>>(t, n, qmn_.as<S>(), qmx_.as<S>(), nullptr, kept_off_.as<uint64_t>(), oc_.as<uint32_t>());
+            AVN_CUDA(cudaGetLastError());
+        }
+        return list_download(out, n, kept_off_.as<uint64_t>(), total, false);
+    }
+
+   private:
+    Tree<S> tree() const {
+        Tree<S> t{};
+        t.n = n_;
+        t.m = meta_.as<int>();
+        t.shape = shape_.as<uint8_t>(); t.dims = dims_.as<S>(); t.pos = pos_.as<S>(); t.rot = rot_.as<S>();
+        t.memb = has_memb_ ? memb_.as<uint32_t>() : nullptr;
+        t.tmn = tmn_.as<S>(); t.tmx = tmx_.as<S>();
+        t.nodes = nodes_.as<NodeBox>(); t.child = child_.as<int2>(); t.leaf = v0_.as<uint32_t>();
+        return t;
+    }
+
+    // validate on the host, then upload the ray columns into rays_
+    AvnStatus rays_in(const AvnRayBatch* r, const char* what) {
+        if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
+        if (const char* why = qm::check_rays(r)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
+        if (r->count >= 0x7fffffffu) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: too many rays", what);
+        const size_t n = r->count;
+        rays_ = Rays<S>{};
+        rays_.n = int(n);
+        if (n == 0) return AVN_OK;
+        AvnStatus st;
+#define UPR(buf, host, cnt, T, dst) if ((st = up<T>(buf, host, cnt, &dst)) != AVN_OK) return st
+        UPR(r_o_, r->origin, 3 * n, S, rays_.o);
+        UPR(r_d_, r->direction, 3 * n, S, rays_.d);
+        UPR(r_maxd_, r->max_distance, n, S, rays_.maxd);
+        UPR(r_solid_, r->solid, n, uint8_t, rays_.solid);
+        UPR(r_mh_, r->max_hits, n, uint32_t, rays_.max_hits);
+        UPR(r_mask_, r->mask, n, uint32_t, rays_.mask);
+        UPR(r_xoff_, r->exclude_offsets, n + 1, uint32_t, rays_.xoff);
+        if (r->exclude_offsets) UPR(r_xs_, r->exclude_count ? r->exclude : nullptr, r->exclude_count, uint32_t, rays_.xs);
+#undef UPR
+        return AVN_OK;
+    }
+    AvnStatus list_out(AvnHitList* out, const char* what) {
+        if (!out || !out->offsets || (out->capacity && !out->collider))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: offsets and (with a capacity) collider are required", what);
+        return AVN_OK;
+    }
+    // exclusive scan of n counts -> offsets[0..n], offsets[n] = total
+    AvnStatus scan(const uint32_t* counts, int n, uint64_t* offsets) {
+        if (n == 0) {
+            AVN_CUDA(cudaMemsetAsync(offsets, 0, 8, stream_));
+            return AVN_OK;
+        }
+        const int sblocks = (n + 1023) / 1024;
+        AVN_CUDA(block_sums_.ensure(size_t(sblocks) * 8));
+        scan_block_sums<<<sblocks, 1024, 0, stream_>>>(counts, n, block_sums_.as<uint64_t>());
+        scan_block_offsets<<<1, 1024, 0, stream_>>>(block_sums_.as<uint64_t>(), sblocks, offsets + n);
+        scan_apply<<<sblocks, 1024, 0, stream_>>>(counts, n, block_sums_.as<uint64_t>(), offsets);
+        AVN_CUDA(cudaGetLastError());
+        return AVN_OK;
+    }
+    AvnStatus list_download(AvnHitList* out, int n, const uint64_t* d_off, uint64_t total, bool ray) {
+        AVN_CUDA(cudaMemcpyAsync(out->offsets, d_off, size_t(n + 1) * 8, cudaMemcpyDeviceToHost, stream_));
+        if (total) {
+            AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, total * 4, cudaMemcpyDeviceToHost, stream_));
+            if (ray && out->distance) AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, total * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+            if (ray && out->normal) AVN_CUDA(cudaMemcpyAsync(out->normal, on_.p, 3 * total * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        }
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+    template <class T> AvnStatus up(DevBuf& buf, const void* host, size_t count, const T** dev) {
+        *dev = nullptr;
+        if (!host || count == 0) return AVN_OK;
+        AVN_CUDA(buf.ensure(count * sizeof(T)));
+        AVN_CUDA(cudaMemcpyAsync(buf.p, host, count * sizeof(T), cudaMemcpyHostToDevice, stream_));
+        *dev = buf.as<T>();
+        return AVN_OK;
+    }
+
+    cudaStream_t stream_;
+    ErrorSink* err_;
+    bool built_ = false, has_memb_ = false;
+    int n_ = 0;
+    Rays<S> rays_{};
+    DevBuf pos_, rot_, shape_, dims_, memb_, tmn_, tmx_, cbox_, centre_, valid_, k0_, k1_, v0_, v1_, hist_, nodes_, child_, parent_, arrived_, meta_;
+    DevBuf r_o_, r_d_, r_maxd_, r_solid_, r_mh_, r_mask_, r_xoff_, r_xs_;
+    DevBuf full_, kept_, full_off_, kept_off_, block_sums_, tmp_t_, tmp_c_, oc_, ot_, on_, qmn_, qmx_;
+};
+
+}  // namespace
+
+QueriesBase* make_queries(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err) {
+    if (scalar_bits == 32) return new Queries<float>(stream, err);
+    if (scalar_bits == 64) return new Queries<double>(stream, err);
+    return nullptr;
+}
+
+}  // namespace avn

@@ -48,6 +48,14 @@ def _load():
         lib.avh_raw_manifolds.restype = None
         lib.avh_pair_count.argtypes = [_vp]
         lib.avh_pair_count.restype = C.c_uint32
+        P = C.POINTER
+        lib.avh_query_error.argtypes = []
+        lib.avh_query_error.restype = C.c_char_p
+        lib.avh_query_cast_ray.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnRayBatch), P(api.AvnRayClosest)]
+        lib.avh_query_ray_hits.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnRayBatch), P(api.AvnHitList)]
+        lib.avh_query_aabb_intersections.argtypes = [C.c_uint32, P(api.AvnQueryColliders), C.c_uint32, _vp, _vp, P(api.AvnHitList)]
+        for f in (lib.avh_query_cast_ray, lib.avh_query_ray_hits, lib.avh_query_aabb_intersections):
+            f.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -78,6 +86,54 @@ def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders:
     if f64_anchors:
         out["anchor1_f64"], out["anchor2_f64"] = a1d, a2d
     return out
+
+
+# ---- spatial queries by brute force over every collider (csrc/query_math.hpp): what the device tree must reproduce bit for bit
+def _query_check(lib, st: int) -> None:
+    if st != api.OK:
+        raise api.AvianError(st, lib.avh_query_error().decode())
+
+
+def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays") -> dict:
+    """The closest hit of every ray (same output as Context.cast_ray)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    r, keep_r = rays.as_struct(dt)
+    n = rays.count
+    out = {"collider": np.zeros(n, dtype=np.int32), "distance": np.zeros(n, dtype=dt), "normal": np.zeros((n, 3), dtype=dt)}
+    o = api.AvnRayClosest(*(_p(out[k]) for k in ("collider", "distance", "normal")))
+    _query_check(lib, lib.avh_query_cast_ray(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(o)))
+    return out
+
+
+def query_ray_hits(scalar, colliders: "api.QueryColliders", rays: "api.Rays") -> dict:
+    """Every ray's max_hits nearest hits in (t, collider) order as CSR (same output as Context.ray_hits)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    r, keep_r = rays.as_struct(dt)
+    h, out = api.hit_list(rays.count, 0, dt, True)
+    st = lib.avh_query_ray_hits(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(h))
+    if st == api.ERR_CAPACITY:
+        h, out = api.hit_list(rays.count, int(h.count), dt, True)
+        st = lib.avh_query_ray_hits(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(h))
+    _query_check(lib, st)
+    return api.hit_list_result(h, out)
+
+
+def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, aabb_max) -> dict:
+    """Per query box the colliders whose tight AABB it touches, ascending (same output as Context.aabb_intersections)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    mn = np.ascontiguousarray(aabb_min, dtype=dt).reshape(-1, 3)
+    mx = np.ascontiguousarray(aabb_max, dtype=dt).reshape(-1, 3)
+    n, bits = int(mn.shape[0]), 32 if dt == np.float32 else 64
+    h, out = api.hit_list(n, 0, dt, False)
+    st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
+    if st == api.ERR_CAPACITY:
+        h, out = api.hit_list(n, int(h.count), dt, False)
+        st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
+    _query_check(lib, st)
+    return api.hit_list_result(h, out)
 
 
 class HostPipeline:

@@ -8,10 +8,12 @@
 //     the status-change loop and ConstraintGraph push/pop colouring (narrow_phase/system_param.rs:136-389,
 //     constraint_graph.rs:163-296)
 //   * export of the manifolds as per-colour columns in the layout of AvnManifoldColumns.
+//   * spatial queries by brute force over every collider (csrc/query_math.hpp): the checker of the device tree (csrc/queries.cu).
 // It contains no solver or broad-phase code: those are the GPU library (product) or oracle/ (tests).
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <queue>
 #include <unordered_map>
@@ -20,6 +22,7 @@
 #include "../../include/avian_b200.h"
 #include "../csrc/narrow_math.hpp"
 #include "../csrc/contact_rows.hpp"
+#include "../csrc/query_math.hpp"
 
 namespace {
 
@@ -573,5 +576,140 @@ void avh_rows_narrow(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c
 }
 
 uint32_t avh_pair_count(AvhPipeline* h) { return uint32_t(reinterpret_cast<Pipeline*>(h)->active.size()); }
+
+}  // extern "C"
+
+// ---- spatial queries, brute force over every collider (the checker of csrc/queries.cu; same header, same conventions) ----------------
+// Arguments are the ABI structs of avn_query_*; the colliders are passed with every call.  Returns an AvnStatus; avh_query_error() says why.
+namespace {
+thread_local char g_query_error[256];
+int query_fail(AvnStatus st, const char* why) {
+    snprintf(g_query_error, sizeof g_query_error, "%s", why);
+    return st;
+}
+
+struct QueryScene {
+    const AvnQueryColliders* c; bool f64;
+    Col dims, pos, rot;
+    QueryScene(const AvnQueryColliders* cc, bool f) : c(cc), f64(f), dims{cc->dims, f}, pos{cc->position, f}, rot{cc->rotation, f} {}
+    bool valid(uint32_t i) const { return qm::collider_valid(dims.v3(i), pos.v3(i), rot.q(i)); }
+    uint32_t memb(uint32_t i) const { return c->memberships ? c->memberships[i] : 1u; }
+};
+struct RayView {
+    V3 o, d; S maxd; bool solid, ok; uint32_t mask; const uint32_t* xs; uint32_t nx;
+};
+RayView ray_at(const AvnRayBatch* r, bool f64, uint32_t i) {
+    Col o{r->origin, f64}, d{r->direction, f64}, m{r->max_distance, f64};
+    RayView v;
+    v.o = o.v3(i); v.d = d.v3(i); v.maxd = m.at(i);
+    v.solid = r->solid ? r->solid[i] != 0 : true;
+    v.mask = r->mask ? r->mask[i] : 0xffffffffu;
+    v.xs = r->exclude_offsets ? r->exclude + r->exclude_offsets[i] : nullptr;
+    v.nx = r->exclude_offsets ? r->exclude_offsets[i + 1] - r->exclude_offsets[i] : 0u;
+    v.ok = qm::ray_finite(v.o, v.d, v.maxd);
+    return v;
+}
+struct RayHit { S t; uint32_t c; V3 n; };
+// every hit of one ray, sorted by (t, collider)
+void all_hits(const QueryScene& sc, const RayView& v, std::vector<RayHit>& out) {
+    out.clear();
+    if (!v.ok) return;
+    for (uint32_t c = 0; c < sc.c->count; ++c) {
+        if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
+        RayHit h{0, c, V3{0, 0, 0}};
+        if (qm::ray_collider(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), v.o, v.d, v.maxd, v.solid, h.t, h.n)) out.push_back(h);
+    }
+    std::sort(out.begin(), out.end(), [](const RayHit& a, const RayHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
+}
+template <class T>
+void query_aabbs(const QueryScene& sc, uint32_t n, const T* mn, const T* mx, std::vector<std::vector<uint32_t>>& per) {
+    for (uint32_t c = 0; c < sc.c->count; ++c) {
+        if (!sc.valid(c)) continue;
+        V3 a, b;
+        qm::collider_aabb(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), a, b);
+        const T tmn[3] = {T(a.x), T(a.y), T(a.z)}, tmx[3] = {T(b.x), T(b.y), T(b.z)};
+        for (uint32_t i = 0; i < n; ++i)
+            if (qm::aabb_overlap(mn + 3 * size_t(i), mx + 3 * size_t(i), tmn, tmx)) per[i].push_back(c);
+    }
+}
+
+int query_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r) {
+    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (r)
+        if (const char* why = qm::check_rays(r)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    return AVN_OK;
+}
+}  // namespace
+
+extern "C" {
+
+const char* avh_query_error() { return g_query_error; }
+
+int avh_query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out) {
+    if (int st = query_inputs(scalar_bits, c, r)) return st;
+    if (!out || (r->count && (!out->collider || !out->distance || !out->normal))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    ColW ot{out->distance, f64}, on{out->normal, f64};
+    std::vector<RayHit> hits;
+    for (uint32_t i = 0; i < r->count; ++i) {
+        all_hits(sc, ray_at(r, f64, i), hits);
+        out->collider[i] = hits.empty() ? -1 : int32_t(hits[0].c);
+        ot.set(i, hits.empty() ? 0 : hits[0].t);
+        on.set3(i, hits.empty() ? V3{0, 0, 0} : hits[0].n);
+    }
+    return AVN_OK;
+}
+
+int avh_query_ray_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out) {
+    if (int st = query_inputs(scalar_bits, c, r)) return st;
+    if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    std::vector<std::vector<RayHit>> per(r->count);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < r->count; ++i) {
+        all_hits(sc, ray_at(r, f64, i), per[i]);
+        const uint32_t mh = r->max_hits ? r->max_hits[i] : 0xffffffffu;
+        if (per[i].size() > mh) per[i].resize(mh);
+        total += per[i].size();
+    }
+    out->count = total;
+    if (total > out->capacity) return query_fail(AVN_ERR_CAPACITY, "capacity");
+    ColW ot{out->distance, f64}, on{out->normal, f64};
+    uint64_t k = 0;
+    for (uint32_t i = 0; i < r->count; ++i) {
+        out->offsets[i] = k;
+        for (const RayHit& h : per[i]) {
+            out->collider[k] = h.c;
+            if (out->distance) ot.set(k, h.t);
+            if (out->normal) on.set3(k, h.n);
+            ++k;
+        }
+    }
+    out->offsets[r->count] = k;
+    return AVN_OK;
+}
+
+int avh_query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, uint32_t n, const void* mn, const void* mx, AvnHitList* out) {
+    if (int st = query_inputs(scalar_bits, c, nullptr)) return st;
+    if (n && (!mn || !mx)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "min and max are required");
+    if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
+    const QueryScene sc(c, scalar_bits == 64);
+    std::vector<std::vector<uint32_t>> per(n);
+    if (scalar_bits == 64) query_aabbs(sc, n, static_cast<const double*>(mn), static_cast<const double*>(mx), per);
+    else query_aabbs(sc, n, static_cast<const float*>(mn), static_cast<const float*>(mx), per);
+    uint64_t total = 0;
+    for (const auto& v : per) total += v.size();
+    out->count = total;
+    if (total > out->capacity) return query_fail(AVN_ERR_CAPACITY, "capacity");
+    uint64_t k = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        out->offsets[i] = k;
+        for (uint32_t col : per[i]) out->collider[k++] = col;
+    }
+    out->offsets[n] = k;
+    return AVN_OK;
+}
 
 }  // extern "C"

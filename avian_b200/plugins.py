@@ -77,6 +77,46 @@ class SolverPlugin:
         self.ctx.solver_step(params, bodies, manifolds, joints)
 
 
+class SpatialQueryPlugin:
+    """spatial_query/mod.rs:400-417 on the GPU: update_spatial_query_pipeline (avn_query_update over every collider of the world) and the
+    raycast system (RayCaster -> RayHits through avn_query_ray_hits).  Collider = body, as in the narrow phase of this fixture.
+    Runs after the physics step (PhysicsStepSystems::SpatialQuery), so it sees the poses the step produced."""
+    def __init__(self, ctx: api.Context):
+        self.ctx = ctx
+
+    @staticmethod
+    def colliders(world: "World", memberships: np.ndarray | None = None) -> api.QueryColliders:
+        return api.QueryColliders(shape=world.scene.shape_type.astype(np.uint8), dims=world.scene.dims, position=world.bodies.position,
+                                  rotation=world.bodies.rotation, memberships=memberships)
+
+    def update_pipeline(self, world: "World", memberships: np.ndarray | None = None, shapes_unchanged: bool = False) -> None:
+        """SpatialQueryPipeline::update from the world's current poses.  shapes_unchanged: the caller vouches that shapes, dims and
+        memberships equal those of its previous update of this context (AVN_QUERY_SHAPES_UNCHANGED); only the poses are copied, and
+        `memberships` is then not read."""
+        self.ctx.query_update(self.colliders(world, memberships), shapes_unchanged=shapes_unchanged)
+
+    @staticmethod
+    def ray_casters(origin, direction, max_distance, max_hits=None, solid=None, mask=None, enabled=None, owner=None, ignore_self=None,
+                    exclude=None) -> api.Rays:
+        """A batch of RayCaster components as rays: a disabled caster keeps no hits (max_hits 0); ignore_self excludes the caster's own
+        collider `owner` (-1 = none) on top of its filter's excluded entities `exclude` (per caster, iterables)."""
+        n = int(np.asarray(origin).reshape(-1, 3).shape[0])
+        mh = np.full(n, api.MAX_HITS_ALL, dtype=np.uint32) if max_hits is None else np.array(max_hits, dtype=np.uint32)
+        if enabled is not None:
+            mh = np.where(np.asarray(enabled, dtype=bool), mh, 0).astype(np.uint32)
+        ex = [list(e) for e in exclude] if exclude is not None else [[] for _ in range(n)]
+        if owner is not None:
+            own = np.asarray(owner, dtype=np.int64)
+            ign = np.ones(n, dtype=bool) if ignore_self is None else np.asarray(ignore_self, dtype=bool)   # RayCaster::ignore_self defaults to true
+            for i in np.nonzero(ign & (own >= 0))[0]:
+                ex[i].append(int(own[i]))
+        return api.Rays(origin=origin, direction=direction, max_distance=max_distance, solid=solid, max_hits=mh, mask=mask, exclude=ex)
+
+    def raycast(self, rays: api.Rays) -> dict:
+        """The raycast system: every caster's RayHits (CSR; per caster its max_hits nearest, sorted by distance)."""
+        return self.ctx.ray_hits(rays)
+
+
 class PhysicsPlugins:
     """The plugin group (src/lib.rs:813-843) restricted to the hot path."""
     def __init__(self, ctx: api.Context | None = None):

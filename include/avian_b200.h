@@ -576,6 +576,75 @@ typedef struct AvnIslandsStep {
 /* Once per step, after avn_contacts_step and the solver stage of the same step (it consumes that step's contact events). */
 AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step);
 
+/* ---- spatial queries (SpatialQueryPlugin, src/lib.rs:839; spatial_query/pipeline.rs): a collider tree rebuilt on the device by every
+ *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid and sphere colliders.
+ *      The per-shape arithmetic is this repository's own (avian_b200/csrc/query_math.hpp, shared with the host fixture; parry3d is not
+ *      vendored), so results equal the host brute force over every collider bit for bit, independent of the tree.  Conventions:
+ *        - a ray is origin + t * direction, t in units of |direction| (pass a unit Dir3); a hit counts when 0 <= t <= max_distance;
+ *        - shapes are closed; origin inside and solid -> t = 0, normal 0; origin inside and hollow -> the exit, outward normal there;
+ *        - cuboid normal: outward normal of the entering face (largest entering slab parameter, ties to the lowest local axis); a direction
+ *          component that is exactly 0 leaves its axis unconstrained when the origin is inside that slab and misses otherwise;
+ *        - filter (SpatialQueryFilter::test, query_filter.rs:97-101): (memberships & mask) != 0 and not in the ray's excluded list;
+ *        - AABB test: inclusive compares (Aabb::intersects) against the collider's tight AABB (compute_aabb) rounded to the column scalar,
+ *          no filter, as pipeline.rs:709-729;
+ *        - the rotation is the quaternion's, normalised: the AABB and the ray test see the same box for a quaternion of any nonzero length;
+ *        - colliders with a non-finite pose or dims or a zero quaternion are never reported; negative dims are refused; rays with a
+ *          non-finite origin, direction or max_distance hit nothing.
+ *      Stated deviations: the closest hit is the lexicographic minimum of (t, collider index), where the reference takes the first in tree
+ *      order; ray_hits keeps the max_hits NEAREST hits sorted by (t, collider index) — RayHits::iter_sorted order — where the reference keeps
+ *      the first max_hits in tree order, unordered (pipeline.rs:213-216); the two sets are equal when a ray has no more than max_hits hits.
+ *      Not covered: shape casts, point projection, shape / point intersections, the *_callback early exits, several GPUs. ----------------- */
+typedef struct AvnQueryColliders {
+    uint32_t count;
+    uint32_t _pad;
+    const uint8_t* shape;              /* [C] AvnShape */
+    const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] */
+    const void* position;              /* [C][3] collider Position */
+    const void* rotation;              /* [C][4] collider Rotation */
+    const uint32_t* memberships;       /* [C] CollisionLayers::memberships; NULL = 1 (the default layer) */
+} AvnQueryColliders;
+#define AVN_QUERY_SHAPES_UNCHANGED 0x1u   /* shape, dims and memberships equal the previous update's (same count): not copied again */
+
+typedef struct AvnRayBatch {
+    uint32_t count;
+    uint32_t exclude_count;            /* length of exclude[] */
+    const void* origin;                /* [n][3] */
+    const void* direction;             /* [n][3] */
+    const void* max_distance;          /* [n] */
+    const uint8_t* solid;              /* [n] NULL = all solid */
+    const uint32_t* max_hits;          /* [n] ray_hits only: 0 = none, 0xFFFFFFFF = all; NULL = all */
+    const uint32_t* mask;              /* [n] SpatialQueryFilter::mask; NULL = all layers */
+    const uint32_t* exclude_offsets;   /* [n + 1] CSR of excluded collider indices (excluded_entities, RayCaster::ignore_self); NULL = none */
+    const uint32_t* exclude;           /* [exclude_count] */
+} AvnRayBatch;
+
+typedef struct AvnRayClosest {         /* per ray */
+    int32_t* collider;                 /* [n] out: collider index, -1 = no hit */
+    void* distance;                    /* [n] out (0 when no hit) */
+    void* normal;                      /* [n][3] out (0 when no hit) */
+} AvnRayClosest;
+
+typedef struct AvnHitList {            /* CSR: the hits of query i are [offsets[i], offsets[i+1]) */
+    uint64_t capacity;                 /* in: entries collider / distance / normal can hold */
+    uint64_t count;                    /* out: total hits; above capacity -> AVN_ERR_CAPACITY and nothing else is written */
+    uint64_t* offsets;                 /* [n + 1] out */
+    uint32_t* collider;                /* [capacity] out */
+    void* distance;                    /* [capacity] out, ray hits only (NULL = not wanted) */
+    void* normal;                      /* [capacity][3] out, ray hits only (NULL = not wanted) */
+} AvnHitList;
+
+/* Replaces update_spatial_query_pipeline / SpatialQueryPipeline::update (spatial_query/system_param.rs:80-82, pipeline.rs:96-133): the
+ * tree over every collider passed, rebuilt from scratch (LBVH: Morton codes, Karras hierarchy, bottom-up refit).  Collider index = row. */
+AvnStatus avn_query_update(AvnContext* ctx, const AvnQueryColliders* colliders, uint32_t flags);
+/* Replaces SpatialQueryPipeline::cast_ray (pipeline.rs:156-180), one query per ray.  Before any update: AVN_ERR_INVALID_ARGUMENT. */
+AvnStatus avn_query_cast_ray(AvnContext* ctx, const AvnRayBatch* rays, AvnRayClosest* out);
+/* Replaces SpatialQueryPipeline::ray_hits (pipeline.rs:182-216) and the raycast system's RayHits (ray_caster.rs:250-309): per ray its
+ * max_hits nearest hits in (t, collider index) order. */
+AvnStatus avn_query_ray_hits(AvnContext* ctx, const AvnRayBatch* rays, AvnHitList* out);
+/* Replaces SpatialQueryPipeline::aabb_intersections_with_aabb (pipeline.rs:690-729): per query box the colliders whose tight AABB it
+ * touches, ascending by index.  min / max: [n][3] in the column scalar. */
+AvnStatus avn_query_aabb_intersections(AvnContext* ctx, uint32_t count, const void* min, const void* max, AvnHitList* out);
+
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out);
 
 /*
