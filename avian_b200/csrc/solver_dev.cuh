@@ -31,14 +31,10 @@ enum { CP_N = 0, CP_T1 = 1, CP_TV = 2, CP_IDX = 3, CP_PT0 = 4, CP_PLANES = CP_PT
 // precedes it in the same allocation (vel | dlt | counters | pcr) it is the "hot" range pinned in L2 by the access-policy window.
 // info lane of plane CP_IDX
 enum { CI_NP_MASK = 0x7, CI_ZERO1 = 1 << 4, CI_ZERO2 = 1 << 5, CI_NONDYN = 1 << 6, CI_TANGENT = 1 << 7,
-       CI_VER1 = 1 << 8, CI_VER2 = 1 << 9,     // VERx: side x is a versioned body (has a SolverBody) in wavefront mode
-       CI_FIV1 = 1 << 10, CI_FIV2 = 1 << 11,  // this constraint is the LAST relax event of body x: it also integrates its velocity
-       CI_FIP1 = 1 << 12, CI_FIP2 = 1 << 13 }; // this constraint is the LAST solve event of body x: it also integrates its position
+       CI_VER1 = 1 << 8, CI_VER2 = 1 << 9 };   // VERx: side x is a versioned body (has a SolverBody) in wavefront mode
 // flags lane of inr[2*i]
 enum { BF_LOCK_MASK = 0x3f, BF_HAS_SOLVER_BODY = 1 << 8, BF_KINEMATIC = 1 << 9, BF_GYRO = 1 << 10, BF_DYNAMIC = 1 << 11,
-       BF_CUSTOM_VEL = 1 << 12, BF_CUSTOM_POS = 1 << 13, BF_FUSE_IV = 1 << 14, BF_FUSE_IP = 1 << 15, BF_DOMINANCE_SHIFT = 16 };
-// BF_FUSE_IV / BF_FUSE_IP (wavefront mode): the body's integrate_velocities / integrate_positions step is plain enough (no gyroscopic
-// torque, no speed clamp, no custom-integration marker) to be executed by the contact item that holds the body's state right before it.
+       BF_CUSTOM_VEL = 1 << 12, BF_CUSTOM_POS = 1 << 13, BF_DOMINANCE_SHIFT = 16 };
 
 enum { JP_IDX = 0,   // {body1, body2, type | limit_enabled<<8 | damping<<16 | zero1<<24 | zero2<<25, original index}
        JP_R1 = 1,    // {world_r1.xyz, compliance0}
@@ -64,7 +60,6 @@ struct DevSolver {
     int color_off[AVN_GRAPH_COLOR_COUNT + 1];    // SLOT ranges per colour, each start a multiple of 32; [24] = Mpad
     int color_len[AVN_GRAPH_COLOR_COUNT];        // manifolds in the colour
     int wave;                                    // 1: wavefront (dependency-counter) substep loop, 0: grid barriers
-    int* sm_slots;                               // [SMs] block tickets for the SM-major warp numbering of the wavefront loop (NULL = block-major)
     unsigned int* ver;                           // [B+1] per-body event counter (wavefront mode)
     int* deg;                                    // [B+1] contact constraints touching the body (wavefront mode)
     int* stamp;                                  // [B+1] 1 + last colour that ranked the body: detects a body listed twice in one colour
@@ -102,10 +97,6 @@ struct DevSolver {
     const int* jbody1[AVN_JOINT_TYPE_COUNT]; const int* jbody2[AVN_JOINT_TYPE_COUNT];
     S* jforce[AVN_JOINT_TYPE_COUNT]; S* jtorque[AVN_JOINT_TYPE_COUNT];
     int any_joint_damping;
-    // island-per-warp schedule (island_lists.hpp): isl_count > 0 selects it.  Island i: bodies isl_bodies[isl_body_off[i] .. [i+1]), manifold slots of
-    // colour c isl_mslots[isl_m_off[i*25+c] .. [i*25+c+1]), joint slots of level l isl_jslots[isl_j_off[i*(L+1)+l] .. [+1])
-    int isl_count, isl_levels;
-    const int* isl_body_off; const int* isl_bodies; const int* isl_m_off; const int* isl_mslots; const int* isl_j_off; const int* isl_jslots;
     // launch range (avn_solver_run_range): which parts of the step this launch runs.  A plain avn_solver_run does everything.
     int do_prepare, sub_begin, sub_end, do_restitution, do_finalize;
     // x-slab partition (multi-GPU, include/avian_b200.h "boundary bodies"): bnd_of[b] = index into the boundary list or -1 (NULL when
@@ -183,19 +174,6 @@ __device__ void prepare_body_item(const DevSolver<S>& d, int i) {
         bool iso = !(avn_abs(il.m00 - il.m11) > eps || avn_abs(il.m11 - il.m22) > eps) && avn_abs(il.m01) < eps &&
                    avn_abs(il.m02) < eps && avn_abs(il.m12) < eps;
         if (!rot_locked && !iso) flags |= BF_GYRO;
-        const bool clamped = (d.max_lin && avn_finite(d.max_lin[i])) || (d.max_ang && avn_finite(d.max_ang[i]));
-        // (fusing even the 12-flop velocity step into the contact item lengthens the contact item, whose own latency is the critical
-        //  resource, by more than the dependency level it saves; kept behind AVN_FUSE_IV for reference)
-#ifdef AVN_FUSE_IV
-        if (kind == AVN_BODY_DYNAMIC && !(flags & (BF_CUSTOM_VEL | BF_GYRO)) && !clamped) flags |= BF_FUSE_IV;
-#else
-        (void)clamped;
-#endif
-        // (fusing integrate_positions the same way is off as well: its double-precision sincos diverges the
-        //  warps of every late colour of the solve pass instead of costing one cheap level; kept behind AVN_FUSE_IP for reference)
-#ifdef AVN_FUSE_IP
-        if (!(flags & BF_CUSTOM_POS)) flags |= BF_FUSE_IP;
-#endif
         ia = mk4<S>(inv_mass, int_as(S(0), flags), iw.m00, iw.m01);
         ib = mk4<S>(iw.m02, iw.m11, iw.m12, iw.m22);
     }
@@ -397,12 +375,10 @@ __device__ __forceinline__ void wave_wait(const unsigned* ver, bool need1, int b
         if (spins > (1u << 22)) { *watchdog = 1; break; }
     }
 }
-// n1 / n2 = events this item consumed on each body (2 when it also ran the body's integrate step)
-__device__ __forceinline__ void wave_publish(unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2, unsigned n1 = 1u,
-                                             unsigned n2 = 1u) {
+__device__ __forceinline__ void wave_publish(unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2) {
     fence_acq_rel();  // release: this item's stores are visible before the counters move
-    if (need1) st_relaxed(ver + b1, e1 + n1);
-    if (need2) st_relaxed(ver + b2, e2 + n2);
+    if (need1) st_relaxed(ver + b1, e1 + 1u);
+    if (need2) st_relaxed(ver + b2, e2 + 1u);
 }
 
 // ---- shared-memory staging of the immutable per-point constraint rows -------------------------------------------------
@@ -428,7 +404,7 @@ template <class S> __host__ __device__ constexpr size_t stage_bytes(int threads,
     return size_t(4 * max_points + 1) * threads * sizeof(Vec4<S>);
 }
 
-// Barrier schedules (grid-wide phases, island groups, phase kernels); the wavefront schedule runs wave_contact_item below.
+// Barrier schedules (grid-wide phases, phase kernels); the wavefront schedule runs wave_contact_item below.
 // `slot` indexes the padded colour-major planes (a padding slot returns at once).
 // MAXP: compile-time bound on the points of a manifold (1 for sphere-only scenes: a quarter of the registers and no dead unrolled code)
 template <class S, int PASS, int MAXP = AVN_MAX_MANIFOLD_POINTS>
@@ -617,16 +593,16 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot) {
 //     computes every point's separation.  Stage 2 waits for the exact event and loads the velocities and impulses.  The two quaternion
 //     rotations per point are off the dependent chain.
 //   * Acquire / release counters (wave_wait / wave_publish): no membar after a successful poll, one fence before the counter stores.
-// PASS = PASS_WARM or PASS_SOLVE_BIAS.  Every lane of the warp must call this (warp-collective waits); an inactive lane of a partial chunk
-// behaves like a padding slot.  Counters count from the prepare launch on, so `s` is the absolute substep index in every launch of a step.
+// PASS = PASS_WARM or PASS_SOLVE_BIAS.  Every lane of the warp must call this (warp-collective waits).  Counters count from the prepare
+// launch on, so `s` is the absolute substep index in every launch of a step.
 template <class S, int PASS, int MAXP>
-__device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slot, int s, int it, bool lane_active, bool relax) {
+__device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slot, int s, int it, bool relax) {
     constexpr bool SOLVE = PASS == PASS_SOLVE_BIAS;
     relax = SOLVE && relax;
     const size_t MP = size_t(d.Mpad);
-    const Vec4<S>* c = d.cst + (lane_active ? slot : 0);
+    const Vec4<S>* c = d.cst + slot;
     const Vec4<S> hidx = ld4(&c[CP_IDX * MP]);
-    const int info = lane_active ? as_int(hidx.z) : 0;
+    const int info = as_int(hidx.z);
     const int np = info & CI_NP_MASK;
     const int b1 = as_int(hidx.x), b2 = as_int(hidx.y);
     Vec4<S>* const stage = stage_base<S>() + threadIdx.x;   // this thread's column; row r at stage[r * T]
@@ -659,21 +635,6 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
     const int kind = SOLVE ? (relax ? WV_RELAX : WV_SOLVE) : WV_WARM;
     const unsigned e1 = wave_event(kind, it, s, d.iters, k1, rk & 0xff);
     const unsigned e2 = wave_event(kind, it, s, d.iters, k2, (rk >> 16) & 0xff);
-    // fused integrate steps (experiments, off by default: prepare_body_item): the last relax event of a body also runs its next
-    // integrate_velocities, the last biased-solve event its integrate_positions
-#ifdef AVN_FUSE_IV
-    const bool fiv1 = relax && (info & CI_FIV1) && s + 1 < d.substeps, fiv2 = relax && (info & CI_FIV2) && s + 1 < d.substeps;
-#else
-    constexpr bool fiv1 = false, fiv2 = false;
-#endif
-#ifdef AVN_FUSE_IP
-    const bool fip1 = SOLVE && !relax && (info & CI_FIP1) && it + 1 == d.iters, fip2 = SOLVE && !relax && (info & CI_FIP2) && it + 1 == d.iters;
-#else
-    constexpr bool fip1 = false, fip2 = false;
-#endif
-    Vec4<S> il1, ia1, il2, ia2;   // VelocityIntegrationData rows (immutable): fetched before the wait
-    if (fiv1) { il1 = ld4(&d.itg[2 * b1]); ia1 = ld4(&d.itg[2 * b1 + 1]); }
-    if (fiv2) { il2 = ld4(&d.itg[2 * b2]); ia2 = ld4(&d.itg[2 * b2 + 1]); }
     int* const watchdog = d.any_restitution + FLAG_WAVE;
     const V3<S> n = xyz(hn), t1 = xyz(ht1);
 
@@ -709,7 +670,7 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
     AVN_TRACE_T(t_w0);
     wave_wait(d.ver, ver1, b1, e1, ver2, b2, e2, watchdog);
     AVN_TRACE_ADD(d, 0, clock64() - t_w0);
-    if (np == 0) return;   // padding slot / inactive lane (after the warp-collective waits)
+    if (np == 0) return;   // padding slot (after the warp-collective waits)
     AVN_TRACE_T(t_l0);
     const Vec4<S> l1 = ld4_cg(&d.vel[2 * b1]), a1 = ld4_cg(&d.vel[2 * b1 + 1]);
     const Vec4<S> l2 = ld4_cg(&d.vel[2 * b2]), a2 = ld4_cg(&d.vel[2 * b2 + 1]);
@@ -817,36 +778,15 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
 #pragma unroll 1
         for (int k = 0; k < np; ++k) pc_store(pc_ptr(d, k, slot), ROW_PC(k));
     }
-    // integrate_positions of a body whose last biased-solve event this is (integrator/mod.rs:503-535): dp += v h, dq = exp(w h) dq.  Its
-    // deltas are the ones stage 1 read (nothing else writes them before this item publishes).
-    if (fip1) {
-        const Vec4<S> dp = ld4_cg(&d.dlt[2 * b1]), dq4 = ld4_cg(&d.dlt[2 * b1 + 1]);
-        V3<S> ndp = xyz(dp) + v1 * d.h;
-        Q4<S> q; q.x = dq4.x; q.y = dq4.y; q.z = dq4.z; q.w = dq4.w;
-        Q4<S> nq = qmul(q_from_scaled_axis(w1 * d.h, d.fast_trig != 0), q);
-        st4(&d.dlt[2 * b1], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
-        st4(&d.dlt[2 * b1 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
-    }
-    if (fip2) {
-        const Vec4<S> dp = ld4_cg(&d.dlt[2 * b2]), dq4 = ld4_cg(&d.dlt[2 * b2 + 1]);
-        V3<S> ndp = xyz(dp) + v2 * d.h;
-        Q4<S> q; q.x = dq4.x; q.y = dq4.y; q.z = dq4.z; q.w = dq4.w;
-        Q4<S> nq = qmul(q_from_scaled_axis(w2 * d.h, d.fast_trig != 0), q);
-        st4(&d.dlt[2 * b2], mk4<S>(ndp.x, ndp.y, ndp.z, S(0)));
-        st4(&d.dlt[2 * b2 + 1], mk4<S>(nq.x, nq.y, nq.z, nq.w));
-    }
-    // integrate_velocities of the NEXT substep for a body whose last relax event this is (integrator/mod.rs:362-368)
-    if (fiv1) { v1 = v1 * il1.w; w1 = w1 * ia1.w; v1 = v1 + xyz(il1); w1 = w1 + xyz(ia1); }
-    if (fiv2) { v2 = v2 * il2.w; w2 = w2 * ia2.w; v2 = v2 + xyz(il2); w2 = w2 + xyz(ia2); }
-    if (!(info & CI_ZERO1) || fiv1) {
+    if (!(info & CI_ZERO1)) {
         st4(&d.vel[2 * b1], mk4<S>(v1.x, v1.y, v1.z, S(0)));
         st4(&d.vel[2 * b1 + 1], mk4<S>(w1.x, w1.y, w1.z, S(0)));
     }
-    if (!(info & CI_ZERO2) || fiv2) {
+    if (!(info & CI_ZERO2)) {
         st4(&d.vel[2 * b2], mk4<S>(v2.x, v2.y, v2.z, S(0)));
         st4(&d.vel[2 * b2 + 1], mk4<S>(w2.x, w2.y, w2.z, S(0)));
     }
-    wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2, (fiv1 || fip1) ? 2u : 1u, (fiv2 || fip2) ? 2u : 1u);
+    wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2);
 #ifdef AVN_WAVE_TRACE
     AVN_TRACE_ADD(d, 3, clock64() - t_s0);
     AVN_TRACE_ADD(d, 4, 1);
@@ -862,13 +802,11 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
 // ---------------------------------------------------------------------------------------------------------
 // WAVE: every lane of the warp calls this (i may be >= B: padding); `s` = substep index
 template <class S, bool WAVE = false>
-__device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, int i, int s = 0, bool lane_active = true) {
-    const bool in_range = lane_active && i < d.B;
+__device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, int i, int s = 0) {
+    const bool in_range = i < d.B;
     int f = 0;
     if (in_range) f = as_int(ld4(&d.inr[2 * i]).y);
-    bool live = in_range && (f & BF_HAS_SOLVER_BODY);
-    // wavefront mode: from the second substep on, a fusable body's step was already run by its last relax item
-    if (WAVE && live && (f & BF_FUSE_IV) && s >= 1 && d.deg[i] > 0) live = false;
+    const bool live = in_range && (f & BF_HAS_SOLVER_BODY);
     unsigned e = 0;
     if (WAVE) {
         if (live) e = wave_event(WV_IV, 0, s, d.iters, d.deg[i], 0);
@@ -932,12 +870,11 @@ __device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, i
 
 // integrate_positions (integrator/mod.rs:503-535)
 template <class S, bool WAVE = false>
-__device__ __forceinline__ void integrate_position_item(const DevSolver<S>& d, int i, int s = 0, bool lane_active = true) {
-    const bool in_range = lane_active && i < d.B;
+__device__ __forceinline__ void integrate_position_item(const DevSolver<S>& d, int i, int s = 0) {
+    const bool in_range = i < d.B;
     int f = 0;
     if (in_range) f = as_int(ld4(&d.inr[2 * i]).y);
-    bool live = in_range && (f & BF_HAS_SOLVER_BODY);
-    if (WAVE && live && (f & BF_FUSE_IP) && d.deg[i] > 0) live = false;   // run by the body's last biased-solve item
+    const bool live = in_range && (f & BF_HAS_SOLVER_BODY);
     unsigned e = 0;
     if (WAVE) {
         if (live) e = wave_event(WV_IP, 0, s, d.iters, d.deg[i], 0);
@@ -991,18 +928,9 @@ __device__ __forceinline__ void wave_pack_item(const DevSolver<S>& d, int slot) 
     const int info = as_int(hidx.z);
     if ((info & CI_NP_MASK) == 0) return;
     const int b1 = as_int(hidx.x), b2 = as_int(hidx.y);
-    int rk = as_int(hidx.w), ninfo = info;
-    if (info & CI_VER1) {
-        const int k1 = d.deg[b1], f1 = as_int(ld4(&d.inr[2 * b1]).y);
-        rk |= (k1 & 0xff) << 8;
-        if ((rk & 0xff) == k1 - 1) ninfo |= ((f1 & BF_FUSE_IV) ? CI_FIV1 : 0) | ((f1 & BF_FUSE_IP) ? CI_FIP1 : 0);
-    }
-    if (info & CI_VER2) {
-        const int k2 = d.deg[b2], f2 = as_int(ld4(&d.inr[2 * b2]).y);
-        rk |= (k2 & 0xff) << 24;
-        if (((rk >> 16) & 0xff) == k2 - 1) ninfo |= ((f2 & BF_FUSE_IV) ? CI_FIV2 : 0) | ((f2 & BF_FUSE_IP) ? CI_FIP2 : 0);
-    }
-    hidx.z = int_as(S(0), ninfo);
+    int rk = as_int(hidx.w);
+    if (info & CI_VER1) rk |= (d.deg[b1] & 0xff) << 8;
+    if (info & CI_VER2) rk |= (d.deg[b2] & 0xff) << 24;
     hidx.w = int_as(S(0), rk);
     st4(&c[CP_IDX * MP], hidx);
 }

@@ -7,7 +7,6 @@
 
 #include "context.hpp"
 #include "joint_schedule.hpp"
-#include "island_lists.hpp"
 #include "solver_kernels.cuh"
 
 namespace avn {
@@ -56,10 +55,8 @@ class Solver final : public SolverBase {
         // state is twice as wide).  AVN_MEGA_BPS = 2|3|4 overrides the default for experiments.
         const char* bps = getenv("AVN_MEGA_BPS");
         mega_bps_ = bps ? atoi(bps) : (sizeof(S) == 8 ? 2 : 3);
-        if (mega_bps_ < 2 || mega_bps_ > 6) mega_bps_ = 3;
+        if (mega_bps_ < 2 || mega_bps_ > 4) mega_bps_ = 3;
         if (mode && !strcmp(mode, "wave")) force_wave_ = true;
-        if (const char* w = getenv("AVN_ISLAND_MODE")) island_mode_ = atoi(w) != 0;
-        if (const char* w = getenv("AVN_WAVE_SM_ORDER")) sm_order_ = atoi(w) != 0;
         coop_ok_ = coop_ok_ && select_megakernel(AVN_MAX_MANIFOLD_POINTS);
         for (auto& e : ev_) cudaEventCreate(&e);
         up_stream_ = stream_;
@@ -206,10 +203,6 @@ class Solver final : public SolverBase {
         switch (bps) {
             case 2: return (const void*)step_megakernel<S, 2, MAXP>;
             case 4: return (const void*)step_megakernel<S, 4, MAXP>;
-#ifdef AVN_EXPERIMENT_BPS56   // experiment: 5 / 6 blocks per SM (102 / 85 registers: the wavefront routines spill)
-            case 5: return (const void*)step_megakernel<S, 5, MAXP>;
-            case 6: return (const void*)step_megakernel<S, 6, MAXP>;
-#endif
             default: return (const void*)step_megakernel<S, 3, MAXP>;
         }
     }
@@ -281,14 +274,7 @@ class Solver final : public SolverBase {
     DevBuf o_pos_, o_rot_, o_lv_, o_av_;
     DevBuf s_inr_, s_itg_, s_pre_;
     DevBuf m_b1_, m_b2_, m_n_, m_f_, m_r_, m_tv_, m_po_, p_a1_, p_a2_, p_pen_, p_ns_, p_wn_, p_wt_, p_ni_, p_nin_, p_own_, p_owt_;
-    DevBuf hot_, c_flag_, isl_buf_, sm_slots_;
-    bool sm_order_ = false;
-    IslandLists isl_;
-    std::vector<int> isl_jb1_, isl_jb2_;
-    // island-group schedule (solver_kernels.cuh island_substep_loop): bit-identical, but slower than the barrier schedule on the scene it
-    // was built for (5 000 ragdolls) when it was introduced — every block is in a different phase, so the SM's
-    // instruction stream thrashes, and an island's few joints per level keep one warp busy.  Off by default; AVN_ISLAND_MODE=1 enables it.
-    bool island_mode_ = false;
+    DevBuf hot_, c_flag_;
     size_t hot_bytes_ = 0;
     DevBuf j_type_, j_index_, j_level_, j_planes_;
     DevBuf jcol_[AVN_JOINT_TYPE_COUNT][12], jb1_[AVN_JOINT_TYPE_COUNT], jb2_[AVN_JOINT_TYPE_COUNT], jle_[AVN_JOINT_TYPE_COUNT],
@@ -665,39 +651,6 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
         }
     }
 #undef UP
-    // ---- island-group schedule for jointed scenes made of many small islands (island_lists.hpp); needs the constraint bodies on the host
-    d.isl_count = 0;
-    if (island_mode_ && have_j_ && (!have_m_ || (!mc->device_list && !mc->reuse_graph && mc->body1 && mc->body2))) {
-        const int J = d.J;
-        isl_jb1_.resize(J); isl_jb2_.resize(J);
-        for (int sl = 0; sl < J; ++sl) {
-            const AvnJointColumns& jc = js->types[h_type_[sl]];
-            isl_jb1_[sl] = jc.body1[h_index_[sl]];
-            isl_jb2_[sl] = jc.body2[h_index_[sl]];
-        }
-        int zero_off[AVN_GRAPH_COLOR_COUNT + 1] = {};
-        build_island_lists(int(B), bc->kind, have_m_ ? d.M : 0, have_m_ ? mc->body1 : nullptr, have_m_ ? mc->body2 : nullptr, have_m_ ? d.m_color_off : zero_off,
-                           have_m_ ? d.color_off : zero_off, J, isl_jb1_.data(), isl_jb2_.data(), h_level_off_.data(), d.n_levels, 3 * sm_count_, isl_);
-        // worth it when there are enough islands to fill the warps and none is big enough to make one warp the critical path
-        if (isl_.ok && isl_.islands >= 2 * sm_count_ && isl_.max_bodies <= 128) {
-            const size_t n_body_off = isl_.body_off.size(), n_bodies = isl_.bodies.size(), n_m_off = isl_.m_off.size(), n_ms = isl_.mslots.size(),
-                         n_j_off = isl_.j_off.size(), n_js = isl_.jslots.size();
-            const size_t total = n_body_off + n_bodies + n_m_off + n_ms + n_j_off + n_js;
-            AVN_CUDA(isl_buf_.ensure(total * sizeof(int) + 64));
-            int* p = isl_buf_.as<int>();
-            auto put = [&](const std::vector<int>& v, const int** dst) -> cudaError_t {
-                *dst = p;
-                cudaError_t e = v.empty() ? cudaSuccess : cudaMemcpyAsync(p, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, stream_);
-                p += v.size();
-                return e;
-            };
-            AVN_CUDA(put(isl_.body_off, &d.isl_body_off)); AVN_CUDA(put(isl_.bodies, &d.isl_bodies)); AVN_CUDA(put(isl_.m_off, &d.isl_m_off));
-            AVN_CUDA(put(isl_.mslots, &d.isl_mslots)); AVN_CUDA(put(isl_.j_off, &d.isl_j_off)); AVN_CUDA(put(isl_.jslots, &d.isl_jslots));
-            AVN_CUDA(cudaStreamSynchronize(stream_));   // the lists are pageable host vectors that the next upload rebuilds
-            d.isl_count = isl_.count;
-            d.isl_levels = isl_.levels;
-        }
-    }
     cudaEventRecord(ev_[EV_H2D1], stream_);
     uploaded_ = true;
     prepared_ = false;
@@ -744,16 +697,6 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
         for (int c = 0; c < AVN_COLOR_OVERFLOW; ++c) widest_colour = std::max(widest_colour, dev_.color_len[c]);
         const bool chain_bound = force_wave_ || widest_colour <= 2 * mega_grid_ * MEGA_BLOCK;
         dev_.wave = (mega && use_wave_ && chain_bound && dev_.M > 0 && dev_.J == 0 && dev_.color_len[AVN_COLOR_OVERFLOW] == 0) ? 1 : 0;
-        {
-            dev_.sm_slots = nullptr;
-            if (sm_order_ && mega_grid_ == step_bps_ * sm_count_) {
-                if (!sm_slots_.p) {
-                    AVN_CUDA(sm_slots_.ensure(1024 * sizeof(int)));
-                    AVN_CUDA(cudaMemsetAsync(sm_slots_.p, 0, 1024 * sizeof(int), stream_));
-                }
-                dev_.sm_slots = sm_slots_.as<int>();
-            }
-        }
         if (dev_.M > 0) {
             // padding slots must read as "no points": clear the index plane before prepare fills the live slots
             AVN_CUDA(cudaMemsetAsync(dev_.cst + size_t(CP_IDX) * dev_.Mpad, 0, size_t(dev_.Mpad) * sizeof(Vec4<S>), stream_));
@@ -766,17 +709,7 @@ AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
     } else {
         mega = mega && mega_step_;   // a step keeps the launch mode its prepare launch chose
     }
-    if (l2_persist_ && dev_.isl_count > 0) {
-        // island-per-warp schedule: the state of an island lives in its SM's L1; no L2 window (an access-policy window turns
-        // the island loop's L1 hits into L2 round trips)
-        cudaStreamAttrValue attr{};
-        attr.accessPolicyWindow.base_ptr = nullptr;
-        attr.accessPolicyWindow.num_bytes = 0;
-        attr.accessPolicyWindow.hitRatio = 0.f;
-        attr.accessPolicyWindow.hitProp = cudaAccessPropertyNormal;
-        attr.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
-        cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &attr);
-    } else if (l2_persist_ && hot_bytes_ > 0) {
+    if (l2_persist_ && hot_bytes_ > 0) {
         // pin the mutable state (body velocities/deltas, event counters, impulse planes) in L2: it sits on the critical dependency
         // chain, while the immutable constraint rows only stream through
         cudaStreamAttrValue attr{};
@@ -1097,7 +1030,7 @@ AvnStatus Solver<S>::download() {
     uint32_t ac = 0;
     for (int c = 0; c < AVN_GRAPH_COLOR_COUNT; ++c) ac += dev_.color_len[c] > 0;
     tm_.active_colors = ac;
-    tm_.launch_mode = !mega_step_ ? AVN_LAUNCH_PHASES : (dev_.wave ? AVN_LAUNCH_MEGA_WAVE : (dev_.isl_count > 0 ? AVN_LAUNCH_MEGA_ISLANDS : AVN_LAUNCH_MEGA_BARRIER));
+    tm_.launch_mode = !mega_step_ ? AVN_LAUNCH_PHASES : (dev_.wave ? AVN_LAUNCH_MEGA_WAVE : AVN_LAUNCH_MEGA_BARRIER);
     return AVN_OK;
 }
 

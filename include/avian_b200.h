@@ -268,7 +268,6 @@ typedef struct AvnTimings {
 #define AVN_LAUNCH_PHASES 0u        /* one kernel launch per phase (~500 per step) */
 #define AVN_LAUNCH_MEGA_BARRIER 1u  /* one persistent cooperative kernel, grid barriers between colours */
 #define AVN_LAUNCH_MEGA_WAVE 2u     /* one persistent cooperative kernel, per-body event counters instead of barriers */
-#define AVN_LAUNCH_MEGA_ISLANDS 3u  /* one persistent cooperative kernel, one warp per simulation island through the whole substep loop (many small islands) */
 
 /* lifecycle ------------------------------------------------------------------------------------------- */
 AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx);

@@ -19,7 +19,6 @@ hist() { grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed -E 's/^\s+\/\*[0-9a-f]+\*\/\s+(@
   echo "#   MEMBAR.SC.GPU                                          __threadfence() (grid barriers); none in the wavefront routines"
   echo "#   LDL / STL                                              local memory (spills); none in the f32 wavefront routines"
   echo "#   LDGSTS.E.BYPASS.128                                    cp.async staging of the constraint rows into shared memory"
-  echo "#   CCTL.E.PF2                                             prefetch.global.L2 of the next chunk's rows"
   for f in solver_host broadphase contacts narrow aabb; do
     echo "== $f.cu: memory / synchronisation opcodes"
     nvdisasm -c $f.sm_90a.cubin 2>/dev/null | hist | grep -E "LDG|STG|LDGSTS|MEMBAR|CCTL|LDS|STS|ATOM|RED|BAR|ERRBAR|LDL|STL|UBLKCP|UTMA|SYNCS|MATCH|VOTE|SHFL" || true

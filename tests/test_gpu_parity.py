@@ -158,12 +158,12 @@ def test_launch_modes_agree(gpu_ctx, iters):
     bw, mw, tw = _run_in_mode("", prm, b, m)
     bb, mb, tb = _run_in_mode("barrier", prm, b, m)
     bp, mp, tp = _run_in_mode("phases", prm, b, m)
-    bs, ms, ts = _run_in_mode("", prm, b, m, env={"AVN_WARM_BY_BODY": "1"})   # wavefront schedule with the body-centric warm start (experiment)
+    bs, ms, ts = _run_in_mode("", prm, b, m)   # the wavefront schedule again: run-to-run deterministic
     assert tw["kernel_launches"] == 1 and tb["kernel_launches"] == 1, "megakernel paths are ONE launch per step"
     assert tw["launch_mode"] == ts["launch_mode"] == 2   # AVN_LAUNCH_MEGA_WAVE
     assert tp["kernel_launches"] > 10
     assert np.array_equal(mw.normal_impulse, ms.normal_impulse) and np.array_equal(mw.warm_start_tangent_impulse, ms.warm_start_tangent_impulse)
-    for other, what in ((bb, "barrier"), (bp, "phases"), (bs, "body-centric warm start")):
+    for other, what in ((bb, "barrier"), (bp, "phases"), (bs, "wavefront rerun")):
         for name in ("position", "rotation", "linear_velocity", "angular_velocity"):
             assert np.array_equal(getattr(bw, name), getattr(other, name)), (what, name)
     assert np.array_equal(mw.warm_start_normal_impulse, mb.warm_start_normal_impulse)
@@ -174,9 +174,9 @@ def test_launch_modes_agree(gpu_ctx, iters):
     assert_bodies_close(bw, bo, what=f"iters={iters}: ")
 
 
-def test_body_centric_warm_start_with_many_contacts(gpu_ctx):
-    """a body with more contact points than the warp's slice of the staging tile holds (32): the body-centric warm start computes the
-    rest on the spot; a wide plate resting on a 4 x 4 field of cubes carries 16 manifolds x 4 points.  Bit-identical to the barrier schedule."""
+def test_wavefront_equals_barrier_with_16_manifolds_on_one_body(gpu_ctx):
+    """a wide plate resting on a 4 x 4 field of cubes carries 16 manifolds x 4 points: 16 events of the plate per pass, each one waiting for
+    the previous.  The wavefront schedule is bit-identical to the barrier schedule."""
     cubes = np.array([[1.5 * ix, 0.49, 1.5 * iz] for ix in range(4) for iz in range(4)])
     pos = np.concatenate([[[2.25, -0.5, 2.25]], cubes, [[2.25, 1.22, 2.25]]])
     he = np.concatenate([[[20.0, 0.5, 20.0]], np.full((16, 3), 0.5), [[3.5, 0.25, 3.5]]])
@@ -186,7 +186,7 @@ def test_body_centric_warm_start_with_many_contacts(gpu_ctx):
     _, (prm, b, m, j) = advance_to_solver_input(sc, steps=3, substeps=4)
     per_body = np.bincount(np.concatenate([m.body1[m.body1 >= 0], m.body2[m.body2 >= 0]]), minlength=b.count)
     assert per_body.max() >= 16 and m.color_offsets[api.COLOR_OVERFLOW + 1] == m.color_offsets[api.COLOR_OVERFLOW], (per_body.max(), m.color_offsets)
-    bw, mw, tw = _run_in_mode("wave", prm, b, m, env={"AVN_WARM_BY_BODY": "1"})
+    bw, mw, tw = _run_in_mode("wave", prm, b, m)
     bb, mb, _ = _run_in_mode("barrier", prm, b, m)
     assert tw["launch_mode"] == 2   # AVN_LAUNCH_MEGA_WAVE
     for name in ("position", "rotation", "linear_velocity", "angular_velocity"):
@@ -215,36 +215,6 @@ def test_prefetched_body_columns(gpu_ctx):
         ctx.solver_prefetch_bodies(other)                            # not the columns the upload is given
         ctx.solver_step(prm, b3, m3)
         assert np.array_equal(b3.position, ref_b.position) and np.array_equal(m3.normal_impulse, ref_m.normal_impulse)
-
-
-def test_island_per_warp_schedule_is_bit_identical(gpu_ctx):
-    """a field of ragdolls = many small islands: one thread block takes a group of islands through the whole substep loop
-    (AVN_LAUNCH_MEGA_ISLANDS); same per-item routines in the same per-body order as the barrier schedule, so bit-identical bodies, impulses
-    and joint forces; and equal to the oracle."""
-    w, (prm, b, m, j) = advance_to_solver_input(scenes.ragdoll_field(320, pitch=1.6, drop_height=0.1), steps=25, substeps=4)
-    assert m is not None and m.count > 50 and j.count == 320 * 16, (None if m is None else m.count, j.count)
-    def run(env):
-        os.environ.update(env)
-        try:
-            with api.Context(device=0) as ctx:
-                bb, mm, jj = b.copy(), m.copy(), j.copy()
-                ctx.solver_step(prm, bb, mm, jj)
-                return bb, mm, jj, ctx.timings()
-        finally:
-            for k in env:
-                os.environ.pop(k, None)
-    bi, mi, ji, ti = run({"AVN_ISLAND_MODE": "1"})     # (an experiment: slower than the barrier schedule, off by default)
-    bb, mb, jb, tb = run({})
-    assert ti["launch_mode"] == 3 and tb["launch_mode"] == 1 and ti["kernel_launches"] == 1   # AVN_LAUNCH_MEGA_ISLANDS / _BARRIER
-    for name in ("position", "rotation", "linear_velocity", "angular_velocity"):
-        assert np.array_equal(getattr(bi, name), getattr(bb, name)), name
-    assert np.array_equal(mi.warm_start_normal_impulse, mb.warm_start_normal_impulse) and np.array_equal(mi.normal_impulse, mb.normal_impulse)
-    for t, jt in ji.types.items():
-        if jt.count and jt.force is not None:
-            assert np.array_equal(jt.force, jb.types[t].force) and np.array_equal(jt.torque, jb.types[t].torque)
-    bo, mo, jo = b.copy(), m.copy(), j.copy()
-    oracle_lib.solver_step(prm, bo, mo, jo)
-    assert_bodies_close(bi, bo, what="island schedule vs oracle: ")
 
 
 def test_wavefront_equals_barrier_at_headline_size(gpu_ctx):
