@@ -377,8 +377,33 @@ class AvnHitList(C.Structure):
     _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [(n, _vp) for n in ("offsets", "collider", "distance", "normal")]
 
 
+class AvnShapeBatch(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("exclude_count", C.c_uint32)] + [
+        (n, _vp) for n in ("shape", "dims", "position", "rotation", "direction", "max_distance", "target_distance", "flags", "max_hits", "mask",
+                           "exclude_offsets", "exclude")]
+
+
+class AvnPointBatch(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("exclude_count", C.c_uint32)] + [(n, _vp) for n in ("point", "solid", "mask", "exclude_offsets", "exclude")]
+
+
+class AvnShapeClosest(C.Structure):
+    _fields_ = [(n, _vp) for n in ("collider", "distance", "point1", "point2", "normal1", "normal2")]
+
+
+class AvnShapeHitList(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [
+        (n, _vp) for n in ("offsets", "collider", "distance", "point1", "point2", "normal1", "normal2")]
+
+
+class AvnPointProjection(C.Structure):
+    _fields_ = [(n, _vp) for n in ("collider", "point", "is_inside")]
+
+
 QUERY_SHAPES_UNCHANGED = 1
 MAX_HITS_ALL = 0xFFFFFFFF
+CAST_IGNORE_ORIGIN_PENETRATION = 0x1
+CAST_NO_CONTACT_ON_PENETRATION = 0x2
 
 
 def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
@@ -434,6 +459,11 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "query_cast_ray": ([_vp, P(AvnRayBatch), P(AvnRayClosest)], C.c_int),
         "query_ray_hits": ([_vp, P(AvnRayBatch), P(AvnHitList)], C.c_int),
         "query_aabb_intersections": ([_vp, C.c_uint32, _vp, _vp, P(AvnHitList)], C.c_int),
+        "query_cast_shape": ([_vp, P(AvnShapeBatch), P(AvnShapeClosest)], C.c_int),
+        "query_shape_hits": ([_vp, P(AvnShapeBatch), P(AvnShapeHitList)], C.c_int),
+        "query_project_point": ([_vp, P(AvnPointBatch), P(AvnPointProjection)], C.c_int),
+        "query_point_intersections": ([_vp, P(AvnPointBatch), P(AvnHitList)], C.c_int),
+        "query_shape_intersections": ([_vp, P(AvnShapeBatch), P(AvnHitList)], C.c_int),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(lib, f"{prefix}_{name}")
@@ -450,7 +480,8 @@ ABI_SYMBOLS = [
     "avn_contacts_reserve", "avn_contacts_add", "avn_contacts_remove", "avn_contacts_narrow_phase", "avn_contacts_download_impulses",
     "avn_contacts_configure", "avn_contacts_step", "avn_solver_upload_resident", "avn_broadphase_download_order", "avn_contacts_download_graph",
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
-    "avn_query_aabb_intersections"]
+    "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
+    "avn_query_shape_intersections"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -536,6 +567,100 @@ class Rays:
             st.exclude_offsets = xoff.ctypes.data
             st.exclude = xs.ctypes.data if xs.size else None
         return st, keep
+
+
+def _exclusion_csr(exclude, n: int):
+    """per query an iterable of excluded collider indices -> (offsets[n+1], indices), or (None, None)"""
+    if exclude is None:
+        return None, None
+    lists = [np.asarray(list(e), dtype=np.uint32) for e in exclude]
+    xoff = np.zeros(n + 1, dtype=np.uint32)
+    xoff[1:] = np.cumsum([len(e) for e in lists])
+    xs = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, dtype=np.uint32), dtype=np.uint32)
+    return xoff, xs
+
+
+@dataclass
+class ShapeQueries:
+    """A batch of query shapes (AvnShapeBatch): cuboids / spheres with a pose, for shape casts (direction, max_distance, flags, max_hits)
+    and shape intersections (which ignore the cast columns).  exclude: per shape an iterable of collider indices it ignores, or None."""
+    shape: np.ndarray                        # uint8[n] SHAPE_CUBOID / SHAPE_SPHERE
+    dims: np.ndarray                         # [n,3] half extents / radius in [0]
+    position: np.ndarray                     # [n,3]
+    rotation: np.ndarray                     # [n,4] (x, y, z, w)
+    direction: np.ndarray | None = None      # [n,3] casts
+    max_distance: np.ndarray | None = None   # [n] casts
+    target_distance: np.ndarray | None = None   # [n] casts: must be 0 (None = 0)
+    flags: np.ndarray | None = None          # uint32[n] CAST_* (None = 0)
+    max_hits: np.ndarray | None = None       # uint32[n] shape_hits (None = all)
+    mask: np.ndarray | None = None           # uint32[n] (None = all layers)
+    exclude: list | None = None
+
+    @property
+    def count(self) -> int:
+        return int(np.asarray(self.position).reshape(-1, 3).shape[0])
+
+    def as_struct(self, scalar) -> tuple["AvnShapeBatch", list]:
+        dt, n = np.dtype(scalar), self.count
+        col = lambda a, w: None if a is None else np.ascontiguousarray(a, dtype=dt).reshape(-1, w)
+        per = lambda a: None if a is None else np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=dt), (n,)))
+        opt = lambda a, t: None if a is None else np.ascontiguousarray(a, dtype=t)
+        xoff, xs = _exclusion_csr(self.exclude, n)
+        keep = [opt(self.shape, np.uint8), col(self.dims, 3), col(self.position, 3), col(self.rotation, 4), col(self.direction, 3),
+                per(self.max_distance), per(self.target_distance), opt(self.flags, np.uint32), opt(self.max_hits, np.uint32),
+                opt(self.mask, np.uint32), xoff, xs]
+        st = AvnShapeBatch(n, 0 if xs is None else int(xs.shape[0]), *(_ptr(a) if a is None or a.size else None for a in keep))
+        if xoff is not None:
+            st.exclude_offsets = xoff.ctypes.data
+            st.exclude = xs.ctypes.data if xs.size else None
+        return st, keep
+
+
+@dataclass
+class Points:
+    """A batch of query points (AvnPointBatch).  solid: project_point only."""
+    point: np.ndarray                    # [n,3]
+    solid: np.ndarray | None = None      # bool/uint8[n] (None = all solid)
+    mask: np.ndarray | None = None       # uint32[n] (None = all layers)
+    exclude: list | None = None
+
+    @property
+    def count(self) -> int:
+        return int(np.asarray(self.point).reshape(-1, 3).shape[0])
+
+    def as_struct(self, scalar) -> tuple["AvnPointBatch", list]:
+        dt, n = np.dtype(scalar), self.count
+        opt = lambda a, t: None if a is None else np.ascontiguousarray(a, dtype=t)
+        xoff, xs = _exclusion_csr(self.exclude, n)
+        keep = [np.ascontiguousarray(self.point, dtype=dt).reshape(-1, 3), opt(self.solid, np.uint8), opt(self.mask, np.uint32), xoff, xs]
+        st = AvnPointBatch(n, 0 if xs is None else int(xs.shape[0]), *(_ptr(a) if a is None or a.size else None for a in keep))
+        if xoff is not None:
+            st.exclude_offsets = xoff.ctypes.data
+            st.exclude = xs.ctypes.data if xs.size else None
+        return st, keep
+
+
+SHAPE_HIT_FIELDS = ("point1", "point2", "normal1", "normal2")
+
+
+def shape_closest(n: int, scalar) -> tuple["AvnShapeClosest", dict]:
+    out = {"collider": np.zeros(n, dtype=np.int32), "distance": np.zeros(n, dtype=scalar)}
+    out.update({k: np.zeros((n, 3), dtype=scalar) for k in SHAPE_HIT_FIELDS})
+    return AvnShapeClosest(*(_ptr(out[k]) for k in ("collider", "distance") + SHAPE_HIT_FIELDS)), out
+
+
+def shape_hit_list(n: int, capacity: int, scalar) -> tuple["AvnShapeHitList", dict]:
+    """An AvnShapeHitList over fresh numpy arrays (offsets[n+1], collider, distance, point1, point2, normal1, normal2)."""
+    cap = max(int(capacity), 0)
+    m = max(cap, 1)
+    out = {"offsets": np.zeros(n + 1, dtype=np.uint64), "collider": np.zeros(m, dtype=np.uint32), "distance": np.zeros(m, dtype=scalar)}
+    out.update({k: np.zeros((m, 3), dtype=scalar) for k in SHAPE_HIT_FIELDS})
+    return AvnShapeHitList(cap, 0, *(_ptr(out[k]) for k in ("offsets", "collider", "distance") + SHAPE_HIT_FIELDS)), out
+
+
+def point_projection(n: int, scalar) -> tuple["AvnPointProjection", dict]:
+    out = {"collider": np.zeros(n, dtype=np.int32), "point": np.zeros((n, 3), dtype=scalar), "is_inside": np.zeros(n, dtype=np.uint8)}
+    return AvnPointProjection(*(_ptr(out[k]) for k in ("collider", "point", "is_inside"))), out
 
 
 def hit_list(n: int, capacity: int, scalar, ray: bool) -> tuple["AvnHitList", dict]:
@@ -981,5 +1106,55 @@ class Context:
         if st == ERR_CAPACITY and capacity is None:
             h, out = hit_list(n, int(h.count), self.scalar, False)
             st = self.lib.avn_query_aabb_intersections(self.handle, n, _ptr(mn), _ptr(mx), C.byref(h))
+        self._check_list(st, h)
+        return hit_list_result(h, out)
+
+    def cast_shape(self, shapes: "ShapeQueries") -> dict:
+        """avn_query_cast_shape: per query shape the closest hit — collider (-1 = none), distance, point1, point2, normal1, normal2."""
+        s, keep = shapes.as_struct(self.scalar)
+        o, out = shape_closest(shapes.count, self.scalar)
+        self._check(self.lib.avn_query_cast_shape(self.handle, C.byref(s), C.byref(o)))
+        return out
+
+    def shape_hits(self, shapes: "ShapeQueries", capacity: int | None = None) -> dict:
+        """avn_query_shape_hits: CSR offsets[n+1], collider, distance, point1, point2, normal1, normal2 (per shape its max_hits nearest).
+        capacity=None sizes the output from the required count; a capacity that is too small raises AvianError(ERR_CAPACITY) with .required."""
+        s, keep = shapes.as_struct(self.scalar)
+        h, out = shape_hit_list(shapes.count, 4 * shapes.count if capacity is None else capacity, self.scalar)
+        st = self.lib.avn_query_shape_hits(self.handle, C.byref(s), C.byref(h))
+        if st == ERR_CAPACITY and capacity is None:
+            h, out = shape_hit_list(shapes.count, int(h.count), self.scalar)
+            st = self.lib.avn_query_shape_hits(self.handle, C.byref(s), C.byref(h))
+        self._check_list(st, h)
+        return hit_list_result(h, out)
+
+    def project_point(self, points: "Points") -> dict:
+        """avn_query_project_point: per point the closest collider (-1 = none), the projection and is_inside."""
+        p, keep = points.as_struct(self.scalar)
+        o, out = point_projection(points.count, self.scalar)
+        self._check(self.lib.avn_query_project_point(self.handle, C.byref(p), C.byref(o)))
+        return out
+
+    def point_intersections(self, points: "Points", capacity: int | None = None) -> dict:
+        """avn_query_point_intersections: per point the colliders containing it (CSR offsets[n+1], collider ascending)."""
+        p, keep = points.as_struct(self.scalar)
+        n = points.count
+        h, out = hit_list(n, 4 * n if capacity is None else capacity, self.scalar, False)
+        st = self.lib.avn_query_point_intersections(self.handle, C.byref(p), C.byref(h))
+        if st == ERR_CAPACITY and capacity is None:
+            h, out = hit_list(n, int(h.count), self.scalar, False)
+            st = self.lib.avn_query_point_intersections(self.handle, C.byref(p), C.byref(h))
+        self._check_list(st, h)
+        return hit_list_result(h, out)
+
+    def shape_intersections(self, shapes: "ShapeQueries", capacity: int | None = None) -> dict:
+        """avn_query_shape_intersections: per query shape the colliders it intersects (CSR offsets[n+1], collider ascending)."""
+        s, keep = shapes.as_struct(self.scalar)
+        n = shapes.count
+        h, out = hit_list(n, 4 * n if capacity is None else capacity, self.scalar, False)
+        st = self.lib.avn_query_shape_intersections(self.handle, C.byref(s), C.byref(h))
+        if st == ERR_CAPACITY and capacity is None:
+            h, out = hit_list(n, int(h.count), self.scalar, False)
+            st = self.lib.avn_query_shape_intersections(self.handle, C.byref(s), C.byref(h))
         self._check_list(st, h)
         return hit_list_result(h, out)

@@ -297,6 +297,22 @@ AvnStatus avn_query_ray_hits(AvnContext* ctx, const AvnRayBatch* rays, AvnHitLis
 AvnStatus avn_query_aabb_intersections(AvnContext* ctx, uint32_t count, const void* min, const void* max, AvnHitList* out) {
     return guarded(ctx, [&] { return ctx->queries->aabb_intersections(count, min, max, out); });
 }
+// SpatialQueryPipeline::cast_shape / shape_hits / project_point / point_intersections / shape_intersections
+AvnStatus avn_query_cast_shape(AvnContext* ctx, const AvnShapeBatch* shapes, AvnShapeClosest* out) {
+    return guarded(ctx, [&] { return ctx->queries->cast_shape(shapes, out); });
+}
+AvnStatus avn_query_shape_hits(AvnContext* ctx, const AvnShapeBatch* shapes, AvnShapeHitList* out) {
+    return guarded(ctx, [&] { return ctx->queries->shape_hits(shapes, out); });
+}
+AvnStatus avn_query_project_point(AvnContext* ctx, const AvnPointBatch* points, AvnPointProjection* out) {
+    return guarded(ctx, [&] { return ctx->queries->project_point(points, out); });
+}
+AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* points, AvnHitList* out) {
+    return guarded(ctx, [&] { return ctx->queries->point_intersections(points, out); });
+}
+AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out) {
+    return guarded(ctx, [&] { return ctx->queries->shape_intersections(shapes, out); });
+}
 
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out) {
     if (!ctx || !out) return AVN_ERR_INVALID_ARGUMENT;

@@ -130,6 +130,11 @@ struct QueriesBase {
     virtual AvnStatus cast_ray(const AvnRayBatch* rays, AvnRayClosest* out) = 0;
     virtual AvnStatus ray_hits(const AvnRayBatch* rays, AvnHitList* out) = 0;
     virtual AvnStatus aabb_intersections(uint32_t count, const void* min, const void* max, AvnHitList* out) = 0;
+    virtual AvnStatus cast_shape(const AvnShapeBatch* shapes, AvnShapeClosest* out) = 0;
+    virtual AvnStatus shape_hits(const AvnShapeBatch* shapes, AvnShapeHitList* out) = 0;
+    virtual AvnStatus project_point(const AvnPointBatch* points, AvnPointProjection* out) = 0;
+    virtual AvnStatus point_intersections(const AvnPointBatch* points, AvnHitList* out) = 0;
+    virtual AvnStatus shape_intersections(const AvnShapeBatch* shapes, AvnHitList* out) = 0;
 };
 QueriesBase* make_queries(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 

@@ -15,6 +15,9 @@
 // Queries: one thread per query, a stack traversal that culls against the f32 bounds (double slab test clipped to [0, max_distance]) and
 // runs the exact test at the leaves.  cast_ray keeps the lexicographic minimum (t, collider); ray_hits and aabb_intersections use the broad
 // phase's count -> exclusive scan -> emit -> per-segment sort pattern into CSR lists.
+// Shape casts (pipeline.rs:335-554) cull against the node boxes grown by the cast shape's AABB half size, nearer child first for the closest
+// hit; project_point (570-615) prunes on the squared point-box distance; point and shape intersections (628-683, 744-826) use the same CSR
+// pattern.  Their geometry is the shape-cast part of query_math.hpp.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -399,6 +402,278 @@ __global__ void __launch_bounds__(Q_THREADS) q_aabb(const __grid_constant__ Tree
     sort_segment(w, [&](uint32_t x, uint32_t y) { return seg[x] < seg[y]; }, [&](uint32_t x, uint32_t y) { const uint32_t v = seg[x]; seg[x] = seg[y]; seg[y] = v; });
 }
 
+// ---- shape casts, point projection, point and shape intersections ----------------------------------------------------------------------
+template <class S>
+struct Shapes {
+    int n;
+    const uint8_t* shape; const S* dims; const S* pos; const S* rot; const S* d; const S* maxd;
+    const uint32_t* flags; const uint32_t* max_hits; const uint32_t* mask; const uint32_t* xoff; const uint32_t* xs;
+};
+template <class S>
+struct Points {
+    int n;
+    const S* p; const uint8_t* solid; const uint32_t* mask; const uint32_t* xoff; const uint32_t* xs;
+};
+
+// one query shape.  ext: the f32 half size of its tight AABB, rounded up plus one ulp (qm::culling_bounds of [-e, e]); lo / hi: its culling box
+struct ShapeIn {
+    int shape;
+    nm::V3 he, c, d;
+    nm::Q q;
+    double maxd;
+    uint32_t flags, mask, nx;
+    const uint32_t* xs;
+    float ext[3], lo[3], hi[3];
+    bool ok;
+};
+template <class S>
+__device__ __forceinline__ ShapeIn load_shape(const Shapes<S>& s, int i, bool cast) {
+    ShapeIn q;
+    q.shape = s.shape[i];
+    q.he = ld3(s.dims, i);
+    q.c = ld3(s.pos, i);
+    q.q = ldq(s.rot, i);
+    q.d = cast ? ld3(s.d, i) : nm::V3{0, 0, 0};
+    q.maxd = cast ? double(s.maxd[i]) : 0.0;
+    q.flags = cast && s.flags ? s.flags[i] : 0u;
+    q.mask = s.mask ? s.mask[i] : 0xffffffffu;
+    q.xs = s.xoff ? s.xs + s.xoff[i] : nullptr;
+    q.nx = s.xoff ? s.xoff[i + 1] - s.xoff[i] : 0u;
+    q.ok = cast ? qm::cast_finite(q.he, q.c, q.q, q.d, q.maxd) : qm::collider_valid(q.he, q.c, q.q);
+    if (q.ok) {
+        const nm::V3 e = qm::half_size(q.shape, q.he, qm::rot_mat(q.q));
+        for (int k = 0; k < 3; ++k) {
+            float l, h;
+            qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, h);
+            q.ext[k] = h;
+            qm::culling_bounds(nm::comp(q.c, k) - nm::comp(e, k), nm::comp(q.c, k) + nm::comp(e, k), q.lo[k], q.hi[k]);
+        }
+    }
+    return q;
+}
+
+// where the cast shape's centre enters a node box grown by the shape's half size, clipped to [0, tmax]; INFINITY when it never does.
+// The swept shape can touch a collider in the node only while its AABB overlaps the node box, i.e. while its centre is in the grown box.
+__device__ __forceinline__ double grown_entry(const NodeBox& b, const float* ext, nm::V3 o, nm::V3 d, double tmax) {
+    const float lo[3] = {b.lo.x, b.lo.y, b.lo.z}, hi[3] = {b.hi.x, b.hi.y, b.hi.z};
+    double t0 = 0, t1 = tmax;
+    for (int k = 0; k < 3; ++k) {
+        const double ok = nm::comp(o, k), dk = nm::comp(d, k), l = double(lo[k]) - double(ext[k]), h = double(hi[k]) + double(ext[k]);
+        if (dk == 0) {
+            if (ok < l || ok > h) return INFINITY;
+            continue;
+        }
+        double a = (l - ok) / dk, c = (h - ok) / dk;
+        if (a > c) { const double s = a; a = c; c = s; }
+        t0 = nm::smax(t0, a);
+        t1 = nm::smin(t1, c);
+    }
+    return t0 <= t1 ? t0 : INFINITY;
+}
+
+// nearest-first traversal with a shrinking bound: key(box) orders and culls (a node is searched while key <= bound; with CULL_INF a key of
+// INFINITY also culls), leaf(collider) runs the exact test and may lower bound.  The nearer child is searched first; the answer does not
+// depend on the order (the leaf keeps a lexicographic minimum).
+template <bool CULL_INF, class S, class Key, class Leaf>
+__device__ __forceinline__ void traverse_nearest(const Tree<S>& t, int m, const double& bound, Key key, Leaf leaf) {
+    auto pass = [&](double k) { return (!CULL_INF || k != INFINITY) && k <= bound; };
+    if (m <= 0 || !pass(key(t.nodes[0]))) return;
+    if (m == 1) { leaf(t.leaf[0]); return; }
+    int stack[Q_STACK];
+    int sp = 0;
+    stack[sp++] = 0;
+    while (sp > 0) {
+        const int2 c = t.child[stack[--sp]];
+        const double ka = key(t.nodes[c.x]), kb = key(t.nodes[c.y]);
+        const bool b_first = kb < ka;
+        const int near = b_first ? c.y : c.x, far = b_first ? c.x : c.y;
+        const double kn = b_first ? kb : ka, kf = b_first ? ka : kb;
+        if (!pass(kn)) continue;
+        if (near >= m - 1) leaf(t.leaf[near - (m - 1)]);
+        if (pass(kf)) {
+            if (far >= m - 1) leaf(t.leaf[far - (m - 1)]);
+            else stack[sp++] = far;
+        }
+        if (near < m - 1) stack[sp++] = near;
+    }
+}
+
+template <class S>
+__device__ __forceinline__ bool cast_leaf(const Tree<S>& t, const ShapeIn& q, uint32_t c, double& th, int& axis) {
+    const uint32_t memb = t.memb ? t.memb[c] : 1u;
+    if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
+    return qm::cast_collider(q.shape, q.he, q.c, q.q, q.d, q.maxd, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+}
+template <class S>
+__device__ __forceinline__ void cast_store(const Tree<S>& t, const ShapeIn& q, uint32_t c, double th, int axis, size_t o, S* p1, S* p2, S* n1, S* n2) {
+    qm::ShapeContact h;
+    qm::cast_output(q.shape, q.he, q.c, q.q, q.d, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis, h);
+    const nm::V3 v[4] = {h.p1, h.p2, h.n1, h.n2};
+    S* dst[4] = {p1, p2, n1, n2};
+    for (int k = 0; k < 4; ++k)
+        if (dst[k]) { dst[k][3 * o] = S(v[k].x); dst[k][3 * o + 1] = S(v[k].y); dst[k][3 * o + 2] = S(v[k].z); }
+}
+__device__ __forceinline__ bool cast_visit(const NodeBox& b, const ShapeIn& q) { return grown_entry(b, q.ext, q.c, q.d, q.maxd) != INFINITY; }
+
+// cast_shape: the lexicographic minimum of (t, collider)
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_cast_shape(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, int32_t* __restrict__ out_c,
+                                                           S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2, S* __restrict__ n1, S* __restrict__ n2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s.n) return;
+    const ShapeIn q = load_shape(s, i, true);
+    double best_t = INFINITY;
+    uint32_t best_c = 0xffffffffu;
+    int best_axis = -1;
+    if (q.ok)
+        traverse_nearest<true>(t, *t.m, best_t, [&](const NodeBox& b) { return grown_entry(b, q.ext, q.c, q.d, q.maxd); },
+                               [&](uint32_t c) {
+                                   double th;
+                                   int ax;
+                                   if (cast_leaf(t, q, c, th, ax) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_axis = ax; }
+                               });
+    const bool hit = best_c != 0xffffffffu;
+    out_c[i] = hit ? int32_t(best_c) : -1;
+    out_t[i] = hit ? S(best_t) : S(0);
+    if (hit) {
+        cast_store(t, q, best_c, best_t, best_axis, size_t(i), p1, p2, n1, n2);
+    } else {
+        for (int k = 0; k < 3; ++k) p1[3 * i + k] = p2[3 * i + k] = n1[3 * i + k] = n2[3 * i + k] = S(0);
+    }
+}
+
+// shape_hits count pass: every hit, and the part of it the query keeps (max_hits)
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_shape_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ full,
+                                                            uint32_t* __restrict__ kept) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s.n) return;
+    const ShapeIn q = load_shape(s, i, true);
+    uint32_t cnt = 0;
+    if (q.ok)
+        traverse(t, *t.m, [&](const NodeBox& b) { return cast_visit(b, q); },
+                 [&](uint32_t c) { double th; int ax; if (cast_leaf(t, q, c, th, ax)) ++cnt; });
+    full[i] = cnt;
+    const uint32_t mh = s.max_hits ? s.max_hits[i] : 0xffffffffu;
+    kept[i] = cnt < mh ? cnt : mh;
+}
+
+// shape_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their contacts
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, const uint64_t* __restrict__ full_off,
+                                                           const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
+                                                           uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2,
+                                                           S* __restrict__ n1, S* __restrict__ n2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s.n) return;
+    const ShapeIn q = load_shape(s, i, true);
+    if (!q.ok) return;
+    const uint64_t base = full_off[i];
+    const uint32_t n = uint32_t(full_off[i + 1] - base), keep = uint32_t(kept_off[i + 1] - kept_off[i]);
+    if (keep == 0) return;
+    double* ts = tmp_t + base;
+    uint32_t* cs = tmp_c + base;
+    uint32_t w = 0;
+    traverse(t, *t.m, [&](const NodeBox& b) { return cast_visit(b, q); },
+             [&](uint32_t c) {
+                 double th;
+                 int ax;
+                 if (cast_leaf(t, q, c, th, ax) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+             });
+    sort_segment(
+        w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
+        [&](uint32_t a, uint32_t b) { const double x = ts[a]; ts[a] = ts[b]; ts[b] = x; const uint32_t y = cs[a]; cs[a] = cs[b]; cs[b] = y; });
+    const uint64_t o = kept_off[i];
+    for (uint32_t k = 0; k < keep && k < w; ++k) {
+        const uint32_t c = cs[k];
+        double th = 0;
+        int ax = -1;
+        cast_leaf(t, q, c, th, ax);    // the same exact test again: the axis of this hit
+        out_c[o + k] = c;
+        if (out_t) out_t[o + k] = S(ts[k]);
+        cast_store(t, q, c, ts[k], ax, size_t(o + k), p1, p2, n1, n2);
+    }
+}
+
+// project_point: the lexicographic minimum of (distance, collider); a node is pruned when its squared distance exceeds the best so far
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, int32_t* __restrict__ out_c,
+                                                              S* __restrict__ out_p, uint8_t* __restrict__ out_in) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= pts.n) return;
+    const nm::V3 p = ld3(pts.p, i);
+    const bool solid = pts.solid ? pts.solid[i] != 0 : true;
+    const uint32_t mask = pts.mask ? pts.mask[i] : 0xffffffffu;
+    const uint32_t* xs = pts.xoff ? pts.xs + pts.xoff[i] : nullptr;
+    const uint32_t nx = pts.xoff ? pts.xoff[i + 1] - pts.xoff[i] : 0u;
+    double best_d = INFINITY, bound = INFINITY;
+    uint32_t best_c = 0xffffffffu;
+    nm::V3 best_p{0, 0, 0};
+    bool best_in = false;
+    if (qm::finite3(p))
+        traverse_nearest<false>(t, *t.m, bound, [&](const NodeBox& b) { return qm::point_box_d2(&b.lo.x, &b.hi.x, p); },
+                                [&](uint32_t c) {
+                                    const uint32_t memb = t.memb ? t.memb[c] : 1u;
+                                    if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
+                                    nm::V3 pr;
+                                    bool in;
+                                    const double dd = qm::project_point(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p, solid, pr, in);
+                                    if (qm::hit_before(dd, c, best_d, best_c)) { best_d = dd; best_c = c; best_p = pr; best_in = in; bound = dd * dd; }
+                                });
+    const bool hit = best_c != 0xffffffffu;
+    out_c[i] = hit ? int32_t(best_c) : -1;
+    out_p[3 * i] = S(best_p.x); out_p[3 * i + 1] = S(best_p.y); out_p[3 * i + 2] = S(best_p.z);
+    out_in[i] = hit && best_in ? 1 : 0;
+}
+
+// point_intersections: count, then emit + sort ascending by collider
+template <class S, bool EMIT>
+__global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, uint32_t* __restrict__ counts,
+                                                            const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= pts.n) return;
+    const nm::V3 p = ld3(pts.p, i);
+    const uint32_t mask = pts.mask ? pts.mask[i] : 0xffffffffu;
+    const uint32_t* xs = pts.xoff ? pts.xs + pts.xoff[i] : nullptr;
+    const uint32_t nx = pts.xoff ? pts.xoff[i + 1] - pts.xoff[i] : 0u;
+    uint32_t w = 0;
+    uint32_t* seg = EMIT ? out_c + off[i] : nullptr;
+    if (qm::finite3(p))
+        traverse(t, *t.m, [&](const NodeBox& b) { return qm::point_box_d2(&b.lo.x, &b.hi.x, p) == 0; },
+                 [&](uint32_t c) {
+                     const uint32_t memb = t.memb ? t.memb[c] : 1u;
+                     if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
+                     if (!qm::contains_point(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p)) return;
+                     if (EMIT) seg[w] = c;
+                     ++w;
+                 });
+    if (!EMIT) { counts[i] = w; return; }
+    sort_segment(w, [&](uint32_t x, uint32_t y) { return seg[x] < seg[y]; }, [&](uint32_t x, uint32_t y) { const uint32_t v = seg[x]; seg[x] = seg[y]; seg[y] = v; });
+}
+
+// shape_intersections: count, then emit + sort ascending by collider
+template <class S, bool EMIT>
+__global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ counts,
+                                                            const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s.n) return;
+    const ShapeIn q = load_shape(s, i, false);
+    uint32_t w = 0;
+    uint32_t* seg = EMIT ? out_c + off[i] : nullptr;
+    if (q.ok)
+        traverse(t, *t.m,
+                 [&](const NodeBox& b) { return qm::aabb_overlap(q.lo, q.hi, &b.lo.x, &b.hi.x); },
+                 [&](uint32_t c) {
+                     const uint32_t memb = t.memb ? t.memb[c] : 1u;
+                     if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return;
+                     if (!qm::shapes_intersect(q.shape, q.he, q.c, q.q, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c))) return;
+                     if (EMIT) seg[w] = c;
+                     ++w;
+                 });
+    if (!EMIT) { counts[i] = w; return; }
+    sort_segment(w, [&](uint32_t x, uint32_t y) { return seg[x] < seg[y]; }, [&](uint32_t x, uint32_t y) { const uint32_t v = seg[x]; seg[x] = seg[y]; seg[y] = v; });
+}
+
 template <class S>
 class Queries final : public QueriesBase {
    public:
@@ -563,7 +838,187 @@ class Queries final : public QueriesBase {
         return list_download(out, n, kept_off_.as<uint64_t>(), total, false);
     }
 
+    AvnStatus cast_shape(const AvnShapeBatch* s, AvnShapeClosest* out) override {
+        AvnStatus st = shapes_in(s, true, "avn_query_cast_shape");
+        if (st != AVN_OK) return st;
+        if (!out || (s->count && (!out->collider || !out->distance || !out->point1 || !out->point2 || !out->normal1 || !out->normal2)))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_cast_shape: collider, distance, point1, point2, normal1 and normal2 outputs are required");
+        const int n = int(s->count);
+        if (n == 0) return AVN_OK;
+        AVN_CUDA(oc_.ensure(size_t(n) * 4));
+        AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
+        for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * size_t(n) * sizeof(S)));
+        q_cast_shape<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), shapes_, oc_.as<int32_t>(), ot_.as<S>(), op1_.as<S>(),
+                                                                                             op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
+        AVN_CUDA(cudaGetLastError());
+        AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        void* dst[4] = {out->point1, out->point2, out->normal1, out->normal2};
+        const DevBuf* src[4] = {&op1_, &op2_, &on1_, &on2_};
+        for (int k = 0; k < 4; ++k) AVN_CUDA(cudaMemcpyAsync(dst[k], src[k]->p, 3 * size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    AvnStatus shape_hits(const AvnShapeBatch* s, AvnShapeHitList* out) override {
+        AvnStatus st = shapes_in(s, true, "avn_query_shape_hits");
+        if (st != AVN_OK) return st;
+        if (!out || !out->offsets || (out->capacity && !out->collider))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_shape_hits: offsets and (with a capacity) collider are required");
+        const int n = int(s->count);
+        AVN_CUDA(full_.ensure(size_t(n + 1) * 4));
+        AVN_CUDA(kept_.ensure(size_t(n + 1) * 4));
+        AVN_CUDA(full_off_.ensure(size_t(n + 1) * 8));
+        AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
+        const Tree<S> t = tree();
+        const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        if (n > 0) q_shape_count<S><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        uint64_t tot[2];
+        if ((st = scan(full_.as<uint32_t>(), n, full_off_.as<uint64_t>())) != AVN_OK) return st;
+        if ((st = scan(kept_.as<uint32_t>(), n, kept_off_.as<uint64_t>())) != AVN_OK) return st;
+        AVN_CUDA(cudaMemcpyAsync(&tot[0], full_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(&tot[1], kept_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        out->count = tot[1];
+        if (tot[1] > out->capacity)
+            return err_->fail(AVN_ERR_CAPACITY, "avn_query_shape_hits: %llu hits, capacity %llu", (unsigned long long)tot[1], (unsigned long long)out->capacity);
+        const size_t nf = size_t(std::max<uint64_t>(tot[0], 1)), nk = size_t(std::max<uint64_t>(tot[1], 1));
+        AVN_CUDA(tmp_t_.ensure(nf * 8));
+        AVN_CUDA(tmp_c_.ensure(nf * 4));
+        AVN_CUDA(oc_.ensure(nk * 4));
+        AVN_CUDA(ot_.ensure(nk * sizeof(S)));
+        for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * nk * sizeof(S)));
+        if (n > 0 && tot[1] > 0) {
+            q_shape_emit<S><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
+                                                           oc_.as<uint32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
+            AVN_CUDA(cudaGetLastError());
+        }
+        AVN_CUDA(cudaMemcpyAsync(out->offsets, kept_off_.as<uint64_t>(), size_t(n + 1) * 8, cudaMemcpyDeviceToHost, stream_));
+        if (tot[1]) {
+            const size_t k = tot[1];
+            AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, k * 4, cudaMemcpyDeviceToHost, stream_));
+            if (out->distance) AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, k * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+            void* dst[4] = {out->point1, out->point2, out->normal1, out->normal2};
+            const DevBuf* src[4] = {&op1_, &op2_, &on1_, &on2_};
+            for (int j = 0; j < 4; ++j)
+                if (dst[j]) AVN_CUDA(cudaMemcpyAsync(dst[j], src[j]->p, 3 * k * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        }
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    AvnStatus project_point(const AvnPointBatch* p, AvnPointProjection* out) override {
+        AvnStatus st = points_in(p, "avn_query_project_point");
+        if (st != AVN_OK) return st;
+        if (!out || (p->count && (!out->collider || !out->point || !out->is_inside)))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_project_point: collider, point and is_inside outputs are required");
+        const int n = int(p->count);
+        if (n == 0) return AVN_OK;
+        AVN_CUDA(oc_.ensure(size_t(n) * 4));
+        AVN_CUDA(op1_.ensure(3 * size_t(n) * sizeof(S)));
+        AVN_CUDA(oin_.ensure(size_t(n)));
+        q_project_point<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), points_, oc_.as<int32_t>(), op1_.as<S>(), oin_.as<uint8_t>());
+        AVN_CUDA(cudaGetLastError());
+        AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->point, op1_.p, 3 * size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->is_inside, oin_.p, size_t(n), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    AvnStatus point_intersections(const AvnPointBatch* p, AvnHitList* out) override {
+        AvnStatus st = points_in(p, "avn_query_point_intersections");
+        if (st != AVN_OK) return st;
+        if ((st = list_out(out, "avn_query_point_intersections")) != AVN_OK) return st;
+        const int n = int(p->count);
+        return intersections(n, out, "avn_query_point_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
+            if (counts) q_point_isect<S, false><<<g, Q_THREADS, 0, stream_>>>(t, points_, counts, nullptr, nullptr);
+            else q_point_isect<S, true><<<g, Q_THREADS, 0, stream_>>>(t, points_, nullptr, off, oc);
+        });
+    }
+
+    AvnStatus shape_intersections(const AvnShapeBatch* s, AvnHitList* out) override {
+        AvnStatus st = shapes_in(s, false, "avn_query_shape_intersections");
+        if (st != AVN_OK) return st;
+        if ((st = list_out(out, "avn_query_shape_intersections")) != AVN_OK) return st;
+        const int n = int(s->count);
+        return intersections(n, out, "avn_query_shape_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
+            if (counts) q_shape_isect<S, false><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, counts, nullptr, nullptr);
+            else q_shape_isect<S, true><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, nullptr, off, oc);
+        });
+    }
+
    private:
+    // count -> scan -> (capacity check) -> emit of a collider-only CSR list; launch(t, grid, counts, nullptr, nullptr) counts,
+    // launch(t, grid, nullptr, offsets, out) emits
+    template <class Launch>
+    AvnStatus intersections(int n, AvnHitList* out, const char* what, Launch launch) {
+        const size_t nn = size_t(std::max(n, 1));
+        AVN_CUDA(full_.ensure((nn + 1) * 4));
+        AVN_CUDA(kept_off_.ensure((nn + 1) * 8));
+        const Tree<S> t = tree();
+        const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        if (n > 0) launch(t, g, full_.as<uint32_t>(), nullptr, nullptr);
+        AvnStatus st = scan(full_.as<uint32_t>(), n, kept_off_.as<uint64_t>());
+        if (st != AVN_OK) return st;
+        uint64_t total = 0;
+        AVN_CUDA(cudaMemcpyAsync(&total, kept_off_.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        out->count = total;
+        if (total > out->capacity)
+            return err_->fail(AVN_ERR_CAPACITY, "%s: %llu hits, capacity %llu", what, (unsigned long long)total, (unsigned long long)out->capacity);
+        AVN_CUDA(oc_.ensure(size_t(std::max<uint64_t>(total, 1)) * 4));
+        if (n > 0 && total > 0) {
+            launch(t, g, nullptr, kept_off_.as<uint64_t>(), oc_.as<uint32_t>());
+            AVN_CUDA(cudaGetLastError());
+        }
+        return list_download(out, n, kept_off_.as<uint64_t>(), total, false);
+    }
+
+    // validate on the host, then upload the shape columns into shapes_ (cast: the cast-only columns too)
+    AvnStatus shapes_in(const AvnShapeBatch* s, bool cast, const char* what) {
+        if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
+        if (const char* why = qm::check_shapes(s, cast, sizeof(S) == 8)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
+        const size_t n = s->count;
+        shapes_ = Shapes<S>{};
+        shapes_.n = int(n);
+        if (n == 0) return AVN_OK;
+        AvnStatus st;
+#define UPS(buf, host, cnt, T, dst) if ((st = up<T>(buf, host, cnt, &dst)) != AVN_OK) return st
+        UPS(s_shape_, s->shape, n, uint8_t, shapes_.shape);
+        UPS(s_dims_, s->dims, 3 * n, S, shapes_.dims);
+        UPS(s_pos_, s->position, 3 * n, S, shapes_.pos);
+        UPS(s_rot_, s->rotation, 4 * n, S, shapes_.rot);
+        if (cast) {
+            UPS(s_d_, s->direction, 3 * n, S, shapes_.d);
+            UPS(s_maxd_, s->max_distance, n, S, shapes_.maxd);
+            UPS(s_flags_, s->flags, n, uint32_t, shapes_.flags);
+            UPS(s_mh_, s->max_hits, n, uint32_t, shapes_.max_hits);
+        }
+        UPS(s_mask_, s->mask, n, uint32_t, shapes_.mask);
+        UPS(s_xoff_, s->exclude_offsets, n + 1, uint32_t, shapes_.xoff);
+        if (s->exclude_offsets) UPS(s_xs_, s->exclude_count ? s->exclude : nullptr, s->exclude_count, uint32_t, shapes_.xs);
+#undef UPS
+        return AVN_OK;
+    }
+    AvnStatus points_in(const AvnPointBatch* p, const char* what) {
+        if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
+        if (const char* why = qm::check_points(p)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
+        const size_t n = p->count;
+        points_ = Points<S>{};
+        points_.n = int(n);
+        if (n == 0) return AVN_OK;
+        AvnStatus st;
+#define UPP(buf, host, cnt, T, dst) if ((st = up<T>(buf, host, cnt, &dst)) != AVN_OK) return st
+        UPP(r_o_, p->point, 3 * n, S, points_.p);
+        UPP(r_solid_, p->solid, n, uint8_t, points_.solid);
+        UPP(r_mask_, p->mask, n, uint32_t, points_.mask);
+        UPP(r_xoff_, p->exclude_offsets, n + 1, uint32_t, points_.xoff);
+        if (p->exclude_offsets) UPP(r_xs_, p->exclude_count ? p->exclude : nullptr, p->exclude_count, uint32_t, points_.xs);
+#undef UPP
+        return AVN_OK;
+    }
+
     Tree<S> tree() const {
         Tree<S> t{};
         t.n = n_;
@@ -640,6 +1095,9 @@ class Queries final : public QueriesBase {
     bool built_ = false, has_memb_ = false;
     int n_ = 0;
     Rays<S> rays_{};
+    Shapes<S> shapes_{};
+    Points<S> points_{};
+    DevBuf s_shape_, s_dims_, s_pos_, s_rot_, s_d_, s_maxd_, s_flags_, s_mh_, s_mask_, s_xoff_, s_xs_, op1_, op2_, on1_, on2_, oin_;
     DevBuf pos_, rot_, shape_, dims_, memb_, tmn_, tmx_, cbox_, centre_, valid_, k0_, k1_, v0_, v1_, hist_, nodes_, child_, parent_, arrived_, meta_;
     DevBuf r_o_, r_d_, r_maxd_, r_solid_, r_mh_, r_mask_, r_xoff_, r_xs_;
     DevBuf full_, kept_, full_off_, kept_off_, block_sums_, tmp_t_, tmp_c_, oc_, ot_, on_, qmn_, qmx_;

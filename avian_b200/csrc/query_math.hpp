@@ -180,6 +180,407 @@ NM_HD inline S ray_box_entry(const float* lo, const float* hi, V3 o, V3 d, S tma
     return t0 <= t1 ? t0 : INFINITY;
 }
 
+// ---- shape casts, point projection, point and shape intersections (cuboid / sphere) ---------------------------------------------------
+// Reference call sites: spatial_query/pipeline.rs:315-615 (cast_shape, shape_hits, project_point), 617-683 (point_intersections), 731-826
+// (shape_intersections), shape_caster.rs:335-400 (ShapeCaster::cast).  The reference hands the arithmetic to parry3d; these conventions are ours.
+//
+//   * Shape cast.  The cast shape A (pose c, q) moves along d; t is in units of |d|, as for rays.  The time of impact (TOI) with a collider B is
+//     the smallest t in [0, max_distance] at which the closed shapes intersect.  target_distance is always 0 (the ABI refuses anything else).
+//       - sphere-sphere: a solid ray cast of c against the sphere of radius rA + rB at B's centre.  The discriminant is evaluated as
+//         a (rA + rB)² - |oc × d|² (Lagrange's identity), so it does not cancel for small radii.
+//       - sphere-cuboid, cuboid-sphere: the sphere's centre (moving with +d, or with -d when the cuboid is cast) against the box rounded by
+//         the radius, in the box's frame.  The times where the point crosses a slab face ±h_k split [0, inf) into at most 7 segments; on each
+//         the squared distance to the box is one quadratic in t, and the first t where it reaches r² is its smaller root (the same identity
+//         for the discriminant).  A segment whose every coordinate lies inside its slab is a hit at its start, which makes a radius-0 sphere
+//         exact at the slab faces (the ray-like cast).
+//       - cuboid-cuboid: a moving separating-axis test over the 15 axes in the fixed order A's 3 faces, B's 3 faces, A_i × B_j (i major);
+//         an axis that is exactly zero is skipped.  On each axis the overlap is an interval of t (unnormalised); t_enter = the largest start
+//         (ties to the lowest axis), t_exit = the smallest end.  Hit when t_enter <= t_exit, t_exit >= 0 and max(t_enter, 0) <= max_distance.
+//     Origin penetration: TOI 0 (the shapes touch or overlap at t = 0).  Its normal is the axis of least penetration for boxes (depth / |axis|,
+//     ties to the lowest axis), nm::box_sphere's inside rule for a sphere centre inside a box (the face of least depth, ties to the lowest
+//     axis, + side when the coordinate is 0), the centre difference for two spheres (+y when the centres coincide).
+//     Outputs (ShapeHitData, shape_caster.rs:562-592), world space: point1 / normal1 on the hit collider (normal1 outward, so it points towards
+//     the cast shape), point2 / normal2 = -normal1 on the cast shape at its TOI pose.  Spheres: the centre-to-centre / closest-point
+//     direction.  Box-box on a face axis: the face of the other box most anti-parallel to that face (the incident face) is clipped against the
+//     reference face's side planes (nm::box_face / nm::clip_poly, as the narrow phase does); the witness is the clipped vertex nearest to the
+//     reference plane (the first such vertex on a tie), projected onto that plane for the reference box's point.  Box-box on an edge axis: the
+//     closest points of the two supporting edges.
+//     AVN_CAST_IGNORE_ORIGIN_PENETRATION drops a TOI-0 collider when d · normal1 > 0 (the cast moves away from it);
+//     AVN_CAST_NO_CONTACT_ON_PENETRATION writes the points and normals of a TOI-0 hit as 0.
+//   * Point projection: cuboid = clamp in its frame, sphere = centre + r · unit(p - centre).  Closed shapes: the surface counts as inside.
+//     Inside and solid -> the point itself, is_inside.  Inside and hollow -> the nearest face of a cuboid (ties to the lowest axis, then the
+//     + side) or the sphere surface along p - centre (+y at the centre).  Distance = |projection - p|; the closest collider is the
+//     lexicographic minimum of (distance, collider index).
+//   * Point intersections: closed containment.  Shape intersections: exact separating-axis test for two cuboids (touching intersects; no bias),
+//     closest point for sphere-cuboid, centre distance for two spheres.  Both apply the filter.
+//   * A query shape with a non-finite pose, dims, direction or max_distance, or a zero quaternion, hits nothing; a point that is not finite
+//     projects onto nothing and lies in nothing.  A sphere of radius 0 is legal.
+
+constexpr uint32_t CAST_IGNORE_ORIGIN_PENETRATION = 0x1u;   // = AVN_CAST_IGNORE_ORIGIN_PENETRATION
+constexpr uint32_t CAST_NO_CONTACT_ON_PENETRATION = 0x2u;   // = AVN_CAST_NO_CONTACT_ON_PENETRATION
+
+// half size of the tight AABB of a shape (collider_aabb's e)
+NM_HD inline V3 half_size(int shape, V3 he, const nm::M3& r) {
+    if (shape == nm::SHAPE_SPHERE) return V3{he.x, he.x, he.x};
+    return V3{fabs(r.c[0].x) * he.x + fabs(r.c[1].x) * he.y + fabs(r.c[2].x) * he.z,
+              fabs(r.c[0].y) * he.x + fabs(r.c[1].y) * he.y + fabs(r.c[2].y) * he.z,
+              fabs(r.c[0].z) * he.x + fabs(r.c[1].z) * he.y + fabs(r.c[2].z) * he.z};
+}
+
+NM_HD inline V3 to_local(const nm::M3& r, V3 v) { return V3{nm::dot(v, r.c[0]), nm::dot(v, r.c[1]), nm::dot(v, r.c[2])}; }
+NM_HD inline V3 to_world(const nm::M3& r, V3 v) { return r.c[0] * v.x + r.c[1] * v.y + r.c[2] * v.z; }
+NM_HD inline V3 clamp_box(V3 p, V3 h) {
+    return V3{nm::smax(-h.x, nm::smin(h.x, p.x)), nm::smax(-h.y, nm::smin(h.y, p.y)), nm::smax(-h.z, nm::smin(h.z, p.z))};
+}
+NM_HD inline bool in_box(V3 p, V3 h) { return fabs(p.x) <= h.x && fabs(p.y) <= h.y && fabs(p.z) <= h.z; }
+// squared distance from a local point to the box [-h, h]
+NM_HD inline S box_d2(V3 p, V3 h) { const V3 e = p - clamp_box(p, h); return nm::dot(e, e); }
+
+// the feature of the box [-h, h] nearest to the local point p: on_box and the outward unit normal there.  Outside: the clamp and the
+// direction to p.  Inside (or on the surface with p == clamp): nm::box_sphere's inside rule, the face of least depth h_k - |p_k| (ties to the
+// lowest axis, + side when p_k >= 0), on_box = p moved onto that face.
+NM_HD inline void box_feature(V3 p, V3 h, V3& on_box, V3& n) {
+    on_box = clamp_box(p, h);
+    const V3 e = p - on_box;
+    const S l = nm::len(e);
+    if (l > 0) { n = e * (1 / l); return; }
+    int ax = 0;
+    S best = INFINITY;
+    for (int k = 0; k < 3; ++k) {
+        const S v = nm::comp(h, k) - fabs(nm::comp(p, k));
+        if (v < best) { best = v; ax = k; }
+    }
+    const S sg = nm::comp(p, ax) >= 0 ? 1 : -1;
+    n = V3{ax == 0 ? sg : 0, ax == 1 ? sg : 0, ax == 2 ? sg : 0};
+    on_box = p;
+    if (ax == 0) on_box.x = sg * h.x; else if (ax == 1) on_box.y = sg * h.y; else on_box.z = sg * h.z;
+}
+
+// sphere-sphere TOI: centre c moving along d against a sphere of radius R at p
+NM_HD inline bool sphere_sphere_toi(V3 c, V3 d, V3 p, S R, S& t) {
+    const V3 oc = c - p;
+    const S cc = nm::dot(oc, oc) - R * R;
+    if (cc <= 0) { t = 0; return true; }
+    const S a = nm::dot(d, d), b = nm::dot(oc, d);
+    if (a == 0 || b >= 0) return false;                  // not moving, or moving away from the centre
+    const V3 x = nm::cross(oc, d);
+    const S disc = a * (R * R) - nm::dot(x, x);
+    if (disc < 0) return false;
+    t = (-b - sqrt(disc)) / a;
+    if (t < 0) t = 0;
+    return true;
+}
+
+// rounded-box TOI: the local point p moving along v against the box [-h, h] rounded by r; t = 0 when it already lies within r
+NM_HD inline bool point_rounded_box_toi(V3 p, V3 v, V3 h, S r, S maxd, S& t) {
+    const S r2 = r * r;
+    if (box_d2(p, h) <= r2) { t = 0; return true; }
+    S bp[6];
+    int nb = 0;
+    for (int k = 0; k < 3; ++k) {
+        const S pk = nm::comp(p, k), vk = nm::comp(v, k), hk = nm::comp(h, k);
+        if (vk == 0) continue;
+        const S a = (-hk - pk) / vk, b = (hk - pk) / vk;
+        if (a > 0) bp[nb++] = a;
+        if (b > 0) bp[nb++] = b;
+    }
+    for (int i = 1; i < nb; ++i)
+        for (int j = i; j > 0 && bp[j] < bp[j - 1]; --j) { const S s = bp[j]; bp[j] = bp[j - 1]; bp[j - 1] = s; }
+    S lo = 0;
+    for (int i = 0; i <= nb; ++i) {
+        const S hi = i < nb ? bp[i] : INFINITY;
+        if (lo > maxd) return false;
+        if (!(hi > lo)) continue;
+        const S mid = hi == INFINITY ? lo + 1 : lo + (hi - lo) * 0.5;
+        // per axis on this segment: the offset o_k of the face the point is outside of (p_k -/+ h_k), or inside the slab
+        S o[3], w[3];
+        bool out[3];
+        S A = 0, B = 0, C = 0;
+        for (int k = 0; k < 3; ++k) {
+            const S pk = nm::comp(p, k), vk = nm::comp(v, k), hk = nm::comp(h, k), x = pk + mid * vk;
+            out[k] = x > hk || x < -hk;
+            o[k] = x > hk ? pk - hk : pk + hk;
+            w[k] = vk;
+            if (!out[k]) continue;
+            A += vk * vk;
+            B += o[k] * vk;
+            C += o[k] * o[k];
+        }
+        if (A == 0) {
+            if (C <= r2) { t = lo; return t <= maxd; }   // every moving coordinate inside its slab: within reach from the segment's start
+        } else {
+            // B² - A (C - r²) = A r² - sum over pairs of outside axes (o_i w_j - o_j w_i)²
+            S disc = A * r2;
+            for (int a = 0; a < 3; ++a)
+                for (int b = a + 1; b < 3; ++b) {
+                    if (!out[a] || !out[b]) continue;
+                    const S x = o[a] * w[b] - o[b] * w[a];
+                    disc = disc - x * x;
+                }
+            if (disc >= 0) {
+                const S sq = sqrt(disc), rs = (-B - sq) / A, rl = (-B + sq) / A;
+                if (rs <= hi && rl >= lo) { t = nm::smax(rs, lo); return t <= maxd; }
+            }
+        }
+        lo = hi;
+    }
+    return false;
+}
+
+// the 15 separating axes of two boxes in the fixed order: A's faces, B's faces, A_i × B_j
+NM_HD inline V3 sat_axis(const nm::M3& ra, const nm::M3& rb, int k) {
+    if (k < 3) return ra.c[k];
+    if (k < 6) return rb.c[k - 3];
+    k -= 6;
+    return nm::cross(ra.c[k / 3], rb.c[k % 3]);
+}
+NM_HD inline bool is_zero3(V3 v) { return v.x == 0 && v.y == 0 && v.z == 0; }
+NM_HD inline S box_extent(const nm::M3& r, V3 he, V3 L) {
+    return fabs(nm::dot(r.c[0], L)) * he.x + fabs(nm::dot(r.c[1], L)) * he.y + fabs(nm::dot(r.c[2], L)) * he.z;
+}
+
+// moving SAT: box A (ra, ha, ca) along d against box B.  axis = the entering axis, or at TOI 0 the axis of least penetration
+NM_HD inline bool box_box_toi(const nm::M3& ra, V3 ha, V3 ca, V3 d, const nm::M3& rb, V3 hb, V3 cb, S maxd, S& t, int& axis) {
+    const V3 s = cb - ca;
+    S t_in = -INFINITY, t_out = INFINITY;
+    int ax = -1;
+    for (int k = 0; k < 15; ++k) {
+        const V3 L = sat_axis(ra, rb, k);
+        if (is_zero3(L)) continue;
+        const S s0 = nm::dot(L, s), v = nm::dot(L, d), rho = box_extent(ra, ha, L) + box_extent(rb, hb, L);
+        if (v == 0) {
+            if (fabs(s0) > rho) return false;
+            continue;
+        }
+        const S t1 = (s0 - rho) / v, t2 = (s0 + rho) / v;
+        const S a = nm::smin(t1, t2), b = nm::smax(t1, t2);
+        if (a > t_in) { t_in = a; ax = k; }
+        if (b < t_out) t_out = b;
+    }
+    if (!(t_in <= t_out) || t_out < 0 || nm::smax(t_in, 0) > maxd) return false;
+    if (t_in > 0) { t = t_in; axis = ax; return true; }
+    t = 0;
+    S best = INFINITY;
+    for (int k = 0; k < 15; ++k) {
+        const V3 L = sat_axis(ra, rb, k);
+        if (is_zero3(L)) continue;
+        const S pen = (box_extent(ra, ha, L) + box_extent(rb, hb, L) - fabs(nm::dot(L, s))) / nm::len(L);
+        if (pen < best) { best = pen; axis = k; }
+    }
+    return true;
+}
+
+struct ShapeContact { V3 p1, p2, n1, n2; };
+
+// witnesses of two boxes touching on SAT axis `axis`; n = unit normal from A to B
+NM_HD inline void box_box_witness(const nm::Box& A, const nm::Box& B, int axis, V3 n, ShapeContact& c) {
+    c.n1 = -n;
+    c.n2 = n;
+    if (axis >= 6) {                                     // edge-edge: closest points of the supporting edges
+        const int i = (axis - 6) / 3, j = (axis - 6) % 3;
+        const V3 ea = A.r.c[i], eb = B.r.c[j];
+        V3 pa = A.c, pb = B.c;
+        for (int k = 0; k < 3; ++k) {
+            if (k != i) pa = pa + A.r.c[k] * (nm::comp(A.he, k) * (nm::dot(A.r.c[k], n) > 0 ? 1 : -1));
+            if (k != j) pb = pb + B.r.c[k] * (nm::comp(B.he, k) * (nm::dot(B.r.c[k], n) < 0 ? 1 : -1));
+        }
+        const V3 r = pa - pb;
+        const S a = nm::dot(ea, ea), e = nm::dot(eb, eb), f = nm::dot(eb, r), cc = nm::dot(ea, r), b = nm::dot(ea, eb);
+        const S den = a * e - b * b;
+        S s = den > 0 ? (b * f - cc * e) / den : 0;
+        S u = (b * s + f) / e;
+        const S ha = nm::comp(A.he, i), hb = nm::comp(B.he, j);
+        s = nm::smax(-ha, nm::smin(ha, s));
+        u = nm::smax(-hb, nm::smin(hb, u));
+        c.p2 = pa + ea * s;
+        c.p1 = pb + eb * u;
+        return;
+    }
+    const bool ref_is_a = axis < 3;
+    const nm::Box& R = ref_is_a ? A : B;
+    const nm::Box& I = ref_is_a ? B : A;
+    const int ra = axis % 3;
+    const V3 rn = ref_is_a ? n : -n;                     // outward normal of the reference face
+    int ia = 0;
+    S ib = -1;
+    for (int k = 0; k < 3; ++k) {
+        const S v = fabs(nm::dot(I.r.c[k], rn));
+        if (v > ib) { ib = v; ia = k; }
+    }
+    V3 poly[16], tmp[16];
+    nm::box_face(I, ia, nm::dot(I.r.c[ia], rn) > 0 ? -1 : 1, poly);
+    int np = 4;
+    const int side[2] = {(ra + 1) % 3, (ra + 2) % 3};
+    for (int a = 0; a < 2 && np > 0; ++a) {
+        const V3 sn = R.r.c[side[a]];
+        const S he = nm::comp(R.he, side[a]);
+        np = nm::clip_poly(poly, np, sn, nm::dot(sn, R.c) + he, tmp);
+        np = nm::clip_poly(tmp, np, -sn, -nm::dot(sn, R.c) + he, poly);
+    }
+    const S face_d = nm::dot(rn, R.c) + nm::comp(R.he, ra);
+    V3 w;
+    if (np > 0) {
+        int best = 0;
+        for (int k = 1; k < np; ++k)
+            if (nm::dot(rn, poly[k]) < nm::dot(rn, poly[best])) best = k;
+        w = poly[best];
+    } else {                                             // clipped away by rounding: the incident box's support point towards the face
+        w = I.c;
+        for (int k = 0; k < 3; ++k) w = w + I.r.c[k] * (nm::comp(I.he, k) * (nm::dot(I.r.c[k], rn) > 0 ? -1 : 1));
+    }
+    const V3 on_ref = w - rn * (nm::dot(rn, w) - face_d);
+    if (ref_is_a) { c.p2 = on_ref; c.p1 = w; } else { c.p1 = on_ref; c.p2 = w; }
+}
+
+// The TOI of cast shape A against collider B (before the origin-penetration flag); axis: the box-box SAT axis the cast chose
+NM_HD inline bool cast_toi(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, int sb, V3 hb, V3 cb, Q qb, S& t, int& axis) {
+    axis = -1;
+    bool hit;
+    if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
+        hit = sphere_sphere_toi(ca, d, cb, ha.x + hb.x, t);
+    } else if (sa == nm::SHAPE_SPHERE) {                 // the sphere's centre moves with +d against B's rounded box
+        const nm::M3 r = rot_mat(qb);
+        hit = point_rounded_box_toi(to_local(r, ca - cb), to_local(r, d), hb, ha.x, maxd, t);
+    } else if (sb == nm::SHAPE_SPHERE) {                 // B's centre moves with -d against A's rounded box
+        const nm::M3 r = rot_mat(qa);
+        hit = point_rounded_box_toi(to_local(r, cb - ca), to_local(r, -d), ha, hb.x, maxd, t);
+    } else {
+        hit = box_box_toi(rot_mat(qa), ha, ca, d, rot_mat(qb), hb, cb, maxd, t, axis);
+    }
+    return hit && t <= maxd;
+}
+
+// points and normals of a cast hit at TOI t (A at ca + d t)
+NM_HD inline void cast_contact(int sa, V3 ha, V3 ca, Q qa, V3 d, int sb, V3 hb, V3 cb, Q qb, S t, int axis, ShapeContact& c) {
+    const V3 at = ca + d * t;
+    if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
+        const V3 e = at - cb;
+        const S l = nm::len(e);
+        c.n1 = l > 0 ? e * (1 / l) : V3{0, 1, 0};
+        c.n2 = -c.n1;
+        c.p1 = cb + c.n1 * hb.x;
+        c.p2 = at + c.n2 * ha.x;
+    } else if (sa == nm::SHAPE_SPHERE) {
+        const nm::M3 r = rot_mat(qb);
+        V3 on, n;
+        box_feature(to_local(r, at - cb), hb, on, n);
+        c.n1 = to_world(r, n);
+        c.n2 = -c.n1;
+        c.p1 = cb + to_world(r, on);
+        c.p2 = at + c.n2 * ha.x;
+    } else if (sb == nm::SHAPE_SPHERE) {
+        const nm::M3 r = rot_mat(qa);
+        V3 on, n;
+        box_feature(to_local(r, cb - at), ha, on, n);
+        c.n2 = to_world(r, n);
+        c.n1 = -c.n2;
+        c.p2 = at + to_world(r, on);
+        c.p1 = cb + c.n1 * hb.x;
+    } else {
+        const nm::Box A{at, rot_mat(qa), ha}, B{cb, rot_mat(qb), hb};
+        const V3 L = sat_axis(A.r, B.r, axis);
+        // from A to B along the axis: the side B is entered from (t > 0), the side B's centre lies on (t = 0)
+        const S side = t > 0 ? nm::dot(L, d) : nm::dot(L, cb - at);
+        const V3 n = L * ((side >= 0 ? 1 : -1) / nm::len(L));
+        box_box_witness(A, B, axis, n, c);
+    }
+}
+
+// one collider, acceptance included: the TOI in [0, max_distance] and the origin-penetration flag
+NM_HD inline bool cast_collider(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, uint32_t flags, int sb, V3 hb, V3 cb, Q qb, S& t, int& axis) {
+    if (!cast_toi(sa, ha, ca, qa, d, maxd, sb, hb, cb, qb, t, axis)) return false;
+    if (t == 0 && (flags & CAST_IGNORE_ORIGIN_PENETRATION)) {
+        ShapeContact c;
+        cast_contact(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
+        if (nm::dot(d, c.n1) > 0) return false;
+    }
+    return true;
+}
+
+// the outputs of a hit: its contact, or zeros for a TOI-0 hit with AVN_CAST_NO_CONTACT_ON_PENETRATION
+NM_HD inline void cast_output(int sa, V3 ha, V3 ca, Q qa, V3 d, uint32_t flags, int sb, V3 hb, V3 cb, Q qb, S t, int axis, ShapeContact& c) {
+    if (t == 0 && (flags & CAST_NO_CONTACT_ON_PENETRATION)) {
+        c.p1 = c.p2 = c.n1 = c.n2 = V3{0, 0, 0};
+        return;
+    }
+    cast_contact(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
+}
+
+NM_HD inline bool cast_finite(V3 he, V3 c, Q q, V3 d, S maxd) { return collider_valid(he, c, q) && finite3(d) && std::isfinite(maxd); }
+
+// project_point against one collider: the projection, inside or not; returns |projection - p|
+NM_HD inline S project_point(int shape, V3 he, V3 c, Q q, V3 p, bool solid, V3& proj, bool& inside) {
+    if (shape == nm::SHAPE_SPHERE) {
+        const V3 e = p - c;
+        const S l2 = nm::dot(e, e);
+        inside = l2 <= he.x * he.x;
+        if (inside && solid) { proj = p; return 0; }
+        const S l = sqrt(l2);
+        proj = l > 0 ? c + e * (he.x / l) : c + V3{0, he.x, 0};
+    } else {
+        const nm::M3 r = rot_mat(q);
+        const V3 lp = to_local(r, p - c);
+        inside = in_box(lp, he);
+        if (inside && solid) { proj = p; return 0; }
+        V3 on = clamp_box(lp, he);
+        if (inside) {                                    // the nearest face: ties to the lowest axis, then the + side
+            int ax = 0;
+            S best = INFINITY;
+            for (int k = 0; k < 3; ++k) {
+                const S v = nm::comp(he, k) - fabs(nm::comp(lp, k));
+                if (v < best) { best = v; ax = k; }
+            }
+            const S sg = nm::comp(lp, ax) >= 0 ? 1 : -1;
+            if (ax == 0) on.x = sg * he.x; else if (ax == 1) on.y = sg * he.y; else on.z = sg * he.z;
+        }
+        proj = c + to_world(r, on);
+    }
+    return nm::len(proj - p);
+}
+
+// closed containment
+NM_HD inline bool contains_point(int shape, V3 he, V3 c, Q q, V3 p) {
+    if (shape == nm::SHAPE_SPHERE) {
+        const V3 e = p - c;
+        return nm::dot(e, e) <= he.x * he.x;
+    }
+    return in_box(to_local(rot_mat(q), p - c), he);
+}
+
+// closed intersection of two posed shapes
+NM_HD inline bool shapes_intersect(int sa, V3 ha, V3 ca, Q qa, int sb, V3 hb, V3 cb, Q qb) {
+    if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
+        const V3 e = ca - cb;
+        const S R = ha.x + hb.x;
+        return nm::dot(e, e) <= R * R;
+    }
+    if (sa == nm::SHAPE_SPHERE || sb == nm::SHAPE_SPHERE) {
+        const bool a_sphere = sa == nm::SHAPE_SPHERE;
+        const nm::M3 r = rot_mat(a_sphere ? qb : qa);
+        const V3 lp = to_local(r, a_sphere ? ca - cb : cb - ca);
+        const S rad = a_sphere ? ha.x : hb.x;
+        return box_d2(lp, a_sphere ? hb : ha) <= rad * rad;
+    }
+    const nm::M3 ra = rot_mat(qa), rb = rot_mat(qb);
+    const V3 s = cb - ca;
+    for (int k = 0; k < 15; ++k) {
+        const V3 L = sat_axis(ra, rb, k);
+        if (is_zero3(L)) continue;
+        if (fabs(nm::dot(L, s)) > box_extent(ra, ha, L) + box_extent(rb, hb, L)) return false;
+    }
+    return true;
+}
+
+// squared distance from a point to a culling box (0 inside)
+NM_HD inline S point_box_d2(const float* lo, const float* hi, V3 p) {
+    S s = 0;
+    for (int k = 0; k < 3; ++k) {
+        const S x = nm::comp(p, k), e = x < lo[k] ? S(lo[k]) - x : (x > hi[k] ? x - S(hi[k]) : 0);
+        s += e * e;
+    }
+    return s;
+}
+
 }  // namespace qm
 
 // ---- host-side validation shared by the ABI (before any upload) and the host fixture --------------------------------------------------
@@ -214,5 +615,42 @@ inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_requi
         }
     }
     return nullptr;
+}
+// the exclusion CSR of a shape or point batch
+inline const char* check_exclusions(uint32_t count, uint32_t exclude_count, const uint32_t* offsets, const uint32_t* exclude) {
+    if (!offsets) return nullptr;       // (NULL: no query excludes anything; exclude is then ignored)
+    if (exclude_count && !exclude) return "exclude_count > 0 needs exclude";
+    for (uint32_t i = 0; i < count; ++i)
+        if (offsets[i] > offsets[i + 1]) return "exclude_offsets must be monotone";
+    if (offsets[count] > exclude_count) return "exclude_offsets run past exclude_count";
+    return nullptr;
+}
+// cast: the batch feeds a shape cast (direction and max_distance required, target_distance must be 0)
+inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64) {
+    if (!s) return "shape batch is required";
+    if (s->count >= 0x7fffffffu) return "shapes: too many shapes";
+    if (s->count == 0) return nullptr;
+    if (!s->shape || !s->dims || !s->position || !s->rotation) return "shapes: shape, dims, position and rotation are required";
+    if (cast && (!s->direction || !s->max_distance)) return "shapes: direction and max_distance are required for a cast";
+    for (uint32_t i = 0; i < s->count; ++i) {
+        if (s->shape[i] > AVN_SHAPE_SPHERE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
+        for (int k = 0; k < (s->shape[i] == AVN_SHAPE_SPHERE ? 1 : 3); ++k) {
+            const double v = f64 ? static_cast<const double*>(s->dims)[3 * size_t(i) + k] : static_cast<const float*>(s->dims)[3 * size_t(i) + k];
+            if (v < 0) return "shapes: negative half extent or radius";
+        }
+        if (cast && s->target_distance) {
+            const double td = f64 ? static_cast<const double*>(s->target_distance)[i] : static_cast<const float*>(s->target_distance)[i];
+            if (td != 0) return "shapes: target_distance must be 0 (a cast with a target distance is not supported)";
+        }
+    }
+    if (const char* why = check_exclusions(s->count, s->exclude_count, s->exclude_offsets, s->exclude)) return why;
+    return nullptr;
+}
+inline const char* check_points(const AvnPointBatch* p) {
+    if (!p) return "point batch is required";
+    if (p->count >= 0x7fffffffu) return "points: too many points";
+    if (p->count == 0) return nullptr;
+    if (!p->point) return "points: point is required";
+    return check_exclusions(p->count, p->exclude_count, p->exclude_offsets, p->exclude);
 }
 }  // namespace qm

@@ -54,7 +54,13 @@ def _load():
         lib.avh_query_cast_ray.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnRayBatch), P(api.AvnRayClosest)]
         lib.avh_query_ray_hits.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnRayBatch), P(api.AvnHitList)]
         lib.avh_query_aabb_intersections.argtypes = [C.c_uint32, P(api.AvnQueryColliders), C.c_uint32, _vp, _vp, P(api.AvnHitList)]
-        for f in (lib.avh_query_cast_ray, lib.avh_query_ray_hits, lib.avh_query_aabb_intersections):
+        lib.avh_query_cast_shape.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnShapeBatch), P(api.AvnShapeClosest)]
+        lib.avh_query_shape_hits.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnShapeBatch), P(api.AvnShapeHitList)]
+        lib.avh_query_project_point.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnPointBatch), P(api.AvnPointProjection)]
+        lib.avh_query_point_intersections.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnPointBatch), P(api.AvnHitList)]
+        lib.avh_query_shape_intersections.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnShapeBatch), P(api.AvnHitList)]
+        for f in (lib.avh_query_cast_ray, lib.avh_query_ray_hits, lib.avh_query_aabb_intersections, lib.avh_query_cast_shape, lib.avh_query_shape_hits,
+                  lib.avh_query_project_point, lib.avh_query_point_intersections, lib.avh_query_shape_intersections):
             f.restype = C.c_int
         _lib = lib
     return _lib
@@ -134,6 +140,65 @@ def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, 
         st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
+
+
+def query_cast_shape(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+    """The closest hit of every cast (same output as Context.cast_shape)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    s, keep_s = shapes.as_struct(dt)
+    o, out = api.shape_closest(shapes.count, dt)
+    _query_check(lib, lib.avh_query_cast_shape(32 if dt == np.float32 else 64, C.byref(c), C.byref(s), C.byref(o)))
+    return out
+
+
+def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+    """Every cast's max_hits nearest hits in (t, collider) order as CSR (same output as Context.shape_hits)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    s, keep_s = shapes.as_struct(dt)
+    bits = 32 if dt == np.float32 else 64
+    h, out = api.shape_hit_list(shapes.count, 0, dt)
+    st = lib.avh_query_shape_hits(bits, C.byref(c), C.byref(s), C.byref(h))
+    if st == api.ERR_CAPACITY:
+        h, out = api.shape_hit_list(shapes.count, int(h.count), dt)
+        st = lib.avh_query_shape_hits(bits, C.byref(c), C.byref(s), C.byref(h))
+    _query_check(lib, st)
+    return api.hit_list_result(h, out)
+
+
+def query_project_point(scalar, colliders: "api.QueryColliders", points: "api.Points") -> dict:
+    """The closest collider of every point and the projection onto it (same output as Context.project_point)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    p, keep_p = points.as_struct(dt)
+    o, out = api.point_projection(points.count, dt)
+    _query_check(lib, lib.avh_query_project_point(32 if dt == np.float32 else 64, C.byref(c), C.byref(p), C.byref(o)))
+    return out
+
+
+def _query_list(fn, scalar, colliders, batch) -> dict:
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    b, keep_b = batch.as_struct(dt)
+    bits, n = 32 if dt == np.float32 else 64, batch.count
+    h, out = api.hit_list(n, 0, dt, False)
+    st = getattr(lib, fn)(bits, C.byref(c), C.byref(b), C.byref(h))
+    if st == api.ERR_CAPACITY:
+        h, out = api.hit_list(n, int(h.count), dt, False)
+        st = getattr(lib, fn)(bits, C.byref(c), C.byref(b), C.byref(h))
+    _query_check(lib, st)
+    return api.hit_list_result(h, out)
+
+
+def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "api.Points") -> dict:
+    """Per point the colliders containing it, ascending (same output as Context.point_intersections)."""
+    return _query_list("avh_query_point_intersections", scalar, colliders, points)
+
+
+def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+    """Per query shape the colliders it intersects, ascending (same output as Context.shape_intersections)."""
+    return _query_list("avh_query_shape_intersections", scalar, colliders, shapes)
 
 
 class HostPipeline:

@@ -713,3 +713,195 @@ int avh_query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* 
 }
 
 }  // extern "C"
+
+// ---- shape casts, point projection, point and shape intersections, brute force over every collider ------------------------------------
+namespace {
+struct ShapeView {
+    int shape; V3 he, c, d; Q q; S maxd; uint32_t flags, mask; const uint32_t* xs; uint32_t nx; bool ok;
+};
+ShapeView shape_at(const AvnShapeBatch* s, bool f64, uint32_t i, bool cast) {
+    Col dims{s->dims, f64}, pos{s->position, f64}, rot{s->rotation, f64}, dir{s->direction, f64}, md{s->max_distance, f64};
+    ShapeView v;
+    v.shape = s->shape[i];
+    v.he = dims.v3(i); v.c = pos.v3(i); v.q = rot.q(i);
+    v.d = cast ? dir.v3(i) : V3{0, 0, 0};
+    v.maxd = cast ? md.at(i) : 0;
+    v.flags = cast && s->flags ? s->flags[i] : 0u;
+    v.mask = s->mask ? s->mask[i] : 0xffffffffu;
+    v.xs = s->exclude_offsets ? s->exclude + s->exclude_offsets[i] : nullptr;
+    v.nx = s->exclude_offsets ? s->exclude_offsets[i + 1] - s->exclude_offsets[i] : 0u;
+    v.ok = cast ? qm::cast_finite(v.he, v.c, v.q, v.d, v.maxd) : qm::collider_valid(v.he, v.c, v.q);
+    return v;
+}
+struct CastHit { S t; uint32_t c; int axis; };
+// every hit of one cast, sorted by (t, collider)
+void all_cast_hits(const QueryScene& sc, const ShapeView& v, std::vector<CastHit>& out) {
+    out.clear();
+    if (!v.ok) return;
+    for (uint32_t c = 0; c < sc.c->count; ++c) {
+        if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
+        CastHit h{0, c, -1};
+        if (qm::cast_collider(v.shape, v.he, v.c, v.q, v.d, v.maxd, v.flags, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), h.t, h.axis))
+            out.push_back(h);
+    }
+    std::sort(out.begin(), out.end(), [](const CastHit& a, const CastHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
+}
+qm::ShapeContact cast_contact_of(const QueryScene& sc, const ShapeView& v, const CastHit& h) {
+    qm::ShapeContact k;
+    qm::cast_output(v.shape, v.he, v.c, v.q, v.d, v.flags, sc.c->shape[h.c], sc.dims.v3(h.c), sc.pos.v3(h.c), sc.rot.q(h.c), h.t, h.axis, k);
+    return k;
+}
+int shape_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, bool cast) {
+    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_shapes(s, cast, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    return AVN_OK;
+}
+int point_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p) {
+    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_points(p)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    return AVN_OK;
+}
+int write_list(AvnHitList* out, const std::vector<std::vector<uint32_t>>& per) {
+    uint64_t total = 0;
+    for (const auto& v : per) total += v.size();
+    out->count = total;
+    if (total > out->capacity) return query_fail(AVN_ERR_CAPACITY, "capacity");
+    uint64_t k = 0;
+    for (size_t i = 0; i < per.size(); ++i) {
+        out->offsets[i] = k;
+        for (uint32_t col : per[i]) out->collider[k++] = col;
+    }
+    out->offsets[per.size()] = k;
+    return AVN_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int avh_query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeClosest* out) {
+    if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
+    if (!out || (s->count && (!out->collider || !out->distance || !out->point1 || !out->point2 || !out->normal1 || !out->normal2)))
+        return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    ColW ot{out->distance, f64}, p1{out->point1, f64}, p2{out->point2, f64}, n1{out->normal1, f64}, n2{out->normal2, f64};
+    std::vector<CastHit> hits;
+    for (uint32_t i = 0; i < s->count; ++i) {
+        const ShapeView v = shape_at(s, f64, i, true);
+        all_cast_hits(sc, v, hits);
+        qm::ShapeContact k{};
+        if (!hits.empty()) k = cast_contact_of(sc, v, hits[0]);
+        out->collider[i] = hits.empty() ? -1 : int32_t(hits[0].c);
+        ot.set(i, hits.empty() ? 0 : hits[0].t);
+        p1.set3(i, k.p1); p2.set3(i, k.p2); n1.set3(i, k.n1); n2.set3(i, k.n2);
+    }
+    return AVN_OK;
+}
+
+int avh_query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeHitList* out) {
+    if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
+    if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    std::vector<std::vector<CastHit>> per(s->count);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < s->count; ++i) {
+        all_cast_hits(sc, shape_at(s, f64, i, true), per[i]);
+        const uint32_t mh = s->max_hits ? s->max_hits[i] : 0xffffffffu;
+        if (per[i].size() > mh) per[i].resize(mh);
+        total += per[i].size();
+    }
+    out->count = total;
+    if (total > out->capacity) return query_fail(AVN_ERR_CAPACITY, "capacity");
+    ColW ot{out->distance, f64}, p1{out->point1, f64}, p2{out->point2, f64}, n1{out->normal1, f64}, n2{out->normal2, f64};
+    uint64_t k = 0;
+    for (uint32_t i = 0; i < s->count; ++i) {
+        out->offsets[i] = k;
+        const ShapeView v = shape_at(s, f64, i, true);
+        for (const CastHit& h : per[i]) {
+            const qm::ShapeContact w = cast_contact_of(sc, v, h);
+            out->collider[k] = h.c;
+            if (out->distance) ot.set(k, h.t);
+            if (out->point1) p1.set3(k, w.p1);
+            if (out->point2) p2.set3(k, w.p2);
+            if (out->normal1) n1.set3(k, w.n1);
+            if (out->normal2) n2.set3(k, w.n2);
+            ++k;
+        }
+    }
+    out->offsets[s->count] = k;
+    return AVN_OK;
+}
+
+int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnPointProjection* out) {
+    if (int st = point_inputs(scalar_bits, c, p)) return st;
+    if (!out || (p->count && (!out->collider || !out->point || !out->is_inside))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    Col pc{p->point, f64};
+    ColW op{out->point, f64};
+    for (uint32_t i = 0; i < p->count; ++i) {
+        const V3 x = pc.v3(i);
+        const bool solid = p->solid ? p->solid[i] != 0 : true;
+        const uint32_t mask = p->mask ? p->mask[i] : 0xffffffffu;
+        const uint32_t* xs = p->exclude_offsets ? p->exclude + p->exclude_offsets[i] : nullptr;
+        const uint32_t nx = p->exclude_offsets ? p->exclude_offsets[i + 1] - p->exclude_offsets[i] : 0u;
+        S best_d = INFINITY;
+        uint32_t best_c = 0xffffffffu;
+        V3 best_p{0, 0, 0};
+        bool best_in = false;
+        if (qm::finite3(x))
+            for (uint32_t col = 0; col < c->count; ++col) {
+                if (!sc.valid(col) || !qm::passes_filter(sc.memb(col), mask, xs, nx, col)) continue;
+                V3 pr;
+                bool in;
+                const S d = qm::project_point(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x, solid, pr, in);
+                if (qm::hit_before(d, col, best_d, best_c)) { best_d = d; best_c = col; best_p = pr; best_in = in; }
+            }
+        const bool hit = best_c != 0xffffffffu;
+        out->collider[i] = hit ? int32_t(best_c) : -1;
+        op.set3(i, best_p);
+        out->is_inside[i] = hit && best_in ? 1 : 0;
+    }
+    return AVN_OK;
+}
+
+int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnHitList* out) {
+    if (int st = point_inputs(scalar_bits, c, p)) return st;
+    if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    Col pc{p->point, f64};
+    std::vector<std::vector<uint32_t>> per(p->count);
+    for (uint32_t i = 0; i < p->count; ++i) {
+        const V3 x = pc.v3(i);
+        if (!qm::finite3(x)) continue;
+        const uint32_t mask = p->mask ? p->mask[i] : 0xffffffffu;
+        const uint32_t* xs = p->exclude_offsets ? p->exclude + p->exclude_offsets[i] : nullptr;
+        const uint32_t nx = p->exclude_offsets ? p->exclude_offsets[i + 1] - p->exclude_offsets[i] : 0u;
+        for (uint32_t col = 0; col < c->count; ++col)
+            if (sc.valid(col) && qm::passes_filter(sc.memb(col), mask, xs, nx, col) &&
+                qm::contains_point(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x))
+                per[i].push_back(col);
+    }
+    return write_list(out, per);
+}
+
+int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnHitList* out) {
+    if (int st = shape_inputs(scalar_bits, c, s, false)) return st;
+    if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
+    const bool f64 = scalar_bits == 64;
+    const QueryScene sc(c, f64);
+    std::vector<std::vector<uint32_t>> per(s->count);
+    for (uint32_t i = 0; i < s->count; ++i) {
+        const ShapeView v = shape_at(s, f64, i, false);
+        if (!v.ok) continue;
+        for (uint32_t col = 0; col < c->count; ++col)
+            if (sc.valid(col) && qm::passes_filter(sc.memb(col), v.mask, v.xs, v.nx, col) &&
+                qm::shapes_intersect(v.shape, v.he, v.c, v.q, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col)))
+                per[i].push_back(col);
+    }
+    return write_list(out, per);
+}
+
+}  // extern "C"

@@ -116,6 +116,35 @@ class SpatialQueryPlugin:
         """The raycast system: every caster's RayHits (CSR; per caster its max_hits nearest, sorted by distance)."""
         return self.ctx.ray_hits(rays)
 
+    @staticmethod
+    def shape_casters(shape, dims, origin, rotation, direction, max_distance=None, max_hits=None, enabled=None, owner=None, ignore_self=None,
+                      compute_contact_on_penetration=None, ignore_origin_penetration=None, target_distance=None, mask=None,
+                      exclude=None) -> api.ShapeQueries:
+        """A batch of ShapeCaster components (shape_caster.rs:63-175) with their global origin, rotation and direction, and the reference
+        defaults: max_hits 1, max_distance Scalar::MAX (f32's, finite in both scalars), target_distance 0, compute_contact_on_penetration
+        true, ignore_origin_penetration false, ignore_self true (excludes the caster's own collider `owner`, -1 = none).  A disabled caster
+        keeps no hits (max_hits 0)."""
+        n = int(np.asarray(origin).reshape(-1, 3).shape[0])
+        col = lambda v, default, dt: np.full(n, default, dtype=dt) if v is None else np.broadcast_to(np.asarray(v, dtype=dt), (n,)).copy()
+        mh = col(max_hits, 1, np.uint32)
+        if enabled is not None:
+            mh = np.where(np.asarray(enabled, dtype=bool), mh, 0).astype(np.uint32)
+        flags = np.where(col(compute_contact_on_penetration, True, bool), 0, api.CAST_NO_CONTACT_ON_PENETRATION).astype(np.uint32)
+        flags |= np.where(col(ignore_origin_penetration, False, bool), api.CAST_IGNORE_ORIGIN_PENETRATION, 0).astype(np.uint32)
+        ex = [list(e) for e in exclude] if exclude is not None else [[] for _ in range(n)]
+        if owner is not None:
+            own = np.asarray(owner, dtype=np.int64)
+            for i in np.nonzero(col(ignore_self, True, bool) & (own >= 0))[0]:
+                ex[i].append(int(own[i]))
+        return api.ShapeQueries(shape=shape, dims=dims, position=origin, rotation=rotation, direction=direction,
+                                max_distance=col(max_distance, float(np.finfo(np.float32).max), np.float64),
+                                target_distance=None if target_distance is None else col(target_distance, 0.0, np.float64), flags=flags, max_hits=mh,
+                                mask=mask, exclude=ex)
+
+    def shapecast(self, shapes: api.ShapeQueries) -> dict:
+        """The shapecast system: every caster's ShapeHits (CSR; per caster its max_hits nearest, sorted by distance)."""
+        return self.ctx.shape_hits(shapes)
+
 
 class PhysicsPlugins:
     """The plugin group (src/lib.rs:813-843) restricted to the hot path."""

@@ -592,7 +592,8 @@ AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step);
  *      Stated deviations: the closest hit is the lexicographic minimum of (t, collider index), where the reference takes the first in tree
  *      order; ray_hits keeps the max_hits NEAREST hits sorted by (t, collider index) — RayHits::iter_sorted order — where the reference keeps
  *      the first max_hits in tree order, unordered (pipeline.rs:213-216); the two sets are equal when a ray has no more than max_hits hits.
- *      Not covered: shape casts, point projection, shape / point intersections, the *_callback early exits, several GPUs. ----------------- */
+ *      Shape casts, point projection and point / shape intersections (cuboid and sphere query shapes) are further down, with their own
+ *      conventions.  Not covered: target_distance != 0, other shapes, predicates and the *_callback early exits, several GPUs. ------------- */
 typedef struct AvnQueryColliders {
     uint32_t count;
     uint32_t _pad;
@@ -643,6 +644,104 @@ AvnStatus avn_query_ray_hits(AvnContext* ctx, const AvnRayBatch* rays, AvnHitLis
 /* Replaces SpatialQueryPipeline::aabb_intersections_with_aabb (pipeline.rs:690-729): per query box the colliders whose tight AABB it
  * touches, ascending by index.  min / max: [n][3] in the column scalar. */
 AvnStatus avn_query_aabb_intersections(AvnContext* ctx, uint32_t count, const void* min, const void* max, AvnHitList* out);
+
+/* ---- shape casts, point projection, point and shape intersections (pipeline.rs:315-826, ShapeCaster shape_caster.rs:335-400) against
+ *      the tree of the last avn_query_update.  Same arithmetic sharing as above (query_math.hpp), so results equal the host brute force bit
+ *      for bit.  Conventions:
+ *        - a cast moves the query shape along direction; distances are in units of |direction|.  The TOI is the smallest t in
+ *          [0, max_distance] at which the closed shapes intersect.  Sphere-sphere: a solid ray cast against radius rA + rB.  Sphere-cuboid:
+ *          the centre against the box rounded by the radius (exact piecewise quadratic).  Cuboid-cuboid: moving separating-axis test over
+ *          the 15 axes (A's faces, B's faces, A_i x B_j; exactly-zero axes skipped); the entering axis is the largest interval start, ties
+ *          to the lowest axis;
+ *        - outputs (ShapeHitData): point1 / normal1 on the hit collider, normal1 outward (towards the cast shape); point2 / normal2 =
+ *          -normal1 on the cast shape at its TOI pose.  Box-box face contacts report the clipped incident-face vertex nearest to the
+ *          reference face; edge contacts the closest points of the two edges;
+ *        - origin penetration (touching or overlapping at t = 0) is a hit at t = 0, normal along the axis of least penetration (boxes), the
+ *          nearest face of a box holding the sphere's centre, or the centre difference (+y for coincident centres).
+ *          AVN_CAST_IGNORE_ORIGIN_PENETRATION drops such a collider when direction . normal1 > 0; AVN_CAST_NO_CONTACT_ON_PENETRATION
+ *          writes its points and normals as 0;
+ *        - target_distance must be 0 (ShapeCaster's default): any other value is refused with AVN_ERR_INVALID_ARGUMENT;
+ *        - project_point: cuboid = clamp in its frame, sphere = centre + r * unit(p - centre); the surface counts as inside; inside and solid
+ *          -> the point itself, is_inside = 1; inside and hollow -> the nearest face (ties to the lowest axis, then the + side), +y from a
+ *          sphere's centre; the closest collider is the lexicographic minimum of (distance, collider index);
+ *        - point intersections: closed containment; shape intersections: exact SAT for two cuboids (touching intersects), closest point for
+ *          sphere-cuboid, centre distance for two spheres; both apply the filter;
+ *        - query shapes with a non-finite pose, dims, direction or max_distance or a zero quaternion hit nothing; non-finite points project
+ *          onto nothing and lie in nothing; negative dims and unknown shapes are refused; a sphere of radius 0 is legal.
+ *      Stated deviations: closest = minimum of (t, collider index) where the reference takes the first in tree order; shape_hits keeps the
+ *      max_hits nearest sorted by (t, collider index) — the same set as the reference's repeated cast with the previous hits excluded
+ *      (shape_caster.rs:372-399, pipeline.rs:524-554), since each collider's TOI does not depend on the others; only ties are ordered
+ *      differently (by index instead of tree order); point and shape intersections are ascending by index, where the reference returns
+ *      tree order. -------------------------------------------------------------------------------------------------------------------- */
+#define AVN_CAST_IGNORE_ORIGIN_PENETRATION 0x1u   /* ShapeCastConfig::ignore_origin_penetration */
+#define AVN_CAST_NO_CONTACT_ON_PENETRATION 0x2u   /* !ShapeCastConfig::compute_contact_on_penetration */
+
+typedef struct AvnShapeBatch {
+    uint32_t count;
+    uint32_t exclude_count;            /* length of exclude[] */
+    const uint8_t* shape;              /* [n] AvnShape */
+    const void* dims;                  /* [n][3] cuboid half extents / sphere radius in [0] */
+    const void* position;              /* [n][3] */
+    const void* rotation;              /* [n][4] */
+    const void* direction;             /* [n][3] casts only */
+    const void* max_distance;          /* [n] casts only */
+    const void* target_distance;       /* [n] casts only; NULL = 0; must be 0 */
+    const uint32_t* flags;             /* [n] casts only: AVN_CAST_*; NULL = 0 */
+    const uint32_t* max_hits;          /* [n] shape_hits only: 0 = none, 0xFFFFFFFF = all; NULL = all */
+    const uint32_t* mask;              /* [n] SpatialQueryFilter::mask; NULL = all layers */
+    const uint32_t* exclude_offsets;   /* [n + 1] CSR of excluded collider indices; NULL = none */
+    const uint32_t* exclude;           /* [exclude_count] */
+} AvnShapeBatch;
+
+typedef struct AvnPointBatch {
+    uint32_t count;
+    uint32_t exclude_count;
+    const void* point;                 /* [n][3] */
+    const uint8_t* solid;              /* [n] project_point only; NULL = all solid */
+    const uint32_t* mask;              /* [n] NULL = all layers */
+    const uint32_t* exclude_offsets;   /* [n + 1] NULL = none */
+    const uint32_t* exclude;           /* [exclude_count] */
+} AvnPointBatch;
+
+typedef struct AvnShapeClosest {       /* per cast */
+    int32_t* collider;                 /* [n] out: collider index, -1 = no hit */
+    void* distance;                    /* [n] out (0 when no hit) */
+    void* point1;                      /* [n][3] out, on the collider (0 when no hit) */
+    void* point2;                      /* [n][3] out, on the cast shape */
+    void* normal1;                     /* [n][3] out */
+    void* normal2;                     /* [n][3] out */
+} AvnShapeClosest;
+
+typedef struct AvnShapeHitList {       /* CSR as AvnHitList; the per-hit columns other than collider may be NULL (not wanted) */
+    uint64_t capacity;
+    uint64_t count;                    /* out: total hits; above capacity -> AVN_ERR_CAPACITY and nothing else is written */
+    uint64_t* offsets;                 /* [n + 1] out */
+    uint32_t* collider;                /* [capacity] out */
+    void* distance;                    /* [capacity] out */
+    void* point1;                      /* [capacity][3] out */
+    void* point2;
+    void* normal1;
+    void* normal2;
+} AvnShapeHitList;
+
+typedef struct AvnPointProjection {    /* per point */
+    int32_t* collider;                 /* [n] out: closest collider, -1 = none */
+    void* point;                       /* [n][3] out: the projection (0 when none) */
+    uint8_t* is_inside;                /* [n] out */
+} AvnPointProjection;
+
+/* Replaces SpatialQueryPipeline::cast_shape (pipeline.rs:335-375): per query shape the closest hit.  Before any update: AVN_ERR_INVALID_ARGUMENT. */
+AvnStatus avn_query_cast_shape(AvnContext* ctx, const AvnShapeBatch* shapes, AvnShapeClosest* out);
+/* Replaces SpatialQueryPipeline::shape_hits (pipeline.rs:443-554) and the shapecast system's ShapeHits (shape_caster.rs:335-400): per query
+ * shape its max_hits nearest hits in (t, collider index) order. */
+AvnStatus avn_query_shape_hits(AvnContext* ctx, const AvnShapeBatch* shapes, AvnShapeHitList* out);
+/* Replaces SpatialQueryPipeline::project_point (pipeline.rs:570-615). */
+AvnStatus avn_query_project_point(AvnContext* ctx, const AvnPointBatch* points, AvnPointProjection* out);
+/* Replaces SpatialQueryPipeline::point_intersections (pipeline.rs:628-683): per point the colliders containing it, ascending by index. */
+AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* points, AvnHitList* out);
+/* Replaces SpatialQueryPipeline::shape_intersections (pipeline.rs:744-826): per query shape the colliders it intersects, ascending by index.
+ * The cast-only columns of the batch are ignored. */
+AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out);
 
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out);
 

@@ -5,7 +5,11 @@ Times, each warmed up and repeated (median, min, max):
   * avn_query_update over all 100 001 colliders, with and without AVN_QUERY_SHAPES_UNCHANGED;
   * 1 000 000 closest-hit rays: a downward grid over the stack + random directions from inside it;
   * 100 000 ray_hits rays keeping all hits (downward grid);
-  * 100 000 AABB queries (a box of half size 0.6 around random cubes).
+  * 100 000 AABB queries (a box of half size 0.6 around random cubes);
+  * 1 000 000 closest sphere casts and 1 000 000 closest cuboid casts straight down over the stack;
+  * 100 000 shape_hits casts keeping all hits (downward, half spheres, half cubes);
+  * 1 000 000 project_point queries around random cubes (half solid, half hollow);
+  * 100 000 point intersections and 100 000 shape intersections around random cubes.
 Every query time is one C-ABI call from host columns (already in the context's scalar) to host results (upload, kernels, download): CUDA
 events on the library's stream and the host clock, both closed by the call's own stream synchronise.  Prints the card and its power limit
 (nvidia-smi, read-only) and writes OUT_DIR/query_timing.json.   usage: python scripts/query_timing.py OUT_DIR [--repeats R]"""
@@ -119,6 +123,42 @@ def main():
         res["aabb_100k_total_hits"] = int(q["collider"].shape[0])
         acap = res["aabb_100k_total_hits"]
         res["aabb_100k_ms"] = timed(ctx, lambda: ctx.aabb_intersections(qmn, qmx, capacity=acap), a.warmup, a.repeats)
+
+        # shape casts straight down over the stack (a 1000 x 1000 grid), spheres of radius 0.25 and unrotated cubes of half size 0.25
+        side = 1000
+        gx, gz = np.meshgrid(np.linspace(lo[0], hi[0], side), np.linspace(lo[2], hi[2], side), indexing="ij")
+        k = gx.size
+        cast_o = np.stack([gx.ravel(), np.full(k, hi[1] + 5.0), gz.ravel()], 1).astype(f)
+        for name, shape in (("sphere", 1), ("cuboid", 0)):
+            casts = api.ShapeQueries(shape=np.full(k, shape, np.uint8), dims=np.full((k, 3), 0.25, dtype=f), position=cast_o,
+                                     rotation=np.tile(np.array([0, 0, 0, 1], dtype=f), (k, 1)), direction=np.tile(np.array([0, -1, 0], dtype=f), (k, 1)),
+                                     max_distance=np.full(k, 100.0, dtype=f))
+            res[f"cast_shape_{name}_1m_ms"] = timed(ctx, lambda: ctx.cast_shape(casts), a.warmup, a.repeats)
+            res[f"cast_shape_{name}_1m_hit_fraction"] = float((ctx.cast_shape(casts)["collider"] >= 0).mean())
+        m = 100_000
+        idx = np.linspace(0, k - 1, m).astype(np.int64)
+        hits_casts = api.ShapeQueries(shape=(np.arange(m) % 2).astype(np.uint8), dims=np.full((m, 3), 0.25, dtype=f), position=cast_o[idx],
+                                      rotation=np.tile(np.array([0, 0, 0, 1], dtype=f), (m, 1)), direction=np.tile(np.array([0, -1, 0], dtype=f), (m, 1)),
+                                      max_distance=np.full(m, 100.0, dtype=f), max_hits=np.full(m, api.MAX_HITS_ALL, np.uint32))
+        sh = ctx.shape_hits(hits_casts)
+        scap = int(sh["collider"].shape[0])
+        res["shape_hits_100k_total_hits"] = scap
+        res["shape_hits_100k_ms"] = timed(ctx, lambda: ctx.shape_hits(hits_casts, capacity=scap), a.warmup, a.repeats)
+
+        # 1M points around random cubes (half of them hollow), and 100k points / shapes for the intersection tests
+        c = pos[rng.integers(0, n - 1, 1_000_000)] + rng.uniform(-0.8, 0.8, (1_000_000, 3))
+        pts = api.Points(point=c.astype(f), solid=(np.arange(c.shape[0]) % 2 == 0))
+        res["project_point_1m_ms"] = timed(ctx, lambda: ctx.project_point(pts), a.warmup, a.repeats)
+        ipts = api.Points(point=c[:m].astype(f))
+        res["point_intersections_100k_total_hits"] = int(ctx.point_intersections(ipts)["collider"].shape[0])
+        pcap = res["point_intersections_100k_total_hits"]
+        res["point_intersections_100k_ms"] = timed(ctx, lambda: ctx.point_intersections(ipts, capacity=pcap), a.warmup, a.repeats)
+        q = rng.normal(size=(m, 4))
+        isect = api.ShapeQueries(shape=(np.arange(m) % 2).astype(np.uint8), dims=np.full((m, 3), 0.4, dtype=f), position=c[:m].astype(f),
+                                 rotation=(q / np.linalg.norm(q, axis=1, keepdims=True)).astype(f))
+        res["shape_intersections_100k_total_hits"] = int(ctx.shape_intersections(isect)["collider"].shape[0])
+        icap = res["shape_intersections_100k_total_hits"]
+        res["shape_intersections_100k_ms"] = timed(ctx, lambda: ctx.shape_intersections(isect, capacity=icap), a.warmup, a.repeats)
     (out_dir / "query_timing.json").write_text(json.dumps(res, indent=1))
     print(json.dumps(res))
 
