@@ -2,7 +2,7 @@
 // Stands where NarrowPhase::update calls contact_manifolds for every contact pair (narrow_phase/system_param.rs:437-830,
 // collider/parry/contact_query.rs:156-261).  The arithmetic is csrc/narrow_math.hpp — the same header the host fixture compiles — evaluated
 // in double like the fixture and rounded to the column scalar on store, so the device manifolds equal the fixture's bit for bit
-// (tests/test_gpu_narrow.py).  One thread per pair: ~100 registers and a 1.6 KB local frame for the clipped polygon; 2 poses + 2 velocities
+// (tests/test_gpu_narrow.py).  One thread per pair: 128 registers and a 1.8 KB local frame for the clipped polygon (ptxas figures in DESIGN.md §7); 2 poses + 2 velocities
 // in (≈ 150 B), ≤ 4 points out (≈ 150 B): a streaming kernel, HBM/L2-bound by the gathers of the pose rows.
 #include "context.hpp"
 #include "narrow_math.hpp"

@@ -11,8 +11,12 @@
 
 #if defined(__CUDACC__)
 #define NM_HD __host__ __device__
+#define NM_COLD __host__ __device__ __noinline__
+#define NM_ROLLED _Pragma("unroll 1")
 #else
 #define NM_HD
+#define NM_COLD
+#define NM_ROLLED
 #endif
 
 namespace nm {
@@ -44,7 +48,8 @@ NM_HD inline M3 to_mat(Q q) { return {{rot(q, {1, 0, 0}), rot(q, {0, 1, 0}), rot
 enum ShapeType { SHAPE_CUBOID = 0, SHAPE_SPHERE = 1 };
 struct Box { V3 c; M3 r; V3 he; };
 
-// witness points of a contact: on shape A, on shape B (world space).  A quad clipped by four planes has at most 8 vertices.
+// witness points of a contact: on shape A, on shape B (world axes, origin at A's position: see collide).  A quad clipped by four planes
+// has at most 8 vertices.
 constexpr int MAX_RAW_POINTS = 8;
 struct Witness { V3 a, b; };
 struct Contacts {
@@ -78,8 +83,95 @@ NM_HD inline S box_radius(const Box& b, V3 n) {
     return fabs(dot(b.r.c[0], n)) * b.he.x + fabs(dot(b.r.c[1], n)) * b.he.y + fabs(dot(b.r.c[2], n)) * b.he.z;
 }
 
+// Closest points of the segments p + u*s, |s| <= hu and q + w*t, |t| <= hw: clamp s, recompute t from it, and when t has to be clamped
+// recompute s from the clamped t (dependent clamping, Ericson, Real-Time Collision Detection §5.1.9).  Returns true when the pair is not
+// interior to both segments: an end is active, or the segments are too close to parallel for an interior pair to be defined.
+NM_HD inline bool segment_closest(V3 p, V3 u, S hu, V3 q, V3 w, S hw, S& s, S& t) {
+    V3 r = p - q;
+    S a = dot(u, u), e = dot(w, w), f = dot(w, r), c = dot(u, r), b = dot(u, w);
+    S den = a * e - b * b;
+    S s0 = den > 1e-12 ? (b * f - c * e) / den : 0;
+    s = smax(-hu, smin(hu, s0));
+    bool end = den <= 1e-12 || s != s0;
+    t = (b * s + f) / e;
+    if (t < -hw || t > hw) {
+        t = t < -hw ? -hw : hw;
+        s = smax(-hu, smin(hu, (b * t - c) / a));
+        end = true;
+    }
+    return end;
+}
+
+// The point of box b closest to p (p itself when inside); returns the squared distance.
+NM_HD inline S box_point_closest(const Box& b, V3 p, V3& on) {
+    V3 d = p - b.c;
+    on = b.c;
+    for (int k = 0; k < 3; ++k) on = on + b.r.c[k] * smax(-comp(b.he, k), smin(comp(b.he, k), dot(d, b.r.c[k])));
+    V3 e = p - on;
+    return dot(e, e);
+}
+
+// The closest pair of points of two disjoint boxes: the minimum over every vertex against the other box and every edge against every
+// edge.  Returns the distance.  box_box uses it only for separated pairs whose SAT feature misses the closest features: a rare branch,
+// kept out of line and rolled so that its 16 + 144 candidates are not unrolled into the kernels that inline box_box (fully inlined,
+// they took 255 registers and spilled).  The call still costs registers: see DESIGN.md §7 for the ptxas figures.
+NM_COLD inline S box_box_closest(const Box& A, const Box& B, V3& on_a, V3& on_b) {
+    S best = 1e300;
+NM_ROLLED
+    for (int side = 0; side < 2; ++side) {
+        const Box& P = side == 0 ? A : B;
+        const Box& O = side == 0 ? B : A;
+NM_ROLLED
+        for (int m = 0; m < 8; ++m) {
+            V3 v = P.c + P.r.c[0] * (m & 1 ? P.he.x : -P.he.x) + P.r.c[1] * (m & 2 ? P.he.y : -P.he.y) + P.r.c[2] * (m & 4 ? P.he.z : -P.he.z);
+            V3 on;
+            S d2 = box_point_closest(O, v, on);
+            if (d2 < best) { best = d2; on_a = side == 0 ? v : on; on_b = side == 0 ? on : v; }
+        }
+    }
+    // edge k of a box, number m: the segment along axis k through the centre offset by the signs of m on the other two axes
+    auto edge_mid = [](const Box& b, int k, int m) {
+        int u = (k + 1) % 3, v = (k + 2) % 3;
+        return b.c + b.r.c[u] * (m & 1 ? comp(b.he, u) : -comp(b.he, u)) + b.r.c[v] * (m & 2 ? comp(b.he, v) : -comp(b.he, v));
+    };
+NM_ROLLED
+    for (int ei = 0; ei < 12; ++ei) {
+        const int i = ei >> 2, mi = ei & 3;
+        V3 pa = edge_mid(A, i, mi);
+NM_ROLLED
+        for (int ej = 0; ej < 12; ++ej) {
+            const int j = ej >> 2, mj = ej & 3;
+            V3 pb = edge_mid(B, j, mj);
+            S s, t;
+            segment_closest(pa, A.r.c[i], comp(A.he, i), pb, B.r.c[j], comp(B.he, j), s, t);
+            V3 qa = pa + A.r.c[i] * s, qb = pb + B.r.c[j] * t, e = qb - qa;
+            S d2 = dot(e, e);
+            if (d2 < best) { best = d2; on_a = qa; on_b = qb; }
+        }
+    }
+    return sqrt(best);
+}
+
+// A separated pair as its closest points (from box_box_closest): one witness pair, the normal along it (from A to B).  False when it
+// is beyond max_dist.
+NM_HD inline bool closest_pair(V3 on_a, V3 on_b, S dist, S max_dist, V3& normal, Contacts& pts) {
+    pts.clear();
+    if (dist > max_dist) return false;
+    if (dist > 1e-12) normal = (on_b - on_a) * (1 / dist);
+    pts.push(on_a, on_b);
+    return true;
+}
+
+// How much farther than the true distance the nearest clipped point of a separated face contact may be before the closest feature pair
+// replaces the clipped polygon: a face contact whose nearest point is the closest feature (a box resting or landing flat) keeps its
+// polygon, and a box whose nearest corner or edge hangs past the reference face gets that corner or edge instead.
+constexpr S FACE_GAP_SLACK = 1e-4;
+
 // SAT over the 15 axes, then either the closest points of the two supporting edges or the incident face clipped against the
 // reference face's side planes.  Returns false when the boxes are farther apart than max_dist.  normal points from A to B.
+// Separated pairs whose SAT feature does not give the closest points (the edges' closest points lie at an end, or the clipped face
+// lies farther than FACE_GAP_SLACK beyond the true distance) report their closest feature pair instead.  Overlapping pairs whose edges'
+// closest points lie at an end use the best face axis.
 NM_HD inline bool box_box(const Box& A, const Box& B, S max_dist, V3& normal, Contacts& pts) {
     pts.clear();
     V3 d = B.c - A.c;
@@ -97,6 +189,9 @@ NM_HD inline bool box_box(const Box& A, const Box& B, S max_dist, V3& normal, Co
     };
     for (int i = 0; i < 3; ++i) consider(A.r.c[i], 0, i, 0, 0);
     for (int i = 0; i < 3; ++i) consider(B.r.c[i], 1, i, 0, 0);
+    const S face_sep = best_sep;
+    const int face_kind = best_kind, face_i = best_i;
+    const V3 face_n = best_n;
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) consider(cross(A.r.c[i], B.r.c[j]), 2, i, j, 1e-4);
     S sep = best_kind == 2 ? best_sep + 1e-4 : best_sep;
@@ -110,16 +205,18 @@ NM_HD inline bool box_box(const Box& A, const Box& B, S max_dist, V3& normal, Co
             if (k != best_i) pa = pa + A.r.c[k] * (comp(A.he, k) * (dot(A.r.c[k], normal) > 0 ? 1 : -1));
             if (k != best_j) pb = pb + B.r.c[k] * (comp(B.he, k) * (dot(B.r.c[k], normal) < 0 ? 1 : -1));
         }
-        V3 r = pa - pb;
-        S a = dot(ea, ea), e = dot(eb, eb), f = dot(eb, r), c = dot(ea, r), b = dot(ea, eb);
-        S den = a * e - b * b;
-        S s = den > 1e-12 ? (b * f - c * e) / den : 0;
-        S t = (b * s + f) / e;
-        S ha = comp(A.he, best_i), hb = comp(B.he, best_j);
-        s = smax(-ha, smin(ha, s));
-        t = smax(-hb, smin(hb, t));
-        pts.push(pa + ea * s, pb + eb * t);
-        return true;
+        S s, t;
+        if (!segment_closest(pa, ea, comp(A.he, best_i), pb, eb, comp(B.he, best_j), s, t)) {
+            pts.push(pa + ea * s, pb + eb * t);
+            return true;
+        }
+        // an end is active: the edges are not the closest features
+        if (sep > 0) {
+            V3 on_a, on_b;
+            S dist = box_box_closest(A, B, on_a, on_b);
+            return closest_pair(on_a, on_b, dist, max_dist, normal, pts);
+        }
+        sep = face_sep; best_kind = face_kind; best_i = face_i; normal = face_n;
     }
     // face contact: reference box R (face axis), incident box I
     const bool ref_is_a = best_kind == 0;
@@ -146,9 +243,11 @@ NM_HD inline bool box_box(const Box& A, const Box& B, S max_dist, V3& normal, Co
         np = clip_poly(tmp, np, -sn, -dot(sn, R.c) + he, poly);
     }
     S face_d = dot(rn, R.c) + comp(R.he, best_i) * 1.0;
+    S nearest = 1e300;
     for (int k = 0; k < np; ++k) {
         S dist = dot(rn, poly[k]) - face_d;  // signed distance of the incident point above the reference face
         if (dist > max_dist) continue;
+        nearest = smin(nearest, dist);
         V3 on_ref = poly[k] - rn * dist;
         // drop near-duplicates
         bool dup = false;
@@ -159,6 +258,13 @@ NM_HD inline bool box_box(const Box& A, const Box& B, S max_dist, V3& normal, Co
         if (dup) continue;
         if (pts.n == MAX_RAW_POINTS) break;
         if (ref_is_a) pts.push(on_ref, poly[k]); else pts.push(poly[k], on_ref);
+    }
+    // separated, and the clipped face does not reach down to the SAT separation: the closest features may lie outside the reference
+    // face's prism (a corner hanging past its edge), so compare with the true distance
+    if (sep > 0 && nearest > sep + FACE_GAP_SLACK) {
+        V3 on_a, on_b;
+        S dist = box_box_closest(A, B, on_a, on_b);
+        if (nearest > dist + FACE_GAP_SLACK) return closest_pair(on_a, on_b, dist, max_dist, normal, pts);
     }
     return pts.n != 0;
 }
@@ -207,7 +313,10 @@ NM_HD inline bool box_sphere(const Box& A, V3 cs, S rs, S max_dist, V3& normal, 
     V3 on_box = A.c + A.r.c[0] * cl.x + A.r.c[1] * cl.y + A.r.c[2] * cl.z;
     V3 e = cs - on_box;
     S l = len(e);
-    if (l > 1e-9) {
+    // inside is decided on the local coordinates: an f32 quaternion is unit only to an ulp, so rebuilding the centre from them misses
+    // it by ~1e-8 and the distance alone cannot tell a centre inside from one just outside
+    const bool inside = fabs(local.x) <= A.he.x && fabs(local.y) <= A.he.y && fabs(local.z) <= A.he.z;
+    if (!inside && l > 1e-9) {
         if (l - rs > max_dist) return false;
         normal = e * (1 / l);
     } else {  // centre inside the box: push out through the nearest face
@@ -222,7 +331,11 @@ NM_HD inline bool box_sphere(const Box& A, V3 cs, S rs, S max_dist, V3& normal, 
 }
 
 // One collider pair -> normal (from A to B) and at most 4 witness pairs.  he = half extents of a cuboid, radius in he.x of a sphere.
+// The geometry runs in a frame centred on A, so the result does not depend on where the pair is in the world (the header's absolute
+// thresholds, e.g. prune4's 1e-12 depth tie, would otherwise meet the rounding of world coordinates): the witnesses are relative to pa.
 NM_HD inline bool collide(int type_a, V3 he_a, V3 pa, Q qa, int type_b, V3 he_b, V3 pb, Q qb, S max_dist, V3& normal, Contacts& pts) {
+    pb = pb - pa;
+    pa = V3{0, 0, 0};
     bool hit;
     if (type_a == SHAPE_CUBOID && type_b == SHAPE_CUBOID) {
         Box A{pa, to_mat(qa), he_a}, B{pb, to_mat(qb), he_b};
@@ -248,14 +361,15 @@ NM_HD inline bool collide(int type_a, V3 he_a, V3 pa, Q qa, int type_b, V3 he_b,
 // origins (collider at the body origin, centre of mass at the origin), penetration, normal speed.
 struct PointOut { V3 anchor1, anchor2; S penetration, normal_speed; };
 
-// From the witness pairs to the manifold's points: the speculative keep rule of narrow_phase/system_param.rs:748-756.
-// rel = v2 - v1, eff_margin = dt * |rel| (margin = MAX).  Returns the number of points written to out[0..4).
+// From the witness pairs of collide (relative to pa) to the manifold's points: the speculative keep rule of
+// narrow_phase/system_param.rs:748-756.  rel = v2 - v1, eff_margin = dt * |rel| (margin = MAX).  Returns the number of points written
+// to out[0..4).
 NM_HD inline int manifold_points(const Contacts& pts, V3 normal, V3 pa, V3 pb, V3 rel, V3 w1, V3 w2, S dt, S eff_margin, PointOut out[4]) {
     int m = 0;
     for (int k = 0; k < pts.n && m < 4; ++k) {
         PointOut pt;
-        pt.anchor1 = pts.p[k].a - pa;
-        pt.anchor2 = pts.p[k].b - pb;
+        pt.anchor1 = pts.p[k].a;
+        pt.anchor2 = pts.p[k].b - (pb - pa);
         pt.penetration = dot(pts.p[k].a - pts.p[k].b, normal);
         V3 rv = rel + cross(w2, pt.anchor2) - cross(w1, pt.anchor1);
         pt.normal_speed = dot(rv, normal);
