@@ -315,8 +315,9 @@ __device__ __forceinline__ void apply_impulse(V3<S>& v1, V3<S>& w1, V3<S>& v2, V
 // optional trace counters
 enum { FLAG_RESTITUTION = 0, FLAG_WAVE = 1, FLAG_WORDS = 4 };
 // Optional latency trace of the wavefront items (build with -DAVN_WAVE_TRACE; scripts/wave_trace.py): per-warp SM-cycle sums of
-// [0] wait for the exact event  [1] mutable loads (velocities, impulses) + staged rows  [2] arithmetic  [3] stores + release fence + publish,
-// [4] item count, [5] stage 1 of a solve item (wait for the deltas + the separations).  The buffer is 8 unsigned long long counters behind
+// [0] wait for the exact event  [1] mutable loads (velocities, impulses) + staged rows  [2] arithmetic (with the impulse record stores)
+// [3] velocity stores + release fence + publish, [4] item count, [5] stage 1 of a solve item (wait for the deltas, the separations and the
+// normal-impulse coefficients).  The buffer is 8 unsigned long long counters behind
 // the FLAG_WORDS int flags of any_restitution.
 #ifdef AVN_WAVE_TRACE
 #define AVN_TRACE_T(var) const long long var = clock64()
@@ -365,12 +366,13 @@ template <bool WAVE, class S> __device__ __forceinline__ Vec4<S> pc_load(const V
 // at least (counters only grow).  A lane stops polling a counter once it has seen its target: with EXACT the counter cannot move on
 // before this item publishes, and either way the acquire of that poll orders the loads that follow it.
 // A watchdog bounds the spin (a schedule bug must not hang the device): after ~4M polls the warp gives up and raises
-// *watchdog, which the host turns into an error.
+// *watchdog, which the host turns into an error.  seen1 / seen2 (optional) receive the last value each lane's poll of that counter read.
 template <bool EXACT = true>
-__device__ __forceinline__ void wave_wait(const unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2, int* watchdog) {
+__device__ __forceinline__ void wave_wait(const unsigned* ver, bool need1, int b1, unsigned e1, bool need2, int b2, unsigned e2, int* watchdog,
+                                          unsigned* seen1 = nullptr, unsigned* seen2 = nullptr) {
     for (unsigned spins = 0;; ++spins) {
-        if (need1) { const unsigned v = ld_acquire(ver + b1); need1 = EXACT ? v != e1 : v < e1; }
-        if (need2) { const unsigned v = ld_acquire(ver + b2); need2 = EXACT ? v != e2 : v < e2; }
+        if (need1) { const unsigned v = ld_acquire(ver + b1); need1 = EXACT ? v != e1 : v < e1; if (seen1) *seen1 = v; }
+        if (need2) { const unsigned v = ld_acquire(ver + b2); need2 = EXACT ? v != e2 : v < e2; if (seen2) *seen2 = v; }
         if (__all_sync(0xffffffffu, !(need1 || need2))) break;
         if (spins > (1u << 22)) { *watchdog = 1; break; }
     }
@@ -399,9 +401,9 @@ __device__ __forceinline__ void stage_copy(Vec4<double>* dst, const Vec4<double>
 }
 // the tile only needs the rows of the widest manifold of the upload (single-point sphere contacts: a quarter of the tile, the rest
 // of the SM's shared-memory / L1 array stays L1)
-// (3 staged rows per point + 1 scratch row per point for its impulses + 1 row of separations: wave_contact_item)
+// (3 staged rows per point + 1 scratch row per point for its impulses: wave_contact_item)
 template <class S> __host__ __device__ constexpr size_t stage_bytes(int threads, int max_points = AVN_MAX_MANIFOLD_POINTS) {
-    return size_t(4 * max_points + 1) * threads * sizeof(Vec4<S>);
+    return size_t(4 * max_points) * threads * sizeof(Vec4<S>);
 }
 
 // Barrier schedules (grid-wide phases, phase kernels); the wavefront schedule runs wave_contact_item below.
@@ -585,13 +587,18 @@ __device__ __forceinline__ void contact_item(const DevSolver<S>& d, int slot) {
 
 // ---- wavefront mode: warm_start / solve_contacts<BIAS> / relax of ONE manifold --------------------------------------------------------
 // The same arithmetic in the same order as contact_item (bit-identical); what differs is where the operands live and when the item waits.
-//   * Rolled point loops.  Each point's impulses and separation live in this thread's scratch rows of the staging tile (rows 3*MAXP + k and
-//     4*MAXP), so no register array is indexed dynamically and nothing goes to local memory.  One routine serves the biased and the relax
-//     pass (`relax`): fewer routines compete for the SM's instruction cache, whose warps are in several routines at once.
+//   * Rolled point loops.  Each point's impulses live in this thread's scratch rows of the staging tile (rows 3*MAXP + k), so no register
+//     array is indexed dynamically and nothing goes to local memory.  One routine serves the biased and the relax pass (`relax`): fewer
+//     routines compete for the SM's instruction cache, whose warps are in several routines at once.
 //   * Two-stage wait (solve passes).  A body's deltas change only at its integrate_positions, so stage 1 waits until each body's counter has
 //     passed the integrate_positions event that wrote the deltas this pass reads — nearly always true at the first look — then loads them and
-//     computes every point's separation.  Stage 2 waits for the exact event and loads the velocities and impulses.  The two quaternion
-//     rotations per point are off the dependent chain.
+//     computes every point's separation and the velocity-independent coefficients of its normal impulse.  Stage 2 waits for the exact event
+//     (no poll for a lane whose stage-1 poll already read it) and loads the velocities and impulses.  When about as many warps are resident
+//     as a colour has chunks, a warp goes from one level's item straight to the next one's and stage 1 is on the chain, so it is kept short.
+//   * Branch-free normal part.  Every case of ContactNormalPart::solve_impulse is impulse = -M * (vn + B) - C, with M and B from stage 1 and
+//     C a select, so the lanes of a warp no longer run the separated, biased and relax paths one after another.
+//   * Early record stores.  A point's record is stored as soon as it is final (in the normal loop without friction, in the friction loop
+//     with it), so those stores are in flight during the rest of the arithmetic and the release fence mostly waits for the velocities.
 //   * Acquire / release counters (wave_wait / wave_publish): no membar after a successful poll, one fence before the counter stores.
 // PASS = PASS_WARM or PASS_SOLVE_BIAS.  Every lane of the warp must call this (warp-collective waits).  Counters count from the prepare
 // launch on, so `s` is the absolute substep index in every launch of a step.
@@ -607,11 +614,12 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
     const int b1 = as_int(hidx.x), b2 = as_int(hidx.y);
     Vec4<S>* const stage = stage_base<S>() + threadIdx.x;   // this thread's column; row r at stage[r * T]
     const int T = blockDim.x;
+    // Staged rows of point k.  Stage 1 of a solve pass overwrites the w lanes of A and B (the initial separation and the normal effective
+    // mass, which nothing after it reads) with the coefficients B and M of the point's normal impulse.
 #define ROW_A(k) stage[(3 * (k) + 0) * T]
 #define ROW_B(k) stage[(3 * (k) + 1) * T]
 #define ROW_D(k) stage[(3 * (k) + 2) * T]
 #define ROW_PC(k) stage[(3 * MAXP + (k)) * T]
-    S* const sepv = reinterpret_cast<S*>(&stage[(4 * MAXP) * T]);
     // ---- immutable part (planes written by prepare, inertia): issued before any wait
     Vec4<S> hn = mk4<S>(0, 0, 0, 0), ht1 = hn, htv = hn;
     BodyInertia<S> in1 = zero_inertia<S>(), in2 = zero_inertia<S>();
@@ -637,14 +645,19 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
     const unsigned e2 = wave_event(kind, it, s, d.iters, k2, (rk >> 16) & 0xff);
     int* const watchdog = d.any_restitution + FLAG_WAVE;
     const V3<S> n = xyz(hn), t1 = xyz(ht1);
+    const Soft<S> soft = (info & CI_NONDYN) ? d.soft_nondyn : d.soft_dyn;
+    unsigned biased_points = 0;   // bit k: point k takes the biased case (C = impulse_scale * accumulated impulse)
+    // the counter values stage 1's polls last read: a lane that already read its exact event there skips the first poll of stage 2 (the
+    // counter cannot pass that event before this item publishes, and the acquire of that poll orders every later load)
+    unsigned seen1 = 0u, seen2 = 0u;
 
-    // ---- stage 1 (solve passes): the deltas -> the separation of every point, before the velocities are waited for
+    // ---- stage 1 (solve passes): the deltas -> the separation of every point -> the coefficients of its normal impulse
     if (SOLVE) {
         AVN_TRACE_T(t_d0);
         const int sd = relax ? s : s - 1;   // the substep whose integrate_positions wrote the deltas this pass reads (-1: prepare did)
         if (sd >= 0)
             wave_wait<false>(d.ver, ver1, b1, wave_event(WV_IP, 0, sd, d.iters, k1, 0) + 1u, ver2, b2, wave_event(WV_IP, 0, sd, d.iters, k2, 0) + 1u,
-                             watchdog);
+                             watchdog, &seen1, &seen2);
         __pipeline_wait_prior(0);   // this thread's staged rows have landed (only the issuing thread reads them)
         if (np != 0) {
             const Vec4<S> dp1 = ld4_cg(&d.dlt[2 * b1]), dq1 = ld4_cg(&d.dlt[2 * b1 + 1]);
@@ -652,23 +665,37 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
             Q4<S> q1; q1.x = dq1.x; q1.y = dq1.y; q1.z = dq1.z; q1.w = dq1.w;
             Q4<S> q2; q2.x = dq2.x; q2.y = dq2.y; q2.z = dq2.z; q2.w = dq2.w;
             const V3<S> delta_translation = xyz(dp2) - xyz(dp1);
-#pragma unroll 1
-            for (int k = 0; k < np; ++k) {
+            // unrolled: the points are independent here, so their rotations and coefficients interleave instead of running one after another
+#pragma unroll
+            for (int k = 0; k < MAXP; ++k) {
+                if (k >= np) break;
                 const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k);
                 V3<S> rr1 = qrot(q1, xyz(PAk)), rr2 = qrot(q2, xyz(PBk));
                 V3<S> dsep = delta_translation + (rr2 - rr1);
-                sepv[k] = dot(dsep, n) + PAk.w;
+                const S separation = dot(dsep, n) + PAk.w;
+                // ContactNormalPart::solve_impulse (normal_part.rs:116-166) as impulse = -M * (vn + B) - C.  Per case, the operations of
+                // the reference in the same order:
+                //   separation > 0:  -meff * (vn + separation / h)                  M = meff,               B = separation / h,  C = +0
+                //   biased:          -scaled_mass * (vn + bias) - scaled_impulse     M = mass_scale * meff,  B = bias,            C = impulse_scale * acc
+                //   relax:           -meff * vn                                      M = meff,               B = -0,              C = +0
+                // with bias = max(soft.bias * separation, -max_overlap_speed).  The added operations are exact: x - (+0) == x and
+                // x + (-0) == x bit for bit for every x, -0 included.
+                const S meff = PBk.w;
+                const bool separated = separation > S(0), biased = !separated && !relax;
+                ROW_A(k).w = separated ? separation / d.h : biased ? avn_max(soft.bias * separation, -d.max_overlap_speed) : S(-0.0);   // B
+                ROW_B(k).w = biased ? soft.mass_scale * meff : meff;                                                                    // M
+                biased_points |= unsigned(biased) << k;
             }
         }
 #ifdef AVN_WAVE_TRACE
-        if (np != 0 && sepv[0] == S(1.2345e33)) d.any_restitution[1] = 2;   // the separations are done here
+        if (np != 0 && ROW_A(0).w == S(1.2345e33)) d.any_restitution[1] = 2;   // the coefficients are done here
         AVN_TRACE_ADD(d, 5, clock64() - t_d0);
 #endif
     }
 
     // ---- stage 2: the exact event, then the velocities of the two bodies and the impulses of the points
     AVN_TRACE_T(t_w0);
-    wave_wait(d.ver, ver1, b1, e1, ver2, b2, e2, watchdog);
+    wave_wait(d.ver, ver1 && seen1 != e1, b1, e1, ver2 && seen2 != e2, b2, e2, watchdog);
     AVN_TRACE_ADD(d, 0, clock64() - t_w0);
     if (np == 0) return;   // padding slot (after the warp-collective waits)
     AVN_TRACE_T(t_l0);
@@ -704,36 +731,27 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
         }
     } else {
         // ContactConstraint::solve (contact/mod.rs:267-354)
-        const Soft<S> soft = (info & CI_NONDYN) ? d.soft_nondyn : d.soft_dyn;
+        const bool tangent = (info & CI_TANGENT) != 0;
 #pragma unroll 1
         for (int k = 0; k < np; ++k) {
             const Vec4<S> PAk = ROW_A(k), PBk = ROW_B(k);
             Vec4<S> pck = ROW_PC(k);
             V3<S> r1 = xyz(PAk), r2 = xyz(PBk);
-            const S separation = sepv[k];
             V3<S> relv = (v2 + cross(w2, r2)) - (v1 + cross(w1, r1));
-            // ContactNormalPart::solve_impulse (normal_part.rs:116-166)
+            // ContactNormalPart::solve_impulse (normal_part.rs:116-166), M and B from stage 1
             S vn = dot(relv, n);
-            S meff = PBk.w, acc = pck.x;
-            S impulse;
-            if (separation > S(0)) {
-                impulse = -meff * (vn + separation / d.h);
-            } else if (!relax) {
-                S bias = avn_max(soft.bias * separation, -d.max_overlap_speed);
-                S scaled_mass = soft.mass_scale * meff;
-                S scaled_impulse = soft.impulse_scale * acc;
-                impulse = -scaled_mass * (vn + bias) - scaled_impulse;
-            } else {
-                impulse = -meff * vn;
-            }
+            S acc = pck.x;
+            const S C = ((biased_points >> k) & 1u) ? soft.impulse_scale * acc : S(0);
+            S impulse = -PBk.w * (vn + PAk.w) - C;
             S new_impulse = avn_max(acc + impulse, S(0));
             impulse = new_impulse - acc;
             pck.x = new_impulse;
             pck.y = pck.y + new_impulse;
-            ROW_PC(k) = pck;
+            if (tangent) ROW_PC(k) = pck;
+            else pc_store(pc_ptr(d, k, slot), pck);   // final: no friction part
             apply_impulse(v1, w1, v2, w2, in1, in2, r1, r2, impulse * n);
         }
-        if (info & CI_TANGENT) {
+        if (tangent) {
             const S friction = hn.w;
             const V3<S> surf = xyz(htv);
 #pragma unroll 1
@@ -761,23 +779,19 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
                     S dx = nx - pck.z, dy = ny - pck.w;
                     pck.z = nx;
                     pck.w = ny;
-                    ROW_PC(k) = pck;
                     imp = dx * t1 + dy * t2;
                 }
+                pc_store(pc_ptr(d, k, slot), pck);   // final
                 apply_impulse(v1, w1, v2, w2, in1, in2, r1, r2, imp);
             }
         }
     }
-    // ---- write back: impulses, the velocities of the non-dominant sides, then the counters
+    // ---- write back: the velocities of the non-dominant sides, then the counters
 #ifdef AVN_WAVE_TRACE
     if ((v1.x + v2.x + w1.x + w2.x) == S(1.2345e33)) d.any_restitution[1] = 2;
     AVN_TRACE_T(t_s0);
     AVN_TRACE_ADD(d, 2, t_s0 - t_c0);
 #endif
-    if (SOLVE) {
-#pragma unroll 1
-        for (int k = 0; k < np; ++k) pc_store(pc_ptr(d, k, slot), ROW_PC(k));
-    }
     if (!(info & CI_ZERO1)) {
         st4(&d.vel[2 * b1], mk4<S>(v1.x, v1.y, v1.z, S(0)));
         st4(&d.vel[2 * b1 + 1], mk4<S>(w1.x, w1.y, w1.z, S(0)));
@@ -786,7 +800,7 @@ __device__ __forceinline__ void wave_contact_item(const DevSolver<S>& d, int slo
         st4(&d.vel[2 * b2], mk4<S>(v2.x, v2.y, v2.z, S(0)));
         st4(&d.vel[2 * b2 + 1], mk4<S>(w2.x, w2.y, w2.z, S(0)));
     }
-    wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2);
+    wave_publish(d.ver, ver1, b1, e1, ver2, b2, e2);   // the fence also orders the record stores before the counters
 #ifdef AVN_WAVE_TRACE
     AVN_TRACE_ADD(d, 3, clock64() - t_s0);
     AVN_TRACE_ADD(d, 4, 1);
@@ -807,6 +821,19 @@ __device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, i
     int f = 0;
     if (in_range) f = as_int(ld4(&d.inr[2 * i]).y);
     const bool live = in_range && (f & BF_HAS_SOLVER_BODY);
+    // the immutable inputs are loaded before the wait: the poll's "memory" clobber would keep them behind it, one more round trip on the chain
+    const bool integrate = live && !(f & BF_CUSTOM_VEL) && !(f & BF_KINEMATIC), gyro = integrate && (f & BF_GYRO);
+    Vec4<S> li = mk4<S>(0, 0, 0, 0), ai = li;
+    Q4<S> rot0; rot0.x = rot0.y = rot0.z = rot0.w = S(0);
+    Sym3<S> il; il.m00 = il.m01 = il.m02 = il.m11 = il.m12 = il.m22 = S(0);
+    if (integrate) { li = ld4(&d.itg[2 * i]); ai = ld4(&d.itg[2 * i + 1]); }
+    if (gyro) {
+        rot0 = ldq(d.rotation, i);
+        il.m00 = d.inv_inertia_local[6 * i]; il.m01 = d.inv_inertia_local[6 * i + 1]; il.m02 = d.inv_inertia_local[6 * i + 2];
+        il.m11 = d.inv_inertia_local[6 * i + 3]; il.m12 = d.inv_inertia_local[6 * i + 4]; il.m22 = d.inv_inertia_local[6 * i + 5];
+    }
+    const S max_lin = live && d.max_lin ? d.max_lin[i] : S(0), max_ang = live && d.max_ang ? d.max_ang[i] : S(0);
+    const int bnd = live && d.bnd_of ? d.bnd_of[i] : -1;
     unsigned e = 0;
     if (WAVE) {
         if (live) e = wave_event(WV_IV, 0, s, d.iters, d.deg[i], 0);
@@ -816,20 +843,16 @@ __device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, i
     Vec4<S> l = ldm<WAVE>(&d.vel[2 * i]), a = ldm<WAVE>(&d.vel[2 * i + 1]);
     V3<S> v = xyz(l), w = xyz(a);
     bool touched = false;
-    if (!(f & BF_CUSTOM_VEL) && !(f & BF_KINEMATIC)) {
-        Vec4<S> li = ld4(&d.itg[2 * i]), ai = ld4(&d.itg[2 * i + 1]);
+    if (integrate) {
         v = v * li.w;
         w = w * ai.w;
         v = v + xyz(li);
         w = w + xyz(ai);
-        if (f & BF_GYRO) {
+        if (gyro) {
             // solve_gyroscopic_torque (integrator/mod.rs:403-460)
             Vec4<S> dq4 = ldm<WAVE>(&d.dlt[2 * i + 1]);
             Q4<S> dq; dq.x = dq4.x; dq.y = dq4.y; dq.z = dq4.z; dq.w = dq4.w;
-            Q4<S> rot = qmul(dq, ldq(d.rotation, i));
-            Sym3<S> il;
-            il.m00 = d.inv_inertia_local[6 * i]; il.m01 = d.inv_inertia_local[6 * i + 1]; il.m02 = d.inv_inertia_local[6 * i + 2];
-            il.m11 = d.inv_inertia_local[6 * i + 3]; il.m12 = d.inv_inertia_local[6 * i + 4]; il.m22 = d.inv_inertia_local[6 * i + 5];
+            Q4<S> rot = qmul(dq, rot0);
             V3<S> lw = qrot(qconj(rot), w);
             Sym3<S> tensor = sym_inverse_or_zero(il);
             V3<S> L = smul(tensor, lw);
@@ -845,25 +868,20 @@ __device__ __forceinline__ void integrate_velocity_item(const DevSolver<S>& d, i
         touched = true;
     }
     if (d.max_lin) {
-        S ms = d.max_lin[i];
         S l2 = len2(v);
-        if (avn_finite(ms) && l2 > ms * ms) { v = v * (ms / avn_sqrt(l2)); touched = true; }
+        if (avn_finite(max_lin) && l2 > max_lin * max_lin) { v = v * (max_lin / avn_sqrt(l2)); touched = true; }
     }
     if (d.max_ang) {
-        S ms = d.max_ang[i];
         S l2 = len2(w);
-        if (avn_finite(ms) && l2 > ms * ms) { w = w * (ms / avn_sqrt(l2)); touched = true; }
+        if (avn_finite(max_ang) && l2 > max_ang * max_ang) { w = w * (max_ang / avn_sqrt(l2)); touched = true; }
     }
     if (touched) {
         st4(&d.vel[2 * i], mk4<S>(v.x, v.y, v.z, S(0)));
         st4(&d.vel[2 * i + 1], mk4<S>(w.x, w.y, w.z, S(0)));
     }
-    if (d.bnd_of) {  // partitioned step: the reference point of this substep's constraint impulses on a boundary body
-        const int k = d.bnd_of[i];
-        if (k >= 0) {
-            st4(&d.vel_ref[2 * k], mk4<S>(v.x, v.y, v.z, S(0)));
-            st4(&d.vel_ref[2 * k + 1], mk4<S>(w.x, w.y, w.z, S(0)));
-        }
+    if (bnd >= 0) {  // partitioned step: the reference point of this substep's constraint impulses on a boundary body
+        st4(&d.vel_ref[2 * bnd], mk4<S>(v.x, v.y, v.z, S(0)));
+        st4(&d.vel_ref[2 * bnd + 1], mk4<S>(w.x, w.y, w.z, S(0)));
     }
     if (WAVE) wave_publish(d.ver, true, i, e, false, 0, 0u);
 }

@@ -1009,7 +1009,7 @@ AvnStatus Solver<S>::download() {
     {
         unsigned long long tr[8];
         cudaMemcpy(tr, dev_.any_restitution + FLAG_WORDS, sizeof tr, cudaMemcpyDeviceToHost);
-        if (tr[4]) fprintf(stderr, "[avn wave trace] contact item-warps %llu  avg cycles: stage 1 (wait deltas + separations) %.0f  wait %.0f  loads %.0f  compute %.0f  "
+        if (tr[4]) fprintf(stderr, "[avn wave trace] contact item-warps %llu  avg cycles: stage 1 (wait deltas + separations + coefficients) %.0f  wait %.0f  loads %.0f  compute %.0f  "
                            "store+publish %.0f\n", tr[4], double(tr[5]) / tr[4], double(tr[0]) / tr[4], double(tr[1]) / tr[4], double(tr[2]) / tr[4], double(tr[3]) / tr[4]);
     }
 #endif
