@@ -400,6 +400,29 @@ class AvnPointProjection(C.Structure):
     _fields_ = [(n, _vp) for n in ("collider", "point", "is_inside")]
 
 
+class AvnCcdConfig(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("body", "collider", "mode", "include_dynamic", "linear_threshold",
+                                                                                   "angular_threshold")] + [("prediction_distance", C.c_double)]
+
+
+class AvnCcdResult(C.Structure):
+    _fields_ = [(n, _vp) for n in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")] + [("pass_ms", C.c_float), ("total_candidates", C.c_uint32)]
+
+
+SWEEP_LINEAR, SWEEP_NON_LINEAR = 0, 1
+
+
+def ccd_config(body, collider, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
+               prediction_distance: float = float("inf")) -> tuple["AvnCcdConfig", tuple]:
+    """An AvnCcdConfig over numpy copies of the columns (returned alongside: they must outlive the struct's use)."""
+    cols = (np.ascontiguousarray(body, dtype=np.int32), np.ascontiguousarray(collider, dtype=np.uint32),
+            None if mode is None else np.ascontiguousarray(mode, dtype=np.uint8),
+            None if include_dynamic is None else np.ascontiguousarray(include_dynamic, dtype=np.uint8),
+            None if linear_threshold is None else np.ascontiguousarray(linear_threshold, dtype=np.float64),
+            None if angular_threshold is None else np.ascontiguousarray(angular_threshold, dtype=np.float64))
+    return AvnCcdConfig(int(cols[0].shape[0]), 0, *(_ptr(a) for a in cols), float(prediction_distance)), cols
+
+
 QUERY_SHAPES_UNCHANGED = 1
 MAX_HITS_ALL = 0xFFFFFFFF
 CAST_IGNORE_ORIGIN_PENETRATION = 0x1
@@ -464,6 +487,8 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "query_project_point": ([_vp, P(AvnPointBatch), P(AvnPointProjection)], C.c_int),
         "query_point_intersections": ([_vp, P(AvnPointBatch), P(AvnHitList)], C.c_int),
         "query_shape_intersections": ([_vp, P(AvnShapeBatch), P(AvnHitList)], C.c_int),
+        "ccd_configure": ([_vp, P(AvnCcdConfig)], C.c_int),
+        "ccd_download": ([_vp, P(AvnCcdResult)], C.c_int),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(lib, f"{prefix}_{name}")
@@ -481,7 +506,7 @@ ABI_SYMBOLS = [
     "avn_contacts_configure", "avn_contacts_step", "avn_solver_upload_resident", "avn_broadphase_download_order", "avn_contacts_download_graph",
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
-    "avn_query_shape_intersections"]
+    "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -1033,6 +1058,28 @@ class Context:
         self._check(self.lib.avn_islands_step(self.handle, C.byref(st)))
         for n in ("island_count", "sleeping_islands", "islands_put_to_sleep", "islands_woken", "split_bodies", "merges"):
             out[n] = int(getattr(st, n))
+        return out
+
+    # ---- swept CCD (include/avian_b200.h avn_ccd_*): solve_swept_ccd inside the device-resident solver stage
+    def ccd_configure(self, body=None, collider=None, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
+                      prediction_distance: float = float("inf")) -> None:
+        """avn_ccd_configure: the SweptCcd bodies in query order and their own colliders; body=None clears the configuration."""
+        if body is None or len(body) == 0:
+            self._check(self.lib.avn_ccd_configure(self.handle, None))
+            self._ccd_n = 0
+            return
+        cfg, cols = ccd_config(body, collider, mode, include_dynamic, linear_threshold, angular_threshold, prediction_distance)
+        self._check(self.lib.avn_ccd_configure(self.handle, C.byref(cfg)))
+        self._ccd_n = int(cfg.count)
+
+    def ccd_download(self) -> dict:
+        """avn_ccd_download: per configured body the last step's min_toi, hit_body, hit_contact, candidates, hits; plus pass_ms, total_candidates."""
+        n = getattr(self, "_ccd_n", 0)
+        out = {"min_toi": np.zeros(n, dtype=self.scalar), "hit_body": np.zeros(n, dtype=np.int32), "hit_contact": np.zeros(n, dtype=np.int32),
+               "candidates": np.zeros(n, dtype=np.uint32), "hits": np.zeros(n, dtype=np.uint32)}
+        r = AvnCcdResult(*(_ptr(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")), 0.0, 0)
+        self._check(self.lib.avn_ccd_download(self.handle, C.byref(r)))
+        out["pass_ms"], out["total_candidates"] = float(r.pass_ms), int(r.total_candidates)
         return out
 
     def contacts_download_impulses(self, capacity: int):

@@ -19,6 +19,7 @@ struct AvnContext {
     std::unique_ptr<avn::ContactsBase> contacts;
     std::unique_ptr<avn::QueriesBase> queries;
     std::unique_ptr<avn::CommBase> comm;
+    std::unique_ptr<avn::CcdBase> ccd;
     AvnTimings last{};
 };
 
@@ -86,11 +87,13 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
         ctx->contacts.reset(avn::make_contacts(config->scalar_bits, ctx->stream, &ctx->err));
         ctx->queries.reset(avn::make_queries(config->scalar_bits, ctx->stream, &ctx->err));
         ctx->comm.reset(avn::make_comm(ctx->stream, &ctx->err));
-        if (!ctx->solver || !ctx->broadphase || !ctx->aabbs || !ctx->narrow || !ctx->contacts || !ctx->queries) {
+        ctx->ccd.reset(avn::make_ccd(config->scalar_bits, ctx->stream, &ctx->err));
+        if (!ctx->solver || !ctx->broadphase || !ctx->aabbs || !ctx->narrow || !ctx->contacts || !ctx->queries || !ctx->ccd) {
             ctx.reset();   // the members hold the stream: release them before it goes
             cudaStreamDestroy(stream);
             return create_fail(AVN_ERR_UNSUPPORTED, "scalar type not available");
         }
+        ctx->solver->attach_ccd(ctx->ccd.get(), ctx->contacts.get());
         *out_ctx = ctx.release();
         return AVN_OK;
     } catch (...) {
@@ -105,6 +108,7 @@ void avn_destroy(AvnContext* ctx) {
     cudaStreamSynchronize(ctx->stream);
     ctx->comm.reset();
     ctx->solver.reset();
+    ctx->ccd.reset();
     ctx->broadphase.reset();
     ctx->aabbs.reset();
     ctx->narrow.reset();
@@ -312,6 +316,18 @@ AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* po
 }
 AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out) {
     return guarded(ctx, [&] { return ctx->queries->shape_intersections(shapes, out); });
+}
+
+// swept CCD (ccd.cu): solve_swept_ccd inside avn_solver_run
+AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
+    return guarded(ctx, [&] {
+        avn::CcdRows rows;
+        ctx->contacts->ccd_rows(&rows);
+        return ctx->ccd->configure(config, rows);
+    });
+}
+AvnStatus avn_ccd_download(AvnContext* ctx, AvnCcdResult* out) {
+    return guarded(ctx, [&] { return ctx->ccd->download(out); });
 }
 
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out) {

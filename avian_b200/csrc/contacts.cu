@@ -812,6 +812,14 @@ class Contacts final : public ContactsBase {
     }
 
     AvnStatus graph_view(ResidentGraph* out) override { *out = graph_; return AVN_OK; }
+    void ccd_rows(CcdRows* out) override {
+        out->rows = std::min(hw_, E_);
+        out->bodies = configured_ ? n_bodies_ : 0;
+        out->colliders = configured_ ? n_colliders_ : 0;
+        out->c1 = c1_.as<uint32_t>(); out->c2 = c2_.as<uint32_t>(); out->b1 = b1_.as<uint32_t>(); out->b2 = b2_.as<uint32_t>(); out->live = live_.as<uint8_t>();
+        out->shape = in_.shape;
+        out->dims = in_.dims;
+    }
     void pair_set(const uint64_t** table, uint64_t* mask) override {
         *table = (configured_ && table_.p && !table_dirty_) ? table_.as<uint64_t>() : nullptr;
         *mask = table_mask_;

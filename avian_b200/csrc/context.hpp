@@ -67,6 +67,8 @@ struct CommBase {
 CommBase* make_comm(cudaStream_t stream, ErrorSink* err);
 
 struct ContactsBase;
+struct CcdBase;
+struct CcdRows;
 struct SolverBase {
     virtual ~SolverBase() {}
     virtual AvnStatus upload(const AvnStepParams* prm, AvnBodyColumns* bodies, AvnManifoldColumns* manifolds, AvnJointSet* joints) = 0;
@@ -88,6 +90,9 @@ struct SolverBase {
     virtual AvnStatus prefetch_bodies(AvnBodyColumns* bodies, uint32_t flags) = 0;
     virtual AvnStatus download() = 0;
     virtual void timings(AvnTimings* t) const = 0;
+    // the context's CCD pass and the contact store it reads: avn_solver_run runs the pass between the substeps and restitution when the pass is
+    // configured and the upload came from the contact store
+    virtual void attach_ccd(CcdBase* ccd, ContactsBase* contacts) = 0;
 };
 // the new pairs of the last broad-phase run where the run left them (device memory); count is known on the host after the run settled
 struct DevicePairs {
@@ -167,8 +172,37 @@ struct ContactsBase {
     // ---- persistent simulation islands + sleeping decisions (contacts.cu)
     virtual AvnStatus islands_configure(const AvnIslandsConfig* cfg) = 0;
     virtual AvnStatus islands_step(AvnIslandsStep* step) = 0;
+    // ---- the rows and collider shapes swept CCD visits (ccd.cu)
+    virtual void ccd_rows(CcdRows* out) = 0;
 };
 ContactsBase* make_contacts(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
+
+// ---- swept CCD (ccd.cu): what the pass reads from the contact store and from the solver's step state (device pointers, column scalar)
+struct CcdRows {
+    uint32_t rows = 0;                 // ContactIds in use: [0, rows)
+    uint32_t bodies = 0, colliders = 0;   // avn_contacts_configure's counts (0 before it)
+    const uint32_t* c1 = nullptr; const uint32_t* c2 = nullptr; const uint32_t* b1 = nullptr; const uint32_t* b2 = nullptr;
+    const uint8_t* live = nullptr;
+    const uint8_t* shape = nullptr;    // [C] of the last avn_contacts_step (NULL = cuboid)
+    const void* dims = nullptr;        // [C][3]
+};
+struct CcdSolverState {
+    int B = 0;
+    double dt = 0, length_unit = 1;
+    const uint8_t* kind = nullptr;     // NULL = dynamic
+    const void* position = nullptr; const void* rotation = nullptr; const void* com = nullptr;   // pre-step pose, local centre of mass (NULL = 0)
+    void* vel = nullptr;               // Vec4 rows {lin}{ang} per body (solver_dev.cuh)
+    void* dlt = nullptr;               // Vec4 rows {delta_position}{delta_rotation}
+};
+struct CcdBase {
+    virtual ~CcdBase() {}
+    virtual AvnStatus configure(const AvnCcdConfig* cfg, const CcdRows& rows) = 0;
+    virtual bool active() const = 0;
+    // enqueued on the context's stream; adds its kernel launches to *launches
+    virtual AvnStatus run(const CcdSolverState& st, const CcdRows& rows, uint32_t* launches) = 0;
+    virtual AvnStatus download(AvnCcdResult* out) = 0;
+};
+CcdBase* make_ccd(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
 SolverBase* make_solver(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err, uint32_t cfg_flags, int device);
 BroadphaseBase* make_broadphase(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err, int device);

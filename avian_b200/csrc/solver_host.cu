@@ -102,6 +102,7 @@ class Solver final : public SolverBase {
     AvnStatus run() override;
     AvnStatus download() override;
     void timings(AvnTimings* t) const override { *t = tm_; }
+    void attach_ccd(CcdBase* ccd, ContactsBase* contacts) override { ccd_ = ccd; ccd_contacts_ = contacts; }
 
    private:
     static constexpr int kBlock = 256;
@@ -173,6 +174,12 @@ class Solver final : public SolverBase {
         return AVN_OK;
     }
     AvnStatus build_joint_schedule(const AvnBodyColumns& bc, const AvnJointSet& js);
+    AvnStatus launch_range(uint32_t first, uint32_t count, uint32_t flags);
+    bool ccd_active() const { return ccd_ && ccd_->active(); }
+    CcdBase* ccd_ = nullptr;
+    ContactsBase* ccd_contacts_ = nullptr;
+    bool from_store_ = false;     // the upload's manifolds are the contact store's rows (upload_graph / upload_resident): swept CCD can run
+    double length_unit_ = 1;
     template <int OP> void launch_phase(int begin, int count, bool serial = false) {
         if (count <= 0) return;
         int grid = serial ? 1 : std::min((count + kBlock - 1) / kBlock, sm_count_ * 8);
@@ -301,6 +308,7 @@ AvnStatus Solver<S>::build_joint_schedule(const AvnBodyColumns& bc, const AvnJoi
 
 template <class S>
 AvnStatus Solver<S>::upload(const AvnStepParams* prm, AvnBodyColumns* bc, AvnManifoldColumns* mc, AvnJointSet* js) {
+    from_store_ = false;
     if (!mc || mc->count == 0) return upload_impl(prm, bc, nullptr, js);
     if (!mc->body1 || !mc->body2 || !mc->normal || !mc->friction || !mc->restitution || !mc->point_offsets || !mc->anchor1 || !mc->anchor2 ||
         !mc->penetration || !mc->normal_speed || !mc->warm_start_normal_impulse || !mc->warm_start_tangent_impulse || !mc->normal_impulse)
@@ -317,6 +325,7 @@ AvnStatus Solver<S>::upload(const AvnStepParams* prm, AvnBodyColumns* bc, AvnMan
 
 template <class S>
 AvnStatus Solver<S>::upload_edges(const AvnStepParams* prm, AvnBodyColumns* bc, AvnEdgeManifolds* em, AvnJointSet* js) {
+    from_store_ = false;
     if (!em || em->count == 0) return upload_impl(prm, bc, nullptr, js);
     if (!em->edge || !em->body1 || !em->body2 || !em->friction || !em->restitution || !em->point_count || !em->normal || !em->anchor1 || !em->anchor2 ||
         !em->penetration || !em->normal_speed || !em->warm_start_normal_impulse || !em->warm_start_tangent_impulse || !em->normal_impulse)
@@ -336,6 +345,7 @@ AvnStatus Solver<S>::upload_edges(const AvnStepParams* prm, AvnBodyColumns* bc, 
 template <class S>
 AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* bc, ContactsBase* contacts, AvnJointSet* js) {
     if (!contacts) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: no contact store");
+    from_store_ = true;
     ContactsBase::ResidentGraph g;
     AvnStatus st = contacts->graph_view(&g);
     if (st != AVN_OK) return st;
@@ -359,6 +369,7 @@ AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* b
 
 template <class S>
 AvnStatus Solver<S>::upload_graph(const AvnStepParams* prm, AvnBodyColumns* bc, const AvnEdgeManifolds* g, ContactsBase* contacts, AvnJointSet* js) {
+    from_store_ = true;
     if (!g || g->count == 0) return upload_impl(prm, bc, nullptr, js);
     if (!contacts) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_graph: no contact store");
     // edge == NULL: "the graph has not changed since the last avn_solver_upload_graph" — the list stays on the device, only count and
@@ -429,6 +440,7 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
     d.match_contacts = int(prm->match_contacts);
     d.h = S(prm->h);
     d.dt = S(prm->dt);
+    length_unit_ = prm->length_unit;
     d.max_overlap_speed = S(prm->max_overlap_solve_speed) * S(prm->length_unit);
     d.warm_coeff = S(prm->warm_start_coefficient);
     d.rest_threshold = S(prm->restitution_threshold) * S(prm->length_unit);
@@ -665,13 +677,33 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
 
 template <class S>
 AvnStatus Solver<S>::run() {
-    return run_range(0, dev_.substeps, AVN_RUN_PREPARE | AVN_RUN_RESTITUTION | AVN_RUN_FINALIZE);
+    if (!ccd_active()) return launch_range(0, dev_.substeps, AVN_RUN_PREPARE | AVN_RUN_RESTITUTION | AVN_RUN_FINALIZE);
+    // swept CCD (ccd.cu) runs after the substeps and before restitution (ccd/mod.rs:257-261): the step is split around it
+    if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run before avn_solver_upload");
+    if (!from_store_ || !ccd_contacts_)
+        return err_->fail(AVN_ERR_UNSUPPORTED, "swept CCD is configured: it needs the contact store's ContactGraph (avn_solver_upload_resident / avn_solver_upload_graph), "
+                                               "not host manifolds");
+    AvnStatus st = launch_range(0, uint32_t(dev_.substeps), AVN_RUN_PREPARE);
+    if (st != AVN_OK) return st;
+    CcdRows rows;
+    ccd_contacts_->ccd_rows(&rows);
+    CcdSolverState s;
+    s.B = dev_.B; s.dt = double(dev_.dt); s.length_unit = length_unit_;
+    s.kind = dev_.kind; s.position = dev_.position; s.rotation = dev_.rotation; s.com = dev_.com; s.vel = dev_.vel; s.dlt = dev_.dlt;
+    if ((st = ccd_->run(s, rows, &launches_)) != AVN_OK) return st;
+    return launch_range(uint32_t(dev_.substeps), 0, AVN_RUN_RESTITUTION | AVN_RUN_FINALIZE);
+}
+
+template <class S>
+AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
+    if (ccd_active()) return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run_range: swept CCD is configured (avn_solver_run runs the split step itself)");
+    return launch_range(first, count, flags);
 }
 
 // One launch covering: prepare (flags & AVN_RUN_PREPARE), substeps [first, first + count), the restitution pass, the finalize phases.
 // avn_solver_run is the whole step in one launch; the x-slab partition launches substep by substep with a boundary exchange in between.
 template <class S>
-AvnStatus Solver<S>::run_range(uint32_t first, uint32_t count, uint32_t flags) {
+AvnStatus Solver<S>::launch_range(uint32_t first, uint32_t count, uint32_t flags) {
     if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run before avn_solver_upload");
     const bool prepare = (flags & AVN_RUN_PREPARE) != 0;
     if (!prepare && !prepared_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run_range: the first launch after an upload must include AVN_RUN_PREPARE");
@@ -928,6 +960,7 @@ AvnStatus Solver<S>::boundary_apply(const void* device_gathered) {
 template <class S>
 AvnStatus Solver<S>::step_partitioned(CommBase* comm) {
     if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_step_partitioned before avn_solver_upload");
+    if (ccd_active()) return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_step_partitioned: swept CCD is not supported in the x-slab partition");
     if (!comm) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "no communicator");
     const int world = comm->world();
     if (bnd_slots_ > 0 && (bnd_world_ != world || bnd_rank_ != comm->rank()))

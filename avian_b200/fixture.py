@@ -62,6 +62,14 @@ def _load():
         for f in (lib.avh_query_cast_ray, lib.avh_query_ray_hits, lib.avh_query_aabb_intersections, lib.avh_query_cast_shape, lib.avh_query_shape_hits,
                   lib.avh_query_project_point, lib.avh_query_point_intersections, lib.avh_query_shape_intersections):
             f.restype = C.c_int
+        lib.avh_ccd_solve.argtypes = [C.c_uint32, C.c_double, C.c_double, C.c_uint32] + [_vp] * 10 + [C.c_uint32] + [_vp] * 5 + [P(api.AvnCcdConfig)] + [_vp] * 5
+        lib.avh_ccd_solve.restype = C.c_int
+        lib.avh_ccd_pair_toi.argtypes = [C.c_uint32, C.c_int, _vp, _vp, C.c_double, C.c_double, C.c_double]
+        lib.avh_ccd_pair_toi.restype = C.c_double
+        lib.avh_ccd_nonlinear_toi.argtypes = [_vp, _vp, C.c_double, C.c_double, P(C.c_double), P(C.c_int)]
+        lib.avh_ccd_nonlinear_toi.restype = C.c_int
+        lib.avh_ccd_apply_record.argtypes = [C.c_uint32, C.c_double, _vp, _vp, _vp, _vp]
+        lib.avh_ccd_apply_record.restype = None
         _lib = lib
     return _lib
 
@@ -301,3 +309,60 @@ class HostPipeline:
     @property
     def pair_count(self) -> int:
         return int(self.lib.avh_pair_count(self.h))
+
+
+# ---- swept CCD (csrc/ccd_math.hpp): the host brute force the device pass is compared with ----------------------------------------------------
+def ccd_motion(shape: int, dims, position, rotation, linear_velocity=(0, 0, 0), angular_velocity=(0, 0, 0), com=(0, 0, 0)) -> np.ndarray:
+    """One body of a CCD pair as the 20 doubles avh_ccd_pair_toi takes."""
+    return np.concatenate([[float(shape)], np.asarray(dims, float).reshape(3), np.asarray(position, float).reshape(3), np.asarray(rotation, float).reshape(4),
+                           np.asarray(com, float).reshape(3), np.asarray(linear_velocity, float).reshape(3), np.asarray(angular_velocity, float).reshape(3)])
+
+
+def ccd_pair_toi(scalar, mode: int, a: np.ndarray, b: np.ndarray, dt: float, eps: float = 1e-4, prediction_distance: float = float("inf")) -> float:
+    """compute_ccd_toi of one pair against the bound dt, rounded to the column scalar (-1 = no hit)."""
+    a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
+    return _load().avh_ccd_pair_toi(32 if np.dtype(scalar) == np.float32 else 64, int(mode), a.ctypes.data, b.ctypes.data, float(dt), float(eps),
+                                    float(prediction_distance))
+
+
+def ccd_nonlinear_toi(a: np.ndarray, b: np.ndarray, t_max: float, eps: float = 1e-4, iterations: bool = False):
+    """The raw conservative-advancement TOI in double, or None; with iterations=True, (TOI or None, distance evaluations)."""
+    a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
+    t, its = C.c_double(), C.c_int(0)
+    hit = _load().avh_ccd_nonlinear_toi(a.ctypes.data, b.ctypes.data, float(t_max), float(eps), C.byref(t), C.byref(its))
+    out = t.value if hit else None
+    return (out, its.value) if iterations else out
+
+
+def ccd_apply_record(scalar, m: float, v, w, dp, dq):
+    """The delta write of one CCD record (overwrite dp, compose from_scaled_axis(w m) onto dq) in the column scalar; returns (dp, dq)."""
+    v, w = np.ascontiguousarray(v, dtype=np.float64), np.ascontiguousarray(w, dtype=np.float64)
+    dp, dq = np.array(dp, dtype=np.float64), np.array(dq, dtype=np.float64)
+    _load().avh_ccd_apply_record(32 if np.dtype(scalar) == np.float32 else 64, float(m), v.ctypes.data, w.ctypes.data, dp.ctypes.data, dq.ctypes.data)
+    return dp, dq
+
+
+def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, rows: dict, cfg: dict, delta_position=None, delta_rotation=None) -> dict:
+    """solve_swept_ccd over the contact rows (dict c1, c2, b1, b2, live) by the reference's sequential loop.  bodies: dict kind, position,
+    rotation, linear_velocity, angular_velocity (SolverBody velocities after the substeps), center_of_mass (optional).  cfg: the keyword
+    arguments of api.ccd_config.  delta_position / delta_rotation are updated in place when given.  Returns what Context.ccd_download returns."""
+    lib, dt_ = _load(), np.dtype(scalar)
+    col = lambda a, t=dt_: None if a is None else np.ascontiguousarray(a, dtype=t)
+    kind = col(bodies.get("kind"), np.uint8)
+    pos, rot, com, lv, av = (col(bodies.get(k)) for k in ("position", "rotation", "center_of_mass", "linear_velocity", "angular_velocity"))
+    B = int(pos.shape[0])
+    sh, dm = col(shape, np.uint8), col(dims)
+    c1, c2, b1, b2 = (col(rows[k], np.uint32) for k in ("c1", "c2", "b1", "b2"))
+    live = col(rows["live"], np.uint8)
+    conf, keep = api.ccd_config(**cfg)
+    n = int(conf.count)
+    out = {"min_toi": np.zeros(n, dtype=dt_), "hit_body": np.zeros(n, dtype=np.int32), "hit_contact": np.zeros(n, dtype=np.int32),
+           "candidates": np.zeros(n, dtype=np.uint32), "hits": np.zeros(n, dtype=np.uint32)}
+    for a in (delta_position, delta_rotation):
+        assert a is None or (a.dtype == dt_ and a.flags["C_CONTIGUOUS"])
+    st = lib.avh_ccd_solve(32 if dt_ == np.float32 else 64, float(dt), float(length_unit), B, _p(kind), _p(pos), _p(rot), _p(com), _p(lv), _p(av),
+                           _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
+                           *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
+    if st != 0:
+        raise ValueError("avh_ccd_solve: invalid configuration")
+    return out

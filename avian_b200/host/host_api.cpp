@@ -9,6 +9,7 @@
 //     constraint_graph.rs:163-296)
 //   * export of the manifolds as per-colour columns in the layout of AvnManifoldColumns.
 //   * spatial queries by brute force over every collider (csrc/query_math.hpp): the checker of the device tree (csrc/queries.cu).
+//   * swept CCD as the reference's sequential loop (csrc/ccd_math.hpp): the checker of the device pass (csrc/ccd.cu).
 // It contains no solver or broad-phase code: those are the GPU library (product) or oracle/ (tests).
 #include <algorithm>
 #include <cmath>
@@ -23,6 +24,7 @@
 #include "../csrc/narrow_math.hpp"
 #include "../csrc/contact_rows.hpp"
 #include "../csrc/query_math.hpp"
+#include "../csrc/ccd_math.hpp"
 
 namespace {
 
@@ -902,6 +904,152 @@ int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders*
                 per[i].push_back(col);
     }
     return write_list(out, per);
+}
+
+}  // extern "C"
+
+// ---- swept CCD: solve_swept_ccd (dynamics/ccd/mod.rs:523-687) as the reference's sequential loop over the configured bodies, each scanning the
+//      live rows that hold its collider in ascending ContactId with the strict `<` — the checker of csrc/ccd.cu -------------------------------
+namespace {
+
+template <class T>
+ccd::Motion ccd_motion(const T* shape_dims, const uint8_t* shape, uint32_t c, const T* pos, const T* rot, const T* com, ccd::V3T<T> v, ccd::V3T<T> w, uint32_t b) {
+    ccd::Motion m;
+    m.shape = shape ? shape[c] : SHAPE_CUBOID;
+    m.he = V3{S(shape_dims[3 * c]), S(shape_dims[3 * c + 1]), S(shape_dims[3 * c + 2])};
+    m.p = V3{S(pos[3 * b]), S(pos[3 * b + 1]), S(pos[3 * b + 2])};
+    m.q = Q{S(rot[4 * b]), S(rot[4 * b + 1]), S(rot[4 * b + 2]), S(rot[4 * b + 3])};
+    m.lc = com ? V3{S(com[3 * b]), S(com[3 * b + 1]), S(com[3 * b + 2])} : V3{0, 0, 0};
+    m.v = V3{S(v.x), S(v.y), S(v.z)};
+    m.w = V3{S(w.x), S(w.y), S(w.z)};
+    return m;
+}
+
+template <class T>
+int ccd_solve(double dt_d, double length_unit, uint32_t B, const uint8_t* kind, const T* pos, const T* rot, const T* com, const T* lv, const T* av, T* dpos,
+              T* drot, const uint8_t* shape, const T* dims, uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2,
+              const uint8_t* live, const AvnCcdConfig* cfg, T* out_min, int32_t* out_body, int32_t* out_contact, uint32_t* out_cand, uint32_t* out_hits) {
+    const T dt = T(dt_d);
+    const S eps = ccd::CCD_EPS_PER_LENGTH_UNIT * length_unit;
+    auto kind_of = [&](uint32_t b) { return kind ? kind[b] : uint8_t(AVN_BODY_DYNAMIC); };
+    auto has_sb = [&](uint32_t b) { return b < B && kind_of(b) != AVN_BODY_STATIC; };
+    auto vel = [&](uint32_t b, const T* col) { return has_sb(b) ? ccd::V3T<T>{col[3 * b], col[3 * b + 1], col[3 * b + 2]} : ccd::V3T<T>{T(0), T(0), T(0)}; };
+    std::unordered_map<uint32_t, size_t> slot_of_body;
+    for (size_t k = 0; k < cfg->count; ++k) slot_of_body[uint32_t(cfg->body[k])] = k;
+    auto mode_of = [&](size_t k) { return cfg->mode ? int(cfg->mode[k]) : ccd::MODE_NON_LINEAR; };
+    // each CCD collider's rows in ascending ContactId (the visiting order whose first minimum the strict `<` keeps)
+    std::unordered_map<uint32_t, std::vector<uint32_t>> adjacency;
+    for (size_t k = 0; k < cfg->count; ++k) adjacency[cfg->collider[k]];
+    for (uint32_t e = 0; e < rows; ++e) {
+        if (!live[e]) continue;
+        auto a = adjacency.find(c1[e]);
+        if (a != adjacency.end()) a->second.push_back(e);
+        if (c2[e] != c1[e] && (a = adjacency.find(c2[e])) != adjacency.end()) a->second.push_back(e);
+    }
+    for (size_t k = 0; k < cfg->count; ++k) {
+        const uint32_t body1 = uint32_t(cfg->body[k]), own = cfg->collider[k];
+        T min_toi = dt;
+        int32_t hit = -1, hit_row = -1;
+        uint32_t cand = 0, hits = 0;
+        if (has_sb(body1)) {
+            const T lthr = T(cfg->linear_threshold ? cfg->linear_threshold[k] : 0.0), athr = T(cfg->angular_threshold ? cfg->angular_threshold[k] : 0.0);
+            const bool include_dynamic = cfg->include_dynamic ? cfg->include_dynamic[k] != 0 : true;
+            for (const uint32_t e : adjacency[own]) {
+                const bool first = c1[e] == own;
+                const uint32_t other = first ? c2[e] : c1[e], body2 = first ? b2[e] : b1[e];
+                if (body2 >= B || body2 == body1) continue;
+                if (!include_dynamic && kind_of(body2) == AVN_BODY_DYNAMIC) continue;
+                const ccd::V3T<T> v1 = vel(body1, lv), w1 = vel(body1, av), v2 = vel(body2, lv), w2 = vel(body2, av);
+                if (ccd::below_thresholds<T>(v1, w1, v2, w2, lthr, athr)) continue;
+                const auto it = slot_of_body.find(body2);
+                const int mode = (mode_of(k) == ccd::MODE_LINEAR && (it == slot_of_body.end() || mode_of(it->second) == ccd::MODE_LINEAR)) ? ccd::MODE_LINEAR
+                                                                                                                                      : ccd::MODE_NON_LINEAR;
+                ++cand;
+                const T t = ccd::pair_toi<T>(mode, ccd_motion(dims, shape, own, pos, rot, com, v1, w1, body1),
+                                             ccd_motion(dims, shape, other, pos, rot, com, v2, w2, body2), dt, eps, cfg->prediction_distance);
+                if (t > T(0) && t < dt) ++hits;
+                if (t > T(0) && t < min_toi) { min_toi = t; hit = int32_t(body2); hit_row = int32_t(e); }
+            }
+        }
+        if (out_min) out_min[k] = min_toi;
+        if (out_body) out_body[k] = hit;
+        if (out_contact) out_contact[k] = hit_row;
+        if (out_cand) out_cand[k] = cand;
+        if (out_hits) out_hits[k] = hits;
+        if (hit < 0 || !dpos || !drot) continue;
+        // application, in list order (ccd/mod.rs:620-670)
+        const T m = ccd::overshoot(min_toi);
+        for (int side = 0; side < 2; ++side) {
+            const uint32_t b = side == 0 ? body1 : uint32_t(hit);
+            if (!has_sb(b)) continue;   // the dummy SolverBody: writes are discarded
+            ccd::V3T<T> dp{dpos[3 * b], dpos[3 * b + 1], dpos[3 * b + 2]};
+            ccd::QT<T> dq{drot[4 * b], drot[4 * b + 1], drot[4 * b + 2], drot[4 * b + 3]};
+            ccd::apply_record(m, vel(b, lv), vel(b, av), dp, dq);
+            dpos[3 * b] = dp.x; dpos[3 * b + 1] = dp.y; dpos[3 * b + 2] = dp.z;
+            drot[4 * b] = dq.x; drot[4 * b + 1] = dq.y; drot[4 * b + 2] = dq.z; drot[4 * b + 3] = dq.w;
+        }
+    }
+    return 0;
+}
+
+ccd::Motion motion_from(const double* m) {   // shape, he[3], p[3], q[4], local com[3], v[3], w[3]
+    ccd::Motion r;
+    r.shape = int(m[0]);
+    r.he = V3{m[1], m[2], m[3]}; r.p = V3{m[4], m[5], m[6]}; r.q = Q{m[7], m[8], m[9], m[10]}; r.lc = V3{m[11], m[12], m[13]};
+    r.v = V3{m[14], m[15], m[16]}; r.w = V3{m[17], m[18], m[19]};
+    return r;
+}
+
+}  // namespace
+
+extern "C" {
+
+// solve_swept_ccd over the given contact rows.  Velocities: the SolverBody velocities after the substeps; delta_position / delta_rotation
+// ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration.
+int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position, const void* rotation,
+                  const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation, const uint8_t* shape, const void* dims,
+                  uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2, const uint8_t* live, const AvnCcdConfig* cfg,
+                  void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates, uint32_t* hits) {
+    if (!cfg || (cfg->count && (!cfg->body || !cfg->collider))) return -1;
+    if (scalar_bits == 64)
+        return ccd_solve<double>(dt, length_unit, body_count, kind, static_cast<const double*>(position), static_cast<const double*>(rotation),
+                                 static_cast<const double*>(com), static_cast<const double*>(linvel), static_cast<const double*>(angvel),
+                                 static_cast<double*>(delta_position), static_cast<double*>(delta_rotation), shape, static_cast<const double*>(dims), rows, c1, c2,
+                                 b1, b2, live, cfg, static_cast<double*>(min_toi), hit_body, hit_contact, candidates, hits);
+    return ccd_solve<float>(dt, length_unit, body_count, kind, static_cast<const float*>(position), static_cast<const float*>(rotation),
+                            static_cast<const float*>(com), static_cast<const float*>(linvel), static_cast<const float*>(angvel),
+                            static_cast<float*>(delta_position), static_cast<float*>(delta_rotation), shape, static_cast<const float*>(dims), rows, c1, c2, b1,
+                            b2, live, cfg, static_cast<float*>(min_toi), hit_body, hit_contact, candidates, hits);
+}
+
+// One pair's compute_ccd_toi against the bound dt (ccd::pair_toi, fallback included), rounded to the column scalar and returned as a double;
+// -1 = no hit.  Motions: 20 doubles each (shape, half extents / radius, position, rotation, local com, linear and angular velocity).
+double avh_ccd_pair_toi(uint32_t scalar_bits, int mode, const double* a, const double* b, double dt, double eps, double prediction_distance) {
+    if (scalar_bits == 64) return ccd::pair_toi<double>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance);
+    return double(ccd::pair_toi<float>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance));
+}
+
+// The raw non-linear TOI in double (no rounding, no fallback): 1 and *toi on a hit, 0 otherwise; *iterations = distance evaluations.
+int avh_ccd_nonlinear_toi(const double* a, const double* b, double t_max, double eps, double* toi, int* iterations) {
+    double t = 0;
+    const bool hit = ccd::nonlinear_toi(motion_from(a), motion_from(b), t_max, eps, t, iterations);
+    *toi = t;
+    return hit ? 1 : 0;
+}
+
+// Quat::from_scaled_axis and the delta write of one record, in the column scalar (tests)
+void avh_ccd_apply_record(uint32_t scalar_bits, double m, const double* v, const double* w, double* dp, double* dq) {
+    if (scalar_bits == 64) {
+        ccd::V3T<double> p{dp[0], dp[1], dp[2]};
+        ccd::QT<double> q{dq[0], dq[1], dq[2], dq[3]};
+        ccd::apply_record<double>(m, {v[0], v[1], v[2]}, {w[0], w[1], w[2]}, p, q);
+        dp[0] = p.x; dp[1] = p.y; dp[2] = p.z; dq[0] = q.x; dq[1] = q.y; dq[2] = q.z; dq[3] = q.w;
+        return;
+    }
+    ccd::V3T<float> p{float(dp[0]), float(dp[1]), float(dp[2])};
+    ccd::QT<float> q{float(dq[0]), float(dq[1]), float(dq[2]), float(dq[3])};
+    ccd::apply_record<float>(float(m), {float(v[0]), float(v[1]), float(v[2])}, {float(w[0]), float(w[1]), float(w[2])}, p, q);
+    dp[0] = p.x; dp[1] = p.y; dp[2] = p.z; dq[0] = q.x; dq[1] = q.y; dq[2] = q.z; dq[3] = q.w;
 }
 
 }  // extern "C"

@@ -186,8 +186,12 @@ def _slot_of(plugin) -> str:
 class World:
     """A headless world: body columns + the CPU fixture around the hot path + the plugin group."""
 
-    def __init__(self, scene: Scene, plugins: PhysicsPlugins, dt: float = 1.0 / 60.0, substeps: int = 6, solver_iterations: int = 1):
+    def __init__(self, scene: Scene, plugins: PhysicsPlugins, dt: float = 1.0 / 60.0, substeps: int = 6, solver_iterations: int = 1,
+                 ccd: dict | None = None):
+        """ccd: the SweptCcd bodies — the keyword arguments of api.Context.ccd_configure (body, collider, mode, include_dynamic,
+        linear_threshold, angular_threshold, prediction_distance).  The solver plugin must run solve_swept_ccd (a `step_ccd` method)."""
         self.scene = scene
+        self.ccd = ccd
         self.bodies = scene.bodies
         self.joints = scene.joints
         self.scalar = scene.bodies.position.dtype
@@ -221,7 +225,13 @@ class World:
 
     def solve(self) -> None:
         m = self.last_manifolds
-        self.plugins.get("SolverPlugin").step(self.params, self.bodies, m, self.joints)
+        solver = self.plugins.get("SolverPlugin")
+        if self.ccd is not None:
+            if not hasattr(solver, "step_ccd"):
+                raise ValueError(f"{type(solver).__name__} does not run swept CCD: on the GPU it needs the device-resident pipeline (DeviceGraphWorld)")
+            solver.step_ccd(self.params, self.bodies, m, self.joints, self.ccd, self.pipeline.active_edges(), self.scene.shape_type, self.scene.dims)
+        else:
+            solver.step(self.params, self.bodies, m, self.joints)
         if m is not None and m.count:
             self.pipeline.store_impulses(m)
 
@@ -450,6 +460,8 @@ class DeviceGraphWorld(World):
         self._dims = np.ascontiguousarray(scene.dims, dtype=self.scalar)
         self._order_out = np.empty(n, dtype=np.uint32)
         self._uploaded_once = False     # from the second step on the static columns (shapes, mass properties ...) stay on the device
+        if self.ccd is not None:
+            ctx.ccd_configure(**self.ccd)   # solve_swept_ccd inside the device-resident solver stage
 
     def intervals(self, aabb_min: np.ndarray, aabb_max: np.ndarray) -> api.Aabbs:
         o, kind = self.order, self.bodies.kind

@@ -743,6 +743,54 @@ AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* po
  * The cast-only columns of the batch are ignored. */
 AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out);
 
+/* ---- swept continuous collision detection (SweptCcd, dynamics/ccd/mod.rs:523-780) on the device-resident solver stage ----------------
+ *      Replaces solve_swept_ccd, which the reference runs after the substeps and before solve_restitution: for every SweptCcd body, in the
+ *      order of the configured list, every collider adjacent to its own collider in the ContactGraph (every live contact row, touching or
+ *      not) is a candidate.  Filters in the reference's order: a dynamic body 2 is skipped unless include_dynamic; the pair is skipped when
+ *      |w1 - w2|^2 < angular_threshold^2 and |v1 - v2|^2 < linear_threshold^2.  The sweep is Linear when body 1 is Linear and body 2 has no
+ *      configured entry or is Linear too, otherwise NonLinear.  A TOI counts when 0 < toi < min_toi (min_toi starts at dt); a TOI of exactly
+ *      0 is cast again against a ball of radius prediction_distance at body 2's pose.  The body of the smallest TOI is the hit; then
+ *      m = min_toi * 1.0001 and, for body 1 and for body 2 when it has a SolverBody (dynamic or kinematic): delta_position = m * v
+ *      (overwritten), delta_rotation = from_scaled_axis(w * m) * delta_rotation.  Velocities are never changed.  The writes happen in the
+ *      order of the configured list, so a body hit by several CCD bodies ends with the last one's delta_position.
+ *      Assumptions, as the narrow phase makes them: a collider sits at its body's origin and its pose is the body's pose before the step; the
+ *      body columns and the collider rows of the contact pipeline (avn_contacts_configure / avn_contacts_step) describe the same bodies.
+ *      Geometry: cuboid and sphere colliders, conventions in avian_b200/csrc/ccd_math.hpp (linear: the shape casts of the spatial queries;
+ *      non-linear: conservative advancement to eps = 1e-4 * length_unit, at most 64 iterations).
+ *      Stated deviation: equal TOIs go to the lowest ContactId, where the reference keeps the first in ContactGraph adjacency order.
+ *      Runs inside avn_solver_run when the upload came from the contact store (avn_solver_upload_resident / avn_solver_upload_graph): the
+ *      step becomes prepare + substeps -> CCD pass -> restitution + finalize.  While CCD is configured, avn_solver_run_range,
+ *      avn_solver_step_partitioned and a run after avn_solver_upload / avn_solver_upload_edges / avn_solver_step return AVN_ERR_UNSUPPORTED. */
+typedef enum AvnSweepMode { AVN_SWEEP_LINEAR = 0, AVN_SWEEP_NON_LINEAR = 1 } AvnSweepMode;
+
+typedef struct AvnCcdConfig {
+    uint32_t count;                    /* SweptCcd bodies, in query order */
+    uint32_t _pad;
+    const int32_t* body;               /* [n] index into AvnBodyColumns; no body twice */
+    const uint32_t* collider;          /* [n] the body's own collider: a row of the contact pipeline's collider columns */
+    const uint8_t* mode;               /* [n] AvnSweepMode; NULL = AVN_SWEEP_NON_LINEAR (SweptCcd::default) */
+    const uint8_t* include_dynamic;    /* [n] NULL = 1 */
+    const double* linear_threshold;    /* [n] NULL = 0 */
+    const double* angular_threshold;   /* [n] NULL = 0 */
+    double prediction_distance;        /* NarrowPhaseConfig::default_speculative_margin * PhysicsLengthUnit (default Scalar::MAX: pass +inf) */
+} AvnCcdConfig;
+
+typedef struct AvnCcdResult {          /* per configured body, the last step's pass; any pointer may be NULL */
+    void* min_toi;                     /* [n] column scalar: the smallest accepted TOI before the overshoot, dt when nothing was hit */
+    int32_t* hit_body;                 /* [n] the body hit, -1 = none */
+    int32_t* hit_contact;              /* [n] ContactId of the hit, -1 = none */
+    uint32_t* candidates;              /* [n] candidates that passed the filters (TOIs computed) */
+    uint32_t* hits;                    /* [n] candidates with an accepted TOI (0 < toi < dt) */
+    float pass_ms;                     /* out: device time of the pass */
+    uint32_t total_candidates;         /* out */
+} AvnCcdResult;
+
+/* Persists across steps; NULL or count == 0 clears it.  Needs avn_contacts_configure first (bodies and colliders are checked against its counts).
+ * Refused with AVN_ERR_INVALID_ARGUMENT: bodies or colliders out of range, a body listed twice, NaN thresholds, an unknown mode. */
+AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config);
+/* The results of the last step that ran the pass (AVN_ERR_INVALID_ARGUMENT before any). */
+AvnStatus avn_ccd_download(AvnContext* ctx, AvnCcdResult* out);
+
 AvnStatus avn_get_timings(const AvnContext* ctx, AvnTimings* out);
 
 /*
