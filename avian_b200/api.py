@@ -400,6 +400,19 @@ class AvnPointProjection(C.Structure):
     _fields_ = [(n, _vp) for n in ("collider", "point", "is_inside")]
 
 
+class AvnCollisionEvents(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [(n, _vp) for n in ("collider1", "collider2", "body1", "body2", "flags")]
+
+
+class AvnContactReport(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [
+        (n, _vp) for n in ("contact_id", "collider1", "collider2", "body1", "body2", "flags", "point_count", "normal", "total_normal_impulse",
+                           "max_normal_impulse", "max_penetration")]
+
+
+REPORT_EVENTS_ONLY = 0x1
+
+
 class AvnCcdConfig(C.Structure):
     _fields_ = [("count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("body", "collider", "mode", "include_dynamic", "linear_threshold",
                                                                                    "angular_threshold")] + [("prediction_distance", C.c_double)]
@@ -489,6 +502,10 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "query_shape_intersections": ([_vp, P(AvnShapeBatch), P(AvnHitList)], C.c_int),
         "ccd_configure": ([_vp, P(AvnCcdConfig)], C.c_int),
         "ccd_download": ([_vp, P(AvnCcdResult)], C.c_int),
+        "contacts_set_sensors": ([_vp, C.c_uint32, _vp], C.c_int),
+        "contacts_remove_colliders": ([_vp, C.c_uint32, _vp], C.c_int),
+        "contacts_events": ([_vp, P(AvnCollisionEvents), P(AvnCollisionEvents)], C.c_int),
+        "contacts_report": ([_vp, C.c_uint32, P(AvnContactReport)], C.c_int),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(lib, f"{prefix}_{name}")
@@ -506,7 +523,8 @@ ABI_SYMBOLS = [
     "avn_contacts_configure", "avn_contacts_step", "avn_solver_upload_resident", "avn_broadphase_download_order", "avn_contacts_download_graph",
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
-    "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download"]
+    "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download", "avn_contacts_set_sensors", "avn_contacts_remove_colliders",
+    "avn_contacts_events", "avn_contacts_report"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -701,6 +719,27 @@ def hit_list(n: int, capacity: int, scalar, ray: bool) -> tuple["AvnHitList", di
 def hit_list_result(h: "AvnHitList", out: dict) -> dict:
     total = int(h.count)
     return {k: (v if k == "offsets" else v[:total]) for k, v in out.items()}
+
+
+EVENT_COLUMNS = (("collider1", np.uint32), ("collider2", np.uint32), ("body1", np.uint32), ("body2", np.uint32), ("flags", np.uint8))
+
+
+def collision_events(capacity: int) -> tuple["AvnCollisionEvents", dict]:
+    """An AvnCollisionEvents over fresh numpy arrays of `capacity` entries (returned alongside: they must outlive the struct's use)."""
+    cap = max(int(capacity), 0)
+    out = {k: np.zeros(max(cap, 1), dtype=d) for k, d in EVENT_COLUMNS}
+    return AvnCollisionEvents(cap, 0, *(_ptr(out[k]) for k, _ in EVENT_COLUMNS)), out
+
+
+def contact_report(capacity: int, scalar) -> tuple["AvnContactReport", dict]:
+    """An AvnContactReport over fresh numpy arrays of `capacity` entries, scalars in `scalar` (returned alongside: they must outlive the
+    struct's use)."""
+    cap = max(int(capacity), 1)
+    out = {k: np.zeros(cap, dtype=np.uint32) for k in ("contact_id", "collider1", "collider2", "body1", "body2")}
+    out.update({"flags": np.zeros(cap, dtype=np.uint8), "point_count": np.zeros(cap, dtype=np.uint8), "normal": np.zeros((cap, 3), dtype=scalar)})
+    out.update({k: np.zeros(cap, dtype=scalar) for k in ("total_normal_impulse", "max_normal_impulse", "max_penetration")})
+    r = AvnContactReport(max(int(capacity), 0), 0, *(_ptr(out[n]) for n, _ in AvnContactReport._fields_[2:]))
+    return r, out
 
 
 def aabb_params(dt: float, contact_tolerance: float = 0.005, default_speculative_margin: float = float("inf")) -> "AvnAabbParams":
@@ -1081,6 +1120,52 @@ class Context:
         self._check(self.lib.avn_ccd_download(self.handle, C.byref(r)))
         out["pass_ms"], out["total_candidates"] = float(r.pass_ms), int(r.total_candidates)
         return out
+
+    # ---- the pipeline's output to the application (include/avian_b200.h avn_contacts_set_sensors / _remove_colliders / _events / _report)
+    def contacts_set_sensors(self, sensor, collider_count: int | None = None) -> None:
+        """avn_contacts_set_sensors: the Sensor flag per collider (None = no sensor; then collider_count is required)."""
+        col = None if sensor is None else np.ascontiguousarray(sensor, dtype=bool).astype(np.uint8)
+        n = int(col.shape[0]) if collider_count is None else int(collider_count)
+        self._check(self.lib.avn_contacts_set_sensors(self.handle, n, _ptr(col)))
+
+    def contacts_remove_colliders(self, colliders) -> None:
+        """avn_contacts_remove_colliders: remove_collider for each listed collider (despawned, disabled)."""
+        ids = np.ascontiguousarray(colliders, dtype=np.uint32)
+        self._check(self.lib.avn_contacts_remove_colliders(self.handle, int(ids.shape[0]), _ptr(ids)))
+
+    def contacts_events(self, capacity: int | None = None) -> tuple[dict, dict]:
+        """avn_contacts_events: (started, ended) of the last avn_contacts_step, each a dict of numpy columns collider1, collider2, body1, body2,
+        flags.  capacity=None retries once with the required sizes; an explicit capacity that is too small raises AvianError(ERR_CAPACITY)
+        with .required = (started, ended)."""
+        cap = 256 if capacity is None else int(capacity)
+        (s, so), (e, eo) = collision_events(cap), collision_events(cap)
+        st = self.lib.avn_contacts_events(self.handle, C.byref(s), C.byref(e))
+        if st == ERR_CAPACITY and capacity is None:
+            (s, so), (e, eo) = collision_events(int(s.count)), collision_events(int(e.count))
+            st = self.lib.avn_contacts_events(self.handle, C.byref(s), C.byref(e))
+        if st == ERR_CAPACITY:
+            err = AvianError(st, self.lib.avn_last_error(self.handle).decode())
+            err.required = (int(s.count), int(e.count))
+            raise err
+        self._check(st)
+        return ({k: v[:int(s.count)] for k, v in so.items()}, {k: v[:int(e.count)] for k, v in eo.items()})
+
+    def contacts_report(self, events_only: bool = False, capacity: int | None = None) -> dict:
+        """avn_contacts_report: one entry per touching pair in ascending ContactId (contact_id, collider1, collider2, body1, body2, flags,
+        point_count, normal, total_normal_impulse, max_normal_impulse, max_penetration).  Capacity protocol as contacts_events."""
+        cap = 1024 if capacity is None else int(capacity)
+        flags = REPORT_EVENTS_ONLY if events_only else 0
+        r, out = contact_report(cap, self.scalar)
+        st = self.lib.avn_contacts_report(self.handle, flags, C.byref(r))
+        if st == ERR_CAPACITY and capacity is None:
+            r, out = contact_report(int(r.count), self.scalar)
+            st = self.lib.avn_contacts_report(self.handle, flags, C.byref(r))
+        if st == ERR_CAPACITY:
+            err = AvianError(st, self.lib.avn_last_error(self.handle).decode())
+            err.required = int(r.count)
+            raise err
+        self._check(st)
+        return {k: v[:int(r.count)] for k, v in out.items()}
 
     def contacts_download_impulses(self, capacity: int):
         wn, wt, ni = (np.zeros((capacity, 4), dtype=self.scalar), np.zeros((capacity, 4, 2), dtype=self.scalar), np.zeros((capacity, 4), dtype=self.scalar))

@@ -282,6 +282,33 @@ AvnStatus avn_contacts_download_graph(AvnContext* ctx, uint32_t capacity, uint32
                                       uint32_t* edge_list) {
     return guarded(ctx, [&] { return ctx->contacts->download_graph(capacity, collider1, collider2, live, touching, colour, edge_list); });
 }
+// the pipeline's output to the application (contacts.cu): a removal rebuilds the pair set, which the next broad phase filters against
+AvnStatus avn_contacts_set_sensors(AvnContext* ctx, uint32_t collider_count, const uint8_t* sensor) {
+    return guarded(ctx, [&] {
+        AvnStatus st = ctx->contacts->set_sensors(collider_count, sensor);
+        const uint64_t* table = nullptr;
+        uint64_t mask = 0;
+        ctx->contacts->pair_set(&table, &mask);
+        ctx->broadphase->set_existing_device(table, mask);
+        return st;
+    });
+}
+AvnStatus avn_contacts_remove_colliders(AvnContext* ctx, uint32_t n, const uint32_t* colliders) {
+    return guarded(ctx, [&] {
+        AvnStatus st = ctx->contacts->remove_colliders(n, colliders);
+        const uint64_t* table = nullptr;
+        uint64_t mask = 0;
+        ctx->contacts->pair_set(&table, &mask);
+        ctx->broadphase->set_existing_device(table, mask);
+        return st;
+    });
+}
+AvnStatus avn_contacts_events(AvnContext* ctx, AvnCollisionEvents* started, AvnCollisionEvents* ended) {
+    return guarded(ctx, [&] { return ctx->contacts->events(started, ended); });
+}
+AvnStatus avn_contacts_report(AvnContext* ctx, uint32_t flags, AvnContactReport* out) {
+    return guarded(ctx, [&] { return ctx->contacts->report(flags, out); });
+}
 AvnStatus avn_islands_configure(AvnContext* ctx, const AvnIslandsConfig* config) { return guarded(ctx, [&] { return ctx->contacts->islands_configure(config); }); }
 AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step) { return guarded(ctx, [&] { return ctx->contacts->islands_step(step); }); }
 AvnStatus avn_contacts_download_impulses(AvnContext* ctx, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse) {

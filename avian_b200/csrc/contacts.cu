@@ -57,6 +57,8 @@ struct GraphRows {
     uint8_t* pflags; uint8_t* touching; uint8_t* colour /* 0 = none, c + 1 */; uint8_t* change; uint8_t* old_colour;
     uint8_t* fresh;                               // the row was added in this step (its geometry is still to be computed)
     uint8_t* isl_event;                           // this step's event for the islands: ISL_ADD / ISL_REMOVE (a linked contact came or went)
+    uint8_t* event;                               // this step's collision event: EV_STARTED / EV_ENDED | the pair's AVN_PAIR_* flags (0 = none)
+    const uint8_t* sensor;                        // [C] Sensor per collider (avn_contacts_set_sensors); NULL = none
     uint32_t* ovf_pos; uint32_t* ovf;
     const uint8_t* body_kind; int n_bodies;
     uint32_t* body_bits;                          // [B] bit c: the body is in colour c's body set
@@ -80,7 +82,9 @@ __global__ void add_rows_kernel(GraphRows g, uint32_t n_new, const uint32_t* __r
         return;
     }
     g.c1[e] = pc1[k]; g.c2[e] = pc2[k]; g.b1[e] = pb1[k]; g.b2[e] = pb2[k];
-    g.pflags[e] = pfl[k];
+    // a pair that involves a sensor never generates constraints (narrow_phase/system_param.rs:583-599)
+    const bool sensor = g.sensor && (g.sensor[pc1[k]] | g.sensor[pc2[k]]);
+    g.pflags[e] = sensor ? uint8_t(pfl[k] & ~AVN_PAIR_GENERATE_CONSTRAINTS) : pfl[k];
     g.isl_event[e] = 0;
     g.fresh[e] = 1;
     g.live[e] = 1;            // a ContactId handed to a new pair starts without history
@@ -95,32 +99,41 @@ __global__ void free_keys_kernel(const uint8_t* __restrict__ live, int n, uint32
     vals[e] = uint32_t(e);
 }
 
+// the collision event of a row (GraphRows::event): the transition bit plus the pair's AVN_PAIR_* flags (bits 0-3), captured when the row changes
+// (finalize_rows_kernel clears the flags of a removed row and the next step may hand its ContactId to a new pair)
+enum { EV_STARTED = 0x40, EV_ENDED = 0x80, EV_FLAGS = 0x0f };
+
 // the touching state machine of one row -> its change for the graphs
 __global__ void classify_kernel(GraphRows g, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= g.hw) return;
-    uint8_t ch = CH_NONE, ev = ISL_NONE;
+    uint8_t ch = CH_NONE, ev = ISL_NONE, cev = 0;
     if (g.live[e]) {
-        const bool gen = (g.pflags[e] & AVN_PAIR_GENERATE_CONSTRAINTS) != 0;
+        const uint8_t pf = g.pflags[e];
+        const bool gen = (pf & AVN_PAIR_GENERATE_CONSTRAINTS) != 0;
         if (g.disjoint[e]) {
             ch = CH_REMOVE | (g.colour[e] ? 0 : CH_DONE);
             atomicAdd(&g.ctr->removed, 1u);
+            if (g.touching[e]) cev = EV_ENDED | pf;       // CollisionEnd (system_param.rs:155-170)
             if (gen && g.touching[e]) ev = ISL_REMOVE;    // PhysicsIslands::remove_contact (system_param.rs:196-205)
         } else {
             const bool now = g.count[e] > 0, was = g.touching[e] != 0;
             if (now && !was) {
                 g.touching[e] = 1;
                 atomicAdd(&g.ctr->started, 1u);
+                cev = EV_STARTED | pf;                     // CollisionStart (system_param.rs:208-218)
                 if (gen) { ch = CH_PUSH; ev = ISL_ADD; }   // add_contact (system_param.rs:244-258)
             } else if (!now && was) {
                 g.touching[e] = 0;
                 atomicAdd(&g.ctr->stopped, 1u);
+                cev = EV_ENDED | pf;                       // CollisionEnd (system_param.rs:263-273)
                 if (gen && g.colour[e]) ch = CH_POP;
                 if (gen) ev = ISL_REMOVE;                  // remove_contact (system_param.rs:306-313)
             }
         }
     }
     g.isl_event[e] = ev;
+    g.event[e] = cev;
     g.change[e] = ch;
     if (ch) atomicAdd(&g.ctr->changed, 1u);
     keys[e] = ch ? 0u : 1u;
@@ -350,6 +363,89 @@ __global__ void pair_set_kernel(GraphRows g, uint64_t* __restrict__ table, uint6
     }
 }
 
+// =====================================================================================================================================
+// The contact pipeline's output to the application (DESIGN.md §7f): collision events, contact reports and the removal of colliders.
+//   Events: classify_kernel leaves one byte per row (GraphRows::event); avn_contacts_events turns the bytes into the started and ended lists in
+//     ascending ContactId with one stable radix pass (key 0 = started, 1 = ended, 2 = none) and a gather.
+//   Removal (remove_collider, narrow_phase/mod.rs:399-459): every live row that names a removed collider is popped from its colour, unlinked from
+//     its island, queued as a CollisionEnd when it was touching and freed; then the colour-major list and the pair set are rebuilt by the
+//     step's own kernels.
+//   Reports: the touching rows in ascending ContactId with their manifold reduced in slot order.
+// =====================================================================================================================================
+__global__ void event_keys_kernel(const uint8_t* __restrict__ event, int n, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const uint8_t v = event[e];
+    keys[e] = (v & EV_STARTED) ? 0u : (v & EV_ENDED) ? 1u : 2u;
+    vals[e] = uint32_t(e);
+}
+// key 0 = a touching row the report lists
+__global__ void report_keys_kernel(GraphRows g, uint32_t flags, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= g.hw) return;
+    const bool sel = g.live[e] && g.touching[e] && (!(flags & AVN_REPORT_EVENTS_ONLY) || (g.pflags[e] & AVN_PAIR_CONTACT_EVENTS));
+    keys[e] = sel ? 0u : 1u;
+    vals[e] = uint32_t(e);
+}
+// out[k - 1] = lower bound of key k in the sorted keys, k = 1 .. nb
+__global__ void key_bounds_kernel(const uint32_t* __restrict__ sorted_keys, int n, int nb, uint32_t* __restrict__ out) {
+    const int k = threadIdx.x + 1;
+    if (k > nb) return;
+    int lo = 0, hi = n;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (sorted_keys[mid] < uint32_t(k)) lo = mid + 1; else hi = mid; }
+    out[k - 1] = uint32_t(lo);
+}
+// An event list in device memory, N entries as columns: u32 collider1[N], collider2[N], body1[N], body2[N], then u8 flags[N].
+// Entry i < n_started of the sorted rows goes to slot i, the rest (the step's ended rows) behind the `skip` queued CollisionEnds.
+__global__ void event_gather_kernel(GraphRows g, const uint32_t* __restrict__ list, uint32_t n_started, uint32_t n, uint32_t skip, uint32_t N,
+                                    uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t e = list[i], j = i < n_started ? i : i + skip;
+    out[j] = g.c1[e]; out[N + j] = g.c2[e]; out[2 * size_t(N) + j] = g.b1[e]; out[3 * size_t(N) + j] = g.b2[e];
+    reinterpret_cast<uint8_t*>(out + 4 * size_t(N))[j] = g.event[e] & EV_FLAGS;
+}
+__global__ void mark_colliders_kernel(const uint32_t* __restrict__ ids, uint32_t n, uint8_t* __restrict__ removed) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) removed[ids[k]] = 1;
+}
+// the CollisionEnds of the touching removed rows (the first n of the sorted list) appended to the pending list (layout of event_gather_kernel,
+// capacity cap) behind its `base` entries
+__global__ void queue_ends_kernel(GraphRows g, const uint32_t* __restrict__ list, uint32_t n, uint32_t base, uint32_t cap, uint32_t* __restrict__ pend) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t e = list[i], j = base + i;
+    pend[j] = g.c1[e]; pend[cap + j] = g.c2[e]; pend[2 * size_t(cap) + j] = g.b1[e]; pend[3 * size_t(cap) + j] = g.b2[e];
+    reinterpret_cast<uint8_t*>(pend + 4 * size_t(cap))[j] = g.pflags[e] & EV_FLAGS;
+}
+// One report entry per listed row, columns of n entries: S normal[n][3], total[n], max[n], penetration[n]; u32 contact_id[n], collider1[n],
+// collider2[n], body1[n], body2[n]; u8 flags[n], point_count[n].  The points are reduced in slot order in S, so a sequential host loop in the
+// same type gives the same bits.  Only a row in the ConstraintGraph was solved: any other row (a sensor pair) reports 0 impulses.
+template <class S>
+__global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ list, uint32_t n, const S* __restrict__ normal, const S* __restrict__ pen,
+                                     const S* __restrict__ nimp, void* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t e = list[i];
+    S* os = static_cast<S*>(out);
+    uint32_t* ou = reinterpret_cast<uint32_t*>(os + 6 * size_t(n));
+    uint8_t* ob = reinterpret_cast<uint8_t*>(ou + 5 * size_t(n));
+    const int cnt = g.count[e];
+    const bool solved = g.colour[e] != 0;
+    S total = S(0), mx = S(0), deep = S(0);
+    for (int k = 0; k < cnt; ++k) {
+        const S v = solved ? nimp[4 * size_t(e) + k] : S(0);
+        total = total + v;
+        if (v > mx) mx = v;
+        const S p = pen[4 * size_t(e) + k];
+        if (k == 0 || p >= deep) deep = p;
+    }
+    for (int c = 0; c < 3; ++c) os[3 * size_t(i) + c] = normal[3 * size_t(e) + c];
+    os[3 * size_t(n) + i] = total; os[4 * size_t(n) + i] = mx; os[5 * size_t(n) + i] = deep;
+    ou[i] = e; ou[n + i] = g.c1[e]; ou[2 * size_t(n) + i] = g.c2[e]; ou[3 * size_t(n) + i] = g.b1[e]; ou[4 * size_t(n) + i] = g.b2[e];
+    ob[i] = g.pflags[e] & EV_FLAGS; ob[n + i] = uint8_t(cnt);
+}
+
 __global__ void edge_add_kernel(int n, const uint32_t* __restrict__ ids, const uint32_t* __restrict__ c1, const uint32_t* __restrict__ c2,
                                 const uint32_t* __restrict__ b1, const uint32_t* __restrict__ b2, uint32_t* rc1, uint32_t* rc2, uint32_t* rb1, uint32_t* rb2,
                                 uint8_t* live, uint8_t* count, uint8_t* prev_count) {
@@ -568,6 +664,45 @@ __global__ void isl_finish_kernel(IslandState s, uint32_t* __restrict__ out_isla
     }
 }
 
+// remove_collider for every live row that names a removed collider: pop its manifold from its colour (pops only clear bits: one pass does them
+// all; the overflow colour's list is fixed by overflow_list_kernel), remove_contact on its island when it was a touching, constraint-generating
+// contact (islands: 0 = not configured, 1 = the last step's island events were applied, 2 = they are still pending: a contact that avn_islands_step
+// has not linked yet is not unlinked either) and mark it CH_REMOVE for finalize_rows_kernel.
+// keys: 0 = removed while touching (a CollisionEnd to queue), 1 = removed, 2 = kept.
+__global__ void remove_rows_kernel(GraphRows g, const uint8_t* __restrict__ removed, IslandState s, int islands, uint32_t* __restrict__ keys,
+                                   uint32_t* __restrict__ vals) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= g.hw) return;
+    uint8_t ch = CH_NONE;
+    uint32_t key = 2;
+    if (g.live[e] && (removed[g.c1[e]] | removed[g.c2[e]])) {
+        ch = CH_REMOVE;
+        const bool touching = g.touching[e] != 0;
+        key = touching ? 0u : 1u;
+        atomicAdd(&g.ctr->removed, 1u);
+        atomicAdd(&g.ctr->changed, 1u);
+        if (touching) atomicAdd(&g.ctr->stopped, 1u);
+        const uint32_t b1 = g.b1[e], b2 = g.b2[e];
+        const int c = int(g.colour[e]) - 1;
+        g.old_colour[e] = g.colour[e];
+        if (c == AVN_COLOR_OVERFLOW) {
+            g.ctr->ovf_dirty = 1;
+        } else if (c >= 0) {
+            if (!graph_static(g, b1)) atomicAnd(&g.body_bits[b1], ~(1u << c));
+            if (!graph_static(g, b2)) atomicAnd(&g.body_bits[b2], ~(1u << c));
+        }
+        g.colour[e] = 0;
+        if (islands == 2 && g.isl_event[e] == ISL_ADD) {
+            g.isl_event[e] = ISL_NONE;
+        } else if (islands && touching && (g.pflags[e] & AVN_PAIR_GENERATE_CONSTRAINTS)) {
+            const uint32_t x = !isl_static(s, b1) ? b1 : b2;
+            if (!isl_static(s, x)) atomicAdd(&s.removed[s.root[x]], 1u);
+        }
+    }
+    g.change[e] = ch;
+    keys[e] = key;
+    vals[e] = uint32_t(e);
+}
 template <class S>
 class Contacts final : public ContactsBase {
    public:
@@ -598,7 +733,8 @@ class Contacts final : public ContactsBase {
                       {&prev_a2_, 12 * sizeof(double)}, {&ws_n_in_, 4 * sizeof(S)}, {&ws_t_in_, 8 * sizeof(S)}, {&ws_n_out_, 4 * sizeof(S)},
                       {&ws_t_out_, 8 * sizeof(S)}, {&nimp_in_, 4 * sizeof(S)}, {&nimp_out_, 4 * sizeof(S)},
                       // graph state per row (zero = no flags, not touching, no colour)
-                      {&pflags_, 1}, {&touching_, 1}, {&colour_, 1}, {&change_, 1}, {&old_colour_, 1}, {&ovf_pos_, 4}, {&ovf_, 4}, {&isl_event_, 1}, {&fresh_, 1}};
+                      {&pflags_, 1}, {&touching_, 1}, {&colour_, 1}, {&change_, 1}, {&old_colour_, 1}, {&ovf_pos_, 4}, {&ovf_, 4}, {&isl_event_, 1}, {&fresh_, 1},
+                      {&event_, 1}};
         for (Col& c : cols) {   // grow, keep the old rows, zero the new ones
             void* fresh = nullptr;
             AVN_CUDA(cudaMalloc(&fresh, n * c.bytes_per_row));
@@ -613,6 +749,7 @@ class Contacts final : public ContactsBase {
         // work buffers of the graph step (contents do not outlive a step) and the pair set (rebuilt by the next step)
         const size_t nblocks = (n + RS_TILE - 1) / RS_TILE;
         AVN_CUDA(k0_.ensure(n * 4)); AVN_CUDA(k1_.ensure(n * 4)); AVN_CUDA(v0_.ensure(n * 4)); AVN_CUDA(v1_.ensure(n * 4)); AVN_CUDA(list_.ensure(n * 4));
+        AVN_CUDA(evl_.ensure(n * 4));
         AVN_CUDA(hist_.ensure(256 * nblocks * 4));
         AVN_CUDA(m_b1_.ensure(n * 4)); AVN_CUDA(m_b2_.ensure(n * 4)); AVN_CUDA(m_fr_.ensure(n * sizeof(S))); AVN_CUDA(m_re_.ensure(n * sizeof(S)));
         uint64_t cap = 1024;
@@ -690,6 +827,7 @@ class Contacts final : public ContactsBase {
         AVN_CUDA(cudaStreamSynchronize(stream_));   // the host arrays may be reused by the caller
         configured_ = true;
         graph_ = ResidentGraph{};
+        sensor_h_.clear();                          // a (re)configuration starts without sensors
         return AVN_OK;
     }
 
@@ -722,6 +860,9 @@ class Contacts final : public ContactsBase {
         if (n_new64 > 0x7fffffffull - hw_) return err_->fail(AVN_ERR_CAPACITY, "contacts_step: too many contact pairs");
         const uint32_t n_new = uint32_t(n_new64);
         added_this_step_ = n_new > 0;
+        // the CollisionEnds queued by removals since the previous step are reported with this step's events; a new queue starts
+        pend_cur_ ^= 1;
+        pend_n_[pend_cur_] = 0;
         if (hw_ + n_new > E_ || E_ == 0) {
             if (prefetched_) AVN_CUDA(cudaStreamWaitEvent(stream_, ev_in_, 0));   // the early narrow pass writes the rows that are about to move
             AvnStatus st = reserve(std::max<uint32_t>(1024u, std::max(2 * E_, hw_ + n_new + 1024u)));
@@ -808,6 +949,116 @@ class Contacts final : public ContactsBase {
         graph_.count = h_ctr_->manifolds; graph_.any_restitution = h_ctr_->any_restitution;
         memcpy(graph_.color_offsets, h_ctr_->color_offsets, sizeof graph_.color_offsets);
         graph_.edge = v1_.as<uint32_t>(); graph_.body1 = m_b1_.as<int32_t>(); graph_.body2 = m_b2_.as<int32_t>(); graph_.friction = m_fr_.p; graph_.restitution = m_re_.p;
+        stepped_ = true;
+        isl_pending_ = true;
+        return AVN_OK;
+    }
+
+    // ---- collision events, sensors, removal of colliders, contact reports -----------------------------------------------------------
+    AvnStatus set_sensors(uint32_t collider_count, const uint8_t* sensor) override {
+        if (!configured_) return err_->fail(AVN_ERR_UNSUPPORTED, "contacts_set_sensors before avn_contacts_configure");
+        if (collider_count != n_colliders_)
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_set_sensors: %u colliders, configured %u", collider_count, n_colliders_);
+        std::vector<uint8_t> now(n_colliders_, 0);
+        if (sensor) for (uint32_t c = 0; c < n_colliders_; ++c) now[c] = sensor[c] ? 1 : 0;
+        std::vector<uint32_t> changed;   // On<Add, Sensor> / On<Remove, Sensor>: remove_collider for every collider whose flag changed
+        for (uint32_t c = 0; c < n_colliders_; ++c)
+            if (now[c] != (c < sensor_h_.size() ? sensor_h_[c] : 0)) changed.push_back(c);
+        const bool any = std::find(now.begin(), now.end(), uint8_t(1)) != now.end();
+        if (any) {
+            AVN_CUDA(sensor_.ensure(n_colliders_));
+            AVN_CUDA(cudaMemcpyAsync(sensor_.p, now.data(), n_colliders_, cudaMemcpyHostToDevice, stream_));
+            AVN_CUDA(cudaStreamSynchronize(stream_));
+        }
+        sensor_h_ = any ? std::move(now) : std::vector<uint8_t>();   // no sensor: add_rows_kernel sees NULL, as before any call
+        if (!stepped_ || changed.empty()) return AVN_OK;
+        return remove_rows(uint32_t(changed.size()), changed.data());
+    }
+
+    AvnStatus remove_colliders(uint32_t n, const uint32_t* colliders) override {
+        if (!stepped_) return err_->fail(AVN_ERR_UNSUPPORTED, "contacts_remove_colliders: no avn_contacts_step has run on this context");
+        if (n && !colliders) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_remove_colliders: colliders are required");
+        for (uint32_t k = 0; k < n; ++k)
+            if (colliders[k] >= n_colliders_)
+                return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_remove_colliders: collider %u >= the configured %u: nothing removed", colliders[k], n_colliders_);
+        return remove_rows(n, colliders);
+    }
+
+    AvnStatus events(AvnCollisionEvents* started, AvnCollisionEvents* ended) override {
+        if (!stepped_) return err_->fail(AVN_ERR_UNSUPPORTED, "contacts_events: no avn_contacts_step has run on this context");
+        const int rep = pend_cur_ ^ 1;
+        const uint32_t n_pend = pend_n_[rep];
+        uint32_t bounds[2] = {0, 0};
+        if (hw_) {
+            event_keys_kernel<<<(hw_ + 255) / 256, 256, 0, stream_>>>(event_.as<uint8_t>(), int(hw_), k0_.as<uint32_t>(), v0_.as<uint32_t>());
+            radix_pass(int(hw_), evl_.as<uint32_t>());   // started rows, then ended rows, each in ascending ContactId
+            const AvnStatus st = small_bounds(2, bounds);
+            if (st != AVN_OK) return st;
+        }
+        const uint32_t n_s = bounds[0], n_e = bounds[1] - bounds[0];
+        const bool short_s = started && started->capacity < n_s, short_e = ended && ended->capacity < uint64_t(n_pend) + n_e;
+        if (started) started->count = n_s;
+        if (ended) ended->count = uint64_t(n_pend) + n_e;
+        if (short_s || short_e)
+            return err_->fail(AVN_ERR_CAPACITY, "contacts_events: %u started / %u ended events exceed the capacities", n_s, n_pend + n_e);
+        const uint32_t N = n_s + n_pend + n_e;
+        if (N == 0) return AVN_OK;
+        AVN_CUDA(evout_.ensure(size_t(N) * 17));
+        uint32_t* o = evout_.as<uint32_t>();
+        if (n_s + n_e)
+            event_gather_kernel<<<(n_s + n_e + 255) / 256, 256, 0, stream_>>>(graph_rows(), evl_.as<uint32_t>(), n_s, n_s + n_e, n_pend, N, o);
+        AVN_CUDA(cudaGetLastError());
+        if (n_pend) {   // the queued CollisionEnds of the removals, in call order, head the ended list
+            const uint32_t* p = pend_[rep].as<uint32_t>();
+            const size_t cap = pend_cap_[rep];
+            for (int c = 0; c < 4; ++c)
+                AVN_CUDA(cudaMemcpyAsync(o + size_t(c) * N + n_s, p + c * cap, size_t(n_pend) * 4, cudaMemcpyDeviceToDevice, stream_));
+            AVN_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(o + 4 * size_t(N)) + n_s, reinterpret_cast<const uint8_t*>(p + 4 * cap), n_pend,
+                                     cudaMemcpyDeviceToDevice, stream_));
+        }
+        struct { AvnCollisionEvents* list; uint32_t first, count; } parts[2] = {{started, 0, n_s}, {ended, n_s, n_pend + n_e}};
+        for (auto& part : parts) {
+            if (!part.list || !part.count) continue;
+            uint32_t* cols[4] = {part.list->collider1, part.list->collider2, part.list->body1, part.list->body2};
+            for (int c = 0; c < 4; ++c)
+                if (cols[c]) AVN_CUDA(cudaMemcpyAsync(cols[c], o + size_t(c) * N + part.first, size_t(part.count) * 4, cudaMemcpyDeviceToHost, stream_));
+            if (part.list->flags)
+                AVN_CUDA(cudaMemcpyAsync(part.list->flags, reinterpret_cast<uint8_t*>(o + 4 * size_t(N)) + part.first, part.count, cudaMemcpyDeviceToHost, stream_));
+        }
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    AvnStatus report(uint32_t flags, AvnContactReport* out) override {
+        if (!out) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_report: out is required");
+        if (!stepped_) return err_->fail(AVN_ERR_UNSUPPORTED, "contacts_report: no avn_contacts_step has run on this context");
+        uint32_t n = 0;
+        GraphRows g = graph_rows();
+        if (hw_) {
+            report_keys_kernel<<<(hw_ + 255) / 256, 256, 0, stream_>>>(g, flags, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+            radix_pass(int(hw_), evl_.as<uint32_t>());   // the listed rows first, in ascending ContactId
+            const AvnStatus st = small_bounds(1, &n);
+            if (st != AVN_OK) return st;
+        }
+        const bool fits = out->capacity >= n;
+        out->count = n;
+        if (!fits) return err_->fail(AVN_ERR_CAPACITY, "contacts_report: %u touching pairs exceed the capacity %llu", n, (unsigned long long)out->capacity);
+        if (n == 0) return AVN_OK;
+        const size_t S_ = sizeof(S);
+        AVN_CUDA(repout_.ensure(size_t(n) * (6 * S_ + 22)));
+        report_gather_kernel<S><<<(n + 255) / 256, 256, 0, stream_>>>(g, evl_.as<uint32_t>(), n, normal_.as<S>(), pen_.as<S>(), nimp_out_.as<S>(), repout_.p);
+        AVN_CUDA(cudaGetLastError());
+        const char* r = repout_.as<char>();
+        const char* u = r + 6 * S_ * n;
+        const char* b = u + 20 * size_t(n);
+        struct { void* dst; const char* src; size_t bytes; } cols[] = {
+            {out->normal, r, 3 * S_ * n}, {out->total_normal_impulse, r + 3 * S_ * n, S_ * n}, {out->max_normal_impulse, r + 4 * S_ * n, S_ * n},
+            {out->max_penetration, r + 5 * S_ * n, S_ * n}, {out->contact_id, u, 4 * size_t(n)}, {out->collider1, u + 4 * size_t(n), 4 * size_t(n)},
+            {out->collider2, u + 8 * size_t(n), 4 * size_t(n)}, {out->body1, u + 12 * size_t(n), 4 * size_t(n)}, {out->body2, u + 16 * size_t(n), 4 * size_t(n)},
+            {out->flags, b, n}, {out->point_count, b + n, n}};
+        for (auto& c : cols)
+            if (c.dst) AVN_CUDA(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
         return AVN_OK;
     }
 
@@ -975,6 +1226,7 @@ class Contacts final : public ContactsBase {
         AVN_CUDA(cudaStreamSynchronize(stream_));
         st->island_count = h_isl_->islands; st->sleeping_islands = h_isl_->sleeping; st->islands_put_to_sleep = h_isl_->put_to_sleep;
         st->islands_woken = h_isl_->woken; st->split_bodies = h_isl_->split_bodies; st->merges = h_isl_->merges;
+        isl_pending_ = false;
         return AVN_OK;
     }
 
@@ -1032,18 +1284,93 @@ class Contacts final : public ContactsBase {
         AVN_CUDA(cudaGetLastError());
         return AVN_OK;
     }
-    // one stable 8-bit radix pass (digit = the low byte of the key): (k0_, v0_) -> (k1_, v1_)
-    void radix_pass(int n) {
+    // one stable 8-bit radix pass (digit = the low byte of the key): (k0_, v0_) -> (k1_, vals_out or v1_).  The event lists, the reports and the
+    // removal sort into evl_: v1_ holds the colour-major list the solver reads until the next step
+    void radix_pass(int n, uint32_t* vals_out = nullptr) {
+        uint32_t* vo = vals_out ? vals_out : v1_.as<uint32_t>();
         const int nblocks = (n + RS_TILE - 1) / RS_TILE;
         rs_histogram<uint32_t><<<nblocks, RS_THREADS, 0, stream_>>>(k0_.as<uint32_t>(), n, 0, hist_.as<uint32_t>(), nblocks);
         if (nblocks <= RS_FUSE_MAX_BLOCKS) {
-            rs_scatter<uint32_t, true><<<nblocks, RS_THREADS, 0, stream_>>>(k0_.as<uint32_t>(), v0_.as<uint32_t>(), n, 0, hist_.as<uint32_t>(), nblocks, k1_.as<uint32_t>(),
-                                                                            v1_.as<uint32_t>());
+            rs_scatter<uint32_t, true><<<nblocks, RS_THREADS, 0, stream_>>>(k0_.as<uint32_t>(), v0_.as<uint32_t>(), n, 0, hist_.as<uint32_t>(), nblocks, k1_.as<uint32_t>(), vo);
         } else {
             rs_scan<<<1, 1024, 0, stream_>>>(hist_.as<uint32_t>(), 256 * nblocks);
-            rs_scatter<uint32_t, false><<<nblocks, RS_THREADS, 0, stream_>>>(k0_.as<uint32_t>(), v0_.as<uint32_t>(), n, 0, hist_.as<uint32_t>(), nblocks, k1_.as<uint32_t>(),
-                                                                             v1_.as<uint32_t>());
+            rs_scatter<uint32_t, false><<<nblocks, RS_THREADS, 0, stream_>>>(k0_.as<uint32_t>(), v0_.as<uint32_t>(), n, 0, hist_.as<uint32_t>(), nblocks, k1_.as<uint32_t>(), vo);
         }
+    }
+    // after a radix pass over hw_ rows: out[k - 1] = the number of rows whose key is below k, k = 1 .. nb (on the host)
+    AvnStatus small_bounds(int nb, uint32_t* out) {
+        AVN_CUDA(bounds_.ensure(16));
+        key_bounds_kernel<<<1, 32, 0, stream_>>>(k1_.as<uint32_t>(), int(hw_), nb, bounds_.as<uint32_t>());
+        AVN_CUDA(cudaGetLastError());
+        AVN_CUDA(cudaMemcpyAsync(out, bounds_.p, size_t(nb) * 4, cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+    // room for `need` queued CollisionEnds in pending list i (keeps its entries)
+    AvnStatus pend_reserve(int i, uint32_t need) {
+        if (need <= pend_cap_[i]) return AVN_OK;
+        const uint32_t cap = std::max(need, std::max(2 * pend_cap_[i], 256u)), old = pend_cap_[i];
+        void* p = nullptr;
+        AVN_CUDA(cudaMalloc(&p, size_t(cap) * 17));
+        if (pend_n_[i]) {
+            const uint32_t* src = pend_[i].as<uint32_t>();
+            uint32_t* dst = static_cast<uint32_t*>(p);
+            for (int c = 0; c < 4; ++c)
+                AVN_CUDA(cudaMemcpyAsync(dst + size_t(c) * cap, src + size_t(c) * old, size_t(pend_n_[i]) * 4, cudaMemcpyDeviceToDevice, stream_));
+            AVN_CUDA(cudaMemcpyAsync(dst + 4 * size_t(cap), src + 4 * size_t(old), pend_n_[i], cudaMemcpyDeviceToDevice, stream_));
+            AVN_CUDA(cudaStreamSynchronize(stream_));
+        }
+        if (pend_[i].p) cudaFree(pend_[i].p);
+        pend_[i].p = p;
+        pend_[i].cap = size_t(cap) * 17;
+        pend_cap_[i] = cap;
+        return AVN_OK;
+    }
+    // remove_collider for each listed collider (indices checked by the caller), then the colour-major list, the colour offsets and the pair set
+    // rebuilt as a step leaves them
+    AvnStatus remove_rows(uint32_t n, const uint32_t* colliders) {
+        if (n == 0 || hw_ == 0) return AVN_OK;
+        AVN_CUDA(rm_.ensure(std::max<size_t>(n_colliders_, 1)));
+        AVN_CUDA(cudaMemsetAsync(rm_.p, 0, std::max<size_t>(n_colliders_, 1), stream_));
+        AVN_CUDA(stage_.ensure(size_t(n) * 4));
+        AVN_CUDA(cudaMemcpyAsync(stage_.p, colliders, size_t(n) * 4, cudaMemcpyHostToDevice, stream_));
+        mark_colliders_kernel<<<(n + 255) / 256, 256, 0, stream_>>>(stage_.as<uint32_t>(), n, rm_.as<uint8_t>());
+        AVN_CUDA(cudaMemsetAsync(ctr_.p, 0, offsetof(GraphCounters, ovf_count), stream_));   // (the step's counters went to the host already)
+        GraphRows g = graph_rows();
+        const unsigned rb = (hw_ + 255) / 256;
+        const int islands = !isl_configured_ ? 0 : isl_pending_ ? 2 : 1;
+        remove_rows_kernel<<<rb, 256, 0, stream_>>>(g, rm_.as<uint8_t>(), isl_, islands, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+        radix_pass(int(hw_), evl_.as<uint32_t>());   // removed touching rows, then the other removed rows, each in ascending ContactId
+        AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        const uint32_t n_rm = h_ctr_->removed, n_end = h_ctr_->stopped;
+        if (n_rm == 0) return AVN_OK;   // nothing named these colliders: the graphs are as the last step left them
+        AvnStatus st = pend_reserve(pend_cur_, pend_n_[pend_cur_] + n_end);
+        if (st != AVN_OK) return st;
+        if (n_end) {
+            queue_ends_kernel<<<(n_end + 255) / 256, 256, 0, stream_>>>(g, evl_.as<uint32_t>(), n_end, pend_n_[pend_cur_], pend_cap_[pend_cur_],
+                                                                         pend_[pend_cur_].as<uint32_t>());
+            pend_n_[pend_cur_] += n_end;
+        }
+        // only touching rows hold a colour, and they lead the list in ascending ContactId: the overflow colour's swap_removes in that order
+        overflow_list_kernel<<<1, 32, 0, stream_>>>(g, evl_.as<uint32_t>());
+        finalize_rows_kernel<<<rb, 256, 0, stream_>>>(g, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+        radix_pass(int(hw_));
+        color_offsets_kernel<<<1, 64, 0, stream_>>>(g, k1_.as<uint32_t>(), v1_.as<uint32_t>());
+        gather_graph_kernel<S><<<std::min<unsigned>(rb, unsigned(sm_count_) * 8u), 256, 0, stream_>>>(g, v1_.as<uint32_t>(), have_fr_ ? fr_.as<double>() : nullptr,
+                                                                                                    have_re_ ? re_.as<double>() : nullptr, m_b1_.as<int32_t>(),
+                                                                                                    m_b2_.as<int32_t>(), m_fr_.as<S>(), m_re_.as<S>());
+        AVN_CUDA(cudaMemsetAsync(table_.p, 0, (table_mask_ + 1) * sizeof(uint64_t), stream_));
+        pair_set_kernel<<<rb, 256, 0, stream_>>>(g, table_.as<uint64_t>(), table_mask_);
+        AVN_CUDA(cudaGetLastError());
+        table_dirty_ = false;
+        AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        live_n_ -= n_rm;
+        graph_.count = h_ctr_->manifolds;
+        graph_.any_restitution = h_ctr_->any_restitution;
+        memcpy(graph_.color_offsets, h_ctr_->color_offsets, sizeof graph_.color_offsets);
+        return AVN_OK;
     }
     GraphRows graph_rows() {
         GraphRows g{};
@@ -1052,6 +1379,7 @@ class Contacts final : public ContactsBase {
         g.live = live_.as<uint8_t>(); g.count = count_.as<uint8_t>(); g.disjoint = disjoint_.as<uint8_t>(); g.prev_count = prev_count_.as<uint8_t>();
         g.pflags = pflags_.as<uint8_t>(); g.touching = touching_.as<uint8_t>(); g.colour = colour_.as<uint8_t>(); g.change = change_.as<uint8_t>();
         g.old_colour = old_colour_.as<uint8_t>(); g.ovf_pos = ovf_pos_.as<uint32_t>(); g.ovf = ovf_.as<uint32_t>(); g.isl_event = isl_event_.as<uint8_t>(); g.fresh = fresh_.as<uint8_t>();
+        g.event = event_.as<uint8_t>(); g.sensor = sensor_h_.empty() ? nullptr : sensor_.as<uint8_t>();
         g.body_kind = kind_.as<uint8_t>(); g.n_bodies = int(n_bodies_);
         g.body_bits = body_bits_.as<uint32_t>(); g.body_min = body_min_.as<unsigned long long>();
         g.ctr = ctr_.as<GraphCounters>();
@@ -1100,6 +1428,12 @@ class Contacts final : public ContactsBase {
         m_fr_, m_re_, table_;
     GraphCounters* h_ctr_ = nullptr;
     ResidentGraph graph_{};
+    // collision events, sensors, removals, reports
+    DevBuf event_, evl_, evout_, repout_, bounds_, sensor_, rm_, pend_[2];
+    std::vector<uint8_t> sensor_h_;           // the sensor column as last set (empty = no sensor)
+    uint32_t pend_n_[2] = {0, 0}, pend_cap_[2] = {0, 0};
+    int pend_cur_ = 0;                        // pend_[pend_cur_] queues the removals' CollisionEnds; the other list is reported with the last step
+    bool stepped_ = false, isl_pending_ = false;
     uint64_t table_mask_ = 0;
     uint32_t hw_ = 0, live_n_ = 0, n_bodies_ = 0, n_colliders_ = 0;
     int sm_count_ = 132;

@@ -169,6 +169,11 @@ struct ContactsBase {
     virtual AvnStatus graph_view(ResidentGraph* out) = 0;
     virtual void pair_set(const uint64_t** table, uint64_t* mask) = 0;
     virtual AvnStatus download_graph(uint32_t capacity, uint32_t* c1, uint32_t* c2, uint8_t* live, uint8_t* touching, int8_t* colour, uint32_t* edge_list) = 0;
+    // ---- the pipeline's output to the application: sensors, removal of colliders, collision events, contact reports (contacts.cu)
+    virtual AvnStatus set_sensors(uint32_t collider_count, const uint8_t* sensor) = 0;
+    virtual AvnStatus remove_colliders(uint32_t n, const uint32_t* colliders) = 0;
+    virtual AvnStatus events(AvnCollisionEvents* started, AvnCollisionEvents* ended) = 0;
+    virtual AvnStatus report(uint32_t flags, AvnContactReport* out) = 0;
     // ---- persistent simulation islands + sleeping decisions (contacts.cu)
     virtual AvnStatus islands_configure(const AvnIslandsConfig* cfg) = 0;
     virtual AvnStatus islands_step(AvnIslandsStep* step) = 0;

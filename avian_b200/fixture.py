@@ -46,6 +46,14 @@ def _load():
         lib.avh_rows_narrow.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 27 + [C.c_double, C.c_double, C.c_double, C.c_uint32]
         lib.avh_rows_narrow.restype = None
         lib.avh_raw_manifolds.restype = None
+        lib.avh_remove_colliders.argtypes = [_vp, C.c_uint32, _vp]
+        lib.avh_remove_colliders.restype = None
+        lib.avh_set_sensors.argtypes = [_vp, _vp]
+        lib.avh_set_sensors.restype = None
+        lib.avh_events.argtypes = [_vp, C.c_uint32] + [_vp] * 5
+        lib.avh_events.restype = C.c_uint32
+        lib.avh_report.argtypes = [_vp, C.c_uint32, C.c_uint32] + [_vp] * 11
+        lib.avh_report.restype = C.c_uint32
         lib.avh_pair_count.argtypes = [_vp]
         lib.avh_pair_count.restype = C.c_uint32
         P = C.POINTER
@@ -305,6 +313,35 @@ class HostPipeline:
 
     def store_impulses(self, man: api.Manifolds) -> None:
         self.lib.avh_store_impulses(self.h, self.bits, _p(man.warm_start_normal_impulse), _p(man.warm_start_tangent_impulse), _p(man.normal_impulse))
+
+    # ---- the pipeline's output to the application: what avn_contacts_set_sensors / _remove_colliders / _events / _report do on the device
+    def set_sensors(self, sensor) -> None:
+        """The Sensor column (None = none); remove_collider for every collider whose flag changed."""
+        col = None if sensor is None else np.ascontiguousarray(sensor, dtype=bool).astype(np.uint8)
+        self.lib.avh_set_sensors(self.h, _p(col))
+
+    def remove_colliders(self, colliders) -> None:
+        ids = np.ascontiguousarray(colliders, dtype=np.uint32)
+        self.lib.avh_remove_colliders(self.h, int(ids.shape[0]), _p(ids))
+
+    def events(self) -> tuple[dict, dict]:
+        """(started, ended) of the last status loop, as Context.contacts_events returns them."""
+        lists = []
+        for which in (0, 1):
+            n = int(self.lib.avh_events(self.h, which, None, None, None, None, None))
+            out = {k: np.zeros(n, dtype=d) for k, d in api.EVENT_COLUMNS}
+            self.lib.avh_events(self.h, which, *(_p(out[k]) for k, _ in api.EVENT_COLUMNS))
+            lists.append(out)
+        return lists[0], lists[1]
+
+    def report(self, events_only: bool = False) -> dict:
+        """The touching pairs in ascending ContactId from the stored impulses, as Context.contacts_report returns them."""
+        eo = 1 if events_only else 0
+        n = int(self.lib.avh_report(self.h, self.bits, eo, *([None] * 11)))
+        _, out = api.contact_report(n, self.scalar)
+        out = {k: v[:n].copy() for k, v in out.items()}
+        self.lib.avh_report(self.h, self.bits, eo, *(_p(out[k]) for k, _ in api.AvnContactReport._fields_[2:]))
+        return out
 
     @property
     def pair_count(self) -> int:

@@ -88,6 +88,10 @@ struct Pipeline {
     std::priority_queue<uint32_t, std::vector<uint32_t>, std::greater<uint32_t>> free_ids;  // IdPool: lowest free id
     std::unordered_map<uint64_t, uint32_t> pair_set;  // PairKey -> ContactId
     std::vector<uint32_t> active;         // ContactGraph::active_pairs order
+    std::vector<uint8_t> sensor;          // Sensor per collider (empty = none)
+    struct Event { uint32_t c1, c2, b1, b2; uint8_t flags; };
+    std::vector<Event> started, ended;    // CollisionStart / CollisionEnd of the last status loop (ended: the removals' first)
+    std::vector<Event> pending_ended;     // CollisionEnds of removals since the last status loop
     Color colors[AVN_GRAPH_COLOR_COUNT];
     S contact_tolerance = 0.005, length_unit = 1.0;
     // export bookkeeping: the (contact id, manifold, point) of every exported point, in column order
@@ -256,6 +260,8 @@ void avh_add_pairs(AvhPipeline* h, const uint32_t* c1, const uint32_t* c2, const
         Pair& pr = P.pairs[id];
         pr = Pair{};
         pr.collider1 = c1[k]; pr.collider2 = c2[k]; pr.body1 = b1[k]; pr.body2 = b2[k]; pr.flags = flags[k]; pr.alive = true;
+        // a pair that involves a sensor never generates constraints (narrow_phase/system_param.rs:583-599)
+        if (!P.sensor.empty() && (P.sensor[c1[k]] || P.sensor[c2[k]])) pr.flags &= uint8_t(~AVN_PAIR_GENERATE_CONSTRAINTS);
         P.pair_set[key] = id;
         P.active.push_back(id);
     }
@@ -266,9 +272,16 @@ void avh_add_pairs(AvhPipeline* h, const uint32_t* c1, const uint32_t* c2, const
 static uint32_t apply_status_changes(Pipeline& P, std::vector<uint32_t>& changed, const std::vector<uint8_t>& disjoint, const std::vector<uint8_t>& started,
                                      const std::vector<uint8_t>& stopped, const std::vector<int>& count_change, uint32_t* out_points) {
     std::sort(changed.begin(), changed.end());
+    P.started.clear();
+    P.ended.swap(P.pending_ended);
+    P.pending_ended.clear();
     for (uint32_t id : changed) {
         Pair& pr = P.pairs[id];
         const bool gen = pr.flags & AVN_PAIR_GENERATE_CONSTRAINTS;
+        const Pipeline::Event ev{pr.collider1, pr.collider2, pr.body1, pr.body2, uint8_t(pr.flags & 0x0f)};
+        if (disjoint[id] && pr.touching) P.ended.push_back(ev);   // CollisionEnd (system_param.rs:155-170)
+        else if (!disjoint[id] && started[id]) P.started.push_back(ev);
+        else if (!disjoint[id] && stopped[id]) P.ended.push_back(ev);
         if (disjoint[id]) {
             if (gen) while (!pr.handles.empty()) pop_manifold(P, id);
             P.pair_set.erase(pair_key(pr.collider1, pr.collider2));
@@ -293,6 +306,93 @@ static uint32_t apply_status_changes(Pipeline& P, std::vector<uint32_t>& changed
         for (auto& hnd : P.colors[c].handles) { ++M; Pn += uint32_t(P.pairs[hnd.first].manifolds[hnd.second].pts.size()); }
     if (out_points) *out_points = Pn;
     return M;
+}
+
+// remove_collider (narrow_phase/mod.rs:399-459) for each listed collider: every pair that names one of them, in ascending ContactId (the device's
+// stated order), queues a CollisionEnd when it was touching, leaves the ConstraintGraph and the ContactGraph.
+void avh_remove_colliders(AvhPipeline* h, uint32_t n, const uint32_t* colliders) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    std::vector<uint8_t> gone(P.n, 0);
+    for (uint32_t k = 0; k < n; ++k) if (colliders[k] < P.n) gone[colliders[k]] = 1;
+    for (uint32_t id = 0; id < P.pairs.size(); ++id) {
+        Pair& pr = P.pairs[id];
+        if (!pr.alive || !(gone[pr.collider1] || gone[pr.collider2])) continue;
+        if (pr.touching) P.pending_ended.push_back({pr.collider1, pr.collider2, pr.body1, pr.body2, uint8_t(pr.flags & 0x0f)});
+        while (!pr.handles.empty()) pop_manifold(P, id);
+        P.pair_set.erase(pair_key(pr.collider1, pr.collider2));
+        auto it = std::find(P.active.begin(), P.active.end(), id);
+        if (it != P.active.end()) { *it = P.active.back(); P.active.pop_back(); }
+        pr = Pair{};
+        P.free_ids.push(id);
+    }
+}
+
+// The Sensor column (NULL = none): the On<Add, Sensor> / On<Remove, Sensor> observers run remove_collider for every collider whose flag changed.
+void avh_set_sensors(AvhPipeline* h, const uint8_t* sensor) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    std::vector<uint8_t> now(P.n, 0);
+    if (sensor) for (uint32_t c = 0; c < P.n; ++c) now[c] = sensor[c] ? 1 : 0;
+    std::vector<uint32_t> changed;
+    for (uint32_t c = 0; c < P.n; ++c)
+        if (now[c] != (P.sensor.empty() ? 0 : P.sensor[c])) changed.push_back(c);
+    P.sensor = std::find(now.begin(), now.end(), uint8_t(1)) != now.end() ? now : std::vector<uint8_t>();
+    avh_remove_colliders(h, uint32_t(changed.size()), changed.data());
+}
+
+// The started (which = 0) or ended (which = 1) list of the last status loop; arrays may be NULL.  Returns the length of the list.
+uint32_t avh_events(AvhPipeline* h, uint32_t which, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* flags) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    const auto& list = which ? P.ended : P.started;
+    for (size_t i = 0; i < list.size(); ++i) {
+        if (c1) c1[i] = list[i].c1;
+        if (c2) c2[i] = list[i].c2;
+        if (b1) b1[i] = list[i].b1;
+        if (b2) b2[i] = list[i].b2;
+        if (flags) flags[i] = list[i].flags;
+    }
+    return uint32_t(list.size());
+}
+
+// The touching pairs in ascending ContactId with their manifold reduced in slot order in the column type (what avn_contacts_report computes
+// from the stored impulses).  Arrays sized by a first call with contact_id == NULL.  Returns the number of entries.
+}  // extern "C"
+template <class T>
+static uint32_t report_rows(Pipeline& P, uint32_t events_only, uint32_t* contact_id, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* flags,
+                            uint8_t* point_count, T* normal, T* total, T* mx, T* deep) {
+    uint32_t n = 0;
+    for (uint32_t id = 0; id < P.pairs.size(); ++id) {
+        const Pair& pr = P.pairs[id];
+        if (!pr.alive || !pr.touching || (events_only && !(pr.flags & AVN_PAIR_CONTACT_EVENTS))) continue;
+        if (contact_id) {
+            contact_id[n] = id; c1[n] = pr.collider1; c2[n] = pr.collider2; b1[n] = pr.body1; b2[n] = pr.body2; flags[n] = uint8_t(pr.flags & 0x0f);
+            const Manifold* m = pr.manifolds.empty() ? nullptr : &pr.manifolds[0];
+            const int cnt = m ? int(m->pts.size()) : 0;
+            point_count[n] = uint8_t(cnt);
+            T tot = T(0), big = T(0), d = T(0);
+            for (int k = 0; k < cnt; ++k) {
+                const T v = T(m->pts[k].normal_impulse);
+                tot = tot + v;
+                if (v > big) big = v;
+                const T p = T(m->pts[k].penetration);
+                if (k == 0 || p >= d) d = p;
+            }
+            const V3 nv = m ? m->normal : V3{0, 0, 0};
+            normal[3 * n] = T(nv.x); normal[3 * n + 1] = T(nv.y); normal[3 * n + 2] = T(nv.z);
+            total[n] = tot; mx[n] = big; deep[n] = d;
+        }
+        ++n;
+    }
+    return n;
+}
+extern "C" {
+uint32_t avh_report(AvhPipeline* h, uint32_t scalar_bits, uint32_t events_only, uint32_t* contact_id, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2,
+                    uint8_t* flags, uint8_t* point_count, void* normal, void* total, void* mx, void* deep) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    if (scalar_bits == 64)
+        return report_rows<double>(P, events_only, contact_id, c1, c2, b1, b2, flags, point_count, static_cast<double*>(normal), static_cast<double*>(total),
+                                   static_cast<double*>(mx), static_cast<double*>(deep));
+    return report_rows<float>(P, events_only, contact_id, c1, c2, b1, b2, flags, point_count, static_cast<float*>(normal), static_cast<float*>(total),
+                              static_cast<float*>(mx), static_cast<float*>(deep));
 }
 
 // NarrowPhase::update (narrow_phase/system_param.rs:114-400) with the fixture manifold generator.

@@ -187,10 +187,15 @@ class World:
     """A headless world: body columns + the CPU fixture around the hot path + the plugin group."""
 
     def __init__(self, scene: Scene, plugins: PhysicsPlugins, dt: float = 1.0 / 60.0, substeps: int = 6, solver_iterations: int = 1,
-                 ccd: dict | None = None):
+                 ccd: dict | None = None, sensor=None, events_enabled=None):
         """ccd: the SweptCcd bodies — the keyword arguments of api.Context.ccd_configure (body, collider, mode, include_dynamic,
-        linear_threshold, angular_threshold, prediction_distance).  The solver plugin must run solve_swept_ccd (a `step_ccd` method)."""
+        linear_threshold, angular_threshold, prediction_distance).  The solver plugin must run solve_swept_ccd (a `step_ccd` method).
+        sensor / events_enabled: optional per-collider columns (Sensor, CollisionEventsEnabled).  After every step `events` holds the
+        (started, ended) lists of api.Context.contacts_events (DeviceGraphWorld: when either column is given)."""
         self.scene = scene
+        self.sensor = None if sensor is None else np.asarray(sensor, dtype=bool)
+        self.events_enabled = None if events_enabled is None else np.asarray(events_enabled, dtype=bool)
+        self.events: tuple[dict, dict] | None = None
         self.ccd = ccd
         self.bodies = scene.bodies
         self.joints = scene.joints
@@ -203,6 +208,8 @@ class World:
                                               contact_damping_ratio=cfg.contact_damping_ratio, contact_frequency_factor=cfg.contact_frequency_factor,
                                               max_overlap_solve_speed=cfg.max_overlap_solve_speed, warm_start_coefficient=cfg.warm_start_coefficient,
                                               restitution_threshold=cfg.restitution_threshold, restitution_iterations=cfg.restitution_iterations)
+        if self.sensor is not None:
+            self.pipeline.set_sensors(self.sensor)
         self.last_manifolds: api.Manifolds | None = None
         self.last_pairs: api.PairList | None = None
         self.last_aabbs: api.Aabbs | None = None
@@ -213,14 +220,41 @@ class World:
         dt = self.params.dt
         self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, dt)
         aabbs = self.pipeline.intervals(self.bodies, self.aabb_min, self.aabb_max)
+        aabbs.flags = self.interval_flags(aabbs.collider, aabbs.flags)
         aabbs.joint_disabled_body_pairs = self.scene.joint_disabled_body_pairs
         pairs = self.plugins.get("BroadPhasePlugin").collect_collision_pairs(aabbs)
         self.pipeline.commit_broadphase(aabbs, pairs)
         self.last_aabbs, self.last_pairs = aabbs, pairs
         return pairs
 
+    def interval_flags(self, order: np.ndarray, flags: np.ndarray) -> np.ndarray:
+        """init_aabb_interval_flags (broad_phase.rs:318-335) for the optional columns: events_enabled sets CONTACT_EVENTS, a sensor clears
+        GENERATE_CONSTRAINTS.  `order` = the colliders of the interval columns."""
+        if self.events_enabled is None and self.sensor is None:
+            return flags
+        f = flags.copy()
+        if self.events_enabled is not None:
+            f |= np.where(self.events_enabled[order], api.AABB_CONTACT_EVENTS, 0).astype(np.uint8)
+        if self.sensor is not None:
+            f &= np.where(self.sensor[order], ~np.uint8(api.AABB_GENERATE_CONSTRAINTS), np.uint8(0xFF)).astype(np.uint8)
+        return f
+
+    def set_sensors(self, sensor) -> None:
+        """The Sensor column changes (On<Add, Sensor> / On<Remove, Sensor>): the changed colliders' pairs leave the graphs at once."""
+        self.sensor = None if sensor is None else np.asarray(sensor, dtype=bool)
+        self.pipeline.set_sensors(self.sensor)
+
+    def remove_colliders(self, colliders) -> None:
+        """remove_collider for despawned / disabled colliders: their pairs leave the graphs, touching ones queue a CollisionEnd."""
+        self.pipeline.remove_colliders(colliders)
+
+    def report(self, events_only: bool = False) -> dict:
+        """The touching pairs with their impulses as the last solve left them (api.Context.contacts_report)."""
+        return self.pipeline.report(events_only)
+
     def narrow_phase(self) -> api.Manifolds:
         self.last_manifolds = self.pipeline.narrow_phase(self.bodies, self.aabb_min, self.aabb_max, self.params.dt, bool(self.params.match_contacts))
+        self.events = self.pipeline.events()
         return self.last_manifolds
 
     def solve(self) -> None:
@@ -453,6 +487,8 @@ class DeviceGraphWorld(World):
         n = int(scene.bodies.count)
         self.n = n
         ctx.contacts_configure(scene.bodies.kind if scene.bodies.kind is not None else np.zeros(n, dtype=np.uint8), n, scene.friction, scene.restitution)
+        if self.sensor is not None:
+            ctx.contacts_set_sensors(self.sensor)
         self.order = np.arange(n, dtype=np.uint32)       # AabbIntervals' persistent order (colliders = bodies in this fixture)
         self.stats: dict | None = None
         self.new_pairs = 0
@@ -466,6 +502,7 @@ class DeviceGraphWorld(World):
     def intervals(self, aabb_min: np.ndarray, aabb_max: np.ndarray) -> api.Aabbs:
         o, kind = self.order, self.bodies.kind
         flags = np.where(kind[o] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
+        flags = self.interval_flags(o, flags)
         a = api.Aabbs(collider=o.copy(), body=o.copy(), aabb_min=np.ascontiguousarray(aabb_min[o]), aabb_max=np.ascontiguousarray(aabb_max[o]),
                       flags=np.ascontiguousarray(flags), order_out=self._order_out)
         a.joint_disabled_body_pairs = self.scene.joint_disabled_body_pairs
@@ -486,10 +523,22 @@ class DeviceGraphWorld(World):
         oo = aabbs.order_out[:kept]
         if kept != aabbs.collider.shape[0] or oo[0] != 0 or not (oo[1:] == oo[:-1] + 1).all():   # (a sorted scene keeps its order: nothing to permute)
             self.order = np.ascontiguousarray(aabbs.collider[oo])
+        if self.sensor is not None or self.events_enabled is not None:
+            self.events = ctx.contacts_events()
         ctx.solver_step_resident(self.params, b, self.joints)
         self._uploaded_once = True
         self.step_index += 1
         return self.stats
+
+    def set_sensors(self, sensor) -> None:
+        self.sensor = None if sensor is None else np.asarray(sensor, dtype=bool)
+        self.ctx.contacts_set_sensors(self.sensor, collider_count=self.n)
+
+    def remove_colliders(self, colliders) -> None:
+        self.ctx.contacts_remove_colliders(colliders)
+
+    def report(self, events_only: bool = False) -> dict:
+        return self.ctx.contacts_report(events_only=events_only)
 
     def step(self) -> None:
         self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, self.params.dt)

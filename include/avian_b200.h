@@ -536,6 +536,66 @@ AvnStatus avn_broadphase_download_order(AvnContext* ctx, uint64_t* out_pair_coun
 AvnStatus avn_contacts_download_graph(AvnContext* ctx, uint32_t capacity, uint32_t* collider1, uint32_t* collider2, uint8_t* live, uint8_t* touching,
                                       int8_t* colour, uint32_t* edge_list);
 
+/* ---- the contact pipeline's output to the application: collision events, sensors, removal of colliders, contact reports.  All of it works on
+ *      the ContactGraph of avn_contacts_step; before the first avn_contacts_step of the context (before avn_contacts_configure for
+ *      avn_contacts_set_sensors) these calls return AVN_ERR_UNSUPPORTED.  Nothing changes for a caller that never makes them.
+ *      Lists use the capacity protocol of the hit lists: on AVN_ERR_CAPACITY `count` is the required size and nothing else was written.
+ *      Stated deviation: inside one removal call the rows of the removed colliders are visited in ascending ContactId, where the reference walks
+ *      the collider's edge list (the order of the queued CollisionEnds and of the overflow colour's swap_removes). -------------------------- */
+typedef struct AvnCollisionEvents {   /* CollisionStart / CollisionEnd (collision/collision_events.rs:171, :268) */
+    uint64_t capacity;                 /* in: entries the arrays hold */
+    uint64_t count;                    /* out: entries of the list (AVN_ERR_CAPACITY when > capacity) */
+    uint32_t* collider1;               /* [capacity] out; any array may be NULL (not wanted) */
+    uint32_t* collider2;
+    uint32_t* body1;
+    uint32_t* body2;
+    uint8_t* flags;                    /* the pair's AVN_PAIR_* flags: CONTACT_EVENTS = an events-enabled pair, GENERATE_CONSTRAINTS clear = a sensor pair */
+} AvnCollisionEvents;
+
+typedef struct AvnContactReport {     /* one entry per touching pair, ascending ContactId; scalars in the context's type; any array may be NULL */
+    uint64_t capacity;
+    uint64_t count;
+    uint32_t* contact_id;
+    uint32_t* collider1;
+    uint32_t* collider2;
+    uint32_t* body1;
+    uint32_t* body2;
+    uint8_t* flags;                    /* AVN_PAIR_* */
+    uint8_t* point_count;
+    void* normal;                      /* [n][3] manifold normal, from collider1 to collider2 */
+    void* total_normal_impulse;        /* ContactManifold::total_normal_impulse: the points' normal_impulse summed in slot order */
+    void* max_normal_impulse;          /* ContactManifold::max_normal_impulse (0 when no point) */
+    void* max_penetration;             /* penetration of find_deepest_contact (contact_types/mod.rs:318-327) */
+} AvnContactReport;
+#define AVN_REPORT_EVENTS_ONLY 0x1u   /* only pairs with AVN_PAIR_CONTACT_EVENTS */
+
+/* The Sensor column (Collider::is_sensor): a row generates constraints only when its broad-phase flags do and neither collider is a sensor
+ * (narrow_phase/system_param.rs:583-599).  Sensor rows are narrow-phased, touch, produce events and appear in reports (with zero impulses); they
+ * never take a colour and never link islands.  Plays the On<Add, Sensor> / On<Remove, Sensor> observers (narrow_phase/mod.rs:614-668): every
+ * collider whose flag changed goes through remove_collider at once, and the next broad phase finds its pairs again with the new flags.  A call
+ * before any row exists only stores the column.  sensor: [collider_count], NULL = none; collider_count must equal avn_contacts_configure's
+ * (AVN_ERR_INVALID_ARGUMENT otherwise).  avn_contacts_configure clears the column. */
+AvnStatus avn_contacts_set_sensors(AvnContext* ctx, uint32_t collider_count, const uint8_t* sensor);
+/* remove_collider (narrow_phase/mod.rs:399-459) for each listed collider, on the device, now: every live row that names one of them queues a
+ * CollisionEnd when it was touching, leaves its colour (the overflow colour keeps its swap_remove order), applies remove_contact to its island
+ * when it was a touching, constraint-generating contact and islands are configured (islands/mod.rs:594-667), and is freed.  The colour-major
+ * list, the colour offsets and the pair set are rebuilt: avn_solver_upload_resident and the next broad phase see the new graph.  Despawned
+ * colliders, ColliderDisabled.  A collider >= the configured count is AVN_ERR_INVALID_ARGUMENT and nothing is removed.  Waking the islands of
+ * the removed collider's body stays with the caller (AvnIslandsStep::wake). */
+AvnStatus avn_contacts_remove_colliders(AvnContext* ctx, uint32_t n, const uint32_t* colliders);
+/* The collision events of the last avn_contacts_step; repeatable until the next step.  Every transition is listed with its pair flags, events
+ * enabled or not: the caller writes CollisionStart / CollisionEnd for the AVN_PAIR_CONTACT_EVENTS entries and updates CollidingEntities from all
+ * of them (system_param.rs:155-321).
+ *   started: rows that started touching, ascending ContactId (the order of the reference's status loop);
+ *   ended:   first the CollisionEnds of the removals since the previous step (touching rows, call order), then the rows that stopped touching
+ *            or whose AABBs separated while touching, ascending ContactId.
+ * Either list may be NULL. */
+AvnStatus avn_contacts_events(AvnContext* ctx, AvnCollisionEvents* started, AvnCollisionEvents* ended);
+/* ContactPair::total_normal_impulse / max_normal_impulse (contact_types/mod.rs:227-277) of the touching pairs as the last solve left them:
+ * call it after avn_solver_run.  Geometry from this step's narrow phase, impulses from store_contact_impulses (solver/plugin.rs:722-754).  A row
+ * that was not solved this step (a sensor pair) reports 0 impulses, as the reference's fresh points do.  flags: AVN_REPORT_*. */
+AvnStatus avn_contacts_report(AvnContext* ctx, uint32_t flags, AvnContactReport* out);
+
 /* ---- simulation islands and sleeping on the device (SURVEY.md 8f "next #4").  Replaces the bookkeeping and the decisions of
  *        PhysicsIslands::add_contact / remove_contact / add_joint / merge_islands / split_island   (dynamics/solver/islands/mod.rs:513-1270)
  *        update_sleeping_states, wake_islands_with_sleeping_disabled, sleep_islands                 (dynamics/solver/islands/sleeping.rs:164-292)
