@@ -345,6 +345,11 @@ class AvnIslandsStep(C.Structure):
                                                                                      "split_bodies", "merges")]
 
 
+class AvnIslandsWake(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("islands_woken", "rows_woken", "rows_asleep", "bodies_asleep", "manifold_count", "colouring_rounds")] + [
+        ("color_offsets", C.c_uint32 * (GRAPH_COLOR_COUNT + 1))]
+
+
 class AvnNarrowInput(C.Structure):
     _fields_ = [("pair_count", C.c_uint32), ("collider_count", C.c_uint32), ("body_count", C.c_uint32), ("_pad", C.c_uint32)] + [
         (n, _vp) for n in ("collider1", "collider2", "body1", "body2", "shape", "dims", "position", "rotation", "linear_velocity", "angular_velocity",
@@ -491,6 +496,9 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "solver_prefetch_bodies": ([_vp, P(AvnBodyColumns), C.c_uint32], C.c_int),
         "islands_configure": ([_vp, P(AvnIslandsConfig)], C.c_int),
         "islands_step": ([_vp, P(AvnIslandsStep)], C.c_int),
+        "islands_apply": ([_vp, C.c_uint32], C.c_int),
+        "islands_wake": ([_vp, _vp, P(AvnIslandsWake)], C.c_int),
+        "contacts_download_sleeping": ([_vp, C.c_uint32, _vp, C.c_uint32, _vp], C.c_int),
         "query_update": ([_vp, P(AvnQueryColliders), C.c_uint32], C.c_int),
         "query_cast_ray": ([_vp, P(AvnRayBatch), P(AvnRayClosest)], C.c_int),
         "query_ray_hits": ([_vp, P(AvnRayBatch), P(AvnHitList)], C.c_int),
@@ -524,7 +532,7 @@ ABI_SYMBOLS = [
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
     "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download", "avn_contacts_set_sensors", "avn_contacts_remove_colliders",
-    "avn_contacts_events", "avn_contacts_report"]
+    "avn_contacts_events", "avn_contacts_report", "avn_islands_apply", "avn_islands_wake", "avn_contacts_download_sleeping"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -1097,6 +1105,26 @@ class Context:
         self._check(self.lib.avn_islands_step(self.handle, C.byref(st)))
         for n in ("island_count", "sleeping_islands", "islands_put_to_sleep", "islands_woken", "split_bodies", "merges"):
             out[n] = int(getattr(st, n))
+        return out
+
+    # ---- applied sleeping (include/avian_b200.h avn_islands_apply / _wake)
+    def islands_apply(self, enable: bool = True) -> None:
+        """avn_islands_apply: from now on the library plays SleepIslands / WakeIslands on its rows, graphs and solver stage."""
+        self._check(self.lib.avn_islands_apply(self.handle, 1 if enable else 0))
+
+    def islands_wake(self, wake=None) -> dict:
+        """avn_islands_wake: between contacts_step and solver_step_resident.  Returns the counters and the colour offsets after the wake."""
+        wk = None if wake is None else np.ascontiguousarray(wake, dtype=np.uint8)
+        out = AvnIslandsWake()
+        self._check(self.lib.avn_islands_wake(self.handle, _ptr(wk), C.byref(out)))
+        st = {n: int(getattr(out, n)) for n, _ in AvnIslandsWake._fields_ if n != "color_offsets"}
+        st["color_offsets"] = np.array(list(out.color_offsets), dtype=np.uint32)
+        return st
+
+    def contacts_download_sleeping(self, capacity: int, body_count: int) -> dict:
+        out = {"row_asleep": np.zeros(capacity, dtype=np.uint8), "body_asleep": np.zeros(body_count, dtype=np.uint8)}
+        self._check(self.lib.avn_contacts_download_sleeping(self.handle, int(capacity), _ptr(out["row_asleep"]) if capacity else None, int(body_count),
+                                                            _ptr(out["body_asleep"]) if body_count else None))
         return out
 
     # ---- swept CCD (include/avian_b200.h avn_ccd_*): solve_swept_ccd inside the device-resident solver stage

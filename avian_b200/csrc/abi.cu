@@ -311,6 +311,17 @@ AvnStatus avn_contacts_report(AvnContext* ctx, uint32_t flags, AvnContactReport*
 }
 AvnStatus avn_islands_configure(AvnContext* ctx, const AvnIslandsConfig* config) { return guarded(ctx, [&] { return ctx->contacts->islands_configure(config); }); }
 AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step) { return guarded(ctx, [&] { return ctx->contacts->islands_step(step); }); }
+AvnStatus avn_islands_apply(AvnContext* ctx, uint32_t enable) {
+    return guarded(ctx, [&] {
+        if (enable && ctx->ccd->active())
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "islands_apply: swept CCD is configured (avn_ccd_configure); sleeping bodies are not swept against");
+        return ctx->contacts->islands_apply(enable);
+    });
+}
+AvnStatus avn_islands_wake(AvnContext* ctx, const uint8_t* wake, AvnIslandsWake* out) { return guarded(ctx, [&] { return ctx->contacts->islands_wake(wake, out); }); }
+AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep) {
+    return guarded(ctx, [&] { return ctx->contacts->download_sleeping(capacity, row_asleep, body_count, body_asleep); });
+}
 AvnStatus avn_contacts_download_impulses(AvnContext* ctx, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse) {
     return guarded(ctx, [&] { return ctx->contacts->download_impulses(warm_start_normal, warm_start_tangent, normal_impulse); });
 }
@@ -348,6 +359,10 @@ AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* sh
 // swept CCD (ccd.cu): solve_swept_ccd inside avn_solver_run
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
     return guarded(ctx, [&] {
+        avn::ContactsBase::AsleepBodies asleep;
+        ctx->contacts->asleep_bodies(&asleep);
+        if (asleep.body_asleep && config && config->count)
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
         avn::CcdRows rows;
         ctx->contacts->ccd_rows(&rows);
         return ctx->ccd->configure(config, rows);

@@ -15,6 +15,7 @@ struct EdgeRows {
     uint8_t* count; uint8_t* disjoint; S* normal; S* a1; S* a2; S* pen; S* ns;
     uint8_t* prev_count; double* prev_a1; double* prev_a2;
     S* ws_n_in; S* ws_t_in; S* ws_n_out; S* ws_t_out; S* nimp_in; S* nimp_out;
+    const uint8_t* asleep;   // the row sleeps with an island (NULL = no row does): it is left completely alone
 };
 
 template <class S>
@@ -32,6 +33,7 @@ template <class S> NM_HD inline void std3(S* p, size_t i, nm::V3 v) { p[3 * i] =
 template <class S>
 NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e) {
     const EdgeRows<S>& r = a.r;
+    if (r.asleep && r.asleep[e]) return;   // update_contacts runs over active_pairs only (narrow_phase/system_param.rs:437)
     if (!r.live[e]) { r.count[e] = 0; r.disjoint[e] = 0; return; }
     const uint32_t ca = r.c1[e], cb = r.c2[e], ba = r.b1[e], bb = r.b2[e];
     int np = 0;

@@ -44,10 +44,12 @@ enum { ISL_NONE = 0, ISL_ADD = 1, ISL_REMOVE = 2 };
 struct GraphCounters {          // device block, copied to the host once per step
     // cleared at the start of every step
     uint32_t removed, started, stopped, changed, rounds, ovf_dirty, manifolds, any_restitution, aborted, bad_pairs;
+    uint32_t rows_woken, rows_slept, bodies_asleep;   // applied sleeping: what the last wake / sleep pass did, bodies asleep after it
     uint32_t round_left[3];
     uint32_t color_offsets[AVN_GRAPH_COLOR_COUNT + 1];
     // persistent
     uint32_t ovf_count;
+    uint32_t rows_asleep;
 };
 
 struct GraphRows {
@@ -58,6 +60,7 @@ struct GraphRows {
     uint8_t* fresh;                               // the row was added in this step (its geometry is still to be computed)
     uint8_t* isl_event;                           // this step's event for the islands: ISL_ADD / ISL_REMOVE (a linked contact came or went)
     uint8_t* event;                               // this step's collision event: EV_STARTED / EV_ENDED | the pair's AVN_PAIR_* flags (0 = none)
+    uint8_t* asleep;                              // the row sleeps with an island (avn_islands_apply): live and touching, out of the ConstraintGraph, left alone
     const uint8_t* sensor;                        // [C] Sensor per collider (avn_contacts_set_sensors); NULL = none
     uint32_t* ovf_pos; uint32_t* ovf;
     const uint8_t* body_kind; int n_bodies;
@@ -78,7 +81,7 @@ __global__ void add_rows_kernel(GraphRows g, uint32_t n_new, const uint32_t* __r
     if (bad) {
         atomicAdd(&g.ctr->bad_pairs, 1u);
         g.c1[e] = 0; g.c2[e] = 0; g.b1[e] = 0; g.b2[e] = 0; g.pflags[e] = 0; g.isl_event[e] = 0; g.fresh[e] = 0;
-        g.live[e] = 0; g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.change[e] = 0;
+        g.live[e] = 0; g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.change[e] = 0; g.asleep[e] = 0;
         return;
     }
     g.c1[e] = pc1[k]; g.c2[e] = pc2[k]; g.b1[e] = pb1[k]; g.b2[e] = pb2[k];
@@ -88,7 +91,7 @@ __global__ void add_rows_kernel(GraphRows g, uint32_t n_new, const uint32_t* __r
     g.isl_event[e] = 0;
     g.fresh[e] = 1;
     g.live[e] = 1;            // a ContactId handed to a new pair starts without history
-    g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.change[e] = 0;
+    g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.change[e] = 0; g.asleep[e] = 0;
 }
 
 // key 0 for rows that satisfy the predicate, 1 otherwise: one stable radix pass then lists them in ascending ContactId
@@ -108,7 +111,7 @@ __global__ void classify_kernel(GraphRows g, uint32_t* __restrict__ keys, uint32
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= g.hw) return;
     uint8_t ch = CH_NONE, ev = ISL_NONE, cev = 0;
-    if (g.live[e]) {
+    if (g.live[e] && !g.asleep[e]) {   // update_contacts runs over active_pairs only: a sleeping pair changes nothing
         const uint8_t pf = g.pflags[e];
         const bool gen = (pf & AVN_PAIR_GENERATE_CONSTRAINTS) != 0;
         if (g.disjoint[e]) {
@@ -307,7 +310,10 @@ __global__ void finalize_rows_kernel(GraphRows g, uint32_t* __restrict__ keys, u
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= g.hw) return;
     const uint8_t ch = g.change[e];
-    if ((ch & CH_MASK) == CH_REMOVE) { g.live[e] = 0; g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.pflags[e] = 0; }
+    if ((ch & CH_MASK) == CH_REMOVE) {
+        g.live[e] = 0; g.count[e] = 0; g.prev_count[e] = 0; g.touching[e] = 0; g.colour[e] = 0; g.pflags[e] = 0;
+        if (g.asleep[e]) { g.asleep[e] = 0; atomicSub(&g.ctr->rows_asleep, 1u); }   // a freed ContactId never hands its sleep on
+    }
     g.old_colour[e] = 0;
     const int c = int(g.colour[e]) - 1;
     keys[e] = (c >= 0 && c < AVN_COLOR_OVERFLOW) ? uint32_t(c) : 255u;
@@ -420,7 +426,7 @@ __global__ void queue_ends_kernel(GraphRows g, const uint32_t* __restrict__ list
 }
 // One report entry per listed row, columns of n entries: S normal[n][3], total[n], max[n], penetration[n]; u32 contact_id[n], collider1[n],
 // collider2[n], body1[n], body2[n]; u8 flags[n], point_count[n].  The points are reduced in slot order in S, so a sequential host loop in the
-// same type gives the same bits.  Only a row in the ConstraintGraph was solved: any other row (a sensor pair) reports 0 impulses.
+// same type gives the same bits.  Only a row in the ConstraintGraph, or asleep out of it, was solved: any other row (a sensor pair) reports 0 impulses.
 template <class S>
 __global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ list, uint32_t n, const S* __restrict__ normal, const S* __restrict__ pen,
                                      const S* __restrict__ nimp, void* __restrict__ out) {
@@ -431,7 +437,7 @@ __global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ l
     uint32_t* ou = reinterpret_cast<uint32_t*>(os + 6 * size_t(n));
     uint8_t* ob = reinterpret_cast<uint8_t*>(ou + 5 * size_t(n));
     const int cnt = g.count[e];
-    const bool solved = g.colour[e] != 0;
+    const bool solved = g.colour[e] != 0 || g.asleep[e] != 0;   // an asleep row keeps the impulses of its last solve
     S total = S(0), mx = S(0), deep = S(0);
     for (int k = 0; k < cnt; ++k) {
         const S v = solved ? nimp[4 * size_t(e) + k] : S(0);
@@ -484,7 +490,11 @@ __global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant
 // goes (constraints_removed += 1) or when the split candidate is split (its bodies are reset to singletons and re-linked through the contacts
 // and joints that are still there).
 // =====================================================================================================================================
-struct IslandCounters { uint32_t islands, sleeping, put_to_sleep, woken, split_bodies, merges, split_root, _pad; unsigned long long cand; };
+struct IslandCounters {
+    uint32_t islands, sleeping, put_to_sleep, woken, split_bodies, merges, split_root;
+    uint32_t absorbed;   // sleeping islands that were merged into another island (their bodies are awake with it, without a WakeIslands)
+    unsigned long long cand;
+};
 constexpr uint32_t ISL_NONE_BODY = 0xffffffffu;
 
 struct IslandState {
@@ -563,7 +573,7 @@ __global__ void isl_flatten_kernel(IslandState s, int split_only) {
     s.root[b] = r;
     if (s.root_prev[b] == uint32_t(b) && r != uint32_t(b)) {
         if (s.removed[b]) { atomicAdd(&s.removed[r], s.removed[b]); s.removed[b] = 0; }
-        if (s.isl_sleeping[b]) { s.isl_sleeping[b] = 0; s.need_wake[r] = 1; s.touched[b] = 1; }
+        if (s.isl_sleeping[b]) { s.isl_sleeping[b] = 0; s.need_wake[r] = 1; s.touched[b] = 1; atomicAdd(&s.ctr->absorbed, 1u); }
     }
 }
 __global__ void isl_wake_marks_kernel(IslandState s) {
@@ -606,6 +616,11 @@ __global__ void isl_split_link_kernel(IslandState s, GraphRows g) {
     const uint32_t a = g.b1[e], b = g.b2[e];
     if (isl_static(s, a) || isl_static(s, b) || !s.in_split[a] || !s.in_split[b]) return;
     isl_union(s.parent, a, b);
+}
+// every island is to wake (sleeping stops being applied)
+__global__ void isl_mark_all_kernel(IslandState s, uint8_t mark) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < s.B && !isl_static(s, uint32_t(b))) s.need_wake[b] = mark;
 }
 // WakeIslands for the marked islands: timers back to zero (sleeping.rs WakeIslands::apply)
 __global__ void isl_wake_bodies_kernel(IslandState s) {
@@ -664,6 +679,21 @@ __global__ void isl_finish_kernel(IslandState s, uint32_t* __restrict__ out_isla
     }
 }
 
+// pop_manifold for a row outside the colouring rounds (pops only clear bits, so one pass may do any number of them; the overflow colour's list
+// is fixed afterwards by overflow_list_kernel, which reads old_colour)
+__device__ __forceinline__ void graph_pop_now(const GraphRows& g, uint32_t e) {
+    const uint32_t b1 = g.b1[e], b2 = g.b2[e];
+    const int c = int(g.colour[e]) - 1;
+    g.old_colour[e] = g.colour[e];
+    if (c == AVN_COLOR_OVERFLOW) {
+        g.ctr->ovf_dirty = 1;
+    } else if (c >= 0) {
+        if (!graph_static(g, b1)) atomicAnd(&g.body_bits[b1], ~(1u << c));
+        if (!graph_static(g, b2)) atomicAnd(&g.body_bits[b2], ~(1u << c));
+    }
+    g.colour[e] = 0;
+}
+
 // remove_collider for every live row that names a removed collider: pop its manifold from its colour (pops only clear bits: one pass does them
 // all; the overflow colour's list is fixed by overflow_list_kernel), remove_contact on its island when it was a touching, constraint-generating
 // contact (islands: 0 = not configured, 1 = the last step's island events were applied, 2 = they are still pending: a contact that avn_islands_step
@@ -683,15 +713,7 @@ __global__ void remove_rows_kernel(GraphRows g, const uint8_t* __restrict__ remo
         atomicAdd(&g.ctr->changed, 1u);
         if (touching) atomicAdd(&g.ctr->stopped, 1u);
         const uint32_t b1 = g.b1[e], b2 = g.b2[e];
-        const int c = int(g.colour[e]) - 1;
-        g.old_colour[e] = g.colour[e];
-        if (c == AVN_COLOR_OVERFLOW) {
-            g.ctr->ovf_dirty = 1;
-        } else if (c >= 0) {
-            if (!graph_static(g, b1)) atomicAnd(&g.body_bits[b1], ~(1u << c));
-            if (!graph_static(g, b2)) atomicAnd(&g.body_bits[b2], ~(1u << c));
-        }
-        g.colour[e] = 0;
+        graph_pop_now(g, uint32_t(e));
         if (islands == 2 && g.isl_event[e] == ISL_ADD) {
             g.isl_event[e] = ISL_NONE;
         } else if (islands && touching && (g.pflags[e] & AVN_PAIR_GENERATE_CONSTRAINTS)) {
@@ -703,6 +725,70 @@ __global__ void remove_rows_kernel(GraphRows g, const uint8_t* __restrict__ remo
     keys[e] = key;
     vals[e] = uint32_t(e);
 }
+
+// =====================================================================================================================================
+// Applying sleeping and waking (SleepIslands::apply / WakeIslands::apply, sleeping.rs:354-533; ContactGraph::sleep_entity_with / wake_entity_with,
+// contact_graph.rs:702-826).  isl_sleeping[root] is the DECISION, body_asleep[b] the APPLIED state; a pass brings the second in line with the first
+// and moves the rows: a touching row sleeps with either endpoint, an asleep row wakes with either endpoint.
+// =====================================================================================================================================
+// body_asleep := the decision; fell[b] = the body fell asleep in this pass
+__global__ void sleep_bodies_kernel(IslandState s, uint8_t* __restrict__ body_asleep, uint8_t* __restrict__ fell, GraphCounters* ctr) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= s.B) return;
+    const uint8_t want = (!isl_static(s, uint32_t(b)) && s.isl_sleeping[s.root[b]]) ? 1 : 0;
+    fell[b] = (want && !body_asleep[b]) ? 1 : 0;
+    body_asleep[b] = want;
+    if (want) atomicAdd(&ctr->bodies_asleep, 1u);
+}
+__device__ __forceinline__ bool row_body_flag(const GraphRows& g, uint32_t b, const uint8_t* __restrict__ flag) { return !graph_static(g, b) && flag[b]; }
+// wake_entity_with: an asleep row with an awake (non-static) endpoint returns to the active pairs; a constraint-generating one is keyed as a push
+// (key 0) for the colouring rounds, and its warm start is what its last solve left.
+template <class S>
+__global__ void wake_rows_kernel(GraphRows g, const uint8_t* __restrict__ body_asleep, S* __restrict__ ws_n_in, S* __restrict__ ws_t_in,
+                                 const S* __restrict__ ws_n_out, const S* __restrict__ ws_t_out, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= g.hw) return;
+    uint8_t ch = CH_NONE;
+    if (g.live[e] && g.asleep[e]) {
+        const uint32_t b1 = g.b1[e], b2 = g.b2[e];
+        const bool awake = (!graph_static(g, b1) && !body_asleep[b1]) || (!graph_static(g, b2) && !body_asleep[b2]);
+        if (awake) {
+            g.asleep[e] = 0;
+            atomicAdd(&g.ctr->rows_woken, 1u);
+            atomicSub(&g.ctr->rows_asleep, 1u);
+            if (g.pflags[e] & AVN_PAIR_GENERATE_CONSTRAINTS) {
+                ch = CH_PUSH;
+                atomicAdd(&g.ctr->changed, 1u);
+                for (int k = 0; k < 4; ++k) ws_n_in[4 * size_t(e) + k] = ws_n_out[4 * size_t(e) + k];
+                for (int k = 0; k < 8; ++k) ws_t_in[8 * size_t(e) + k] = ws_t_out[8 * size_t(e) + k];
+            }
+        }
+    }
+    g.change[e] = ch;
+    keys[e] = ch ? 0u : 1u;
+    vals[e] = uint32_t(e);
+}
+// sleep_entity_with: a touching, not yet sleeping row with an endpoint that just fell asleep leaves the active pairs; its manifold is popped here
+// (key 0: the overflow colour's swap_removes follow in ascending ContactId).  No CH_REMOVE, no remove_contact, no event.
+__global__ void sleep_rows_kernel(GraphRows g, const uint8_t* __restrict__ fell, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= g.hw) return;
+    uint8_t ch = CH_NONE;
+    if (g.live[e] && g.touching[e] && !g.asleep[e] && (row_body_flag(g, g.b1[e], fell) || row_body_flag(g, g.b2[e], fell))) {
+        g.asleep[e] = 1;
+        atomicAdd(&g.ctr->rows_slept, 1u);
+        atomicAdd(&g.ctr->rows_asleep, 1u);
+        if (g.colour[e]) {
+            graph_pop_now(g, uint32_t(e));
+            ch = CH_POP | CH_DONE;
+            atomicAdd(&g.ctr->changed, 1u);
+        }
+    }
+    g.change[e] = ch;
+    keys[e] = ch ? 0u : 1u;
+    vals[e] = uint32_t(e);
+}
+
 template <class S>
 class Contacts final : public ContactsBase {
    public:
@@ -734,7 +820,7 @@ class Contacts final : public ContactsBase {
                       {&ws_t_out_, 8 * sizeof(S)}, {&nimp_in_, 4 * sizeof(S)}, {&nimp_out_, 4 * sizeof(S)},
                       // graph state per row (zero = no flags, not touching, no colour)
                       {&pflags_, 1}, {&touching_, 1}, {&colour_, 1}, {&change_, 1}, {&old_colour_, 1}, {&ovf_pos_, 4}, {&ovf_, 4}, {&isl_event_, 1}, {&fresh_, 1},
-                      {&event_, 1}};
+                      {&event_, 1}, {&asleep_, 1}};
         for (Col& c : cols) {   // grow, keep the old rows, zero the new ones
             void* fresh = nullptr;
             AVN_CUDA(cudaMalloc(&fresh, n * c.bytes_per_row));
@@ -806,6 +892,8 @@ class Contacts final : public ContactsBase {
     // ---- the graphs on the device ---------------------------------------------------------------------------------------------------
     AvnStatus configure(const AvnContactGraphConfig* cfg) override {
         if (!cfg || !cfg->body_kind) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_configure: config and body_kind are required");
+        // the applied state is sized and kept for the configured bodies and rows: a reconfiguration starts from avn_islands_apply(ctx, 0)
+        if (apply_) return err_->fail(AVN_ERR_UNSUPPORTED, "contacts_configure while sleeping is applied: call avn_islands_apply(ctx, 0) first");
         n_bodies_ = cfg->body_count;
         n_colliders_ = cfg->collider_count;
         AVN_CUDA(kind_.ensure(std::max<size_t>(n_bodies_, 1)));
@@ -823,7 +911,9 @@ class Contacts final : public ContactsBase {
         if (E_) {
             AVN_CUDA(cudaMemsetAsync(colour_.p, 0, E_, stream_));
             AVN_CUDA(cudaMemsetAsync(touching_.p, 0, E_, stream_));
+            AVN_CUDA(cudaMemsetAsync(asleep_.p, 0, E_, stream_));
         }
+        bodies_asleep_ = rows_asleep_ = 0;
         AVN_CUDA(cudaStreamSynchronize(stream_));   // the host arrays may be reused by the caller
         configured_ = true;
         graph_ = ResidentGraph{};
@@ -894,34 +984,9 @@ class Contacts final : public ContactsBase {
             classify_kernel<<<rb, 256, 0, stream_>>>(g, k0_.as<uint32_t>(), v0_.as<uint32_t>());
             radix_pass(int(hw_));
             AVN_CUDA(cudaMemcpyAsync(list_.p, v1_.p, size_t(hw_) * 4, cudaMemcpyDeviceToDevice, stream_));   // changed rows first, ascending ContactId
-            AVN_CUDA(cudaMemsetAsync(body_min_.p, 0xff, std::max<size_t>(n_bodies_, 1) * 16, stream_));
-            if (use_cluster_) {   // small change sets: one thread-block cluster (returns at once when there are more than CL_MAX changed edges)
-                cudaLaunchConfig_t cfg{};
-                cfg.gridDim = dim3(CL_BLOCKS); cfg.blockDim = dim3(CL_THREADS); cfg.dynamicSmemBytes = 0; cfg.stream = stream_;
-                cudaLaunchAttribute attr[1];
-                attr[0].id = cudaLaunchAttributeClusterDimension;
-                attr[0].val.clusterDim.x = CL_BLOCKS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-                cfg.attrs = attr; cfg.numAttrs = 1;
-                const uint32_t* list = list_.as<uint32_t>();
-                cudaError_t ce = cudaLaunchKernelEx(&cfg, colour_rounds_cluster_kernel, g, list);
-                if (ce != cudaSuccess) { (void)cudaGetLastError(); use_cluster_ = false; }
-            }
-            {
-                const uint32_t* list = list_.as<uint32_t>();
-                uint32_t skip_upto = use_cluster_ ? CL_MAX : 0u;
-                void* args[] = {(void*)&g, (void*)&list, (void*)&skip_upto};
-                int per_sm = 0;
-                AVN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, colour_rounds_kernel, 256, 0));
-                if (per_sm < 1) return err_->fail(AVN_ERR_CUDA, "contacts_step: the colouring kernel does not fit the device");
-                AVN_CUDA(cudaLaunchCooperativeKernel((const void*)colour_rounds_kernel, dim3(sm_count_), dim3(256), args, 0, stream_));
-            }
+            if ((st = colour_changed(g)) != AVN_OK) return st;
             overflow_list_kernel<<<1, 32, 0, stream_>>>(g, list_.as<uint32_t>());
-            finalize_rows_kernel<<<rb, 256, 0, stream_>>>(g, k0_.as<uint32_t>(), v0_.as<uint32_t>());
-            radix_pass(int(hw_));   // -> k1_ sorted colour keys, v1_ = the colour-major list (ascending ContactId inside a colour)
-            color_offsets_kernel<<<1, 64, 0, stream_>>>(g, k1_.as<uint32_t>(), v1_.as<uint32_t>());
-            gather_graph_kernel<S><<<std::min<unsigned>(rb, unsigned(sm_count_) * 8u), 256, 0, stream_>>>(g, v1_.as<uint32_t>(), have_fr_ ? fr_.as<double>() : nullptr,
-                                                                                                        have_re_ ? re_.as<double>() : nullptr, m_b1_.as<int32_t>(),
-                                                                                                        m_b2_.as<int32_t>(), m_fr_.as<S>(), m_re_.as<S>());
+            rebuild_list(g);
             AVN_CUDA(cudaGetLastError());
         }
         AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
@@ -951,6 +1016,7 @@ class Contacts final : public ContactsBase {
         graph_.edge = v1_.as<uint32_t>(); graph_.body1 = m_b1_.as<int32_t>(); graph_.body2 = m_b2_.as<int32_t>(); graph_.friction = m_fr_.p; graph_.restitution = m_re_.p;
         stepped_ = true;
         isl_pending_ = true;
+        wake_done_ = false;
         return AVN_OK;
     }
 
@@ -1116,6 +1182,7 @@ class Contacts final : public ContactsBase {
     AvnStatus islands_configure(const AvnIslandsConfig* cfg) override {
         if (!cfg || !cfg->body_kind) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "islands_configure: config and body_kind are required");
         if (cfg->joint_count && (!cfg->joint_body1 || !cfg->joint_body2)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "islands_configure: joint bodies are required");
+        if (apply_) return err_->fail(AVN_ERR_UNSUPPORTED, "islands_configure while sleeping is applied: call avn_islands_apply(ctx, 0) first");
         const size_t B = cfg->body_count, Bp = std::max<size_t>(B, 1);
         // one allocation, every array 16-byte aligned
         auto up16 = [](size_t x) { return (x + 15) & ~size_t(15); };
@@ -1201,8 +1268,12 @@ class Contacts final : public ContactsBase {
         GraphRows g = graph_rows();
         const unsigned rb = g.hw > 0 ? unsigned((g.hw + 255) / 256) : 0;
         // narrow-phase part: contacts that came (merge) and went (constraints_removed), islands reached by a new contact wake up
-        if (rb) isl_add_kernel<<<rb, 256, 0, stream_>>>(s, g);
-        isl_flatten_kernel<<<bb, 256, 0, stream_>>>(s, 0);
+        // (avn_islands_wake has linked this step's contacts already when sleeping is applied; the marks of the `wake` column are still to do)
+        const bool linked = apply_ && wake_done_ && isl_pending_;
+        if (!linked) {
+            if (rb) isl_add_kernel<<<rb, 256, 0, stream_>>>(s, g);
+            isl_flatten_kernel<<<bb, 256, 0, stream_>>>(s, 0);
+        }
         isl_wake_marks_kernel<<<bb, 256, 0, stream_>>>(s);
         if (rb) isl_remove_kernel<<<rb, 256, 0, stream_>>>(s, g);
         // WakeIslands queued by the narrow phase are applied before the solver runs
@@ -1227,7 +1298,107 @@ class Contacts final : public ContactsBase {
         st->island_count = h_isl_->islands; st->sleeping_islands = h_isl_->sleeping; st->islands_put_to_sleep = h_isl_->put_to_sleep;
         st->islands_woken = h_isl_->woken; st->split_bodies = h_isl_->split_bodies; st->merges = h_isl_->merges;
         isl_pending_ = false;
+        if (apply_) {
+            // SleepIslands for the islands put to sleep, WakeIslands for the ones the `wake` column woke after the solve: awake from the next step on
+            const bool wakes = h_isl_->woken > 0 || h_isl_->absorbed > 0, sleeps = h_isl_->put_to_sleep > 0;
+            if (linked) { st->islands_woken += wake_woken_; st->merges += wake_merges_; }
+            wake_woken_ = wake_merges_ = 0;
+            if (wakes || sleeps) return apply_pass(wakes, sleeps);
+        }
         return AVN_OK;
+    }
+
+    // ---- applied sleeping ---------------------------------------------------------------------------------------------------------------
+    AvnStatus islands_apply(uint32_t enable) override {
+        if (!enable) {
+            if (!apply_) return AVN_OK;
+            if (isl_pending_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "islands_apply(0) between avn_contacts_step and avn_islands_step: finish the step first");
+            if (bodies_asleep_) {   // wake everything first: WakeIslands for every island, then the rows return
+                const unsigned bb = unsigned((size_t(isl_B_) + 255) / 256);
+                AVN_CUDA(cudaMemsetAsync(isl_.ctr, 0, sizeof(IslandCounters), stream_));
+                isl_mark_all_kernel<<<bb, 256, 0, stream_>>>(isl_, 1);
+                isl_wake_bodies_kernel<<<bb, 256, 0, stream_>>>(isl_);
+                isl_wake_roots_kernel<<<bb, 256, 0, stream_>>>(isl_);
+                isl_mark_all_kernel<<<bb, 256, 0, stream_>>>(isl_, 0);
+                const AvnStatus st = apply_pass(true, false);
+                if (st != AVN_OK) return st;
+            }
+            apply_ = false;
+            wake_done_ = false;
+            return AVN_OK;
+        }
+        if (!isl_configured_ || !configured_) return err_->fail(AVN_ERR_UNSUPPORTED, "islands_apply before avn_contacts_configure and avn_islands_configure");
+        if (isl_B_ != n_bodies_)
+            return err_->fail(AVN_ERR_UNSUPPORTED, "islands_apply: avn_islands_configure has %u bodies, avn_contacts_configure %u", isl_B_, n_bodies_);
+        if (apply_) return AVN_OK;
+        const size_t Bp = std::max<size_t>(n_bodies_, 1);
+        AVN_CUDA(body_asleep_.ensure(2 * Bp));
+        AVN_CUDA(cudaMemsetAsync(body_asleep_.p, 0, 2 * Bp, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        bodies_asleep_ = 0;
+        wake_woken_ = wake_merges_ = 0;
+        apply_ = true;
+        return AVN_OK;
+    }
+
+    AvnStatus islands_wake(const uint8_t* wake, AvnIslandsWake* out) override {
+        if (!out) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "islands_wake: out is required");
+        if (!apply_) return err_->fail(AVN_ERR_UNSUPPORTED, "avn_islands_wake while sleeping is not applied (avn_islands_apply)");
+        if (!stepped_ || !isl_pending_ || wake_done_)
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_islands_wake runs once after every avn_contacts_step, before the solver stage");
+        const size_t B = isl_B_;
+        IslandState s = isl_;
+        if (wake && B) {
+            AVN_CUDA(isl_wake_.ensure(B));
+            AVN_CUDA(cudaMemcpyAsync(isl_wake_.p, wake, B, cudaMemcpyHostToDevice, stream_));
+            s.host_wake = isl_wake_.as<uint8_t>();
+        }
+        AVN_CUDA(cudaMemsetAsync(s.ctr, 0, sizeof(IslandCounters), stream_));
+        GraphRows g = graph_rows();
+        if (B) {
+            const unsigned bb = unsigned((B + 255) / 256);
+            if (g.hw > 0) isl_add_kernel<<<unsigned((g.hw + 255) / 256), 256, 0, stream_>>>(s, g);
+            isl_flatten_kernel<<<bb, 256, 0, stream_>>>(s, 0);
+            isl_wake_marks_kernel<<<bb, 256, 0, stream_>>>(s);
+            isl_wake_bodies_kernel<<<bb, 256, 0, stream_>>>(s);
+            isl_wake_roots_kernel<<<bb, 256, 0, stream_>>>(s);
+            AVN_CUDA(cudaGetLastError());
+        }
+        AVN_CUDA(cudaMemcpyAsync(h_isl_, s.ctr, sizeof(IslandCounters), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));   // (the caller's wake column may be reused)
+        wake_woken_ = h_isl_->woken;
+        wake_merges_ = h_isl_->merges;
+        wake_done_ = true;
+        *out = AvnIslandsWake{};
+        out->islands_woken = wake_woken_;
+        if (wake_woken_ || h_isl_->absorbed) {   // no woken island: the graph is the one avn_contacts_step left
+            const AvnStatus st = apply_pass(true, false);
+            if (st != AVN_OK) return st;
+            out->rows_woken = h_ctr_->rows_woken;
+            out->colouring_rounds = h_ctr_->rounds;
+        }
+        out->rows_asleep = rows_asleep_; out->bodies_asleep = bodies_asleep_; out->manifold_count = graph_.count;
+        memcpy(out->color_offsets, graph_.color_offsets, sizeof out->color_offsets);
+        return AVN_OK;
+    }
+
+    AvnStatus download_sleeping(uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep) override {
+        const size_t n = std::min(capacity, E_), nb = std::min(body_count, n_bodies_);
+        if (row_asleep && n) AVN_CUDA(cudaMemcpyAsync(row_asleep, asleep_.p, n, cudaMemcpyDeviceToHost, stream_));
+        if (body_asleep && nb) {
+            if (apply_) AVN_CUDA(cudaMemcpyAsync(body_asleep, body_asleep_.p, nb, cudaMemcpyDeviceToHost, stream_));
+            else memset(body_asleep, 0, nb);
+        }
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        return AVN_OK;
+    }
+
+    void asleep_bodies(AsleepBodies* out) override {
+        *out = AsleepBodies{};
+        if (!apply_) return;
+        out->body_asleep = body_asleep_.as<uint8_t>();
+        out->count = n_bodies_;
+        out->wake_skipped = isl_pending_ && !wake_done_;
     }
 
    private:
@@ -1338,7 +1509,8 @@ class Contacts final : public ContactsBase {
         AVN_CUDA(cudaMemsetAsync(ctr_.p, 0, offsetof(GraphCounters, ovf_count), stream_));   // (the step's counters went to the host already)
         GraphRows g = graph_rows();
         const unsigned rb = (hw_ + 255) / 256;
-        const int islands = !isl_configured_ ? 0 : isl_pending_ ? 2 : 1;
+        // (avn_islands_wake has applied the step's add events already: a contact it linked is unlinked like any other)
+        const int islands = !isl_configured_ ? 0 : (isl_pending_ && !(apply_ && wake_done_)) ? 2 : 1;
         remove_rows_kernel<<<rb, 256, 0, stream_>>>(g, rm_.as<uint8_t>(), isl_, islands, k0_.as<uint32_t>(), v0_.as<uint32_t>());
         radix_pass(int(hw_), evl_.as<uint32_t>());   // removed touching rows, then the other removed rows, each in ascending ContactId
         AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
@@ -1354,12 +1526,7 @@ class Contacts final : public ContactsBase {
         }
         // only touching rows hold a colour, and they lead the list in ascending ContactId: the overflow colour's swap_removes in that order
         overflow_list_kernel<<<1, 32, 0, stream_>>>(g, evl_.as<uint32_t>());
-        finalize_rows_kernel<<<rb, 256, 0, stream_>>>(g, k0_.as<uint32_t>(), v0_.as<uint32_t>());
-        radix_pass(int(hw_));
-        color_offsets_kernel<<<1, 64, 0, stream_>>>(g, k1_.as<uint32_t>(), v1_.as<uint32_t>());
-        gather_graph_kernel<S><<<std::min<unsigned>(rb, unsigned(sm_count_) * 8u), 256, 0, stream_>>>(g, v1_.as<uint32_t>(), have_fr_ ? fr_.as<double>() : nullptr,
-                                                                                                    have_re_ ? re_.as<double>() : nullptr, m_b1_.as<int32_t>(),
-                                                                                                    m_b2_.as<int32_t>(), m_fr_.as<S>(), m_re_.as<S>());
+        rebuild_list(g);
         AVN_CUDA(cudaMemsetAsync(table_.p, 0, (table_mask_ + 1) * sizeof(uint64_t), stream_));
         pair_set_kernel<<<rb, 256, 0, stream_>>>(g, table_.as<uint64_t>(), table_mask_);
         AVN_CUDA(cudaGetLastError());
@@ -1367,10 +1534,86 @@ class Contacts final : public ContactsBase {
         AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaStreamSynchronize(stream_));
         live_n_ -= n_rm;
+        rows_asleep_ = h_ctr_->rows_asleep;
+        take_list_counters();
+        return AVN_OK;
+    }
+    // Brings the applied state in line with the islands' decisions: body_asleep, then the rows of the woken islands (pushed by the colouring
+    // rounds in ascending ContactId), then the rows of the islands that fell asleep (popped; the overflow colour's swap_removes in ascending
+    // ContactId), then the colour-major list as a step leaves it.  The pair set does not change: an asleep row stays in the ContactGraph.
+    AvnStatus apply_pass(bool wakes, bool sleeps) {
+        // the step's counters went to the host and into AvnContactStep already; from here on the device block and h_ctr_ describe this pass, not
+        // the contact step (nothing reads the step's removed / started / stopped from them afterwards: the events come from the rows' event bytes)
+        AVN_CUDA(cudaMemsetAsync(ctr_.p, 0, offsetof(GraphCounters, ovf_count), stream_));
+        GraphRows g = graph_rows();
+        uint8_t* body_asleep = body_asleep_.as<uint8_t>();
+        uint8_t* fell = body_asleep + std::max<size_t>(n_bodies_, 1);
+        if (isl_B_) sleep_bodies_kernel<<<unsigned((size_t(isl_B_) + 255) / 256), 256, 0, stream_>>>(isl_, body_asleep, fell, g.ctr);
+        if (hw_) {
+            const unsigned rb = (hw_ + 255) / 256;
+            if (wakes) {
+                wake_rows_kernel<S><<<rb, 256, 0, stream_>>>(g, body_asleep, ws_n_in_.as<S>(), ws_t_in_.as<S>(), ws_n_out_.as<S>(), ws_t_out_.as<S>(),
+                                                             k0_.as<uint32_t>(), v0_.as<uint32_t>());
+                radix_pass(int(hw_), list_.as<uint32_t>());   // the pushes first, in ascending ContactId
+                const AvnStatus st = colour_changed(g);
+                if (st != AVN_OK) return st;
+                overflow_list_kernel<<<1, 32, 0, stream_>>>(g, list_.as<uint32_t>());
+            }
+            if (sleeps) {
+                if (wakes) AVN_CUDA(cudaMemsetAsync(&g.ctr->changed, 0, sizeof(uint32_t), stream_));   // the list below is the sleeping rows' alone
+                sleep_rows_kernel<<<rb, 256, 0, stream_>>>(g, fell, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+                radix_pass(int(hw_), list_.as<uint32_t>());
+                overflow_list_kernel<<<1, 32, 0, stream_>>>(g, list_.as<uint32_t>());
+            }
+            rebuild_list(g);
+            AVN_CUDA(cudaGetLastError());
+        }
+        AVN_CUDA(cudaMemcpyAsync(h_ctr_, ctr_.p, sizeof(GraphCounters), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        if (h_ctr_->aborted) return err_->fail(AVN_ERR_CUDA, "islands: the colouring of the woken rows did not converge");
+        bodies_asleep_ = h_ctr_->bodies_asleep;
+        rows_asleep_ = h_ctr_->rows_asleep;
+        if (hw_) take_list_counters();
+        return AVN_OK;
+    }
+    // ConstraintGraph pushes / pops of the rows list_[0, ctr->changed) in ascending ContactId: the dependency wavefront (see the top of the file)
+    AvnStatus colour_changed(GraphRows& g) {
+        AVN_CUDA(cudaMemsetAsync(body_min_.p, 0xff, std::max<size_t>(n_bodies_, 1) * 16, stream_));
+        if (use_cluster_) {   // small change sets: one thread-block cluster (returns at once when there are more than CL_MAX changed edges)
+            cudaLaunchConfig_t cfg{};
+            cfg.gridDim = dim3(CL_BLOCKS); cfg.blockDim = dim3(CL_THREADS); cfg.dynamicSmemBytes = 0; cfg.stream = stream_;
+            cudaLaunchAttribute attr[1];
+            attr[0].id = cudaLaunchAttributeClusterDimension;
+            attr[0].val.clusterDim.x = CL_BLOCKS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+            cfg.attrs = attr; cfg.numAttrs = 1;
+            const uint32_t* list = list_.as<uint32_t>();
+            cudaError_t ce = cudaLaunchKernelEx(&cfg, colour_rounds_cluster_kernel, g, list);
+            if (ce != cudaSuccess) { (void)cudaGetLastError(); use_cluster_ = false; }
+        }
+        const uint32_t* list = list_.as<uint32_t>();
+        uint32_t skip_upto = use_cluster_ ? CL_MAX : 0u;
+        void* args[] = {(void*)&g, (void*)&list, (void*)&skip_upto};
+        int per_sm = 0;
+        AVN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, colour_rounds_kernel, 256, 0));
+        if (per_sm < 1) return err_->fail(AVN_ERR_CUDA, "contacts_step: the colouring kernel does not fit the device");
+        AVN_CUDA(cudaLaunchCooperativeKernel((const void*)colour_rounds_kernel, dim3(sm_count_), dim3(256), args, 0, stream_));
+        return AVN_OK;
+    }
+    // the colour-major list from the rows' colours: frees the removed rows, one stable radix pass over the colour byte -> k1_ sorted colour keys,
+    // v1_ = the list (ascending ContactId inside a colour), then the offsets and the per-manifold columns
+    void rebuild_list(const GraphRows& g) {
+        const unsigned rb = (hw_ + 255) / 256;
+        finalize_rows_kernel<<<rb, 256, 0, stream_>>>(g, k0_.as<uint32_t>(), v0_.as<uint32_t>());
+        radix_pass(int(hw_));
+        color_offsets_kernel<<<1, 64, 0, stream_>>>(g, k1_.as<uint32_t>(), v1_.as<uint32_t>());
+        gather_graph_kernel<S><<<std::min<unsigned>(rb, unsigned(sm_count_) * 8u), 256, 0, stream_>>>(g, v1_.as<uint32_t>(), have_fr_ ? fr_.as<double>() : nullptr,
+                                                                                                    have_re_ ? re_.as<double>() : nullptr, m_b1_.as<int32_t>(),
+                                                                                                    m_b2_.as<int32_t>(), m_fr_.as<S>(), m_re_.as<S>());
+    }
+    void take_list_counters() {   // h_ctr_ holds the counters rebuild_list left
         graph_.count = h_ctr_->manifolds;
         graph_.any_restitution = h_ctr_->any_restitution;
         memcpy(graph_.color_offsets, h_ctr_->color_offsets, sizeof graph_.color_offsets);
-        return AVN_OK;
     }
     GraphRows graph_rows() {
         GraphRows g{};
@@ -1379,7 +1622,7 @@ class Contacts final : public ContactsBase {
         g.live = live_.as<uint8_t>(); g.count = count_.as<uint8_t>(); g.disjoint = disjoint_.as<uint8_t>(); g.prev_count = prev_count_.as<uint8_t>();
         g.pflags = pflags_.as<uint8_t>(); g.touching = touching_.as<uint8_t>(); g.colour = colour_.as<uint8_t>(); g.change = change_.as<uint8_t>();
         g.old_colour = old_colour_.as<uint8_t>(); g.ovf_pos = ovf_pos_.as<uint32_t>(); g.ovf = ovf_.as<uint32_t>(); g.isl_event = isl_event_.as<uint8_t>(); g.fresh = fresh_.as<uint8_t>();
-        g.event = event_.as<uint8_t>(); g.sensor = sensor_h_.empty() ? nullptr : sensor_.as<uint8_t>();
+        g.event = event_.as<uint8_t>(); g.asleep = asleep_.as<uint8_t>(); g.sensor = sensor_h_.empty() ? nullptr : sensor_.as<uint8_t>();
         g.body_kind = kind_.as<uint8_t>(); g.n_bodies = int(n_bodies_);
         g.body_bits = body_bits_.as<uint32_t>(); g.body_min = body_min_.as<unsigned long long>();
         g.ctr = ctr_.as<GraphCounters>();
@@ -1393,6 +1636,7 @@ class Contacts final : public ContactsBase {
         r.pen = pen_.as<S>(); r.ns = ns_.as<S>(); r.prev_count = prev_count_.as<uint8_t>(); r.prev_a1 = prev_a1_.as<double>(); r.prev_a2 = prev_a2_.as<double>();
         r.ws_n_in = ws_n_in_.as<S>(); r.ws_t_in = ws_t_in_.as<S>(); r.ws_n_out = ws_n_out_.as<S>(); r.ws_t_out = ws_t_out_.as<S>();
         r.nimp_in = nimp_in_.as<S>(); r.nimp_out = nimp_out_.as<S>();
+        r.asleep = asleep_.as<uint8_t>();
         return r;
     }
     template <class T> AvnStatus up(DevBuf& buf, const void* host, size_t count, const T** dev) {
@@ -1430,6 +1674,10 @@ class Contacts final : public ContactsBase {
     ResidentGraph graph_{};
     // collision events, sensors, removals, reports
     DevBuf event_, evl_, evout_, repout_, bounds_, sensor_, rm_, pend_[2];
+    // applied sleeping: asleep_ per row; body_asleep_ = [B] applied state, then [B] "fell asleep in this pass"
+    DevBuf asleep_, body_asleep_, isl_wake_;
+    bool apply_ = false, wake_done_ = false;
+    uint32_t bodies_asleep_ = 0, rows_asleep_ = 0, wake_woken_ = 0, wake_merges_ = 0;
     std::vector<uint8_t> sensor_h_;           // the sensor column as last set (empty = no sensor)
     uint32_t pend_n_[2] = {0, 0}, pend_cap_[2] = {0, 0};
     int pend_cur_ = 0;                        // pend_[pend_cur_] queues the removals' CollisionEnds; the other list is reported with the last step

@@ -177,6 +177,16 @@ struct ContactsBase {
     // ---- persistent simulation islands + sleeping decisions (contacts.cu)
     virtual AvnStatus islands_configure(const AvnIslandsConfig* cfg) = 0;
     virtual AvnStatus islands_step(AvnIslandsStep* step) = 0;
+    // ---- applied sleeping (contacts.cu): the switch, the narrow-phase half of the island step, and what the solver stage needs of it
+    virtual AvnStatus islands_apply(uint32_t enable) = 0;
+    virtual AvnStatus islands_wake(const uint8_t* wake, AvnIslandsWake* out) = 0;
+    virtual AvnStatus download_sleeping(uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep) = 0;
+    struct AsleepBodies {           // body_asleep: device column [count], NULL while application is off
+        const uint8_t* body_asleep = nullptr;
+        uint32_t count = 0;
+        bool wake_skipped = false;  // avn_islands_wake has not run for the current contact step
+    };
+    virtual void asleep_bodies(AsleepBodies* out) = 0;
     // ---- the rows and collider shapes swept CCD visits (ccd.cu)
     virtual void ccd_rows(CcdRows* out) = 0;
 };

@@ -277,6 +277,8 @@ class Solver final : public SolverBase {
     bool have_m_ = false, have_j_ = false;
 
     // device storage
+    const uint8_t* body_asleep_ = nullptr;   // upload_resident: the contact store's applied sleeping state for the upload in progress
+    DevBuf b_kind_eff_;
     DevBuf b_kind_, b_locked_, b_dom_, b_iflags_, b_pos_, b_rot_, b_lv_, b_av_, b_im_, b_iil_, b_com_, b_ld_, b_ad_, b_gs_, b_la_, b_aa_, b_ml_, b_ma_;
     DevBuf o_pos_, o_rot_, o_lv_, o_av_;
     DevBuf s_inr_, s_itg_, s_pre_;
@@ -345,6 +347,14 @@ AvnStatus Solver<S>::upload_edges(const AvnStepParams* prm, AvnBodyColumns* bc, 
 template <class S>
 AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* bc, ContactsBase* contacts, AvnJointSet* js) {
     if (!contacts) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: no contact store");
+    ContactsBase::AsleepBodies asleep;
+    contacts->asleep_bodies(&asleep);
+    if (asleep.wake_skipped)
+        return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: sleeping is applied (avn_islands_apply) and avn_islands_wake has not run since the last avn_contacts_step");
+    if (asleep.body_asleep && asleep.count != bc->count)
+        return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: %zu bodies, sleeping is applied to %u", size_t(bc->count), asleep.count);
+    struct Reset { const uint8_t*& p; ~Reset() { p = nullptr; } } reset{body_asleep_};   // only this upload reads the column
+    body_asleep_ = asleep.body_asleep;
     from_store_ = true;
     ContactsBase::ResidentGraph g;
     AvnStatus st = contacts->graph_view(&g);
@@ -405,6 +415,12 @@ AvnStatus Solver<S>::upload_graph(const AvnStepParams* prm, AvnBodyColumns* bc, 
         memcpy(graph_color_offsets_, g->color_offsets, sizeof graph_color_offsets_);
     }
     return st;
+}
+
+// the kind column the stage runs with while sleeping is applied: asleep -> static (kind == NULL: every body is dynamic)
+__global__ void effective_kind_kernel(int B, const uint8_t* __restrict__ kind, const uint8_t* __restrict__ body_asleep, uint8_t* __restrict__ out) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < B) out[b] = body_asleep[b] ? uint8_t(AVN_BODY_STATIC) : kind ? kind[b] : uint8_t(AVN_BODY_DYNAMIC);
 }
 
 // fills the point ranges of the manifolds of an edge-indexed upload: 4 slots per edge, the first point_count[edge] of them live
@@ -473,6 +489,14 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
         if ((st = upload_body_columns(*bc, false, d)) != AVN_OK) return st;
     }
     prefetched_ = false;
+    if (body_asleep_ && B) {
+        // a body that is asleep has no SolverBody (solver_body/plugin.rs:46-110): the stage sees it as static.  The uploaded column stays as it is
+        // for AVN_BODIES_STATIC_UNCHANGED
+        AVN_CUDA(b_kind_eff_.ensure(B));
+        effective_kind_kernel<<<unsigned((B + 255) / 256), 256, 0, stream_>>>(int(B), d.kind, body_asleep_, b_kind_eff_.as<uint8_t>());
+        AVN_CUDA(cudaGetLastError());
+        d.kind = b_kind_eff_.as<uint8_t>();
+    }
     AVN_CUDA(o_pos_.ensure(3 * B * sizeof(S) + 16)); d.out_position = o_pos_.as<S>();
     AVN_CUDA(o_rot_.ensure(4 * B * sizeof(S) + 16)); d.out_rotation = o_rot_.as<S>();
     AVN_CUDA(o_lv_.ensure(3 * B * sizeof(S) + 16)); d.out_linvel = o_lv_.as<S>();

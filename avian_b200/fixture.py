@@ -48,6 +48,13 @@ def _load():
         lib.avh_raw_manifolds.restype = None
         lib.avh_remove_colliders.argtypes = [_vp, C.c_uint32, _vp]
         lib.avh_remove_colliders.restype = None
+        for fn in (lib.avh_sleep_edges, lib.avh_wake_edges):
+            fn.argtypes = [_vp, C.c_uint32, _vp]
+            fn.restype = None
+        lib.avh_graph_size.argtypes = [_vp, C.POINTER(C.c_uint32)]
+        lib.avh_graph_size.restype = C.c_uint32
+        lib.avh_edge_states.argtypes = [_vp, _vp, _vp, _vp]
+        lib.avh_edge_states.restype = C.c_uint32
         lib.avh_set_sensors.argtypes = [_vp, _vp]
         lib.avh_set_sensors.restype = None
         lib.avh_events.argtypes = [_vp, C.c_uint32] + [_vp] * 5
@@ -275,7 +282,14 @@ class HostPipeline:
         kind = np.ascontiguousarray(bodies.kind, dtype=np.uint8)
         m = int(self.lib.avh_narrow_phase(self.h, self.bits, _p(kind), _p(bodies.position), _p(bodies.rotation), _p(bodies.linear_velocity),
                                           _p(bodies.angular_velocity), _p(aabb_min), _p(aabb_max), dt, 1 if match_contacts else 0, C.byref(pts)))
-        p = int(pts.value)
+        return self.export_manifolds(m, int(pts.value))
+
+    def export_manifolds(self, m: int | None = None, p: int | None = None) -> api.Manifolds:
+        """The constraint graph's manifolds grouped by colour (m manifolds with p points; None = ask the graph, e.g. after wake_edges)."""
+        if m is None:
+            pts = C.c_uint32(0)
+            m = int(self.lib.avh_graph_size(self.h, C.byref(pts)))
+            p = int(pts.value)
         s = self.scalar
         man = api.Manifolds(
             color_offsets=np.zeros(api.GRAPH_COLOR_COUNT + 1, dtype=np.uint32), body1=np.zeros(m, dtype=np.int32), body2=np.zeros(m, dtype=np.int32),
@@ -323,6 +337,24 @@ class HostPipeline:
     def remove_colliders(self, colliders) -> None:
         ids = np.ascontiguousarray(colliders, dtype=np.uint32)
         self.lib.avh_remove_colliders(self.h, int(ids.shape[0]), _p(ids))
+
+    def sleep_edges(self, ids) -> None:
+        """ContactGraph::sleep_entity_with for these ContactIds (ascending): out of the ConstraintGraph, skipped by the narrow phase."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        self.lib.avh_sleep_edges(self.h, int(ids.shape[0]), _p(ids))
+
+    def wake_edges(self, ids) -> None:
+        """ContactGraph::wake_entity_with for these ContactIds (ascending): touching, constraint-generating pairs are pushed again."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        self.lib.avh_wake_edges(self.h, int(ids.shape[0]), _p(ids))
+
+    def edge_states(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """(ContactId, touching, asleep) of every live pair, ascending ContactId."""
+        n = int(self.lib.avh_edge_states(self.h, None, None, None))
+        ids, t, a = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint8), np.zeros(n, dtype=np.uint8)
+        if n:
+            self.lib.avh_edge_states(self.h, _p(ids), _p(t), _p(a))
+        return ids, t.astype(bool), a.astype(bool)
 
     def events(self) -> tuple[dict, dict]:
         """(started, ended) of the last status loop, as Context.contacts_events returns them."""

@@ -67,6 +67,7 @@ struct Pair {
     uint32_t collider1, collider2, body1, body2;
     uint8_t flags;                 // AVN_PAIR_*
     bool alive = false, touching = false, static1 = false, static2 = false;
+    bool asleep = false;           // in ContactGraph::sleeping_pairs (avh_sleep_edges): out of the ConstraintGraph, skipped by the narrow phase
     std::vector<Manifold> manifolds;
     std::vector<Handle> handles;   // ContactEdge::constraint_handles
 };
@@ -267,6 +268,16 @@ void avh_add_pairs(AvhPipeline* h, const uint32_t* c1, const uint32_t* c2, const
     }
 }
 
+// the manifolds in the constraint graph; *out_points = their points
+static uint32_t graph_size(const Pipeline& P, uint32_t* out_points) {
+    uint32_t M = 0, Pn = 0;
+    for (int c = 0; c < AVN_GRAPH_COLOR_COUNT; ++c)
+        for (auto& hnd : P.colors[c].handles) { ++M; Pn += uint32_t(P.pairs[hnd.first].manifolds[hnd.second].pts.size()); }
+    if (out_points) *out_points = Pn;
+    return M;
+}
+uint32_t avh_graph_size(AvhPipeline* h, uint32_t* out_points) { return graph_size(*reinterpret_cast<Pipeline*>(h), out_points); }
+
 // The second half of NarrowPhase::update: status changes in ascending ContactId (system_param.rs:136-389) -> ContactGraph removals and
 // ConstraintGraph push / pop.  Returns the number of manifolds in the constraint graph; *out_points = their points.
 static uint32_t apply_status_changes(Pipeline& P, std::vector<uint32_t>& changed, const std::vector<uint8_t>& disjoint, const std::vector<uint8_t>& started,
@@ -301,11 +312,7 @@ static uint32_t apply_status_changes(Pipeline& P, std::vector<uint32_t>& changed
             for (int k = 0; k < -count_change[id]; ++k) pop_manifold(P, id);
         }
     }
-    uint32_t M = 0, Pn = 0;
-    for (int c = 0; c < AVN_GRAPH_COLOR_COUNT; ++c)
-        for (auto& hnd : P.colors[c].handles) { ++M; Pn += uint32_t(P.pairs[hnd.first].manifolds[hnd.second].pts.size()); }
-    if (out_points) *out_points = Pn;
-    return M;
+    return graph_size(P, out_points);
 }
 
 // remove_collider (narrow_phase/mod.rs:399-459) for each listed collider: every pair that names one of them, in ascending ContactId (the device's
@@ -325,6 +332,45 @@ void avh_remove_colliders(AvhPipeline* h, uint32_t n, const uint32_t* colliders)
         pr = Pair{};
         P.free_ids.push(id);
     }
+}
+
+// ContactGraph::sleep_entity_with / wake_entity_with (contact_graph.rs:702-826) for the listed ContactIds, in ascending id (the device's stated
+// order): a pair put to sleep leaves the ConstraintGraph and keeps its manifolds and impulses; a woken pair that is touching and generates
+// constraints is pushed again.  Which edges follow which island is the caller's business.
+void avh_sleep_edges(AvhPipeline* h, uint32_t n, const uint32_t* ids) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    std::vector<uint32_t> list(ids, ids + n);
+    std::sort(list.begin(), list.end());
+    for (uint32_t id : list) {
+        Pair& pr = P.pairs[id];
+        if (!pr.alive || pr.asleep) continue;
+        pr.asleep = true;
+        while (!pr.handles.empty()) pop_manifold(P, id);
+    }
+}
+void avh_wake_edges(AvhPipeline* h, uint32_t n, const uint32_t* ids) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    std::vector<uint32_t> list(ids, ids + n);
+    std::sort(list.begin(), list.end());
+    for (uint32_t id : list) {
+        Pair& pr = P.pairs[id];
+        if (!pr.alive || !pr.asleep) continue;
+        pr.asleep = false;
+        if (pr.touching && (pr.flags & AVN_PAIR_GENERATE_CONSTRAINTS))
+            for (size_t k = 0; k < pr.manifolds.size(); ++k) push_manifold(P, id);
+    }
+}
+// per live pair: ContactId, touching, asleep (arrays sized avh_pair_count(); may be NULL to count)
+uint32_t avh_edge_states(AvhPipeline* h, uint32_t* ids, uint8_t* touching, uint8_t* asleep) {
+    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    uint32_t n = 0;
+    for (uint32_t id = 0; id < P.pairs.size(); ++id) {
+        const Pair& pr = P.pairs[id];
+        if (!pr.alive) continue;
+        if (ids) { ids[n] = id; touching[n] = pr.touching; asleep[n] = pr.asleep; }
+        ++n;
+    }
+    return n;
 }
 
 // The Sensor column (NULL = none): the On<Add, Sensor> / On<Remove, Sensor> observers run remove_collider for every collider whose flag changed.
@@ -409,6 +455,7 @@ uint32_t avh_narrow_phase(AvhPipeline* h, uint32_t scalar_bits, const uint8_t* k
     Contacts pts;
     for (uint32_t id : P.active) {
         Pair& pr = P.pairs[id];
+        if (pr.asleep) continue;   // update_contacts runs over active_pairs only
         const uint32_t a = pr.collider1, b = pr.collider2;
         V3 mina = amin.v3(a), maxa = amax.v3(a), minb = amin.v3(b), maxb = amax.v3(b);
         bool overlap = !(mina.x > maxb.x || maxa.x < minb.x || mina.y > maxb.y || maxa.y < minb.y || mina.z > maxb.z || maxa.z < minb.z);
@@ -588,6 +635,7 @@ uint32_t avh_apply_counts(AvhPipeline* h, const uint8_t* kind, const uint32_t* i
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t id = ids[i];
         Pair& pr = P.pairs[id];
+        if (pr.asleep) continue;
         if (disjoint_in[i]) { disjoint[id] = 1; changed.push_back(id); continue; }
         pr.static1 = kind[pr.body1] == AVN_BODY_STATIC;
         pr.static2 = kind[pr.body2] == AVN_BODY_STATIC;

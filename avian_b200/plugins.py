@@ -474,14 +474,51 @@ class DeviceResidentWorld(World):
         return mn, mx
 
 
+def island_joint_bodies(joints: "api.JointSet | None") -> np.ndarray | None:
+    """[J, 2] the bodies every joint links, in type order: what PhysicsIslands::add_joint sees (avn_islands_configure)."""
+    if joints is None or not joints.count:
+        return None
+    return np.concatenate([np.stack([t.body1, t.body2], axis=1) for t in joints.types.values() if t.count]).astype(np.uint32)
+
+
+def awake_joints(joints: "api.JointSet | None", still: np.ndarray):
+    """The joints the solver runs while sleeping is applied: a joint whose two bodies are both `still` (asleep or static) is left out, the
+    others keep their order (a joint links its bodies' islands, so it is never half asleep).  Returns (joint set, kept) where kept[type] is
+    the mask of the joints taken, for `restore_joint_outputs`; (joints, None) when nothing is left out."""
+    if joints is None or not joints.count or not still.any():
+        return joints, None
+    kept = {t: ~(still[j.body1] & still[j.body2]) for t, j in joints.types.items()}
+    if all(k.all() for k in kept.values()):
+        return joints, None
+    sub = api.JointSet({t: api.Joints(**{n: (None if v is None else np.ascontiguousarray(v[kept[t]])) for n, v in j.__dict__.items()})
+                        for t, j in joints.types.items()})
+    return sub, kept
+
+
+def restore_joint_outputs(joints: "api.JointSet", sub: "api.JointSet", kept: dict | None) -> None:
+    """the solver's joint outputs (force, torque) of the joints that ran, back in the full set"""
+    if kept is None:
+        return
+    for t, j in joints.types.items():
+        for n in ("force", "torque"):
+            if getattr(j, n) is not None:
+                getattr(j, n)[kept[t]] = getattr(sub.types[t], n)
+
+
 class DeviceGraphWorld(World):
     """The whole contact pipeline on the device (SURVEY.md 8f #1 + #3): broad phase -> new pairs taken in device memory by the contact store ->
     geometry + match_contacts -> touching state machine, ContactGraph, ConstraintGraph colouring, colour-major list -> solver stage reading
     all of it in place (avn_contacts_step + avn_solver_upload_resident).  The host keeps the body columns and the persistent interval order;
     per step it sends the AABB and body columns and reads back the order, ~40 counters and the bodies.  Steps bit for bit like World
-    (tests/test_gpu_graph.py): same ContactIds, same colours, same bodies."""
+    (tests/test_gpu_graph.py): same ContactIds, same colours, same bodies.
 
-    def __init__(self, scene: Scene, plugins: PhysicsPlugins, ctx: "api.Context", **kw):
+    sleeping: None, or the keyword arguments of api.Context.islands_configure besides the bodies and the joints (time_to_sleep, thr_lin,
+    thr_ang, disabled, length_unit).  The world then configures the islands, lets the library apply their decisions (avn_islands_apply) and
+    steps  broad phase (sleeping bodies' intervals inactive) -> contacts_step -> islands_wake -> solver -> islands_step.  `wake` ([B], optional,
+    consumed by the next step) marks bodies the application touched before the step, `late_wake` bodies it touched after the solve.  `sleeping_flags`, `island`, `sleep_timer`, `islands` hold the last
+    islands_step's output, `wake_stats` the last islands_wake's."""
+
+    def __init__(self, scene: Scene, plugins: PhysicsPlugins, ctx: "api.Context", sleeping: dict | None = None, **kw):
         super().__init__(scene, plugins, **kw)
         self.ctx = ctx
         n = int(scene.bodies.count)
@@ -498,15 +535,35 @@ class DeviceGraphWorld(World):
         self._uploaded_once = False     # from the second step on the static columns (shapes, mass properties ...) stay on the device
         if self.ccd is not None:
             ctx.ccd_configure(**self.ccd)   # solve_swept_ccd inside the device-resident solver stage
+        self.sleeping = sleeping
+        self.wake: np.ndarray | None = None
+        self.late_wake: np.ndarray | None = None     # bodies touched after the solve: passed to islands_step, awake from the next step on
+        self.sleeping_flags = np.zeros(n, dtype=np.uint8)
+        self.island = np.arange(n, dtype=np.uint32)
+        self.sleep_timer = np.zeros(n, dtype=np.float32)
+        self.islands: dict | None = None
+        self.wake_stats: dict | None = None
+        if sleeping is not None:
+            ctx.islands_configure(self.bodies.kind, joints=island_joint_bodies(self.joints), **sleeping)
+            ctx.islands_apply(True)
 
     def intervals(self, aabb_min: np.ndarray, aabb_max: np.ndarray) -> api.Aabbs:
         o, kind = self.order, self.bodies.kind
         flags = np.where(kind[o] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
         flags = self.interval_flags(o, flags)
+        if self.sleeping is not None:      # Has<Sleeping> when the intervals are refreshed (broad_phase.rs:223-260), minus the islands about to wake
+            flags = flags | np.where(self.inactive_bodies()[o], api.AABB_IS_INACTIVE, 0).astype(np.uint8)
         a = api.Aabbs(collider=o.copy(), body=o.copy(), aabb_min=np.ascontiguousarray(aabb_min[o]), aabb_max=np.ascontiguousarray(aabb_max[o]),
                       flags=np.ascontiguousarray(flags), order_out=self._order_out)
         a.joint_disabled_body_pairs = self.scene.joint_disabled_body_pairs
         return a
+
+    def inactive_bodies(self) -> np.ndarray:
+        """the bodies that enter this step's broad phase asleep: the last islands_step's Sleeping flags minus the islands `wake` reaches"""
+        asleep = self.sleeping_flags.astype(bool)
+        if self.wake is not None and asleep.any():
+            asleep &= ~np.isin(self.island, self.island[np.nonzero(self.wake)[0]])
+        return asleep
 
     def step_from(self, aabbs: api.Aabbs, aabb_min: np.ndarray, aabb_max: np.ndarray) -> dict:
         """One step from host columns: `aabbs` = the interval columns in the persistent order, aabb_min / aabb_max = the same AABBs in collider order."""
@@ -525,7 +582,23 @@ class DeviceGraphWorld(World):
             self.order = np.ascontiguousarray(aabbs.collider[oo])
         if self.sensor is not None or self.events_enabled is not None:
             self.events = ctx.contacts_events()
-        ctx.solver_step_resident(self.params, b, self.joints)
+        if self.sleeping is None:
+            ctx.solver_step_resident(self.params, b, self.joints)
+        else:
+            self.wake_stats = ctx.islands_wake(self.wake)
+            self.wake = None
+            # the bodies asleep after the wake half are a subset of the last island step's flags: the same count means the same set
+            still = self.sleeping_flags.astype(bool)
+            if self.wake_stats["bodies_asleep"] == 0:
+                still = np.zeros(self.n, dtype=bool)
+            elif self.wake_stats["bodies_asleep"] != int(still.sum()):
+                still = ctx.contacts_download_sleeping(0, self.n)["body_asleep"].astype(bool)
+            joints, kept = awake_joints(self.joints, still | (b.kind == api.BODY_STATIC))
+            ctx.solver_step_resident(self.params, b, joints)
+            restore_joint_outputs(self.joints, joints, kept)
+            self.islands = ctx.islands_step(float(self.params.dt), b.linear_velocity, b.angular_velocity, wake=self.late_wake)
+            self.late_wake = None
+            self.sleeping_flags, self.island, self.sleep_timer = self.islands["sleeping"], self.islands["island"], self.islands["sleep_timer"]
         self._uploaded_once = True
         self.step_index += 1
         return self.stats

@@ -593,7 +593,8 @@ AvnStatus avn_contacts_remove_colliders(AvnContext* ctx, uint32_t n, const uint3
 AvnStatus avn_contacts_events(AvnContext* ctx, AvnCollisionEvents* started, AvnCollisionEvents* ended);
 /* ContactPair::total_normal_impulse / max_normal_impulse (contact_types/mod.rs:227-277) of the touching pairs as the last solve left them:
  * call it after avn_solver_run.  Geometry from this step's narrow phase, impulses from store_contact_impulses (solver/plugin.rs:722-754).  A row
- * that was not solved this step (a sensor pair) reports 0 impulses, as the reference's fresh points do.  flags: AVN_REPORT_*. */
+ * that was not solved this step (a sensor pair) reports 0 impulses, as the reference's fresh points do; a row that is asleep
+ * (avn_islands_apply) is listed with the impulses of its last solve.  flags: AVN_REPORT_*. */
 AvnStatus avn_contacts_report(AvnContext* ctx, uint32_t flags, AvnContactReport* out);
 
 /* ---- simulation islands and sleeping on the device (SURVEY.md 8f "next #4").  Replaces the bookkeeping and the decisions of
@@ -603,8 +604,8 @@ AvnStatus avn_contacts_report(AvnContext* ctx, uint32_t flags, AvnContactReport*
  *      marked (constraints_removed) when such a contact goes, and split lazily — one island per step, the one holding the sleepiest body
  *      that wants to sleep — by recomputing its connected components.  The contact events come from the last avn_contacts_step of this
  *      context (the rows on the device); the body velocities are the solver's results of the same step.  Output: island label and Sleeping
- *      flag per body; APPLYING a decision (taking a sleeping body's constraints out of the step, `Sleeping` component) stays with the host
- *      shim, like the reference's SleepIslands / WakeIslands commands.
+ *      flag per body.  APPLYING a decision is opt-in (avn_islands_apply below): the library then plays the SleepIslands / WakeIslands commands
+ *      on its own rows, graphs and solver stage, and the shim only mirrors the flags (`Sleeping` component, AVN_AABB_IS_INACTIVE).
  *      One deviation, stated: the reference tracks the split candidate as an island id that a merge can retire (when the candidate is the
  *      smaller island of the merge); here the candidate is the sleepiest BODY, and the island that holds it one step later is split. -------- */
 typedef struct AvnIslandsConfig {
@@ -634,6 +635,45 @@ typedef struct AvnIslandsStep {
 } AvnIslandsStep;
 /* Once per step, after avn_contacts_step and the solver stage of the same step (it consumes that step's contact events). */
 AvnStatus avn_islands_step(AvnContext* ctx, AvnIslandsStep* step);
+
+/* ---- applying sleeping and waking on the device (SleepIslands::apply / WakeIslands::apply, islands/sleeping.rs:354-533; opt-in).
+ *      State: one `asleep` byte per contact row and one per body.  When an island is put to sleep every touching row of its bodies leaves the
+ *      ConstraintGraph (ContactGraph::sleep_entity_with, contact_graph.rs:765-826) and keeps its manifold, matched anchors and impulses
+ *      untouched: avn_contacts_step neither narrow-phases nor classifies an asleep row, so it produces no event.  A body that is asleep enters the
+ *      solver stage of avn_solver_upload_resident as AVN_BODY_STATIC (no SolverBody: not integrated, not written back; its velocities stay as
+ *      they are — the reference does not zero them either).  When the island wakes the rows are pushed back (wake_entity_with, :702-763) and
+ *      the solve warm-starts from the impulses of the last solve before the sleep.  An edge follows EITHER endpoint, as in the reference: a
+ *      touching sensor pair between a sleeping body and an awake body of another island sleeps with the first and is not updated until one of
+ *      the two islands wakes.  avn_contacts_report lists asleep rows with the impulses of their last solve; avn_contacts_remove_colliders and
+ *      avn_contacts_set_sensors remove them like any other row.  The broad phase is not changed: the caller sets AVN_AABB_IS_INACTIVE on the
+ *      intervals of the bodies whose `sleeping` flag the last avn_islands_step returned.
+ *      Stated deviations: woken rows are pushed, and rows put to sleep leave the overflow colour, in ascending ContactId (the reference walks each
+ *      island's body list and each collider's edge list).  The colouring is the sequential greedy result for that order and conflict-free,
+ *      but after a wake a manifold may hold another colour than in the reference, and the colours are the Gauss-Seidel order.
+ *      Order of one step:  avn_contacts_step -> avn_islands_wake -> avn_solver_upload_resident / run / download -> avn_islands_step. -------- */
+/* enable != 0: from now on the decisions are applied.  AVN_ERR_UNSUPPORTED before avn_islands_configure (whose body count must equal
+ * avn_contacts_configure's) and while avn_ccd_configure holds a body list (avn_ccd_configure is refused the same way while application is on).
+ * enable == 0: every sleeping island is woken first, then the context behaves as if the call had never been made; only between steps
+ * (AVN_ERR_INVALID_ARGUMENT between avn_contacts_step and the avn_islands_step that ends the step).
+ * While application is on avn_contacts_configure and avn_islands_configure return AVN_ERR_UNSUPPORTED: turn it off, reconfigure, turn it on. */
+AvnStatus avn_islands_apply(AvnContext* ctx, uint32_t enable);
+
+typedef struct AvnIslandsWake {
+    uint32_t islands_woken;              /* islands woken by this call */
+    uint32_t rows_woken;                 /* contact rows that left the sleeping set */
+    uint32_t rows_asleep, bodies_asleep; /* now */
+    uint32_t manifold_count;             /* of the list the solver will read */
+    uint32_t colouring_rounds;           /* of the woken rows' pushes; 0 when no island woke (the list is avn_contacts_step's) */
+    uint32_t color_offsets[AVN_GRAPH_COLOR_COUNT + 1];   /* the colour-major list as the solver will read it (AvnContactStep's values are stale after a wake) */
+} AvnIslandsWake;
+/* The narrow-phase half of the island step (system_param.rs:253-258 queues WakeIslands, applied before the solver of the same step): links the
+ * islands of the contacts that started touching, wakes the sleeping islands they reach and the islands of the bodies marked in `wake`
+ * ([B] or NULL), and pushes the woken islands' rows after the step's own changes.  Once per step between avn_contacts_step and
+ * avn_solver_upload_resident, which returns AVN_ERR_INVALID_ARGUMENT when application is on and this call was skipped.  avn_islands_step then
+ * skips what was done here.  AVN_ERR_UNSUPPORTED while application is off. */
+AvnStatus avn_islands_wake(AvnContext* ctx, const uint8_t* wake, AvnIslandsWake* out);
+/* tests, tools: row_asleep [capacity], body_asleep [body_count]; either may be NULL */
+AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep);
 
 /* ---- spatial queries (SpatialQueryPlugin, src/lib.rs:839; spatial_query/pipeline.rs): a collider tree rebuilt on the device by every
  *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid and sphere colliders.
