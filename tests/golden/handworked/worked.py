@@ -8,8 +8,12 @@ inputs and results as `vectors.json`; tests/test_handworked.py demands that BOTH
 
 Every function cites the Rust it restates (paths relative to the reference root, avianphysics/avian @ 5bef382).  glam 0.30.8 is not in
 the reference tree; its primitives are restated from its published algorithms (scalar formulas; glam's SSE2 `Quat` may associate a
-product differently in the last bit, which is why the vectors are compared at 1e-5 relative, not bit for bit).
+product differently in the last bit, which is why the vectors are compared at 1e-5 relative, not bit for bit — `step(...,
+quat_product="sse2")` evaluates the f32 quaternion product in the SSE2 association instead).
 f32 transcendentals are taken correctly rounded (evaluated in double, rounded once).
+
+Beyond the tiny vectors, tests/test_wave_scenes_cpu.py evaluates `step` on generated scenes of up to a few hundred manifolds (speed
+limits, custom-integration markers, accelerations, full local inverse inertia, several solver iterations) against the oracle.
 """
 import math
 
@@ -60,6 +64,18 @@ def quat_mul(q, r):   # Hamilton product q * r, glam Quat::mul_quat; components 
         ((w0 * y1 - x0 * z1) + y0 * w1) + z0 * x1,
         ((w0 * z1 + x0 * y1) - y0 * x1) + z0 * w1,
         ((w0 * w1 - x0 * x1) - y0 * y1) - z0 * z1], dtype=q.dtype)
+
+
+def quat_mul_sse2(q, r):
+    """glam's SSE2 Quat::mul_quat (the f32 Quat of an x86-64 build): w0 * r and the sign-flipped x0 * r' are summed as one pair, the
+    y0 and z0 terms as another, and the two pair sums added last"""
+    x0, y0, z0, w0 = q
+    x1, y1, z1, w1 = r
+    return np.array([
+        (w0 * x1 + x0 * w1) + (y0 * z1 - z0 * y1),
+        (w0 * y1 - x0 * z1) + (y0 * w1 + z0 * x1),
+        (w0 * z1 + x0 * y1) + (-(y0 * x1) + z0 * w1),
+        (w0 * w1 - x0 * x1) + (-(y0 * y1) - z0 * z1)], dtype=q.dtype)
 
 
 def quat_rotate(q, v):   # glam Quat * Vec3: v (w^2 - b.b) + 2 b (v.b) + 2 w (b x v)
@@ -127,6 +143,23 @@ def rotate_inverse_inertia(il, q):
     return np.array([B[0][0], B[1][0], B[2][0], B[1][1], B[2][1], B[2][2]], dtype=q.dtype)
 
 
+def sym_inverse_or_zero(m):
+    """SymmetricMat3::inverse_or_zero (src/math/mod.rs:515-524): zero when the determinant is zero, else the inverse by cofactors
+    (the adjugate over the determinant, expanded along the first row).  Any symmetric tensor, not only a diagonal one."""
+    m00, m01, m02, m11, m12, m22 = m
+    c00 = m11 * m22 - m12 * m12
+    c01 = m02 * m12 - m01 * m22
+    c02 = m01 * m12 - m02 * m11
+    det = (m00 * c00 + m01 * c01) + m02 * c02
+    if det == 0:
+        return np.zeros(6, dtype=m.dtype)
+    inv = m.dtype.type(1) / det
+    c11 = m00 * m22 - m02 * m02
+    c12 = m01 * m02 - m00 * m12
+    c22 = m00 * m11 - m01 * m01
+    return np.array([c00 * inv, c01 * inv, c02 * inv, c11 * inv, c12 * inv, c22 * inv], dtype=m.dtype)
+
+
 def mat3_mul_vec(M, v):   # glam Mat3 * Vec3: x_axis * v.x + y_axis * v.y + z_axis * v.z
     return (M[0] * v[0] + M[1] * v[1]) + M[2] * v[2]
 
@@ -174,13 +207,20 @@ def softness(N, damping_ratio, hz, h):
     return {"bias": angular_frequency / a1, "impulse_scale": a3, "mass_scale": a2 * a3}
 
 
-def step(scene, dtype=np.float32):
-    """One PhysicsSchedule solver stage over a tiny scene (dict, see derive.py); returns the outputs as a dict of lists."""
+def step(scene, dtype=np.float32, quat_product="scalar"):
+    """One PhysicsSchedule solver stage over a small scene (dict, see derive.py); returns the outputs as a dict of lists.
+
+    quat_product: "scalar" (glam's scalar formulas, what vectors.json holds) or "sse2" (glam's SSE2 association of the f32 quaternion
+    product, which an x86-64 build of the reference runs).  The two differ by an ulp per product; in f32 contact scenes of several
+    substeps the soft contact (separation / h in the bias) amplifies that ulp to ~1e-5, so comparisons with code that follows the SSE2
+    association use "sse2".  f64 quaternions have no SIMD path in glam: the option changes nothing there."""
     N = Num(dtype)
     T = N.T
+    qmul = quat_mul_sse2 if (quat_product == "sse2" and np.dtype(dtype) == np.float32) else quat_mul
     prm = scene["params"]
     dt, h = T(prm["dt"]), T(prm["h"])
     substeps = int(prm["substeps"])
+    solver_iterations = max(int(prm.get("solver_iterations", 1)), 1)
     g = N.v(*[T(x) for x in prm["gravity"]])
     nb = len(scene["bodies"])
 
@@ -213,14 +253,21 @@ def step(scene, dtype=np.float32):
         eps = T(1e-6)
         iso = (not (abs(il[0] - il[3]) > eps or abs(il[3] - il[5]) > eps)) and abs(il[1]) < eps and abs(il[2]) < eps and abs(il[4]) < eps
         sb["gyro"] = (locked & 0b111) != 0b111 and not iso   # plugin.rs:241-247: rotation unlocked on at least one axis and not isotropic
-        # pre_process_velocity_increments (integrator/mod.rs:260-313), dynamic bodies only
+        # integration markers CustomVelocityIntegration (bit 0) / CustomPositionIntegration (bit 1) (integrator/mod.rs:169-195)
+        flags = int(b.get("integration_flags", 0))
+        sb["custom_vel"], sb["custom_pos"] = bool(flags & 1), bool(flags & 2)
+        # MaxLinearSpeed / MaxAngularSpeed: absent = no clamp (clamp_velocities queries only the bodies that have them)
+        sb["max_lin"] = None if b.get("max_linear_speed") is None else T(b["max_linear_speed"])
+        sb["max_ang"] = None if b.get("max_angular_speed") is None else T(b["max_angular_speed"])
+        # pre_process_velocity_increments (integrator/mod.rs:260-313), dynamic bodies only.  The increments arrive holding the
+        # accelerations ForcePlugin wrote (VelocityIntegrationData::apply_linear/angular_acceleration, integrator/mod.rs:236-244)
         sb["lin_rhs"], sb["ang_rhs"] = T(1), T(1)
         sb["lin_inc"], sb["ang_inc"] = N.v(0, 0, 0), N.v(0, 0, 0)
         if kind == DYNAMIC:
             sb["lin_rhs"] = T(1) / (T(1) + h * T(b.get("linear_damping", 0.0)))
             sb["ang_rhs"] = T(1) / (T(1) + h * T(b.get("angular_damping", 0.0)))
-            li = N.v(0, 0, 0) + g * T(b.get("gravity_scale", 1.0))
-            ai = N.v(0, 0, 0)
+            li = np.array(b.get("linear_acceleration", [0, 0, 0]), dtype=T) + g * T(b.get("gravity_scale", 1.0))
+            ai = np.array(b.get("angular_acceleration", [0, 0, 0]), dtype=T)
             # LockedAxes::apply_to_vec / apply_to_angular_velocity on the increments (integrator/mod.rs:296-300)
             for ax, (tb, rb) in enumerate(((0b100_000, 0b000_100), (0b010_000, 0b000_010), (0b001_000, 0b000_001))):
                 if locked & tb: li[ax] = T(0)
@@ -408,20 +455,20 @@ def step(scene, dtype=np.float32):
         if j["type"] == PRISMATIC:                            # xpbd/joints/prismatic.rs:43-77
             basis1 = np.array(j.get("local_basis1", [0, 0, 0, 1]), dtype=T)
             basis2 = np.array(j.get("local_basis2", [0, 0, 0, 1]), dtype=T)
-            d["rd"] = quat_mul(quat_mul(b1["rot"], basis1), quat_conj(quat_mul(b2["rot"], basis2)))   # FixedAngleConstraintShared::prepare
-            d["ax1"] = quat_rotate(quat_mul(b1["rot"], basis1), np.array(j.get("axis", [1, 0, 0]), dtype=T))   # free_axis1
+            d["rd"] = qmul(qmul(b1["rot"], basis1), quat_conj(qmul(b2["rot"], basis2)))   # FixedAngleConstraintShared::prepare
+            d["ax1"] = quat_rotate(qmul(b1["rot"], basis1), np.array(j.get("axis", [1, 0, 0]), dtype=T))   # free_axis1
         if j["type"] in (FIXED, REVOLUTE):
             basis1 = np.array(j.get("local_basis1", [0, 0, 0, 1]), dtype=T)
             basis2 = np.array(j.get("local_basis2", [0, 0, 0, 1]), dtype=T)
             if j["type"] == REVOLUTE:
                 axis = np.array(j.get("axis", [0, 0, 1]), dtype=T)
-                d["a1"] = quat_rotate(quat_mul(b1["rot"], basis1), axis)
-                d["a2"] = quat_rotate(quat_mul(b2["rot"], basis2), axis)
+                d["a1"] = quat_rotate(qmul(b1["rot"], basis1), axis)
+                d["a2"] = quat_rotate(qmul(b2["rot"], basis2), axis)
                 ortho = any_orthonormal_vector(N, axis)            # revolute.rs:86-89
-                d["b1"] = quat_rotate(quat_mul(b1["rot"], basis1), ortho)
-                d["b2"] = quat_rotate(quat_mul(b2["rot"], basis2), ortho)
+                d["b1"] = quat_rotate(qmul(b1["rot"], basis1), ortho)
+                d["b2"] = quat_rotate(qmul(b2["rot"], basis2), ortho)
             else:
-                d["rd"] = quat_mul(quat_mul(b1["rot"], basis1), quat_conj(quat_mul(b2["rot"], basis2)))
+                d["rd"] = qmul(qmul(b1["rot"], basis1), quat_conj(qmul(b2["rot"], basis2)))
         if j["type"] == SPHERICAL:                            # xpbd/joints/spherical.rs:45-82: through rotation MATRICES here
             basis1 = np.array(j.get("local_basis1", [0, 0, 0, 1]), dtype=T)
             basis2 = np.array(j.get("local_basis2", [0, 0, 0, 1]), dtype=T)
@@ -455,9 +502,9 @@ def step(scene, dtype=np.float32):
     def positional_impulse(b1, b2, in1, in2, imp, r1, r2):    # xpbd/positional_constraint.rs:9-50
         (im1, ii1), (im2, ii2) = in1, in2
         b1["dp"] = b1["dp"] + imp * im1
-        b1["dq"] = quat_mul(quat_from_scaled_axis(N, sym_mul(ii1, cross(r1, imp))), b1["dq"])
+        b1["dq"] = qmul(quat_from_scaled_axis(N, sym_mul(ii1, cross(r1, imp))), b1["dq"])
         b2["dp"] = b2["dp"] - imp * im2
-        b2["dq"] = quat_mul(quat_from_scaled_axis(N, sym_mul(ii2, cross(r2, -imp))), b2["dq"])
+        b2["dq"] = qmul(quat_from_scaled_axis(N, sym_mul(ii2, cross(r2, -imp))), b2["dq"])
 
     def generalized_inverse_mass(im, ii, r, n):               # positional_constraint.rs:66-79 with inv_mass.max_element()
         rxn = cross(r, n)
@@ -487,8 +534,8 @@ def step(scene, dtype=np.float32):
         dl = lagrange_update(angle, [w1, w2], compliance)
         if abs(dl) > N.eps:
             imp = -dl * axis
-            b1["dq"] = quat_mul(quat_from_scaled_axis(N, sym_mul(in1[1], imp)), b1["dq"])
-            b2["dq"] = quat_mul(quat_from_scaled_axis(N, sym_mul(in2[1], -imp)), b2["dq"])
+            b1["dq"] = qmul(quat_from_scaled_axis(N, sym_mul(in1[1], imp)), b1["dq"])
+            b2["dq"] = qmul(quat_from_scaled_axis(N, sym_mul(in2[1], -imp)), b2["dq"])
         return dl * axis
 
     def solve_joint(j):
@@ -554,7 +601,7 @@ def step(scene, dtype=np.float32):
                     j["lam_b"] = j["lam_b"] + align_orientation(j, b1, b2, in1, in2, corr, T(j.get("compliance2", 0.0)))
             point_constraint(j, b1, b2, in1, in2, c0)
         elif j["type"] == PRISMATIC:                          # xpbd/joints/prismatic.rs:79-193: fixed angle, then translation off the free axis
-            q = quat_mul(quat_mul(j["rd"], b1["dq"]), quat_conj(b2["dq"]))
+            q = qmul(qmul(j["rd"], b1["dq"]), quat_conj(b2["dq"]))
             j["lam_a"] = j["lam_a"] + align_orientation(j, b1, b2, in1, in2, T(-2) * q[:3], c1)      # angle_compliance
             wr1, wr2 = quat_rotate(b1["dq"], j["r1"]), quat_rotate(b2["dq"], j["r2"])
             axis1 = quat_rotate(b1["dq"], j["ax1"])
@@ -584,7 +631,7 @@ def step(scene, dtype=np.float32):
             j["lam_p"] = j["lam_p"] + imp
             positional_impulse(b1, b2, in1, in2, imp, wr1, wr2)
         elif j["type"] == FIXED:                              # xpbd/joints/fixed.rs:73-89, shared/fixed_angle_constraint.rs:59-96
-            q = quat_mul(quat_mul(j["rd"], b1["dq"]), quat_conj(b2["dq"]))
+            q = qmul(qmul(j["rd"], b1["dq"]), quat_conj(b2["dq"]))
             difference = T(-2) * q[:3]
             j["lam_a"] = j["lam_a"] + align_orientation(j, b1, b2, in1, in2, difference, c1)
             point_constraint(j, b1, b2, in1, in2, c0)
@@ -592,19 +639,18 @@ def step(scene, dtype=np.float32):
     # ---- run_substep_schedule (solver/schedule.rs:59-69,194-213)
     for _ in range(substeps):
         for b in B:                                           # integrate_velocities (integrator/mod.rs:343-391)
-            if not b["has_solver_body"] or b["kind"] == KINEMATIC:
+            if not b["has_solver_body"] or b["kind"] == KINEMATIC or b["custom_vel"]:
                 continue
             b["v"] = b["v"] * b["lin_rhs"]
             b["w"] = b["w"] * b["ang_rhs"]
             b["v"] = b["v"] + b["lin_inc"]
             b["w"] = b["w"] + b["ang_inc"]
             if b["gyro"]:                                     # solve_gyroscopic_torque (integrator/mod.rs:403-460)
-                rot = quat_mul(b["dq"], b["rot"])
+                rot = qmul(b["dq"], b["rot"])
                 lw = quat_rotate(quat_conj(rot), b["w"])
                 il = b["il"]
-                # ComputedAngularInertia::tensor() = inverse of the stored inverse tensor; these scenes use diagonal local tensors
-                assert il[1] == 0 and il[2] == 0 and il[4] == 0, "hand-worked gyroscopic case wants a diagonal local tensor"
-                tensor = np.array([T(1) / il[0], 0, 0, T(1) / il[3], 0, T(1) / il[5]], dtype=T)
+                # ComputedAngularInertia::tensor() = inverse_or_zero of the stored inverse tensor (computed.rs:617-619)
+                tensor = sym_inverse_or_zero(il)
                 L = sym_mul(tensor, lw)
                 Ln = L - h * cross(lw, L)
                 l2 = dot(Ln, Ln)
@@ -613,15 +659,25 @@ def step(scene, dtype=np.float32):
                 else:
                     Ln = Ln * N.sqrt(dot(L, L) / l2)
                     b["w"] = quat_rotate(rot, sym_mul(il, Ln))
-        for k in order:
-            warm_start(C[k])
-        for k in order:
-            solve(C[k], True)
-        for b in B:                                           # integrate_positions (integrator/mod.rs:503-535)
+        for b in B:                                           # clamp_velocities (integrator/mod.rs:467-500), chained after it
             if not b["has_solver_body"]:
                 continue
+            for key, ms in (("v", b["max_lin"]), ("w", b["max_ang"])):
+                if ms is None:
+                    continue
+                l2 = dot(b[key], b[key])
+                if l2 > ms * ms:
+                    b[key] = b[key] * (ms / N.sqrt(l2))
+        for k in order:
+            warm_start(C[k])
+        for _ in range(solver_iterations):                    # solve_contacts::<true>, done `iterations` times (solver/plugin.rs:517-531)
+            for k in order:
+                solve(C[k], True)
+        for b in B:                                           # integrate_positions (integrator/mod.rs:503-535)
+            if not b["has_solver_body"] or b["custom_pos"]:
+                continue
             b["dp"] = b["dp"] + b["v"] * h
-            b["dq"] = quat_mul(quat_from_scaled_axis(N, b["w"] * h), b["dq"])
+            b["dq"] = qmul(quat_from_scaled_axis(N, b["w"] * h), b["dq"])
         for k in order:
             solve(C[k], False)
         if J:
@@ -634,7 +690,7 @@ def step(scene, dtype=np.float32):
                 if not b["has_solver_body"]:
                     continue
                 b["v"] = b["v"] + (b["dp"] - pdp) / h
-                dr = quat_mul(b["dq"], quat_conj(pdq))
+                dr = qmul(b["dq"], quat_conj(pdq))
                 nw = T(2) * dr[:3] / h
                 if dr[3] < 0:
                     nw = -nw
@@ -667,7 +723,7 @@ def step(scene, dtype=np.float32):
         pos, rot, lv, av = b["pos"], b["rot"], np.array(b["lin0"], dtype=T), None
         if b["has_solver_body"]:
             old_com = quat_rotate(rot, b["com"])
-            q = quat_mul(b["dq"], rot)
+            q = qmul(b["dq"], rot)
             q = q * (T(0.5) * (T(3) - ((q[0] * q[0] + q[1] * q[1]) + (q[2] * q[2] + q[3] * q[3]))))   # fast_renormalize (transform.rs:811-817)
             new_com = quat_rotate(q, b["com"])
             pos = pos + ((b["dp"] + old_com) - new_com)
