@@ -5,7 +5,8 @@
 // ~2 hits).  The set of pairs and their order are properties of the x-sorted RANKS only, so the search may use any index that finds
 // exactly the pairs {i < j < end_i, y/z overlap}:
 //   * every interval is binned by the (y, z) cell of its min corner; the cell edge per axis is the largest "small" extent on that axis
-//     (extents above 4x the mean are "large"), so a small j that overlaps i lies in the cell range [cell(min_i - edge), cell(max_i)];
+//     (extents above 4x the mean are "large"), so a small j that overlaps i lies in the cell range [cell(min_i - edge), cell(max_i)]
+//     (with the extents rounded up and min_i - edge rounded down: see query_lo);
 //   * one stable radix sort of the ranks by cell id groups the ranks per cell IN RANK ORDER, so the x-window of i is a contiguous
 //     sub-range of each cell list (two binary searches);
 //   * large intervals share one extra list (cell id 0xFFFF) that every i scans inside its x-window;
@@ -27,6 +28,18 @@ struct CellGrid {
     S y0, z0, inv_cy, inv_cz, edge_y, edge_z;   // origin, 1/cell edge, small-extent bound per axis
     int ny, nz;
 };
+
+template <class S> __device__ __forceinline__ int cell_coord(S v, S v0, S inv_c, int n) {
+    S t = (v - v0) * inv_c;
+    int c = t > S(0) ? (t < S(n) ? int(t) : n - 1) : 0;   // clamps; NaN cannot occur (non-finite AABBs never reach the intervals)
+    return c;
+}
+
+// directed rounding: query_lo(min_i, edge) <= min_i - edge <= max_j - extent_up(j) <= min_j for every small j overlapping i (cell_coord is monotone)
+__device__ __forceinline__ float sub_dir(float a, float b, bool up) { return up ? __fsub_ru(a, b) : __fsub_rd(a, b); }
+__device__ __forceinline__ double sub_dir(double a, double b, bool up) { return up ? __dsub_ru(a, b) : __dsub_rd(a, b); }
+template <class S> __device__ __forceinline__ S extent_up(S lo, S hi) { return sub_dir(hi, lo, true); }     // decides small / large and the edge
+template <class S> __device__ __forceinline__ S query_lo(S v, S edge) { return sub_dir(v, edge, false); }
 
 // per-block partial reductions of yz_stats
 template <class S>
@@ -99,7 +112,7 @@ __global__ void __launch_bounds__(256) yz_small_max(const Vec4<S>* __restrict__ 
     S my = 0, mz = 0;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         Vec4<S> v = yz[i];
-        S ey = v.y - v.x, ez = v.w - v.z;
+        S ey = extent_up(v.x, v.y), ez = extent_up(v.z, v.w);
         if (ey <= thr_y) my = avn_max(my, ey);
         if (ez <= thr_z) mz = avn_max(mz, ez);
     }
@@ -135,16 +148,10 @@ __global__ void yz_grid(const YzPartial<S>* __restrict__ partial, const S* __res
     *grid = g;
 }
 
-template <class S> __device__ __forceinline__ int cell_coord(S v, S v0, S inv_c, int n) {
-    S t = (v - v0) * inv_c;
-    int c = t > S(0) ? (t < S(n) ? int(t) : n - 1) : 0;   // clamps; NaN cannot occur (non-finite AABBs never reach the intervals)
-    return c;
-}
-
 // number of cells in the query range of an interval with y/z bounds yi (the cells a small overlapping j can live in)
 template <class S> __device__ __forceinline__ long long query_cell_count(const CellGrid<S>& g, Vec4<S> yi) {
-    const int cy_lo = cell_coord(yi.x - g.edge_y, g.y0, g.inv_cy, g.ny), cy_hi = cell_coord(yi.y, g.y0, g.inv_cy, g.ny);
-    const int cz_lo = cell_coord(yi.z - g.edge_z, g.z0, g.inv_cz, g.nz), cz_hi = cell_coord(yi.w, g.z0, g.inv_cz, g.nz);
+    const int cy_lo = cell_coord(query_lo(yi.x, g.edge_y), g.y0, g.inv_cy, g.ny), cy_hi = cell_coord(yi.y, g.y0, g.inv_cy, g.ny);
+    const int cz_lo = cell_coord(query_lo(yi.z, g.edge_z), g.z0, g.inv_cz, g.nz), cz_hi = cell_coord(yi.w, g.z0, g.inv_cz, g.nz);
     return (long long)(cy_hi - cy_lo + 1) * (cz_hi - cz_lo + 1);
 }
 
@@ -155,7 +162,7 @@ __global__ void cell_keys(const Vec4<S>* __restrict__ yz, int n, const CellGrid<
     if (r >= n) return;
     const CellGrid<S> g = *grid;
     Vec4<S> v = yz[r];
-    const bool large = (v.y - v.x) > g.edge_y || (v.w - v.z) > g.edge_z;
+    const bool large = extent_up(v.x, v.y) > g.edge_y || extent_up(v.z, v.w) > g.edge_z;   // the same extents as yz_small_max
     keys[r] = large ? CG_LARGE : uint32_t(cell_coord(v.x, g.y0, g.inv_cy, g.ny) * g.nz + cell_coord(v.z, g.z0, g.inv_cz, g.nz));
     vals[r] = uint32_t(r);
 }
@@ -222,8 +229,8 @@ __global__ void __launch_bounds__(256) sweep_cells_kernel(const __grid_constant_
                 wr = x - mine;
             }
             if (e > i + 1) {
-                const int cy_lo = cell_coord(yi.x - g.edge_y, g.y0, g.inv_cy, g.ny), cy_hi = cell_coord(yi.y, g.y0, g.inv_cy, g.ny);
-                const int cz_lo = cell_coord(yi.z - g.edge_z, g.z0, g.inv_cz, g.nz), cz_hi = cell_coord(yi.w, g.z0, g.inv_cz, g.nz);
+                const int cy_lo = cell_coord(query_lo(yi.x, g.edge_y), g.y0, g.inv_cy, g.ny), cy_hi = cell_coord(yi.y, g.y0, g.inv_cy, g.ny);
+                const int cz_lo = cell_coord(query_lo(yi.z, g.edge_z), g.z0, g.inv_cz, g.nz), cz_hi = cell_coord(yi.w, g.z0, g.inv_cz, g.nz);
                 const int wz = cz_hi - cz_lo + 1, ncell = (cy_hi - cy_lo + 1) * wz;
                 if (ncell > e - i - 1) {
                     // more cells than x-candidates (a big footprint with a short window): test the window directly, lane-strided

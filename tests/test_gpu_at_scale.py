@@ -15,6 +15,7 @@ import pytest
 
 from avian_b200 import api, fixture, plugins, scenes
 
+import cell_grid_model as cgm
 import sap_reference as ref
 from test_gpu_ccd import pile_with_projectiles, step_and_check
 from test_gpu_graph import _check_graphs
@@ -26,7 +27,6 @@ RS_TILE = 2048
 FUSED_MAX_KEYS = 128 * RS_TILE            # the last size the fused scatter sorts
 SCAN_CHUNK_COUNTERS = 1024 * 16           # rs_scan: counters per iteration
 SCAN_OFFSET_CHUNK = 1024 * 1024           # scan_block_offsets: counts per iteration
-SW_WIDE, SW_WIDE_CAP = 4096, 1 << 14      # csrc/broadphase.cu
 
 
 # ---- broad phase ---------------------------------------------------------------------------------------------------------------------
@@ -155,39 +155,8 @@ def test_persistent_order_across_steps(gpu_ctx):
         a.order_out = np.zeros(n, dtype=np.uint32)
 
 
-def cell_grid_dims(mn, mx):
-    """(ny, nz) of the broad phase's (y, z) cell grid before and after coarsening, and the small-extent edges (csrc/broadphase_cells.cuh
-    yz_grid, evaluated in float64)"""
-    out = []
-    for ax in (1, 2):
-        ext = mx[:, ax].astype(np.float64) - mn[:, ax].astype(np.float64)
-        thr = 4.0 * ext.mean()
-        edge = ext[ext <= thr].max()
-        rng_ = float(mn[:, ax].max()) - float(mn[:, ax].min())
-        c = max(edge, rng_ / 1024)
-        out.append((max(1, min(int(rng_ / c) + 1, 1024)), c, edge, float(mn[:, ax].min())))
-    (ny, cy, ey, y0), (nz, cz, ez, z0) = out
-    before = (ny, nz)
-    while ny * nz > 0xFFFF:
-        if ny >= nz:
-            ny, cy = (ny + 1) // 2, cy * 2
-        else:
-            nz, cz = (nz + 1) // 2, cz * 2
-    return before, (ny, nz, cy, cz, ey, ez, y0, z0)
-
-
-def query_cells(grid, mn, mx):
-    ny, nz, cy, cz, ey, ez, y0, z0 = grid
-    cell = lambda v, v0, c, k: np.clip(np.floor((v - v0) / c), 0, k - 1)
-    wy = cell(mx[:, 1].astype(np.float64), y0, cy, ny) - cell(mn[:, 1] - ey, y0, cy, ny) + 1
-    wz = cell(mx[:, 2].astype(np.float64), z0, cz, nz) - cell(mn[:, 2] - ez, z0, cz, nz) + 1
-    return wy * wz
-
-
-def test_over_cap_wide_intervals(gpu_ctx):
-    """17 000 intervals that each reach over 5 000 x-candidates with a (y, z) footprint of far more than 32 cells: 16 384 go to the brute-force
-    kernel, the rest stay in the tiled sweep, whose segment sort then orders segments of tens to hundreds of pairs.  The wide intervals are
-    thin z layers, disjoint from every other wide interval in their x-window, so each has only tens to hundreds of pairs."""
+def over_cap_columns():
+    """200 000 small intervals and 17 000 wide thin z layers (see test_over_cap_wide_intervals), in random input order"""
     rng = np.random.default_rng(8)
     ns, nw, L = 200_000, 17_000, 2000.0
     sc = np.column_stack([rng.uniform(0, L, ns), rng.uniform(0, 40, ns), rng.uniform(0, 50, ns)])
@@ -200,15 +169,22 @@ def test_over_cap_wide_intervals(gpu_ctx):
     mn = np.concatenate([sc - sh, wmn]).astype(np.float32)
     mx = np.concatenate([sc + sh, wmx]).astype(np.float32)
     perm = rng.permutation(ns + nw)
-    mn, mx = mn[perm], mx[perm]
-    n = ns + nw
+    return mn[perm], mx[perm]
+
+
+def test_over_cap_wide_intervals(gpu_ctx):
+    """17 000 intervals that each reach over 5 000 x-candidates with a (y, z) footprint of far more than 32 cells: 16 384 go to the brute-force
+    kernel, the rest stay in the tiled sweep, whose segment sort then orders segments of tens to hundreds of pairs.  The wide intervals are
+    thin z layers, disjoint from every other wide interval in their x-window, so each has only tens to hundreds of pairs."""
+    mn, mx = over_cap_columns()
+    n = mn.shape[0]
     a = api.Aabbs(collider=np.arange(n, dtype=np.uint32), body=np.arange(n, dtype=np.uint32), aabb_min=mn, aabb_max=mx,
                   flags=np.full(n, api.AABB_GENERATE_CONSTRAINTS, np.uint8), order_out=np.zeros(n, np.uint32))
     r = reference(a)
-    _, grid = cell_grid_dims(mn[r.order], mx[r.order])
-    smn, smx = mn[r.order], mx[r.order]
-    wide = (r.x_candidates() > SW_WIDE) & (query_cells(grid, smn, smx) > 32)
-    assert wide.sum() > SW_WIDE_CAP, wide.sum()
+    m = cgm.CellGridModel(mn, mx, "directed")
+    assert np.array_equal(m.order, r.order) and np.array_equal(m.candidates, r.x_candidates())
+    wide = m.wide
+    assert wide.sum() > cgm.SW_WIDE_CAP, wide.sum()
     rank = np.empty(n, np.int64)
     rank[r.order] = np.arange(n)
     i_rank = rank[r.collider1]
@@ -219,8 +195,8 @@ def test_over_cap_wide_intervals(gpu_ctx):
     assert_matches(g, r, a)
 
 
-def test_cell_grid_coarsening(gpu_ctx):
-    """small intervals in clusters spread over 1 000 x 1 000 in (y, z): a grid of more than 0xFFFF cells before coarsening"""
+def coarsening_columns():
+    """300 000 small intervals in 2 000 clusters spread over 1 000 x 1 000 in (y, z)"""
     rng = np.random.default_rng(12)
     n, k = 300_000, 2000
     assert (n + RS_TILE - 1) // RS_TILE > 128
@@ -228,10 +204,16 @@ def test_cell_grid_coarsening(gpu_ctx):
     c = centre[rng.integers(0, k, n)] + rng.uniform(-1.5, 1.5, (n, 3))
     h = rng.uniform(0.1, 0.3, (n, 3))
     h[:, 0] = 0.25
-    mn, mx = (c - h).astype(np.float32), (c + h).astype(np.float32)
+    return (c - h).astype(np.float32), (c + h).astype(np.float32)
+
+
+def test_cell_grid_coarsening(gpu_ctx):
+    """small intervals in clusters spread over 1 000 x 1 000 in (y, z): a grid of more than 0xFFFF cells before coarsening"""
+    mn, mx = coarsening_columns()
+    n = mn.shape[0]
     a = api.Aabbs(collider=np.arange(n, dtype=np.uint32), body=np.arange(n, dtype=np.uint32), aabb_min=mn, aabb_max=mx,
                   flags=np.full(n, api.AABB_GENERATE_CONSTRAINTS, np.uint8), order_out=np.zeros(n, np.uint32))
-    (ny, nz), _ = cell_grid_dims(mn, mx)
+    ny, nz = cgm.CellGridModel(mn, mx, "directed").before
     assert ny * nz > 0xFFFF, (ny, nz)
     r = reference(a)
     assert r.count > n // 10
