@@ -311,12 +311,6 @@ class PairList:
         return PairList(self.collider1[:n], self.collider2[:n], self.body1[:n], self.body2[:n], self.flags[:n], n)
 
 
-class AvnEdgeManifolds(C.Structure):
-    _fields_ = [("count", C.c_uint32), ("edge_capacity", C.c_uint32), ("color_offsets", C.c_uint32 * (GRAPH_COLOR_COUNT + 1))] + [
-        (n, _vp) for n in ("edge", "body1", "body2", "friction", "restitution", "point_count", "normal", "anchor1", "anchor2", "penetration",
-                           "normal_speed", "warm_start_normal_impulse", "warm_start_tangent_impulse", "normal_impulse")]
-
-
 class AvnNarrowParams(C.Structure):
     _fields_ = [("dt", C.c_double), ("contact_tolerance", C.c_double)]
 
@@ -481,13 +475,7 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "comm_destroy": ([_vp], C.c_int),
         "comm_all_gather": ([_vp, _vp, _vp, C.c_size_t], C.c_int),
         "narrow_phase": ([_vp, P(AvnNarrowParams), P(AvnNarrowInput), P(AvnRawManifolds)], C.c_int),
-        "solver_upload_edges": ([_vp, P(AvnStepParams), P(AvnBodyColumns), P(AvnEdgeManifolds), P(AvnJointSet)], C.c_int),
-        "solver_upload_graph": ([_vp, P(AvnStepParams), P(AvnBodyColumns), P(AvnEdgeManifolds), P(AvnJointSet)], C.c_int),
-        "contacts_reserve": ([_vp, C.c_uint32], C.c_int),
-        "contacts_add": ([_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp], C.c_int),
-        "contacts_remove": ([_vp, C.c_uint32, _vp], C.c_int),
-        "contacts_narrow_phase": ([_vp, P(AvnNarrowParams), P(AvnNarrowInput), C.c_uint32, C.c_double, _vp, _vp], C.c_int),
-        "contacts_download_impulses": ([_vp, _vp, _vp, _vp], C.c_int),
+        "contacts_download_impulses": ([_vp, C.c_uint32, _vp, _vp, _vp], C.c_int),
         "contacts_configure": ([_vp, P(AvnContactGraphConfig)], C.c_int),
         "contacts_step": ([_vp, P(AvnNarrowParams), P(AvnNarrowInput), C.c_uint32, C.c_double, C.c_uint32, P(AvnContactStep)], C.c_int),
         "solver_upload_resident": ([_vp, P(AvnStepParams), P(AvnBodyColumns), P(AvnJointSet)], C.c_int),
@@ -526,8 +514,7 @@ ABI_SYMBOLS = [
     "avn_solver_upload", "avn_solver_run", "avn_solver_download", "avn_broadphase", "avn_broadphase_upload", "avn_broadphase_run",
     "avn_broadphase_download", "avn_get_timings", "avn_joint_levels", "avn_update_aabbs", "avn_solver_run_range", "avn_solver_set_boundary",
     "avn_solver_boundary_snapshot", "avn_solver_boundary_pack", "avn_solver_boundary_apply", "avn_solver_needs_restitution", "avn_get_stream",
-    "avn_solver_step_partitioned", "avn_comm_unique_id", "avn_comm_init", "avn_comm_destroy", "avn_comm_all_gather", "avn_narrow_phase", "avn_solver_upload_edges", "avn_solver_upload_graph",
-    "avn_contacts_reserve", "avn_contacts_add", "avn_contacts_remove", "avn_contacts_narrow_phase", "avn_contacts_download_impulses",
+    "avn_solver_step_partitioned", "avn_comm_unique_id", "avn_comm_init", "avn_comm_destroy", "avn_comm_all_gather", "avn_narrow_phase", "avn_contacts_download_impulses",
     "avn_contacts_configure", "avn_contacts_step", "avn_solver_upload_resident", "avn_broadphase_download_order", "avn_contacts_download_graph",
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
@@ -950,81 +937,6 @@ class Context:
         self._check(self.lib.avn_get_stream(self.handle, C.byref(out)))
         return int(out.value or 0)
 
-    def solver_step_edges(self, params, bodies: Bodies, graph: dict, edges: dict, joints: JointSet | None = None) -> None:
-        """avn_solver_upload_edges + run + download.  graph = dict(color_offsets, edge, body1, body2, friction, restitution) (per manifold);
-        edges = dict(point_count, normal, anchor1, anchor2, penetration, normal_speed, warm_start_normal_impulse,
-        warm_start_tangent_impulse, normal_impulse) (edge-indexed, 4 slots per edge; the three impulse columns are updated in place)."""
-        b = bodies.as_struct()
-        j = joints.as_struct() if joints is not None and joints.count else None
-        em = AvnEdgeManifolds()
-        em.count = int(graph["edge"].shape[0])
-        em.edge_capacity = int(edges["point_count"].shape[0])
-        for i in range(GRAPH_COLOR_COUNT + 1):
-            em.color_offsets[i] = int(graph["color_offsets"][i])
-        keep = []
-        def col(a, dtype):
-            a = np.ascontiguousarray(a, dtype=dtype)
-            keep.append(a)
-            return a.ctypes.data
-        em.edge = col(graph["edge"], np.uint32); em.body1 = col(graph["body1"], np.int32); em.body2 = col(graph["body2"], np.int32)
-        em.friction = col(graph["friction"], self.scalar); em.restitution = col(graph["restitution"], self.scalar)
-        em.point_count = col(edges["point_count"], np.uint8)
-        for k in ("normal", "anchor1", "anchor2", "penetration", "normal_speed"):
-            setattr(em, k, col(edges[k], self.scalar))
-        for k in ("warm_start_normal_impulse", "warm_start_tangent_impulse", "normal_impulse"):
-            assert edges[k].flags["C_CONTIGUOUS"] and edges[k].dtype == self.scalar
-            setattr(em, k, edges[k].ctypes.data)
-        self._keep = (params, bodies, graph, edges, joints, b, em, j, keep)
-        self._check(self.lib.avn_solver_upload_edges(self.handle, C.byref(params), C.byref(b), C.byref(em) if em.count else None, C.byref(j) if j is not None else None))
-        self._check(self.lib.avn_solver_run(self.handle))
-        self._check(self.lib.avn_solver_download(self.handle))
-
-    # ---- device-resident contact edges (include/avian_b200.h)
-    def contacts_reserve(self, capacity: int) -> None:
-        self._check(self.lib.avn_contacts_reserve(self.handle, int(capacity)))
-
-    def contacts_add(self, ids, c1, c2, b1, b2) -> None:
-        a = [np.ascontiguousarray(x, dtype=np.uint32) for x in (ids, c1, c2, b1, b2)]
-        self._check(self.lib.avn_contacts_add(self.handle, int(a[0].shape[0]), *(x.ctypes.data for x in a)))
-
-    def contacts_remove(self, ids) -> None:
-        ids = np.ascontiguousarray(ids, dtype=np.uint32)
-        self._check(self.lib.avn_contacts_remove(self.handle, int(ids.shape[0]), ids.ctypes.data))
-
-    def contacts_narrow_phase(self, dt: float, contact_tolerance: float, colliders: dict, lin_vel, ang_vel, capacity: int, match_contacts: bool = True,
-                              length_unit: float = 1.0):
-        """Geometry + match_contacts for every live row.  Returns (point_count[capacity], disjoint[capacity])."""
-        dt_ = self.scalar
-        cols = {k: (None if colliders.get(k) is None else np.ascontiguousarray(colliders[k], dtype=(np.uint8 if k == "shape" else dt_)))
-                for k in ("shape", "dims", "position", "rotation", "aabb_min", "aabb_max")}
-        lv, av = np.ascontiguousarray(lin_vel, dtype=dt_), np.ascontiguousarray(ang_vel, dtype=dt_)
-        inp = AvnNarrowInput(0, int(cols["position"].shape[0]), int(lv.shape[0]), 0, None, None, None, None, _ptr(cols["shape"]), _ptr(cols["dims"]),
-                             _ptr(cols["position"]), _ptr(cols["rotation"]), _ptr(lv), _ptr(av), _ptr(cols["aabb_min"]), _ptr(cols["aabb_max"]))
-        count, disjoint = np.zeros(capacity, dtype=np.uint8), np.zeros(capacity, dtype=np.uint8)
-        prm = AvnNarrowParams(float(dt), float(contact_tolerance))
-        self._check(self.lib.avn_contacts_narrow_phase(self.handle, C.byref(prm), C.byref(inp), 1 if match_contacts else 0, float(length_unit),
-                                                       count.ctypes.data, disjoint.ctypes.data))
-        return count, disjoint
-
-    def solver_step_graph(self, params, bodies: Bodies, graph: dict, joints: JointSet | None = None, reuse_graph: bool = False) -> None:
-        """avn_solver_upload_graph + run + download: the manifolds come from the resident rows, graph = dict(color_offsets, edge, body1, body2,
-        friction, restitution)."""
-        b = bodies.as_struct()
-        j = joints.as_struct() if joints is not None and joints.count else None
-        em = AvnEdgeManifolds()
-        em.count = int(graph["edge"].shape[0])
-        for i in range(GRAPH_COLOR_COUNT + 1):
-            em.color_offsets[i] = int(graph["color_offsets"][i])
-        keep = [np.ascontiguousarray(graph["edge"], dtype=np.uint32), np.ascontiguousarray(graph["body1"], dtype=np.int32),
-                np.ascontiguousarray(graph["body2"], dtype=np.int32), np.ascontiguousarray(graph["friction"], dtype=self.scalar),
-                np.ascontiguousarray(graph["restitution"], dtype=self.scalar)]
-        if not reuse_graph:     # reuse: edge stays NULL = "the list of the previous call is still resident"
-            em.edge, em.body1, em.body2, em.friction, em.restitution = (x.ctypes.data for x in keep)
-        self._keep = (params, bodies, graph, joints, b, em, j, keep)
-        self._check(self.lib.avn_solver_upload_graph(self.handle, C.byref(params), C.byref(b), C.byref(em) if em.count else None, C.byref(j) if j is not None else None))
-        self._check(self.lib.avn_solver_run(self.handle))
-        self._check(self.lib.avn_solver_download(self.handle))
-
     # ---- the ContactGraph + ConstraintGraph on the device (include/avian_b200.h avn_contacts_configure / _step)
     def contacts_configure(self, body_kind, collider_count: int, friction=None, restitution=None) -> None:
         kind = np.ascontiguousarray(body_kind, dtype=np.uint8)
@@ -1196,8 +1108,10 @@ class Context:
         return {k: v[:int(r.count)] for k, v in out.items()}
 
     def contacts_download_impulses(self, capacity: int):
+        """avn_contacts_download_impulses: (warm_start_normal [capacity, 4], warm_start_tangent [capacity, 4, 2], normal_impulse [capacity, 4]) of the
+        rows as the last solve left them; rows beyond the store's stay zero."""
         wn, wt, ni = (np.zeros((capacity, 4), dtype=self.scalar), np.zeros((capacity, 4, 2), dtype=self.scalar), np.zeros((capacity, 4), dtype=self.scalar))
-        self._check(self.lib.avn_contacts_download_impulses(self.handle, wn.ctypes.data, wt.ctypes.data, ni.ctypes.data))
+        self._check(self.lib.avn_contacts_download_impulses(self.handle, int(capacity), wn.ctypes.data, wt.ctypes.data, ni.ctypes.data))
         return wn, wt, ni
 
     def narrow_phase(self, dt: float, contact_tolerance: float, pairs, colliders: dict, lin_vel: np.ndarray, ang_vel: np.ndarray) -> dict:

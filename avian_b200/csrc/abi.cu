@@ -148,9 +148,6 @@ AvnStatus avn_solver_upload(AvnContext* ctx, const AvnStepParams* params, AvnBod
 AvnStatus avn_solver_run(AvnContext* ctx) {
     return guarded(ctx, [&] { return ctx->solver->run(); });
 }
-AvnStatus avn_solver_upload_edges(AvnContext* ctx, const AvnStepParams* params, AvnBodyColumns* bodies, AvnEdgeManifolds* manifolds, AvnJointSet* joints) {
-    return guarded(ctx, [&] { return ctx->solver->upload_edges(params, bodies, manifolds, joints); });
-}
 AvnStatus avn_solver_run_range(AvnContext* ctx, uint32_t first_substep, uint32_t substep_count, uint32_t run_flags) {
     return guarded(ctx, [&] { return ctx->solver->run_range(first_substep, substep_count, run_flags); });
 }
@@ -233,19 +230,6 @@ AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const
     return guarded(ctx, [&] { return ctx->narrow->run(params, input, out); });
 }
 
-AvnStatus avn_contacts_reserve(AvnContext* ctx, uint32_t capacity) { return guarded(ctx, [&] { return ctx->contacts->reserve(capacity); }); }
-AvnStatus avn_contacts_add(AvnContext* ctx, uint32_t n, const uint32_t* ids, const uint32_t* collider1, const uint32_t* collider2, const uint32_t* body1,
-                           const uint32_t* body2) {
-    return guarded(ctx, [&] { return ctx->contacts->add(n, ids, collider1, collider2, body1, body2); });
-}
-AvnStatus avn_contacts_remove(AvnContext* ctx, uint32_t n, const uint32_t* ids) { return guarded(ctx, [&] { return ctx->contacts->remove(n, ids); }); }
-AvnStatus avn_contacts_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, uint32_t match_contacts, double length_unit,
-                                    uint8_t* out_point_count, uint8_t* out_disjoint) {
-    return guarded(ctx, [&] { return ctx->contacts->narrow_phase(params, input, match_contacts, length_unit, out_point_count, out_disjoint); });
-}
-AvnStatus avn_solver_upload_graph(AvnContext* ctx, const AvnStepParams* params, AvnBodyColumns* bodies, const AvnEdgeManifolds* graph, AvnJointSet* joints) {
-    return guarded(ctx, [&] { return ctx->solver->upload_graph(params, bodies, graph, ctx->contacts.get(), joints); });
-}
 AvnStatus avn_contacts_configure(AvnContext* ctx, const AvnContactGraphConfig* config) { return guarded(ctx, [&] { return ctx->contacts->configure(config); }); }
 AvnStatus avn_contacts_step(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, uint32_t match_contacts, double length_unit, uint32_t flags,
                             AvnContactStep* out) {
@@ -322,8 +306,8 @@ AvnStatus avn_islands_wake(AvnContext* ctx, const uint8_t* wake, AvnIslandsWake*
 AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep) {
     return guarded(ctx, [&] { return ctx->contacts->download_sleeping(capacity, row_asleep, body_count, body_asleep); });
 }
-AvnStatus avn_contacts_download_impulses(AvnContext* ctx, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse) {
-    return guarded(ctx, [&] { return ctx->contacts->download_impulses(warm_start_normal, warm_start_tangent, normal_impulse); });
+AvnStatus avn_contacts_download_impulses(AvnContext* ctx, uint32_t capacity, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse) {
+    return guarded(ctx, [&] { return ctx->contacts->download_impulses(capacity, warm_start_normal, warm_start_tangent, normal_impulse); });
 }
 
 // spatial queries (queries.cu): SpatialQueryPipeline::update / cast_ray / ray_hits / aabb_intersections_with_aabb

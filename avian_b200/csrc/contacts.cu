@@ -1,9 +1,8 @@
-// Device-resident contact edges (SURVEY.md 8f #1/#3; protocol: plugins.ResidentWorld, DESIGN.md §8).
-// One row per ContactId (contact_graph.rs:521-631 assigns them; the host keeps that graph).  A row holds the pair (colliders, bodies), the
-// manifold the last narrow phase found (4 point slots, column scalar type: what the solver reads through avn_solver_upload_graph), the
+// The device-resident contact store (SURVEY.md 8f #1/#3, DESIGN.md §7b).
+// One row per ContactId (contact_graph.rs:521-631 assigns them; so does the ContactGraph below).  A row holds the pair (colliders, bodies), the
+// manifold the last narrow phase found (4 point slots, column scalar type: what the solver reads through avn_solver_upload_resident), the
 // unrounded anchors of that manifold (double: what the next step's match_contacts compares) and the warm-start impulses (in = what the
 // next solve starts from, written by the matching; out = what the last solve left, written by store_contact_impulses).
-// Per step only point counts and disjoint flags go to the host (2 B per row) and the edge list of the constraint graph comes back.
 #include <cooperative_groups.h>
 
 #include <algorithm>
@@ -452,24 +451,6 @@ __global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ l
     ob[i] = g.pflags[e] & EV_FLAGS; ob[n + i] = uint8_t(cnt);
 }
 
-__global__ void edge_add_kernel(int n, const uint32_t* __restrict__ ids, const uint32_t* __restrict__ c1, const uint32_t* __restrict__ c2,
-                                const uint32_t* __restrict__ b1, const uint32_t* __restrict__ b2, uint32_t* rc1, uint32_t* rc2, uint32_t* rb1, uint32_t* rb2,
-                                uint8_t* live, uint8_t* count, uint8_t* prev_count) {
-    int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= n) return;
-    const uint32_t e = ids[k];
-    rc1[e] = c1[k]; rc2[e] = c2[k]; rb1[e] = b1[k]; rb2[e] = b2[k];
-    live[e] = 1;        // a ContactId handed to a new pair starts without history
-    count[e] = 0;
-    prev_count[e] = 0;
-}
-__global__ void edge_remove_kernel(int n, const uint32_t* __restrict__ ids, uint8_t* live, uint8_t* count, uint8_t* prev_count) {
-    int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= n) return;
-    const uint32_t e = ids[k];
-    live[e] = 0; count[e] = 0; prev_count[e] = 0;
-}
-
 template <class S>
 __global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -810,85 +791,6 @@ class Contacts final : public ContactsBase {
         if (copy_stream_) { cudaStreamSynchronize(copy_stream_); cudaStreamDestroy(copy_stream_); }
     }
 
-    AvnStatus reserve(uint32_t capacity) override {
-        if (capacity <= E_) return AVN_OK;
-        const size_t n = capacity;
-        struct Col { DevBuf* buf; size_t bytes_per_row; };
-        Col cols[] = {{&c1_, 4}, {&c2_, 4}, {&b1_, 4}, {&b2_, 4}, {&live_, 1}, {&count_, 1}, {&disjoint_, 1}, {&normal_, 3 * sizeof(S)}, {&a1_, 12 * sizeof(S)},
-                      {&a2_, 12 * sizeof(S)}, {&pen_, 4 * sizeof(S)}, {&ns_, 4 * sizeof(S)}, {&prev_count_, 1}, {&prev_a1_, 12 * sizeof(double)},
-                      {&prev_a2_, 12 * sizeof(double)}, {&ws_n_in_, 4 * sizeof(S)}, {&ws_t_in_, 8 * sizeof(S)}, {&ws_n_out_, 4 * sizeof(S)},
-                      {&ws_t_out_, 8 * sizeof(S)}, {&nimp_in_, 4 * sizeof(S)}, {&nimp_out_, 4 * sizeof(S)},
-                      // graph state per row (zero = no flags, not touching, no colour)
-                      {&pflags_, 1}, {&touching_, 1}, {&colour_, 1}, {&change_, 1}, {&old_colour_, 1}, {&ovf_pos_, 4}, {&ovf_, 4}, {&isl_event_, 1}, {&fresh_, 1},
-                      {&event_, 1}, {&asleep_, 1}};
-        for (Col& c : cols) {   // grow, keep the old rows, zero the new ones
-            void* fresh = nullptr;
-            AVN_CUDA(cudaMalloc(&fresh, n * c.bytes_per_row));
-            AVN_CUDA(cudaMemsetAsync(fresh, 0, n * c.bytes_per_row, stream_));
-            if (c.buf->p && E_) AVN_CUDA(cudaMemcpyAsync(fresh, c.buf->p, size_t(E_) * c.bytes_per_row, cudaMemcpyDeviceToDevice, stream_));
-            AVN_CUDA(cudaStreamSynchronize(stream_));
-            if (c.buf->p) cudaFree(c.buf->p);
-            c.buf->p = fresh;
-            c.buf->cap = n * c.bytes_per_row;
-        }
-        E_ = capacity;
-        // work buffers of the graph step (contents do not outlive a step) and the pair set (rebuilt by the next step)
-        const size_t nblocks = (n + RS_TILE - 1) / RS_TILE;
-        AVN_CUDA(k0_.ensure(n * 4)); AVN_CUDA(k1_.ensure(n * 4)); AVN_CUDA(v0_.ensure(n * 4)); AVN_CUDA(v1_.ensure(n * 4)); AVN_CUDA(list_.ensure(n * 4));
-        AVN_CUDA(evl_.ensure(n * 4));
-        AVN_CUDA(hist_.ensure(256 * nblocks * 4));
-        AVN_CUDA(m_b1_.ensure(n * 4)); AVN_CUDA(m_b2_.ensure(n * 4)); AVN_CUDA(m_fr_.ensure(n * sizeof(S))); AVN_CUDA(m_re_.ensure(n * sizeof(S)));
-        uint64_t cap = 1024;
-        while (cap < uint64_t(n) * 2) cap <<= 1;
-        AVN_CUDA(table_.ensure(cap * sizeof(uint64_t)));
-        table_mask_ = cap - 1;
-        table_dirty_ = true;
-        return AVN_OK;
-    }
-
-    AvnStatus add(uint32_t n, const uint32_t* ids, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2) override {
-        if (n == 0) return AVN_OK;
-        if (!ids || !c1 || !c2 || !b1 || !b2) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_add: every array is required");
-        for (uint32_t k = 0; k < n; ++k)
-            if (ids[k] >= E_) return err_->fail(AVN_ERR_CAPACITY, "contacts_add: id %u >= capacity %u (avn_contacts_reserve first)", ids[k], E_);
-        AVN_CUDA(stage_.ensure(size_t(5) * n * 4));
-        uint32_t* s = stage_.as<uint32_t>();
-        const uint32_t* src[5] = {ids, c1, c2, b1, b2};
-        for (int c = 0; c < 5; ++c) AVN_CUDA(cudaMemcpyAsync(s + size_t(c) * n, src[c], size_t(n) * 4, cudaMemcpyHostToDevice, stream_));
-        edge_add_kernel<<<(n + 255) / 256, 256, 0, stream_>>>(int(n), s, s + n, s + 2 * size_t(n), s + 3 * size_t(n), s + 4 * size_t(n), c1_.as<uint32_t>(),
-                                                              c2_.as<uint32_t>(), b1_.as<uint32_t>(), b2_.as<uint32_t>(), live_.as<uint8_t>(), count_.as<uint8_t>(),
-                                                              prev_count_.as<uint8_t>());
-        AVN_CUDA(cudaGetLastError());
-        for (uint32_t k = 0; k < n; ++k) hw_ = std::max(hw_, ids[k] + 1);   // rows managed by the host protocol: the high-water mark follows
-        AVN_CUDA(cudaStreamSynchronize(stream_));   // the host arrays may be reused by the caller
-        return AVN_OK;
-    }
-
-    AvnStatus remove(uint32_t n, const uint32_t* ids) override {
-        if (n == 0) return AVN_OK;
-        if (!ids) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_remove: ids are required");
-        for (uint32_t k = 0; k < n; ++k)
-            if (ids[k] >= E_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_remove: id %u >= capacity %u", ids[k], E_);
-        AVN_CUDA(stage_.ensure(size_t(n) * 4));
-        AVN_CUDA(cudaMemcpyAsync(stage_.p, ids, size_t(n) * 4, cudaMemcpyHostToDevice, stream_));
-        edge_remove_kernel<<<(n + 255) / 256, 256, 0, stream_>>>(int(n), stage_.as<uint32_t>(), live_.as<uint8_t>(), count_.as<uint8_t>(), prev_count_.as<uint8_t>());
-        AVN_CUDA(cudaGetLastError());
-        AVN_CUDA(cudaStreamSynchronize(stream_));
-        return AVN_OK;
-    }
-
-    AvnStatus narrow_phase(const AvnNarrowParams* prm, const AvnNarrowInput* in, uint32_t match_contacts, double length_unit, uint8_t* out_count,
-                           uint8_t* out_disjoint) override {
-        if (!prm || !in || !out_count || !out_disjoint) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_narrow_phase: params, input and outputs are required");
-        if (E_ == 0) return AVN_OK;
-        AvnStatus st = launch_narrow(prm, in, match_contacts, length_unit, E_);
-        if (st != AVN_OK) return st;
-        AVN_CUDA(cudaMemcpyAsync(out_count, count_.p, E_, cudaMemcpyDeviceToHost, stream_));
-        AVN_CUDA(cudaMemcpyAsync(out_disjoint, disjoint_.p, E_, cudaMemcpyDeviceToHost, stream_));
-        AVN_CUDA(cudaStreamSynchronize(stream_));
-        return AVN_OK;
-    }
-
     // ---- the graphs on the device ---------------------------------------------------------------------------------------------------
     AvnStatus configure(const AvnContactGraphConfig* cfg) override {
         if (!cfg || !cfg->body_kind) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_configure: config and body_kind are required");
@@ -1156,24 +1058,23 @@ class Contacts final : public ContactsBase {
         return AVN_OK;
     }
 
-    AvnStatus view(AvnEdgeManifolds* out) override {   // DEVICE pointers: the source of avn_solver_upload_graph
-        if (!out) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "out is required");
-        out->edge_capacity = E_;
+    void view(RowColumns* out) override {
+        out->rows = E_;
         out->point_count = count_.as<uint8_t>();
         out->normal = normal_.p; out->anchor1 = a1_.p; out->anchor2 = a2_.p; out->penetration = pen_.p; out->normal_speed = ns_.p;
         out->warm_start_normal_impulse = ws_n_in_.p;
         out->warm_start_tangent_impulse = ws_t_in_.p;
         out->normal_impulse = nimp_in_.p;
-        return AVN_OK;
     }
     void outputs(void** ws_n, void** ws_t, void** nimp) override { *ws_n = ws_n_out_.p; *ws_t = ws_t_out_.p; *nimp = nimp_out_.p; }
-    uint32_t capacity() const override { return E_; }
 
-    AvnStatus download_impulses(void* ws_n, void* ws_t, void* nimp) override {   // tests / debugging: the solver's outputs per edge
-        if (E_ == 0) return AVN_OK;
-        if (ws_n) AVN_CUDA(cudaMemcpyAsync(ws_n, ws_n_out_.p, size_t(E_) * 4 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
-        if (ws_t) AVN_CUDA(cudaMemcpyAsync(ws_t, ws_t_out_.p, size_t(E_) * 8 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
-        if (nimp) AVN_CUDA(cudaMemcpyAsync(nimp, nimp_out_.p, size_t(E_) * 4 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+    AvnStatus download_impulses(uint32_t capacity, void* ws_n, void* ws_t, void* nimp) override {   // tests / tools: the solver's outputs per row
+        const size_t n = std::min(capacity, E_);
+        if (n) {
+            if (ws_n) AVN_CUDA(cudaMemcpyAsync(ws_n, ws_n_out_.p, n * 4 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+            if (ws_t) AVN_CUDA(cudaMemcpyAsync(ws_t, ws_t_out_.p, n * 8 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+            if (nimp) AVN_CUDA(cudaMemcpyAsync(nimp, nimp_out_.p, n * 4 * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        }
         AVN_CUDA(cudaStreamSynchronize(stream_));
         return AVN_OK;
     }
@@ -1402,11 +1303,46 @@ class Contacts final : public ContactsBase {
     }
 
    private:
+    AvnStatus reserve(uint32_t capacity) {
+        if (capacity <= E_) return AVN_OK;
+        const size_t n = capacity;
+        struct Col { DevBuf* buf; size_t bytes_per_row; };
+        Col cols[] = {{&c1_, 4}, {&c2_, 4}, {&b1_, 4}, {&b2_, 4}, {&live_, 1}, {&count_, 1}, {&disjoint_, 1}, {&normal_, 3 * sizeof(S)}, {&a1_, 12 * sizeof(S)},
+                      {&a2_, 12 * sizeof(S)}, {&pen_, 4 * sizeof(S)}, {&ns_, 4 * sizeof(S)}, {&prev_count_, 1}, {&prev_a1_, 12 * sizeof(double)},
+                      {&prev_a2_, 12 * sizeof(double)}, {&ws_n_in_, 4 * sizeof(S)}, {&ws_t_in_, 8 * sizeof(S)}, {&ws_n_out_, 4 * sizeof(S)},
+                      {&ws_t_out_, 8 * sizeof(S)}, {&nimp_in_, 4 * sizeof(S)}, {&nimp_out_, 4 * sizeof(S)},
+                      // graph state per row (zero = no flags, not touching, no colour)
+                      {&pflags_, 1}, {&touching_, 1}, {&colour_, 1}, {&change_, 1}, {&old_colour_, 1}, {&ovf_pos_, 4}, {&ovf_, 4}, {&isl_event_, 1}, {&fresh_, 1},
+                      {&event_, 1}, {&asleep_, 1}};
+        for (Col& c : cols) {   // grow, keep the old rows, zero the new ones
+            void* fresh = nullptr;
+            AVN_CUDA(cudaMalloc(&fresh, n * c.bytes_per_row));
+            AVN_CUDA(cudaMemsetAsync(fresh, 0, n * c.bytes_per_row, stream_));
+            if (c.buf->p && E_) AVN_CUDA(cudaMemcpyAsync(fresh, c.buf->p, size_t(E_) * c.bytes_per_row, cudaMemcpyDeviceToDevice, stream_));
+            AVN_CUDA(cudaStreamSynchronize(stream_));
+            if (c.buf->p) cudaFree(c.buf->p);
+            c.buf->p = fresh;
+            c.buf->cap = n * c.bytes_per_row;
+        }
+        E_ = capacity;
+        // work buffers of the graph step (contents do not outlive a step) and the pair set (rebuilt by the next step)
+        const size_t nblocks = (n + RS_TILE - 1) / RS_TILE;
+        AVN_CUDA(k0_.ensure(n * 4)); AVN_CUDA(k1_.ensure(n * 4)); AVN_CUDA(v0_.ensure(n * 4)); AVN_CUDA(v1_.ensure(n * 4)); AVN_CUDA(list_.ensure(n * 4));
+        AVN_CUDA(evl_.ensure(n * 4));
+        AVN_CUDA(hist_.ensure(256 * nblocks * 4));
+        AVN_CUDA(m_b1_.ensure(n * 4)); AVN_CUDA(m_b2_.ensure(n * 4)); AVN_CUDA(m_fr_.ensure(n * sizeof(S))); AVN_CUDA(m_re_.ensure(n * sizeof(S)));
+        uint64_t cap = 1024;
+        while (cap < uint64_t(n) * 2) cap <<= 1;
+        AVN_CUDA(table_.ensure(cap * sizeof(uint64_t)));
+        table_mask_ = cap - 1;
+        table_dirty_ = true;
+        return AVN_OK;
+    }
     // the collider / body columns of a step -> device (on `s`); keep_shapes: shape and dims are those of the previous call
     AvnStatus upload_inputs(const AvnNarrowInput* in, bool keep_shapes, cudaStream_t s) {
         const size_t C = in->collider_count, B = in->body_count;
         if (!in->dims || !in->position || !in->rotation || !in->linear_velocity || !in->angular_velocity || !in->aabb_min || !in->aabb_max)
-            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_narrow_phase: dims, position, rotation, velocities and AABBs are required");
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: dims, position, rotation, velocities and AABBs are required");
         keep_shapes = keep_shapes && in_.colliders == C && in_.dims != nullptr;
         AvnStatus st;
         up_stream_ = s;

@@ -72,10 +72,8 @@ struct CcdRows;
 struct SolverBase {
     virtual ~SolverBase() {}
     virtual AvnStatus upload(const AvnStepParams* prm, AvnBodyColumns* bodies, AvnManifoldColumns* manifolds, AvnJointSet* joints) = 0;
-    virtual AvnStatus upload_edges(const AvnStepParams* prm, AvnBodyColumns* bodies, AvnEdgeManifolds* manifolds, AvnJointSet* joints) = 0;
-    // the same with the edge-indexed columns already on the device (ContactsBase::view / outputs): only the graph columns are uploaded
-    virtual AvnStatus upload_graph(const AvnStepParams* prm, AvnBodyColumns* bodies, const AvnEdgeManifolds* graph, ContactsBase* contacts, AvnJointSet* joints) = 0;
-    // the same with the colour-major list on the device as well (ContactsBase::graph_view): nothing of the constraints crosses the bus
+    // the same fed from the contact store: the rows (ContactsBase::view / outputs) and the colour-major list (ContactsBase::graph_view) are on the
+    // device, nothing of the constraints crosses the bus
     virtual AvnStatus upload_resident(const AvnStepParams* prm, AvnBodyColumns* bodies, ContactsBase* contacts, AvnJointSet* joints) = 0;
     virtual AvnStatus run() = 0;
     virtual AvnStatus run_range(uint32_t first, uint32_t count, uint32_t flags) = 0;
@@ -145,15 +143,16 @@ QueriesBase* make_queries(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* 
 
 struct ContactsBase {
     virtual ~ContactsBase() {}
-    virtual AvnStatus reserve(uint32_t capacity) = 0;
-    virtual AvnStatus add(uint32_t n, const uint32_t* ids, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2) = 0;
-    virtual AvnStatus remove(uint32_t n, const uint32_t* ids) = 0;
-    virtual AvnStatus narrow_phase(const AvnNarrowParams* prm, const AvnNarrowInput* in, uint32_t match_contacts, double length_unit, uint8_t* out_count,
-                                   uint8_t* out_disjoint) = 0;
-    virtual AvnStatus view(AvnEdgeManifolds* out) = 0;                       // device pointers of the edge-indexed columns
+    struct RowColumns {             // device pointers of the row columns (ContactId-indexed, 4 point slots per row, column scalar type)
+        uint32_t rows = 0;          // allocated rows
+        const uint8_t* point_count = nullptr;
+        const void* normal = nullptr; const void* anchor1 = nullptr; const void* anchor2 = nullptr; const void* penetration = nullptr;
+        const void* normal_speed = nullptr;
+        void* warm_start_normal_impulse = nullptr; void* warm_start_tangent_impulse = nullptr; void* normal_impulse = nullptr;
+    };
+    virtual void view(RowColumns* out) = 0;                                  // what the solver reads
     virtual void outputs(void** ws_n, void** ws_t, void** nimp) = 0;         // device pointers store_contact_impulses writes
-    virtual uint32_t capacity() const = 0;
-    virtual AvnStatus download_impulses(void* ws_n, void* ws_t, void* nimp) = 0;
+    virtual AvnStatus download_impulses(uint32_t capacity, void* ws_n, void* ws_t, void* nimp) = 0;
     // ---- the ContactGraph + ConstraintGraph on the device (contacts.cu)
     virtual AvnStatus configure(const AvnContactGraphConfig* cfg) = 0;
     // start the host-to-device copy of step()'s collider / body columns on a second stream (before the broad phase is waited for)

@@ -71,8 +71,6 @@ class Solver final : public SolverBase {
     }
 
     AvnStatus upload(const AvnStepParams* prm, AvnBodyColumns* bc, AvnManifoldColumns* mc, AvnJointSet* js) override;
-    AvnStatus upload_edges(const AvnStepParams* prm, AvnBodyColumns* bc, AvnEdgeManifolds* em, AvnJointSet* js) override;
-    AvnStatus upload_graph(const AvnStepParams* prm, AvnBodyColumns* bc, const AvnEdgeManifolds* graph, ContactsBase* contacts, AvnJointSet* js) override;
     AvnStatus upload_resident(const AvnStepParams* prm, AvnBodyColumns* bc, ContactsBase* contacts, AvnJointSet* js) override;
     AvnStatus run_range(uint32_t first, uint32_t count, uint32_t flags) override;
     AvnStatus set_boundary(const AvnBoundary* bnd) override;
@@ -178,7 +176,7 @@ class Solver final : public SolverBase {
     bool ccd_active() const { return ccd_ && ccd_->active(); }
     CcdBase* ccd_ = nullptr;
     ContactsBase* ccd_contacts_ = nullptr;
-    bool from_store_ = false;     // the upload's manifolds are the contact store's rows (upload_graph / upload_resident): swept CCD can run
+    bool from_store_ = false;     // the upload came from the contact store (upload_resident): swept CCD can run
     double length_unit_ = 1;
     template <int OP> void launch_phase(int begin, int count, bool serial = false) {
         if (count <= 0) return;
@@ -250,29 +248,25 @@ class Solver final : public SolverBase {
     DevSolver<S> dev_{};
     // host pointers for download
     AvnBodyColumns hb_{};
-    // where the manifolds of an upload come from: the CSR columns of AvnManifoldColumns or the edge-indexed columns of AvnEdgeManifolds
+    // where the manifolds of an upload come from: the CSR columns of AvnManifoldColumns (host), or the contact store (resident)
     struct ManifoldSource {
-        size_t M = 0, P = 0, normal_rows = 0;             // manifolds, rows of the point columns, rows of the normal column
+        size_t M = 0, P = 0;                               // manifolds, rows of the point columns
         const uint32_t* color_offsets = nullptr;
         const int32_t* body1 = nullptr; const int32_t* body2 = nullptr;
         const void* friction = nullptr; const void* restitution = nullptr; const void* tangent_velocity = nullptr; const void* normal = nullptr;
         const uint32_t* point_offsets = nullptr;           // CSR
-        const uint32_t* edge = nullptr; const uint8_t* edge_point_count = nullptr;   // edge-indexed
+        const uint32_t* edge = nullptr; const uint8_t* edge_point_count = nullptr;   // resident: ContactId of manifold m, points per row
         const void* anchor1 = nullptr; const void* anchor2 = nullptr; const void* penetration = nullptr; const void* normal_speed = nullptr;
         void* ws_normal = nullptr; void* ws_tangent = nullptr; void* normal_impulse = nullptr;
-        // device == true: the edge-indexed columns above (point counts, normal, point columns, impulse inputs) are DEVICE pointers owned by the
-        // contact store, and store_contact_impulses writes to out_* (device) instead of buffers of this solver; nothing of them is copied
-        bool device = false;
-        bool reuse_graph = false;   // upload_graph: the colour-major list (edge, body1, body2, friction, restitution) of the previous upload is still valid
-        bool device_list = false;   // upload_resident: edge, body1, body2, friction, restitution are DEVICE pointers too (the contact store's list)
+        // resident == true: every column above is a DEVICE pointer owned by the contact store (its rows, 4 point slots per row, and its
+        // colour-major list), store_contact_impulses writes to out_* (device) instead of buffers of this solver; nothing of them is copied
+        bool resident = false;
         bool list_restitution = false;
         void* out_ws_normal = nullptr; void* out_ws_tangent = nullptr; void* out_normal_impulse = nullptr;
     };
     AvnStatus upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, const ManifoldSource* src, AvnJointSet* js);
     ManifoldSource hm_{};
-    bool graph_on_device_ = false, graph_restitution_ = false;   // avn_solver_upload_graph: the resident colour-major list
-    uint32_t graph_count_ = 0, graph_color_offsets_[AVN_GRAPH_COLOR_COUNT + 1] = {};
-    DevBuf m_edge_, m_pbegin_, m_pend_, e_cnt_;
+    DevBuf m_pbegin_, m_pend_;
     AvnJointSet hj_{};
     bool have_m_ = false, have_j_ = false;
 
@@ -310,37 +304,16 @@ AvnStatus Solver<S>::build_joint_schedule(const AvnBodyColumns& bc, const AvnJoi
 
 template <class S>
 AvnStatus Solver<S>::upload(const AvnStepParams* prm, AvnBodyColumns* bc, AvnManifoldColumns* mc, AvnJointSet* js) {
-    from_store_ = false;
     if (!mc || mc->count == 0) return upload_impl(prm, bc, nullptr, js);
     if (!mc->body1 || !mc->body2 || !mc->normal || !mc->friction || !mc->restitution || !mc->point_offsets || !mc->anchor1 || !mc->anchor2 ||
         !mc->penetration || !mc->normal_speed || !mc->warm_start_normal_impulse || !mc->warm_start_tangent_impulse || !mc->normal_impulse)
         return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: every column except tangent_velocity is required");
-    graph_on_device_ = false;
     ManifoldSource src;
-    src.M = mc->count; src.P = mc->point_count; src.normal_rows = mc->count;
+    src.M = mc->count; src.P = mc->point_count;
     src.color_offsets = mc->color_offsets; src.body1 = mc->body1; src.body2 = mc->body2; src.friction = mc->friction; src.restitution = mc->restitution;
     src.tangent_velocity = mc->tangent_velocity; src.normal = mc->normal; src.point_offsets = mc->point_offsets;
     src.anchor1 = mc->anchor1; src.anchor2 = mc->anchor2; src.penetration = mc->penetration; src.normal_speed = mc->normal_speed;
     src.ws_normal = mc->warm_start_normal_impulse; src.ws_tangent = mc->warm_start_tangent_impulse; src.normal_impulse = mc->normal_impulse;
-    return upload_impl(prm, bc, &src, js);
-}
-
-template <class S>
-AvnStatus Solver<S>::upload_edges(const AvnStepParams* prm, AvnBodyColumns* bc, AvnEdgeManifolds* em, AvnJointSet* js) {
-    from_store_ = false;
-    if (!em || em->count == 0) return upload_impl(prm, bc, nullptr, js);
-    if (!em->edge || !em->body1 || !em->body2 || !em->friction || !em->restitution || !em->point_count || !em->normal || !em->anchor1 || !em->anchor2 ||
-        !em->penetration || !em->normal_speed || !em->warm_start_normal_impulse || !em->warm_start_tangent_impulse || !em->normal_impulse)
-        return err_->fail(AVN_ERR_INVALID_ARGUMENT, "edge manifolds: every column is required");
-    for (size_t m = 0; m < em->count; ++m)
-        if (em->edge[m] >= em->edge_capacity) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "edge manifolds: edge[%zu] = %u >= edge_capacity %u", m, em->edge[m], em->edge_capacity);
-    graph_on_device_ = false;
-    ManifoldSource src;
-    src.M = em->count; src.P = size_t(4) * em->edge_capacity; src.normal_rows = em->edge_capacity;
-    src.color_offsets = em->color_offsets; src.body1 = em->body1; src.body2 = em->body2; src.friction = em->friction; src.restitution = em->restitution;
-    src.normal = em->normal; src.edge = em->edge; src.edge_point_count = em->point_count;
-    src.anchor1 = em->anchor1; src.anchor2 = em->anchor2; src.penetration = em->penetration; src.normal_speed = em->normal_speed;
-    src.ws_normal = em->warm_start_normal_impulse; src.ws_tangent = em->warm_start_tangent_impulse; src.normal_impulse = em->normal_impulse;
     return upload_impl(prm, bc, &src, js);
 }
 
@@ -355,20 +328,16 @@ AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* b
         return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: %zu bodies, sleeping is applied to %u", size_t(bc->count), asleep.count);
     struct Reset { const uint8_t*& p; ~Reset() { p = nullptr; } } reset{body_asleep_};   // only this upload reads the column
     body_asleep_ = asleep.body_asleep;
-    from_store_ = true;
     ContactsBase::ResidentGraph g;
     AvnStatus st = contacts->graph_view(&g);
     if (st != AVN_OK) return st;
-    graph_on_device_ = false;
-    if (g.count == 0) return upload_impl(prm, bc, nullptr, js);
-    AvnEdgeManifolds v{};
-    if ((st = contacts->view(&v)) != AVN_OK) return st;
+    ContactsBase::RowColumns v;
+    contacts->view(&v);
     ManifoldSource src;
-    src.M = g.count; src.P = size_t(4) * v.edge_capacity; src.normal_rows = v.edge_capacity;
+    src.resident = true;
+    src.M = g.count; src.P = size_t(4) * v.rows;
     src.color_offsets = g.color_offsets; src.body1 = g.body1; src.body2 = g.body2; src.friction = g.friction; src.restitution = g.restitution;
     src.edge = g.edge;
-    src.device = true;
-    src.device_list = true;
     src.list_restitution = g.any_restitution != 0;
     src.normal = v.normal; src.edge_point_count = v.point_count;
     src.anchor1 = v.anchor1; src.anchor2 = v.anchor2; src.penetration = v.penetration; src.normal_speed = v.normal_speed;
@@ -377,53 +346,13 @@ AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* b
     return upload_impl(prm, bc, &src, js);
 }
 
-template <class S>
-AvnStatus Solver<S>::upload_graph(const AvnStepParams* prm, AvnBodyColumns* bc, const AvnEdgeManifolds* g, ContactsBase* contacts, AvnJointSet* js) {
-    from_store_ = true;
-    if (!g || g->count == 0) return upload_impl(prm, bc, nullptr, js);
-    if (!contacts) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_graph: no contact store");
-    // edge == NULL: "the graph has not changed since the last avn_solver_upload_graph" — the list stays on the device, only count and
-    // color_offsets are read (they must equal the previous upload's)
-    const bool reuse = g->edge == nullptr;
-    if (reuse) {
-        if (!graph_on_device_ || g->count != graph_count_ || memcmp(g->color_offsets, graph_color_offsets_, sizeof graph_color_offsets_) != 0)
-            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "graph: edge == NULL asks to reuse the previous graph, but none with %u manifolds and these colour offsets is resident", g->count);
-    } else if (!g->body1 || !g->body2 || !g->friction || !g->restitution) {
-        return err_->fail(AVN_ERR_INVALID_ARGUMENT, "graph: edge, body1, body2, friction and restitution are required");
-    }
-    AvnEdgeManifolds v{};
-    AvnStatus st = contacts->view(&v);
-    if (st != AVN_OK) return st;
-    if (!reuse)
-        for (size_t m = 0; m < g->count; ++m)
-            if (g->edge[m] >= v.edge_capacity) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "graph: edge[%zu] = %u >= capacity %u", m, g->edge[m], v.edge_capacity);
-    ManifoldSource src;
-    src.M = g->count; src.P = size_t(4) * v.edge_capacity; src.normal_rows = v.edge_capacity;
-    src.color_offsets = g->color_offsets; src.body1 = g->body1; src.body2 = g->body2; src.friction = g->friction; src.restitution = g->restitution;
-    src.edge = g->edge;
-    src.device = true;
-    src.reuse_graph = reuse;
-    src.normal = v.normal; src.edge_point_count = v.point_count;
-    src.anchor1 = v.anchor1; src.anchor2 = v.anchor2; src.penetration = v.penetration; src.normal_speed = v.normal_speed;
-    src.ws_normal = v.warm_start_normal_impulse; src.ws_tangent = v.warm_start_tangent_impulse; src.normal_impulse = v.normal_impulse;
-    contacts->outputs(&src.out_ws_normal, &src.out_ws_tangent, &src.out_normal_impulse);
-    graph_on_device_ = false;
-    st = upload_impl(prm, bc, &src, js);
-    if (st == AVN_OK) {
-        graph_on_device_ = true;
-        graph_count_ = g->count;
-        memcpy(graph_color_offsets_, g->color_offsets, sizeof graph_color_offsets_);
-    }
-    return st;
-}
-
 // the kind column the stage runs with while sleeping is applied: asleep -> static (kind == NULL: every body is dynamic)
 __global__ void effective_kind_kernel(int B, const uint8_t* __restrict__ kind, const uint8_t* __restrict__ body_asleep, uint8_t* __restrict__ out) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < B) out[b] = body_asleep[b] ? uint8_t(AVN_BODY_STATIC) : kind ? kind[b] : uint8_t(AVN_BODY_DYNAMIC);
 }
 
-// fills the point ranges of the manifolds of an edge-indexed upload: 4 slots per edge, the first point_count[edge] of them live
+// fills the point ranges of the manifolds of a resident upload: 4 slots per row, the first point_count[row] of them live
 __global__ void edge_ranges_kernel(const uint32_t* __restrict__ edge, const uint8_t* __restrict__ count, int M, uint32_t* __restrict__ begin,
                                    uint32_t* __restrict__ end) {
     int m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -439,6 +368,7 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
     if (bc->count && (!bc->position || !bc->rotation || !bc->linear_velocity || !bc->angular_velocity || !bc->inverse_mass || !bc->inverse_inertia_local))
         return err_->fail(AVN_ERR_INVALID_ARGUMENT, "bodies: position, rotation, velocities, inverse_mass and inverse_inertia_local are required");
     if (!(prm->h > 0) || !(prm->dt > 0) || prm->substeps == 0) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "dt, h and substeps must be positive");
+    from_store_ = mc && mc->resident;
     uploaded_ = false;
     ran_ = false;
     agreed_valid_ = false;
@@ -518,29 +448,22 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: color_offsets must span [0, count]");
         for (int c = 0; c < AVN_GRAPH_COLOR_COUNT; ++c)
             if (mc->color_offsets[c] > mc->color_offsets[c + 1]) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: color_offsets must be non-decreasing");
-        {   // widest manifold: sizes the shared-memory staging tile (3 rows per point) and validates the point ranges
+        if (mc->resident) {
+            max_np_ = AVN_MAX_MANIFOLD_POINTS;   // the point counts live on the device: take the general kernel build
+        } else {
+            // widest manifold: sizes the shared-memory staging tile (3 rows per point) and validates the point ranges
+            const uint32_t* po = mc->point_offsets;
+            if (po[M] != P) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: point_offsets[count] != point_count");
             uint32_t widest = 0, bad = 0;
-            if (mc->point_offsets) {
-                const uint32_t* po = mc->point_offsets;
-                if (po[M] != P) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: point_offsets[count] != point_count");
-                for (size_t i = 0; i < M; ++i) {
-                    bad |= uint32_t(po[i + 1] < po[i]);
-                    const uint32_t n = po[i + 1] - po[i];
-                    widest = n > widest ? n : widest;
-                }
-            } else if (mc->device) {
-                widest = AVN_MAX_MANIFOLD_POINTS;   // the counts live on the device: take the general kernel build
-            } else {
-                for (size_t i = 0; i < M; ++i) {
-                    const uint32_t n = mc->edge_point_count[mc->edge[i]];
-                    widest = n > widest ? n : widest;
-                }
+            for (size_t i = 0; i < M; ++i) {
+                bad |= uint32_t(po[i + 1] < po[i]);
+                const uint32_t n = po[i + 1] - po[i];
+                widest = n > widest ? n : widest;
             }
             if (bad || widest > AVN_MAX_MANIFOLD_POINTS)
                 return err_->fail(AVN_ERR_INVALID_ARGUMENT, "manifolds: at most %d points per manifold, point ranges must not decrease", AVN_MAX_MANIFOLD_POINTS);
             max_np_ = int(std::max<uint32_t>(widest, 1));
-        }
-        if (!mc->reuse_graph && !mc->device_list) {   // body indices are gathered through on the device (inr[2*b], vel[2*b], ver[b] ...): anything outside [AVN_NO_BODY, B) would read and
+            // body indices are gathered through on the device (inr[2*b], vel[2*b], ver[b] ...): anything outside [AVN_NO_BODY, B) would read and
             // write out of bounds, so it is rejected here (streaming pass over two int columns)
             const int32_t* hb1 = mc->body1; const int32_t* hb2 = mc->body2;
             const int64_t Bi = int64_t(B);
@@ -566,44 +489,33 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
             d.color_off[AVN_GRAPH_COLOR_COUNT] = slot;
             d.Mpad = std::max(slot, 32);
         }
-        if (mc->device_list) {   // the contact store's list (its bodies are the rows' bodies, validated when the pairs were formed)
+        if (mc->resident) {   // the contact store's list and rows, read in place (its bodies are the rows' bodies, validated when the pairs were formed)
             d.m_body1 = reinterpret_cast<const int*>(mc->body1); d.m_body2 = reinterpret_cast<const int*>(mc->body2);
             d.m_friction = static_cast<const S*>(mc->friction); d.m_restitution = static_cast<const S*>(mc->restitution);
-        } else if (mc->reuse_graph) {   // the list of the previous avn_solver_upload_graph is still in these buffers
-            d.m_body1 = m_b1_.as<int>(); d.m_body2 = m_b2_.as<int>(); d.m_friction = m_f_.as<S>(); d.m_restitution = m_r_.as<S>();
-        } else {
-            UP(m_b1_, mc->body1, M, int, m_body1);
-            UP(m_b2_, mc->body2, M, int, m_body2);
-            UP(m_f_, mc->friction, M, S, m_friction);
-            UP(m_r_, mc->restitution, M, S, m_restitution);
-        }
-        if (mc->device) d.m_normal = static_cast<const S*>(mc->normal); else UP(m_n_, mc->normal, 3 * mc->normal_rows, S, m_normal);
-        UP(m_tv_, mc->tangent_velocity, 3 * M, S, m_tanvel);
-        if (mc->point_offsets) {
-            UP(m_po_, mc->point_offsets, M + 1, uint32_t, m_point_begin);
-            d.m_point_end = d.m_point_begin + 1;
-            d.m_src = nullptr;
-        } else {
-            const uint8_t* d_count = nullptr;
-            if (mc->device_list) d.m_src = mc->edge;
-            else if (mc->reuse_graph) d.m_src = m_edge_.as<uint32_t>(); else UP(m_edge_, mc->edge, M, uint32_t, m_src);
-            if (mc->device) d_count = mc->edge_point_count;
-            else if ((st = up<uint8_t>(e_cnt_, mc->edge_point_count, mc->normal_rows, &d_count)) != AVN_OK) return st;
+            d.m_normal = static_cast<const S*>(mc->normal);
+            d.m_src = mc->edge;
             AVN_CUDA(m_pbegin_.ensure(M * sizeof(uint32_t)));
             AVN_CUDA(m_pend_.ensure(M * sizeof(uint32_t)));
-            edge_ranges_kernel<<<unsigned((M + 255) / 256), 256, 0, stream_>>>(d.m_src, d_count, int(M), m_pbegin_.as<uint32_t>(), m_pend_.as<uint32_t>());
+            edge_ranges_kernel<<<unsigned((M + 255) / 256), 256, 0, stream_>>>(d.m_src, mc->edge_point_count, int(M), m_pbegin_.as<uint32_t>(), m_pend_.as<uint32_t>());
             AVN_CUDA(cudaGetLastError());
             d.m_point_begin = m_pbegin_.as<uint32_t>();
             d.m_point_end = m_pend_.as<uint32_t>();
-        }
-        if (mc->device) {
             d.p_anchor1 = static_cast<const S*>(mc->anchor1); d.p_anchor2 = static_cast<const S*>(mc->anchor2);
             d.p_penetration = static_cast<const S*>(mc->penetration); d.p_normal_speed = static_cast<const S*>(mc->normal_speed);
             d.p_ws_normal = static_cast<const S*>(mc->ws_normal); d.p_ws_tangent = static_cast<const S*>(mc->ws_tangent);
             d.p_in_normal_impulse = static_cast<const S*>(mc->normal_impulse);
             d.p_out_ws_normal = static_cast<S*>(mc->out_ws_normal); d.p_out_ws_tangent = static_cast<S*>(mc->out_ws_tangent);
             d.p_normal_impulse = static_cast<S*>(mc->out_normal_impulse);
+            host_any_restitution_ = mc->list_restitution;
         } else {
+            UP(m_b1_, mc->body1, M, int, m_body1);
+            UP(m_b2_, mc->body2, M, int, m_body2);
+            UP(m_f_, mc->friction, M, S, m_friction);
+            UP(m_r_, mc->restitution, M, S, m_restitution);
+            UP(m_n_, mc->normal, 3 * M, S, m_normal);
+            UP(m_tv_, mc->tangent_velocity, 3 * M, S, m_tanvel);
+            UP(m_po_, mc->point_offsets, M + 1, uint32_t, m_point_begin);
+            d.m_point_end = d.m_point_begin + 1;
             UP(p_a1_, mc->anchor1, 3 * P, S, p_anchor1);
             UP(p_a2_, mc->anchor2, 3 * P, S, p_anchor2);
             UP(p_pen_, mc->penetration, P, S, p_penetration);
@@ -616,26 +528,11 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
             AVN_CUDA(p_owt_.ensure(2 * P * sizeof(S) + 16)); d.p_out_ws_tangent = p_owt_.as<S>();
             AVN_CUDA(p_ni_.ensure(P * sizeof(S) + 16));
             d.p_normal_impulse = p_ni_.as<S>();
-            if (!mc->point_offsets) {
-                // edge-indexed: rows of edges that are not in the constraint graph are not written by store_contact_impulses; they keep their
-                // input values (the reference leaves such ContactPoints untouched)
-                AVN_CUDA(cudaMemcpyAsync(d.p_out_ws_normal, d.p_ws_normal, P * sizeof(S), cudaMemcpyDeviceToDevice, stream_));
-                AVN_CUDA(cudaMemcpyAsync(d.p_out_ws_tangent, d.p_ws_tangent, 2 * P * sizeof(S), cudaMemcpyDeviceToDevice, stream_));
-                AVN_CUDA(cudaMemcpyAsync(d.p_normal_impulse, d.p_in_normal_impulse, P * sizeof(S), cudaMemcpyDeviceToDevice, stream_));
-            }
-        }
-
-        hm_ = *mc;
-        if (mc->device_list) {
-            host_any_restitution_ = mc->list_restitution;
-        } else if (mc->reuse_graph) {
-            host_any_restitution_ = graph_restitution_;
-        } else {
             host_any_restitution_ = false;
             const S* r = static_cast<const S*>(mc->restitution);
-            for (size_t i = 0; i < mc->M; ++i) host_any_restitution_ |= (r[i] != S(0));
-            graph_restitution_ = host_any_restitution_;
+            for (size_t i = 0; i < M; ++i) host_any_restitution_ |= (r[i] != S(0));
         }
+        hm_ = *mc;
     }
     {
         auto up256 = [](size_t x) { return (x + 255) & ~size_t(255); };
@@ -705,7 +602,7 @@ AvnStatus Solver<S>::run() {
     // swept CCD (ccd.cu) runs after the substeps and before restitution (ccd/mod.rs:257-261): the step is split around it
     if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run before avn_solver_upload");
     if (!from_store_ || !ccd_contacts_)
-        return err_->fail(AVN_ERR_UNSUPPORTED, "swept CCD is configured: it needs the contact store's ContactGraph (avn_solver_upload_resident / avn_solver_upload_graph), "
+        return err_->fail(AVN_ERR_UNSUPPORTED, "swept CCD is configured: it needs the contact store's ContactGraph (avn_solver_upload_resident), "
                                                "not host manifolds");
     AvnStatus st = launch_range(0, uint32_t(dev_.substeps), AVN_RUN_PREPARE);
     if (st != AVN_OK) return st;
@@ -1045,7 +942,7 @@ AvnStatus Solver<S>::download() {
         AVN_CUDA(cudaMemcpyAsync(hb_.linear_velocity, dev_.out_linvel, 3 * B * sizeof(S), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(hb_.angular_velocity, dev_.out_angvel, 3 * B * sizeof(S), cudaMemcpyDeviceToHost, stream_));
     }
-    if (have_m_ && !hm_.device) {
+    if (have_m_ && !hm_.resident) {
         const size_t P = hm_.P;
         AVN_CUDA(cudaMemcpyAsync(hm_.ws_normal, dev_.p_out_ws_normal, P * sizeof(S), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(hm_.ws_tangent, dev_.p_out_ws_tangent, 2 * P * sizeof(S), cudaMemcpyDeviceToHost, stream_));

@@ -37,8 +37,6 @@ def _load():
         lib.avh_raw_manifolds.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 12 + [C.c_double, C.c_double] + [_vp] * 9
         lib.avh_active_edges.argtypes = [_vp] * 6
         lib.avh_active_edges.restype = C.c_uint32
-        lib.avh_apply_counts.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_uint32, C.POINTER(C.c_uint32)]
-        lib.avh_apply_counts.restype = C.c_uint32
         lib.avh_export_edges.argtypes = [_vp] * 7
         lib.avh_export_edges.restype = None
         lib.avh_match_raw.argtypes = [C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, C.c_double, C.c_uint32, _vp, _vp, _vp, _vp, _vp]
@@ -302,20 +300,12 @@ class HostPipeline:
                                       _p(man.normal_speed), _p(man.warm_start_normal_impulse), _p(man.warm_start_tangent_impulse))
         return man
 
-    # ---- resident mode: the geometry runs elsewhere, the host keeps only the graphs (SURVEY.md 8f #1/#3)
+    # ---- the graphs in the contact store's terms: ContactId-indexed edges (SURVEY.md 8f #1/#3)
     def active_edges(self):
         n = self.pair_count
         ids, c1, c2, b1, b2 = (np.zeros(n, dtype=np.uint32) for _ in range(5))
         k = int(self.lib.avh_active_edges(self.h, _p(ids), _p(c1), _p(c2), _p(b1), _p(b2)))
         return ids[:k], c1[:k], c2[:k], b1[:k], b2[:k]
-
-    def apply_counts(self, bodies: api.Bodies, ids: np.ndarray, point_count: np.ndarray, disjoint: np.ndarray):
-        """Touching state machine + contact / constraint graph updates from per-edge point counts.  Returns (manifolds, points) in the graph."""
-        pts = C.c_uint32(0)
-        kind = np.ascontiguousarray(bodies.kind, dtype=np.uint8)
-        ids, point_count, disjoint = np.ascontiguousarray(ids, dtype=np.uint32), np.ascontiguousarray(point_count, dtype=np.uint8), np.ascontiguousarray(disjoint, dtype=np.uint8)
-        m = int(self.lib.avh_apply_counts(self.h, _p(kind), _p(ids), _p(point_count), _p(disjoint), int(ids.shape[0]), C.byref(pts)))
-        return m, int(pts.value)
 
     def export_edges(self, m: int):
         """The constraint graph as a colour-major list of edge ids + per-edge bodies and material."""

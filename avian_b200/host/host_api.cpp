@@ -611,7 +611,7 @@ void avh_raw_manifolds(uint32_t scalar_bits, uint32_t pair_count, const uint32_t
     }
 }
 
-// ---- resident mode (SURVEY.md 8f #1/#3): the geometry runs elsewhere (avn_narrow_phase), the host keeps only the graphs -------------
+// ---- the graphs and the per-row state in the contact store's terms (SURVEY.md 8f #1/#3): ContactId-indexed edges, 4 point slots per row ----
 // The active contact edges in ContactGraph order: edge id (ContactId), colliders, bodies.  Arrays sized avh_pair_count().
 uint32_t avh_active_edges(AvhPipeline* h, uint32_t* ids, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2) {
     Pipeline& P = *reinterpret_cast<Pipeline*>(h);
@@ -624,40 +624,8 @@ uint32_t avh_active_edges(AvhPipeline* h, uint32_t* ids, uint32_t* c1, uint32_t*
     return n;
 }
 
-// The host half of the narrow phase from the per-edge results computed elsewhere: point_count[i] (0 = not touching) and disjoint[i] for
-// edge ids[i].  Same status machine, same graph updates as avh_narrow_phase; the manifolds only remember how many points they have.
-uint32_t avh_apply_counts(AvhPipeline* h, const uint8_t* kind, const uint32_t* ids, const uint8_t* point_count, const uint8_t* disjoint_in, uint32_t n,
-                          uint32_t* out_points) {
-    Pipeline& P = *reinterpret_cast<Pipeline*>(h);
-    std::vector<uint32_t> changed;
-    std::vector<uint8_t> disjoint(P.pairs.size(), 0), started(P.pairs.size(), 0), stopped(P.pairs.size(), 0);
-    std::vector<int> count_change(P.pairs.size(), 0);
-    for (uint32_t i = 0; i < n; ++i) {
-        const uint32_t id = ids[i];
-        Pair& pr = P.pairs[id];
-        if (pr.asleep) continue;
-        if (disjoint_in[i]) { disjoint[id] = 1; changed.push_back(id); continue; }
-        pr.static1 = kind[pr.body1] == AVN_BODY_STATIC;
-        pr.static2 = kind[pr.body2] == AVN_BODY_STATIC;
-        const size_t old_count = pr.manifolds.size();
-        pr.manifolds.clear();
-        if (point_count[i] > 0) {
-            Manifold m;
-            m.normal = V3{0, 0, 0};
-            m.pts.resize(point_count[i]);
-            pr.manifolds.push_back(std::move(m));
-        }
-        const bool touching = !pr.manifolds.empty();
-        count_change[id] = int(pr.manifolds.size()) - int(old_count);
-        if (touching && !pr.touching) { started[id] = 1; changed.push_back(id); }
-        else if (!touching && pr.touching) { stopped[id] = 1; changed.push_back(id); }
-        else if (count_change[id] != 0) changed.push_back(id);
-    }
-    return apply_status_changes(P, changed, disjoint, started, stopped, count_change, out_points);
-}
-
 // The constraint graph as a colour-major list of edge ids (manifold_handles order) with the per-edge material (what the solver's prepare
-// needs besides the geometry).  Arrays sized from avh_apply_counts' return value.
+// needs besides the geometry).  Arrays sized by the number of manifolds in the graph.
 void avh_export_edges(AvhPipeline* h, uint32_t* color_offsets /*[25]*/, uint32_t* edge, int32_t* body1, int32_t* body2, double* friction, double* restitution) {
     Pipeline& P = *reinterpret_cast<Pipeline*>(h);
     uint32_t m = 0;

@@ -276,204 +276,6 @@ class World:
         self.step_index += 1
 
 
-class ResidentWorld(World):
-    """The same world stepped through the RESIDENT protocol (SURVEY.md 8f #1/#3, DESIGN.md §8): what a device-resident pipeline keeps
-    on the GPU lives here in edge-indexed arrays (ContactId-indexed, 4 point slots per edge), the host keeps only the graphs.
-
-        geometry (per edge, no host state)  ->  point counts + disjoint flags to the host  ->  touching state machine, contact graph,
-        constraint-graph colouring  ->  colour-major list of edge ids back  ->  the solver gathers its manifolds from the edge arrays
-        ->  warm-start impulses scattered back into the edge arrays.
-
-    `geometry(dt, tol, pairs, colliders, lin_vel, ang_vel, f64_anchors=True)` is fixture.raw_manifolds here and avn_narrow_phase on the
-    device; everything else is the bookkeeping the device kernels will replace one by one.  Stepping this world gives the same
-    manifolds, bit for bit, as World (tests/test_resident_cpu.py): it is the executable specification of the protocol."""
-
-    def __init__(self, scene: Scene, plugins: PhysicsPlugins, geometry=None, **kw):
-        super().__init__(scene, plugins, **kw)
-        from avian_b200 import fixture
-        self.geometry = geometry or fixture.raw_manifolds
-        self._fixture = fixture
-        self.capacity = 0
-        self._grow(1024)
-        self.edge_key = np.zeros(0, dtype=np.uint64)
-        self.bytes_to_host = 0        # what crosses PCIe per step in a device-resident pipeline (counts + flags; pairs come on top)
-        self.bytes_to_device = 0      # (edge list of the graph)
-
-    def _grow(self, capacity: int) -> None:
-        s = self.scalar
-        def grown(name, shape, dtype):
-            new = np.zeros((capacity,) + shape, dtype=dtype)
-            old = getattr(self, name, None)
-            if old is not None:
-                new[:old.shape[0]] = old
-            setattr(self, name, new)
-        grown("e_count", (), np.uint8)                 # resident per-edge state
-        grown("e_normal", (3,), s)
-        grown("e_anchor1", (4, 3), s); grown("e_anchor2", (4, 3), s)
-        grown("e_penetration", (4,), s); grown("e_normal_speed", (4,), s)
-        grown("e_prev_count", (), np.uint8)            # what match_contacts compares against, in double like the fixture
-        grown("e_prev_a1", (4, 3), np.float64); grown("e_prev_a2", (4, 3), np.float64)
-        grown("e_ws_n", (4,), s); grown("e_ws_t", (4, 2), s)
-        grown("e_key", (), np.uint64)
-        self.capacity = capacity
-
-    def narrow_phase(self) -> api.Manifolds:
-        p, b, s = self.pipeline, self.bodies, self.scalar
-        ids, c1, c2, b1, b2 = p.active_edges()
-        if ids.size and int(ids.max()) >= self.capacity:
-            self._grow(max(2 * self.capacity, int(ids.max()) + 1))
-        # a ContactId handed to a new pair starts without history
-        key = (c1.astype(np.uint64) << np.uint64(32)) | c2.astype(np.uint64)
-        fresh = self.e_key[ids] != key
-        self.e_prev_count[ids[fresh]] = 0
-        self.e_ws_n[ids[fresh]] = 0
-        self.e_ws_t[ids[fresh]] = 0
-        self.e_key[ids] = key
-        colliders = {"shape": self.scene.shape_type.astype(np.uint8), "dims": np.asarray(self.scene.dims, dtype=s), "position": b.position,
-                     "rotation": b.rotation, "aabb_min": self.aabb_min, "aabb_max": self.aabb_max}
-        raw = self.geometry(s, self.params.dt, 0.005, (c1, c2, b1, b2), colliders, b.linear_velocity, b.angular_velocity, f64_anchors=True)
-        # device side: scatter into the edge arrays, carry the warm-start impulses over (match_contacts)
-        self.e_count[ids] = raw["point_count"]
-        for k in ("normal", "anchor1", "anchor2", "penetration", "normal_speed"):
-            getattr(self, "e_" + k)[ids] = raw[k]
-        lib = p.lib
-        lib.avh_match_raw(p.bits, int(ids.shape[0]), ids.ctypes.data, raw["point_count"].ctypes.data, raw["anchor1_f64"].ctypes.data,
-                          raw["anchor2_f64"].ctypes.data, 1.0, 1 if self.params.match_contacts else 0, self.e_prev_count.ctypes.data,
-                          self.e_prev_a1.ctypes.data, self.e_prev_a2.ctypes.data, self.e_ws_n.ctypes.data, self.e_ws_t.ctypes.data)
-        # host side: counts + flags in, graph updates, edge list out
-        self.bytes_to_host = 2 * int(ids.shape[0])
-        m, npts = p.apply_counts(b, ids, raw["point_count"], raw["disjoint"])
-        co, edge, eb1, eb2, fr, re = p.export_edges(m)
-        self.bytes_to_device = 4 * m
-        self._edges = edge
-        # solver input: gathered from the edge arrays by the edge list (on the device: an indirection in prepare_constraint_item)
-        cnt = self.e_count[edge].astype(np.int64)
-        po = np.concatenate([[0], np.cumsum(cnt)]).astype(np.uint32)
-        slot = np.arange(4)[None, :] < cnt[:, None]                      # [m, 4] live point slots, row-major = CSR order
-        self._slot = slot
-        take = lambda a: np.ascontiguousarray(a[edge][slot])
-        man = api.Manifolds(color_offsets=co, body1=eb1, body2=eb2, normal=np.ascontiguousarray(self.e_normal[edge]), friction=fr.astype(s),
-                            restitution=re.astype(s), point_offsets=po, anchor1=take(self.e_anchor1), anchor2=take(self.e_anchor2),
-                            penetration=take(self.e_penetration), normal_speed=take(self.e_normal_speed),
-                            warm_start_normal_impulse=take(self.e_ws_n), warm_start_tangent_impulse=take(self.e_ws_t),
-                            normal_impulse=np.zeros(int(po[-1]), dtype=s))
-        assert int(po[-1]) == npts
-        self.last_manifolds = man
-        return man
-
-    def solve(self) -> None:
-        m = self.last_manifolds
-        self.plugins.get("SolverPlugin").step(self.params, self.bodies, m, self.joints)
-        if m is not None and m.count:          # store_contact_impulses: back into the edge arrays
-            wn, wt = self.e_ws_n[self._edges], self.e_ws_t[self._edges]
-            wn[self._slot] = m.warm_start_normal_impulse
-            wt[self._slot] = m.warm_start_tangent_impulse
-            self.e_ws_n[self._edges] = wn
-            self.e_ws_t[self._edges] = wt
-
-
-class DeviceResidentWorld(World):
-    """The resident protocol with the device doing its part (ResidentWorld is the CPU specification): contact rows, manifolds and warm-start
-    impulses live in the library's contact store; per step the host sends the contact-graph changes (new / removed edges), receives one
-    point count and one disjoint flag per row, updates its graphs and sends the colour-major edge list; avn_solver_upload_graph reads the
-    manifolds where avn_contacts_narrow_phase left them."""
-
-    def __init__(self, scene: Scene, plugins: PhysicsPlugins, ctx: "api.Context", **kw):
-        super().__init__(scene, plugins, **kw)
-        self.ctx = ctx
-        self.capacity = 0
-        self.known = {}          # ContactId -> pair key of the row on the device
-        self.bytes_to_host = self.bytes_to_device = 0
-        self._steady = None      # step_steady's memory: which rows were touching, which ids are live
-        self._colliders = None
-
-    def narrow_phase(self):
-        p, b, s = self.pipeline, self.bodies, self.scalar
-        ids, c1, c2, b1, b2 = p.active_edges()
-        need = int(ids.max()) + 1 if ids.size else 0
-        if need > self.capacity:
-            self.capacity = max(1024, 2 * need)
-            self.ctx.contacts_reserve(self.capacity)
-        # contact-graph changes since the last step
-        key = (c1.astype(np.uint64) << np.uint64(32)) | c2.astype(np.uint64)
-        now = dict(zip(ids.tolist(), key.tolist()))
-        gone = [e for e in self.known if e not in now]
-        fresh = np.array([i for i, (e, k) in enumerate(now.items()) if self.known.get(e) != k], dtype=np.int64)
-        if gone:
-            self.ctx.contacts_remove(np.array(gone, dtype=np.uint32))
-        if fresh.size:
-            self.ctx.contacts_add(ids[fresh], c1[fresh], c2[fresh], b1[fresh], b2[fresh])
-        self.known = now
-        colliders = {"shape": self.scene.shape_type.astype(np.uint8), "dims": np.asarray(self.scene.dims, dtype=s), "position": b.position,
-                     "rotation": b.rotation, "aabb_min": self.aabb_min, "aabb_max": self.aabb_max}
-        count, disjoint = self.ctx.contacts_narrow_phase(self.params.dt, 0.005, colliders, b.linear_velocity, b.angular_velocity, self.capacity,
-                                                         bool(self.params.match_contacts))
-        self.bytes_to_host = 2 * self.capacity
-        self.bytes_to_device = 20 * int(fresh.size) + 4 * len(gone)
-        m, npts = p.apply_counts(b, ids, count[ids], disjoint[ids])
-        co, edge, eb1, eb2, fr, re = p.export_edges(m)
-        self.bytes_to_device += 4 * m
-        self.graph = {"color_offsets": co, "edge": edge, "body1": eb1, "body2": eb2, "friction": fr.astype(s), "restitution": re.astype(s)}
-        self.last_counts = count
-        self.last_manifolds = None
-        return self.graph
-
-    def solve(self) -> None:
-        self.ctx.solver_step_graph(self.params, self.bodies, self.graph, self.joints)
-
-    # ---- the steady-state step, incremental on the host: what an application pays per frame once the contact set has settled ------------
-    def step_steady(self, aabbs: api.Aabbs, pairs_out: api.PairList) -> bool:
-        """One whole step from HOST body columns through the resident protocol: avn_broadphase (host AABB columns in, new pairs out) ->
-        avn_contacts_narrow_phase (collider poses + velocities in, one point count and one disjoint flag per contact row out) ->
-        avn_solver_upload_graph + run + download (body columns in and out).  The host touches its graphs only when the device reports that
-        a pair appeared, separated, or started / stopped touching; otherwise the colour-major edge list of the previous step is still valid and
-        stays on the device.  Returns True when the fast path was taken."""
-        ctx, p, b, s = self.ctx, self.pipeline, self.bodies, self.scalar
-        ctx.broadphase_upload(aabbs)
-        ctx.broadphase_run()
-        ctx.broadphase_download(pairs_out)
-        if pairs_out.count or self._steady is None:
-            # contact-graph changes: the general path (edge deltas, graph update, new edge list)
-            if pairs_out.count:
-                p.commit_broadphase(aabbs, pairs_out.trimmed())
-            self.aabb_min, self.aabb_max = self._aabb_rows(aabbs)
-            self.narrow_phase()
-            self._steady = {"touching": self.last_counts > 0, "ids": p.active_edges()[0]}
-            self.solve()
-            return False
-        colliders = self._colliders
-        colliders["position"], colliders["rotation"] = b.position, b.rotation
-        count, disjoint = ctx.contacts_narrow_phase(self.params.dt, 0.005, colliders, b.linear_velocity, b.angular_velocity, self.capacity,
-                                                    bool(self.params.match_contacts))
-        touching = count > 0
-        reuse = not disjoint.any() and np.array_equal(touching, self._steady["touching"])
-        if not reuse:
-            ids = self._steady["ids"]
-            m, _ = p.apply_counts(b, ids, count[ids], disjoint[ids])
-            co, edge, eb1, eb2, fr, re = p.export_edges(m)
-            self.graph = {"color_offsets": co, "edge": edge, "body1": eb1, "body2": eb2, "friction": fr.astype(s), "restitution": re.astype(s)}
-            self._steady = None if disjoint.any() else {"touching": touching, "ids": ids}   # a separated pair changes the id set: general path next
-        self.last_counts = count
-        ctx.solver_step_graph(self.params, b, self.graph, self.joints, reuse_graph=reuse)
-        return reuse
-
-    def prepare_steady(self, aabbs: api.Aabbs) -> None:
-        """After the settle steps: freeze what does not change per step (shapes, the AABB columns of the broad-phase input in body order)."""
-        s = self.scalar
-        self.aabb_min, self.aabb_max = self._aabb_rows(aabbs)
-        self._colliders = {"shape": self.scene.shape_type.astype(np.uint8), "dims": np.asarray(self.scene.dims, dtype=s), "position": self.bodies.position,
-                           "rotation": self.bodies.rotation, "aabb_min": self.aabb_min, "aabb_max": self.aabb_max}
-        self._steady = None
-
-    @staticmethod
-    def _aabb_rows(aabbs: api.Aabbs):
-        """the interval columns (persistent order) back in collider order (collider index == row of the body columns in this fixture)"""
-        n = int(aabbs.collider.shape[0])
-        mn, mx = np.empty_like(aabbs.aabb_min), np.empty_like(aabbs.aabb_max)
-        mn[aabbs.collider], mx[aabbs.collider] = aabbs.aabb_min, aabbs.aabb_max
-        return mn, mx
-
-
 def island_joint_bodies(joints: "api.JointSet | None") -> np.ndarray | None:
     """[J, 2] the bodies every joint links, in type order: what PhysicsIslands::add_joint sees (avn_islands_configure)."""
     if joints is None or not joints.count:

@@ -302,31 +302,6 @@ AvnStatus avn_solver_upload(AvnContext* ctx, const AvnStepParams* params, AvnBod
 AvnStatus avn_solver_run(AvnContext* ctx);
 AvnStatus avn_solver_download(AvnContext* ctx);
 
-/* The same stage fed from EDGE-INDEXED manifold storage: the layout avn_narrow_phase writes (4 point slots per contact edge, indexed by
- * ContactId) plus the constraint graph as a colour-major list of edge ids.  prepare_contact_constraints reads manifold m through
- * edge[m]; store_contact_impulses writes the impulses back to the edge's slots.  This is the input form of a device-resident pipeline:
- * the geometry never has to be compacted or sent through the host, only the edge list changes hands (SURVEY.md 8f #1/#3). */
-typedef struct AvnEdgeManifolds {
-    uint32_t count;                                     /* M: manifolds in the constraint graph */
-    uint32_t edge_capacity;                             /* E: rows of the edge-indexed columns */
-    uint32_t color_offsets[AVN_GRAPH_COLOR_COUNT + 1];  /* colour c owns edge[off[c], off[c+1]) */
-    const uint32_t* edge;             /* [M] ContactId of manifold m */
-    const int32_t* body1;             /* [M] */
-    const int32_t* body2;
-    const void* friction;             /* [M] */
-    const void* restitution;          /* [M] */
-    const uint8_t* point_count;       /* [E] 0..4 */
-    const void* normal;               /* [E][3] */
-    const void* anchor1;              /* [E][4][3] */
-    const void* anchor2;
-    const void* penetration;          /* [E][4] */
-    const void* normal_speed;         /* [E][4] */
-    void* warm_start_normal_impulse;  /* [E][4]    in/out */
-    void* warm_start_tangent_impulse; /* [E][4][2] in/out */
-    void* normal_impulse;             /* [E][4]    out */
-} AvnEdgeManifolds;
-AvnStatus avn_solver_upload_edges(AvnContext* ctx, const AvnStepParams* params, AvnBodyColumns* bodies, AvnEdgeManifolds* manifolds, AvnJointSet* joints);
-
 /* ---- one coupled scene over several GPUs: the x-slab partition (SURVEY.md 8e, BASELINE north_star "single all-gather of boundary
  *      state per substep where the scene spans GPUs").  Not a reference interface: the reference is single-process. -------------
  * Each rank uploads its own bodies and constraints plus copies ("ghosts") of the remote bodies its constraints touch.  A body held
@@ -426,10 +401,10 @@ typedef struct AvnColliderColumns {
  */
 AvnStatus avn_update_aabbs(AvnContext* ctx, const AvnAabbParams* params, AvnColliderColumns* colliders);
 
-/* ---- contact manifolds (SURVEY.md 8f "next #1", geometry stage): one manifold of at most 4 points per contact pair of cuboid / sphere
- *      colliders.  Stands where NarrowPhase::update calls contact_manifolds (narrow_phase/system_param.rs:437-830,
+/* ---- contact manifolds, the stand-alone geometry stage (SURVEY.md 8f "next #1"): one manifold of at most 4 points per listed pair of
+ *      cuboid / sphere colliders.  Stands where NarrowPhase::update calls contact_manifolds (narrow_phase/system_param.rs:437-830,
  *      collider/parry/contact_query.rs:156-261); the arithmetic is this repository's generator (csrc/narrow_math.hpp — parry3d is not
- *      vendored), shared with the host fixture.  Matching, the touching state machine and the constraint graph stay on the host. -------- */
+ *      vendored), shared with the host fixture.  avn_contacts_step runs the same geometry on the rows of the contact store. -------------- */
 typedef struct AvnNarrowParams {
     double dt;                         /* Time::delta (narrow_phase/mod.rs:289) */
     double contact_tolerance;          /* PhysicsLengthUnit * NarrowPhaseConfig::contact_tolerance */
@@ -437,7 +412,7 @@ typedef struct AvnNarrowParams {
 
 typedef struct AvnNarrowInput {
     uint32_t pair_count, collider_count, body_count, _pad;
-    const uint32_t* collider1;         /* [pairs] row of the collider columns below (ascending ContactId order is the caller's business) */
+    const uint32_t* collider1;         /* [pairs] row of the collider columns below (avn_contacts_step ignores the pair arrays) */
     const uint32_t* collider2;
     const uint32_t* body1;             /* [pairs] row of the body velocity columns */
     const uint32_t* body2;
@@ -462,25 +437,6 @@ typedef struct AvnRawManifolds {      /* fixed stride: 4 point slots per pair, u
 } AvnRawManifolds;
 
 AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, AvnRawManifolds* out);
-
-/* ---- device-resident contact edges: the contact pairs, their manifolds and warm-start impulses stay on the device between steps; the host
- *      keeps the ContactGraph and the ConstraintGraph (contact_graph.rs, constraint_graph.rs) and exchanges a few bytes per edge with the
- *      device (protocol and its CPU specification: avian_b200/plugins.py ResidentWorld).  Row = ContactId. ---------------------------------- */
-AvnStatus avn_contacts_reserve(AvnContext* ctx, uint32_t capacity);                  /* rows; grows, keeps the existing rows */
-AvnStatus avn_contacts_add(AvnContext* ctx, uint32_t n, const uint32_t* ids, const uint32_t* collider1, const uint32_t* collider2,
-                           const uint32_t* body1, const uint32_t* body2);            /* ContactGraph::add_edge: the row starts without history */
-AvnStatus avn_contacts_remove(AvnContext* ctx, uint32_t n, const uint32_t* ids);     /* ContactGraph::remove_edge */
-/* Geometry + match_contacts for every live row (input: only the collider / body columns of AvnNarrowInput; the pair arrays are ignored).
- * out_point_count / out_disjoint: [capacity] host arrays — all the host needs for the touching state machine and the graphs. */
-AvnStatus avn_contacts_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, uint32_t match_contacts,
-                                    double length_unit, uint8_t* out_point_count, uint8_t* out_disjoint);
-/* The solver stage reading its manifolds from the resident rows: `graph` carries only count, color_offsets, edge, body1, body2, friction,
- * restitution (host); store_contact_impulses writes into the rows.  Then avn_solver_run / avn_solver_download (bodies only) as usual. */
-/* graph->edge == NULL: the constraint graph has not changed since the previous avn_solver_upload_graph (no contact started or stopped
- * touching) — the list stays on the device and only the bodies are uploaded; count and color_offsets must repeat the previous call's. */
-AvnStatus avn_solver_upload_graph(AvnContext* ctx, const AvnStepParams* params, AvnBodyColumns* bodies, const AvnEdgeManifolds* graph, AvnJointSet* joints);
-/* the impulses of the rows as the last solve left them (tests, tools): [capacity][4], [capacity][4][2], [capacity][4]; any may be NULL */
-AvnStatus avn_contacts_download_impulses(AvnContext* ctx, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse);
 
 /* ---- the ContactGraph and the ConstraintGraph on the device (SURVEY.md 8f "next #3"): after this nothing of the contact pipeline lives on
  *      the host.  Replaces, for the pairs the device narrow phase covers,
@@ -535,6 +491,9 @@ AvnStatus avn_broadphase_download_order(AvnContext* ctx, uint64_t* out_pair_coun
  * constraint graph); edge_list [manifold_count] = the colour-major list.  Any pointer may be NULL. */
 AvnStatus avn_contacts_download_graph(AvnContext* ctx, uint32_t capacity, uint32_t* collider1, uint32_t* collider2, uint8_t* live, uint8_t* touching,
                                       int8_t* colour, uint32_t* edge_list);
+/* the impulses of the rows as the last solve left them (tests, tools), in the context's scalar type: per row [capacity][4] warm-start normal,
+ * [capacity][4][2] warm-start tangent, [capacity][4] normal impulse; min(capacity, rows) rows are written.  Any pointer may be NULL. */
+AvnStatus avn_contacts_download_impulses(AvnContext* ctx, uint32_t capacity, void* warm_start_normal, void* warm_start_tangent, void* normal_impulse);
 
 /* ---- the contact pipeline's output to the application: collision events, sensors, removal of colliders, contact reports.  All of it works on
  *      the ContactGraph of avn_contacts_step; before the first avn_contacts_step of the context (before avn_contacts_configure for
@@ -858,9 +817,9 @@ AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* sh
  *      Geometry: cuboid and sphere colliders, conventions in avian_b200/csrc/ccd_math.hpp (linear: the shape casts of the spatial queries;
  *      non-linear: conservative advancement to eps = 1e-4 * length_unit, at most 64 iterations).
  *      Stated deviation: equal TOIs go to the lowest ContactId, where the reference keeps the first in ContactGraph adjacency order.
- *      Runs inside avn_solver_run when the upload came from the contact store (avn_solver_upload_resident / avn_solver_upload_graph): the
- *      step becomes prepare + substeps -> CCD pass -> restitution + finalize.  While CCD is configured, avn_solver_run_range,
- *      avn_solver_step_partitioned and a run after avn_solver_upload / avn_solver_upload_edges / avn_solver_step return AVN_ERR_UNSUPPORTED. */
+ *      Runs inside avn_solver_run when the upload came from the contact store (avn_solver_upload_resident): the step becomes
+ *      prepare + substeps -> CCD pass -> restitution + finalize.  While CCD is configured, avn_solver_run_range,
+ *      avn_solver_step_partitioned and a run after avn_solver_upload / avn_solver_step return AVN_ERR_UNSUPPORTED. */
 typedef enum AvnSweepMode { AVN_SWEEP_LINEAR = 0, AVN_SWEEP_NON_LINEAR = 1 } AvnSweepMode;
 
 typedef struct AvnCcdConfig {

@@ -37,7 +37,7 @@ def test_struct_layouts_match_the_header():
     """sizeof of every ABI struct, compiled from the header with gcc, equals the ctypes mirror"""
     import subprocess, tempfile
     names = ["AvnConfig", "AvnStepParams", "AvnBodyColumns", "AvnManifoldColumns", "AvnJointColumns", "AvnJointSet", "AvnAabbColumns",
-             "AvnPairList", "AvnTimings", "AvnEdgeManifolds", "AvnBoundary", "AvnNarrowParams", "AvnNarrowInput", "AvnRawManifolds",
+             "AvnPairList", "AvnTimings", "AvnBoundary", "AvnNarrowParams", "AvnNarrowInput", "AvnRawManifolds",
              "AvnContactGraphConfig", "AvnContactStep", "AvnIslandsConfig", "AvnIslandsStep"]
     src = '#include <stdio.h>\n#include "avian_b200.h"\nint main(){' + "".join(f'printf("{n} %zu\\n", sizeof({n}));' for n in names) + "return 0;}"
     with tempfile.TemporaryDirectory() as d:

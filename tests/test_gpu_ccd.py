@@ -162,14 +162,6 @@ def test_large_scene_and_refusals():
         with pytest.raises(api.AvianError) as e:
             ctx.solver_step_partitioned()
         assert e.value.status == api.ERR_UNSUPPORTED
-        graph = dict(color_offsets=np.zeros(api.GRAPH_COLOR_COUNT + 1, np.uint32), edge=np.zeros(0, np.uint32), body1=np.zeros(0, np.int32),
-                     body2=np.zeros(0, np.int32), friction=np.zeros(0), restitution=np.zeros(0))
-        edges = dict(point_count=np.zeros(1, np.uint8), normal=np.zeros((1, 3), scalar), anchor1=np.zeros((1, 4, 3), scalar), anchor2=np.zeros((1, 4, 3), scalar),
-                     penetration=np.zeros((1, 4), scalar), normal_speed=np.zeros((1, 4), scalar), warm_start_normal_impulse=np.zeros((1, 4), scalar),
-                     warm_start_tangent_impulse=np.zeros((1, 4, 2), scalar), normal_impulse=np.zeros((1, 4), scalar))
-        with pytest.raises(api.AvianError) as e:
-            ctx.solver_step_edges(prm, bodies, graph, edges)   # avn_solver_upload_edges, then the run is refused
-        assert e.value.status == api.ERR_UNSUPPORTED
         for bad in (dict(body=[0, 0], collider=[1, 2]), dict(body=[scene.bodies.count], collider=[0]), dict(body=[1], collider=[10 ** 7]),
                     dict(body=[1], collider=[1], mode=[7]), dict(body=[1], collider=[1], linear_threshold=[np.nan])):
             with pytest.raises(api.AvianError) as e:

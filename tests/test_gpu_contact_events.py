@@ -194,6 +194,24 @@ def _host_report(ctx, w, rep, capacity):
     return np.array(tot, dtype=w.scalar), np.array(mx, dtype=w.scalar), g
 
 
+def test_download_impulses_writes_at_most_capacity_rows(gpu_ctx):
+    """avn_contacts_download_impulses copies min(capacity, rows) rows: a buffer sized below the store is filled to its capacity and not beyond"""
+    with api.Context(device=0) as ctx:
+        w = plugins.DeviceGraphWorld(scenes.cube_stack(4, 3, 4, brick=True), plugins.PhysicsPlugins(ctx), ctx, substeps=4)
+        for _ in range(3):
+            w.step()
+        hw = int(w.stats["rows_high_water"])
+        n = hw // 2
+        assert n > 0
+        full = ctx.contacts_download_impulses(hw)
+        bufs = [np.full((hw,) + shape, np.float32(-7.5), dtype=np.float32) for shape in ((4,), (4, 2), (4,))]
+        ctx._check(ctx.lib.avn_contacts_download_impulses(ctx.handle, n, *(b.ctypes.data for b in bufs)))
+        for b, f in zip(bufs, full):
+            assert np.array_equal(b[:n], f[:n]), "the first rows differ from a download at full capacity"
+            assert (b[n:] == np.float32(-7.5)).all(), "rows past the capacity were written"
+        assert any((f[:n] != 0).any() for f in full), "the scene was meant to leave impulses in the first rows"
+
+
 @pytest.mark.parametrize("scene_fn", [lambda: scenes.cube_stack(6, 5, 5, brick=True),
                                       lambda: scenes.falling_spheres(400, seed=3, box=(6.0, 4.0, 6.0), scalar=np.float64)])
 def test_report_equals_a_host_computation(gpu_ctx, scene_fn):
@@ -213,7 +231,7 @@ def test_report_equals_a_host_computation(gpu_ctx, scene_fn):
                 assert np.array_equal(rep[k], host[k]), f"step {i}: {k}"
             for k in ("normal", "max_penetration"):
                 assert np.array_equal(rep[k].view(np.uint8), host[k].view(np.uint8)), f"step {i}: {k}"
-            tot, mx, g = _host_report(ctx_b, wb, rep, 1 << 16)
+            tot, mx, g = _host_report(ctx_b, wb, rep, wb.stats["rows_high_water"])
             assert np.array_equal(rep["total_normal_impulse"].view(np.uint8), tot.view(np.uint8)), f"step {i}: total"
             assert np.array_equal(rep["max_normal_impulse"].view(np.uint8), mx.view(np.uint8)), f"step {i}: max"
             touching = np.nonzero(g["live"].astype(bool) & g["touching"].astype(bool))[0]

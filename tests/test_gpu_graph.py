@@ -1,7 +1,8 @@
 """The ContactGraph and the ConstraintGraph on the device (SURVEY.md 8f #3; avn_contacts_configure / avn_contacts_step /
 avn_solver_upload_resident): DeviceGraphWorld against the ordinary GPU World, whose graphs live in the host fixture (a restatement of
 contact_graph.rs:521-631 and constraint_graph.rs:163-296).  Every step: the same ContactId for every pair, the same colour for every manifold,
-the overflow colour in the same list order, and the bodies bit for bit — i.e. nothing of the contact pipeline needs the host any more."""
+the overflow colour in the same list order, the impulses the solve leaves in the rows, and the bodies bit for bit — i.e. nothing of the
+contact pipeline needs the host any more."""
 import sys
 from pathlib import Path
 
@@ -65,11 +66,24 @@ def _check_graphs(wa, wb, ctx_b, step):
             assert np.array_equal(mine, np.sort(theirs)), f"step {step}: colour {c}"
 
 
+def _check_impulses(wa, wb, ctx_b, step):
+    """store_contact_impulses into the rows: the rows of the World's colour-major ContactIds hold the World's manifold columns, point by point"""
+    ma = wa.last_manifolds
+    if ma is None or not ma.count:
+        return
+    _, _, _, _, edge = _host_graph(wa)
+    wn, _, ni = ctx_b.contacts_download_impulses(wb.stats["rows_high_water"])
+    slot = np.arange(4)[None, :] < np.diff(ma.point_offsets.astype(np.int64))[:, None]
+    assert np.array_equal(wn[edge][slot], ma.warm_start_normal_impulse), f"step {step}: warm-start impulses"
+    assert np.array_equal(ni[edge][slot], ma.normal_impulse), f"step {step}: normal impulses"
+
+
 @pytest.mark.parametrize("scene_fn,steps,substeps,kick", [
     (lambda: scenes.cubes_example(4), 70, 4, True),                   # tumbling cubes: pairs appear, separate, ContactIds are reused
     (lambda: scenes.cube_stack(6, 5, 5, brick=True), 12, 4, False),   # a settling brick pile: contacts start and stop touching
     (lambda: _plate_on_cubes(5), 25, 4, False),                       # 25 manifolds on one body: the overflow colour
     (lambda: scenes.falling_spheres(400, seed=3, box=(6.0, 4.0, 6.0), scalar=np.float64), 30, 4, False),   # f64, sphere contacts
+    (lambda: scenes.ragdoll_field(9, pitch=1.2, drop_height=0.5), 40, 4, False),                          # joints next to the contacts
 ])
 def test_device_graphs_equal_the_host_graphs(gpu_ctx, scene_fn, steps, substeps, kick):
     sc_a, sc_b = scene_fn(), scene_fn()
@@ -83,6 +97,7 @@ def test_device_graphs_equal_the_host_graphs(gpu_ctx, scene_fn, steps, substeps,
         for i in range(steps):
             wa.step(); wb.step()
             _check_graphs(wa, wb, ctx_b, i)
+            _check_impulses(wa, wb, ctx_b, i)
             for k in ("position", "rotation", "linear_velocity", "angular_velocity"):
                 assert np.array_equal(getattr(wa.bodies, k), getattr(wb.bodies, k)), f"step {i}: {k}"
             st = wb.stats

@@ -1,6 +1,7 @@
-"""Device narrow phase, geometry stage (SURVEY.md 8f #1): avn_narrow_phase against the host fixture's generator — the same header
-(csrc/narrow_math.hpp) compiled by g++ and by nvcc — bit for bit: point counts, normals, anchors, penetrations, normal speeds and the
-disjoint flags, on random cuboid / sphere soups (face, edge and vertex contacts, deep overlaps, near misses) in f32 and f64."""
+"""Device narrow phase, the stand-alone geometry stage (SURVEY.md 8f #1): avn_narrow_phase against the host fixture's generator — the same
+header (csrc/narrow_math.hpp) compiled by g++ and by nvcc — bit for bit: point counts, normals, anchors, penetrations, normal speeds and the
+disjoint flags, on random cuboid / sphere soups (face, edge and vertex contacts, deep overlaps, near misses) in f32 and f64.  The contact
+store runs the same geometry on its rows inside avn_contacts_step (tests/test_gpu_graph.py)."""
 import sys
 from pathlib import Path
 
@@ -59,109 +60,3 @@ def test_without_aabbs_and_empty_input(gpu_ctx):
     bad = (np.array([1000], dtype=np.uint32),) * 4
     with pytest.raises(api.AvianError):
         gpu_ctx.narrow_phase(1.0 / 60.0, 0.005, bad, cols, lv, av)
-
-
-# ---- the solver fed from edge-indexed storage --------------------------------------------------------------------------------
-def test_solver_from_edge_indexed_manifolds_equals_the_csr_input(gpu_ctx):
-    """avn_solver_upload_edges: the same manifolds scattered over ContactId-indexed rows (4 slots per edge, gaps, arbitrary ids) and
-    listed colour by colour give the step of the CSR input bit for bit; impulses come back in the edges' slots, rows of edges that are
-    not in the graph keep their values."""
-    from avian_b200 import scenes
-    from helpers import advance_to_solver_input
-    _, (prm, b, m, j) = advance_to_solver_input(scenes.cube_stack(6, 4, 5, brick=True), steps=3, substeps=4)
-    bs, ms = b.copy(), m.copy()
-    gpu_ctx.solver_step(prm, bs, ms)
-    M = m.count
-    rng = np.random.default_rng(0)
-    E = 3 * M + 17
-    edge = rng.permutation(E)[:M].astype(np.uint32)            # arbitrary ContactIds with gaps
-    s = b.position.dtype
-    cnt = np.diff(m.point_offsets.astype(np.int64))
-    slot = np.arange(4)[None, :] < cnt[:, None]
-    edges = {"point_count": np.zeros(E, dtype=np.uint8), "normal": np.zeros((E, 3), dtype=s), "anchor1": np.zeros((E, 4, 3), dtype=s),
-             "anchor2": np.zeros((E, 4, 3), dtype=s), "penetration": np.zeros((E, 4), dtype=s), "normal_speed": np.zeros((E, 4), dtype=s),
-             "warm_start_normal_impulse": np.full((E, 4), 7.0, dtype=s), "warm_start_tangent_impulse": np.full((E, 4, 2), 7.0, dtype=s),
-             "normal_impulse": np.full((E, 4), 7.0, dtype=s)}
-    edges["point_count"][edge] = cnt
-    edges["normal"][edge] = m.normal
-    for k in ("anchor1", "anchor2", "penetration", "normal_speed", "warm_start_normal_impulse", "warm_start_tangent_impulse", "normal_impulse"):
-        rows = edges[k][edge]
-        rows[slot] = getattr(m, k)
-        edges[k][edge] = rows
-    graph = {"color_offsets": m.color_offsets, "edge": edge, "body1": m.body1, "body2": m.body2, "friction": m.friction, "restitution": m.restitution}
-    be = b.copy()
-    gpu_ctx.solver_step_edges(prm, be, graph, edges)
-    for k in ("position", "rotation", "linear_velocity", "angular_velocity"):
-        assert np.array_equal(getattr(be, k), getattr(bs, k)), k
-    for k in ("warm_start_normal_impulse", "warm_start_tangent_impulse", "normal_impulse"):
-        assert np.array_equal(edges[k][edge][slot], getattr(ms, k)), k
-    untouched = np.ones(E, dtype=bool); untouched[edge] = False
-    assert (edges["warm_start_normal_impulse"][untouched] == 7.0).all() and (edges["normal_impulse"][untouched] == 7.0).all()
-
-
-# ---- the whole resident protocol on the device -----------------------------------------------------------------------------------
-def _tumble(w):
-    rng = np.random.default_rng(5)
-    w.bodies.angular_velocity[1:] = rng.normal(0, 3.0, size=(w.bodies.count - 1, 3)).astype(w.bodies.angular_velocity.dtype)
-    w.bodies.linear_velocity[1:] = rng.normal(0, 1.5, size=(w.bodies.count - 1, 3)).astype(w.bodies.linear_velocity.dtype)
-
-
-@pytest.mark.parametrize("scene_fn,steps,substeps,kick", [
-    (lambda: __import__("avian_b200.scenes", fromlist=["x"]).cubes_example(4), 120, 6, True),          # pairs come and go, ContactIds are reused
-    (lambda: __import__("avian_b200.scenes", fromlist=["x"]).cube_stack(6, 5, 5, brick=True), 25, 4, False),
-    (lambda: __import__("avian_b200.scenes", fromlist=["x"]).ragdoll_field(9, pitch=1.2, drop_height=0.5), 40, 4, False),
-])
-def test_device_resident_world_equals_the_ordinary_world(gpu_ctx, scene_fn, steps, substeps, kick):
-    """Bodies of the device-resident pipeline vs the ordinary GPU world (host narrow phase, CSR upload), step after step, bit for bit;
-    the resident rows' impulses equal the ordinary world's manifold columns; a few bytes per edge cross the bus."""
-    from avian_b200 import plugins
-    wa = plugins.World(scene_fn(), plugins.PhysicsPlugins(gpu_ctx), substeps=substeps)
-    with api.Context(device=0, scalar=wa.scalar) as ctx_b:
-        wb = plugins.DeviceResidentWorld(scene_fn(), plugins.PhysicsPlugins(ctx_b), ctx_b, substeps=substeps)
-        if kick:
-            _tumble(wa); _tumble(wb)
-        for i in range(steps):
-            wa.broad_phase(); wb.broad_phase()
-            ma, gb = wa.narrow_phase(), wb.narrow_phase()
-            assert ma.count == gb["edge"].shape[0], f"step {i}: manifold count"
-            assert np.array_equal(ma.color_offsets, gb["color_offsets"]) and np.array_equal(ma.body1, gb["body1"]), f"step {i}: graph"
-            wa.solve(); wb.solve()
-            for k in ("position", "rotation", "linear_velocity", "angular_velocity"):
-                assert np.array_equal(getattr(wa.bodies, k), getattr(wb.bodies, k)), f"step {i}: {k}"
-            if ma.count:
-                wn, wt, ni = ctx_b.contacts_download_impulses(wb.capacity)
-                cnt = np.diff(ma.point_offsets.astype(np.int64))
-                slot = np.arange(4)[None, :] < cnt[:, None]
-                assert np.array_equal(wn[gb["edge"]][slot], ma.warm_start_normal_impulse), f"step {i}: impulses"
-                assert np.array_equal(ni[gb["edge"]][slot], ma.normal_impulse), f"step {i}: total impulses"
-        assert wb.bytes_to_host <= 2 * wb.capacity
-
-
-@pytest.mark.parametrize("scene_fn,steps,substeps,kick", [
-    (lambda: __import__("avian_b200.scenes", fromlist=["x"]).cubes_example(4), 80, 6, True),
-    (lambda: __import__("avian_b200.scenes", fromlist=["x"]).cube_stack(6, 5, 5, brick=True), 25, 4, False),
-])
-def test_step_steady_on_the_device_equals_the_ordinary_world(gpu_ctx, scene_fn, steps, substeps, kick):
-    """The bench's end-to-end arm: host AABB / body columns -> avn_broadphase -> avn_contacts_narrow_phase -> avn_solver_upload_graph (the resident
-    colour-major list reused while no contact starts or stops touching) -> bodies, against the ordinary GPU world, bit for bit every step."""
-    from avian_b200 import plugins
-    wa = plugins.World(scene_fn(), plugins.PhysicsPlugins(gpu_ctx), substeps=substeps)
-    with api.Context(device=0, scalar=wa.scalar) as ctx_b:
-        wb = plugins.DeviceResidentWorld(scene_fn(), plugins.PhysicsPlugins(ctx_b), ctx_b, substeps=substeps)
-        if kick:
-            _tumble(wa); _tumble(wb)
-        pairs_out = api.PairList.empty(1 << 16)
-        fast = 0
-        for i in range(steps):
-            wa.step()
-            mn, mx = wb.pipeline.update_aabbs(wb.bodies, wb.params.dt)
-            aabbs = wb.pipeline.intervals(wb.bodies, mn, mx)
-            aabbs.joint_disabled_body_pairs = wb.scene.joint_disabled_body_pairs
-            if wb._colliders is None:
-                wb.prepare_steady(aabbs)
-            wb._colliders["aabb_min"], wb._colliders["aabb_max"] = mn, mx
-            fast += bool(wb.step_steady(aabbs, pairs_out))
-            for k in ("position", "rotation", "linear_velocity", "angular_velocity"):
-                assert np.array_equal(getattr(wa.bodies, k), getattr(wb.bodies, k)), f"step {i}: {k}"
-        if not kick:   # (a tumbling scene changes its touching set every step: the reuse path is for settled scenes)
-            assert fast > 0, "the graph-reuse path never ran"
