@@ -309,7 +309,9 @@ template <class S> __device__ __forceinline__ void project_velocity_item(const D
     st4(&d.vel[2 * i], mk4<S>(v.x, v.y, v.z, S(0)));
     st4(&d.vel[2 * i + 1], mk4<S>(w.x, w.y, w.z, S(0)));
 }
-// joint_damping<T> (solver/plugin.rs:759-806); same level schedule as the solve
+// joint_damping<T> (solver/plugin.rs:759-806), on the damping schedule (joint_schedule.hpp).  An end without a SolverBody is the system
+// run's dummy_body1 / dummy_body2 (d.jdummy[2 * type + side]): SolverBody::DUMMY is not kinematic, so delta_omega is written into it and
+// the next such joint of the same type reads it.  Its linear velocity stays zero (0 + p * 0), so only the angular velocity is kept.
 template <class S> __device__ void damp_joint_item(const DevSolver<S>& d, int slot) {
     const size_t JP = size_t(d.Jpad);
     const Vec4<S>* j = d.jnt + slot;
@@ -320,9 +322,10 @@ template <class S> __device__ void damp_joint_item(const DevSolver<S>& d, int sl
     Vec4<S> i1a = ld4(&d.inr[2 * b1]), i2a = ld4(&d.inr[2 * b2]);
     int f1 = as_int(i1a.y), f2 = as_int(i2a.y);
     bool real1 = f1 & BF_HAS_SOLVER_BODY, real2 = f2 & BF_HAS_SOLVER_BODY;
+    Vec4<S>* dummy = d.jdummy + 2 * (info & JI_TYPE_MASK);
     // NOTE: joint_damping does not apply the dominance override, only the missing-SolverBody dummy (plugin.rs:773-787)
-    V3<S> v1 = real1 ? xyz(ld4(&d.vel[2 * b1])) : zero3<S>(), w1 = real1 ? xyz(ld4(&d.vel[2 * b1 + 1])) : zero3<S>();
-    V3<S> v2 = real2 ? xyz(ld4(&d.vel[2 * b2])) : zero3<S>(), w2 = real2 ? xyz(ld4(&d.vel[2 * b2 + 1])) : zero3<S>();
+    V3<S> v1 = real1 ? xyz(ld4(&d.vel[2 * b1])) : zero3<S>(), w1 = xyz(real1 ? ld4(&d.vel[2 * b1 + 1]) : ld4(&dummy[0]));
+    V3<S> v2 = real2 ? xyz(ld4(&d.vel[2 * b2])) : zero3<S>(), w2 = xyz(real2 ? ld4(&d.vel[2 * b2 + 1]) : ld4(&dummy[1]));
     BodyInertia<S> in1 = real1 ? unpack_inertia(i1a, ld4(&d.inr[2 * b1 + 1])) : zero_inertia<S>();
     BodyInertia<S> in2 = real2 ? unpack_inertia(i2a, ld4(&d.inr[2 * b2 + 1])) : zero_inertia<S>();
     V3<S> domega = (w2 - w1) * avn_min(dang * d.h, S(1));
@@ -334,7 +337,9 @@ template <class S> __device__ void damp_joint_item(const DevSolver<S>& d, int sl
     v1 = v1 + cmul(p, in1.inv_mass);
     v2 = v2 - cmul(p, in2.inv_mass);
     if (real1) { st4(&d.vel[2 * b1], mk4<S>(v1.x, v1.y, v1.z, S(0))); st4(&d.vel[2 * b1 + 1], mk4<S>(w1.x, w1.y, w1.z, S(0))); }
+    else st4(&dummy[0], mk4<S>(w1.x, w1.y, w1.z, S(0)));
     if (real2) { st4(&d.vel[2 * b2], mk4<S>(v2.x, v2.y, v2.z, S(0))); st4(&d.vel[2 * b2 + 1], mk4<S>(w2.x, w2.y, w2.z, S(0))); }
+    else st4(&dummy[1], mk4<S>(w2.x, w2.y, w2.z, S(0)));
 }
 // writeback_joint_forces (xpbd/plugin.rs:242-260)
 template <class S> __device__ __forceinline__ void joint_force_item(const DevSolver<S>& d, int slot) {

@@ -55,7 +55,7 @@ struct Soft { S bias, mass_scale, impulse_scale; };
 
 template <class S>
 struct DevSolver {
-    int B, M, P, Mpad, J, Jpad, n_levels;
+    int B, M, P, Mpad, J, Jpad, n_levels, n_damp_levels;
     int m_color_off[AVN_GRAPH_COLOR_COUNT + 1];  // manifold index ranges per colour (ABI order)
     int color_off[AVN_GRAPH_COLOR_COUNT + 1];    // SLOT ranges per colour, each start a multiple of 32; [24] = Mpad
     int color_len[AVN_GRAPH_COLOR_COUNT];        // manifolds in the colour
@@ -96,7 +96,10 @@ struct DevSolver {
     const uint8_t* jlimit_en[AVN_JOINT_TYPE_COUNT]; const uint8_t* jdamp_en[AVN_JOINT_TYPE_COUNT];
     const int* jbody1[AVN_JOINT_TYPE_COUNT]; const int* jbody2[AVN_JOINT_TYPE_COUNT];
     S* jforce[AVN_JOINT_TYPE_COUNT]; S* jtorque[AVN_JOINT_TYPE_COUNT];
-    int any_joint_damping;
+    // joint_damping: damping item -> solve-schedule slot, level ranges of the damping items, and the angular velocities of the two dummy
+    // bodies of each joint type's system run (2 * type + side; reset by the velocity projection before each substep's damping pass)
+    const int* jdamp_slot; const int* damp_level_off;
+    Vec4<S>* jdummy;
     // launch range (avn_solver_run_range): which parts of the step this launch runs.  A plain avn_solver_run does everything.
     int do_prepare, sub_begin, sub_end, do_restitution, do_finalize;
     // x-slab partition (multi-GPU, include/avian_b200.h "boundary bodies"): bnd_of[b] = index into the boundary list or -1 (NULL when

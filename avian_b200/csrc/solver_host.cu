@@ -279,10 +279,10 @@ class Solver final : public SolverBase {
     DevBuf m_b1_, m_b2_, m_n_, m_f_, m_r_, m_tv_, m_po_, p_a1_, p_a2_, p_pen_, p_ns_, p_wn_, p_wt_, p_ni_, p_nin_, p_own_, p_owt_;
     DevBuf hot_, c_flag_;
     size_t hot_bytes_ = 0;
-    DevBuf j_type_, j_index_, j_level_, j_planes_;
+    DevBuf j_type_, j_index_, j_level_, j_planes_, j_damp_slot_, j_damp_level_, j_dummy_;
     DevBuf jcol_[AVN_JOINT_TYPE_COUNT][12], jb1_[AVN_JOINT_TYPE_COUNT], jb2_[AVN_JOINT_TYPE_COUNT], jle_[AVN_JOINT_TYPE_COUNT],
         jde_[AVN_JOINT_TYPE_COUNT], jdl_[AVN_JOINT_TYPE_COUNT], jda_[AVN_JOINT_TYPE_COUNT], jfo_[AVN_JOINT_TYPE_COUNT], jto_[AVN_JOINT_TYPE_COUNT];
-    std::vector<int> h_type_, h_index_, h_level_off_;
+    std::vector<int> h_type_, h_index_, h_level_off_, h_damp_slot_, h_damp_level_off_;
 };
 
 template <class S>
@@ -294,11 +294,13 @@ AvnStatus Solver<S>::build_joint_schedule(const AvnBodyColumns& bc, const AvnJoi
     h_type_.swap(sch.type);
     h_index_.swap(sch.index);
     h_level_off_.swap(sch.level_off);
+    h_damp_slot_.swap(sch.damp_slot);
+    h_damp_level_off_.swap(sch.damp_level_off);
     const size_t J = h_type_.size();
     dev_.J = int(J);
     dev_.Jpad = int((J + 31) & ~size_t(31));
     dev_.n_levels = sch.n_levels;
-    dev_.any_joint_damping = sch.any_damping ? 1 : 0;
+    dev_.n_damp_levels = sch.n_damp_levels;
     return AVN_OK;
 }
 
@@ -578,6 +580,10 @@ AvnStatus Solver<S>::upload_impl(const AvnStepParams* prm, AvnBodyColumns* bc, c
             UP(j_type_, h_type_.data(), h_type_.size(), int, j_src_type);
             UP(j_index_, h_index_.data(), h_index_.size(), int, j_src_index);
             UP(j_level_, h_level_off_.data(), h_level_off_.size(), int, level_off);
+            UP(j_damp_slot_, h_damp_slot_.data(), h_damp_slot_.size(), int, jdamp_slot);
+            UP(j_damp_level_, h_damp_level_off_.data(), h_damp_level_off_.size(), int, damp_level_off);
+            AVN_CUDA(j_dummy_.ensure(2 * AVN_JOINT_TYPE_COUNT * sizeof(Vec4<S>)));
+            d.jdummy = j_dummy_.as<Vec4<S>>();
             AVN_CUDA(j_planes_.ensure(size_t(JP_PLANES) * d.Jpad * sizeof(Vec4<S>)));
             d.jnt = j_planes_.as<Vec4<S>>();
             hj_ = *js;
@@ -708,8 +714,8 @@ AvnStatus Solver<S>::launch_range(uint32_t first, uint32_t count, uint32_t flags
             if (d.J > 0) {
                 for (int l = 0; l < d.n_levels; ++l) launch_phase<OP_SOLVE_JOINT>(h_level_off_[l], h_level_off_[l + 1] - h_level_off_[l]);
                 launch_phase<OP_PROJECT_VEL>(0, d.B);
-                if (d.any_joint_damping)
-                    for (int l = 0; l < d.n_levels; ++l) launch_phase<OP_DAMP_JOINT>(h_level_off_[l], h_level_off_[l + 1] - h_level_off_[l]);
+                for (int l = 0; l < d.n_damp_levels; ++l)
+                    launch_phase<OP_DAMP_JOINT>(h_damp_level_off_[l], h_damp_level_off_[l + 1] - h_damp_level_off_[l]);
             }
         }
         if (d.do_finalize) cudaEventRecord(ev_[EV_LOOP], stream_);

@@ -38,8 +38,12 @@ __device__ __forceinline__ void run_item(const DevSolver<S>& d, int i) {
     else if (OP == OP_RELAX) contact_item<S, PASS_RELAX, MAXP>(d, i);
     else if (OP == OP_RESTITUTION) contact_item<S, PASS_RESTITUTION, MAXP>(d, i);
     else if (OP == OP_SOLVE_JOINT) solve_joint_item(d, i);
-    else if (OP == OP_PROJECT_VEL) project_velocity_item(d, i);
-    else if (OP == OP_DAMP_JOINT) damp_joint_item(d, i);
+    else if (OP == OP_PROJECT_VEL) {
+        project_velocity_item(d, i);
+        if (i == 0)   // the damping pass that follows starts with fresh dummy bodies (one per joint type and side)
+            for (int k = 0; k < 2 * AVN_JOINT_TYPE_COUNT; ++k) d.jdummy[k] = Vec4<S>{};
+    }
+    else if (OP == OP_DAMP_JOINT) damp_joint_item(d, d.jdamp_slot[i]);
     else if (OP == OP_WRITEBACK_BODY) writeback_body_item(d, i);
     else if (OP == OP_STORE_IMPULSE) store_impulse_item(d, i);
     else if (OP == OP_JOINT_FORCE) joint_force_item(d, i);
@@ -181,12 +185,10 @@ __global__ void __launch_bounds__(MEGA_BLOCK, BPS) step_megakernel(const __grid_
             }
             grid_phase<S, OP_PROJECT_VEL>(d, 0, d.B);
             grid.sync();
-            if (d.any_joint_damping) {
-                for (int l = 0; l < d.n_levels; ++l) {
-                    const int b = d.level_off[l], n = d.level_off[l + 1] - b;
-                    grid_phase<S, OP_DAMP_JOINT>(d, b, n);
-                    grid.sync();
-                }
+            for (int l = 0; l < d.n_damp_levels; ++l) {
+                const int b = d.damp_level_off[l], n = d.damp_level_off[l + 1] - b;
+                grid_phase<S, OP_DAMP_JOINT>(d, b, n);
+                grid.sync();
             }
         }
     }

@@ -387,10 +387,14 @@ struct StepState {
             if (dr.w < S(0)) nav = -nav;
             sb.angular_velocity += nav;
         }
-        // joint_damping<T> (solver/plugin.rs:759-806)
+        // joint_damping<T> (solver/plugin.rs:759-806).  Each system run (one joint type, one substep) owns one dummy_body1 and one
+        // dummy_body2 for the joint ends without a SolverBody.  The dummy is not kinematic, so delta_omega is written into it and the
+        // next such joint of the run reads it; its linear velocity stays zero (effective inverse mass 0).
+        SolverBody<S> d1, d2;
+        int run_type = -1;
         for (JointData<S>& j : w.joints) {
             if (!j.damping) continue;
-            SolverBody<S> d1, d2;
+            if (j.type != run_type) { d1 = SolverBody<S>(); d2 = SolverBody<S>(); run_type = j.type; }
             SolverBody<S>* b1 = &d1; SolverBody<S>* b2 = &d2;
             const SolverBodyInertia<S>* i1 = &dummy_inertia; const SolverBodyInertia<S>* i2 = &dummy_inertia;
             if (has_sb[j.body1]) { b1 = &w.bodies[j.body1]; i1 = &w.inertias[j.body1]; }

@@ -19,6 +19,8 @@ Scenes (every branch named is hit at least once, checked by the asserts at the b
   locked_on_kinematic a body with LockedAxes (translation X, rotation Y) in contact with a moving kinematic body
   prismatic_slider    prismatic joint beyond its slider limit and off its axis, with a rotation error: fixed-angle constraint, then the limit
                       along the free axis and the two zero limits along glam's any_orthogonal_vector axes
+  damped_static_pair  two damped distance joints, each from a different static body to a spinning body: joint_damping's dummy_body1 carries
+                      the first joint's angular increment into the second
   sap_six             six intervals swept by hand (ties on min.x with -0.0/+0.0, touching y bounds, same body, layer mismatch, both inactive)
 """
 import json
@@ -142,6 +144,19 @@ SCENES["prismatic_slider"] = {      # slid 0.5 along the free axis against a [-0
                     inv_inertia=(9.0, 0, 0, 9.0, 0, 9.0))],
     "joints": [{"type": W.PRISMATIC, "body1": 0, "body2": 1, "local_anchor1": [0.1, 0, 0], "local_anchor2": [-0.1, 0, 0], "axis": [1, 0, 0],
                 "limits": [-0.2, 0.3], "compliance0": 0.0, "compliance1": 1e-5}],
+}
+
+SCENES["damped_static_pair"] = {    # two damped distance joints, each hanging a spinning body from a DIFFERENT static body: joint_damping's
+    "params": params(2),            # dummy_body1 takes the first joint's delta_omega and hands it to the second (one dummy per type and substep)
+    "bodies": [body(W.STATIC, (0, 2, 0), inv_mass=0.0, inv_inertia=(0,) * 6),
+               body(W.DYNAMIC, (0.9, 2, 0.1), w=(0.5, 2.0, -1.0), inv_mass=1.0, inv_inertia=(4.0, 0, 0, 4.0, 0, 4.0)),
+               body(W.DYNAMIC, (3.1, 1.2, 0), rot=axis_angle((0, 1, 1), 0.4), v=(0, 0.2, 0), w=(-1.5, 0.3, 2.5), inv_mass=0.5,
+                    inv_inertia=(3.0, 0, 0, 3.0, 0, 3.0)),
+               body(W.STATIC, (3, 2, 0), rot=axis_angle((1, 0, 0), 0.3), inv_mass=0.0, inv_inertia=(0,) * 6)],
+    "joints": [{"type": W.DISTANCE, "body1": 0, "body2": 1, "local_anchor1": [0, 0, 0], "local_anchor2": [-0.4, 0, 0], "limit_min": 0.5,
+                "limit_max": 0.5, "compliance0": 0.0, "damping": [0.5, 3.0]},
+               {"type": W.DISTANCE, "body1": 3, "body2": 2, "local_anchor1": [0, -0.2, 0], "local_anchor2": [0, 0.3, 0], "limit_min": 0.2,
+                "limit_max": 0.4, "compliance0": 0.0, "damping": [1.0, 4.0]}],
 }
 
 kp = []

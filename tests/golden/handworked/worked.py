@@ -696,11 +696,16 @@ def step(scene, dtype=np.float32, quat_product="scalar"):
                     nw = -nw
                 b["w"] = b["w"] + nw
             for jt in (FIXED, REVOLUTE, SPHERICAL, PRISMATIC, DISTANCE):   # joint_damping::<T> (solver/plugin.rs:759-806), same order
+                # one dummy_body1 / dummy_body2 per system run (plugin.rs:766-767), i.e. per joint type and substep, shared by every joint
+                # of that run whose end has no SolverBody.  SolverBody::DUMMY has empty flags (not kinematic), so the angular part writes
+                # into it and the next such joint reads that velocity; the linear part adds p * 0 and leaves it at zero.
+                dummies = (body(-1), body(-1))
                 for j in J:
                     if j["type"] != jt or j.get("damping") is None:
                         continue
                     i1, i2 = j["body1"], j["body2"]
-                    jb1, jb2 = body(i1), body(i2)
+                    jb1 = B[i1] if B[i1]["has_solver_body"] else dummies[0]
+                    jb2 = B[i2] if B[i2]["has_solver_body"] else dummies[1]
                     dl, da = T(j["damping"][0]), T(j["damping"][1])
                     d_omega = (jb2["w"] - jb1["w"]) * min(da * h, T(1))
                     if jb1["kind"] != KINEMATIC:
