@@ -399,6 +399,22 @@ class AvnPointProjection(C.Structure):
     _fields_ = [(n, _vp) for n in ("collider", "point", "is_inside")]
 
 
+class AvnMoveConfig(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("delta_time", "length_unit", "skin_width", "max_depenetration_error", "penetration_rejection_threshold",
+                                          "plane_similarity_dot_threshold")] + [
+        (n, C.c_uint32) for n in ("move_and_slide_iterations", "depenetration_iterations", "max_planes", "collider_count")] + [("ignored", _vp)]
+
+
+class AvnMoveBatch(C.Structure):
+    _fields_ = [("count", C.c_uint32), ("exclude_count", C.c_uint32)] + [
+        (n, _vp) for n in ("shape", "dims", "position", "rotation", "velocity", "mask", "exclude_offsets", "exclude", "plane_offsets", "planes")]
+
+
+class AvnMoveResult(C.Structure):
+    _fields_ = [(n, _vp) for n in ("position", "velocity", "hit_collider", "hit_distance", "hit_toi", "hit_point", "hit_normal")] + [
+        ("kernel_ms", C.c_float), ("_pad", C.c_uint32)]
+
+
 class AvnCollisionEvents(C.Structure):
     _fields_ = [("capacity", C.c_uint64), ("count", C.c_uint64)] + [(n, _vp) for n in ("collider1", "collider2", "body1", "body2", "flags")]
 
@@ -502,6 +518,7 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "contacts_remove_colliders": ([_vp, C.c_uint32, _vp], C.c_int),
         "contacts_events": ([_vp, P(AvnCollisionEvents), P(AvnCollisionEvents)], C.c_int),
         "contacts_report": ([_vp, C.c_uint32, P(AvnContactReport)], C.c_int),
+        "move_and_slide": ([_vp, P(AvnMoveConfig), P(AvnMoveBatch), P(AvnMoveResult)], C.c_int),
     }
     for name, (argtypes, restype) in sig.items():
         fn = getattr(lib, f"{prefix}_{name}")
@@ -519,7 +536,8 @@ ABI_SYMBOLS = [
     "avn_solver_prefetch_bodies", "avn_islands_configure", "avn_islands_step", "avn_query_update", "avn_query_cast_ray", "avn_query_ray_hits",
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
     "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download", "avn_contacts_set_sensors", "avn_contacts_remove_colliders",
-    "avn_contacts_events", "avn_contacts_report", "avn_islands_apply", "avn_islands_wake", "avn_contacts_download_sleeping"]
+    "avn_contacts_events", "avn_contacts_report", "avn_islands_apply", "avn_islands_wake", "avn_contacts_download_sleeping",
+    "avn_move_and_slide"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -676,6 +694,88 @@ class Points:
             st.exclude_offsets = xoff.ctypes.data
             st.exclude = xs.ctypes.data if xs.size else None
         return st, keep
+
+
+MOVE_MAX_PLANES = 32
+COS_5_DEGREES = 0.99619469809
+
+
+@dataclass
+class MoveConfig:
+    """MoveAndSlideConfig (AvnMoveConfig), the reference's defaults.  ignored: uint8[C] per collider of the tree, nonzero = not an obstacle
+    (sensors, colliders without a body); None = every collider is one."""
+    delta_time: float = 1.0 / 60.0
+    length_unit: float = 1.0
+    skin_width: float = 0.01
+    max_depenetration_error: float = 0.0001
+    penetration_rejection_threshold: float = 0.5
+    plane_similarity_dot_threshold: float = COS_5_DEGREES
+    move_and_slide_iterations: int = 4
+    depenetration_iterations: int = 16
+    max_planes: int = 20
+    ignored: np.ndarray | None = None
+    collider_count: int | None = None      # None = len(ignored)
+
+    def as_struct(self) -> tuple["AvnMoveConfig", list]:
+        ig = None if self.ignored is None else np.ascontiguousarray(self.ignored, dtype=np.uint8)
+        cc = self.collider_count if self.collider_count is not None else (0 if ig is None else int(ig.shape[0]))
+        st = AvnMoveConfig(float(self.delta_time), float(self.length_unit), float(self.skin_width), float(self.max_depenetration_error),
+                           float(self.penetration_rejection_threshold), float(self.plane_similarity_dot_threshold), int(self.move_and_slide_iterations),
+                           int(self.depenetration_iterations), int(self.max_planes), int(cc), _ptr(ig))
+        return st, [ig]
+
+
+@dataclass
+class MoveBatch:
+    """Characters of one avn_move_and_slide call (AvnMoveBatch).  exclude: per character an iterable of collider indices it ignores (its own
+    collider, as the reference's docs tell users to); planes: per character an array [k,3] of initial planes (MoveAndSlideConfig::planes),
+    or None."""
+    shape: np.ndarray                        # uint8[n] SHAPE_CUBOID / SHAPE_SPHERE
+    dims: np.ndarray                         # [n,3] half extents / radius in [0]
+    position: np.ndarray                     # [n,3]
+    rotation: np.ndarray                     # [n,4] (x, y, z, w)
+    velocity: np.ndarray                     # [n,3] desired velocity
+    mask: np.ndarray | None = None           # uint32[n] (None = all layers)
+    exclude: list | None = None
+    planes: list | None = None
+
+    @property
+    def count(self) -> int:
+        return int(np.asarray(self.position).reshape(-1, 3).shape[0])
+
+    def as_struct(self, scalar) -> tuple["AvnMoveBatch", list]:
+        dt, n = np.dtype(scalar), self.count
+        col = lambda a, w: np.ascontiguousarray(a, dtype=dt).reshape(-1, w)
+        opt = lambda a, t: None if a is None else np.ascontiguousarray(a, dtype=t)
+        xoff, xs = _exclusion_csr(self.exclude, n)
+        poff = pl = None
+        if self.planes is not None:
+            lists = [np.zeros((0, 3)) if p is None else np.asarray(p, dtype=np.float64).reshape(-1, 3) for p in self.planes]
+            poff = np.zeros(n + 1, dtype=np.uint32)
+            poff[1:] = np.cumsum([len(p) for p in lists])
+            pl = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros((0, 3)), dtype=dt).reshape(-1, 3)
+        keep = [opt(self.shape, np.uint8), col(self.dims, 3), col(self.position, 3), col(self.rotation, 4), col(self.velocity, 3),
+                opt(self.mask, np.uint32), xoff, xs, poff, pl]
+        st = AvnMoveBatch(n, 0 if xs is None else int(xs.shape[0]), *(_ptr(a) if a is None or a.size else None for a in keep))
+        if xoff is not None:
+            st.exclude_offsets = xoff.ctypes.data
+            st.exclude = xs.ctypes.data if xs.size else None
+        if poff is not None:
+            st.plane_offsets = poff.ctypes.data
+        return st, keep
+
+
+MOVE_HIT_FIELDS = ("hit_collider", "hit_distance", "hit_toi", "hit_point", "hit_normal")
+
+
+def move_result(n: int, iterations: int, scalar) -> tuple["AvnMoveResult", dict]:
+    """An AvnMoveResult over fresh numpy arrays: position, velocity [n,3]; hit_collider, hit_distance, hit_toi [n,iterations];
+    hit_point, hit_normal [n,iterations,3]."""
+    it = int(iterations)
+    out = {"position": np.zeros((n, 3), dtype=scalar), "velocity": np.zeros((n, 3), dtype=scalar), "hit_collider": np.zeros((n, it), dtype=np.int32),
+           "hit_distance": np.zeros((n, it), dtype=scalar), "hit_toi": np.zeros((n, it), dtype=scalar),
+           "hit_point": np.zeros((n, it, 3), dtype=scalar), "hit_normal": np.zeros((n, it, 3), dtype=scalar)}
+    return AvnMoveResult(*(_ptr(out[k]) if out[k].size else None for k in ("position", "velocity") + MOVE_HIT_FIELDS), 0.0, 0), out
 
 
 SHAPE_HIT_FIELDS = ("point1", "point2", "normal1", "normal2")
@@ -1220,6 +1320,16 @@ class Context:
             st = self.lib.avn_query_point_intersections(self.handle, C.byref(p), C.byref(h))
         self._check_list(st, h)
         return hit_list_result(h, out)
+
+    def move_and_slide(self, config: "MoveConfig", batch: "MoveBatch") -> dict:
+        """avn_move_and_slide against the tree of the last query_update: position, velocity (MoveAndSlideOutput), per iteration the sweep
+        hit (hit_collider -1 = none, hit_distance = safe distance, hit_toi, hit_point, hit_normal) and kernel_ms."""
+        c, keep_c = config.as_struct()
+        b, keep_b = batch.as_struct(self.scalar)
+        o, out = move_result(batch.count, config.move_and_slide_iterations, self.scalar)
+        self._check(self.lib.avn_move_and_slide(self.handle, C.byref(c), C.byref(b), C.byref(o)))
+        out["kernel_ms"] = float(o.kernel_ms)
+        return out
 
     def shape_intersections(self, shapes: "ShapeQueries", capacity: int | None = None) -> dict:
         """avn_query_shape_intersections: per query shape the colliders it intersects (CSR offsets[n+1], collider ascending)."""

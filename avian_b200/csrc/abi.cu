@@ -339,6 +339,10 @@ AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* po
 AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out) {
     return guarded(ctx, [&] { return ctx->queries->shape_intersections(shapes, out); });
 }
+// MoveAndSlide::move_and_slide against the query tree
+AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const AvnMoveBatch* batch, AvnMoveResult* out) {
+    return guarded(ctx, [&] { return ctx->queries->move_and_slide(config, batch, out); });
+}
 
 // swept CCD (ccd.cu): solve_swept_ccd inside avn_solver_run
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {

@@ -138,6 +138,7 @@ struct QueriesBase {
     virtual AvnStatus project_point(const AvnPointBatch* points, AvnPointProjection* out) = 0;
     virtual AvnStatus point_intersections(const AvnPointBatch* points, AvnHitList* out) = 0;
     virtual AvnStatus shape_intersections(const AvnShapeBatch* shapes, AvnHitList* out) = 0;
+    virtual AvnStatus move_and_slide(const AvnMoveConfig* config, const AvnMoveBatch* batch, AvnMoveResult* out) = 0;
 };
 QueriesBase* make_queries(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 

@@ -18,6 +18,7 @@
 // Shape casts (pipeline.rs:335-554) cull against the node boxes grown by the cast shape's AABB half size, nearer child first for the closest
 // hit; project_point (570-615) prunes on the squared point-box distance; point and shape intersections (628-683, 744-826) use the same CSR
 // pattern.  Their geometry is the shape-cast part of query_math.hpp.
+// Move and slide (character_controller/move_and_slide.rs): q_move runs csrc/move_math.hpp's loop per character over this tree (TreeScene).
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -27,6 +28,7 @@
 #include "context.hpp"
 #include "device_prims.cuh"
 #include "query_math.hpp"
+#include "move_math.hpp"
 
 namespace avn {
 namespace {
@@ -674,6 +676,142 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant
     sort_segment(w, [&](uint32_t x, uint32_t y) { return seg[x] < seg[y]; }, [&](uint32_t x, uint32_t y) { const uint32_t v = seg[x]; seg[x] = seg[y]; seg[y] = v; });
 }
 
+// ---- move and slide (csrc/move_math.hpp): one thread per character runs the whole loop against the tree ------------------------------
+template <class S>
+struct Movers {
+    int n;
+    const uint8_t* shape; const S* dims; const S* pos; const S* rot; const S* vel;
+    const uint32_t* mask; const uint32_t* xoff; const uint32_t* xs; const uint32_t* poff; const S* planes;
+    const uint8_t* ignored;                          // [tree n] or NULL
+};
+
+// the cast leaf of a move, out of line: the shape-cast geometry is instanced once in the move kernel, not at each inlined call site
+template <class S>
+__device__ __noinline__ bool move_cast_leaf(const Tree<S>& t, uint32_t c, int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& th, int& axis) {
+    return qm::cast_collider(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+}
+
+// the scene of move_math.hpp over the tree, with one character's filter
+template <class S>
+struct TreeScene {
+    const Tree<S>& t;
+    int m;
+    uint32_t mask, nx;
+    const uint32_t* xs;
+    const uint8_t* ignored;
+
+    __device__ bool pass(uint32_t c) const {
+        const uint32_t memb = t.memb ? t.memb[c] : 1u;
+        return qm::passes_filter(memb, mask, xs, nx, c) && !(ignored && ignored[c]);
+    }
+    __device__ void collider(uint32_t c, int& s, nm::V3& he, nm::V3& p, nm::Q& q) const {
+        s = t.shape[c]; he = ld3(t.dims, c); p = ld3(t.pos, c); q = ldq(t.rot, c);
+    }
+    // the closest filtered cast: nearest-first over the node boxes grown by the shape's half size (as q_cast_shape)
+    __device__ bool cast(int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& t_out, uint32_t& c_out, int& axis_out) const {
+        float ext[3];
+        const nm::V3 e = qm::half_size(shape, he, qm::rot_mat(q));
+        for (int k = 0; k < 3; ++k) {
+            float l;
+            qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, ext[k]);
+        }
+        double best_t = INFINITY;
+        uint32_t best_c = 0xffffffffu;
+        int best_axis = -1;
+        traverse_nearest<true>(t, m, best_t, [&](const NodeBox& b) { return grown_entry(b, ext, ctr, d, maxd); },
+                               [&](uint32_t c) {
+                                   if (!pass(c)) return;
+                                   double th;
+                                   int ax;
+                                   if (move_cast_leaf(t, c, shape, he, ctr, q, d, maxd, th, ax) && qm::hit_before(th, c, best_t, best_c)) {
+                                       best_t = th; best_c = c; best_axis = ax;
+                                   }
+                               });
+        if (best_c == 0xffffffffu) return false;
+        t_out = best_t; c_out = best_c; axis_out = best_axis;
+        return true;
+    }
+    // fn(collider) in ascending index: each walk keeps the MOVE_WINDOW smallest passing indices above the last one handled, in a sorted
+    // window, and notes whether it had to leave any out; the window is handled outside the walk, and the next walk starts above it
+    template <class F>
+    __device__ void candidates(const S lo[3], const S hi[3], F fn) const {
+        const double lod[3] = {double(lo[0]), double(lo[1]), double(lo[2])}, hid[3] = {double(hi[0]), double(hi[1]), double(hi[2])};
+        uint32_t after = 0;
+        bool first = true;
+        for (;;) {
+            uint32_t win[mv::MOVE_WINDOW];
+            int nw = 0;
+            bool more = false;
+            traverse(t, m,
+                     [&](const NodeBox& nb) {
+                         const double blo[3] = {nb.lo.x, nb.lo.y, nb.lo.z}, bhi[3] = {nb.hi.x, nb.hi.y, nb.hi.z};
+                         return qm::aabb_overlap(lod, hid, blo, bhi);
+                     },
+                     [&](uint32_t c) {
+                         if (!first && c <= after) return;
+                         if (nw == mv::MOVE_WINDOW && c > win[nw - 1]) { more = true; return; }
+                         if (!qm::aabb_overlap(lo, hi, t.tmn + 3 * size_t(c), t.tmx + 3 * size_t(c)) || !pass(c)) return;
+                         if (nw == mv::MOVE_WINDOW) { more = true; --nw; }
+                         int j = nw++;
+                         for (; j > 0 && win[j - 1] > c; --j) win[j] = win[j - 1];
+                         win[j] = c;
+                     });
+NM_ROLLED
+            for (int k = 0; k < nw; ++k) fn(win[k]);
+            if (!more || nw == 0) return;
+            after = win[nw - 1];
+            first = false;
+        }
+    }
+};
+
+template <class S>
+struct MoveHits {
+    int32_t* c; S* d; S* t; S* p; S* n;
+    size_t base;
+    __device__ void sweep(uint32_t it, uint32_t col, S safe, S toi, mv::T3<S> p1, mv::T3<S> n1) {
+        const size_t o = base + it;
+        if (c) c[o] = int32_t(col);
+        if (d) d[o] = safe;
+        if (t) t[o] = toi;
+        if (p) { p[3 * o] = p1.x; p[3 * o + 1] = p1.y; p[3 * o + 2] = p1.z; }
+        if (n) { n[3 * o] = n1.x; n[3 * o + 1] = n1.y; n[3 * o + 2] = n1.z; }
+    }
+};
+
+template <class S>
+__global__ void __launch_bounds__(Q_THREADS) q_move(const __grid_constant__ Tree<S> t, const __grid_constant__ Movers<S> mb, const __grid_constant__ mv::Config<S> cfg,
+                                                     S* __restrict__ out_pos, S* __restrict__ out_vel, int32_t* __restrict__ hc, S* __restrict__ hd,
+                                                     S* __restrict__ ht, S* __restrict__ hp, S* __restrict__ hn) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= mb.n) return;
+    MoveHits<S> hits{hc, hd, ht, hp, hn, size_t(i) * cfg.iterations};
+    for (uint32_t it = 0; it < cfg.iterations; ++it) {
+        const size_t o = hits.base + it;
+        if (hc) hc[o] = -1;
+        if (hd) hd[o] = S(0);
+        if (ht) ht[o] = S(0);
+        for (int k = 0; k < 3; ++k) {
+            if (hp) hp[3 * o + k] = S(0);
+            if (hn) hn[3 * o + k] = S(0);
+        }
+    }
+    const mv::Body b{int(mb.shape[i]), ld3(mb.dims, i), ldq(mb.rot, i)};
+    mv::T3<S> pos{mb.pos[3 * i], mb.pos[3 * i + 1], mb.pos[3 * i + 2]}, vel{mb.vel[3 * i], mb.vel[3 * i + 1], mb.vel[3 * i + 2]};
+    if (qm::collider_valid(b.he, mv::to_v3(pos), b.q) && qm::finite3(mv::to_v3(vel))) {
+        mv::T3<float> init[mv::MAX_PLANES];
+        int ni = 0;
+        if (mb.poff)
+            for (uint32_t k = mb.poff[i]; k < mb.poff[i + 1]; ++k)
+                init[ni++] = mv::plane_dir(mv::T3<S>{mb.planes[3 * k], mb.planes[3 * k + 1], mb.planes[3 * k + 2]});
+        const TreeScene<S> sc{t, *t.m, mb.mask ? mb.mask[i] : 0xffffffffu, mb.xoff ? mb.xoff[i + 1] - mb.xoff[i] : 0u,
+                              mb.xoff ? mb.xs + mb.xoff[i] : nullptr, mb.ignored};
+        mv::move_and_slide(sc, cfg, b, pos, vel, init, ni, hits);
+    }
+    out_pos[3 * i] = pos.x; out_pos[3 * i + 1] = pos.y; out_pos[3 * i + 2] = pos.z;
+    out_vel[3 * i] = vel.x; out_vel[3 * i + 1] = vel.y; out_vel[3 * i + 2] = vel.z;
+}
+
 template <class S>
 class Queries final : public QueriesBase {
    public:
@@ -948,6 +1086,68 @@ class Queries final : public QueriesBase {
         });
     }
 
+    AvnStatus move_and_slide(const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) override {
+        if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide before any avn_query_update");
+        if (const char* why = mv::check_move(cfg, b, sizeof(S) == 8, uint32_t(n_))) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: %s", why);
+        if (!out || (b->count && (!out->position || !out->velocity)))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: position and velocity outputs are required");
+        out->kernel_ms = 0.f;
+        const size_t n = b->count;
+        if (n == 0) return AVN_OK;
+        Movers<S> mb{};
+        mb.n = int(n);
+        AvnStatus st;
+#define UPM(buf, host, cnt, T, dst) if ((st = up<T>(buf, host, cnt, &dst)) != AVN_OK) return st
+        UPM(s_shape_, b->shape, n, uint8_t, mb.shape);
+        UPM(s_dims_, b->dims, 3 * n, S, mb.dims);
+        UPM(s_pos_, b->position, 3 * n, S, mb.pos);
+        UPM(s_rot_, b->rotation, 4 * n, S, mb.rot);
+        UPM(s_d_, b->velocity, 3 * n, S, mb.vel);
+        UPM(s_mask_, b->mask, n, uint32_t, mb.mask);
+        UPM(s_xoff_, b->exclude_offsets, n + 1, uint32_t, mb.xoff);
+        if (b->exclude_offsets) UPM(s_xs_, b->exclude_count ? b->exclude : nullptr, b->exclude_count, uint32_t, mb.xs);
+        UPM(m_poff_, b->plane_offsets, n + 1, uint32_t, mb.poff);
+        if (b->plane_offsets) UPM(m_planes_, b->planes, 3 * size_t(b->plane_offsets[n]), S, mb.planes);
+        UPM(m_ignored_, cfg->ignored, size_t(n_), uint8_t, mb.ignored);
+#undef UPM
+        const size_t nh = n * cfg->move_and_slide_iterations;
+        AVN_CUDA(op1_.ensure(3 * n * sizeof(S)));
+        AVN_CUDA(op2_.ensure(3 * n * sizeof(S)));
+        int32_t* hc = nullptr;
+        S *hd = nullptr, *ht = nullptr, *hp = nullptr, *hn = nullptr;
+        if (nh) {
+            if (out->hit_collider) { AVN_CUDA(oc_.ensure(nh * 4)); hc = oc_.as<int32_t>(); }
+            if (out->hit_distance) { AVN_CUDA(ot_.ensure(nh * sizeof(S))); hd = ot_.as<S>(); }
+            if (out->hit_toi) { AVN_CUDA(m_toi_.ensure(nh * sizeof(S))); ht = m_toi_.as<S>(); }
+            if (out->hit_point) { AVN_CUDA(on1_.ensure(3 * nh * sizeof(S))); hp = on1_.as<S>(); }
+            if (out->hit_normal) { AVN_CUDA(on2_.ensure(3 * nh * sizeof(S))); hn = on2_.as<S>(); }
+        }
+        if (!ev_[0]) {
+            AVN_CUDA(cudaEventCreate(&ev_[0]));
+            AVN_CUDA(cudaEventCreate(&ev_[1]));
+        }
+        AVN_CUDA(cudaEventRecord(ev_[0], stream_));
+        q_move<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), mb, mv::config_of<S>(cfg), op1_.as<S>(), op2_.as<S>(), hc, hd, ht,
+                                                                                       hp, hn);
+        AVN_CUDA(cudaGetLastError());
+        AVN_CUDA(cudaEventRecord(ev_[1], stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->position, op1_.p, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaMemcpyAsync(out->velocity, op2_.p, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        if (hc) AVN_CUDA(cudaMemcpyAsync(out->hit_collider, hc, nh * 4, cudaMemcpyDeviceToHost, stream_));
+        if (hd) AVN_CUDA(cudaMemcpyAsync(out->hit_distance, hd, nh * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        if (ht) AVN_CUDA(cudaMemcpyAsync(out->hit_toi, ht, nh * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        if (hp) AVN_CUDA(cudaMemcpyAsync(out->hit_point, hp, 3 * nh * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        if (hn) AVN_CUDA(cudaMemcpyAsync(out->hit_normal, hn, 3 * nh * sizeof(S), cudaMemcpyDeviceToHost, stream_));
+        AVN_CUDA(cudaStreamSynchronize(stream_));
+        AVN_CUDA(cudaEventElapsedTime(&out->kernel_ms, ev_[0], ev_[1]));
+        return AVN_OK;
+    }
+
+    ~Queries() override {
+        for (cudaEvent_t e : ev_)
+            if (e) cudaEventDestroy(e);
+    }
+
    private:
     // count -> scan -> (capacity check) -> emit of a collider-only CSR list; launch(t, grid, counts, nullptr, nullptr) counts,
     // launch(t, grid, nullptr, offsets, out) emits
@@ -1101,6 +1301,8 @@ class Queries final : public QueriesBase {
     DevBuf pos_, rot_, shape_, dims_, memb_, tmn_, tmx_, cbox_, centre_, valid_, k0_, k1_, v0_, v1_, hist_, nodes_, child_, parent_, arrived_, meta_;
     DevBuf r_o_, r_d_, r_maxd_, r_solid_, r_mh_, r_mask_, r_xoff_, r_xs_;
     DevBuf full_, kept_, full_off_, kept_off_, block_sums_, tmp_t_, tmp_c_, oc_, ot_, on_, qmn_, qmx_;
+    DevBuf m_poff_, m_planes_, m_ignored_, m_toi_;
+    cudaEvent_t ev_[2] = {nullptr, nullptr};
 };
 
 }  // namespace

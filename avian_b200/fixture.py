@@ -75,6 +75,12 @@ def _load():
         for f in (lib.avh_query_cast_ray, lib.avh_query_ray_hits, lib.avh_query_aabb_intersections, lib.avh_query_cast_shape, lib.avh_query_shape_hits,
                   lib.avh_query_project_point, lib.avh_query_point_intersections, lib.avh_query_shape_intersections):
             f.restype = C.c_int
+        lib.avh_move_and_slide.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnMoveConfig), P(api.AvnMoveBatch), P(api.AvnMoveResult)]
+        lib.avh_move_and_slide.restype = C.c_int
+        lib.avh_move_project_velocity.argtypes = [C.c_uint32, _vp, _vp, C.c_uint32, _vp]
+        lib.avh_move_project_velocity.restype = None
+        lib.avh_move_contact.argtypes = [C.c_uint32, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_double, _vp, _vp]
+        lib.avh_move_contact.restype = C.c_int
         lib.avh_ccd_solve.argtypes = [C.c_uint32, C.c_double, C.c_double, C.c_uint32] + [_vp] * 10 + [C.c_uint32] + [_vp] * 5 + [P(api.AvnCcdConfig)] + [_vp] * 5
         lib.avh_ccd_solve.restype = C.c_int
         lib.avh_ccd_pair_toi.argtypes = [C.c_uint32, C.c_int, _vp, _vp, C.c_double, C.c_double, C.c_double]
@@ -220,6 +226,40 @@ def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "
 def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
     """Per query shape the colliders it intersects, ascending (same output as Context.shape_intersections)."""
     return _query_list("avh_query_shape_intersections", scalar, colliders, shapes)
+
+
+# ---- move and slide by brute force over every collider (csrc/move_math.hpp): what the device kernel must reproduce bit for bit
+def move_and_slide(scalar, colliders: "api.QueryColliders", config: "api.MoveConfig", batch: "api.MoveBatch") -> dict:
+    """MoveAndSlide::move_and_slide for every character (same output as Context.move_and_slide; kernel_ms is 0)."""
+    lib, dt = _load(), np.dtype(scalar)
+    c, keep_c = colliders.as_struct(dt)
+    m, keep_m = config.as_struct()
+    b, keep_b = batch.as_struct(dt)
+    o, out = api.move_result(batch.count, config.move_and_slide_iterations, dt)
+    _query_check(lib, lib.avh_move_and_slide(32 if dt == np.float32 else 64, C.byref(c), C.byref(m), C.byref(b), C.byref(o)))
+    out["kernel_ms"] = 0.0
+    return out
+
+
+def project_velocity(scalar, v, normals) -> np.ndarray:
+    """The shared project_velocity (velocity_project.rs:122-324) on one velocity; normals are rounded to f32 (Dir)."""
+    lib, dt = _load(), np.dtype(scalar)
+    x = np.ascontiguousarray(v, dtype=dt).reshape(3)
+    ns = np.ascontiguousarray(normals, dtype=np.float32).reshape(-1, 3)
+    out = np.zeros(3, dtype=dt)
+    lib.avh_move_project_velocity(32 if dt == np.float32 else 64, _p(x), _p(ns) if ns.size else None, int(ns.shape[0]), _p(out))
+    return out
+
+
+def move_contact(scalar, shape_a: int, dims_a, pos_a, rot_a, shape_b: int, dims_b, pos_b, rot_b, prediction: float):
+    """One intersection of a move: (f32 plane normal, deepest penetration) of character a against collider b, or None."""
+    lib = _load()
+    d = lambda a, k: np.ascontiguousarray(a, dtype=np.float64).reshape(k)
+    cols = [d(dims_a, 3), d(pos_a, 3), d(rot_a, 4), d(dims_b, 3), d(pos_b, 3), d(rot_b, 4)]
+    n, pen = np.zeros(3, dtype=np.float32), np.zeros(1, dtype=np.float64)
+    hit = lib.avh_move_contact(32 if np.dtype(scalar) == np.float32 else 64, int(shape_a), _p(cols[0]), _p(cols[1]), _p(cols[2]), int(shape_b),
+                               _p(cols[3]), _p(cols[4]), _p(cols[5]), float(prediction), _p(n), _p(pen))
+    return (n, float(pen[0])) if hit else None
 
 
 class HostPipeline:

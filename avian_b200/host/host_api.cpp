@@ -10,6 +10,7 @@
 //   * export of the manifolds as per-colour columns in the layout of AvnManifoldColumns.
 //   * spatial queries by brute force over every collider (csrc/query_math.hpp): the checker of the device tree (csrc/queries.cu).
 //   * swept CCD as the reference's sequential loop (csrc/ccd_math.hpp): the checker of the device pass (csrc/ccd.cu).
+//   * move and slide by brute force over every collider (csrc/move_math.hpp): the checker of the move kernel (csrc/queries.cu).
 // It contains no solver or broad-phase code: those are the GPU library (product) or oracle/ (tests).
 #include <algorithm>
 #include <cmath>
@@ -25,6 +26,7 @@
 #include "../csrc/contact_rows.hpp"
 #include "../csrc/query_math.hpp"
 #include "../csrc/ccd_math.hpp"
+#include "../csrc/move_math.hpp"
 
 namespace {
 
@@ -1020,6 +1022,155 @@ int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders*
                 per[i].push_back(col);
     }
     return write_list(out, per);
+}
+
+}  // extern "C"
+
+// ---- move and slide, brute force over every collider (the checker of q_move in csrc/queries.cu; same header, csrc/move_math.hpp) ------
+namespace {
+template <class T>
+struct HostMoveScene {
+    const QueryScene& sc;
+    const uint8_t* valid; const T* tmn; const T* tmx;   // per collider: in the scene, tight AABB rounded to T
+    uint32_t mask, nx;
+    const uint32_t* xs;
+    const uint8_t* ignored;
+
+    bool pass(uint32_t c) const { return qm::passes_filter(sc.memb(c), mask, xs, nx, c) && !(ignored && ignored[c]); }
+    void collider(uint32_t c, int& s, V3& he, V3& p, Q& q) const { s = sc.c->shape[c]; he = sc.dims.v3(c); p = sc.pos.v3(c); q = sc.rot.q(c); }
+    bool cast(int shape, V3 he, V3 ctr, Q q, V3 d, double maxd, double& t_out, uint32_t& c_out, int& axis_out) const {
+        double best_t = INFINITY;
+        uint32_t best_c = 0xffffffffu;
+        int best_axis = -1;
+        for (uint32_t c = 0; c < sc.c->count; ++c) {
+            if (!valid[c] || !pass(c)) continue;
+            double th;
+            int ax;
+            if (qm::cast_collider(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), th, ax) &&
+                qm::hit_before(th, c, best_t, best_c)) {
+                best_t = th; best_c = c; best_axis = ax;
+            }
+        }
+        if (best_c == 0xffffffffu) return false;
+        t_out = best_t; c_out = best_c; axis_out = best_axis;
+        return true;
+    }
+    template <class F>
+    void candidates(const T lo[3], const T hi[3], F fn) const {
+        for (uint32_t c = 0; c < sc.c->count; ++c)
+            if (valid[c] && qm::aabb_overlap(lo, hi, tmn + 3 * size_t(c), tmx + 3 * size_t(c)) && pass(c)) fn(c);
+    }
+};
+
+template <class T>
+struct HostMoveHits {
+    int32_t* c; void* d; void* t; void* p; void* n;
+    size_t base;
+    void sweep(uint32_t it, uint32_t col, T safe, T toi, mv::T3<T> p1, mv::T3<T> n1) {
+        const size_t o = base + it;
+        if (c) c[o] = int32_t(col);
+        if (d) static_cast<T*>(d)[o] = safe;
+        if (t) static_cast<T*>(t)[o] = toi;
+        if (p) { T* q = static_cast<T*>(p) + 3 * o; q[0] = p1.x; q[1] = p1.y; q[2] = p1.z; }
+        if (n) { T* q = static_cast<T*>(n) + 3 * o; q[0] = n1.x; q[1] = n1.y; q[2] = n1.z; }
+    }
+};
+
+template <class T>
+void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) {
+    const QueryScene sc(c, sizeof(T) == 8);
+    const uint32_t C = c->count;
+    std::vector<uint8_t> valid(C);
+    std::vector<T> tmn(3 * size_t(C)), tmx(3 * size_t(C));
+    for (uint32_t k = 0; k < C; ++k) {
+        valid[k] = sc.valid(k);
+        if (!valid[k]) continue;
+        V3 a, e;
+        qm::collider_aabb(c->shape[k], sc.dims.v3(k), sc.pos.v3(k), sc.rot.q(k), a, e);
+        tmn[3 * k] = T(a.x); tmn[3 * k + 1] = T(a.y); tmn[3 * k + 2] = T(a.z);
+        tmx[3 * k] = T(e.x); tmx[3 * k + 1] = T(e.y); tmx[3 * k + 2] = T(e.z);
+    }
+    const mv::Config<T> mc = mv::config_of<T>(cfg);
+    const T* dims = static_cast<const T*>(b->dims);
+    const T* pos = static_cast<const T*>(b->position);
+    const T* rot = static_cast<const T*>(b->rotation);
+    const T* vel = static_cast<const T*>(b->velocity);
+    const T* planes = static_cast<const T*>(b->planes);
+    T* opos = static_cast<T*>(out->position);
+    T* ovel = static_cast<T*>(out->velocity);
+    const uint32_t iters = cfg->move_and_slide_iterations;
+    for (uint32_t i = 0; i < b->count; ++i) {
+        HostMoveHits<T> hits{out->hit_collider, out->hit_distance, out->hit_toi, out->hit_point, out->hit_normal, size_t(i) * iters};
+        for (uint32_t it = 0; it < iters; ++it) hits.sweep(it, 0xffffffffu, T(0), T(0), mv::T3<T>{0, 0, 0}, mv::T3<T>{0, 0, 0});
+        const mv::Body bd{int(b->shape[i]), V3{S(dims[3 * i]), S(dims[3 * i + 1]), S(dims[3 * i + 2])},
+                          Q{S(rot[4 * i]), S(rot[4 * i + 1]), S(rot[4 * i + 2]), S(rot[4 * i + 3])}};
+        mv::T3<T> p{pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]}, v{vel[3 * i], vel[3 * i + 1], vel[3 * i + 2]};
+        if (qm::collider_valid(bd.he, mv::to_v3(p), bd.q) && qm::finite3(mv::to_v3(v))) {
+            mv::T3<float> init[mv::MAX_PLANES];
+            int ni = 0;
+            if (b->plane_offsets)
+                for (uint32_t k = b->plane_offsets[i]; k < b->plane_offsets[i + 1]; ++k)
+                    init[ni++] = mv::plane_dir(mv::T3<T>{planes[3 * k], planes[3 * k + 1], planes[3 * k + 2]});
+            const HostMoveScene<T> ms{sc, valid.data(), tmn.data(), tmx.data(), b->mask ? b->mask[i] : 0xffffffffu,
+                                      b->exclude_offsets ? b->exclude_offsets[i + 1] - b->exclude_offsets[i] : 0u,
+                                      b->exclude_offsets ? b->exclude + b->exclude_offsets[i] : nullptr, cfg->ignored};
+            mv::move_and_slide(ms, mc, bd, p, v, init, ni, hits);
+        }
+        opos[3 * i] = p.x; opos[3 * i + 1] = p.y; opos[3 * i + 2] = p.z;
+        ovel[3 * i] = v.x; ovel[3 * i + 1] = v.y; ovel[3 * i + 2] = v.z;
+    }
+}
+}  // namespace
+
+extern "C" {
+
+// MoveAndSlide::move_and_slide for every character of the batch against every collider: the same output as avn_move_and_slide
+int avh_move_and_slide(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) {
+    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = mv::check_move(cfg, b, scalar_bits == 64, c->count)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (!out || (b->count && (!out->position || !out->velocity))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "position and velocity outputs are required");
+    out->kernel_ms = 0.f;
+    if (scalar_bits == 64) move_all<double>(c, cfg, b, out);
+    else move_all<float>(c, cfg, b, out);
+    return AVN_OK;
+}
+
+// test infrastructure: the shared project_velocity (velocity_project.rs:122-324) on one velocity, normals as f32 Dirs
+void avh_move_project_velocity(uint32_t scalar_bits, const void* v, const float* normals, uint32_t n, void* out) {
+    std::vector<mv::T3<float>> ns(n);
+    for (uint32_t k = 0; k < n; ++k) ns[k] = mv::T3<float>{normals[3 * k], normals[3 * k + 1], normals[3 * k + 2]};
+    if (scalar_bits == 64) {
+        const double* x = static_cast<const double*>(v);
+        const mv::T3<double> r = mv::project_velocity(mv::T3<double>{x[0], x[1], x[2]}, ns.data(), int(n));
+        double* o = static_cast<double*>(out);
+        o[0] = r.x; o[1] = r.y; o[2] = r.z;
+    } else {
+        const float* x = static_cast<const float*>(v);
+        const mv::T3<float> r = mv::project_velocity(mv::T3<float>{x[0], x[1], x[2]}, ns.data(), int(n));
+        float* o = static_cast<float*>(out);
+        o[0] = r.x; o[1] = r.y; o[2] = r.z;
+    }
+}
+
+// test infrastructure: one intersection of the move (character a against collider b, double columns): the deepest penetration rounded to
+// the column scalar and the f32 plane normal -manifold.normal; 0 when the pair has no point within `prediction`
+int avh_move_contact(uint32_t scalar_bits, int sa, const double* ha, const double* pa, const double* qa, int sb, const double* hb, const double* pb,
+                     const double* qb, double prediction, float* normal, double* penetration) {
+    const V3 A{ha[0], ha[1], ha[2]}, PA{pa[0], pa[1], pa[2]}, B{hb[0], hb[1], hb[2]}, PB{pb[0], pb[1], pb[2]};
+    const Q QA{qa[0], qa[1], qa[2], qa[3]}, QB{qb[0], qb[1], qb[2], qb[3]};
+    mv::T3<float> n{0, 0, 0};
+    bool hit;
+    if (scalar_bits == 64) {
+        double pen = 0;
+        hit = mv::contact_plane<double>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        *penetration = pen;
+    } else {
+        float pen = 0;
+        hit = mv::contact_plane<float>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        *penetration = pen;
+    }
+    normal[0] = n.x; normal[1] = n.y; normal[2] = n.z;
+    return hit ? 1 : 0;
 }
 
 }  // extern "C"

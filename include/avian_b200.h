@@ -802,6 +802,75 @@ AvnStatus avn_query_point_intersections(AvnContext* ctx, const AvnPointBatch* po
  * The cast-only columns of the batch are ignored. */
 AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* shapes, AvnHitList* out);
 
+/* ---- move and slide (MoveAndSlide::move_and_slide, character_controller/move_and_slide.rs:464-609, velocity_project.rs:122-324) for
+ *      kinematic characters, against the tree of the last avn_query_update: one device thread per character runs the whole loop — an
+ *      initial depenetration, up to move_and_slide_iterations rounds of shape cast (AVN_CAST_IGNORE_ORIGIN_PENETRATION), pull-back by
+ *      skin_width / max(dir . -normal1, DOT_EPSILON), plane collection (the configured planes, the sweep hit's plane, every intersection at
+ *      2 * skin_width, similar planes (f32 dot >= plane_similarity_dot_threshold) keeping the more blocking normal) and the cone projection
+ *      of the velocity — then a final depenetration (Gauss-Seidel over the intersections at skin_width, planes deeper than
+ *      penetration_rejection_threshold skipped, stop when the summed error < max_depenetration_error; all three scaled by length_unit).
+ *      The per-character algorithm is avian_b200/csrc/move_math.hpp, shared with the host fixture, so results equal the host brute force
+ *      bit for bit.  Dir is f32 in both builds, as in the reference: the sweep direction, the plane normals and the similarity dot product
+ *      are f32 also for 64-bit columns.  Obstacles: the colliders that pass the character's filter (mask, exclusion list: exclude the
+ *      character's own collider there) and are not marked in `ignored` (sensors, colliders without a body), both for the cast and the
+ *      intersections.  A character with a non-finite pose, velocity or dims or a zero quaternion is returned unmoved with no hits.
+ *      Stated deviations: on_hit cannot run on the device — every hit is accepted and nothing edits the normal, position or velocity; the
+ *      closest sweep hit is the lowest (t, collider index), not the first in tree order; intersections are visited in ascending collider
+ *      index, not tree order; hit_toi reports the TOI, where MoveHitData::collision_distance is the requested movement length (:777);
+ *      characters are cuboids and spheres. ------------------------------------------------------------------------------------------- */
+#define AVN_MOVE_MAX_PLANES 32
+
+/* MoveAndSlideConfig, one per call.  The reference's defaults: skin_width 0.01, max_depenetration_error 0.0001,
+ * penetration_rejection_threshold 0.5, plane_similarity_dot_threshold 0.99619469809 (cos 5 degrees), 4 iterations, 16 depenetration
+ * iterations, 20 planes. */
+typedef struct AvnMoveConfig {
+    double delta_time;
+    double length_unit;                 /* PhysicsLengthUnit */
+    double skin_width;
+    double max_depenetration_error;
+    double penetration_rejection_threshold;
+    double plane_similarity_dot_threshold;
+    uint32_t move_and_slide_iterations;
+    uint32_t depenetration_iterations;  /* 0 = no depenetration */
+    uint32_t max_planes;                /* <= AVN_MOVE_MAX_PLANES */
+    uint32_t collider_count;            /* entries of ignored; must equal the tree's collider count when ignored is set */
+    const uint8_t* ignored;             /* [collider_count] nonzero = not an obstacle (sensors, colliders without a body); NULL = none */
+} AvnMoveConfig;
+
+typedef struct AvnMoveBatch {           /* one character per entry */
+    uint32_t count;
+    uint32_t exclude_count;             /* length of exclude[] */
+    const uint8_t* shape;               /* [n] AvnShape */
+    const void* dims;                   /* [n][3] cuboid half extents / sphere radius in [0] */
+    const void* position;               /* [n][3] */
+    const void* rotation;               /* [n][4] */
+    const void* velocity;               /* [n][3] desired velocity */
+    const uint32_t* mask;               /* [n] SpatialQueryFilter::mask; NULL = all layers */
+    const uint32_t* exclude_offsets;    /* [n + 1] CSR of excluded collider indices; NULL = none */
+    const uint32_t* exclude;            /* [exclude_count] */
+    const uint32_t* plane_offsets;      /* [n + 1] CSR of MoveAndSlideConfig::planes per character (e.g. the ground), at most max_planes each; NULL = none */
+    const void* planes;                 /* [plane_offsets[n]][3] nonzero, finite; normalised in f32 (Dir::new) */
+} AvnMoveBatch;
+
+typedef struct AvnMoveResult {
+    void* position;                     /* [n][3] out: MoveAndSlideOutput::position */
+    void* velocity;                     /* [n][3] out: MoveAndSlideOutput::projected_velocity */
+    /* [n][move_and_slide_iterations] out, fixed stride; collider -1 = no sweep hit in that iteration (the other columns 0 there).
+     * Any of these may be NULL (not wanted). */
+    int32_t* hit_collider;
+    void* hit_distance;                 /* the safe distance moved (MoveHitData::distance) */
+    void* hit_toi;                      /* the TOI of the cast */
+    void* hit_point;                    /* [..][3] point1, on the hit collider (world) */
+    void* hit_normal;                   /* [..][3] normal1, outward from the hit collider */
+    float kernel_ms;                    /* out: device time of the move kernel */
+    uint32_t _pad;
+} AvnMoveResult;
+
+/* Before any update: AVN_ERR_INVALID_ARGUMENT.  Refused with AVN_ERR_INVALID_ARGUMENT: negative dims, unknown shapes, a bad exclusion CSR,
+ * max_planes above AVN_MOVE_MAX_PLANES, more initial planes than max_planes, non-finite or zero initial planes, a NaN config value, an
+ * `ignored` column whose count is not the tree's. */
+AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const AvnMoveBatch* batch, AvnMoveResult* out);
+
 /* ---- swept continuous collision detection (SweptCcd, dynamics/ccd/mod.rs:523-780) on the device-resident solver stage ----------------
  *      Replaces solve_swept_ccd, which the reference runs after the substeps and before solve_restitution: for every SweptCcd body, in the
  *      order of the configured list, every collider adjacent to its own collider in the ContactGraph (every live contact row, touching or
