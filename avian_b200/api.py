@@ -24,6 +24,8 @@ AABB_IS_INACTIVE, AABB_CONTACT_EVENTS, AABB_GENERATE_CONSTRAINTS, AABB_CUSTOM_FI
 PAIR_CONTACT_EVENTS, PAIR_MODIFY_CONTACTS, PAIR_GENERATE_CONSTRAINTS, PAIR_NEEDS_HOOK = 1, 2, 4, 8
 CFG_FAST_TRIG = 1
 OK, ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_OUT_OF_MEMORY, ERR_UNSUPPORTED, ERR_CAPACITY, ERR_NCCL = 0, -1, -2, -3, -4, -5, -6
+# AvnShape; a capsule's dims are [radius, half length, unused] with its segment along the collider's local y
+SHAPE_CUBOID, SHAPE_SPHERE, SHAPE_CAPSULE = 0, 1, 2
 
 _vp = C.c_void_p
 

@@ -1,6 +1,6 @@
-// update_aabb on the device for cuboid and sphere colliders.  Replaces update_aabb::<Collider>
-// (src/collision/collider/backend.rs:498-625); the shape AABBs follow parry3d's Cuboid::aabb / Ball::aabb
-// (center +- |R| half_extents with nalgebra's UnitQuaternion::to_rotation_matrix; center +- radius).
+// update_aabb on the device for cuboid, sphere and capsule colliders.  Replaces update_aabb::<Collider>
+// (src/collision/collider/backend.rs:498-625); the shape AABBs follow parry3d's Cuboid::aabb / Ball::aabb / Capsule::aabb
+// (center +- |R| half_extents with nalgebra's UnitQuaternion::to_rotation_matrix; center +- radius; capsule_aabb below).
 // One thread per collider: 52-68 B in, 24 B out — a pure streaming kernel (HBM-bound, ~90 B per collider).
 #include <cmath>
 #include <limits>
@@ -19,8 +19,24 @@ struct AabbArgs {
     S dt, tol, def_spec, scalar_max;   // scalar_max = Scalar::MAX (what SpeculativeMargin::MAX / SweptCcd stand for)
 };
 
+// parry3d's Capsule::aabb: the segment's end points (0, -+half_length, 0) moved by the pose, their componentwise min / max, loosened by the
+// radius.  The end points are rotated with nalgebra's UnitQuaternion * Vector3 (t = 2 (q.xyz x v), v + q.xyz x t + t w), not the matrix.
 template <class S>
+__device__ __noinline__ void capsule_aabb(V3<S> d, V3<S> p, Q4<S> q, V3<S>& mn, V3<S>& mx) {
+    const V3<S> b = mk3<S>(q.x, q.y, q.z);
+    const V3<S> v0 = mk3<S>(S(0), -d.y, S(0)), v1 = mk3<S>(S(0), d.y, S(0));
+    const V3<S> t0 = cross(b, v0) * S(2), t1 = cross(b, v1) * S(2);
+    const V3<S> e0 = ((v0 + cross(b, t0)) + t0 * q.w) + p, e1 = ((v1 + cross(b, t1)) + t1 * q.w) + p;
+    mn = mk3<S>(avn_min(e0.x, e1.x) - d.x, avn_min(e0.y, e1.y) - d.x, avn_min(e0.z, e1.z) - d.x);
+    mx = mk3<S>(avn_max(e0.x, e1.x) + d.x, avn_max(e0.y, e1.y) + d.x, avn_max(e0.z, e1.z) + d.x);
+}
+
+template <class S, bool CAPSULES>
 __device__ __forceinline__ void shape_aabb(int shape, V3<S> d, V3<S> p, Q4<S> q, V3<S>& mn, V3<S>& mx) {
+    if (CAPSULES && shape == AVN_SHAPE_CAPSULE) {
+        capsule_aabb<S>(d, p, q, mn, mx);
+        return;
+    }
     V3<S> he;
     if (shape == AVN_SHAPE_SPHERE) {
         he = mk3<S>(d.x, d.x, d.x);
@@ -38,10 +54,13 @@ __device__ __forceinline__ void shape_aabb(int shape, V3<S> d, V3<S> p, Q4<S> q,
     mx = p + he;
 }
 
-template <class S>
-__global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a) {
+// One thread per collider.  CAPSULES = false (update_aabbs_kernel): cuboids and spheres, skipping the capsules when `capsules` is set;
+// CAPSULES = true (update_capsule_aabbs_kernel, launched only for a shape column that holds a capsule): the capsules alone.
+template <class S, bool CAPSULES>
+__device__ __forceinline__ void update_aabb(const AabbArgs<S>& a, int capsules) {
     int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= a.n) return;
+    if (capsules && (a.shape[n] == AVN_SHAPE_CAPSULE) != CAPSULES) return;
     V3<S> d = mk3<S>(a.dims[3 * n], a.dims[3 * n + 1], a.dims[3 * n + 2]), p = mk3<S>(a.pos[3 * n], a.pos[3 * n + 1], a.pos[3 * n + 2]);
     Q4<S> q; q.x = a.rot[4 * n]; q.y = a.rot[4 * n + 1]; q.z = a.rot[4 * n + 2]; q.w = a.rot[4 * n + 3];
     const int shape = a.shape ? a.shape[n] : AVN_SHAPE_CUBOID;
@@ -49,15 +68,15 @@ __global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a) {
     S spec = a.sm ? (isinf(a.sm[n]) ? a.scalar_max : a.sm[n]) : a.def_spec;
     V3<S> mn, mx;
     if (spec <= S(0)) {
-        shape_aabb<S>(shape, d, p, q, mn, mx);
+        shape_aabb<S, CAPSULES>(shape, d, p, q, mn, mx);
     } else {
         V3<S> v = a.lv ? mk3<S>(a.lv[3 * n], a.lv[3 * n + 1], a.lv[3 * n + 2]) : zero3<S>();
         V3<S> w = a.av ? mk3<S>(a.av[3 * n], a.av[3 * n + 1], a.av[3 * n + 2]) : zero3<S>();
         Q4<S> end_rot = q_fast_renormalize(qmul(q_from_scaled_axis(w * a.dt, false), q));
         V3<S> end_pos = p + clamp_len_max(v * a.dt, avn_max(spec, a.tol));
         V3<S> mn0, mx0, mn1, mx1;
-        shape_aabb<S>(shape, d, p, q, mn0, mx0);
-        shape_aabb<S>(shape, d, end_pos, end_rot, mn1, mx1);
+        shape_aabb<S, CAPSULES>(shape, d, p, q, mn0, mx0);
+        shape_aabb<S, CAPSULES>(shape, d, end_pos, end_rot, mn1, mx1);
         mn = mk3<S>(avn_min(mn0.x, mn1.x), avn_min(mn0.y, mn1.y), avn_min(mn0.z, mn1.z));
         mx = mk3<S>(avn_max(mx0.x, mx1.x), avn_max(mx0.y, mx1.y), avn_max(mx0.z, mx1.z));
     }
@@ -65,6 +84,11 @@ __global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a) {
     a.omn[3 * n] = mn.x - g; a.omn[3 * n + 1] = mn.y - g; a.omn[3 * n + 2] = mn.z - g;
     a.omx[3 * n] = mx.x + g; a.omx[3 * n + 1] = mx.y + g; a.omx[3 * n + 2] = mx.z + g;
 }
+
+template <class S>
+__global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a, int capsules) { update_aabb<S, false>(a, capsules); }
+template <class S>
+__global__ void update_capsule_aabbs_kernel(const __grid_constant__ AabbArgs<S> a) { update_aabb<S, true>(a, 1); }
 
 template <class S>
 class AabbUpdater final : public AabbBase {
@@ -76,6 +100,10 @@ class AabbUpdater final : public AabbBase {
         if (n == 0) return AVN_OK;
         if (!c->dims || !c->position || !c->rotation || !c->aabb_min || !c->aabb_max)
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "colliders: dims, position, rotation, aabb_min and aabb_max are required");
+        size_t at = 0;
+        bool capsules = false;
+        if (const char* why = check_shape_column(c->shape, c->dims, n, sizeof(S) == 8 ? 64 : 32, &at, &capsules))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "colliders: collider %zu: %s", at, why);
         AabbArgs<S> a{};
         a.n = int(n);
         AvnStatus st;
@@ -95,7 +123,8 @@ class AabbUpdater final : public AabbBase {
         a.dt = S(prm->dt); a.tol = S(prm->contact_tolerance);
         a.scalar_max = std::numeric_limits<S>::max();
         a.def_spec = std::isinf(prm->default_speculative_margin) ? std::numeric_limits<S>::max() : S(prm->default_speculative_margin);
-        update_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a);
+        update_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a, capsules ? 1 : 0);
+        if (capsules) update_capsule_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a);
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(c->aabb_min, a.omn, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(c->aabb_max, a.omx, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));

@@ -236,9 +236,12 @@ AvnStatus avn_contacts_step(AvnContext* ctx, const AvnNarrowParams* params, cons
     return guarded(ctx, [&] {
         avn::DevicePairs pairs;
         const bool take = (flags & AVN_CONTACTS_TAKE_BROADPHASE_PAIRS) != 0;
-        // this step's collider / body columns start moving to the device before the broad phase is waited for
+        // this step's collider / body columns start moving to the device before the broad phase is waited for; a shape column that is
+        // going to be copied is checked first, so a refused step changes nothing
         if (params && input && out) {
-            AvnStatus st = ctx->contacts->prefetch_inputs(params, input, match_contacts, length_unit, flags);
+            AvnStatus st = ctx->contacts->check_shapes(input, flags);
+            if (st != AVN_OK) return st;
+            st = ctx->contacts->prefetch_inputs(params, input, match_contacts, length_unit, flags);
             if (st != AVN_OK) return st;
         }
         if (take) {
@@ -351,6 +354,8 @@ AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
         ctx->contacts->asleep_bodies(&asleep);
         if (asleep.body_asleep && config && config->count)
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
+        if (config && config->count && ctx->contacts->has_capsule())
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a capsule; capsule times of impact are not implemented");
         avn::CcdRows rows;
         ctx->contacts->ccd_rows(&rows);
         return ctx->ccd->configure(config, rows);

@@ -29,8 +29,15 @@ struct NarrowEdgeArgs {
 template <class S> NM_HD inline nm::V3 ldd3(const S* p, size_t i) { return {double(p[3 * i]), double(p[3 * i + 1]), double(p[3 * i + 2])}; }
 template <class S> NM_HD inline void std3(S* p, size_t i, nm::V3 v) { p[3 * i] = S(v.x); p[3 * i + 1] = S(v.y); p[3 * i + 2] = S(v.z); }
 
-// geometry + match_contacts for every live row (same arithmetic as avh_raw_manifolds + avh_match_raw of the host fixture)
+// A live row that names a capsule: the device runs it in a kernel of its own (narrow_capsule_edges_kernel), see nm::collide.
 template <class S>
+NM_HD inline bool capsule_row(const NarrowEdgeArgs<S>& a, int e) {
+    return a.shape && a.r.live[e] && (a.shape[a.r.c1[e]] == nm::SHAPE_CAPSULE || a.shape[a.r.c2[e]] == nm::SHAPE_CAPSULE);
+}
+
+// geometry + match_contacts for every live row (same arithmetic as avh_raw_manifolds + avh_match_raw of the host fixture).  CAPSULES = false:
+// the row holds no capsule (the cuboid / sphere kernel).
+template <class S, bool CAPSULES = true>
 NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e) {
     const EdgeRows<S>& r = a.r;
     if (r.asleep && r.asleep[e]) return;   // update_contacts runs over active_pairs only (narrow_phase/system_param.rs:437)
@@ -55,7 +62,7 @@ NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e) {
         const double max_dist = nm::smax(eff_margin, a.tol);
         nm::Contacts pts;
         const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
-        if (nm::collide(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts))
+        if (nm::collide<CAPSULES>(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts))
             np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
         else
             normal = nm::V3{0, 0, 0};

@@ -451,15 +451,29 @@ __global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ l
     ob[i] = g.pflags[e] & EV_FLAGS; ob[n + i] = uint8_t(cnt);
 }
 
+// capsules != 0: the shape column holds a capsule, and the rows that name one are left to narrow_capsule_edges_kernel
 template <class S>
-__global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh) {
+__global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh, int capsules) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.r.E) return;
+    if (capsules && capsule_row(a, e)) return;
     if (only_fresh) {            // the rows added after the early pass over the existing rows (Contacts::prefetch_inputs)
         if (!fresh[e]) return;
         fresh[e] = 0;
     }
-    narrow_edge_row<S>(a, e);   // csrc/contact_rows.hpp: the same function the CPU tests run
+    narrow_edge_row<S, false>(a, e);   // csrc/contact_rows.hpp: the same function the CPU tests run
+}
+
+// the rows that name a capsule (launched after narrow_edges_kernel, on the same stream, only when the shape column holds a capsule)
+template <class S>
+__global__ void __launch_bounds__(128) narrow_capsule_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.r.E || !capsule_row(a, e)) return;
+    if (only_fresh) {
+        if (!fresh[e]) return;
+        fresh[e] = 0;
+    }
+    narrow_edge_row<S, true>(a, e);
 }
 
 
@@ -1039,6 +1053,19 @@ class Contacts final : public ContactsBase {
         out->shape = in_.shape;
         out->dims = in_.dims;
     }
+    AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) override {
+        if (!in || !in->dims) return AVN_OK;   // step() reports the missing columns
+        checked_ = nullptr;
+        if ((flags & AVN_CONTACTS_SHAPES_UNCHANGED) && in_.colliders == in->collider_count && in_.dims) return AVN_OK;   // the column is not copied
+        size_t at = 0;
+        bool capsule = false;
+        if (const char* why = check_shape_column(in->shape, in->dims, in->collider_count, sizeof(S) == 8 ? 64 : 32, &at, &capsule))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: collider %zu: %s", at, why);
+        checked_ = in;                  // upload_inputs commits has_capsule_ once this column is on the device
+        checked_capsule_ = capsule;
+        return AVN_OK;
+    }
+    bool has_capsule() const override { return has_capsule_; }
     void pair_set(const uint64_t** table, uint64_t* mask) override {
         *table = (configured_ && table_.p && !table_dirty_) ? table_.as<uint64_t>() : nullptr;
         *mask = table_mask_;
@@ -1350,6 +1377,7 @@ class Contacts final : public ContactsBase {
         if (!keep_shapes) {
             UPC(i_shape_, in->shape, C, uint8_t, in_.shape);
             UPC(i_dims_, in->dims, 3 * C, S, in_.dims);
+            if (checked_ == in) has_capsule_ = checked_capsule_;   // the flag describes the column now on the device
         }
         UPC(i_pos_, in->position, 3 * C, S, in_.pos);
         UPC(i_rot_, in->rotation, 4 * C, S, in_.rot);
@@ -1387,7 +1415,8 @@ class Contacts final : public ContactsBase {
         a.tol = prm->contact_tolerance;
         a.thr2 = (0.1 * length_unit) * (0.1 * length_unit);
         a.match = match_contacts ? 1 : 0;
-        narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0);
+        narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
+        if (has_capsule_) narrow_capsule_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0);
         AVN_CUDA(cudaGetLastError());
         return AVN_OK;
     }
@@ -1598,6 +1627,9 @@ class Contacts final : public ContactsBase {
     using ResidentGraph = ContactsBase::ResidentGraph;
     DevBuf isl_event_, fresh_, isl_buf_, isl_in_, isl_out_, isl_j_;
     uint32_t early_rows_ = 0;     // rows whose geometry prefetch_inputs already launched on the copy stream
+    bool has_capsule_ = false;    // the shape column on the device holds a capsule
+    const AvnNarrowInput* checked_ = nullptr;   // the input check_shapes last accepted, and whether its column holds a capsule
+    bool checked_capsule_ = false;
     bool added_this_step_ = false;
     IslandState isl_{};
     IslandCounters* h_isl_ = nullptr;

@@ -53,6 +53,23 @@ struct DevBuf {
     template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
+// The shape column of a collider set on the host, before anything is copied (a refused call changes nothing): every value at most
+// AVN_SHAPE_CAPSULE, and a capsule's radius and half length not negative.  NULL shape = all cuboids.  Returns NULL or the reason, with the
+// first offending collider in *at; *any_capsule (optional) tells whether the column holds a capsule.
+inline const char* check_shape_column(const uint8_t* shape, const void* dims, size_t count, uint32_t scalar_bits, size_t* at, bool* any_capsule = nullptr) {
+    if (any_capsule) *any_capsule = false;
+    if (!shape) return nullptr;
+    for (size_t i = 0; i < count; ++i) {
+        if (shape[i] > AVN_SHAPE_CAPSULE) { *at = i; return "unknown shape (AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE are known)"; }
+        if (shape[i] != AVN_SHAPE_CAPSULE) continue;
+        if (any_capsule) *any_capsule = true;
+        const double r = scalar_bits == 64 ? static_cast<const double*>(dims)[3 * i] : double(static_cast<const float*>(dims)[3 * i]);
+        const double h = scalar_bits == 64 ? static_cast<const double*>(dims)[3 * i + 1] : double(static_cast<const float*>(dims)[3 * i + 1]);
+        if (r < 0 || h < 0) { *at = i; return "a capsule's radius and half length must not be negative"; }
+    }
+    return nullptr;
+}
+
 // the context's communicator (comm.cu): NCCL bound at run time; a communicator of one needs no NCCL at all
 struct CommBase {
     virtual ~CommBase() {}
@@ -189,6 +206,10 @@ struct ContactsBase {
     virtual void asleep_bodies(AsleepBodies* out) = 0;
     // ---- the rows and collider shapes swept CCD visits (ccd.cu)
     virtual void ccd_rows(CcdRows* out) = 0;
+    // ---- the shape column of a step: checked on the host when step() is going to copy it (not under AVN_CONTACTS_SHAPES_UNCHANGED), before
+    //      any state changes; has_capsule: the column of the last accepted step holds a capsule (swept CCD refuses capsules)
+    virtual AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) = 0;
+    virtual bool has_capsule() const = 0;
 };
 ContactsBase* make_contacts(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 

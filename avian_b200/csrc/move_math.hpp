@@ -113,12 +113,13 @@ NM_HD inline T3<T> project_velocity(T3<T> v, const T3<float>* normals, int n) {
 // ---- one intersection (intersections, move_and_slide.rs:1032-1078): the contact of the character with one collider -----------------------
 // nm::collide(character, collider) -> the deepest point (max_by: the last of equal penetrations) and the plane normal -manifold.normal as
 // an f32 Dir.  False when the pair has no point within the prediction distance.  Kept out of line: it holds the narrow phase's box-box
-// generator, and the move kernel calls it from two places.
+// generator, and the move kernel calls it from two places.  Characters and colliders are cuboids and spheres (capsules are refused on the
+// host), so the capsule pairs are not compiled in (nm::collide<false>).
 template <class T>
 NM_COLD inline bool contact_plane(int sa, V3 ha, V3 pa, Q qa, int sb, V3 hb, V3 pb, Q qb, double prediction, T3<float>& normal, T& penetration) {
     V3 n;
     nm::Contacts pts;
-    if (!nm::collide(sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts) || pts.n == 0) return false;
+    if (!nm::collide<false>(sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts) || pts.n == 0) return false;
     T best = T(nm::dot(pts.p[0].a - pts.p[0].b, n));
     for (int k = 1; k < pts.n; ++k) {
         const T p = T(nm::dot(pts.p[k].a - pts.p[k].b, n));

@@ -1,4 +1,4 @@
-// Contact manifolds for cuboid / sphere pairs on the device (SURVEY.md 8f "next #1", geometry stage).
+// Contact manifolds for cuboid / sphere / capsule pairs on the device (SURVEY.md 8f "next #1", geometry stage).
 // Stands where NarrowPhase::update calls contact_manifolds for every contact pair (narrow_phase/system_param.rs:437-830,
 // collider/parry/contact_query.rs:156-261).  The arithmetic is csrc/narrow_math.hpp — the same header the host fixture compiles — evaluated
 // in double like the fixture and rounded to the column scalar on store, so the device manifolds equal the fixture's bit for bit
@@ -24,11 +24,14 @@ struct NarrowArgs {
 template <class S> __device__ __forceinline__ nm::V3 ld3(const S* p, uint32_t i) { return {double(p[3 * i]), double(p[3 * i + 1]), double(p[3 * i + 2])}; }
 template <class S> __device__ __forceinline__ void st3(S* p, size_t i, nm::V3 v) { p[3 * i] = S(v.x); p[3 * i + 1] = S(v.y); p[3 * i + 2] = S(v.z); }
 
-template <class S>
-__global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant__ NarrowArgs<S> a) {
+// One thread per pair.  CAPSULES = false (narrow_phase_kernel): the cuboid / sphere pairs, and when `capsules` is set the pairs with a
+// capsule are skipped; CAPSULES = true (narrow_capsule_kernel, launched only for a shape column that holds a capsule): those pairs alone.
+template <class S, bool CAPSULES>
+__device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.n) return;
     const uint32_t ca = a.c1[k], cb = a.c2[k], ba = a.b1[k], bb = a.b2[k];
+    if (capsules && (a.shape[ca] == nm::SHAPE_CAPSULE || a.shape[cb] == nm::SHAPE_CAPSULE) != CAPSULES) return;
     a.count[k] = 0;
     if (a.amin) {  // the pair is removed when the AABBs no longer overlap (system_param.rs:437-470)
         const nm::V3 mina = ld3(a.amin, ca), maxa = ld3(a.amax, ca), minb = ld3(a.amin, cb), maxb = ld3(a.amax, cb);
@@ -48,7 +51,7 @@ __global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant
     nm::V3 normal;
     nm::Contacts pts;
     const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
-    if (!nm::collide(ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts)) return;
+    if (!nm::collide<CAPSULES>(ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts)) return;
     nm::PointOut out[4];
     const int np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
     a.count[k] = uint8_t(np);
@@ -60,6 +63,11 @@ __global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant
         a.normal_speed[size_t(4) * k + p] = S(out[p].normal_speed);
     }
 }
+
+template <class S>
+__global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant__ NarrowArgs<S> a, int capsules) { narrow_pair<S, false>(a, capsules); }
+template <class S>
+__global__ void __launch_bounds__(128) narrow_capsule_kernel(const __grid_constant__ NarrowArgs<S> a) { narrow_pair<S, true>(a, 1); }
 
 template <class S>
 class Narrow final : public NarrowBase {
@@ -78,6 +86,10 @@ class Narrow final : public NarrowBase {
         for (size_t k = 0; k < n; ++k)
             if (in->collider1[k] >= C || in->collider2[k] >= C || in->body1[k] >= B || in->body2[k] >= B)
                 return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: pair %zu indexes past the collider / body columns", k);
+        size_t at = 0;
+        bool capsules = false;
+        if (const char* why = check_shape_column(in->shape, in->dims, C, sizeof(S) == 8 ? 64 : 32, &at, &capsules))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: collider %zu: %s", at, why);
         NarrowArgs<S> a{};
         a.n = int(n);
         AvnStatus st;
@@ -112,7 +124,8 @@ class Narrow final : public NarrowBase {
         AVN_CUDA(cudaMemsetAsync(a.anchor2, 0, 12 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.penetration, 0, 4 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.normal_speed, 0, 4 * n * sizeof(S), stream_));
-        narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a);
+        narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, capsules ? 1 : 0);
+        if (capsules) narrow_capsule_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a);
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->point_count, a.count, n, cudaMemcpyDeviceToHost, stream_));
         if (out->disjoint) AVN_CUDA(cudaMemcpyAsync(out->disjoint, a.disjoint, n, cudaMemcpyDeviceToHost, stream_));

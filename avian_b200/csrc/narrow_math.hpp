@@ -1,4 +1,4 @@
-// Contact-manifold geometry for cuboid / sphere pairs, written once for the host fixture (g++, -ffp-contract=off) and for the device
+// Contact-manifold geometry for cuboid / sphere / capsule pairs, written once for the host fixture (g++, -ffp-contract=off) and for the device
 // (nvcc, -fmad=false): the same expressions in the same order, IEEE double throughout, so both evaluate to the same bits.
 //
 // What this is: OUR manifold generator (SAT + face clipping for boxes, closed forms for spheres).  The reference delegates this
@@ -45,7 +45,7 @@ NM_HD inline V3 rot(Q q, V3 v) {
 struct M3 { V3 c[3]; };  // columns = world directions of the local axes
 NM_HD inline M3 to_mat(Q q) { return {{rot(q, {1, 0, 0}), rot(q, {0, 1, 0}), rot(q, {0, 0, 1})}}; }
 
-enum ShapeType { SHAPE_CUBOID = 0, SHAPE_SPHERE = 1 };
+enum ShapeType { SHAPE_CUBOID = 0, SHAPE_SPHERE = 1, SHAPE_CAPSULE = 2 };
 struct Box { V3 c; M3 r; V3 he; };
 
 // witness points of a contact: on shape A, on shape B (world axes, origin at A's position: see collide).  A quad clipped by four planes
@@ -330,9 +330,213 @@ NM_HD inline bool box_sphere(const Box& A, V3 cs, S rs, S max_dist, V3& normal, 
     return true;
 }
 
-// One collider pair -> normal (from A to B) and at most 4 witness pairs.  he = half extents of a cuboid, radius in he.x of a sphere.
+// ---- capsules (DESIGN.md §7h): dims = [radius, half_length, unused], the segment from (0, -half_length, 0) to (0, +half_length, 0) of the
+// collider frame grown by the radius.  Every capsule routine is out of line and rolled, and returns through pts and its return value, so the
+// cuboid and sphere pairs compile to the code they had before capsules existed.  A capsule pair has at most 2 points.
+
+// Two directions count as parallel (two-point manifolds) when the sine of their angle is at most this (about 0.06 degrees).
+constexpr S CAPSULE_PARALLEL_SIN = 1e-3;
+// e_k x s axes of the segment-box SAT shorter than this (an edge direction parallel to the segment) are skipped
+constexpr S CAPSULE_EDGE_AXIS_MIN = 1e-6;
+
+struct Capsule { V3 c, u; S h, r; };   // centre, unit axis, half length, radius
+
+// u x e_k, normalised, with e_k the first world axis least aligned with the unit vector u: the fallback normal when two axes or a centre and an
+// axis coincide (perpendicular to u, so a witness grown from an interior segment point stays on the capsule's surface)
+NM_HD inline V3 capsule_perpendicular(V3 u) {
+    const V3 e = (fabs(u.x) <= fabs(u.y) && fabs(u.x) <= fabs(u.z)) ? V3{1, 0, 0} : (fabs(u.y) <= fabs(u.z) ? V3{0, 1, 0} : V3{0, 0, 1});
+    const V3 n = cross(u, e);
+    return n * (1 / len(n));
+}
+
+// Capsule A against a round shape B: the segment q + w*t, |t| <= hw, grown by rb (a sphere: hw = 0, w = A.u).  Normal from A to B.
+// The closest points of the two segments grown by the radii.  Distance 0: n = +-unit(A.u x w), the sign that points from A's centre to
+// B's (u x w itself on a tie); parallel axes (and a sphere centre on A's axis) take capsule_perpendicular(A.u).  Parallel capsules whose
+// projections on A's axis overlap get one point at each end of the overlap.
+NM_COLD inline bool capsule_round(const Capsule& A, V3 q, V3 w, S hw, S rb, S max_dist, V3& normal, Contacts& pts) {
+    S s, t;
+    segment_closest(A.c, A.u, A.h, q, w, hw, s, t);
+    const V3 p = A.c + A.u * s, qq = q + w * t, d = qq - p;
+    const S l = len(d);
+    if (l - A.r - rb > max_dist) return false;
+    const V3 x = cross(A.u, w);
+    const S lx = len(x);
+    const bool parallel = !(hw > 0) || lx <= CAPSULE_PARALLEL_SIN;
+    if (l > 1e-12) {
+        normal = d * (1 / l);
+    } else if (!parallel) {
+        normal = x * (1 / lx);
+        if (dot(normal, q - A.c) < 0) normal = -normal;
+    } else {
+        normal = capsule_perpendicular(A.u);
+    }
+    if (hw > 0 && parallel) {
+        const S t0 = dot(q - w * hw - A.c, A.u), t1 = dot(q + w * hw - A.c, A.u);
+        const S lo = smax(-A.h, smin(t0, t1)), hi = smin(A.h, smax(t0, t1));
+        if (lo < hi) {
+NM_ROLLED
+            for (int i = 0; i < 2; ++i) {
+                const V3 pi = A.c + A.u * (i == 0 ? lo : hi);
+                const S ti = smax(-hw, smin(hw, dot(pi - q, w)));
+                pts.push(pi + normal * A.r, q + w * ti - normal * rb);
+            }
+            return true;
+        }
+    }
+    pts.push(p + normal * A.r, qq - normal * rb);
+    return true;
+}
+
+// The closest points of a segment disjoint from box b: the two end points against the box and the segment against the 12 edges.  Returns the
+// distance.
+NM_COLD inline S segment_box_closest(const Box& b, const Capsule& C, V3& on_seg, V3& on_box) {
+    S best = 1e300;
+NM_ROLLED
+    for (int i = 0; i < 2; ++i) {
+        const V3 p = C.c + C.u * (i == 0 ? -C.h : C.h);
+        V3 on;
+        const S d2 = box_point_closest(b, p, on);
+        if (d2 < best) { best = d2; on_seg = p; on_box = on; }
+    }
+NM_ROLLED
+    for (int ei = 0; ei < 12; ++ei) {
+        const int k = ei >> 2, m = ei & 3, u = (k + 1) % 3, v = (k + 2) % 3;
+        const V3 e = b.c + b.r.c[u] * (m & 1 ? comp(b.he, u) : -comp(b.he, u)) + b.r.c[v] * (m & 2 ? comp(b.he, v) : -comp(b.he, v));
+        S s, t;
+        segment_closest(C.c, C.u, C.h, e, b.r.c[k], comp(b.he, k), s, t);
+        const V3 qs = C.c + C.u * s, qe = e + b.r.c[k] * t, d = qs - qe;
+        const S d2 = dot(d, d);
+        if (d2 < best) { best = d2; on_seg = qs; on_box = qe; }
+    }
+    return sqrt(best);
+}
+
+// The part [lo, hi] of C's segment (parameter along C.u) inside the side planes of b's faces on local axis k.  False when it is empty.
+NM_HD inline bool capsule_face_clip(const Box& b, int k, const Capsule& C, S& lo, S& hi) {
+    lo = -C.h; hi = C.h;
+NM_ROLLED
+    for (int i = 1; i < 3; ++i) {
+        const int j = (k + i) % 3;
+        const S a = dot(b.r.c[j], C.c - b.c), g = dot(b.r.c[j], C.u), he = comp(b.he, j);
+        if (fabs(g) < 1e-12) {
+            if (fabs(a) > he) return false;
+            continue;
+        }
+        const S s0 = (-he - a) / g, s1 = (he - a) / g;
+        lo = smax(lo, smin(s0, s1));
+        hi = smin(hi, smax(s0, s1));
+    }
+    return lo <= hi;
+}
+
+// Box b against capsule C (the segment grown by C.r); normal from the box to the capsule.  A segment disjoint from the box: its exact closest
+// points.  A segment that meets the box: the least-overlap axis of the 6-axis SAT (face normals, then e_k x u; an edge axis has to beat the faces
+// by 1e-4, as in box_box), with the closest points of the segment and that box edge, or the segment clipped to the face's side planes and its
+// deepest clipped point.  Either way, a normal within CAPSULE_PARALLEL_SIN of a face normal with the segment parallel to that face gives the
+// two ends of the clipped segment.
+NM_COLD inline bool box_capsule(const Box& b, const Capsule& C, S max_dist, V3& normal, Contacts& pts) {
+    const V3 d = C.c - b.c;
+    S max_sep = -1e300, best = -1e300, face_best = -1e300;
+    int best_k = 0, face_k = 0;
+    bool best_edge = false;
+    V3 best_n{0, 1, 0}, face_n{0, 1, 0};
+NM_ROLLED
+    for (int i = 0; i < 6; ++i) {
+        V3 n = i < 3 ? b.r.c[i] : cross(b.r.c[i - 3], C.u);
+        const S l = len(n);
+        if (l < CAPSULE_EDGE_AXIS_MIN) continue;
+        n = n * (1 / l);
+        if (dot(n, d) < 0) n = -n;
+        const S sep = dot(n, d) - box_radius(b, n) - C.h * fabs(dot(C.u, n));
+        max_sep = smax(max_sep, sep);
+        const S biased = i < 3 ? sep : sep - 1e-4;
+        if (biased > best + 1e-9) { best = biased; best_k = i % 3; best_edge = i >= 3; best_n = n; }
+        if (i < 3 && sep > face_best + 1e-9) { face_best = sep; face_k = i; face_n = n; }
+    }
+    int fk = -1;   // the face whose normal the contact normal is, or -1
+    if (max_sep > 0) {   // the segment misses the box
+        V3 on_seg, on_box;
+        const S dist = segment_box_closest(b, C, on_seg, on_box);
+        if (dist - C.r > max_dist) return false;
+        normal = (on_seg - on_box) * (1 / dist);
+NM_ROLLED
+        for (int k = 0; k < 3; ++k)
+            if (fabs(dot(normal, b.r.c[k])) >= 1 - 0.5 * CAPSULE_PARALLEL_SIN * CAPSULE_PARALLEL_SIN) fk = k;
+        if (fk < 0 || fabs(dot(C.u, b.r.c[fk])) > CAPSULE_PARALLEL_SIN) {
+            pts.push(on_box, on_seg - normal * C.r);
+            return true;
+        }
+        normal = b.r.c[fk] * (dot(normal, b.r.c[fk]) < 0 ? -1 : 1);
+    } else {
+        if (best_edge) {
+            const V3 n = best_n;
+            V3 e = b.c;
+NM_ROLLED
+            for (int j = 0; j < 3; ++j)
+                if (j != best_k) e = e + b.r.c[j] * (comp(b.he, j) * (dot(b.r.c[j], n) > 0 ? 1 : -1));
+            S s, t;
+            if (!segment_closest(C.c, C.u, C.h, e, b.r.c[best_k], comp(b.he, best_k), s, t)) {
+                normal = n;
+                pts.push(e + b.r.c[best_k] * t, C.c + C.u * s - n * C.r);
+                return true;
+            }
+            // an end is active: the edge is not the deepest feature, the best face axis is used
+        }
+        fk = face_k;
+        normal = face_n;
+    }
+    // face contact on face fk (outward normal `normal`): the segment clipped to the face's side planes
+    const S face_d = dot(normal, b.c) + comp(b.he, fk);
+    S lo, hi;
+    if (!capsule_face_clip(b, fk, C, lo, hi)) {   // the segment passes beside the face: its deepest end point
+        lo = hi = dot(C.u, normal) > 0 ? -C.h : C.h;
+    } else if (fabs(dot(C.u, normal)) > CAPSULE_PARALLEL_SIN || !(lo < hi)) {   // one point: the deepest clipped point
+        lo = hi = dot(C.u, normal) > 0 ? lo : hi;
+    }
+NM_ROLLED
+    for (int i = 0; i < (lo < hi ? 2 : 1); ++i) {
+        const V3 q = C.c + C.u * (i == 0 ? lo : hi);
+        pts.push(q - normal * (dot(normal, q) - face_d), q - normal * C.r);
+    }
+    return true;
+}
+
+// A pair with at least one capsule: the capsule goes first (A's unless only B is one), the result is swapped back as in collide.  Returns the
+// normal (from A to B); pts.n == 0 when the pair is farther apart than max_dist.
+NM_COLD inline V3 capsule_pair(int type_a, V3 dims_a, Q qa, int type_b, V3 dims_b, V3 pb, Q qb, S max_dist, Contacts& pts) {
+    pts.clear();
+    const bool cap_b = type_a != SHAPE_CAPSULE;
+    const int to = cap_b ? type_a : type_b;
+    const V3 dc = cap_b ? dims_b : dims_a, dn = cap_b ? dims_a : dims_b;
+    const Q qc = cap_b ? qb : qa, qo = cap_b ? qa : qb;
+    const V3 pc = cap_b ? pb : V3{0, 0, 0}, po = cap_b ? V3{0, 0, 0} : pb;
+    const Capsule C{pc, rot(qc, {0, 1, 0}), dc.y, dc.x};
+    V3 normal{0, 1, 0};
+    bool flip;
+    if (to == SHAPE_CUBOID) {
+        const Box X{po, to_mat(qo), dn};
+        box_capsule(X, C, max_dist, normal, pts);
+        flip = !cap_b;   // box_capsule reports from the box to the capsule
+    } else {
+        if (to == SHAPE_CAPSULE) capsule_round(C, po, rot(qo, {0, 1, 0}), dn.y, dn.x, max_dist, normal, pts);
+        else capsule_round(C, po, C.u, 0, dn.x, max_dist, normal, pts);
+        flip = cap_b;
+    }
+    if (flip) {
+        normal = -normal;
+NM_ROLLED
+        for (int k = 0; k < pts.n; ++k) { V3 t = pts.p[k].a; pts.p[k].a = pts.p[k].b; pts.p[k].b = t; }
+    }
+    return normal;
+}
+
+// One collider pair -> normal (from A to B) and at most 4 witness pairs.  he = half extents of a cuboid, radius in he.x of a sphere, [radius,
+// half length] of a capsule.
 // The geometry runs in a frame centred on A, so the result does not depend on where the pair is in the world (the header's absolute
 // thresholds, e.g. prune4's 1e-12 depth tie, would otherwise meet the rounding of world coordinates): the witnesses are relative to pa.
+// CAPSULES = false compiles the cuboid / sphere pairs alone: the device kernels that run those leave every pair with a capsule to a kernel
+// of its own (narrow.cu, contacts.cu), so their code and registers are what they were before capsules existed.
+template <bool CAPSULES = true>
 NM_HD inline bool collide(int type_a, V3 he_a, V3 pa, Q qa, int type_b, V3 he_b, V3 pb, Q qb, S max_dist, V3& normal, Contacts& pts) {
     pb = pb - pa;
     pa = V3{0, 0, 0};
@@ -343,6 +547,9 @@ NM_HD inline bool collide(int type_a, V3 he_a, V3 pa, Q qa, int type_b, V3 he_b,
         if (hit) prune4(pts, normal);
     } else if (type_a == SHAPE_SPHERE && type_b == SHAPE_SPHERE) {
         hit = sphere_sphere(pa, he_a.x, pb, he_b.x, max_dist, normal, pts);
+    } else if (CAPSULES && (type_a == SHAPE_CAPSULE || type_b == SHAPE_CAPSULE)) {
+        normal = capsule_pair(type_a, he_a, qa, type_b, he_b, pb, qb, max_dist, pts);
+        hit = pts.n != 0;
     } else if (type_a == SHAPE_CUBOID) {
         Box A{pa, to_mat(qa), he_a};
         hit = box_sphere(A, pb, he_b.x, max_dist, normal, pts);

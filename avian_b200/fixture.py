@@ -12,7 +12,7 @@ from . import _build, api
 _vp = C.c_void_p
 _lib = None
 
-SHAPE_CUBOID, SHAPE_SPHERE = 0, 1
+SHAPE_CUBOID, SHAPE_SPHERE, SHAPE_CAPSULE = 0, 1, 2
 
 
 def _load():
@@ -462,6 +462,8 @@ def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, 
     st = lib.avh_ccd_solve(32 if dt_ == np.float32 else 64, float(dt), float(length_unit), B, _p(kind), _p(pos), _p(rot), _p(com), _p(lv), _p(av),
                            _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
                            *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
+    if st == api.ERR_UNSUPPORTED:
+        raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule (capsule times of impact are not implemented)")
     if st != 0:
         raise ValueError("avh_ccd_solve: invalid configuration")
     return out

@@ -1,8 +1,8 @@
 // libavian_host.so — the host-side FIXTURE that stands in for the parts of an avian3d app that stay on the CPU
 // around the GPU hot path, so the hot path can be exercised and benchmarked without Bevy:
-//   * swept collider AABBs        (restates update_aabb for cuboids/spheres, collider/backend.rs:498-625)
+//   * swept collider AABBs        (restates update_aabb for cuboids/spheres/capsules, collider/backend.rs:498-625)
 //   * ContactGraph bookkeeping    (pair set, lowest-free ContactId, contact_graph.rs:521-631; id_pool.rs:43-52)
-//   * a narrow phase for cuboid / sphere pairs (SAT + face clipping; the reference delegates this arithmetic
+//   * a narrow phase for cuboid / sphere / capsule pairs (SAT + face clipping; the reference delegates this arithmetic
 //     to parry3d 0.25, which is not vendored, so this is OUR manifold generator: a fixture, identical for the
 //     oracle and the GPU path, not a parity claim), contact matching (contact_types/mod.rs:426-470),
 //     the status-change loop and ConstraintGraph push/pop colouring (narrow_phase/system_param.rs:136-389,
@@ -210,6 +210,21 @@ void avh_update_aabbs(AvhPipeline* h, uint32_t scalar_bits, const void* position
         for (int e = 0; e < 2; ++e) {
             V3 c = e ? p1 : p0;
             V3 ext;
+            if (sh.type == SHAPE_CAPSULE) {   // Capsule::aabb: the segment's end points moved by the pose (nalgebra's quaternion product), loosened by the radius
+                const Q q = e ? q1 : q0;
+                const V3 b{q.x, q.y, q.z};
+                V3 ends[2];
+                for (int i = 0; i < 2; ++i) {
+                    const V3 v{0, i ? sh.he.y : -sh.he.y, 0};
+                    const V3 t = cross(b, v) * 2.0;
+                    ends[i] = ((v + cross(b, t)) + t * q.w) + c;
+                }
+                lo = {std::min(lo.x, std::min(ends[0].x, ends[1].x) - sh.he.x), std::min(lo.y, std::min(ends[0].y, ends[1].y) - sh.he.x),
+                      std::min(lo.z, std::min(ends[0].z, ends[1].z) - sh.he.x)};
+                hi = {std::max(hi.x, std::max(ends[0].x, ends[1].x) + sh.he.x), std::max(hi.y, std::max(ends[0].y, ends[1].y) + sh.he.x),
+                      std::max(hi.z, std::max(ends[0].z, ends[1].z) + sh.he.x)};
+                continue;
+            }
             if (sh.type == SHAPE_SPHERE) {
                 ext = {sh.he.x, sh.he.x, sh.he.x};
             } else {
@@ -1278,6 +1293,10 @@ int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t 
                   uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2, const uint8_t* live, const AvnCcdConfig* cfg,
                   void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates, uint32_t* hits) {
     if (!cfg || (cfg->count && (!cfg->body || !cfg->collider))) return -1;
+    // capsule times of impact are not implemented: a configuration with a row that names a capsule is refused, as the device refuses it
+    if (cfg->count && shape)
+        for (uint32_t r = 0; r < rows; ++r)
+            if ((!live || live[r]) && (shape[c1[r]] == SHAPE_CAPSULE || shape[c2[r]] == SHAPE_CAPSULE)) return AVN_ERR_UNSUPPORTED;
     if (scalar_bits == 64)
         return ccd_solve<double>(dt, length_unit, body_count, kind, static_cast<const double*>(position), static_cast<const double*>(rotation),
                                  static_cast<const double*>(com), static_cast<const double*>(linvel), static_cast<const double*>(angvel),

@@ -10,7 +10,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import api
-from .fixture import SHAPE_CUBOID, SHAPE_SPHERE
+from .fixture import SHAPE_CAPSULE, SHAPE_CUBOID, SHAPE_SPHERE
 
 
 @dataclass
@@ -35,6 +35,17 @@ def _cuboid_mass(he: np.ndarray, density: float = 1.0):
     return m, np.stack([ix, iy, iz], axis=1)
 
 
+def _capsule_mass(radius: np.ndarray, half_length: np.ndarray, density: float = 1.0):
+    """mass and local inertia (diagonal, axis along local y) of solid capsules: a cylinder of length 2 half_length plus two hemispheres.
+    Closed form, PARITY UNPINNED: the reference takes capsule mass properties from bevy_heavy, which is not vendored."""
+    r, L = np.asarray(radius, dtype=np.float64), 2.0 * np.asarray(half_length, dtype=np.float64)
+    m_cyl = density * np.pi * r * r * L
+    m_sph = density * 4.0 / 3.0 * np.pi * r ** 3
+    iy = m_cyl * r * r / 2.0 + m_sph * 2.0 * r * r / 5.0
+    ix = m_cyl * (L * L / 12.0 + r * r / 4.0) + m_sph * (2.0 * r * r / 5.0 + L * L / 4.0 + 3.0 * L * r / 8.0)
+    return m_cyl + m_sph, np.stack([ix, iy, ix], axis=1)
+
+
 def _assemble(name, pos, rot, kind, he, shape_type, scalar, friction=0.5, restitution=0.0, linvel=None, angvel=None, density=1.0, **extra) -> Scene:
     n = pos.shape[0]
     s = np.dtype(scalar)
@@ -46,6 +57,9 @@ def _assemble(name, pos, rot, kind, he, shape_type, scalar, friction=0.5, restit
         ms = density * 4.0 / 3.0 * np.pi * r ** 3
         m[sph] = ms
         inertia[sph] = (0.4 * ms * r * r)[:, None]
+    cap = shape_type == SHAPE_CAPSULE
+    if cap.any():
+        m[cap], inertia[cap] = _capsule_mass(he[cap, 0], he[cap, 1], density)
     dyn = kind == api.BODY_DYNAMIC
     inv_m = np.where(dyn, 1.0 / m, 0.0)
     inv_i = np.zeros((n, 6))
@@ -163,11 +177,20 @@ _RAGDOLL = [
 ]
 
 
-def ragdoll_field(count: int, pitch: float = 8.0, drop_height: float = 2.0, seed: int = 1234, scalar=np.float32) -> Scene:
+# the limbs whose long axis is the body's local y: the capsule's axis without a rotated collider frame
+_CAPSULE_LIMBS = ("l_thigh", "l_shin", "r_thigh", "r_shin")
+
+
+def ragdoll_field(count: int, pitch: float = 8.0, drop_height: float = 2.0, seed: int = 1234, scalar=np.float32, limbs: str = "cuboid") -> Scene:
     """BASELINE config 4 (SURVEY §8d): `count` ragdolls on a square grid, 17 cuboid bodies and 16 joints each —
     spherical joints (swing +-60 deg, twist +-30 deg) for neck/spine/shoulders/hips/wrists/ankles, revolute joints
     (0..120 deg) for elbows and knees; every joint disables collision between its bodies (JointCollisionDisabled).
-    A small deterministic pose jitter (PCG64, seed) breaks symmetry."""
+    A small deterministic pose jitter (PCG64, seed) breaks symmetry.
+    limbs="capsule": thighs and shins are capsules along their long axis (local y), radius = the smaller half extent of the cross-section,
+    half length = half height - radius (the same height as the cuboid).  The arms' long axis is local x, and a capsule's segment runs along
+    the collider's local y: they stay cuboids, since turning their bodies would change the joint frames."""
+    if limbs not in ("cuboid", "capsule"):
+        raise ValueError(f"limbs must be 'cuboid' or 'capsule', not {limbs!r}")
     rng = np.random.default_rng(seed)
     side = int(np.ceil(np.sqrt(count)))
     nb = len(_RAGDOLL)
@@ -226,7 +249,48 @@ def ragdoll_field(count: int, pitch: float = 8.0, drop_height: float = 2.0, seed
 
     js = api.JointSet({api.JOINT_REVOLUTE: joints(rj, True), api.JOINT_SPHERICAL: joints(sj, False)})
     dis = np.array([(min(a, b) << 32) | max(a, b) for a, b in disabled], dtype=np.uint64)
-    return _assemble(f"ragdolls_{count}", pos, rot, kind, he, np.full(n + 1, SHAPE_CUBOID), scalar, joints=js, joint_disabled_body_pairs=dis)
+    shape = np.full(n + 1, SHAPE_CUBOID)
+    name = f"ragdolls_{count}"
+    if limbs == "capsule":
+        name += "_capsule_limbs"
+        limb = np.array([part[0] in _CAPSULE_LIMBS for part in _RAGDOLL] * count)
+        rows = 1 + np.flatnonzero(limb)
+        r = np.minimum(he[rows, 0], he[rows, 2])
+        he[rows] = np.stack([r, np.maximum(he[rows, 1] - r, 0.0), np.zeros_like(r)], axis=1)
+        shape[rows] = SHAPE_CAPSULE
+    return _assemble(name, pos, rot, kind, he, shape, scalar, joints=js, joint_disabled_body_pairs=dis)
+
+
+def capsule_pile(n: int, seed: int = 7, layers: int = 10, capsule_share: float = 0.8, sphere_share: float = 0.1, scalar=np.float32) -> Scene:
+    """A seeded pile of n dynamic bodies falling onto a static ground cuboid (body 0): mostly capsules (radius 0.15..0.3, half length
+    0.2..0.5) at uniformly random orientations, plus spheres (radius 0.2..0.4) and cubes (half extent 0.2..0.4, random orientation), on a
+    jittered grid of `layers` layers that starts without overlaps.  Every pair type meets: capsule against capsule, sphere, cube and ground.
+    Spawn order is x-major like cube_stack."""
+    rng = np.random.default_rng(seed)
+    u = rng.uniform(size=n)
+    shape = np.where(u < capsule_share, SHAPE_CAPSULE, np.where(u < capsule_share + sphere_share, SHAPE_SPHERE, SHAPE_CUBOID))
+    he = np.zeros((n, 3))
+    cap, sph, box = shape == SHAPE_CAPSULE, shape == SHAPE_SPHERE, shape == SHAPE_CUBOID
+    he[cap, 0] = rng.uniform(0.15, 0.3, size=cap.sum())
+    he[cap, 1] = rng.uniform(0.2, 0.5, size=cap.sum())
+    he[sph] = rng.uniform(0.2, 0.4, size=sph.sum())[:, None]
+    he[box] = rng.uniform(0.2, 0.4, size=box.sum())[:, None]
+    q = rng.normal(size=(n, 4))
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    q[sph] = [0.0, 0.0, 0.0, 1.0]
+    pitch = 2.0 * (0.5 + 0.3) + 0.2            # the longest capsule plus a gap, in every direction
+    side = int(np.ceil(np.sqrt(n / layers)))
+    k = np.arange(n)
+    layer, cell = k // (side * side), k % (side * side)
+    pos = np.stack([(cell // side) * pitch, 0.9 + layer * pitch, (cell % side) * pitch], axis=1) + rng.uniform(-0.05, 0.05, size=(n, 3))
+    order = np.lexsort((pos[:, 2], pos[:, 1], pos[:, 0]))
+    pos, q, he, shape = pos[order], q[order], he[order], shape[order]
+    extent = side * pitch
+    pos = np.concatenate([[[extent * 0.5, -0.5, extent * 0.5]], pos])
+    he = np.concatenate([[[extent * 0.5 + 10.0, 0.5, extent * 0.5 + 10.0]], he])
+    rot = np.concatenate([[[0.0, 0.0, 0.0, 1.0]], q])
+    kind = np.concatenate([[api.BODY_STATIC], np.full(n, api.BODY_DYNAMIC)])
+    return _assemble(f"capsule_pile_{n}", pos, rot, kind, he, np.concatenate([[SHAPE_CUBOID], shape]), scalar)
 
 
 def _qmul(a, b):

@@ -370,7 +370,10 @@ AvnStatus avn_broadphase_run(AvnContext* ctx);
 AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
 
 /* ---- collider AABBs (SURVEY.md 8f "next #2"): update_aabb for the shapes the device knows ------------------------------- */
-typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1 } AvnShape;
+/* AVN_SHAPE_CAPSULE: Collider::capsule(radius, length), dims = [radius, length / 2, unused]; the segment runs from (0, -length/2, 0) to
+ * (0, +length/2, 0) in the collider frame.  The AABB update, the narrow phase and the contact store take capsules; the spatial queries, move
+ * and slide and swept CCD refuse them. */
+typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2 } AvnShape;
 
 typedef struct AvnAabbParams {
     double dt;                         /* Time::delta (full step, collider/backend.rs:536) */
@@ -382,7 +385,7 @@ typedef struct AvnColliderColumns {
     uint32_t count;
     uint32_t _pad;
     const uint8_t* shape;              /* [C] AvnShape */
-    const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] (scaled shape) */
+    const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] / capsule [radius, half length] (scaled shape) */
     const void* position;              /* [C][3] collider Position */
     const void* rotation;              /* [C][4] collider Rotation */
     const void* linear_velocity;       /* [C][3] the velocity update_aabb uses: the collider's own LinearVelocity, or its body's velocity at
@@ -395,9 +398,10 @@ typedef struct AvnColliderColumns {
 } AvnColliderColumns;
 
 /*
- * Replaces update_aabb::<Collider> (src/collision/collider/backend.rs:498-625) for cuboid and sphere colliders: swept AABB from the
+ * Replaces update_aabb::<Collider> (src/collision/collider/backend.rs:498-625) for cuboid, sphere and capsule colliders: swept AABB from the
  * current pose to the pose after dt (rotation advanced by Quat::from_scaled_axis + fast_renormalize, translation clamped to the
- * speculative margin), grown by contact_tolerance + collision margin.
+ * speculative margin), grown by contact_tolerance + collision margin.  AVN_ERR_INVALID_ARGUMENT, before anything is computed, for a shape
+ * above AVN_SHAPE_CAPSULE or a capsule with a negative radius or half length (avn_narrow_phase and avn_contacts_step check the same).
  */
 AvnStatus avn_update_aabbs(AvnContext* ctx, const AvnAabbParams* params, AvnColliderColumns* colliders);
 
@@ -417,7 +421,7 @@ typedef struct AvnNarrowInput {
     const uint32_t* body1;             /* [pairs] row of the body velocity columns */
     const uint32_t* body2;
     const uint8_t* shape;              /* [C] AvnShape; NULL = cuboid */
-    const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] */
+    const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] / capsule [radius, half length] */
     const void* position;              /* [C][3] collider Position (collider at the body origin, centre of mass at the origin) */
     const void* rotation;              /* [C][4] */
     const void* linear_velocity;       /* [B][3] */
@@ -467,7 +471,7 @@ typedef struct AvnContactStep {
     uint32_t color_offsets[AVN_GRAPH_COLOR_COUNT + 1];
 } AvnContactStep;
 #define AVN_CONTACTS_TAKE_BROADPHASE_PAIRS 0x1u   /* add the new pairs of the context's last avn_broadphase_run (read in device memory) */
-#define AVN_CONTACTS_SHAPES_UNCHANGED 0x2u        /* input->shape and input->dims equal the previous call's: not copied again */
+#define AVN_CONTACTS_SHAPES_UNCHANGED 0x2u        /* input->shape and input->dims equal the previous call's: not copied again (nor checked) */
 /* One step of the contact pipeline on the device: (new pairs ->) rows, geometry + match_contacts for every live row, the status loop, the
  * graphs, the colour-major list.  input: the collider / body columns of AvnNarrowInput (pair arrays ignored).  From the first call on the
  * contact store's pair set is the broad phase's "existing pairs" set (AvnAabbColumns::existing_pairs may stay NULL). */
