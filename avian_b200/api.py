@@ -352,6 +352,10 @@ class AvnNarrowInput(C.Structure):
                            "aabb_min", "aabb_max")]
 
 
+class AvnBodyFrames(C.Structure):
+    _fields_ = [("body_count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("position", "rotation", "center_of_mass")]
+
+
 class AvnRawManifolds(C.Structure):
     _fields_ = [(n, _vp) for n in ("point_count", "disjoint", "normal", "anchor1", "anchor2", "penetration", "normal_speed")]
 
@@ -496,6 +500,7 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "contacts_download_impulses": ([_vp, C.c_uint32, _vp, _vp, _vp], C.c_int),
         "contacts_configure": ([_vp, P(AvnContactGraphConfig)], C.c_int),
         "contacts_step": ([_vp, P(AvnNarrowParams), P(AvnNarrowInput), C.c_uint32, C.c_double, C.c_uint32, P(AvnContactStep)], C.c_int),
+        "contacts_set_body_frames": ([_vp, P(AvnBodyFrames)], C.c_int),
         "solver_upload_resident": ([_vp, P(AvnStepParams), P(AvnBodyColumns), P(AvnJointSet)], C.c_int),
         "broadphase_download_order": ([_vp, P(C.c_uint64)], C.c_int),
         "contacts_download_graph": ([_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -539,7 +544,7 @@ ABI_SYMBOLS = [
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
     "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download", "avn_contacts_set_sensors", "avn_contacts_remove_colliders",
     "avn_contacts_events", "avn_contacts_report", "avn_islands_apply", "avn_islands_wake", "avn_contacts_download_sleeping",
-    "avn_move_and_slide"]
+    "avn_move_and_slide", "avn_contacts_set_body_frames"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
@@ -1071,6 +1076,22 @@ class Context:
         st = {n: int(getattr(out, n)) for n, _ in AvnContactStep._fields_ if n not in ("_pad", "color_offsets")}
         st["color_offsets"] = np.array(list(out.color_offsets), dtype=np.uint32)
         return st
+
+    def contacts_set_body_frames(self, position=None, rotation=None, center_of_mass=None, body_count: int | None = None) -> None:
+        """avn_contacts_set_body_frames: the body Position / Rotation ([B] rows, like the velocity columns) and local centre of mass (None = 0)
+        that every later contacts_step / narrow_phase measures its anchors from, until the next call.  position=None and rotation=None clear
+        them (a collider at its body's origin, the centre of mass at that origin).  body_count defaults to the rows of `position`."""
+        if position is None and rotation is None and center_of_mass is None and body_count is None:
+            self._keep_frames = None
+            self._check(self.lib.avn_contacts_set_body_frames(self.handle, None))
+            return
+        dt_ = self.scalar
+        col = lambda a, w: None if a is None else np.ascontiguousarray(a, dtype=dt_).reshape(-1, w)
+        pos, rot, com = col(position, 3), col(rotation, 4), col(center_of_mass, 3)
+        n = int(body_count if body_count is not None else (pos.shape[0] if pos is not None else 0))
+        f = AvnBodyFrames(n, 0, _ptr(pos), _ptr(rot), _ptr(com))
+        self._keep_frames = (pos, rot, com, f)
+        self._check(self.lib.avn_contacts_set_body_frames(self.handle, C.byref(f)))
 
     def solver_step_resident(self, params, bodies: Bodies, joints: JointSet | None = None) -> None:
         """avn_solver_upload_resident + run + download: manifolds AND constraint graph come from the contact store on the device."""

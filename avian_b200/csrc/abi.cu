@@ -227,7 +227,7 @@ AvnStatus avn_update_aabbs(AvnContext* ctx, const AvnAabbParams* params, AvnColl
 }
 
 AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, AvnRawManifolds* out) {
-    return guarded(ctx, [&] { return ctx->narrow->run(params, input, out); });
+    return guarded(ctx, [&] { return ctx->narrow->run(params, input, out, ctx->contacts->body_frames()); });
 }
 
 AvnStatus avn_contacts_configure(AvnContext* ctx, const AvnContactGraphConfig* config) { return guarded(ctx, [&] { return ctx->contacts->configure(config); }); }
@@ -239,6 +239,9 @@ AvnStatus avn_contacts_step(AvnContext* ctx, const AvnNarrowParams* params, cons
         // this step's collider / body columns start moving to the device before the broad phase is waited for; a shape column that is
         // going to be copied is checked first, so a refused step changes nothing
         if (params && input && out) {
+            const avn::BodyFrames* frames = ctx->contacts->body_frames();
+            if (frames && frames->body_count != input->body_count)
+                return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: the body frames have %u bodies, the input %u", frames->body_count, input->body_count);
             AvnStatus st = ctx->contacts->check_shapes(input, flags);
             if (st != AVN_OK) return st;
             st = ctx->contacts->prefetch_inputs(params, input, match_contacts, length_unit, flags);
@@ -256,6 +259,13 @@ AvnStatus avn_contacts_step(AvnContext* ctx, const AvnNarrowParams* params, cons
         ctx->contacts->pair_set(&table, &mask);
         ctx->broadphase->set_existing_device(table, mask);
         return AVN_OK;
+    });
+}
+AvnStatus avn_contacts_set_body_frames(AvnContext* ctx, const AvnBodyFrames* frames) {
+    return guarded(ctx, [&] {
+        if (frames && ctx->ccd->active())
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "contacts_set_body_frames: swept CCD is configured (avn_ccd_configure); it assumes a collider at its body's origin");
+        return ctx->contacts->set_body_frames(frames);
     });
 }
 AvnStatus avn_solver_upload_resident(AvnContext* ctx, const AvnStepParams* params, AvnBodyColumns* bodies, AvnJointSet* joints) {
@@ -356,6 +366,8 @@ AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
         if (config && config->count && ctx->contacts->has_capsule())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a capsule; capsule times of impact are not implemented");
+        if (config && config->count && ctx->contacts->body_frames())
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: body frames are set (avn_contacts_set_body_frames); swept CCD assumes a collider at its body's origin");
         avn::CcdRows rows;
         ctx->contacts->ccd_rows(&rows);
         return ctx->ccd->configure(config, rows);

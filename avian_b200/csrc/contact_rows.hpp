@@ -29,6 +29,28 @@ struct NarrowEdgeArgs {
 template <class S> NM_HD inline nm::V3 ldd3(const S* p, size_t i) { return {double(p[3 * i]), double(p[3 * i + 1]), double(p[3 * i + 2])}; }
 template <class S> NM_HD inline void std3(S* p, size_t i, nm::V3 v) { p[3 * i] = S(v.x); p[3 * i + 1] = S(v.y); p[3 * i + 2] = S(v.z); }
 
+// The body frames of avn_contacts_set_body_frames on the device (or over host arrays): [B] rows like the velocity columns.
+template <class S>
+struct BodyFrameCols { const S* pos; const S* rot; const S* com; };   // Position [B][3], Rotation [B][4], local centre of mass [B][3] (NULL = 0)
+
+// The frames of the pair (collider ca at pa on body ba, collider cb at pb on body bb).  rot * com is nm::rot, the expression tree of
+// avn::qrot (avn_math.cuh), which the solver's writeback uses for the same product, evaluated in double like the rest of the row.
+template <class S>
+NM_HD inline nm::PairFrames pair_frames(const BodyFrameCols<S>& f, uint32_t ba, nm::V3 pa, uint32_t bb, nm::V3 pb) {
+    nm::PairFrames fr;
+    fr.offset1 = pa - ldd3(f.pos, ba);
+    fr.offset2 = pb - ldd3(f.pos, bb);
+    fr.com1 = nm::V3{0, 0, 0};
+    fr.com2 = nm::V3{0, 0, 0};
+    if (f.com) {
+        const nm::Q q1{double(f.rot[4 * size_t(ba)]), double(f.rot[4 * size_t(ba) + 1]), double(f.rot[4 * size_t(ba) + 2]), double(f.rot[4 * size_t(ba) + 3])};
+        const nm::Q q2{double(f.rot[4 * size_t(bb)]), double(f.rot[4 * size_t(bb) + 1]), double(f.rot[4 * size_t(bb) + 2]), double(f.rot[4 * size_t(bb) + 3])};
+        fr.com1 = nm::rot(q1, ldd3(f.com, ba));
+        fr.com2 = nm::rot(q2, ldd3(f.com, bb));
+    }
+    return fr;
+}
+
 // A live row that names a capsule: the device runs it in a kernel of its own (narrow_capsule_edges_kernel), see nm::collide.
 template <class S>
 NM_HD inline bool capsule_row(const NarrowEdgeArgs<S>& a, int e) {
@@ -36,9 +58,10 @@ NM_HD inline bool capsule_row(const NarrowEdgeArgs<S>& a, int e) {
 }
 
 // geometry + match_contacts for every live row (same arithmetic as avh_raw_manifolds + avh_match_raw of the host fixture).  CAPSULES = false:
-// the row holds no capsule (the cuboid / sphere kernel).
-template <class S, bool CAPSULES = true>
-NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e) {
+// the row holds no capsule (the cuboid / sphere kernel).  FRAMES: the anchors are moved to the bodies' centres of mass by the frames `f`
+// (nm::manifold_points); without it `f` is not read and the row compiles to what it was before body frames existed.
+template <class S, bool CAPSULES = true, bool FRAMES = false>
+NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e, const BodyFrameCols<S>& f = BodyFrameCols<S>{}) {
     const EdgeRows<S>& r = a.r;
     if (r.asleep && r.asleep[e]) return;   // update_contacts runs over active_pairs only (narrow_phase/system_param.rs:437)
     if (!r.live[e]) { r.count[e] = 0; r.disjoint[e] = 0; return; }
@@ -62,9 +85,10 @@ NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e) {
         const double max_dist = nm::smax(eff_margin, a.tol);
         nm::Contacts pts;
         const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
-        if (nm::collide<CAPSULES>(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts))
-            np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
-        else
+        if (nm::collide<CAPSULES>(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts)) {
+            if (FRAMES) np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, pair_frames(f, ba, pa, bb, pb), out);
+            else np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
+        } else
             normal = nm::V3{0, 0, 0};
     }
     // match_contacts against the manifold of the previous step: the impulses the last solve left (ws_*_out) move to the matching new points

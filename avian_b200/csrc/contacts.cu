@@ -476,6 +476,20 @@ __global__ void __launch_bounds__(128) narrow_capsule_edges_kernel(const __grid_
     narrow_edge_row<S, true>(a, e);
 }
 
+// with body frames (avn_contacts_set_body_frames) these two replace the pair above: the same rows, anchors relative to the centres of mass
+template <class S, bool CAPSULES>
+__global__ void __launch_bounds__(128) narrow_framed_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, const BodyFrameCols<S> f, uint8_t* fresh,
+                                                                  int only_fresh, int capsules) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.r.E) return;
+    if (capsules && capsule_row(a, e) != CAPSULES) return;
+    if (only_fresh) {
+        if (!fresh[e]) return;
+        fresh[e] = 0;
+    }
+    narrow_edge_row<S, CAPSULES, true>(a, e, f);
+}
+
 
 // =====================================================================================================================================
 // Persistent simulation islands + sleeping (SURVEY.md 8f #4; dynamics/solver/islands/mod.rs, islands/sleeping.rs).
@@ -1066,6 +1080,23 @@ class Contacts final : public ContactsBase {
         return AVN_OK;
     }
     bool has_capsule() const override { return has_capsule_; }
+    AvnStatus set_body_frames(const AvnBodyFrames* f) override {
+        if (!f) { frames_set_ = false; return AVN_OK; }
+        if (!f->position || !f->rotation)
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_set_body_frames: position and rotation are required");
+        const size_t B = f->body_count;
+        frames_.body_count = f->body_count;
+        auto copy = [&](std::vector<unsigned char>& dst, const void* src, size_t n) {
+            dst.resize(src ? n * sizeof(S) : 0);
+            if (src && n) memcpy(dst.data(), src, n * sizeof(S));
+        };
+        copy(frames_.position, f->position, 3 * B);
+        copy(frames_.rotation, f->rotation, 4 * B);
+        copy(frames_.com, f->center_of_mass, 3 * B);
+        frames_set_ = true;
+        return AVN_OK;
+    }
+    const BodyFrames* body_frames() const override { return frames_set_ ? &frames_ : nullptr; }
     void pair_set(const uint64_t** table, uint64_t* mask) override {
         *table = (configured_ && table_.p && !table_dirty_) ? table_.as<uint64_t>() : nullptr;
         *mask = table_mask_;
@@ -1385,6 +1416,12 @@ class Contacts final : public ContactsBase {
         UPC(i_av_, in->angular_velocity, 3 * B, S, in_.av);
         UPC(i_amin_, in->aabb_min, 3 * C, S, in_.amin);
         UPC(i_amax_, in->aabb_max, 3 * C, S, in_.amax);
+        in_.framed = frames_set_;
+        if (frames_set_) {
+            UPC(i_fpos_, frames_.position.data(), 3 * B, S, in_.frames.pos);
+            UPC(i_frot_, frames_.rotation.data(), 4 * B, S, in_.frames.rot);
+            UPC(i_fcom_, frames_.com.empty() ? nullptr : frames_.com.data(), 3 * B, S, in_.frames.com);
+        }
 #undef UPC
         up_stream_ = stream_;
         in_.colliders = C;
@@ -1404,7 +1441,12 @@ class Contacts final : public ContactsBase {
         }
         prefetched_ = nullptr;
         early_rows_ = 0;
-        return enqueue_narrow(prm, match_contacts, length_unit, n, stream_, only_fresh);
+        AvnStatus st = enqueue_narrow(prm, match_contacts, length_unit, n, stream_, only_fresh);
+        // a full pass has computed the rows added this step too: they are no longer fresh.  Left set, the next step's fresh pass would run
+        // them a second time after its early pass, matching their new points against themselves (visible once two points of one manifold
+        // lie within the matching distance of each other, e.g. the corners of a thin table leg)
+        if (st == AVN_OK && !only_fresh && n) AVN_CUDA(cudaMemsetAsync(fresh_.p, 0, n, stream_));
+        return st;
     }
     AvnStatus enqueue_narrow(const AvnNarrowParams* prm, uint32_t match_contacts, double length_unit, uint32_t n, cudaStream_t s, bool only_fresh) {
         NarrowEdgeArgs<S> a{};
@@ -1415,8 +1457,13 @@ class Contacts final : public ContactsBase {
         a.tol = prm->contact_tolerance;
         a.thr2 = (0.1 * length_unit) * (0.1 * length_unit);
         a.match = match_contacts ? 1 : 0;
-        narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
-        if (has_capsule_) narrow_capsule_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0);
+        if (in_.framed) {
+            narrow_framed_edges_kernel<S, false><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
+            if (has_capsule_) narrow_framed_edges_kernel<S, true><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, 1);
+        } else {
+            narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
+            if (has_capsule_) narrow_capsule_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0);
+        }
         AVN_CUDA(cudaGetLastError());
         return AVN_OK;
     }
@@ -1617,12 +1664,15 @@ class Contacts final : public ContactsBase {
     cudaEvent_t ev_in_ = nullptr;
     const AvnNarrowInput* prefetched_ = nullptr;
     struct { const uint8_t* shape = nullptr; const S* dims = nullptr; const S* pos = nullptr; const S* rot = nullptr; const S* lv = nullptr; const S* av = nullptr;
-             const S* amin = nullptr; const S* amax = nullptr; size_t colliders = 0; } in_;
+             const S* amin = nullptr; const S* amax = nullptr; size_t colliders = 0;
+             bool framed = false; BodyFrameCols<S> frames{}; } in_;   // framed: the body frames below were copied with these columns
     ErrorSink* err_;
     uint32_t E_ = 0;
     DevBuf c1_, c2_, b1_, b2_, live_, count_, disjoint_, normal_, a1_, a2_, pen_, ns_, prev_count_, prev_a1_, prev_a2_, ws_n_in_, ws_t_in_, ws_n_out_, ws_t_out_,
         nimp_in_, nimp_out_, stage_;
-    DevBuf i_shape_, i_dims_, i_pos_, i_rot_, i_lv_, i_av_, i_amin_, i_amax_;
+    DevBuf i_shape_, i_dims_, i_pos_, i_rot_, i_lv_, i_av_, i_amin_, i_amax_, i_fpos_, i_frot_, i_fcom_;
+    BodyFrames frames_;           // avn_contacts_set_body_frames (host copy), in effect while frames_set_
+    bool frames_set_ = false;
     // graphs
     using ResidentGraph = ContactsBase::ResidentGraph;
     DevBuf isl_event_, fresh_, isl_buf_, isl_in_, isl_out_, isl_j_;

@@ -137,9 +137,17 @@ struct AabbBase {
 };
 AabbBase* make_aabb_updater(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
+// The body frames of avn_contacts_set_body_frames: a host copy of the caller's columns in the column scalar, which every later
+// avn_contacts_step / avn_narrow_phase uses until the next call (the contact store keeps it).
+struct BodyFrames {
+    uint32_t body_count = 0;
+    std::vector<unsigned char> position, rotation, com;   // [B][3], [B][4], [B][3] scalars; com empty = 0
+};
+
 struct NarrowBase {
     virtual ~NarrowBase() {}
-    virtual AvnStatus run(const AvnNarrowParams* prm, const AvnNarrowInput* in, AvnRawManifolds* out) = 0;
+    // frames: NULL = a collider at its body's origin, the centre of mass at that origin
+    virtual AvnStatus run(const AvnNarrowParams* prm, const AvnNarrowInput* in, AvnRawManifolds* out, const BodyFrames* frames) = 0;
 };
 NarrowBase* make_narrow(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
@@ -210,6 +218,9 @@ struct ContactsBase {
     //      any state changes; has_capsule: the column of the last accepted step holds a capsule (swept CCD refuses capsules)
     virtual AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) = 0;
     virtual bool has_capsule() const = 0;
+    // ---- body frames (avn_contacts_set_body_frames): checked and copied on the host (NULL clears them); body_frames() = NULL when none are set
+    virtual AvnStatus set_body_frames(const AvnBodyFrames* frames) = 0;
+    virtual const BodyFrames* body_frames() const = 0;
 };
 ContactsBase* make_contacts(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 

@@ -5,7 +5,7 @@
 // (tests/test_gpu_narrow.py).  One thread per pair: 128 registers and a 1.8 KB local frame for the clipped polygon (ptxas figures in DESIGN.md §7); 2 poses + 2 velocities
 // in (≈ 150 B), ≤ 4 points out (≈ 150 B): a streaming kernel, HBM/L2-bound by the gathers of the pose rows.
 #include "context.hpp"
-#include "narrow_math.hpp"
+#include "contact_rows.hpp"
 
 namespace avn {
 namespace {
@@ -26,8 +26,9 @@ template <class S> __device__ __forceinline__ void st3(S* p, size_t i, nm::V3 v)
 
 // One thread per pair.  CAPSULES = false (narrow_phase_kernel): the cuboid / sphere pairs, and when `capsules` is set the pairs with a
 // capsule are skipped; CAPSULES = true (narrow_capsule_kernel, launched only for a shape column that holds a capsule): those pairs alone.
-template <class S, bool CAPSULES>
-__device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules) {
+// FRAMES (narrow_framed_kernel, launched instead of the two when body frames are set): anchors relative to the bodies' centres of mass.
+template <class S, bool CAPSULES, bool FRAMES = false>
+__device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules, const BodyFrameCols<S>& f = BodyFrameCols<S>{}) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.n) return;
     const uint32_t ca = a.c1[k], cb = a.c2[k], ba = a.b1[k], bb = a.b2[k];
@@ -53,7 +54,8 @@ __device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules
     const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
     if (!nm::collide<CAPSULES>(ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts)) return;
     nm::PointOut out[4];
-    const int np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
+    const int np = FRAMES ? nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, pair_frames(f, ba, pa, bb, pb), out)
+                          : nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
     a.count[k] = uint8_t(np);
     st3(a.normal, k, normal);
     for (int p = 0; p < np; ++p) {
@@ -68,12 +70,16 @@ template <class S>
 __global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant__ NarrowArgs<S> a, int capsules) { narrow_pair<S, false>(a, capsules); }
 template <class S>
 __global__ void __launch_bounds__(128) narrow_capsule_kernel(const __grid_constant__ NarrowArgs<S> a) { narrow_pair<S, true>(a, 1); }
+template <class S, bool CAPSULES>
+__global__ void __launch_bounds__(128) narrow_framed_kernel(const __grid_constant__ NarrowArgs<S> a, const BodyFrameCols<S> f, int capsules) {
+    narrow_pair<S, CAPSULES, true>(a, capsules, f);
+}
 
 template <class S>
 class Narrow final : public NarrowBase {
    public:
     Narrow(cudaStream_t stream, ErrorSink* err) : stream_(stream), err_(err) {}
-    AvnStatus run(const AvnNarrowParams* prm, const AvnNarrowInput* in, AvnRawManifolds* out) override {
+    AvnStatus run(const AvnNarrowParams* prm, const AvnNarrowInput* in, AvnRawManifolds* out, const BodyFrames* frames) override {
         if (!prm || !in || !out) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "params, input and output are required");
         const size_t n = in->pair_count, C = in->collider_count, B = in->body_count;
         if (n == 0) return AVN_OK;
@@ -83,6 +89,8 @@ class Narrow final : public NarrowBase {
         if (!out->point_count || !out->normal || !out->anchor1 || !out->anchor2 || !out->penetration || !out->normal_speed)
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: every output column except disjoint is required");
         if ((in->aabb_min == nullptr) != (in->aabb_max == nullptr)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: aabb_min and aabb_max go together");
+        if (frames && frames->body_count != B)
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: the body frames have %u bodies, the input %zu", frames->body_count, B);
         for (size_t k = 0; k < n; ++k)
             if (in->collider1[k] >= C || in->collider2[k] >= C || in->body1[k] >= B || in->body2[k] >= B)
                 return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: pair %zu indexes past the collider / body columns", k);
@@ -106,6 +114,12 @@ class Narrow final : public NarrowBase {
         UPN(i_av_, in->angular_velocity, 3 * B, S, a.av);
         UPN(i_amin_, in->aabb_min, 3 * C, S, a.amin);
         UPN(i_amax_, in->aabb_max, 3 * C, S, a.amax);
+        BodyFrameCols<S> f{};
+        if (frames) {
+            UPN(i_fpos_, frames->position.data(), 3 * B, S, f.pos);
+            UPN(i_frot_, frames->rotation.data(), 4 * B, S, f.rot);
+            if (!frames->com.empty()) UPN(i_fcom_, frames->com.data(), 3 * B, S, f.com);
+        }
 #undef UPN
         AVN_CUDA(o_cnt_.ensure(n));
         AVN_CUDA(o_dis_.ensure(n));
@@ -124,8 +138,13 @@ class Narrow final : public NarrowBase {
         AVN_CUDA(cudaMemsetAsync(a.anchor2, 0, 12 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.penetration, 0, 4 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.normal_speed, 0, 4 * n * sizeof(S), stream_));
-        narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, capsules ? 1 : 0);
-        if (capsules) narrow_capsule_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a);
+        if (frames) {
+            narrow_framed_kernel<S, false><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, capsules ? 1 : 0);
+            if (capsules) narrow_framed_kernel<S, true><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, 1);
+        } else {
+            narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, capsules ? 1 : 0);
+            if (capsules) narrow_capsule_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a);
+        }
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->point_count, a.count, n, cudaMemcpyDeviceToHost, stream_));
         if (out->disjoint) AVN_CUDA(cudaMemcpyAsync(out->disjoint, a.disjoint, n, cudaMemcpyDeviceToHost, stream_));
@@ -149,7 +168,7 @@ class Narrow final : public NarrowBase {
     }
     cudaStream_t stream_;
     ErrorSink* err_;
-    DevBuf i_c1_, i_c2_, i_b1_, i_b2_, i_shape_, i_dims_, i_pos_, i_rot_, i_lv_, i_av_, i_amin_, i_amax_;
+    DevBuf i_c1_, i_c2_, i_b1_, i_b2_, i_shape_, i_dims_, i_pos_, i_rot_, i_lv_, i_av_, i_amin_, i_amax_, i_fpos_, i_frot_, i_fcom_;
     DevBuf o_cnt_, o_dis_, o_nrm_, o_a1_, o_a2_, o_pen_, o_ns_;
 };
 

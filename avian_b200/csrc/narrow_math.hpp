@@ -564,19 +564,30 @@ NM_HD inline bool collide(int type_a, V3 he_a, V3 pa, Q qa, int type_b, V3 he_b,
     return hit;
 }
 
-// A manifold point as the solver's input columns want it (ContactPoint, contact_types/mod.rs:603-660): anchors relative to the body
-// origins (collider at the body origin, centre of mass at the origin), penetration, normal speed.
+// A manifold point as the solver's input columns want it (ContactPoint, contact_types/mod.rs:603-660): anchors relative to each body's
+// centre of mass, penetration, normal speed.  Without body frames a collider sits at its body's origin and the centre of mass at that origin.
 struct PointOut { V3 anchor1, anchor2; S penetration, normal_speed; };
+
+// The body frames of a pair (update_contacts, narrow_phase/system_param.rs:540-570): offset = collider position - body position,
+// com = body rotation * local centre of mass.
+struct PairFrames { V3 offset1, com1, offset2, com2; };
 
 // From the witness pairs of collide (relative to pa) to the manifold's points: the speculative keep rule of
 // narrow_phase/system_param.rs:748-756.  rel = v2 - v1, eff_margin = dt * |rel| (margin = MAX).  Returns the number of points written
-// to out[0..4).
-NM_HD inline int manifold_points(const Contacts& pts, V3 normal, V3 pa, V3 pb, V3 rel, V3 w1, V3 w2, S dt, S eff_margin, PointOut out[4]) {
+// to out[0..4).  FRAMES: every anchor is moved from its collider to its body's centre of mass, (anchor + offset) - com in the reference's
+// order (system_param.rs:731-735), before the normal speed and the keep rule read it.
+template <bool FRAMES>
+NM_HD inline int manifold_points_in(const Contacts& pts, V3 normal, V3 pa, V3 pb, V3 rel, V3 w1, V3 w2, S dt, S eff_margin, const PairFrames* fr,
+                                    PointOut out[4]) {
     int m = 0;
     for (int k = 0; k < pts.n && m < 4; ++k) {
         PointOut pt;
         pt.anchor1 = pts.p[k].a;
         pt.anchor2 = pts.p[k].b - (pb - pa);
+        if (FRAMES) {
+            pt.anchor1 = (pt.anchor1 + fr->offset1) - fr->com1;
+            pt.anchor2 = (pt.anchor2 + fr->offset2) - fr->com2;
+        }
         pt.penetration = dot(pts.p[k].a - pts.p[k].b, normal);
         V3 rv = rel + cross(w2, pt.anchor2) - cross(w1, pt.anchor1);
         pt.normal_speed = dot(rv, normal);
@@ -585,6 +596,13 @@ NM_HD inline int manifold_points(const Contacts& pts, V3 normal, V3 pa, V3 pb, V
         out[m++] = pt;
     }
     return m;
+}
+NM_HD inline int manifold_points(const Contacts& pts, V3 normal, V3 pa, V3 pb, V3 rel, V3 w1, V3 w2, S dt, S eff_margin, PointOut out[4]) {
+    return manifold_points_in<false>(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin, nullptr, out);
+}
+NM_HD inline int manifold_points(const Contacts& pts, V3 normal, V3 pa, V3 pb, V3 rel, V3 w1, V3 w2, S dt, S eff_margin, const PairFrames& fr,
+                                 PointOut out[4]) {
+    return manifold_points_in<true>(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin, &fr, out);
 }
 
 // ContactManifold::match_contacts with unknown feature ids (contact_types/mod.rs:426-470): a new point inherits the warm-start impulses

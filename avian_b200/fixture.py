@@ -30,11 +30,11 @@ def _load():
         lib.avh_existing_pairs.argtypes = [_vp, _vp, C.c_uint64]
         lib.avh_existing_pairs.restype = C.c_uint64
         lib.avh_add_pairs.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64]
-        lib.avh_narrow_phase.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_uint32, C.POINTER(C.c_uint32)]
+        lib.avh_narrow_phase.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_uint32, C.POINTER(C.c_uint32), _vp, _vp, _vp]
         lib.avh_narrow_phase.restype = C.c_uint32
         lib.avh_export_manifolds.argtypes = [_vp, C.c_uint32] + [_vp] * 13
         lib.avh_store_impulses.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp]
-        lib.avh_raw_manifolds.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 12 + [C.c_double, C.c_double] + [_vp] * 9
+        lib.avh_raw_manifolds.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 12 + [C.c_double, C.c_double] + [_vp] * 12
         lib.avh_active_edges.argtypes = [_vp] * 6
         lib.avh_active_edges.restype = C.c_uint32
         lib.avh_export_edges.argtypes = [_vp] * 7
@@ -43,6 +43,8 @@ def _load():
         lib.avh_match_raw.restype = None
         lib.avh_rows_narrow.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 27 + [C.c_double, C.c_double, C.c_double, C.c_uint32]
         lib.avh_rows_narrow.restype = None
+        lib.avh_rows_narrow_framed.argtypes = lib.avh_rows_narrow.argtypes + [_vp] * 3
+        lib.avh_rows_narrow_framed.restype = None
         lib.avh_raw_manifolds.restype = None
         lib.avh_remove_colliders.argtypes = [_vp, C.c_uint32, _vp]
         lib.avh_remove_colliders.restype = None
@@ -97,12 +99,25 @@ def _p(a):
     return None if a is None else a.ctypes.data
 
 
+def body_frame_columns(scalar, frames: dict | None):
+    """(position, rotation, center_of_mass) of a body-frames dict (api.Context.contacts_set_body_frames' columns) in the column scalar;
+    (None, None, None) without frames."""
+    if frames is None:
+        return None, None, None
+    dt_ = np.dtype(scalar)
+    col = lambda k, w: None if frames.get(k) is None else np.ascontiguousarray(frames[k], dtype=dt_).reshape(-1, w)
+    return col("position", 3), col("rotation", 4), col("center_of_mass", 3)
+
+
 def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders: dict, lin_vel: np.ndarray, ang_vel: np.ndarray,
-                  f64_anchors: bool = False) -> dict:
+                  f64_anchors: bool = False, frames: dict | None = None) -> dict:
     """The geometry stage of the fixture's narrow phase for an explicit pair list (same columns as Context.narrow_phase).
-    f64_anchors adds the unrounded anchors (what match_contacts compares on the next step)."""
+    f64_anchors adds the unrounded anchors (what match_contacts compares on the next step).  frames: the body frames (dict position,
+    rotation, center_of_mass=None, [B] rows), as Context.contacts_set_body_frames sets them; the anchors are then relative to the bodies'
+    centres of mass."""
     lib = _load()
     dt_ = np.dtype(scalar)
+    fp, fr, fc = body_frame_columns(dt_, frames)
     c1, c2, b1, b2 = (np.ascontiguousarray(x, dtype=np.uint32) for x in pairs)
     n = int(c1.shape[0])
     cols = {k: (None if colliders.get(k) is None else np.ascontiguousarray(colliders[k], dtype=(np.uint8 if k == "shape" else dt_)))
@@ -115,7 +130,8 @@ def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders:
     a2d = np.zeros((n, 4, 3), dtype=np.float64) if f64_anchors else None
     lib.avh_raw_manifolds(32 if dt_ == np.float32 else 64, n, _p(c1), _p(c2), _p(b1), _p(b2), _p(cols["shape"]), _p(cols["dims"]), _p(cols["position"]),
                           _p(cols["rotation"]), _p(lv), _p(av), _p(cols["aabb_min"]), _p(cols["aabb_max"]), float(dt), float(contact_tolerance),
-                          *(_p(out[k]) for k in ("point_count", "disjoint", "normal", "anchor1", "anchor2", "penetration", "normal_speed")), _p(a1d), _p(a2d))
+                          *(_p(out[k]) for k in ("point_count", "disjoint", "normal", "anchor1", "anchor2", "penetration", "normal_speed")), _p(a1d), _p(a2d),
+                          _p(fp), _p(fr), _p(fc))
     if f64_anchors:
         out["anchor1_f64"], out["anchor2_f64"] = a1d, a2d
     return out
@@ -263,11 +279,14 @@ def move_contact(scalar, shape_a: int, dims_a, pos_a, rot_a, shape_b: int, dims_
 
 
 class HostPipeline:
-    """Contact graph + narrow-phase fixture + constraint graph for a fixed set of bodies (one collider per body,
-    collider Entity::index() == body Entity::index() == row in the body columns)."""
+    """Contact graph + narrow-phase fixture + constraint graph for a fixed set of colliders.  Without collider_body: one collider per body,
+    collider Entity::index() == body Entity::index() == row in the body columns.  collider_body ([C], a collider table): the body of every
+    collider; the AABB update and the narrow phase then take the colliders' world poses (and their velocities) separately."""
 
-    def __init__(self, shape_type: np.ndarray, dims: np.ndarray, friction: np.ndarray, restitution: np.ndarray, scalar=np.float32):
+    def __init__(self, shape_type: np.ndarray, dims: np.ndarray, friction: np.ndarray, restitution: np.ndarray, scalar=np.float32,
+                 collider_body: np.ndarray | None = None):
         self.lib = _load()
+        self.collider_body = None if collider_body is None else np.ascontiguousarray(collider_body, dtype=np.uint32)
         self.n = int(shape_type.shape[0])
         self.scalar = np.dtype(scalar)
         self.bits = 32 if self.scalar == np.float32 else 64
@@ -284,25 +303,30 @@ class HostPipeline:
             self.lib.avh_destroy(self.h)
             self.h = None
 
-    def update_aabbs(self, bodies: api.Bodies, dt: float):
+    def update_aabbs(self, bodies: api.Bodies, dt: float, colliders: dict | None = None):
+        """colliders (a collider table): dict position, rotation, linear_velocity, angular_velocity per collider; None = the body columns."""
         mn = np.empty((self.n, 3), dtype=self.scalar)
         mx = np.empty((self.n, 3), dtype=self.scalar)
-        self.lib.avh_update_aabbs(self.h, self.bits, _p(bodies.position), _p(bodies.rotation), _p(bodies.linear_velocity),
-                                  _p(bodies.angular_velocity), dt, _p(mn), _p(mx))
+        c = {"position": bodies.position, "rotation": bodies.rotation, "linear_velocity": bodies.linear_velocity, "angular_velocity": bodies.angular_velocity}
+        if colliders is not None:
+            c = {k: np.ascontiguousarray(colliders[k], dtype=self.scalar) for k in c}
+        self.lib.avh_update_aabbs(self.h, self.bits, _p(c["position"]), _p(c["rotation"]), _p(c["linear_velocity"]), _p(c["angular_velocity"]), dt,
+                                  _p(mn), _p(mx))
         return mn, mx
 
     def intervals(self, bodies: api.Bodies, aabb_min: np.ndarray, aabb_max: np.ndarray, with_existing: bool = True) -> api.Aabbs:
         """AabbIntervals in the persistent order + the pair set, as the broad phase's input columns."""
         order = np.empty(self.n, dtype=np.uint32)
         self.lib.avh_get_order(self.h, _p(order))
-        flags = np.where(bodies.kind[order] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
+        body = order.copy() if self.collider_body is None else np.ascontiguousarray(self.collider_body[order])
+        flags = np.where(bodies.kind[body] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
         existing = None
         if with_existing:
             cnt = int(self.lib.avh_existing_pairs(self.h, None, 0))
             if cnt:
                 existing = np.empty(cnt, dtype=np.uint64)
                 self.lib.avh_existing_pairs(self.h, _p(existing), cnt)
-        return api.Aabbs(collider=order.copy(), body=order.copy(), aabb_min=np.ascontiguousarray(aabb_min[order]),
+        return api.Aabbs(collider=order.copy(), body=body, aabb_min=np.ascontiguousarray(aabb_min[order]),
                          aabb_max=np.ascontiguousarray(aabb_max[order]), flags=np.ascontiguousarray(flags),
                          order_out=np.empty(self.n, dtype=np.uint32), existing_pairs=existing)
 
@@ -315,11 +339,20 @@ class HostPipeline:
             c1, c2, b1, b2, fl = (np.ascontiguousarray(x[:n]) for x in (pairs.collider1, pairs.collider2, pairs.body1, pairs.body2, pairs.flags))
             self.lib.avh_add_pairs(self.h, _p(c1), _p(c2), _p(b1), _p(b2), _p(fl), n)
 
-    def narrow_phase(self, bodies: api.Bodies, aabb_min: np.ndarray, aabb_max: np.ndarray, dt: float, match_contacts: bool = True) -> api.Manifolds:
+    def narrow_phase(self, bodies: api.Bodies, aabb_min: np.ndarray, aabb_max: np.ndarray, dt: float, match_contacts: bool = True,
+                     colliders: dict | None = None) -> api.Manifolds:
+        """colliders: the collider table's world poses (dict position, rotation, [C] rows); the anchors are then relative to the bodies'
+        centres of mass (bodies.position / rotation / center_of_mass are the body frames).  None: one collider per body."""
         pts = C.c_uint32(0)
         kind = np.ascontiguousarray(bodies.kind, dtype=np.uint8)
-        m = int(self.lib.avh_narrow_phase(self.h, self.bits, _p(kind), _p(bodies.position), _p(bodies.rotation), _p(bodies.linear_velocity),
-                                          _p(bodies.angular_velocity), _p(aabb_min), _p(aabb_max), dt, 1 if match_contacts else 0, C.byref(pts)))
+        if colliders is None:
+            pos, rot, frames = bodies.position, bodies.rotation, (None, None, None)
+        else:
+            pos, rot = (np.ascontiguousarray(colliders[k], dtype=self.scalar) for k in ("position", "rotation"))
+            frames = body_frame_columns(self.scalar, {"position": bodies.position, "rotation": bodies.rotation, "center_of_mass": bodies.center_of_mass})
+        m = int(self.lib.avh_narrow_phase(self.h, self.bits, _p(kind), _p(pos), _p(rot), _p(bodies.linear_velocity),
+                                          _p(bodies.angular_velocity), _p(aabb_min), _p(aabb_max), dt, 1 if match_contacts else 0, C.byref(pts),
+                                          *(_p(f) for f in frames)))
         return self.export_manifolds(m, int(pts.value))
 
     def export_manifolds(self, m: int | None = None, p: int | None = None) -> api.Manifolds:

@@ -154,7 +154,8 @@ template <class T>
 static void rows_narrow(uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* live, uint8_t* count, uint8_t* disjoint, void* normal, void* a1,
                         void* a2, void* pen, void* ns, uint8_t* prev_count, double* prev_a1, double* prev_a2, void* ws_n_in, void* ws_t_in, void* ws_n_out,
                         void* ws_t_out, const uint8_t* shape, const void* dims, const void* pos, const void* rot, const void* lv, const void* av,
-                        const void* amin, const void* amax, double dt, double tol, double length_unit, uint32_t match) {
+                        const void* amin, const void* amax, double dt, double tol, double length_unit, uint32_t match, const void* body_pos = nullptr,
+                        const void* body_rot = nullptr, const void* body_com = nullptr) {
     avn::NarrowEdgeArgs<T> a{};
     a.r.E = int(E);
     a.r.c1 = c1; a.r.c2 = c2; a.r.b1 = b1; a.r.b2 = b2; a.r.live = live; a.r.count = count; a.r.disjoint = disjoint;
@@ -165,7 +166,19 @@ static void rows_narrow(uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, ui
     a.shape = shape; a.dims = static_cast<const T*>(dims); a.pos = static_cast<const T*>(pos); a.rot = static_cast<const T*>(rot);
     a.lv = static_cast<const T*>(lv); a.av = static_cast<const T*>(av); a.amin = static_cast<const T*>(amin); a.amax = static_cast<const T*>(amax);
     a.dt = dt; a.tol = tol; a.thr2 = (0.1 * length_unit) * (0.1 * length_unit); a.match = match ? 1 : 0;
-    for (uint32_t e = 0; e < E; ++e) avn::narrow_edge_row<T>(a, int(e));
+    const avn::BodyFrameCols<T> f{static_cast<const T*>(body_pos), static_cast<const T*>(body_rot), static_cast<const T*>(body_com)};
+    for (uint32_t e = 0; e < E; ++e) {
+        if (body_pos) avn::narrow_edge_row<T, true, true>(a, int(e), f);
+        else avn::narrow_edge_row<T>(a, int(e));
+    }
+}
+
+// The body frames of a pair over host columns in either scalar (what contact_rows.hpp's pair_frames computes from device columns)
+nm::PairFrames host_pair_frames(bool f64, const void* body_pos, const void* body_rot, const void* body_com, uint32_t ba, V3 pa, uint32_t bb, V3 pb) {
+    if (f64) return avn::pair_frames(avn::BodyFrameCols<double>{static_cast<const double*>(body_pos), static_cast<const double*>(body_rot),
+                                                                static_cast<const double*>(body_com)}, ba, pa, bb, pb);
+    return avn::pair_frames(avn::BodyFrameCols<float>{static_cast<const float*>(body_pos), static_cast<const float*>(body_rot),
+                                                      static_cast<const float*>(body_com)}, ba, pa, bb, pb);
 }
 
 }  // namespace
@@ -461,7 +474,8 @@ uint32_t avh_report(AvhPipeline* h, uint32_t scalar_bits, uint32_t events_only, 
 // NarrowPhase::update (narrow_phase/system_param.rs:114-400) with the fixture manifold generator.
 // kind[n] = AvnBodyKind.  Returns the number of exported manifolds; *out_points = number of points.
 uint32_t avh_narrow_phase(AvhPipeline* h, uint32_t scalar_bits, const uint8_t* kind, const void* position, const void* rotation, const void* linvel,
-                          const void* angvel, const void* aabb_min, const void* aabb_max, double dt, uint32_t match_contacts, uint32_t* out_points) {
+                          const void* angvel, const void* aabb_min, const void* aabb_max, double dt, uint32_t match_contacts, uint32_t* out_points,
+                          const void* body_pos, const void* body_rot, const void* body_com) {
     Pipeline& P = *reinterpret_cast<Pipeline*>(h);
     const bool f64 = scalar_bits == 64;
     Col pos{position, f64}, rt{rotation, f64}, lv{linvel, f64}, av{angvel, f64}, amin{aabb_min, f64}, amax{aabb_max, f64};
@@ -492,7 +506,9 @@ uint32_t avh_narrow_phase(AvhPipeline* h, uint32_t scalar_bits, const uint8_t* k
         const bool hit = collide(sa.type, sa.he, pa, rt.q(a), sb.type, sb.he, pb, rt.q(b), max_dist, normal, pts);
         if (hit) {
             PointOut out[4];
-            const int np = manifold_points(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin, out);
+            const int np = body_pos ? manifold_points(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin,
+                                                      host_pair_frames(f64, body_pos, body_rot, body_com, pr.body1, pa, pr.body2, pb), out)
+                                    : manifold_points(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin, out);
             if (np > 0) {
                 Manifold m;
                 m.normal = normal;
@@ -584,7 +600,8 @@ void avh_store_impulses(AvhPipeline* h, uint32_t scalar_bits, const void* ws_nor
 void avh_raw_manifolds(uint32_t scalar_bits, uint32_t pair_count, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2,
                        const uint8_t* shape, const void* dims, const void* position, const void* rotation, const void* linvel, const void* angvel,
                        const void* aabb_min, const void* aabb_max, double dt, double tol, uint8_t* point_count, uint8_t* disjoint, void* normal,
-                       void* anchor1, void* anchor2, void* penetration, void* normal_speed, double* anchor1_f64, double* anchor2_f64) {
+                       void* anchor1, void* anchor2, void* penetration, void* normal_speed, double* anchor1_f64, double* anchor2_f64, const void* body_pos,
+                       const void* body_rot, const void* body_com) {
     const bool f64 = scalar_bits == 64;
     Col dm{dims, f64}, pos{position, f64}, rt{rotation, f64}, lv{linvel, f64}, av{angvel, f64}, amin{aabb_min, f64}, amax{aabb_max, f64};
     ColW on{normal, f64}, oa1{anchor1, f64}, oa2{anchor2, f64}, op{penetration, f64}, os{normal_speed, f64};
@@ -611,7 +628,8 @@ void avh_raw_manifolds(uint32_t scalar_bits, uint32_t pair_count, const uint32_t
         int ta = shape ? shape[a] : SHAPE_CUBOID, tb = shape ? shape[b] : SHAPE_CUBOID;
         if (!collide(ta, dm.v3(a), pa, rt.q(a), tb, dm.v3(b), pb, rt.q(b), max_dist, nrm, pts)) continue;
         PointOut out[4];
-        int np = manifold_points(pts, nrm, pa, pb, rel, w1, w2, dt, eff_margin, out);
+        int np = body_pos ? manifold_points(pts, nrm, pa, pb, rel, w1, w2, dt, eff_margin, host_pair_frames(f64, body_pos, body_rot, body_com, b1[k], pa, b2[k], pb), out)
+                          : manifold_points(pts, nrm, pa, pb, rel, w1, w2, dt, eff_margin, out);
         point_count[k] = uint8_t(np);
         on.set3(k, nrm);
         for (int p = 0; p < np; ++p) {
@@ -708,6 +726,19 @@ void avh_rows_narrow(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c
     else
         rows_narrow<float>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
                            shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match);
+}
+// avh_rows_narrow with body frames: body_pos [B][3], body_rot [B][4], body_com [B][3] (NULL = 0) in the column scalar
+void avh_rows_narrow_framed(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* live, uint8_t* count,
+                            uint8_t* disjoint, void* normal, void* a1, void* a2, void* pen, void* ns, uint8_t* prev_count, double* prev_a1, double* prev_a2,
+                            void* ws_n_in, void* ws_t_in, void* ws_n_out, void* ws_t_out, const uint8_t* shape, const void* dims, const void* pos,
+                            const void* rot, const void* lv, const void* av, const void* amin, const void* amax, double dt, double tol, double length_unit,
+                            uint32_t match, const void* body_pos, const void* body_rot, const void* body_com) {
+    if (scalar_bits == 64)
+        rows_narrow<double>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
+                            shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match, body_pos, body_rot, body_com);
+    else
+        rows_narrow<float>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
+                           shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match, body_pos, body_rot, body_com);
 }
 
 uint32_t avh_pair_count(AvhPipeline* h) { return uint32_t(reinterpret_cast<Pipeline*>(h)->active.size()); }

@@ -86,7 +86,11 @@ class SpatialQueryPlugin:
 
     @staticmethod
     def colliders(world: "World", memberships: np.ndarray | None = None) -> api.QueryColliders:
-        return api.QueryColliders(shape=world.scene.shape_type.astype(np.uint8), dims=world.scene.dims, position=world.bodies.position,
+        sc = world.scene
+        if sc.compound:   # a collider table: every part at its world pose
+            pos, rot = sc.collider_poses(world.bodies)
+            return api.QueryColliders(shape=sc.collider_shape.astype(np.uint8), dims=sc.collider_dims, position=pos, rotation=rot, memberships=memberships)
+        return api.QueryColliders(shape=sc.shape_type.astype(np.uint8), dims=sc.dims, position=world.bodies.position,
                                   rotation=world.bodies.rotation, memberships=memberships)
 
     def update_pipeline(self, world: "World", memberships: np.ndarray | None = None, shapes_unchanged: bool = False) -> None:
@@ -201,7 +205,14 @@ class World:
         self.joints = scene.joints
         self.scalar = scene.bodies.position.dtype
         self.plugins = plugins
-        self.pipeline = HostPipeline(scene.shape_type, scene.dims, scene.friction, scene.restitution, scalar=self.scalar)
+        if scene.compound:
+            if ccd is not None:
+                raise ValueError("swept CCD assumes a collider at its body's origin: a scene with a collider table cannot use it")
+            self.pipeline = HostPipeline(scene.collider_shape, scene.collider_dims, scene.collider_friction, scene.collider_restitution, scalar=self.scalar,
+                                         collider_body=scene.collider_body)
+        else:
+            self.pipeline = HostPipeline(scene.shape_type, scene.dims, scene.friction, scene.restitution, scalar=self.scalar)
+        self.collider_pose: dict | None = None   # a collider table: the colliders' world poses of the current step
         integ = plugins.get("IntegratorPlugin")
         cfg = getattr(plugins.get("SolverPlugin"), "config", None) or SolverConfig()
         self.params = api.default_step_params(dt=dt, substeps=substeps, gravity=integ.gravity.value, solver_iterations=solver_iterations,
@@ -216,9 +227,18 @@ class World:
         self.step_index = 0
 
     # the stages of one PhysicsSchedule run, separately callable so tests/bench can snapshot in between
+    def update_colliders(self) -> dict | None:
+        """A collider table: the colliders' world poses from the body poses, and the body velocity at every collider (for the AABBs)."""
+        if not self.scene.compound:
+            return None
+        pos, rot = self.scene.collider_poses(self.bodies)
+        lv, av = self.scene.collider_velocities(self.bodies, pos)
+        self.collider_pose = {"position": pos, "rotation": rot, "linear_velocity": lv, "angular_velocity": av}
+        return self.collider_pose
+
     def broad_phase(self) -> api.PairList:
         dt = self.params.dt
-        self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, dt)
+        self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, dt, self.update_colliders())
         aabbs = self.pipeline.intervals(self.bodies, self.aabb_min, self.aabb_max)
         aabbs.flags = self.interval_flags(aabbs.collider, aabbs.flags)
         aabbs.joint_disabled_body_pairs = self.scene.joint_disabled_body_pairs
@@ -253,7 +273,8 @@ class World:
         return self.pipeline.report(events_only)
 
     def narrow_phase(self) -> api.Manifolds:
-        self.last_manifolds = self.pipeline.narrow_phase(self.bodies, self.aabb_min, self.aabb_max, self.params.dt, bool(self.params.match_contacts))
+        self.last_manifolds = self.pipeline.narrow_phase(self.bodies, self.aabb_min, self.aabb_max, self.params.dt, bool(self.params.match_contacts),
+                                                         colliders=self.collider_pose)
         self.events = self.pipeline.events()
         return self.last_manifolds
 
@@ -325,15 +346,18 @@ class DeviceGraphWorld(World):
         self.ctx = ctx
         n = int(scene.bodies.count)
         self.n = n
-        ctx.contacts_configure(scene.bodies.kind if scene.bodies.kind is not None else np.zeros(n, dtype=np.uint8), n, scene.friction, scene.restitution)
+        nc = int(scene.collider_body.shape[0]) if scene.compound else n
+        self.collider_count = nc
+        ctx.contacts_configure(scene.bodies.kind if scene.bodies.kind is not None else np.zeros(n, dtype=np.uint8), nc,
+                               scene.collider_friction if scene.compound else scene.friction, scene.collider_restitution if scene.compound else scene.restitution)
         if self.sensor is not None:
             ctx.contacts_set_sensors(self.sensor)
-        self.order = np.arange(n, dtype=np.uint32)       # AabbIntervals' persistent order (colliders = bodies in this fixture)
+        self.order = np.arange(nc, dtype=np.uint32)      # AabbIntervals' persistent order of the colliders
         self.stats: dict | None = None
         self.new_pairs = 0
-        self._shape = np.ascontiguousarray(scene.shape_type, dtype=np.uint8)
-        self._dims = np.ascontiguousarray(scene.dims, dtype=self.scalar)
-        self._order_out = np.empty(n, dtype=np.uint32)
+        self._shape = np.ascontiguousarray(scene.collider_shape if scene.compound else scene.shape_type, dtype=np.uint8)
+        self._dims = np.ascontiguousarray(scene.collider_dims if scene.compound else scene.dims, dtype=self.scalar)
+        self._order_out = np.empty(nc, dtype=np.uint32)
         self._uploaded_once = False     # from the second step on the static columns (shapes, mass properties ...) stay on the device
         if self.ccd is not None:
             ctx.ccd_configure(**self.ccd)   # solve_swept_ccd inside the device-resident solver stage
@@ -351,11 +375,12 @@ class DeviceGraphWorld(World):
 
     def intervals(self, aabb_min: np.ndarray, aabb_max: np.ndarray) -> api.Aabbs:
         o, kind = self.order, self.bodies.kind
-        flags = np.where(kind[o] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
+        body = o.copy() if not self.scene.compound else np.ascontiguousarray(self.scene.collider_body[o], dtype=np.uint32)
+        flags = np.where(kind[body] == api.BODY_STATIC, api.AABB_IS_INACTIVE, 0).astype(np.uint8) | np.uint8(api.AABB_GENERATE_CONSTRAINTS)
         flags = self.interval_flags(o, flags)
         if self.sleeping is not None:      # Has<Sleeping> when the intervals are refreshed (broad_phase.rs:223-260), minus the islands about to wake
-            flags = flags | np.where(self.inactive_bodies()[o], api.AABB_IS_INACTIVE, 0).astype(np.uint8)
-        a = api.Aabbs(collider=o.copy(), body=o.copy(), aabb_min=np.ascontiguousarray(aabb_min[o]), aabb_max=np.ascontiguousarray(aabb_max[o]),
+            flags = flags | np.where(self.inactive_bodies()[body], api.AABB_IS_INACTIVE, 0).astype(np.uint8)
+        a = api.Aabbs(collider=o.copy(), body=body, aabb_min=np.ascontiguousarray(aabb_min[o]), aabb_max=np.ascontiguousarray(aabb_max[o]),
                       flags=np.ascontiguousarray(flags), order_out=self._order_out)
         a.joint_disabled_body_pairs = self.scene.joint_disabled_body_pairs
         return a
@@ -374,7 +399,11 @@ class DeviceGraphWorld(World):
         ctx.broadphase_run()
         # the solver's body columns start moving now, on the library's copy stream, under the broad phase and the contact pipeline
         ctx.solver_prefetch_bodies(b, static_unchanged=self._uploaded_once)
-        colliders = {"shape": self._shape, "dims": self._dims, "position": b.position, "rotation": b.rotation, "aabb_min": aabb_min, "aabb_max": aabb_max}
+        pose = self.collider_pose if self.scene.compound else {"position": b.position, "rotation": b.rotation}
+        colliders = {"shape": self._shape, "dims": self._dims, "position": pose["position"], "rotation": pose["rotation"], "aabb_min": aabb_min,
+                     "aabb_max": aabb_max}
+        if self.scene.compound:   # the anchors are measured from the bodies' centres of mass
+            ctx.contacts_set_body_frames(b.position, b.rotation, b.center_of_mass)
         self.stats = ctx.contacts_step(self.params.dt, 0.005, colliders, b.linear_velocity, b.angular_velocity, bool(self.params.match_contacts), take_pairs=True,
                                        shapes_unchanged=self._uploaded_once)
         self.new_pairs = ctx.broadphase_download_order()
@@ -407,7 +436,7 @@ class DeviceGraphWorld(World):
 
     def set_sensors(self, sensor) -> None:
         self.sensor = None if sensor is None else np.asarray(sensor, dtype=bool)
-        self.ctx.contacts_set_sensors(self.sensor, collider_count=self.n)
+        self.ctx.contacts_set_sensors(self.sensor, collider_count=self.collider_count)
 
     def remove_colliders(self, colliders) -> None:
         self.ctx.contacts_remove_colliders(colliders)
@@ -416,5 +445,5 @@ class DeviceGraphWorld(World):
         return self.ctx.contacts_report(events_only=events_only)
 
     def step(self) -> None:
-        self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, self.params.dt)
+        self.aabb_min, self.aabb_max = self.pipeline.update_aabbs(self.bodies, self.params.dt, self.update_colliders())
         self.step_from(self.intervals(self.aabb_min, self.aabb_max), self.aabb_min, self.aabb_max)

@@ -23,6 +23,38 @@ class Scene:
     restitution: np.ndarray  # float64[n]
     joints: api.JointSet | None = None
     joint_disabled_body_pairs: np.ndarray | None = None
+    # optional collider table (ColliderOf + the collider's Transform relative to its body): several colliders per body, offset from the body
+    # origin.  Absent: one collider per body at its origin, described by shape_type / dims / friction / restitution above.
+    collider_body: np.ndarray | None = None          # int32[C] the body of every collider
+    local_position: np.ndarray | None = None         # float64[C,3] in the body frame
+    local_rotation: np.ndarray | None = None         # float64[C,4] (x, y, z, w)
+    collider_shape: np.ndarray | None = None         # int32[C]
+    collider_dims: np.ndarray | None = None          # float64[C,3]
+    collider_friction: np.ndarray | None = None      # float64[C]
+    collider_restitution: np.ndarray | None = None   # float64[C]
+
+    @property
+    def compound(self) -> bool:
+        return self.collider_body is not None
+
+    def collider_poses(self, bodies: api.Bodies) -> tuple[np.ndarray, np.ndarray]:
+        """The colliders' world poses from the body poses (what the reference's Prepare stage propagates): position = body position +
+        R * local position, rotation = R * local rotation.  Evaluated in float64 and rounded to the body columns' scalar."""
+        b = self.collider_body
+        p = np.asarray(bodies.position, dtype=np.float64)[b]
+        q = np.asarray(bodies.rotation, dtype=np.float64)[b]
+        pos = p + _qrot_rows(q, self.local_position)
+        rot = _qmul_rows(q, self.local_rotation)
+        return pos.astype(bodies.position.dtype), rot.astype(bodies.rotation.dtype)
+
+    def collider_velocities(self, bodies: api.Bodies, position: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+        """The body's velocity at every collider, for the swept AABB (collider/backend.rs:570-585): v + w x (pos - body pos - R com)."""
+        b = self.collider_body
+        f = lambda a: np.asarray(a, dtype=np.float64)[b]
+        off = np.asarray(position, dtype=np.float64) - f(bodies.position) - _qrot_rows(f(bodies.rotation), f(bodies.center_of_mass))
+        w = f(bodies.angular_velocity)
+        lv = f(bodies.linear_velocity) + np.cross(w, off)
+        return lv.astype(bodies.position.dtype), w.astype(bodies.position.dtype)
 
 
 def _cuboid_mass(he: np.ndarray, density: float = 1.0):
@@ -291,6 +323,161 @@ def capsule_pile(n: int, seed: int = 7, layers: int = 10, capsule_share: float =
     rot = np.concatenate([[[0.0, 0.0, 0.0, 1.0]], q])
     kind = np.concatenate([[api.BODY_STATIC], np.full(n, api.BODY_DYNAMIC)])
     return _assemble(f"capsule_pile_{n}", pos, rot, kind, he, np.concatenate([[SHAPE_CUBOID], shape]), scalar)
+
+
+def _qrot_rows(q, v):
+    """rotate the rows of v [n,3] by the rows of q [n,4] (glam's Quat * Vec3)"""
+    b, w = q[:, :3], q[:, 3:4]
+    return v * (w * w - np.sum(b * b, axis=1, keepdims=True)) + b * (2.0 * np.sum(v * b, axis=1, keepdims=True)) + np.cross(b, v) * (2.0 * w)
+
+
+def _qmul_rows(a, b):
+    ax, ay, az, aw = a.T
+    bx, by, bz, bw = b.T
+    return np.stack([aw * bx + ax * bw + ay * bz - az * by, aw * by - ax * bz + ay * bw + az * bx,
+                     aw * bz + ax * by - ay * bx + az * bw, aw * bw - ax * bx - ay * by - az * bz], axis=1)
+
+
+def with_collider_table(scene: Scene, offset=None, center_of_mass=None) -> Scene:
+    """A single-collider scene with an explicit collider table (one collider per body).  offset [B,3] (None = 0): every body's origin moves
+    by -R * offset, its collider sits at local position `offset` and its centre of mass at `center_of_mass` (None = offset), so the collider
+    and the centre of mass stay where they were in the world: the same physical scene, expressed from other body origins."""
+    import dataclasses
+    n = int(scene.bodies.count)
+    d = np.zeros((n, 3)) if offset is None else np.asarray(offset, dtype=np.float64).reshape(n, 3)
+    com = d if center_of_mass is None else np.asarray(center_of_mass, dtype=np.float64).reshape(n, 3)
+    b = scene.bodies
+    s = b.position.dtype
+    q = np.asarray(b.rotation, dtype=np.float64)
+    bodies = dataclasses.replace(b, position=np.ascontiguousarray(np.asarray(b.position, dtype=np.float64) - _qrot_rows(q, d), dtype=s),
+                                 center_of_mass=np.ascontiguousarray(com, dtype=s))
+    return dataclasses.replace(scene, name=scene.name + "_table", bodies=bodies, collider_body=np.arange(n, dtype=np.int32), local_position=d.copy(),
+                               local_rotation=np.tile([0.0, 0.0, 0.0, 1.0], (n, 1)), collider_shape=scene.shape_type.copy(),
+                               collider_dims=scene.dims.copy(), collider_friction=scene.friction.copy(), collider_restitution=scene.restitution.copy())
+
+
+def _part_mass(shape: int, dims, density: float = 1.0):
+    """mass and local inertia (diagonal) of one part"""
+    he = np.asarray(dims, dtype=np.float64).reshape(1, 3)
+    if shape == SHAPE_SPHERE:
+        r = he[0, 0]
+        m = density * 4.0 / 3.0 * np.pi * r ** 3
+        return m, np.full(3, 0.4 * m * r * r)
+    if shape == SHAPE_CAPSULE:
+        m, i = _capsule_mass(he[:, 0], he[:, 1], density)
+        return float(m[0]), i[0]
+    m, i = _cuboid_mass(he, density)
+    return float(m[0]), i[0]
+
+
+def _quat_matrix(q):
+    x, y, z, w = q
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def compound_mass(parts, density: float = 1.0):
+    """(mass, centre of mass, inertia tensor about it) of a body made of parts [(shape, dims, local position, local rotation)]: the parts'
+    masses summed, the mass-weighted centre, each part's inertia rotated into the body frame and moved by the parallel-axis theorem.
+    Closed form, PARITY UNPINNED: the reference takes mass properties from bevy_heavy, which is not vendored."""
+    ms, cs, Is = [], [], []
+    for shape, dims, lp, lr in parts:
+        m, i = _part_mass(shape, dims, density)
+        R = _quat_matrix(lr)
+        ms.append(m)
+        cs.append(np.asarray(lp, dtype=np.float64))
+        Is.append(R @ np.diag(i) @ R.T)
+    M = float(sum(ms))
+    c = sum(m * p for m, p in zip(ms, cs)) / M
+    I = np.zeros((3, 3))
+    for m, p, i in zip(ms, cs, Is):
+        d = p - c
+        I += i + m * (np.dot(d, d) * np.eye(3) - np.outer(d, d))
+    return M, c, I
+
+
+_Z90 = (0.0, 0.0, np.sin(np.pi / 4), np.cos(np.pi / 4))   # local y -> -x: a capsule lying along x
+
+
+def _compound_parts(kind: str, rng):
+    """(parts, origin): parts [(shape, dims, position, rotation)] in a design frame, origin = the body origin in that frame"""
+    I4 = (0.0, 0.0, 0.0, 1.0)
+    if kind == "table":
+        w, d, t, h, leg = rng.uniform(0.5, 0.8), rng.uniform(0.4, 0.6), 0.06, rng.uniform(0.3, 0.5), 0.05
+        parts = [(SHAPE_CUBOID, (w, t, d), (0.0, h + t, 0.0), I4)]
+        for sx in (-1, 1):
+            for sz in (-1, 1):
+                parts.append((SHAPE_CUBOID, (leg, h * 0.5, leg), (sx * (w - leg), h * 0.5, sz * (d - leg)), I4))
+        return parts, np.array([-w, 0.0, -d])                      # origin at a foot corner
+    if kind == "dumbbell":
+        r, hl, rb = rng.uniform(0.06, 0.1), rng.uniform(0.3, 0.5), rng.uniform(0.18, 0.25)
+        parts = [(SHAPE_CAPSULE, (r, hl, 0.0), (0.0, 0.0, 0.0), _Z90), (SHAPE_SPHERE, (rb, 0, 0), (-hl, 0.0, 0.0), I4),
+                 (SHAPE_SPHERE, (rb * rng.uniform(0.7, 1.0), 0, 0), (hl, 0.0, 0.0), I4)]
+        return parts, np.array([-hl, 0.0, 0.0])                    # origin at one weight's centre
+    a, b, t = rng.uniform(0.3, 0.5), rng.uniform(0.3, 0.5), rng.uniform(0.1, 0.15)   # L-block: a foot and an upright
+    parts = [(SHAPE_CUBOID, (a, t, t), (a, t, 0.0), I4), (SHAPE_CUBOID, (t, b, t), (t, 2 * t + b, 0.0), I4)]
+    return parts, np.zeros(3)                                       # origin at the corner of the foot
+
+
+def compound_pile(n: int, seed: int = 11, scalar=np.float32, single_share: float = 0.0, layers: int = 4) -> Scene:
+    """A seeded pile of n dynamic bodies of 2-5 parts over a static ground cuboid (body 0, one collider): tables (a top on four legs),
+    dumbbells (two spheres on a capsule) and L-blocks, at random yaws on a jittered grid that starts without overlaps.  Every body's origin is
+    away from its centre of mass (a foot corner, a weight's centre, the L's corner), and every third body also has an explicit centre-of-mass
+    offset (CenterOfMass), which leaves the inertia about the parts' centre.  single_share: that share of the bodies are single cuboids,
+    spheres or capsules at their body's origin instead.  Mass properties: compound_mass (PARITY UNPINNED)."""
+    rng = np.random.default_rng(seed)
+    pitch = 2.2
+    side = int(np.ceil(np.sqrt(n / layers)))
+    pos, rot, com, inv_m, inv_i = [], [], [], [], []
+    cb, lp, lr, cs, cd = [], [], [], [], []
+    extent = side * pitch
+    ground = (SHAPE_CUBOID, (extent * 0.5 + 10.0, 0.5, extent * 0.5 + 10.0))
+    for i in range(n):
+        layer, cell = i // (side * side), i % (side * side)
+        at = np.array([(cell // side) * pitch, 1.0 + layer * pitch, (cell % side) * pitch]) + rng.uniform(-0.05, 0.05, 3)
+        if rng.uniform() < single_share:
+            k = int(rng.integers(0, 3))
+            dims = (rng.uniform(0.2, 0.4),) * 3 if k != SHAPE_CAPSULE else (rng.uniform(0.15, 0.25), rng.uniform(0.2, 0.4), 0.0)
+            parts, origin = [(k, dims, (0.0, 0.0, 0.0), (0.0, 0.0, 0.0, 1.0))], np.zeros(3)
+        else:
+            parts, origin = _compound_parts(("table", "dumbbell", "lblock")[int(rng.integers(0, 3))], rng)
+        M, c, I = compound_mass(parts)
+        q = _quat_axis_angle((0, 1, 0), rng.uniform(-np.pi, np.pi))
+        c_local = c - origin
+        explicit = len(parts) > 1 and i % 3 == 0
+        com.append(c_local + (rng.uniform(-0.05, 0.05, 3) if explicit else 0.0))
+        pos.append(at - _qrot(q, c_local))
+        rot.append(q)
+        Iinv = np.linalg.inv(I)
+        inv_m.append(1.0 / M)
+        inv_i.append([Iinv[0, 0], Iinv[0, 1], Iinv[0, 2], Iinv[1, 1], Iinv[1, 2], Iinv[2, 2]])
+        for shape, dims, p, r in parts:
+            cb.append(i + 1)
+            lp.append(np.asarray(p) - origin)
+            lr.append(r)
+            cs.append(shape)
+            cd.append(dims)
+    B = n + 1
+    s = np.dtype(scalar)
+    kind = np.concatenate([[api.BODY_STATIC], np.full(n, api.BODY_DYNAMIC)]).astype(np.uint8)
+    P = np.concatenate([[[extent * 0.5, -0.5, extent * 0.5]], np.array(pos).reshape(-1, 3)])
+    R = np.concatenate([[[0.0, 0.0, 0.0, 1.0]], np.array(rot).reshape(-1, 4)])
+    z3 = np.zeros((B, 3))
+    bodies = api.Bodies(kind=kind, position=np.ascontiguousarray(P, dtype=s), rotation=np.ascontiguousarray(R, dtype=s),
+                        linear_velocity=np.ascontiguousarray(z3, dtype=s), angular_velocity=np.ascontiguousarray(z3, dtype=s),
+                        inverse_mass=np.ascontiguousarray(np.concatenate([[0.0], inv_m]), dtype=s),
+                        inverse_inertia_local=np.ascontiguousarray(np.concatenate([np.zeros((1, 6)), np.array(inv_i).reshape(-1, 6)]), dtype=s),
+                        center_of_mass=np.ascontiguousarray(np.concatenate([np.zeros((1, 3)), np.array(com).reshape(-1, 3)]), dtype=s))
+    C_ = len(cb) + 1
+    cshape = np.concatenate([[ground[0]], cs]).astype(np.int32)
+    cdims = np.concatenate([[ground[1]], np.array(cd, dtype=np.float64).reshape(-1, 3)])
+    cbody = np.concatenate([[0], cb]).astype(np.int32)
+    first = np.searchsorted(cbody, np.arange(B))   # the per-body columns describe each body's first collider
+    return Scene(f"compound_pile_{n}", bodies, np.ascontiguousarray(cshape[first]), np.ascontiguousarray(cdims[first]), np.full(B, 0.5), np.zeros(B),
+                 collider_body=cbody, local_position=np.concatenate([np.zeros((1, 3)), np.array(lp).reshape(-1, 3)]),
+                 local_rotation=np.concatenate([[[0.0, 0.0, 0.0, 1.0]], np.array(lr).reshape(-1, 4)]), collider_shape=cshape,
+                 collider_dims=np.ascontiguousarray(cdims), collider_friction=np.full(C_, 0.5), collider_restitution=np.zeros(C_))
 
 
 def _qmul(a, b):

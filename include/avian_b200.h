@@ -422,7 +422,8 @@ typedef struct AvnNarrowInput {
     const uint32_t* body2;
     const uint8_t* shape;              /* [C] AvnShape; NULL = cuboid */
     const void* dims;                  /* [C][3] cuboid half extents / sphere radius in [0] / capsule [radius, half length] */
-    const void* position;              /* [C][3] collider Position (collider at the body origin, centre of mass at the origin) */
+    const void* position;              /* [C][3] collider Position (world pose; without body frames a collider sits at its body's origin and
+                                          the centre of mass at that origin, see avn_contacts_set_body_frames) */
     const void* rotation;              /* [C][4] */
     const void* linear_velocity;       /* [B][3] */
     const void* angular_velocity;      /* [B][3] */
@@ -441,6 +442,26 @@ typedef struct AvnRawManifolds {      /* fixed stride: 4 point slots per pair, u
 } AvnRawManifolds;
 
 AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, AvnRawManifolds* out);
+
+/* ---- body frames: several colliders per body, offset from the body origin, with the centre of mass off the origin (ColliderOf,
+ *      ComputedCenterOfMass).  With frames set, avn_narrow_phase and avn_contacts_step return anchors relative to each body's centre of mass,
+ *      as update_contacts does (narrow_phase/system_param.rs:540-570, 731-747):
+ *        anchor = (witness relative to the collider + (collider position - body position)) - body rotation * center_of_mass
+ *      and take the normal speed, the speculative keep rule and match_contacts from those anchors.  The input's position / rotation stay the
+ *      colliders' world poses, and body1 / body2 (or the contact store's rows) name the bodies. -------------------------------------------- */
+typedef struct AvnBodyFrames {
+    uint32_t body_count, _pad;         /* must equal AvnNarrowInput::body_count of the calls that use the frames */
+    const void* position;              /* [B][3] body Position: the origin the collider offsets are measured from */
+    const void* rotation;              /* [B][4] body Rotation */
+    const void* center_of_mass;        /* [B][3] ComputedCenterOfMass, local; NULL = 0 */
+} AvnBodyFrames;
+/* Copies the frames on the host; every later avn_contacts_step / avn_narrow_phase of the context uses them until the next call.  NULL (or
+ * never called) = a collider at its body's origin and the centre of mass at that origin, bit for bit as before.  Static bodies need a frame
+ * too: a static side's anchor enters initial_separation.  AVN_ERR_INVALID_ARGUMENT without position or rotation; a call that uses the frames
+ * refuses an input whose body_count differs, before anything is copied.  AVN_ERR_UNSUPPORTED while swept CCD is configured: swept CCD
+ * assumes a collider at its body's origin, so avn_ccd_configure refuses a configuration while frames are set, and the two never meet.
+ * A refused call changes nothing. */
+AvnStatus avn_contacts_set_body_frames(AvnContext* ctx, const AvnBodyFrames* frames);
 
 /* ---- the ContactGraph and the ConstraintGraph on the device (SURVEY.md 8f "next #3"): after this nothing of the contact pipeline lives on
  *      the host.  Replaces, for the pairs the device narrow phase covers,
