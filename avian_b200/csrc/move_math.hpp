@@ -1,4 +1,4 @@
-// MoveAndSlide (character_controller/move_and_slide.rs, velocity_project.rs) for cuboid / sphere characters, written once for the host
+// MoveAndSlide (character_controller/move_and_slide.rs, velocity_project.rs) for cuboid / sphere / capsule characters, written once for the host
 // fixture (g++, -ffp-contract=off) and for the device (nvcc, -fmad=false), the query_math.hpp / ccd_math.hpp arrangement: the per-character
 // algorithm is a template over a "scene" that answers two questions, and both builds evaluate the same expressions in the same order.
 //   * sc.cast(shape, he, c, q, d, maxd, t, collider, axis): the closest filtered shape cast (AVN_CAST_IGNORE_ORIGIN_PENETRATION), the
@@ -19,7 +19,10 @@
 //   * the closest sweep hit is the lowest (t, collider index), not the first hit in tree order (the cast_shape rule).
 //   * intersections are visited in ascending collider index, not tree order (plane pruning and Gauss-Seidel depend on the order).
 //   * the reported hit distance is the TOI; the reference's MoveHitData::collision_distance is the requested movement length (:777).
-//   * characters are cuboids and spheres.
+// Capsules (DESIGN.md §7j): the loop is a template over CAPS.  CAPS = true compiles the capsule casts of query_math.hpp and the capsule pairs of
+// nm::collide into the sweep and the intersections; CAPS = false is the cuboid / sphere loop as it was before capsule characters, for trees
+// and batches without a capsule (queries.cu picks the instance on the host).  The host fixture runs CAPS = true, which gives the same bits on
+// cuboids and spheres.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -113,13 +116,13 @@ NM_HD inline T3<T> project_velocity(T3<T> v, const T3<float>* normals, int n) {
 // ---- one intersection (intersections, move_and_slide.rs:1032-1078): the contact of the character with one collider -----------------------
 // nm::collide(character, collider) -> the deepest point (max_by: the last of equal penetrations) and the plane normal -manifold.normal as
 // an f32 Dir.  False when the pair has no point within the prediction distance.  Kept out of line: it holds the narrow phase's box-box
-// generator, and the move kernel calls it from two places.  Characters and colliders are cuboids and spheres (capsules are refused on the
-// host), so the capsule pairs are not compiled in (nm::collide<false>).
-template <class T>
+// generator, and the move kernel calls it from two places.  CAPS = false leaves the capsule pairs out (nm::collide<false>): that instance
+// never sees a capsule.
+template <class T, bool CAPS = false>
 NM_COLD inline bool contact_plane(int sa, V3 ha, V3 pa, Q qa, int sb, V3 hb, V3 pb, Q qb, double prediction, T3<float>& normal, T& penetration) {
     V3 n;
     nm::Contacts pts;
-    if (!nm::collide<false>(sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts) || pts.n == 0) return false;
+    if (!nm::collide<CAPS>(sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts) || pts.n == 0) return false;
     T best = T(nm::dot(pts.p[0].a - pts.p[0].b, n));
     for (int k = 1; k < pts.n; ++k) {
         const T p = T(nm::dot(pts.p[k].a - pts.p[k].b, n));
@@ -137,19 +140,19 @@ template <class T> NM_HD inline T3<float> plane_dir(T3<T> p) { const T3<float> f
 struct Body { int shape; V3 he; Q q; };
 
 // the character's tight AABB at pos, rounded to T, grown by `grow` (Aabb::grow)
-template <class T>
+template <bool CAPS, class T>
 NM_HD inline void grown_aabb(const Body& b, T3<T> pos, T grow, T lo[3], T hi[3]) {
     V3 mn, mx;
-    qm::collider_aabb(b.shape, b.he, to_v3(pos), b.q, mn, mx);
+    qm::collider_aabb<CAPS>(b.shape, b.he, to_v3(pos), b.q, mn, mx);
     lo[0] = T(mn.x) - grow; lo[1] = T(mn.y) - grow; lo[2] = T(mn.z) - grow;
     hi[0] = T(mx.x) + grow; hi[1] = T(mx.y) + grow; hi[2] = T(mx.z) + grow;
 }
 
 // every intersection plane at pos with prediction distance `pred`, in ascending collider index: fn(normal, penetration)
-template <class T, class Scene, class Fn>
+template <class T, bool CAPS, class Scene, class Fn>
 NM_HD inline void intersections(const Scene& sc, const Body& b, T3<T> pos, T pred, Fn fn) {
     T lo[3], hi[3];
-    grown_aabb(b, pos, pred, lo, hi);
+    grown_aabb<CAPS>(b, pos, pred, lo, hi);
     const V3 p = to_v3(pos);
     sc.candidates(lo, hi, [&](uint32_t c) {
         int s;
@@ -158,13 +161,13 @@ NM_HD inline void intersections(const Scene& sc, const Body& b, T3<T> pos, T pre
         sc.collider(c, s, he, cp, cq);
         T3<float> n;
         T pen;
-        if (contact_plane<T>(b.shape, b.he, p, b.q, s, he, cp, cq, double(pred), n, pen)) fn(n, pen);
+        if (contact_plane<T, CAPS>(b.shape, b.he, p, b.q, s, he, cp, cq, double(pred), n, pen)) fn(n, pen);
     });
 }
 
 // depenetrate + depenetrate_intersections (:868-897, :982-1009): Gauss-Seidel over the (normal, penetration + skin) list.  The list is
 // kept when it has at most MOVE_WINDOW entries; a longer one is evaluated again, in the same order, in every iteration.
-template <class T, class Scene>
+template <bool CAPS, class T, class Scene>
 NM_HD inline T3<T> depenetrate(const Scene& sc, const Config<T>& cfg, const Body& b, T3<T> pos) {
     T3<T> fixup{0, 0, 0};
     if (cfg.depenetration_iterations == 0) return fixup;
@@ -174,7 +177,7 @@ NM_HD inline T3<T> depenetrate(const Scene& sc, const Config<T>& cfg, const Body
     T3<float> ln[MOVE_WINDOW];
     T ld[MOVE_WINDOW];
     uint32_t count = 0;
-    intersections<T>(sc, b, pos, skin, [&](T3<float> n, T pen) {
+    intersections<T, CAPS>(sc, b, pos, skin, [&](T3<float> n, T pen) {
         if (count < uint32_t(MOVE_WINDOW)) { ln[count] = n; ld[count] = pen + skin; }
         ++count;
     });
@@ -193,7 +196,7 @@ NM_ROLLED
         if (kept) {
             for (uint32_t k = 0; k < count; ++k) relax(ln[k], ld[k]);
         } else {
-            intersections<T>(sc, b, pos, skin, [&](T3<float> n, T pen) { relax(n, pen + skin); });
+            intersections<T, CAPS>(sc, b, pos, skin, [&](T3<float> n, T pen) { relax(n, pen + skin); });
         }
         if (total < target) break;
     }
@@ -203,12 +206,12 @@ NM_ROLLED
 // MoveAndSlide::move_and_slide (:464-609) with an on_hit that accepts every hit.  pos / vel: in, out.  init: the configured planes
 // (MoveAndSlideConfig::planes) as f32 Dirs, n_init <= max_planes.  hits.sweep(iteration, collider, safe distance, toi, point1, normal1) is
 // called for every iteration that hit something.
-template <class T, class Scene, class Hits>
+template <bool CAPS = false, class T, class Scene, class Hits>
 NM_HD inline void move_and_slide(const Scene& sc, const Config<T>& cfg, const Body& b, T3<T>& pos, T3<T>& vel, const T3<float>* init, int n_init,
                                  Hits& hits) {
     T time_left = cfg.dt;
     const T skin = cfg.length_unit * cfg.skin_width;
-    pos = add(pos, depenetrate(sc, cfg, b, pos));
+    pos = add(pos, depenetrate<CAPS>(sc, cfg, b, pos));
     T3<float> planes[MAX_PLANES + 1];
 NM_ROLLED
     for (uint32_t it = 0; it < cfg.iterations; ++it) {
@@ -234,7 +237,7 @@ NM_ROLLED
         Q cq;
         sc.collider(c, cs, che, cp, cq);
         qm::ShapeContact hc;
-        qm::cast_output(b.shape, b.he, p, b.q, d, qm::CAST_IGNORE_ORIGIN_PENETRATION, cs, che, cp, cq, toi, axis, hc);
+        qm::cast_output<CAPS>(b.shape, b.he, p, b.q, d, qm::CAST_IGNORE_ORIGIN_PENETRATION, cs, che, cp, cq, toi, axis, hc);
         const T3<T> normal1 = from_v3<T>(hc.n1);
         const T hit_distance = T(toi);
         // pull_back (:789-793)
@@ -248,7 +251,7 @@ NM_ROLLED
         for (int k = 0; k < n_init; ++k) planes[np++] = init[k];
         planes[np++] = narrow(normal1);
         const T3<T> v = vel;
-        intersections<T>(sc, b, pos, skin * T(2), [&](T3<float> n, T) {
+        intersections<T, CAPS>(sc, b, pos, skin * T(2), [&](T3<float> n, T) {
             for (int k = 0; k < np; ++k) {
                 if (T(dot(n, planes[k])) >= cfg.plane_similarity_dot_threshold) {
                     // similar: keep the more blocking normal
@@ -261,7 +264,7 @@ NM_ROLLED
         });
         vel = project_velocity(vel, planes, np);
     }
-    pos = add(pos, depenetrate(sc, cfg, b, pos));
+    pos = add(pos, depenetrate<CAPS>(sc, cfg, b, pos));
 }
 
 }  // namespace mv
@@ -270,7 +273,10 @@ NM_ROLLED
 #include "../../include/avian_b200.h"
 namespace mv {
 // NULL when the call is usable; the reason otherwise.  collider_count: the colliders of the scene (the tree's, the host's)
-inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, bool f64, uint32_t collider_count) {
+// capsules: whether AVN_SHAPE_CAPSULE characters are accepted; saw_capsule (optional): set when the batch holds one
+inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, bool f64, uint32_t collider_count, bool capsules = false,
+                              bool* saw_capsule = nullptr) {
+    if (saw_capsule) *saw_capsule = false;
     if (!cfg) return "config is required";
     if (!b) return "batch is required";
     const double vals[6] = {cfg->delta_time, cfg->length_unit, cfg->skin_width, cfg->max_depenetration_error, cfg->penetration_rejection_threshold,
@@ -283,11 +289,13 @@ inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, b
     if (b->count == 0) return nullptr;
     if (!b->shape || !b->dims || !b->position || !b->rotation || !b->velocity) return "batch: shape, dims, position, rotation and velocity are required";
     for (uint32_t i = 0; i < b->count; ++i) {
-        if (b->shape[i] > AVN_SHAPE_SPHERE) return "batch: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
-        for (int k = 0; k < (b->shape[i] == AVN_SHAPE_SPHERE ? 1 : 3); ++k) {
+        if (!capsules && b->shape[i] > AVN_SHAPE_SPHERE) return "batch: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
+        if (b->shape[i] > AVN_SHAPE_CAPSULE) return "batch: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
+        for (int k = 0; k < qm::shape_dims_read(b->shape[i]); ++k) {
             const double v = f64 ? static_cast<const double*>(b->dims)[3 * size_t(i) + k] : static_cast<const float*>(b->dims)[3 * size_t(i) + k];
-            if (v < 0) return "batch: negative half extent or radius";
+            if (v < 0) return "batch: negative half extent, radius or half length";
         }
+        if (saw_capsule && b->shape[i] == AVN_SHAPE_CAPSULE) *saw_capsule = true;
     }
     if (const char* why = qm::check_exclusions(b->count, b->exclude_count, b->exclude_offsets, b->exclude)) return why;
     if (b->plane_offsets) {

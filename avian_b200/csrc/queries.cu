@@ -19,6 +19,9 @@
 // hit; project_point (570-615) prunes on the squared point-box distance; point and shape intersections (628-683, 744-826) use the same CSR
 // pattern.  Their geometry is the shape-cast part of query_math.hpp.
 // Move and slide (character_controller/move_and_slide.rs): q_move runs csrc/move_math.hpp's loop per character over this tree (TreeScene).
+// Capsules (DESIGN.md §7j): every kernel that evaluates a collider's or a query's shape has a CAPS instance of its own, launched when the tree
+// holds a capsule (remembered across AVN_QUERY_SHAPES_UNCHANGED updates) or the batch does; the CAPS = false instances compile the cuboid /
+// sphere code they had before capsules were queried.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -77,7 +80,7 @@ __device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t* p, uint32_t v) {
 __device__ __forceinline__ float f32_clamped(double x) { return float(fmin(fmax(x, -double(FLT_MAX)), double(FLT_MAX))); }
 
 // 1. per collider: validity, tight AABB (rounded to S), f32 culling box, centre; scene bounds of the centres
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(256) q_prepare(const __grid_constant__ Tree<S> t, S* __restrict__ tmn, S* __restrict__ tmx, NodeBox* __restrict__ cbox,
                                                  float4* __restrict__ centre, uint8_t* __restrict__ valid, int* __restrict__ m, uint32_t* __restrict__ sb) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -89,7 +92,7 @@ __global__ void __launch_bounds__(256) q_prepare(const __grid_constant__ Tree<S>
         ok = qm::collider_valid(he, p, q);
         if (ok) {
             nm::V3 mn, mx;
-            qm::collider_aabb(t.shape[i], he, p, q, mn, mx);
+            qm::collider_aabb<CAPS>(t.shape[i], he, p, q, mn, mx);
             tmn[3 * i] = S(mn.x); tmn[3 * i + 1] = S(mn.y); tmn[3 * i + 2] = S(mn.z);
             tmx[3 * i] = S(mx.x); tmx[3 * i + 1] = S(mx.y); tmx[3 * i + 2] = S(mx.z);
             NodeBox b;
@@ -244,11 +247,11 @@ __device__ __forceinline__ RayIn<S> load_ray(const Rays<S>& r, int i) {
     q.ok = qm::ray_finite(q.o, q.d, q.maxd);
     return q;
 }
-template <class S>
+template <bool CAPS, class S>
 __device__ __forceinline__ bool ray_leaf(const Tree<S>& t, const RayIn<S>& q, uint32_t c, double& th, nm::V3& nh) {
     const uint32_t memb = t.memb ? t.memb[c] : 1u;
     if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
-    return qm::ray_collider(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), q.o, q.d, q.maxd, q.solid, th, nh);
+    return qm::ray_collider<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), q.o, q.d, q.maxd, q.solid, th, nh);
 }
 __device__ __forceinline__ bool ray_visit(const NodeBox& b, nm::V3 o, nm::V3 d, double tclip) {
     return qm::ray_box_entry(&b.lo.x, &b.hi.x, o, d, tclip) != INFINITY;
@@ -284,7 +287,7 @@ __device__ __forceinline__ void traverse_closest(const Tree<S>& t, int m, nm::V3
     }
 }
 
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, int32_t* __restrict__ out_c,
                                                          S* __restrict__ out_t, S* __restrict__ out_n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -297,7 +300,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ 
         traverse_closest(t, *t.m, q.o, q.d, q.maxd, best_t, [&](uint32_t c) {
             double th;
             nm::V3 nh;
-            if (ray_leaf(t, q, c, th, nh) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_n = nh; }
+            if (ray_leaf<CAPS>(t, q, c, th, nh) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_n = nh; }
         });
     const bool hit = best_c != 0xffffffffu;
     out_c[i] = hit ? int32_t(best_c) : -1;
@@ -306,7 +309,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ 
 }
 
 // ray_hits count pass: every hit, and the part of it the ray keeps (max_hits)
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_ray_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, uint32_t* __restrict__ full,
                                                           uint32_t* __restrict__ kept) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -315,7 +318,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_count(const __grid_constant__
     uint32_t cnt = 0;
     if (q.ok)
         traverse(t, *t.m, [&](const NodeBox& b) { return ray_visit(b, q.o, q.d, q.maxd); },
-                 [&](uint32_t c) { double th; nm::V3 nh; if (ray_leaf(t, q, c, th, nh)) ++cnt; });
+                 [&](uint32_t c) { double th; nm::V3 nh; if (ray_leaf<CAPS>(t, q, c, th, nh)) ++cnt; });
     full[i] = cnt;
     const uint32_t mh = r.max_hits ? r.max_hits[i] : 0xffffffffu;
     kept[i] = cnt < mh ? cnt : mh;
@@ -345,7 +348,7 @@ __device__ void sort_segment(uint32_t n, Less less, Swap swp) {
 }
 
 // ray_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their normals
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, const uint64_t* __restrict__ full_off,
                                                          const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
                                                          uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ out_n) {
@@ -363,7 +366,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ 
              [&](uint32_t c) {
                  double th;
                  nm::V3 nh;
-                 if (ray_leaf(t, q, c, th, nh) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+                 if (ray_leaf<CAPS>(t, q, c, th, nh) && w < n) { ts[w] = th; cs[w] = c; ++w; }
              });
     sort_segment(
         w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
@@ -373,7 +376,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ 
         const uint32_t c = cs[k];
         double th;
         nm::V3 nh{0, 0, 0};
-        ray_leaf(t, q, c, th, nh);    // the same exact test again: the normal of this hit
+        ray_leaf<CAPS>(t, q, c, th, nh);    // the same exact test again: the normal of this hit
         out_c[o + k] = c;
         if (out_t) out_t[o + k] = S(ts[k]);
         if (out_n) { out_n[3 * (o + k)] = S(nh.x); out_n[3 * (o + k) + 1] = S(nh.y); out_n[3 * (o + k) + 2] = S(nh.z); }
@@ -428,7 +431,7 @@ struct ShapeIn {
     float ext[3], lo[3], hi[3];
     bool ok;
 };
-template <class S>
+template <bool CAPS, class S>
 __device__ __forceinline__ ShapeIn load_shape(const Shapes<S>& s, int i, bool cast) {
     ShapeIn q;
     q.shape = s.shape[i];
@@ -443,7 +446,7 @@ __device__ __forceinline__ ShapeIn load_shape(const Shapes<S>& s, int i, bool ca
     q.nx = s.xoff ? s.xoff[i + 1] - s.xoff[i] : 0u;
     q.ok = cast ? qm::cast_finite(q.he, q.c, q.q, q.d, q.maxd) : qm::collider_valid(q.he, q.c, q.q);
     if (q.ok) {
-        const nm::V3 e = qm::half_size(q.shape, q.he, qm::rot_mat(q.q));
+        const nm::V3 e = qm::half_size<CAPS>(q.shape, q.he, qm::rot_mat(q.q));
         for (int k = 0; k < 3; ++k) {
             float l, h;
             qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, h);
@@ -500,16 +503,16 @@ __device__ __forceinline__ void traverse_nearest(const Tree<S>& t, int m, const 
     }
 }
 
-template <class S>
+template <bool CAPS, class S>
 __device__ __forceinline__ bool cast_leaf(const Tree<S>& t, const ShapeIn& q, uint32_t c, double& th, int& axis) {
     const uint32_t memb = t.memb ? t.memb[c] : 1u;
     if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
-    return qm::cast_collider(q.shape, q.he, q.c, q.q, q.d, q.maxd, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+    return qm::cast_collider<CAPS>(q.shape, q.he, q.c, q.q, q.d, q.maxd, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
 }
-template <class S>
+template <bool CAPS, class S>
 __device__ __forceinline__ void cast_store(const Tree<S>& t, const ShapeIn& q, uint32_t c, double th, int axis, size_t o, S* p1, S* p2, S* n1, S* n2) {
     qm::ShapeContact h;
-    qm::cast_output(q.shape, q.he, q.c, q.q, q.d, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis, h);
+    qm::cast_output<CAPS>(q.shape, q.he, q.c, q.q, q.d, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis, h);
     const nm::V3 v[4] = {h.p1, h.p2, h.n1, h.n2};
     S* dst[4] = {p1, p2, n1, n2};
     for (int k = 0; k < 4; ++k)
@@ -518,12 +521,12 @@ __device__ __forceinline__ void cast_store(const Tree<S>& t, const ShapeIn& q, u
 __device__ __forceinline__ bool cast_visit(const NodeBox& b, const ShapeIn& q) { return grown_entry(b, q.ext, q.c, q.d, q.maxd) != INFINITY; }
 
 // cast_shape: the lexicographic minimum of (t, collider)
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_cast_shape(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, int32_t* __restrict__ out_c,
                                                            S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2, S* __restrict__ n1, S* __restrict__ n2) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape(s, i, true);
+    const ShapeIn q = load_shape<CAPS>(s, i, true);
     double best_t = INFINITY;
     uint32_t best_c = 0xffffffffu;
     int best_axis = -1;
@@ -532,43 +535,43 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_shape(const __grid_constant_
                                [&](uint32_t c) {
                                    double th;
                                    int ax;
-                                   if (cast_leaf(t, q, c, th, ax) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_axis = ax; }
+                                   if (cast_leaf<CAPS>(t, q, c, th, ax) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_axis = ax; }
                                });
     const bool hit = best_c != 0xffffffffu;
     out_c[i] = hit ? int32_t(best_c) : -1;
     out_t[i] = hit ? S(best_t) : S(0);
     if (hit) {
-        cast_store(t, q, best_c, best_t, best_axis, size_t(i), p1, p2, n1, n2);
+        cast_store<CAPS>(t, q, best_c, best_t, best_axis, size_t(i), p1, p2, n1, n2);
     } else {
         for (int k = 0; k < 3; ++k) p1[3 * i + k] = p2[3 * i + k] = n1[3 * i + k] = n2[3 * i + k] = S(0);
     }
 }
 
 // shape_hits count pass: every hit, and the part of it the query keeps (max_hits)
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ full,
                                                             uint32_t* __restrict__ kept) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape(s, i, true);
+    const ShapeIn q = load_shape<CAPS>(s, i, true);
     uint32_t cnt = 0;
     if (q.ok)
         traverse(t, *t.m, [&](const NodeBox& b) { return cast_visit(b, q); },
-                 [&](uint32_t c) { double th; int ax; if (cast_leaf(t, q, c, th, ax)) ++cnt; });
+                 [&](uint32_t c) { double th; int ax; if (cast_leaf<CAPS>(t, q, c, th, ax)) ++cnt; });
     full[i] = cnt;
     const uint32_t mh = s.max_hits ? s.max_hits[i] : 0xffffffffu;
     kept[i] = cnt < mh ? cnt : mh;
 }
 
 // shape_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their contacts
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, const uint64_t* __restrict__ full_off,
                                                            const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
                                                            uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2,
                                                            S* __restrict__ n1, S* __restrict__ n2) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape(s, i, true);
+    const ShapeIn q = load_shape<CAPS>(s, i, true);
     if (!q.ok) return;
     const uint64_t base = full_off[i];
     const uint32_t n = uint32_t(full_off[i + 1] - base), keep = uint32_t(kept_off[i + 1] - kept_off[i]);
@@ -580,7 +583,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant_
              [&](uint32_t c) {
                  double th;
                  int ax;
-                 if (cast_leaf(t, q, c, th, ax) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+                 if (cast_leaf<CAPS>(t, q, c, th, ax) && w < n) { ts[w] = th; cs[w] = c; ++w; }
              });
     sort_segment(
         w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
@@ -590,15 +593,15 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant_
         const uint32_t c = cs[k];
         double th = 0;
         int ax = -1;
-        cast_leaf(t, q, c, th, ax);    // the same exact test again: the axis of this hit
+        cast_leaf<CAPS>(t, q, c, th, ax);    // the same exact test again: the axis of this hit
         out_c[o + k] = c;
         if (out_t) out_t[o + k] = S(ts[k]);
-        cast_store(t, q, c, ts[k], ax, size_t(o + k), p1, p2, n1, n2);
+        cast_store<CAPS>(t, q, c, ts[k], ax, size_t(o + k), p1, p2, n1, n2);
     }
 }
 
 // project_point: the lexicographic minimum of (distance, collider); a node is pruned when its squared distance exceeds the best so far
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, int32_t* __restrict__ out_c,
                                                               S* __restrict__ out_p, uint8_t* __restrict__ out_in) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -619,7 +622,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_consta
                                     if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
                                     nm::V3 pr;
                                     bool in;
-                                    const double dd = qm::project_point(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p, solid, pr, in);
+                                    const double dd = qm::project_point<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p, solid, pr, in);
                                     if (qm::hit_before(dd, c, best_d, best_c)) { best_d = dd; best_c = c; best_p = pr; best_in = in; bound = dd * dd; }
                                 });
     const bool hit = best_c != 0xffffffffu;
@@ -629,7 +632,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_consta
 }
 
 // point_intersections: count, then emit + sort ascending by collider
-template <class S, bool EMIT>
+template <class S, bool EMIT, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, uint32_t* __restrict__ counts,
                                                             const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -645,7 +648,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant
                  [&](uint32_t c) {
                      const uint32_t memb = t.memb ? t.memb[c] : 1u;
                      if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
-                     if (!qm::contains_point(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p)) return;
+                     if (!qm::contains_point<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p)) return;
                      if (EMIT) seg[w] = c;
                      ++w;
                  });
@@ -654,12 +657,12 @@ __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant
 }
 
 // shape_intersections: count, then emit + sort ascending by collider
-template <class S, bool EMIT>
+template <class S, bool EMIT, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ counts,
                                                             const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape(s, i, false);
+    const ShapeIn q = load_shape<CAPS>(s, i, false);
     uint32_t w = 0;
     uint32_t* seg = EMIT ? out_c + off[i] : nullptr;
     if (q.ok)
@@ -668,7 +671,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant
                  [&](uint32_t c) {
                      const uint32_t memb = t.memb ? t.memb[c] : 1u;
                      if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return;
-                     if (!qm::shapes_intersect(q.shape, q.he, q.c, q.q, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c))) return;
+                     if (!qm::shapes_intersect<CAPS>(q.shape, q.he, q.c, q.q, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c))) return;
                      if (EMIT) seg[w] = c;
                      ++w;
                  });
@@ -686,13 +689,13 @@ struct Movers {
 };
 
 // the cast leaf of a move, out of line: the shape-cast geometry is instanced once in the move kernel, not at each inlined call site
-template <class S>
+template <bool CAPS, class S>
 __device__ __noinline__ bool move_cast_leaf(const Tree<S>& t, uint32_t c, int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& th, int& axis) {
-    return qm::cast_collider(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+    return qm::cast_collider<CAPS>(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
 }
 
 // the scene of move_math.hpp over the tree, with one character's filter
-template <class S>
+template <class S, bool CAPS>
 struct TreeScene {
     const Tree<S>& t;
     int m;
@@ -710,7 +713,7 @@ struct TreeScene {
     // the closest filtered cast: nearest-first over the node boxes grown by the shape's half size (as q_cast_shape)
     __device__ bool cast(int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& t_out, uint32_t& c_out, int& axis_out) const {
         float ext[3];
-        const nm::V3 e = qm::half_size(shape, he, qm::rot_mat(q));
+        const nm::V3 e = qm::half_size<CAPS>(shape, he, qm::rot_mat(q));
         for (int k = 0; k < 3; ++k) {
             float l;
             qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, ext[k]);
@@ -723,7 +726,7 @@ struct TreeScene {
                                    if (!pass(c)) return;
                                    double th;
                                    int ax;
-                                   if (move_cast_leaf(t, c, shape, he, ctr, q, d, maxd, th, ax) && qm::hit_before(th, c, best_t, best_c)) {
+                                   if (move_cast_leaf<CAPS>(t, c, shape, he, ctr, q, d, maxd, th, ax) && qm::hit_before(th, c, best_t, best_c)) {
                                        best_t = th; best_c = c; best_axis = ax;
                                    }
                                });
@@ -779,7 +782,7 @@ struct MoveHits {
     }
 };
 
-template <class S>
+template <class S, bool CAPS>
 __global__ void __launch_bounds__(Q_THREADS) q_move(const __grid_constant__ Tree<S> t, const __grid_constant__ Movers<S> mb, const __grid_constant__ mv::Config<S> cfg,
                                                      S* __restrict__ out_pos, S* __restrict__ out_vel, int32_t* __restrict__ hc, S* __restrict__ hd,
                                                      S* __restrict__ ht, S* __restrict__ hp, S* __restrict__ hn) {
@@ -804,9 +807,9 @@ __global__ void __launch_bounds__(Q_THREADS) q_move(const __grid_constant__ Tree
         if (mb.poff)
             for (uint32_t k = mb.poff[i]; k < mb.poff[i + 1]; ++k)
                 init[ni++] = mv::plane_dir(mv::T3<S>{mb.planes[3 * k], mb.planes[3 * k + 1], mb.planes[3 * k + 2]});
-        const TreeScene<S> sc{t, *t.m, mb.mask ? mb.mask[i] : 0xffffffffu, mb.xoff ? mb.xoff[i + 1] - mb.xoff[i] : 0u,
+        const TreeScene<S, CAPS> sc{t, *t.m, mb.mask ? mb.mask[i] : 0xffffffffu, mb.xoff ? mb.xoff[i + 1] - mb.xoff[i] : 0u,
                               mb.xoff ? mb.xs + mb.xoff[i] : nullptr, mb.ignored};
-        mv::move_and_slide(sc, cfg, b, pos, vel, init, ni, hits);
+        mv::move_and_slide<CAPS>(sc, cfg, b, pos, vel, init, ni, hits);
     }
     out_pos[3 * i] = pos.x; out_pos[3 * i + 1] = pos.y; out_pos[3 * i + 2] = pos.z;
     out_vel[3 * i] = vel.x; out_vel[3 * i + 1] = vel.y; out_vel[3 * i + 2] = vel.z;
@@ -819,12 +822,15 @@ class Queries final : public QueriesBase {
 
     AvnStatus update(const AvnQueryColliders* c, uint32_t flags) override {
         const bool keep_shapes = (flags & AVN_QUERY_SHAPES_UNCHANGED) != 0;
-        if (const char* why = qm::check_colliders(c, !keep_shapes, sizeof(S) == 8)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: %s", why);
+        bool saw_capsule = false;
+        if (const char* why = qm::check_colliders(c, !keep_shapes, sizeof(S) == 8, true, &saw_capsule))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: %s", why);
         if (keep_shapes && (!built_ || c->count != uint32_t(n_)))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: AVN_QUERY_SHAPES_UNCHANGED needs a previous update of the same count");
         const int n = int(c->count);
         built_ = false;
         n_ = n;
+        if (!keep_shapes) caps_ = saw_capsule;   // AVN_QUERY_SHAPES_UNCHANGED keeps the shape column, and with it whether it holds a capsule
         const size_t nn = size_t(std::max(n, 1));
         AVN_CUDA(pos_.ensure(3 * nn * sizeof(S)));
         AVN_CUDA(rot_.ensure(4 * nn * sizeof(S)));
@@ -863,7 +869,8 @@ class Queries final : public QueriesBase {
         const Tree<S> t = tree();
         if (n > 0) {
             const unsigned g = unsigned((n + 255) / 256);
-            q_prepare<S><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
+            if (caps_) q_prepare<S, true><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
+            else q_prepare<S, false><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
             q_codes<<<g, 256, 0, stream_>>>(n, centre_.as<float4>(), valid_.as<uint8_t>(), sb, k0_.as<uint32_t>(), v0_.as<uint32_t>());
             uint32_t *ka = k0_.as<uint32_t>(), *kb = k1_.as<uint32_t>(), *va = v0_.as<uint32_t>(), *vb = v1_.as<uint32_t>();
             for (int pass = 0; pass < 4; ++pass) {
@@ -899,7 +906,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(oc_.ensure(size_t(n) * 4));
         AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
         AVN_CUDA(on_.ensure(3 * size_t(n) * sizeof(S)));
-        q_cast_ray<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
+        const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        if (caps_) q_cast_ray<S, true><<<g, Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
+        else q_cast_ray<S, false><<<g, Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
@@ -919,7 +928,10 @@ class Queries final : public QueriesBase {
         AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
         const Tree<S> t = tree();
         const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
-        if (n > 0) q_ray_count<S><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        if (n > 0) {
+            if (caps_) q_ray_count<S, true><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+            else q_ray_count<S, false><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        }
         uint64_t tot[2];
         if ((st = scan(full_.as<uint32_t>(), n, full_off_.as<uint64_t>())) != AVN_OK) return st;
         if ((st = scan(kept_.as<uint32_t>(), n, kept_off_.as<uint64_t>())) != AVN_OK) return st;
@@ -936,8 +948,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(ot_.ensure(nk * sizeof(S)));
         AVN_CUDA(on_.ensure(3 * nk * sizeof(S)));
         if (n > 0 && tot[1] > 0) {
-            q_ray_emit<S><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
-                                                         oc_.as<uint32_t>(), ot_.as<S>(), on_.as<S>());
+            auto emit = caps_ ? q_ray_emit<S, true> : q_ray_emit<S, false>;
+            emit<<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
+                                               oc_.as<uint32_t>(), ot_.as<S>(), on_.as<S>());
             AVN_CUDA(cudaGetLastError());
         }
         return list_download(out, n, kept_off_.as<uint64_t>(), tot[1], true);
@@ -986,8 +999,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(oc_.ensure(size_t(n) * 4));
         AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
         for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * size_t(n) * sizeof(S)));
-        q_cast_shape<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), shapes_, oc_.as<int32_t>(), ot_.as<S>(), op1_.as<S>(),
-                                                                                             op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
+        auto cast = caps_ || shapes_caps_ ? q_cast_shape<S, true> : q_cast_shape<S, false>;
+        cast<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), shapes_, oc_.as<int32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(),
+                                                                                 on1_.as<S>(), on2_.as<S>());
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
@@ -1010,7 +1024,11 @@ class Queries final : public QueriesBase {
         AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
         const Tree<S> t = tree();
         const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
-        if (n > 0) q_shape_count<S><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        const bool caps = caps_ || shapes_caps_;
+        if (n > 0) {
+            auto count = caps ? q_shape_count<S, true> : q_shape_count<S, false>;
+            count<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+        }
         uint64_t tot[2];
         if ((st = scan(full_.as<uint32_t>(), n, full_off_.as<uint64_t>())) != AVN_OK) return st;
         if ((st = scan(kept_.as<uint32_t>(), n, kept_off_.as<uint64_t>())) != AVN_OK) return st;
@@ -1027,8 +1045,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(ot_.ensure(nk * sizeof(S)));
         for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * nk * sizeof(S)));
         if (n > 0 && tot[1] > 0) {
-            q_shape_emit<S><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
-                                                           oc_.as<uint32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
+            auto emit = caps ? q_shape_emit<S, true> : q_shape_emit<S, false>;
+            emit<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
+                                               oc_.as<uint32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
             AVN_CUDA(cudaGetLastError());
         }
         AVN_CUDA(cudaMemcpyAsync(out->offsets, kept_off_.as<uint64_t>(), size_t(n + 1) * 8, cudaMemcpyDeviceToHost, stream_));
@@ -1055,7 +1074,8 @@ class Queries final : public QueriesBase {
         AVN_CUDA(oc_.ensure(size_t(n) * 4));
         AVN_CUDA(op1_.ensure(3 * size_t(n) * sizeof(S)));
         AVN_CUDA(oin_.ensure(size_t(n)));
-        q_project_point<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), points_, oc_.as<int32_t>(), op1_.as<S>(), oin_.as<uint8_t>());
+        auto project = caps_ ? q_project_point<S, true> : q_project_point<S, false>;
+        project<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), points_, oc_.as<int32_t>(), op1_.as<S>(), oin_.as<uint8_t>());
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(out->point, op1_.p, 3 * size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
@@ -1070,8 +1090,8 @@ class Queries final : public QueriesBase {
         if ((st = list_out(out, "avn_query_point_intersections")) != AVN_OK) return st;
         const int n = int(p->count);
         return intersections(n, out, "avn_query_point_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
-            if (counts) q_point_isect<S, false><<<g, Q_THREADS, 0, stream_>>>(t, points_, counts, nullptr, nullptr);
-            else q_point_isect<S, true><<<g, Q_THREADS, 0, stream_>>>(t, points_, nullptr, off, oc);
+            if (counts) (caps_ ? q_point_isect<S, false, true> : q_point_isect<S, false, false>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, counts, nullptr, nullptr);
+            else (caps_ ? q_point_isect<S, true, true> : q_point_isect<S, true, false>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, nullptr, off, oc);
         });
     }
 
@@ -1080,15 +1100,18 @@ class Queries final : public QueriesBase {
         if (st != AVN_OK) return st;
         if ((st = list_out(out, "avn_query_shape_intersections")) != AVN_OK) return st;
         const int n = int(s->count);
+        const bool caps = caps_ || shapes_caps_;
         return intersections(n, out, "avn_query_shape_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
-            if (counts) q_shape_isect<S, false><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, counts, nullptr, nullptr);
-            else q_shape_isect<S, true><<<g, Q_THREADS, 0, stream_>>>(t, shapes_, nullptr, off, oc);
+            if (counts) (caps ? q_shape_isect<S, false, true> : q_shape_isect<S, false, false>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, counts, nullptr, nullptr);
+            else (caps ? q_shape_isect<S, true, true> : q_shape_isect<S, true, false>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, nullptr, off, oc);
         });
     }
 
     AvnStatus move_and_slide(const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) override {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide before any avn_query_update");
-        if (const char* why = mv::check_move(cfg, b, sizeof(S) == 8, uint32_t(n_))) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: %s", why);
+        bool batch_caps = false;
+        if (const char* why = mv::check_move(cfg, b, sizeof(S) == 8, uint32_t(n_), true, &batch_caps))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: %s", why);
         if (!out || (b->count && (!out->position || !out->velocity)))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: position and velocity outputs are required");
         out->kernel_ms = 0.f;
@@ -1127,8 +1150,8 @@ class Queries final : public QueriesBase {
             AVN_CUDA(cudaEventCreate(&ev_[1]));
         }
         AVN_CUDA(cudaEventRecord(ev_[0], stream_));
-        q_move<S><<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), mb, mv::config_of<S>(cfg), op1_.as<S>(), op2_.as<S>(), hc, hd, ht,
-                                                                                       hp, hn);
+        auto move = caps_ || batch_caps ? q_move<S, true> : q_move<S, false>;
+        move<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), mb, mv::config_of<S>(cfg), op1_.as<S>(), op2_.as<S>(), hc, hd, ht, hp, hn);
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaEventRecord(ev_[1], stream_));
         AVN_CUDA(cudaMemcpyAsync(out->position, op1_.p, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
@@ -1178,7 +1201,7 @@ class Queries final : public QueriesBase {
     // validate on the host, then upload the shape columns into shapes_ (cast: the cast-only columns too)
     AvnStatus shapes_in(const AvnShapeBatch* s, bool cast, const char* what) {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
-        if (const char* why = qm::check_shapes(s, cast, sizeof(S) == 8)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
+        if (const char* why = qm::check_shapes(s, cast, sizeof(S) == 8, true, &shapes_caps_)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
         const size_t n = s->count;
         shapes_ = Shapes<S>{};
         shapes_.n = int(n);
@@ -1293,6 +1316,8 @@ class Queries final : public QueriesBase {
     cudaStream_t stream_;
     ErrorSink* err_;
     bool built_ = false, has_memb_ = false;
+    bool caps_ = false;                              // the tree's shape column holds a capsule
+    bool shapes_caps_ = false;                       // the last shape batch holds a capsule
     int n_ = 0;
     Rays<S> rays_{};
     Shapes<S> shapes_{};

@@ -1,4 +1,4 @@
-// Spatial-query geometry for cuboid / sphere colliders, written once for the host fixture (g++, -ffp-contract=off) and for the device
+// Spatial-query geometry for cuboid / sphere / capsule colliders, written once for the host fixture (g++, -ffp-contract=off) and for the device
 // (nvcc, -fmad=false): the same expressions in the same order, IEEE double throughout, so both evaluate to the same bits.
 //
 // What this is: OUR ray and AABB arithmetic.  The reference delegates it to parry3d 0.25 (Cuboid / Ball ray casts, compute_aabb), which is
@@ -23,6 +23,13 @@
 //   * Filter: a collider passes when (memberships & mask) != 0 and it is not in the ray's excluded list.
 //   * AABB test: inclusive compares on all three axes (Aabb::intersects) against the tight AABB, with no filter.
 //   * A collider with a non-finite pose or dims, or a zero rotation quaternion, is never reported (negative dims are refused); a ray with a non-finite origin, direction or max_distance hits nothing.
+//   * Capsules (DESIGN.md §7j): dims = [radius, half_length, unused], the segment from (0, -hl, 0) to (0, +hl, 0) of the collider frame, every
+//     rotation through rot_mat.  AABB: the two posed segment ends, componentwise min / max, grown by the radius.  Ray vs capsule, closed form:
+//     the infinite cylinder's quadratic (a = |d x u|², discriminant a r² - |(o - c) x u x (d x u)|², Lagrange's identity) kept when the root's
+//     axial coordinate lies within [-hl, hl], and the two end spheres (a r² - |(o - e) x d|²); the smallest valid root (the largest exit for a
+//     hollow ray from inside).  Normal: unit(hit - closest point of the segment).  half_length = 0 is a sphere, radius = 0 a closed segment.
+//   Every capsule routine is out of line (NM_COLD) and compiled only into the CAPS = true instances of the templates below, so the cuboid /
+//   sphere code is what it was before capsules were queried.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -54,8 +61,19 @@ NM_HD inline nm::M3 rot_mat(Q q) {
     return m;
 }
 
-// compute_aabb(isometry): cuboid centre ± |R|·he (R = rotation matrix, columns = world directions of the local axes), sphere centre ± r
+// capsule AABB: the segment ends p ∓ u·hl (u = rot_mat(q)'s local y), componentwise min / max, grown by the radius
+NM_HD inline void capsule_aabb(V3 he, V3 p, Q q, V3& mn, V3& mx) {
+    const V3 u = rot_mat(q).c[1];
+    const V3 a = p - u * he.y, b = p + u * he.y;
+    mn = V3{nm::smin(a.x, b.x) - he.x, nm::smin(a.y, b.y) - he.x, nm::smin(a.z, b.z) - he.x};
+    mx = V3{nm::smax(a.x, b.x) + he.x, nm::smax(a.y, b.y) + he.x, nm::smax(a.z, b.z) + he.x};
+}
+
+// compute_aabb(isometry): cuboid centre ± |R|·he (R = rotation matrix, columns = world directions of the local axes), sphere centre ± r,
+// capsule_aabb (CAPS only)
+template <bool CAPS = false>
 NM_HD inline void collider_aabb(int shape, V3 he, V3 p, Q q, V3& mn, V3& mx) {
+    if (CAPS && shape == nm::SHAPE_CAPSULE) { capsule_aabb(he, p, q, mn, mx); return; }
     V3 e;
     if (shape == nm::SHAPE_SPHERE) {
         e = V3{he.x, he.x, he.x};
@@ -130,9 +148,66 @@ NM_HD inline bool ray_sphere(S radius, V3 centre, V3 o, V3 d, bool solid, S& t, 
     return true;
 }
 
+// ray vs capsule: oc = origin - segment centre, u = unit axis, h = half length, r = radius.  Closed: a point at distance <= r from the segment is
+// inside.  Outside: the smallest entry of the lateral surface (root kept when its axial coordinate lies in [-h, h]) and of the two end spheres;
+// ties go to the lateral surface, then the -h end.  Inside and hollow: the largest exit of the same three (the capsule is convex, so the last
+// exit is the capsule's).  The normal is unit(hit - closest segment point), 0 on the segment itself (radius 0).
+NM_COLD inline bool ray_capsule_rel(V3 oc, V3 u, S h, S r, V3 d, bool solid, S& t, V3& n) {
+    const S r2 = r * r;
+    const S s0 = nm::smax(-h, nm::smin(h, nm::dot(oc, u)));
+    const V3 e0 = oc - u * s0;
+    const bool inside = nm::dot(e0, e0) <= r2;
+    if (inside && solid) { t = 0; n = V3{0, 0, 0}; return true; }
+    const S a = nm::dot(d, d);
+    if (a == 0) return false;                // zero direction: never reaches the surface
+    S best = inside ? -INFINITY : INFINITY;
+    bool found = false;
+    // lateral surface: |(oc + t d) x u|² = r²
+    const V3 w = nm::cross(oc, u), v = nm::cross(d, u);
+    const S al = nm::dot(v, v);
+    if (al > 0) {
+        const V3 x = nm::cross(w, v);
+        const S disc = al * r2 - nm::dot(x, x);
+        if (disc >= 0) {
+            const S sq = sqrt(disc), b = nm::dot(w, v);
+            const S tc = inside ? (-b + sq) / al : (-b - sq) / al;
+            const S ax = nm::dot(oc + d * tc, u);
+            if (ax >= -h && ax <= h && (inside || tc >= 0)) { best = tc; found = true; }
+        }
+    }
+NM_ROLLED
+    for (int i = 0; i < 2; ++i) {            // the end spheres at -h, +h
+        const V3 oe = oc - u * (i == 0 ? -h : h);
+        const V3 x = nm::cross(oe, d);
+        const S disc = a * r2 - nm::dot(x, x);
+        if (disc < 0) continue;
+        const S sq = sqrt(disc), b = nm::dot(oe, d);
+        if (inside) {
+            const S te = (-b + sq) / a;
+            if (te > best) { best = te; found = true; }
+        } else {
+            const S ts = (-b - sq) / a;
+            if (ts >= 0 && ts < best) { best = ts; found = true; }
+        }
+    }
+    if (!found || best < 0) return false;
+    t = best;
+    const V3 hp = oc + d * t;
+    const V3 e = hp - u * nm::smax(-h, nm::smin(h, nm::dot(hp, u)));
+    const S l = nm::len(e);
+    n = l > 0 ? e * (1 / l) : V3{0, 0, 0};
+    return true;
+}
+NM_HD inline bool ray_capsule(V3 he, V3 p, Q q, V3 o, V3 d, bool solid, S& t, V3& n) {
+    return ray_capsule_rel(o - p, rot_mat(q).c[1], he.y, he.x, d, solid, t, n);
+}
+
 // one collider, acceptance included: hit when 0 <= t <= max_distance
+template <bool CAPS = false>
 NM_HD inline bool ray_collider(int shape, V3 he, V3 p, Q q, V3 o, V3 d, S max_distance, bool solid, S& t, V3& n) {
-    const bool hit = shape == nm::SHAPE_SPHERE ? ray_sphere(he.x, p, o, d, solid, t, n) : ray_cuboid(he, p, q, o, d, solid, t, n);
+    const bool hit = CAPS && shape == nm::SHAPE_CAPSULE ? ray_capsule(he, p, q, o, d, solid, t, n)
+                   : shape == nm::SHAPE_SPHERE          ? ray_sphere(he.x, p, o, d, solid, t, n)
+                                                        : ray_cuboid(he, p, q, o, d, solid, t, n);
     return hit && t >= 0 && t <= max_distance;
 }
 
@@ -180,7 +255,7 @@ NM_HD inline S ray_box_entry(const float* lo, const float* hi, V3 o, V3 d, S tma
     return t0 <= t1 ? t0 : INFINITY;
 }
 
-// ---- shape casts, point projection, point and shape intersections (cuboid / sphere) ---------------------------------------------------
+// ---- shape casts, point projection, point and shape intersections (cuboid / sphere / capsule) ------------------------------------------
 // Reference call sites: spatial_query/pipeline.rs:315-615 (cast_shape, shape_hits, project_point), 617-683 (point_intersections), 731-826
 // (shape_intersections), shape_caster.rs:335-400 (ShapeCaster::cast).  The reference hands the arithmetic to parry3d; these conventions are ours.
 //
@@ -215,12 +290,34 @@ NM_HD inline S ray_box_entry(const float* lo, const float* hi, V3 o, V3 d, S tma
 //     closest point for sphere-cuboid, centre distance for two spheres.  Both apply the filter.
 //   * A query shape with a non-finite pose, dims, direction or max_distance, or a zero quaternion, hits nothing; a point that is not finite
 //     projects onto nothing and lies in nothing.  A sphere of radius 0 is legal.
+//   * Capsules (CAPS = true instances only; DESIGN.md §7j).  Every cast kind with a capsule is an exact TOI on [0, max_distance]:
+//       - sphere-capsule, capsule-sphere: a solid ray cast of the sphere's centre (+d, or -d when the capsule is cast) against the capsule grown
+//         to rA + rB (ray_capsule_rel).
+//       - capsule-capsule: the origin moving along d against the parallelogram P = (cB - cA) + {uB s - uA σ} grown by R = rA + rB
+//         (seg_seg_toi): the minimum of the four edge casts (an end point of one segment against the other capsule of radius R, as a ray vs
+//         capsule) and of the two faces of P offset by ±R along uA x uB, a face hit counting only inside P.  Parallel axes (uA x uB = 0) have
+//         no face; the edge casts cover them.
+//       - capsule-cuboid, cuboid-capsule: the capsule's two end points against the box rounded by r (point_rounded_box_toi) and the segment
+//         against the box's 12 edges as segment-segment casts of radius r.  Exact: two convex shapes first touch at a feature pair, and a
+//         segment's interior first touches a face's interior only when the two are parallel, when its end points touch at the same t.
+//     Overlap at t = 0 (TOI 0): the closest-feature distance of the pair is at most the summed radii (segment-segment, segment-point,
+//     segment-box with 0 when the segment meets the closed box).
+//     Outputs: nm::capsule_round / nm::box_capsule at the TOI pose with no distance limit, so the normals and the fallbacks for coincident or
+//     crossing axes are the narrow phase's (§7h).  A contact that is a continuum (parallel segments, a capsule lying on a face) has two
+//     witnesses there; the first is reported: the end of the overlap at the lower parameter along the capsule's axis (A's axis for two
+//     capsules).
+//   * Capsule projection: the closest segment point + r · unit(p - closest); a point on the axis goes along the capsule's local +x.  Inside and
+//     hollow: to the surface along p - closest.  Containment: dist(p, segment) <= r.  Intersections: capsule-sphere and capsule-capsule compare
+//     the segment distance with the summed radii, capsule-cuboid the exact segment-box distance (0 when the segment meets the box) with r.
 
 constexpr uint32_t CAST_IGNORE_ORIGIN_PENETRATION = 0x1u;   // = AVN_CAST_IGNORE_ORIGIN_PENETRATION
 constexpr uint32_t CAST_NO_CONTACT_ON_PENETRATION = 0x2u;   // = AVN_CAST_NO_CONTACT_ON_PENETRATION
 
-// half size of the tight AABB of a shape (collider_aabb's e)
+// half size of the tight AABB of a shape (collider_aabb's e; for a capsule |u|·hl + r, u = r.c[1])
+template <bool CAPS = false>
 NM_HD inline V3 half_size(int shape, V3 he, const nm::M3& r) {
+    if (CAPS && shape == nm::SHAPE_CAPSULE)
+        return V3{fabs(r.c[1].x) * he.y + he.x, fabs(r.c[1].y) * he.y + he.x, fabs(r.c[1].z) * he.y + he.x};
     if (shape == nm::SHAPE_SPHERE) return V3{he.x, he.x, he.x};
     return V3{fabs(r.c[0].x) * he.x + fabs(r.c[1].x) * he.y + fabs(r.c[2].x) * he.z,
               fabs(r.c[0].y) * he.x + fabs(r.c[1].y) * he.y + fabs(r.c[2].y) * he.z,
@@ -432,11 +529,193 @@ NM_HD inline void box_box_witness(const nm::Box& A, const nm::Box& B, int axis, 
     if (ref_is_a) { c.p2 = on_ref; c.p1 = w; } else { c.p1 = on_ref; c.p2 = w; }
 }
 
+// ---- capsule casts, contacts, projection and intersections (out of line: only the CAPS instances call them) ------------------------------
+
+// squared distance from p (relative to the segment's centre) to the segment of unit axis u, half length h; the clamped parameter in s
+NM_HD inline S segment_point_d2(V3 p, V3 u, S h, S& s) {
+    s = nm::smax(-h, nm::smin(h, nm::dot(p, u)));
+    const V3 e = p - u * s;
+    return nm::dot(e, e);
+}
+
+// whether the segment of C meets the closed box b: its parameter interval clipped by the three slabs is not empty
+NM_HD inline bool segment_meets_box(const nm::Box& b, const nm::Capsule& C) {
+    S lo = -C.h, hi = C.h;
+NM_ROLLED
+    for (int k = 0; k < 3; ++k) {
+        const S a = nm::dot(b.r.c[k], C.c - b.c), g = nm::dot(b.r.c[k], C.u), he = nm::comp(b.he, k);
+        if (g == 0) {
+            if (fabs(a) > he) return false;
+            continue;
+        }
+        const S s0 = (-he - a) / g, s1 = (he - a) / g;
+        lo = nm::smax(lo, nm::smin(s0, s1));
+        hi = nm::smin(hi, nm::smax(s0, s1));
+    }
+    return lo <= hi;
+}
+
+// the exact distance between C's segment and the box b: 0 when they meet, else nm::segment_box_closest
+NM_COLD inline S segment_box_distance(const nm::Box& b, const nm::Capsule& C) {
+    if (segment_meets_box(b, C)) return 0;
+    V3 on_seg, on_box;
+    return nm::segment_box_closest(b, C, on_seg, on_box);
+}
+
+// The origin moving along d against P = c + {ub s - ua σ : |s| <= hb, |σ| <= ha} grown by R: the first t >= 0 at which the segment
+// (0, ua, ha) moved by d t comes within R of the segment (c, ub, hb).  t = 0 when it already is.
+NM_COLD inline bool seg_seg_toi(V3 c, V3 ua, S ha, V3 ub, S hb, S R, V3 d, S& t) {
+    S s, u;
+    nm::segment_closest(V3{0, 0, 0}, ua, ha, c, ub, hb, s, u);
+    const V3 g = (c + ub * u) - ua * s;
+    if (nm::dot(g, g) <= R * R) { t = 0; return true; }
+    S best = INFINITY;
+    V3 n;
+NM_ROLLED
+    for (int i = 0; i < 4; ++i) {            // the edges of P: B's ends -hb, +hb along ua, A's ends -ha, +ha along ub
+        const bool b_end = i < 2;
+        const S sg = (i & 1) ? 1 : -1;
+        const V3 e = b_end ? c + ub * (sg * hb) : c - ua * (sg * ha);
+        S ti;
+        if (ray_capsule_rel(-e, b_end ? ua : ub, b_end ? ha : hb, R, d, true, ti, n) && ti < best) best = ti;
+    }
+    const V3 m = nm::cross(ua, ub);
+    const S lm2 = nm::dot(m, m);
+    if (lm2 > 0) {                           // the faces of P offset by ±R, entered from the side d comes from
+        const V3 mn = m * (1 / sqrt(lm2));
+        const S dn = nm::dot(d, mn);
+        if (dn != 0) {
+            const S tf = (nm::dot(c, mn) - (dn > 0 ? R : -R)) / dn;
+            if (tf >= 0 && tf < best) {
+                const V3 y = d * tf - c;
+                const S yb = nm::dot(y, ub), ya = nm::dot(y, ua), cab = nm::dot(ua, ub);
+                const S sb = (yb - cab * ya) / lm2, sa = (cab * yb - ya) / lm2;
+                if (fabs(sb) <= hb && fabs(sa) <= ha) best = tf;
+            }
+        }
+    }
+    if (best == INFINITY) return false;
+    t = best;
+    return true;
+}
+
+// capsule C moving along v against the box b (rotation r): the end points against the rounded box, the segment against the 12 edges
+NM_COLD inline bool capsule_box_toi(const nm::Capsule& C, const nm::Box& b, V3 v, S maxd, S& t) {
+    if (segment_box_distance(b, C) <= C.r) { t = 0; return true; }
+    S best = INFINITY;
+    const V3 lv = to_local(b.r, v);
+NM_ROLLED
+    for (int i = 0; i < 2; ++i) {
+        S ti;
+        const V3 e = C.c + C.u * (i == 0 ? -C.h : C.h);
+        if (point_rounded_box_toi(to_local(b.r, e - b.c), lv, b.he, C.r, maxd, ti) && ti < best) best = ti;
+    }
+NM_ROLLED
+    for (int ei = 0; ei < 12; ++ei) {
+        const int k = ei >> 2, m = ei & 3, u = (k + 1) % 3, w = (k + 2) % 3;
+        const V3 ec = b.c + b.r.c[u] * (m & 1 ? nm::comp(b.he, u) : -nm::comp(b.he, u)) + b.r.c[w] * (m & 2 ? nm::comp(b.he, w) : -nm::comp(b.he, w));
+        S ti;
+        if (seg_seg_toi(ec - C.c, C.u, C.h, b.r.c[k], nm::comp(b.he, k), C.r, v, ti) && ti < best) best = ti;
+    }
+    if (best == INFINITY) return false;
+    t = best;
+    return true;
+}
+
+NM_HD inline nm::Capsule capsule_of(V3 he, V3 c, Q q) { return nm::Capsule{c, rot_mat(q).c[1], he.y, he.x}; }
+
+// radius of a sphere about the centre that holds the shape
+NM_HD inline S bounding_radius(int shape, V3 he) {
+    if (shape == nm::SHAPE_CAPSULE) return he.x + he.y;
+    if (shape == nm::SHAPE_SPHERE) return he.x;
+    return nm::len(he);
+}
+
+// the TOI of a pair with at least one capsule (A moves along d).  First a conservative cull: the two bounding spheres, grown by 1e-6
+// relative, never meet on [0, maxd] -> no hit (the constructions below are exact; the cull only skips them for far pairs).
+NM_COLD inline bool capsule_cast_toi(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, int sb, V3 hb, V3 cb, Q qb, S& t) {
+    S tb;
+    if (!sphere_sphere_toi(ca, d, cb, (bounding_radius(sa, ha) + bounding_radius(sb, hb)) * (1 + 1e-6), tb) || tb > maxd) return false;
+    V3 n;
+    if (sa == nm::SHAPE_SPHERE) return ray_capsule_rel(ca - cb, rot_mat(qb).c[1], hb.y, ha.x + hb.x, d, true, t, n);
+    if (sb == nm::SHAPE_SPHERE) return ray_capsule_rel(cb - ca, rot_mat(qa).c[1], ha.y, ha.x + hb.x, -d, true, t, n);
+    if (sa == nm::SHAPE_CAPSULE && sb == nm::SHAPE_CAPSULE)
+        return seg_seg_toi(cb - ca, rot_mat(qa).c[1], ha.y, rot_mat(qb).c[1], hb.y, ha.x + hb.x, d, t);
+    if (sa == nm::SHAPE_CAPSULE) return capsule_box_toi(capsule_of(ha, ca, qa), nm::Box{cb, rot_mat(qb), hb}, d, maxd, t);
+    return capsule_box_toi(capsule_of(hb, cb, qb), nm::Box{ca, rot_mat(qa), ha}, -d, maxd, t);
+}
+
+// the contact of a capsule pair with A at `at`: the narrow phase's closest features with no distance limit, the first witness pair
+NM_COLD inline void capsule_cast_contact(int sa, V3 ha, V3 at, Q qa, int sb, V3 hb, V3 cb, Q qb, ShapeContact& c) {
+    nm::Contacts pts;
+    pts.clear();
+    V3 n{0, 1, 0};
+    bool a_first;                            // whether pts / n run from A to B (else from B to A)
+    if (sa == nm::SHAPE_CAPSULE && sb != nm::SHAPE_CUBOID) {
+        const nm::Capsule A = capsule_of(ha, at, qa);
+        if (sb == nm::SHAPE_CAPSULE) nm::capsule_round(A, cb, rot_mat(qb).c[1], hb.y, hb.x, INFINITY, n, pts);
+        else nm::capsule_round(A, cb, A.u, 0, hb.x, INFINITY, n, pts);
+        a_first = true;
+    } else if (sa == nm::SHAPE_SPHERE) {     // B is the capsule
+        const nm::Capsule B = capsule_of(hb, cb, qb);
+        nm::capsule_round(B, at, B.u, 0, ha.x, INFINITY, n, pts);
+        a_first = false;
+    } else if (sa == nm::SHAPE_CAPSULE) {    // B is a cuboid: box_capsule runs from the box to the capsule
+        nm::box_capsule(nm::Box{cb, rot_mat(qb), hb}, capsule_of(ha, at, qa), INFINITY, n, pts);
+        a_first = false;
+    } else {                                 // A is a cuboid, B the capsule
+        nm::box_capsule(nm::Box{at, rot_mat(qa), ha}, capsule_of(hb, cb, qb), INFINITY, n, pts);
+        a_first = true;
+    }
+    if (a_first) { c.n2 = n; c.n1 = -n; c.p2 = pts.p[0].a; c.p1 = pts.p[0].b; }
+    else { c.n1 = n; c.n2 = -n; c.p1 = pts.p[0].a; c.p2 = pts.p[0].b; }
+}
+
+// project_point against a capsule
+NM_COLD inline S capsule_project(V3 he, V3 c, Q q, V3 p, bool solid, V3& proj, bool& inside) {
+    const nm::M3 r = rot_mat(q);
+    S s;
+    const V3 rel = p - c;
+    const S l2 = segment_point_d2(rel, r.c[1], he.y, s);
+    inside = l2 <= he.x * he.x;
+    if (inside && solid) { proj = p; return 0; }
+    const V3 foot = r.c[1] * s, e = rel - foot;
+    const S l = sqrt(l2);
+    proj = c + (l > 0 ? foot + e * (he.x / l) : foot + r.c[0] * he.x);
+    return nm::len(proj - p);
+}
+
+// closed intersection of a pair with at least one capsule
+NM_COLD inline bool capsule_intersect(int sa, V3 ha, V3 ca, Q qa, int sb, V3 hb, V3 cb, Q qb) {
+    const bool a_cap = sa == nm::SHAPE_CAPSULE;
+    const int so = a_cap ? sb : sa;
+    const V3 hc = a_cap ? ha : hb, ho = a_cap ? hb : ha, cc = a_cap ? ca : cb, co = a_cap ? cb : ca;
+    const Q qc = a_cap ? qa : qb, qo = a_cap ? qb : qa;
+    const nm::Capsule C = capsule_of(hc, cc, qc);
+    if (so == nm::SHAPE_SPHERE) {
+        S s;
+        const S R = hc.x + ho.x;
+        return segment_point_d2(co - cc, C.u, C.h, s) <= R * R;
+    }
+    if (so == nm::SHAPE_CAPSULE) {
+        S s, t;
+        const V3 uo = rot_mat(qo).c[1];
+        nm::segment_closest(cc, C.u, C.h, co, uo, ho.y, s, t);
+        const V3 e = (co + uo * t) - (cc + C.u * s);
+        const S R = hc.x + ho.x;
+        return nm::dot(e, e) <= R * R;
+    }
+    return segment_box_distance(nm::Box{co, rot_mat(qo), ho}, C) <= C.r;
+}
+
 // The TOI of cast shape A against collider B (before the origin-penetration flag); axis: the box-box SAT axis the cast chose
+template <bool CAPS = false>
 NM_HD inline bool cast_toi(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, int sb, V3 hb, V3 cb, Q qb, S& t, int& axis) {
     axis = -1;
     bool hit;
-    if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
+    if (CAPS && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) {
+        hit = capsule_cast_toi(sa, ha, ca, qa, d, maxd, sb, hb, cb, qb, t);
+    } else if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
         hit = sphere_sphere_toi(ca, d, cb, ha.x + hb.x, t);
     } else if (sa == nm::SHAPE_SPHERE) {                 // the sphere's centre moves with +d against B's rounded box
         const nm::M3 r = rot_mat(qb);
@@ -451,9 +730,12 @@ NM_HD inline bool cast_toi(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, int sb, V3 
 }
 
 // points and normals of a cast hit at TOI t (A at ca + d t)
+template <bool CAPS = false>
 NM_HD inline void cast_contact(int sa, V3 ha, V3 ca, Q qa, V3 d, int sb, V3 hb, V3 cb, Q qb, S t, int axis, ShapeContact& c) {
     const V3 at = ca + d * t;
-    if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
+    if (CAPS && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) {
+        capsule_cast_contact(sa, ha, at, qa, sb, hb, cb, qb, c);
+    } else if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
         const V3 e = at - cb;
         const S l = nm::len(e);
         c.n1 = l > 0 ? e * (1 / l) : V3{0, 1, 0};
@@ -487,29 +769,33 @@ NM_HD inline void cast_contact(int sa, V3 ha, V3 ca, Q qa, V3 d, int sb, V3 hb, 
 }
 
 // one collider, acceptance included: the TOI in [0, max_distance] and the origin-penetration flag
+template <bool CAPS = false>
 NM_HD inline bool cast_collider(int sa, V3 ha, V3 ca, Q qa, V3 d, S maxd, uint32_t flags, int sb, V3 hb, V3 cb, Q qb, S& t, int& axis) {
-    if (!cast_toi(sa, ha, ca, qa, d, maxd, sb, hb, cb, qb, t, axis)) return false;
+    if (!cast_toi<CAPS>(sa, ha, ca, qa, d, maxd, sb, hb, cb, qb, t, axis)) return false;
     if (t == 0 && (flags & CAST_IGNORE_ORIGIN_PENETRATION)) {
         ShapeContact c;
-        cast_contact(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
+        cast_contact<CAPS>(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
         if (nm::dot(d, c.n1) > 0) return false;
     }
     return true;
 }
 
 // the outputs of a hit: its contact, or zeros for a TOI-0 hit with AVN_CAST_NO_CONTACT_ON_PENETRATION
+template <bool CAPS = false>
 NM_HD inline void cast_output(int sa, V3 ha, V3 ca, Q qa, V3 d, uint32_t flags, int sb, V3 hb, V3 cb, Q qb, S t, int axis, ShapeContact& c) {
     if (t == 0 && (flags & CAST_NO_CONTACT_ON_PENETRATION)) {
         c.p1 = c.p2 = c.n1 = c.n2 = V3{0, 0, 0};
         return;
     }
-    cast_contact(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
+    cast_contact<CAPS>(sa, ha, ca, qa, d, sb, hb, cb, qb, t, axis, c);
 }
 
 NM_HD inline bool cast_finite(V3 he, V3 c, Q q, V3 d, S maxd) { return collider_valid(he, c, q) && finite3(d) && std::isfinite(maxd); }
 
 // project_point against one collider: the projection, inside or not; returns |projection - p|
+template <bool CAPS = false>
 NM_HD inline S project_point(int shape, V3 he, V3 c, Q q, V3 p, bool solid, V3& proj, bool& inside) {
+    if (CAPS && shape == nm::SHAPE_CAPSULE) return capsule_project(he, c, q, p, solid, proj, inside);
     if (shape == nm::SHAPE_SPHERE) {
         const V3 e = p - c;
         const S l2 = nm::dot(e, e);
@@ -539,7 +825,12 @@ NM_HD inline S project_point(int shape, V3 he, V3 c, Q q, V3 p, bool solid, V3& 
 }
 
 // closed containment
+template <bool CAPS = false>
 NM_HD inline bool contains_point(int shape, V3 he, V3 c, Q q, V3 p) {
+    if (CAPS && shape == nm::SHAPE_CAPSULE) {
+        S s;
+        return segment_point_d2(p - c, rot_mat(q).c[1], he.y, s) <= he.x * he.x;
+    }
     if (shape == nm::SHAPE_SPHERE) {
         const V3 e = p - c;
         return nm::dot(e, e) <= he.x * he.x;
@@ -548,7 +839,9 @@ NM_HD inline bool contains_point(int shape, V3 he, V3 c, Q q, V3 p) {
 }
 
 // closed intersection of two posed shapes
+template <bool CAPS = false>
 NM_HD inline bool shapes_intersect(int sa, V3 ha, V3 ca, Q qa, int sb, V3 hb, V3 cb, Q qb) {
+    if (CAPS && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) return capsule_intersect(sa, ha, ca, qa, sb, hb, cb, qb);
     if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
         const V3 e = ca - cb;
         const S R = ha.x + hb.x;
@@ -599,7 +892,11 @@ inline const char* check_rays(const AvnRayBatch* r) {
     }
     return nullptr;
 }
-inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_required, bool f64) {
+// the dims a shape reads: a cuboid's three half extents, a sphere's radius, a capsule's radius and half length
+inline int shape_dims_read(uint8_t shape) { return shape == AVN_SHAPE_SPHERE ? 1 : (shape == AVN_SHAPE_CAPSULE ? 2 : 3); }
+// capsules: whether AVN_SHAPE_CAPSULE is accepted; saw_capsule (optional): set when the column holds one
+inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_required, bool f64, bool capsules = false, bool* saw_capsule = nullptr) {
+    if (saw_capsule) *saw_capsule = false;
     if (!c) return "colliders are required";
     if (c->count >= 0x80000000u) return "colliders: at most 2^31 - 1";
     if (c->count == 0) return nullptr;
@@ -607,11 +904,13 @@ inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_requi
     if (shapes_required) {
         if (!c->shape || !c->dims) return "colliders: shape and dims are required";
         for (uint32_t i = 0; i < c->count; ++i) {
-            if (c->shape[i] > AVN_SHAPE_SPHERE) return "colliders: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
-            for (int k = 0; k < (c->shape[i] == AVN_SHAPE_SPHERE ? 1 : 3); ++k) {
+            if (!capsules && c->shape[i] > AVN_SHAPE_SPHERE) return "colliders: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
+            if (c->shape[i] > AVN_SHAPE_CAPSULE) return "colliders: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
+            for (int k = 0; k < shape_dims_read(c->shape[i]); ++k) {
                 const double v = f64 ? static_cast<const double*>(c->dims)[3 * size_t(i) + k] : static_cast<const float*>(c->dims)[3 * size_t(i) + k];
-                if (v < 0) return "colliders: negative half extent or radius";
+                if (v < 0) return "colliders: negative half extent, radius or half length";
             }
+            if (saw_capsule && c->shape[i] == AVN_SHAPE_CAPSULE) *saw_capsule = true;
         }
     }
     return nullptr;
@@ -626,18 +925,21 @@ inline const char* check_exclusions(uint32_t count, uint32_t exclude_count, cons
     return nullptr;
 }
 // cast: the batch feeds a shape cast (direction and max_distance required, target_distance must be 0)
-inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64) {
+inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64, bool capsules = false, bool* saw_capsule = nullptr) {
+    if (saw_capsule) *saw_capsule = false;
     if (!s) return "shape batch is required";
     if (s->count >= 0x7fffffffu) return "shapes: too many shapes";
     if (s->count == 0) return nullptr;
     if (!s->shape || !s->dims || !s->position || !s->rotation) return "shapes: shape, dims, position and rotation are required";
     if (cast && (!s->direction || !s->max_distance)) return "shapes: direction and max_distance are required for a cast";
     for (uint32_t i = 0; i < s->count; ++i) {
-        if (s->shape[i] > AVN_SHAPE_SPHERE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
-        for (int k = 0; k < (s->shape[i] == AVN_SHAPE_SPHERE ? 1 : 3); ++k) {
+        if (!capsules && s->shape[i] > AVN_SHAPE_SPHERE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
+        if (s->shape[i] > AVN_SHAPE_CAPSULE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
+        for (int k = 0; k < shape_dims_read(s->shape[i]); ++k) {
             const double v = f64 ? static_cast<const double*>(s->dims)[3 * size_t(i) + k] : static_cast<const float*>(s->dims)[3 * size_t(i) + k];
-            if (v < 0) return "shapes: negative half extent or radius";
+            if (v < 0) return "shapes: negative half extent, radius or half length";
         }
+        if (saw_capsule && s->shape[i] == AVN_SHAPE_CAPSULE) *saw_capsule = true;
         if (cast && s->target_distance) {
             const double td = f64 ? static_cast<const double*>(s->target_distance)[i] : static_cast<const float*>(s->target_distance)[i];
             if (td != 0) return "shapes: target_distance must be 0 (a cast with a target distance is not supported)";

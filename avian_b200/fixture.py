@@ -137,13 +137,22 @@ def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders:
     return out
 
 
-# ---- spatial queries by brute force over every collider (csrc/query_math.hpp): what the device tree must reproduce bit for bit
+# ---- spatial queries by brute force over every collider (csrc/query_math.hpp): what the device tree must reproduce bit for bit.
+# capsules=True accepts capsule colliders and query shapes (characters for move_and_slide); without it a capsule is refused as an unknown
+# shape.  The device accepts capsules with no flag.
 def _query_check(lib, st: int) -> None:
     if st != api.OK:
         raise api.AvianError(st, lib.avh_query_error().decode())
 
 
-def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays") -> dict:
+CAPSULE_BIT = 0x100   # OR-ed into scalar_bits: the brute force accepts capsule colliders, query shapes and characters
+
+
+def _bits(dt, capsules: bool) -> int:
+    return (32 if dt == np.float32 else 64) | (CAPSULE_BIT if capsules else 0)
+
+
+def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False) -> dict:
     """The closest hit of every ray (same output as Context.cast_ray)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
@@ -151,31 +160,31 @@ def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays") ->
     n = rays.count
     out = {"collider": np.zeros(n, dtype=np.int32), "distance": np.zeros(n, dtype=dt), "normal": np.zeros((n, 3), dtype=dt)}
     o = api.AvnRayClosest(*(_p(out[k]) for k in ("collider", "distance", "normal")))
-    _query_check(lib, lib.avh_query_cast_ray(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(o)))
+    _query_check(lib, lib.avh_query_cast_ray(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(o)))
     return out
 
 
-def query_ray_hits(scalar, colliders: "api.QueryColliders", rays: "api.Rays") -> dict:
+def query_ray_hits(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False) -> dict:
     """Every ray's max_hits nearest hits in (t, collider) order as CSR (same output as Context.ray_hits)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     r, keep_r = rays.as_struct(dt)
     h, out = api.hit_list(rays.count, 0, dt, True)
-    st = lib.avh_query_ray_hits(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(h))
+    st = lib.avh_query_ray_hits(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(h))
     if st == api.ERR_CAPACITY:
         h, out = api.hit_list(rays.count, int(h.count), dt, True)
-        st = lib.avh_query_ray_hits(32 if dt == np.float32 else 64, C.byref(c), C.byref(r), C.byref(h))
+        st = lib.avh_query_ray_hits(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
 
 
-def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, aabb_max) -> dict:
+def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, aabb_max, capsules: bool = False) -> dict:
     """Per query box the colliders whose tight AABB it touches, ascending (same output as Context.aabb_intersections)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     mn = np.ascontiguousarray(aabb_min, dtype=dt).reshape(-1, 3)
     mx = np.ascontiguousarray(aabb_max, dtype=dt).reshape(-1, 3)
-    n, bits = int(mn.shape[0]), 32 if dt == np.float32 else 64
+    n, bits = int(mn.shape[0]), _bits(dt, capsules)
     h, out = api.hit_list(n, 0, dt, False)
     st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
     if st == api.ERR_CAPACITY:
@@ -185,22 +194,22 @@ def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, 
     return api.hit_list_result(h, out)
 
 
-def query_cast_shape(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+def query_cast_shape(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
     """The closest hit of every cast (same output as Context.cast_shape)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     s, keep_s = shapes.as_struct(dt)
     o, out = api.shape_closest(shapes.count, dt)
-    _query_check(lib, lib.avh_query_cast_shape(32 if dt == np.float32 else 64, C.byref(c), C.byref(s), C.byref(o)))
+    _query_check(lib, lib.avh_query_cast_shape(_bits(dt, capsules), C.byref(c), C.byref(s), C.byref(o)))
     return out
 
 
-def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
     """Every cast's max_hits nearest hits in (t, collider) order as CSR (same output as Context.shape_hits)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     s, keep_s = shapes.as_struct(dt)
-    bits = 32 if dt == np.float32 else 64
+    bits = _bits(dt, capsules)
     h, out = api.shape_hit_list(shapes.count, 0, dt)
     st = lib.avh_query_shape_hits(bits, C.byref(c), C.byref(s), C.byref(h))
     if st == api.ERR_CAPACITY:
@@ -210,21 +219,21 @@ def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.Shape
     return api.hit_list_result(h, out)
 
 
-def query_project_point(scalar, colliders: "api.QueryColliders", points: "api.Points") -> dict:
+def query_project_point(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False) -> dict:
     """The closest collider of every point and the projection onto it (same output as Context.project_point)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     p, keep_p = points.as_struct(dt)
     o, out = api.point_projection(points.count, dt)
-    _query_check(lib, lib.avh_query_project_point(32 if dt == np.float32 else 64, C.byref(c), C.byref(p), C.byref(o)))
+    _query_check(lib, lib.avh_query_project_point(_bits(dt, capsules), C.byref(c), C.byref(p), C.byref(o)))
     return out
 
 
-def _query_list(fn, scalar, colliders, batch) -> dict:
+def _query_list(fn, scalar, colliders, batch, capsules: bool) -> dict:
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     b, keep_b = batch.as_struct(dt)
-    bits, n = 32 if dt == np.float32 else 64, batch.count
+    bits, n = _bits(dt, capsules), batch.count
     h, out = api.hit_list(n, 0, dt, False)
     st = getattr(lib, fn)(bits, C.byref(c), C.byref(b), C.byref(h))
     if st == api.ERR_CAPACITY:
@@ -234,25 +243,25 @@ def _query_list(fn, scalar, colliders, batch) -> dict:
     return api.hit_list_result(h, out)
 
 
-def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "api.Points") -> dict:
+def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False) -> dict:
     """Per point the colliders containing it, ascending (same output as Context.point_intersections)."""
-    return _query_list("avh_query_point_intersections", scalar, colliders, points)
+    return _query_list("avh_query_point_intersections", scalar, colliders, points, capsules)
 
 
-def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries") -> dict:
+def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
     """Per query shape the colliders it intersects, ascending (same output as Context.shape_intersections)."""
-    return _query_list("avh_query_shape_intersections", scalar, colliders, shapes)
+    return _query_list("avh_query_shape_intersections", scalar, colliders, shapes, capsules)
 
 
 # ---- move and slide by brute force over every collider (csrc/move_math.hpp): what the device kernel must reproduce bit for bit
-def move_and_slide(scalar, colliders: "api.QueryColliders", config: "api.MoveConfig", batch: "api.MoveBatch") -> dict:
+def move_and_slide(scalar, colliders: "api.QueryColliders", config: "api.MoveConfig", batch: "api.MoveBatch", capsules: bool = False) -> dict:
     """MoveAndSlide::move_and_slide for every character (same output as Context.move_and_slide; kernel_ms is 0)."""
     lib, dt = _load(), np.dtype(scalar)
     c, keep_c = colliders.as_struct(dt)
     m, keep_m = config.as_struct()
     b, keep_b = batch.as_struct(dt)
     o, out = api.move_result(batch.count, config.move_and_slide_iterations, dt)
-    _query_check(lib, lib.avh_move_and_slide(32 if dt == np.float32 else 64, C.byref(c), C.byref(m), C.byref(b), C.byref(o)))
+    _query_check(lib, lib.avh_move_and_slide(_bits(dt, capsules), C.byref(c), C.byref(m), C.byref(b), C.byref(o)))
     out["kernel_ms"] = 0.0
     return out
 

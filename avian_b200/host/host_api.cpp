@@ -747,7 +747,13 @@ uint32_t avh_pair_count(AvhPipeline* h) { return uint32_t(reinterpret_cast<Pipel
 
 // ---- spatial queries, brute force over every collider (the checker of csrc/queries.cu; same header, same conventions) ----------------
 // Arguments are the ABI structs of avn_query_*; the colliders are passed with every call.  Returns an AvnStatus; avh_query_error() says why.
+// scalar_bits: 32 or 64 selects the column type; OR-ed with AVH_CAPSULES (0x100) it also accepts capsule colliders, query shapes and
+// characters.  Without that bit a capsule is refused as an unknown shape, as it was before capsules were queried.  The geometry is always
+// the CAPS = true instance of csrc/query_math.hpp, which gives the CAPS = false bits on cuboids and spheres.
 namespace {
+constexpr uint32_t AVH_CAPSULES = 0x100u;
+bool bits_f64(uint32_t scalar_bits) { return (scalar_bits & 0xffu) == 64; }
+bool bits_caps(uint32_t scalar_bits) { return (scalar_bits & AVH_CAPSULES) != 0; }
 thread_local char g_query_error[256];
 int query_fail(AvnStatus st, const char* why) {
     snprintf(g_query_error, sizeof g_query_error, "%s", why);
@@ -783,7 +789,7 @@ void all_hits(const QueryScene& sc, const RayView& v, std::vector<RayHit>& out) 
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
         RayHit h{0, c, V3{0, 0, 0}};
-        if (qm::ray_collider(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), v.o, v.d, v.maxd, v.solid, h.t, h.n)) out.push_back(h);
+        if (qm::ray_collider<true>(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), v.o, v.d, v.maxd, v.solid, h.t, h.n)) out.push_back(h);
     }
     std::sort(out.begin(), out.end(), [](const RayHit& a, const RayHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
 }
@@ -792,7 +798,7 @@ void query_aabbs(const QueryScene& sc, uint32_t n, const T* mn, const T* mx, std
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c)) continue;
         V3 a, b;
-        qm::collider_aabb(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), a, b);
+        qm::collider_aabb<true>(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), a, b);
         const T tmn[3] = {T(a.x), T(a.y), T(a.z)}, tmx[3] = {T(b.x), T(b.y), T(b.z)};
         for (uint32_t i = 0; i < n; ++i)
             if (qm::aabb_overlap(mn + 3 * size_t(i), mx + 3 * size_t(i), tmn, tmx)) per[i].push_back(c);
@@ -800,7 +806,7 @@ void query_aabbs(const QueryScene& sc, uint32_t n, const T* mn, const T* mx, std
 }
 
 int query_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r) {
-    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     if (r)
         if (const char* why = qm::check_rays(r)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
@@ -814,7 +820,7 @@ const char* avh_query_error() { return g_query_error; }
 int avh_query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out) {
     if (int st = query_inputs(scalar_bits, c, r)) return st;
     if (!out || (r->count && (!out->collider || !out->distance || !out->normal))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     ColW ot{out->distance, f64}, on{out->normal, f64};
     std::vector<RayHit> hits;
@@ -830,7 +836,7 @@ int avh_query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const A
 int avh_query_ray_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out) {
     if (int st = query_inputs(scalar_bits, c, r)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     std::vector<std::vector<RayHit>> per(r->count);
     uint64_t total = 0;
@@ -861,9 +867,9 @@ int avh_query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* 
     if (int st = query_inputs(scalar_bits, c, nullptr)) return st;
     if (n && (!mn || !mx)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "min and max are required");
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const QueryScene sc(c, scalar_bits == 64);
+    const QueryScene sc(c, bits_f64(scalar_bits));
     std::vector<std::vector<uint32_t>> per(n);
-    if (scalar_bits == 64) query_aabbs(sc, n, static_cast<const double*>(mn), static_cast<const double*>(mx), per);
+    if (bits_f64(scalar_bits)) query_aabbs(sc, n, static_cast<const double*>(mn), static_cast<const double*>(mx), per);
     else query_aabbs(sc, n, static_cast<const float*>(mn), static_cast<const float*>(mx), per);
     uint64_t total = 0;
     for (const auto& v : per) total += v.size();
@@ -907,23 +913,23 @@ void all_cast_hits(const QueryScene& sc, const ShapeView& v, std::vector<CastHit
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
         CastHit h{0, c, -1};
-        if (qm::cast_collider(v.shape, v.he, v.c, v.q, v.d, v.maxd, v.flags, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), h.t, h.axis))
+        if (qm::cast_collider<true>(v.shape, v.he, v.c, v.q, v.d, v.maxd, v.flags, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), h.t, h.axis))
             out.push_back(h);
     }
     std::sort(out.begin(), out.end(), [](const CastHit& a, const CastHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
 }
 qm::ShapeContact cast_contact_of(const QueryScene& sc, const ShapeView& v, const CastHit& h) {
     qm::ShapeContact k;
-    qm::cast_output(v.shape, v.he, v.c, v.q, v.d, v.flags, sc.c->shape[h.c], sc.dims.v3(h.c), sc.pos.v3(h.c), sc.rot.q(h.c), h.t, h.axis, k);
+    qm::cast_output<true>(v.shape, v.he, v.c, v.q, v.d, v.flags, sc.c->shape[h.c], sc.dims.v3(h.c), sc.pos.v3(h.c), sc.rot.q(h.c), h.t, h.axis, k);
     return k;
 }
 int shape_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, bool cast) {
-    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
-    if (const char* why = qm::check_shapes(s, cast, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_shapes(s, cast, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
 }
 int point_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p) {
-    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     if (const char* why = qm::check_points(p)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
 }
@@ -948,7 +954,7 @@ int avh_query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const
     if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
     if (!out || (s->count && (!out->collider || !out->distance || !out->point1 || !out->point2 || !out->normal1 || !out->normal2)))
         return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     ColW ot{out->distance, f64}, p1{out->point1, f64}, p2{out->point2, f64}, n1{out->normal1, f64}, n2{out->normal2, f64};
     std::vector<CastHit> hits;
@@ -967,7 +973,7 @@ int avh_query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const
 int avh_query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeHitList* out) {
     if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     std::vector<std::vector<CastHit>> per(s->count);
     uint64_t total = 0;
@@ -1002,7 +1008,7 @@ int avh_query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const
 int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnPointProjection* out) {
     if (int st = point_inputs(scalar_bits, c, p)) return st;
     if (!out || (p->count && (!out->collider || !out->point || !out->is_inside))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     Col pc{p->point, f64};
     ColW op{out->point, f64};
@@ -1021,7 +1027,7 @@ int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, co
                 if (!sc.valid(col) || !qm::passes_filter(sc.memb(col), mask, xs, nx, col)) continue;
                 V3 pr;
                 bool in;
-                const S d = qm::project_point(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x, solid, pr, in);
+                const S d = qm::project_point<true>(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x, solid, pr, in);
                 if (qm::hit_before(d, col, best_d, best_c)) { best_d = d; best_c = col; best_p = pr; best_in = in; }
             }
         const bool hit = best_c != 0xffffffffu;
@@ -1035,7 +1041,7 @@ int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, co
 int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnHitList* out) {
     if (int st = point_inputs(scalar_bits, c, p)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     Col pc{p->point, f64};
     std::vector<std::vector<uint32_t>> per(p->count);
@@ -1047,7 +1053,7 @@ int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders*
         const uint32_t nx = p->exclude_offsets ? p->exclude_offsets[i + 1] - p->exclude_offsets[i] : 0u;
         for (uint32_t col = 0; col < c->count; ++col)
             if (sc.valid(col) && qm::passes_filter(sc.memb(col), mask, xs, nx, col) &&
-                qm::contains_point(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x))
+                qm::contains_point<true>(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x))
                 per[i].push_back(col);
     }
     return write_list(out, per);
@@ -1056,7 +1062,7 @@ int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders*
 int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnHitList* out) {
     if (int st = shape_inputs(scalar_bits, c, s, false)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const bool f64 = scalar_bits == 64;
+    const bool f64 = bits_f64(scalar_bits);
     const QueryScene sc(c, f64);
     std::vector<std::vector<uint32_t>> per(s->count);
     for (uint32_t i = 0; i < s->count; ++i) {
@@ -1064,7 +1070,7 @@ int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders*
         if (!v.ok) continue;
         for (uint32_t col = 0; col < c->count; ++col)
             if (sc.valid(col) && qm::passes_filter(sc.memb(col), v.mask, v.xs, v.nx, col) &&
-                qm::shapes_intersect(v.shape, v.he, v.c, v.q, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col)))
+                qm::shapes_intersect<true>(v.shape, v.he, v.c, v.q, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col)))
                 per[i].push_back(col);
     }
     return write_list(out, per);
@@ -1092,7 +1098,7 @@ struct HostMoveScene {
             if (!valid[c] || !pass(c)) continue;
             double th;
             int ax;
-            if (qm::cast_collider(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), th, ax) &&
+            if (qm::cast_collider<true>(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), th, ax) &&
                 qm::hit_before(th, c, best_t, best_c)) {
                 best_t = th; best_c = c; best_axis = ax;
             }
@@ -1132,7 +1138,7 @@ void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMov
         valid[k] = sc.valid(k);
         if (!valid[k]) continue;
         V3 a, e;
-        qm::collider_aabb(c->shape[k], sc.dims.v3(k), sc.pos.v3(k), sc.rot.q(k), a, e);
+        qm::collider_aabb<true>(c->shape[k], sc.dims.v3(k), sc.pos.v3(k), sc.rot.q(k), a, e);
         tmn[3 * k] = T(a.x); tmn[3 * k + 1] = T(a.y); tmn[3 * k + 2] = T(a.z);
         tmx[3 * k] = T(e.x); tmx[3 * k + 1] = T(e.y); tmx[3 * k + 2] = T(e.z);
     }
@@ -1160,7 +1166,7 @@ void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMov
             const HostMoveScene<T> ms{sc, valid.data(), tmn.data(), tmx.data(), b->mask ? b->mask[i] : 0xffffffffu,
                                       b->exclude_offsets ? b->exclude_offsets[i + 1] - b->exclude_offsets[i] : 0u,
                                       b->exclude_offsets ? b->exclude + b->exclude_offsets[i] : nullptr, cfg->ignored};
-            mv::move_and_slide(ms, mc, bd, p, v, init, ni, hits);
+            mv::move_and_slide<true>(ms, mc, bd, p, v, init, ni, hits);
         }
         opos[3 * i] = p.x; opos[3 * i + 1] = p.y; opos[3 * i + 2] = p.z;
         ovel[3 * i] = v.x; ovel[3 * i + 1] = v.y; ovel[3 * i + 2] = v.z;
@@ -1172,11 +1178,11 @@ extern "C" {
 
 // MoveAndSlide::move_and_slide for every character of the batch against every collider: the same output as avn_move_and_slide
 int avh_move_and_slide(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) {
-    if (const char* why = qm::check_colliders(c, true, scalar_bits == 64)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
-    if (const char* why = mv::check_move(cfg, b, scalar_bits == 64, c->count)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (const char* why = mv::check_move(cfg, b, bits_f64(scalar_bits), c->count, bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     if (!out || (b->count && (!out->position || !out->velocity))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "position and velocity outputs are required");
     out->kernel_ms = 0.f;
-    if (scalar_bits == 64) move_all<double>(c, cfg, b, out);
+    if (bits_f64(scalar_bits)) move_all<double>(c, cfg, b, out);
     else move_all<float>(c, cfg, b, out);
     return AVN_OK;
 }
@@ -1208,11 +1214,11 @@ int avh_move_contact(uint32_t scalar_bits, int sa, const double* ha, const doubl
     bool hit;
     if (scalar_bits == 64) {
         double pen = 0;
-        hit = mv::contact_plane<double>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        hit = mv::contact_plane<double, true>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
         *penetration = pen;
     } else {
         float pen = 0;
-        hit = mv::contact_plane<float>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        hit = mv::contact_plane<float, true>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
         *penetration = pen;
     }
     normal[0] = n.x; normal[1] = n.y; normal[2] = n.z;

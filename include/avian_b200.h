@@ -371,8 +371,8 @@ AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
 
 /* ---- collider AABBs (SURVEY.md 8f "next #2"): update_aabb for the shapes the device knows ------------------------------- */
 /* AVN_SHAPE_CAPSULE: Collider::capsule(radius, length), dims = [radius, length / 2, unused]; the segment runs from (0, -length/2, 0) to
- * (0, +length/2, 0) in the collider frame.  The AABB update, the narrow phase and the contact store take capsules; the spatial queries, move
- * and slide and swept CCD refuse them. */
+ * (0, +length/2, 0) in the collider frame.  The AABB update, the narrow phase, the contact store, the spatial queries (colliders and query
+ * shapes) and move and slide (obstacles and characters) take capsules; swept CCD refuses them. */
 typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2 } AvnShape;
 
 typedef struct AvnAabbParams {
@@ -660,13 +660,15 @@ AvnStatus avn_islands_wake(AvnContext* ctx, const uint8_t* wake, AvnIslandsWake*
 AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep);
 
 /* ---- spatial queries (SpatialQueryPlugin, src/lib.rs:839; spatial_query/pipeline.rs): a collider tree rebuilt on the device by every
- *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid and sphere colliders.
+ *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid, sphere and capsule colliders.
  *      The per-shape arithmetic is this repository's own (avian_b200/csrc/query_math.hpp, shared with the host fixture; parry3d is not
  *      vendored), so results equal the host brute force over every collider bit for bit, independent of the tree.  Conventions:
  *        - a ray is origin + t * direction, t in units of |direction| (pass a unit Dir3); a hit counts when 0 <= t <= max_distance;
  *        - shapes are closed; origin inside and solid -> t = 0, normal 0; origin inside and hollow -> the exit, outward normal there;
  *        - cuboid normal: outward normal of the entering face (largest entering slab parameter, ties to the lowest local axis); a direction
  *          component that is exactly 0 leaves its axis unconstrained when the origin is inside that slab and misses otherwise;
+ *        - capsule: tight AABB = the posed segment ends' min / max grown by the radius; normal = unit(hit - closest segment point); a
+ *          radius-0 capsule is a closed segment (avian_b200/csrc/query_math.hpp, DESIGN.md §7j);
  *        - filter (SpatialQueryFilter::test, query_filter.rs:97-101): (memberships & mask) != 0 and not in the ray's excluded list;
  *        - AABB test: inclusive compares (Aabb::intersects) against the collider's tight AABB (compute_aabb) rounded to the column scalar,
  *          no filter, as pipeline.rs:709-729;
@@ -676,7 +678,7 @@ AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uin
  *      Stated deviations: the closest hit is the lexicographic minimum of (t, collider index), where the reference takes the first in tree
  *      order; ray_hits keeps the max_hits NEAREST hits sorted by (t, collider index) — RayHits::iter_sorted order — where the reference keeps
  *      the first max_hits in tree order, unordered (pipeline.rs:213-216); the two sets are equal when a ray has no more than max_hits hits.
- *      Shape casts, point projection and point / shape intersections (cuboid and sphere query shapes) are further down, with their own
+ *      Shape casts, point projection and point / shape intersections (cuboid, sphere and capsule query shapes) are further down, with their own
  *      conventions.  Not covered: target_distance != 0, other shapes, predicates and the *_callback early exits, several GPUs. ------------- */
 typedef struct AvnQueryColliders {
     uint32_t count;
@@ -842,7 +844,7 @@ AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* sh
  *      Stated deviations: on_hit cannot run on the device — every hit is accepted and nothing edits the normal, position or velocity; the
  *      closest sweep hit is the lowest (t, collider index), not the first in tree order; intersections are visited in ascending collider
  *      index, not tree order; hit_toi reports the TOI, where MoveHitData::collision_distance is the requested movement length (:777);
- *      characters are cuboids and spheres. ------------------------------------------------------------------------------------------- */
+ *      characters are cuboids, spheres and capsules (capsule conventions: avian_b200/csrc/query_math.hpp, DESIGN.md §7j). ------------- */
 #define AVN_MOVE_MAX_PLANES 32
 
 /* MoveAndSlideConfig, one per call.  The reference's defaults: skin_width 0.01, max_depenetration_error 0.0001,
