@@ -435,7 +435,7 @@ REPORT_EVENTS_ONLY = 0x1
 
 
 class AvnCcdConfig(C.Structure):
-    _fields_ = [("count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("body", "collider", "mode", "include_dynamic", "linear_threshold",
+    _fields_ = [("count", C.c_uint32), ("flags", C.c_uint32)] + [(n, _vp) for n in ("body", "collider", "mode", "include_dynamic", "linear_threshold",
                                                                                    "angular_threshold")] + [("prediction_distance", C.c_double)]
 
 
@@ -444,17 +444,18 @@ class AvnCcdResult(C.Structure):
 
 
 SWEEP_LINEAR, SWEEP_NON_LINEAR = 0, 1
+CCD_CAPSULES = 0x1   # AvnCcdConfig.flags: capsule colliders take part in swept CCD
 
 
 def ccd_config(body, collider, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
-               prediction_distance: float = float("inf")) -> tuple["AvnCcdConfig", tuple]:
-    """An AvnCcdConfig over numpy copies of the columns (returned alongside: they must outlive the struct's use)."""
+               prediction_distance: float = float("inf"), flags: int = 0) -> tuple["AvnCcdConfig", tuple]:
+    """An AvnCcdConfig over numpy copies of the columns (returned alongside: they must outlive the struct's use).  flags: CCD_CAPSULES or 0."""
     cols = (np.ascontiguousarray(body, dtype=np.int32), np.ascontiguousarray(collider, dtype=np.uint32),
             None if mode is None else np.ascontiguousarray(mode, dtype=np.uint8),
             None if include_dynamic is None else np.ascontiguousarray(include_dynamic, dtype=np.uint8),
             None if linear_threshold is None else np.ascontiguousarray(linear_threshold, dtype=np.float64),
             None if angular_threshold is None else np.ascontiguousarray(angular_threshold, dtype=np.float64))
-    return AvnCcdConfig(int(cols[0].shape[0]), 0, *(_ptr(a) for a in cols), float(prediction_distance)), cols
+    return AvnCcdConfig(int(cols[0].shape[0]), int(flags), *(_ptr(a) for a in cols), float(prediction_distance)), cols
 
 
 QUERY_SHAPES_UNCHANGED = 1
@@ -1164,13 +1165,15 @@ class Context:
 
     # ---- swept CCD (include/avian_b200.h avn_ccd_*): solve_swept_ccd inside the device-resident solver stage
     def ccd_configure(self, body=None, collider=None, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
-                      prediction_distance: float = float("inf")) -> None:
-        """avn_ccd_configure: the SweptCcd bodies in query order and their own colliders; body=None clears the configuration."""
+                      prediction_distance: float = float("inf"), capsules: bool = False) -> None:
+        """avn_ccd_configure: the SweptCcd bodies in query order and their own colliders; body=None clears the configuration.  capsules=True
+        sets AVN_CCD_CAPSULES: capsule colliders are swept (without it a contact store that holds one is refused)."""
         if body is None or len(body) == 0:
             self._check(self.lib.avn_ccd_configure(self.handle, None))
             self._ccd_n = 0
             return
-        cfg, cols = ccd_config(body, collider, mode, include_dynamic, linear_threshold, angular_threshold, prediction_distance)
+        cfg, cols = ccd_config(body, collider, mode, include_dynamic, linear_threshold, angular_threshold, prediction_distance,
+                               CCD_CAPSULES if capsules else 0)
         self._check(self.lib.avn_ccd_configure(self.handle, C.byref(cfg)))
         self._ccd_n = int(cfg.count)
 

@@ -360,11 +360,13 @@ AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const
 // swept CCD (ccd.cu): solve_swept_ccd inside avn_solver_run
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
     return guarded(ctx, [&] {
+        if (config && config->count && (config->flags & ~AVN_CCD_CAPSULES))
+            return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "ccd_configure: unknown flags 0x%x (only AVN_CCD_CAPSULES)", config->flags & ~AVN_CCD_CAPSULES);
         avn::ContactsBase::AsleepBodies asleep;
         ctx->contacts->asleep_bodies(&asleep);
         if (asleep.body_asleep && config && config->count)
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
-        if (config && config->count && ctx->contacts->has_capsule())
+        if (config && config->count && !(config->flags & AVN_CCD_CAPSULES) && ctx->contacts->has_capsule())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a capsule; capsule times of impact are not implemented");
         if (config && config->count && ctx->contacts->body_frames())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: body frames are set (avn_contacts_set_body_frames); swept CCD assumes a collider at its body's origin");

@@ -1,4 +1,4 @@
-// Swept continuous collision detection (solve_swept_ccd, dynamics/ccd/mod.rs:523-780) for cuboid / sphere colliders: the pair time of impact,
+// Swept continuous collision detection (solve_swept_ccd, dynamics/ccd/mod.rs:523-780) for cuboid / sphere / capsule colliders: the pair time of impact,
 // the per-pair filters and the delta arithmetic, written once for the host fixture (g++, -ffp-contract=off) and for the device pass
 // (csrc/ccd.cu, nvcc -fmad=false): the same expressions in the same order, so both evaluate to the same bits.
 //
@@ -19,6 +19,11 @@
 //     The iterates do not depend on t_max, so evaluating every candidate against dt and keeping the minimum equals the reference's
 //     sequential scan with a shrinking bound.
 //   * eps = CCD_EPS_PER_LENGTH_UNIT * PhysicsLengthUnit.
+//   * Capsules (the CAPS = true instances; DESIGN.md §7e): dims = [radius, half length, ·], the segment along the collider's local y
+//     (rot_mat(q(t)).c[1], as qm::capsule_of).  Linear mode: qm::cast_toi<true>'s exact capsule casts.  Non-linear mode: capsule_distance
+//     (point-segment, nm::segment_closest, or 0 when qm::segment_meets_box and else nm::segment_box_closest, less the radii; the swapped
+//     orders negate n), and R = |(|lc.x|, |lc.y| + half length, |lc.z|)| + radius.  Every capsule branch is out of line and comes first,
+//     so with no capsule in the pair the TOI is the CAPS = false one, bit for bit.
 //   * sin / cos of from_scaled_axis come from ccd_sincos below (Cody-Waite reduction, Taylor polynomials, no libm), so the host and the
 //     device round identically in f64 too; otherwise the expression tree is avn_math.cuh's q_from_scaled_axis and qmul.
 #pragma once
@@ -107,8 +112,10 @@ struct Motion {
     V3 v, w;     // linear / angular velocity
 };
 
-// farthest point of the shape from its centre of mass
+// farthest point of the shape from its centre of mass (a capsule: the farther end of its segment, plus the radius)
+template <bool CAPS = false>
 NM_HD inline S motion_radius(const Motion& m) {
+    if (CAPS && m.shape == nm::SHAPE_CAPSULE) return nm::len(V3{fabs(m.lc.x), fabs(m.lc.y) + m.he.y, fabs(m.lc.z)}) + m.he.x;
     if (m.shape == nm::SHAPE_SPHERE) return nm::len(m.lc) + m.he.x;
     const V3 e{fabs(m.lc.x) + m.he.x, fabs(m.lc.y) + m.he.y, fabs(m.lc.z) + m.he.z};
     return nm::len(e);
@@ -124,9 +131,42 @@ NM_HD inline void pose_at(const Motion& m, S t, V3& origin, nm::M3& r) {
     r = qm::rot_mat(qt);
 }
 
+// shape_distance of a pair with at least one capsule C (A when A is one) and the other shape O: the segment's distance to O's centre, to O's
+// segment (nm::segment_closest) or to O's box (0 when the segment meets it, else nm::segment_box_closest), less the radii
+NM_COLD inline S capsule_distance(int sa, V3 ha, V3 ca, const nm::M3& ra, int sb, V3 hb, V3 cb, const nm::M3& rb, V3& n) {
+    n = V3{0, 1, 0};
+    const bool a_cap = sa == nm::SHAPE_CAPSULE;
+    const int so = a_cap ? sb : sa;
+    const V3 hc = a_cap ? ha : hb, ho = a_cap ? hb : ha, co = a_cap ? cb : ca;
+    const nm::M3& rc = a_cap ? ra : rb;
+    const nm::M3& ro = a_cap ? rb : ra;
+    const nm::Capsule C{a_cap ? ca : cb, rc.c[1], hc.y, hc.x};
+    V3 e;        // from C's closest point to O's
+    S l, radii = C.r;
+    if (so == nm::SHAPE_CUBOID) {
+        const nm::Box b{co, ro, ho};
+        if (qm::segment_meets_box(b, C)) return 0;
+        V3 on_seg, on_box;
+        l = nm::segment_box_closest(b, C, on_seg, on_box);
+        e = on_box - on_seg;
+    } else {
+        S s, t = 0;
+        const V3 uo = ro.c[1];
+        if (so == nm::SHAPE_CAPSULE) nm::segment_closest(C.c, C.u, C.h, co, uo, ho.y, s, t);
+        else qm::segment_point_d2(co - C.c, C.u, C.h, s);
+        e = (co + uo * t) - (C.c + C.u * s);
+        l = nm::len(e);
+        radii = radii + ho.x;
+    }
+    if (l > 0) n = (a_cap ? e : -e) * (1 / l);
+    return nm::smax(l - radii, 0);
+}
+
 // Distance between the closed shapes A and B (0 when they overlap or touch) and the unit direction n from A to B.  Out of line and rolled,
-// like nm::box_box_closest which it calls.
+// like nm::box_box_closest which it calls.  CAPS: pairs with a capsule go to capsule_distance (the CAPS = false instance has no such branch).
+template <bool CAPS = false>
 NM_COLD inline S shape_distance(int sa, V3 ha, V3 ca, const nm::M3& ra, int sb, V3 hb, V3 cb, const nm::M3& rb, V3& n) {
+    if (CAPS && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) return capsule_distance(sa, ha, ca, ra, sb, hb, cb, rb, n);
     n = V3{0, 1, 0};
     if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
         const V3 e = cb - ca;
@@ -161,9 +201,10 @@ NM_ROLLED
 
 // conservative advancement on [0, t_max]; see the header comment.  *iterations (optional): the distance evaluations it took; a hit reported
 // with CCD_MAX_ITERATIONS of them stopped at the cap, before reaching eps
+template <bool CAPS = false>
 NM_HD inline bool nonlinear_toi(const Motion& A, const Motion& B, S t_max, S eps, S& toi, int* iterations = nullptr) {
     const V3 rel = B.v - A.v;
-    const S spin = nm::len(A.w) * motion_radius(A) + nm::len(B.w) * motion_radius(B);
+    const S spin = nm::len(A.w) * motion_radius<CAPS>(A) + nm::len(B.w) * motion_radius<CAPS>(B);
     S t = 0;
 NM_ROLLED
     for (int it = 0; it < CCD_MAX_ITERATIONS; ++it) {
@@ -171,7 +212,7 @@ NM_ROLLED
         nm::M3 ra, rb;
         pose_at(A, t, ca, ra);
         pose_at(B, t, cb, rb);
-        const S d = shape_distance(A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n);
+        const S d = shape_distance<CAPS>(A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n);
         if (iterations) *iterations = it + 1;
         if (d != d) return false;
         if (d <= eps) { toi = t; return true; }
@@ -185,24 +226,25 @@ NM_ROLLED
 }
 
 // shape 1 moving with v1 - v2 against shape 2 at rest (qm::cast_toi)
+template <bool CAPS = false>
 NM_HD inline bool linear_toi(const Motion& A, const Motion& B, S t_max, S& toi) {
     int axis;
-    return qm::cast_toi(A.shape, A.he, A.p, A.q, A.v - B.v, t_max, B.shape, B.he, B.p, B.q, toi, axis);
+    return qm::cast_toi<CAPS>(A.shape, A.he, A.p, A.q, A.v - B.v, t_max, B.shape, B.he, B.p, B.q, toi, axis);
 }
 
 // compute_ccd_toi (ccd/mod.rs:692-780) against the bound dt: the TOI rounded to T, with the reference's fallback when it is exactly 0 (shape 2
 // replaced by a ball of radius prediction_distance at body 2's pose); T(-1) when the shapes never come within reach on [0, dt].  The caller
-// accepts the value when 0 < toi < min_toi.
-template <class T> NM_HD inline T pair_toi(int mode, const Motion& A, const Motion& B, T dt, S eps, S prediction_distance) {
+// accepts the value when 0 < toi < min_toi.  CAPS: capsules take part (the CAPS = false instance treats every shape as a cuboid or a sphere).
+template <class T, bool CAPS = false> NM_HD inline T pair_toi(int mode, const Motion& A, const Motion& B, T dt, S eps, S prediction_distance) {
     S t = 0;
-    const bool hit = mode == MODE_LINEAR ? linear_toi(A, B, S(dt), t) : nonlinear_toi(A, B, S(dt), eps, t);
+    const bool hit = mode == MODE_LINEAR ? linear_toi<CAPS>(A, B, S(dt), t) : nonlinear_toi<CAPS>(A, B, S(dt), eps, t);
     if (!hit) return T(-1);
     const T tt = static_cast<T>(t);
     if (tt != T(0)) return tt;
     Motion ball = B;
     ball.shape = nm::SHAPE_SPHERE;
     ball.he = V3{prediction_distance, 0, 0};
-    const bool hit2 = mode == MODE_LINEAR ? linear_toi(A, ball, S(dt), t) : nonlinear_toi(A, ball, S(dt), eps, t);
+    const bool hit2 = mode == MODE_LINEAR ? linear_toi<CAPS>(A, ball, S(dt), t) : nonlinear_toi<CAPS>(A, ball, S(dt), eps, t);
     return hit2 ? static_cast<T>(t) : T(-1);
 }
 

@@ -1066,6 +1066,7 @@ class Contacts final : public ContactsBase {
         out->c1 = c1_.as<uint32_t>(); out->c2 = c2_.as<uint32_t>(); out->b1 = b1_.as<uint32_t>(); out->b2 = b2_.as<uint32_t>(); out->live = live_.as<uint8_t>();
         out->shape = in_.shape;
         out->dims = in_.dims;
+        out->has_capsule = has_capsule_;
     }
     AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) override {
         if (!in || !in->dims) return AVN_OK;   // step() reports the missing columns

@@ -215,7 +215,8 @@ struct ContactsBase {
     // ---- the rows and collider shapes swept CCD visits (ccd.cu)
     virtual void ccd_rows(CcdRows* out) = 0;
     // ---- the shape column of a step: checked on the host when step() is going to copy it (not under AVN_CONTACTS_SHAPES_UNCHANGED), before
-    //      any state changes; has_capsule: the column of the last accepted step holds a capsule (swept CCD refuses capsules)
+    //      any state changes; has_capsule: the column of the last accepted step holds a capsule (swept CCD refuses it unless configured with
+    //      AVN_CCD_CAPSULES, and launches its capsule TOI kernel only when it holds one)
     virtual AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) = 0;
     virtual bool has_capsule() const = 0;
     // ---- body frames (avn_contacts_set_body_frames): checked and copied on the host (NULL clears them); body_frames() = NULL when none are set
@@ -232,6 +233,7 @@ struct CcdRows {
     const uint8_t* live = nullptr;
     const uint8_t* shape = nullptr;    // [C] of the last avn_contacts_step (NULL = cuboid)
     const void* dims = nullptr;        // [C][3]
+    bool has_capsule = false;          // the shape column holds a capsule
 };
 struct CcdSolverState {
     int B = 0;
@@ -245,6 +247,7 @@ struct CcdBase {
     virtual ~CcdBase() {}
     virtual AvnStatus configure(const AvnCcdConfig* cfg, const CcdRows& rows) = 0;
     virtual bool active() const = 0;
+    virtual bool capsules() const = 0;   // configured with AVN_CCD_CAPSULES
     // enqueued on the context's stream; adds its kernel launches to *launches
     virtual AvnStatus run(const CcdSolverState& st, const CcdRows& rows, uint32_t* launches) = 0;
     virtual AvnStatus download(AvnCcdResult* out) = 0;

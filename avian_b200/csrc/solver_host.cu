@@ -322,7 +322,7 @@ AvnStatus Solver<S>::upload(const AvnStepParams* prm, AvnBodyColumns* bc, AvnMan
 template <class S>
 AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* bc, ContactsBase* contacts, AvnJointSet* js) {
     if (!contacts) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "upload_resident: no contact store");
-    if (ccd_active() && contacts->has_capsule())
+    if (ccd_active() && contacts->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "upload_resident: swept CCD is configured (avn_ccd_configure) and the contact store's shape column holds a "
                                                "capsule; capsule times of impact are not implemented");
     ContactsBase::AsleepBodies asleep;
@@ -610,7 +610,7 @@ AvnStatus Solver<S>::run() {
     if (!ccd_active()) return launch_range(0, dev_.substeps, AVN_RUN_PREPARE | AVN_RUN_RESTITUTION | AVN_RUN_FINALIZE);
     // swept CCD (ccd.cu) runs after the substeps and before restitution (ccd/mod.rs:257-261): the step is split around it
     if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run before avn_solver_upload");
-    if (ccd_contacts_ && ccd_contacts_->has_capsule())
+    if (ccd_contacts_ && ccd_contacts_->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run: swept CCD is configured and the contact store's shape column holds a capsule; capsule "
                                                "times of impact are not implemented");
     if (!from_store_ || !ccd_contacts_)

@@ -486,7 +486,8 @@ def ccd_apply_record(scalar, m: float, v, w, dp, dq):
 def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, rows: dict, cfg: dict, delta_position=None, delta_rotation=None) -> dict:
     """solve_swept_ccd over the contact rows (dict c1, c2, b1, b2, live) by the reference's sequential loop.  bodies: dict kind, position,
     rotation, linear_velocity, angular_velocity (SolverBody velocities after the substeps), center_of_mass (optional).  cfg: the keyword
-    arguments of api.ccd_config.  delta_position / delta_rotation are updated in place when given.  Returns what Context.ccd_download returns."""
+    arguments of api.ccd_config, plus capsules=True for api.CCD_CAPSULES (as Context.ccd_configure takes it).  delta_position /
+    delta_rotation are updated in place when given.  Returns what Context.ccd_download returns."""
     lib, dt_ = _load(), np.dtype(scalar)
     col = lambda a, t=dt_: None if a is None else np.ascontiguousarray(a, dtype=t)
     kind = col(bodies.get("kind"), np.uint8)
@@ -495,6 +496,8 @@ def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, 
     sh, dm = col(shape, np.uint8), col(dims)
     c1, c2, b1, b2 = (col(rows[k], np.uint32) for k in ("c1", "c2", "b1", "b2"))
     live = col(rows["live"], np.uint8)
+    cfg = dict(cfg)
+    cfg["flags"] = cfg.get("flags", 0) | (api.CCD_CAPSULES if cfg.pop("capsules", False) else 0)
     conf, keep = api.ccd_config(**cfg)
     n = int(conf.count)
     out = {"min_toi": np.zeros(n, dtype=dt_), "hit_body": np.zeros(n, dtype=np.int32), "hit_contact": np.zeros(n, dtype=np.int32),
@@ -505,7 +508,7 @@ def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, 
                            _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
                            *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
     if st == api.ERR_UNSUPPORTED:
-        raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule (capsule times of impact are not implemented)")
+        raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule and the configuration does not set CCD_CAPSULES")
     if st != 0:
         raise ValueError("avh_ccd_solve: invalid configuration")
     return out

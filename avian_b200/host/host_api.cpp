@@ -1284,7 +1284,7 @@ int ccd_solve(double dt_d, double length_unit, uint32_t B, const uint8_t* kind, 
                 const int mode = (mode_of(k) == ccd::MODE_LINEAR && (it == slot_of_body.end() || mode_of(it->second) == ccd::MODE_LINEAR)) ? ccd::MODE_LINEAR
                                                                                                                                       : ccd::MODE_NON_LINEAR;
                 ++cand;
-                const T t = ccd::pair_toi<T>(mode, ccd_motion(dims, shape, own, pos, rot, com, v1, w1, body1),
+                const T t = ccd::pair_toi<T, true>(mode, ccd_motion(dims, shape, own, pos, rot, com, v1, w1, body1),
                                              ccd_motion(dims, shape, other, pos, rot, com, v2, w2, body2), dt, eps, cfg->prediction_distance);
                 if (t > T(0) && t < dt) ++hits;
                 if (t > T(0) && t < min_toi) { min_toi = t; hit = int32_t(body2); hit_row = int32_t(e); }
@@ -1324,14 +1324,17 @@ ccd::Motion motion_from(const double* m) {   // shape, he[3], p[3], q[4], local 
 extern "C" {
 
 // solve_swept_ccd over the given contact rows.  Velocities: the SolverBody velocities after the substeps; delta_position / delta_rotation
-// ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration.
+// ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration (an
+// unknown cfg->flags bit included) and AVN_ERR_UNSUPPORTED for a live row that names a capsule without AVN_CCD_CAPSULES.  The geometry is
+// the CAPS = true instance either way: with no capsule in a pair it is the device's CAPS = false TOI, bit for bit.
 int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position, const void* rotation,
                   const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation, const uint8_t* shape, const void* dims,
                   uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2, const uint8_t* live, const AvnCcdConfig* cfg,
                   void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates, uint32_t* hits) {
     if (!cfg || (cfg->count && (!cfg->body || !cfg->collider))) return -1;
-    // capsule times of impact are not implemented: a configuration with a row that names a capsule is refused, as the device refuses it
-    if (cfg->count && shape)
+    if (cfg->count && (cfg->flags & ~AVN_CCD_CAPSULES)) return AVN_ERR_INVALID_ARGUMENT;
+    // without AVN_CCD_CAPSULES a configuration with a row that names a capsule is refused, as the device refuses it
+    if (cfg->count && shape && !(cfg->flags & AVN_CCD_CAPSULES))
         for (uint32_t r = 0; r < rows; ++r)
             if ((!live || live[r]) && (shape[c1[r]] == SHAPE_CAPSULE || shape[c2[r]] == SHAPE_CAPSULE)) return AVN_ERR_UNSUPPORTED;
     if (scalar_bits == 64)
@@ -1346,16 +1349,17 @@ int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t 
 }
 
 // One pair's compute_ccd_toi against the bound dt (ccd::pair_toi, fallback included), rounded to the column scalar and returned as a double;
-// -1 = no hit.  Motions: 20 doubles each (shape, half extents / radius, position, rotation, local com, linear and angular velocity).
+// -1 = no hit.  Motions: 20 doubles each (shape, half extents / radius / capsule radius and half length, position, rotation, local com,
+// linear and angular velocity).  Capsules (shape 2) are accepted.
 double avh_ccd_pair_toi(uint32_t scalar_bits, int mode, const double* a, const double* b, double dt, double eps, double prediction_distance) {
-    if (scalar_bits == 64) return ccd::pair_toi<double>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance);
-    return double(ccd::pair_toi<float>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance));
+    if (scalar_bits == 64) return ccd::pair_toi<double, true>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance);
+    return double(ccd::pair_toi<float, true>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance));
 }
 
 // The raw non-linear TOI in double (no rounding, no fallback): 1 and *toi on a hit, 0 otherwise; *iterations = distance evaluations.
 int avh_ccd_nonlinear_toi(const double* a, const double* b, double t_max, double eps, double* toi, int* iterations) {
     double t = 0;
-    const bool hit = ccd::nonlinear_toi(motion_from(a), motion_from(b), t_max, eps, t, iterations);
+    const bool hit = ccd::nonlinear_toi<true>(motion_from(a), motion_from(b), t_max, eps, t, iterations);
     *toi = t;
     return hit ? 1 : 0;
 }

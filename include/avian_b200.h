@@ -372,7 +372,7 @@ AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
 /* ---- collider AABBs (SURVEY.md 8f "next #2"): update_aabb for the shapes the device knows ------------------------------- */
 /* AVN_SHAPE_CAPSULE: Collider::capsule(radius, length), dims = [radius, length / 2, unused]; the segment runs from (0, -length/2, 0) to
  * (0, +length/2, 0) in the collider frame.  The AABB update, the narrow phase, the contact store, the spatial queries (colliders and query
- * shapes) and move and slide (obstacles and characters) take capsules; swept CCD refuses them. */
+ * shapes), move and slide (obstacles and characters) and swept CCD (with AVN_CCD_CAPSULES) take capsules. */
 typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2 } AvnShape;
 
 typedef struct AvnAabbParams {
@@ -910,17 +910,19 @@ AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const
  *      order of the configured list, so a body hit by several CCD bodies ends with the last one's delta_position.
  *      Assumptions, as the narrow phase makes them: a collider sits at its body's origin and its pose is the body's pose before the step; the
  *      body columns and the collider rows of the contact pipeline (avn_contacts_configure / avn_contacts_step) describe the same bodies.
- *      Geometry: cuboid and sphere colliders, conventions in avian_b200/csrc/ccd_math.hpp (linear: the shape casts of the spatial queries;
- *      non-linear: conservative advancement to eps = 1e-4 * length_unit, at most 64 iterations).
+ *      Geometry: cuboid and sphere colliders, and capsules with AVN_CCD_CAPSULES; conventions in avian_b200/csrc/ccd_math.hpp (linear: the
+ *      shape casts of the spatial queries; non-linear: conservative advancement to eps = 1e-4 * length_unit, at most 64 iterations).
  *      Stated deviation: equal TOIs go to the lowest ContactId, where the reference keeps the first in ContactGraph adjacency order.
  *      Runs inside avn_solver_run when the upload came from the contact store (avn_solver_upload_resident): the step becomes
  *      prepare + substeps -> CCD pass -> restitution + finalize.  While CCD is configured, avn_solver_run_range,
  *      avn_solver_step_partitioned and a run after avn_solver_upload / avn_solver_step return AVN_ERR_UNSUPPORTED. */
 typedef enum AvnSweepMode { AVN_SWEEP_LINEAR = 0, AVN_SWEEP_NON_LINEAR = 1 } AvnSweepMode;
 
+#define AVN_CCD_CAPSULES 0x1u           /* AvnCcdConfig.flags: capsule colliders take part (see avn_ccd_configure) */
+
 typedef struct AvnCcdConfig {
     uint32_t count;                    /* SweptCcd bodies, in query order */
-    uint32_t _pad;
+    uint32_t flags;                    /* AVN_CCD_* bits; 0 = cuboid and sphere colliders only */
     const int32_t* body;               /* [n] index into AvnBodyColumns; no body twice */
     const uint32_t* collider;          /* [n] the body's own collider: a row of the contact pipeline's collider columns */
     const uint8_t* mode;               /* [n] AvnSweepMode; NULL = AVN_SWEEP_NON_LINEAR (SweptCcd::default) */
@@ -941,7 +943,10 @@ typedef struct AvnCcdResult {          /* per configured body, the last step's p
 } AvnCcdResult;
 
 /* Persists across steps; NULL or count == 0 clears it.  Needs avn_contacts_configure first (bodies and colliders are checked against its counts).
- * Refused with AVN_ERR_INVALID_ARGUMENT: bodies or colliders out of range, a body listed twice, NaN thresholds, an unknown mode. */
+ * Refused with AVN_ERR_INVALID_ARGUMENT: a flag bit other than AVN_CCD_CAPSULES, bodies or colliders out of range, a body listed twice, NaN
+ * thresholds, an unknown mode.  Capsules: without AVN_CCD_CAPSULES, a contact store whose shape column holds a capsule is refused with
+ * AVN_ERR_UNSUPPORTED here, and so are avn_solver_upload_resident and avn_solver_run once a later avn_contacts_step brings one in.  With it,
+ * capsules are swept like the other shapes (exact capsule casts in Linear mode, exact capsule distances in NonLinear mode). */
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config);
 /* The results of the last step that ran the pass (AVN_ERR_INVALID_ARGUMENT before any). */
 AvnStatus avn_ccd_download(AvnContext* ctx, AvnCcdResult* out);
