@@ -356,6 +356,10 @@ class AvnBodyFrames(C.Structure):
     _fields_ = [("body_count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("position", "rotation", "center_of_mass")]
 
 
+class AvnConvexHulls(C.Structure):
+    _fields_ = [("hull_count", C.c_uint32), ("_pad", C.c_uint32)] + [(n, _vp) for n in ("vertex_offsets", "vertices", "face_offsets", "loop_offsets", "loop")]
+
+
 class AvnRawManifolds(C.Structure):
     _fields_ = [(n, _vp) for n in ("point_count", "disjoint", "normal", "anchor1", "anchor2", "penetration", "normal_speed")]
 
@@ -502,6 +506,7 @@ def bind_abi(lib: C.CDLL, prefix: str = "avn") -> None:
         "contacts_configure": ([_vp, P(AvnContactGraphConfig)], C.c_int),
         "contacts_step": ([_vp, P(AvnNarrowParams), P(AvnNarrowInput), C.c_uint32, C.c_double, C.c_uint32, P(AvnContactStep)], C.c_int),
         "contacts_set_body_frames": ([_vp, P(AvnBodyFrames)], C.c_int),
+        "set_convex_hulls": ([_vp, P(AvnConvexHulls)], C.c_int),
         "solver_upload_resident": ([_vp, P(AvnStepParams), P(AvnBodyColumns), P(AvnJointSet)], C.c_int),
         "broadphase_download_order": ([_vp, P(C.c_uint64)], C.c_int),
         "contacts_download_graph": ([_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -545,11 +550,59 @@ ABI_SYMBOLS = [
     "avn_query_aabb_intersections", "avn_query_cast_shape", "avn_query_shape_hits", "avn_query_project_point", "avn_query_point_intersections",
     "avn_query_shape_intersections", "avn_ccd_configure", "avn_ccd_download", "avn_contacts_set_sensors", "avn_contacts_remove_colliders",
     "avn_contacts_events", "avn_contacts_report", "avn_islands_apply", "avn_islands_wake", "avn_contacts_download_sleeping",
-    "avn_move_and_slide", "avn_contacts_set_body_frames"]
+    "avn_move_and_slide", "avn_contacts_set_body_frames", "avn_set_convex_hulls"]
 
 RUN_PREPARE, RUN_RESTITUTION, RUN_FINALIZE = 1, 2, 4
 COMM_ID_BYTES = 128
 BOUNDARY_RECORD_SCALARS = 16
+
+
+SHAPE_CONVEX_HULL = 3
+HULL_MAX_VERTICES, HULL_MAX_FACES, HULL_MAX_FACE_VERTICES = 64, 128, 32
+
+
+@dataclass
+class ConvexHulls:
+    """A convex hull table (AvnConvexHulls): what parry's ConvexPolyhedron holds for each hull, in CSR columns.  vertices [V,3] hull-local and
+    already scaled; each face a loop of hull-local vertex indices, counter-clockwise seen from outside.  A collider with shape
+    SHAPE_CONVEX_HULL names its hull by index in dims[0]."""
+    vertex_offsets: np.ndarray   # uint32 [H+1]
+    vertices: np.ndarray         # float64 [V,3]
+    face_offsets: np.ndarray     # uint32 [H+1]
+    loop_offsets: np.ndarray     # uint32 [F+1]
+    loop: np.ndarray             # uint32 [L]
+
+    @property
+    def count(self) -> int:
+        return int(self.vertex_offsets.shape[0]) - 1
+
+    @staticmethod
+    def from_polyhedra(hulls) -> "ConvexHulls":
+        """hulls: a list of (vertices [v,3], faces: list of vertex-index loops)."""
+        vo, fo, lo, verts, loop = [0], [0], [0], [], []
+        for v, faces in hulls:
+            v = np.asarray(v, dtype=np.float64).reshape(-1, 3)
+            verts.append(v)
+            vo.append(vo[-1] + v.shape[0])
+            for f in faces:
+                loop.extend(int(i) for i in f)
+                lo.append(len(loop))
+            fo.append(fo[-1] + len(faces))
+        u32 = lambda a: np.ascontiguousarray(a, dtype=np.uint32)
+        return ConvexHulls(u32(vo), np.ascontiguousarray(np.concatenate(verts) if verts else np.zeros((0, 3))), u32(fo), u32(lo), u32(loop))
+
+    def polyhedron(self, h: int):
+        """(vertices, faces) of hull h"""
+        v = self.vertices[self.vertex_offsets[h]:self.vertex_offsets[h + 1]]
+        faces = [self.loop[self.loop_offsets[f]:self.loop_offsets[f + 1]] for f in range(self.face_offsets[h], self.face_offsets[h + 1])]
+        return v, faces
+
+    def as_struct(self, scalar) -> tuple["AvnConvexHulls", tuple]:
+        """the ABI struct with the vertices in the column scalar, and the arrays it points into (keep them alive while it is used)"""
+        keep = (np.ascontiguousarray(self.vertex_offsets, dtype=np.uint32), np.ascontiguousarray(self.vertices, dtype=scalar),
+                np.ascontiguousarray(self.face_offsets, dtype=np.uint32), np.ascontiguousarray(self.loop_offsets, dtype=np.uint32),
+                np.ascontiguousarray(self.loop, dtype=np.uint32))
+        return AvnConvexHulls(self.count, 0, *(_ptr(a) for a in keep)), keep
 
 
 @dataclass
@@ -1093,6 +1146,15 @@ class Context:
         f = AvnBodyFrames(n, 0, _ptr(pos), _ptr(rot), _ptr(com))
         self._keep_frames = (pos, rot, com, f)
         self._check(self.lib.avn_contacts_set_body_frames(self.handle, C.byref(f)))
+
+    def set_convex_hulls(self, hulls: "ConvexHulls | None") -> None:
+        """avn_set_convex_hulls: the hull table every later update_aabbs / narrow_phase / contacts_step reads (None clears it).  Raises
+        AvianError (AVN_ERR_INVALID_ARGUMENT) for a table the library refuses; a refused call changes nothing."""
+        if hulls is None:
+            self._check(self.lib.avn_set_convex_hulls(self.handle, None))
+            return
+        st, keep = hulls.as_struct(self.scalar)
+        self._check(self.lib.avn_set_convex_hulls(self.handle, C.byref(st)))
 
     def solver_step_resident(self, params, bodies: Bodies, joints: JointSet | None = None) -> None:
         """avn_solver_upload_resident + run + download: manifolds AND constraint graph come from the contact store on the device."""

@@ -1,4 +1,4 @@
-// update_aabb on the device for cuboid, sphere and capsule colliders.  Replaces update_aabb::<Collider>
+// update_aabb on the device for cuboid, sphere, capsule and convex hull colliders.  Replaces update_aabb::<Collider>
 // (src/collision/collider/backend.rs:498-625); the shape AABBs follow parry3d's Cuboid::aabb / Ball::aabb / Capsule::aabb
 // (center +- |R| half_extents with nalgebra's UnitQuaternion::to_rotation_matrix; center +- radius; capsule_aabb below).
 // One thread per collider: 52-68 B in, 24 B out — a pure streaming kernel (HBM-bound, ~90 B per collider).
@@ -54,12 +54,30 @@ __device__ __forceinline__ void shape_aabb(int shape, V3<S> d, V3<S> p, Q4<S> q,
     mx = p + he;
 }
 
-// One thread per collider.  CAPSULES = false (update_aabbs_kernel): cuboids and spheres, skipping the capsules when `capsules` is set;
-// CAPSULES = true (update_capsule_aabbs_kernel, launched only for a shape column that holds a capsule): the capsules alone.
+// parry3d's ConvexPolyhedron::aabb: every vertex moved by the pose (nalgebra's UnitQuaternion * Vector3, as capsule_aabb), componentwise
+// min / max.  PARITY UNPINNED: parry is not vendored.  The table's vertices are the column's values widened to double, so S(v) is exact.
+template <class S>
+__device__ __noinline__ void hull_aabb(const hm::Table t, uint32_t h, V3<S> p, Q4<S> q, V3<S>& mn, V3<S>& mx) {
+    const V3<S> b = mk3<S>(q.x, q.y, q.z);
+#pragma unroll 1
+    for (uint32_t k = t.voff[h]; k < t.voff[h + 1]; ++k) {
+        const V3<S> v = mk3<S>(S(t.vert[3 * k]), S(t.vert[3 * k + 1]), S(t.vert[3 * k + 2]));
+        const V3<S> tv = cross(b, v) * S(2);
+        const V3<S> e = ((v + cross(b, tv)) + tv * q.w) + p;
+        if (k == t.voff[h]) { mn = e; mx = e; continue; }
+        mn = mk3<S>(avn_min(mn.x, e.x), avn_min(mn.y, e.y), avn_min(mn.z, e.z));
+        mx = mk3<S>(avn_max(mx.x, e.x), avn_max(mx.y, e.y), avn_max(mx.z, e.z));
+    }
+}
+
+// One thread per collider.  CAPSULES = false (update_aabbs_kernel): cuboids and spheres, skipping the capsules when `capsules` is set and the
+// hulls when `hulls` is set; CAPSULES = true (update_capsule_aabbs_kernel, launched only for a shape column that holds a capsule): the capsules
+// alone.  The hulls run in update_hull_aabbs_kernel.
 template <class S, bool CAPSULES>
-__device__ __forceinline__ void update_aabb(const AabbArgs<S>& a, int capsules) {
+__device__ __forceinline__ void update_aabb(const AabbArgs<S>& a, int capsules, int hulls = 0) {
     int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= a.n) return;
+    if (hulls && a.shape[n] == AVN_SHAPE_CONVEX_HULL) return;
     if (capsules && (a.shape[n] == AVN_SHAPE_CAPSULE) != CAPSULES) return;
     V3<S> d = mk3<S>(a.dims[3 * n], a.dims[3 * n + 1], a.dims[3 * n + 2]), p = mk3<S>(a.pos[3 * n], a.pos[3 * n + 1], a.pos[3 * n + 2]);
     Q4<S> q; q.x = a.rot[4 * n]; q.y = a.rot[4 * n + 1]; q.z = a.rot[4 * n + 2]; q.w = a.rot[4 * n + 3];
@@ -86,9 +104,38 @@ __device__ __forceinline__ void update_aabb(const AabbArgs<S>& a, int capsules) 
 }
 
 template <class S>
-__global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a, int capsules) { update_aabb<S, false>(a, capsules); }
+__global__ void update_aabbs_kernel(const __grid_constant__ AabbArgs<S> a, int capsules, int hulls) { update_aabb<S, false>(a, capsules, hulls); }
 template <class S>
 __global__ void update_capsule_aabbs_kernel(const __grid_constant__ AabbArgs<S> a) { update_aabb<S, true>(a, 1); }
+
+// The hull colliders alone (launched only for a shape column that holds a hull): update_aabb's sweep and margins around hull_aabb.
+template <class S>
+__global__ void update_hull_aabbs_kernel(const __grid_constant__ AabbArgs<S> a, const hm::Table t) {
+    int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= a.n || a.shape[n] != AVN_SHAPE_CONVEX_HULL) return;
+    const uint32_t h = uint32_t(a.dims[3 * n]);
+    V3<S> p = mk3<S>(a.pos[3 * n], a.pos[3 * n + 1], a.pos[3 * n + 2]);
+    Q4<S> q; q.x = a.rot[4 * n]; q.y = a.rot[4 * n + 1]; q.z = a.rot[4 * n + 2]; q.w = a.rot[4 * n + 3];
+    S margin = a.cm ? a.cm[n] : S(0);
+    S spec = a.sm ? (isinf(a.sm[n]) ? a.scalar_max : a.sm[n]) : a.def_spec;
+    V3<S> mn, mx;
+    if (spec <= S(0)) {
+        hull_aabb<S>(t, h, p, q, mn, mx);
+    } else {
+        V3<S> v = a.lv ? mk3<S>(a.lv[3 * n], a.lv[3 * n + 1], a.lv[3 * n + 2]) : zero3<S>();
+        V3<S> w = a.av ? mk3<S>(a.av[3 * n], a.av[3 * n + 1], a.av[3 * n + 2]) : zero3<S>();
+        Q4<S> end_rot = q_fast_renormalize(qmul(q_from_scaled_axis(w * a.dt, false), q));
+        V3<S> end_pos = p + clamp_len_max(v * a.dt, avn_max(spec, a.tol));
+        V3<S> mn0, mx0, mn1, mx1;
+        hull_aabb<S>(t, h, p, q, mn0, mx0);
+        hull_aabb<S>(t, h, end_pos, end_rot, mn1, mx1);
+        mn = mk3<S>(avn_min(mn0.x, mn1.x), avn_min(mn0.y, mn1.y), avn_min(mn0.z, mn1.z));
+        mx = mk3<S>(avn_max(mx0.x, mx1.x), avn_max(mx0.y, mx1.y), avn_max(mx0.z, mx1.z));
+    }
+    S g = a.tol + margin;
+    a.omn[3 * n] = mn.x - g; a.omn[3 * n + 1] = mn.y - g; a.omn[3 * n + 2] = mn.z - g;
+    a.omx[3 * n] = mx.x + g; a.omx[3 * n + 1] = mx.y + g; a.omx[3 * n + 2] = mx.z + g;
+}
 
 template <class S>
 class AabbUpdater final : public AabbBase {
@@ -101,8 +148,9 @@ class AabbUpdater final : public AabbBase {
         if (!c->dims || !c->position || !c->rotation || !c->aabb_min || !c->aabb_max)
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "colliders: dims, position, rotation, aabb_min and aabb_max are required");
         size_t at = 0;
-        bool capsules = false;
-        if (const char* why = check_shape_column(c->shape, c->dims, n, sizeof(S) == 8 ? 64 : 32, &at, &capsules))
+        bool capsules = false, hulls = false;
+        const uint32_t hull_count = hulls_->count();
+        if (const char* why = check_shape_column(c->shape, c->dims, n, sizeof(S) == 8 ? 64 : 32, &at, &capsules, &hull_count, &hulls))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "colliders: collider %zu: %s", at, why);
         AabbArgs<S> a{};
         a.n = int(n);
@@ -123,14 +171,16 @@ class AabbUpdater final : public AabbBase {
         a.dt = S(prm->dt); a.tol = S(prm->contact_tolerance);
         a.scalar_max = std::numeric_limits<S>::max();
         a.def_spec = std::isinf(prm->default_speculative_margin) ? std::numeric_limits<S>::max() : S(prm->default_speculative_margin);
-        update_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a, capsules ? 1 : 0);
+        update_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a, capsules ? 1 : 0, hulls ? 1 : 0);
         if (capsules) update_capsule_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a);
+        if (hulls) update_hull_aabbs_kernel<S><<<unsigned((n + 255) / 256), 256, 0, stream_>>>(a, hulls_->dev);
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(c->aabb_min, a.omn, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(c->aabb_max, a.omx, 3 * n * sizeof(S), cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaStreamSynchronize(stream_));
         return AVN_OK;
     }
+    void attach_hulls(const HullTable* hulls) override { hulls_ = hulls; }
 
    private:
     template <class T> AvnStatus up(DevBuf& buf, const void* host, size_t count, const T** dev) {
@@ -143,6 +193,7 @@ class AabbUpdater final : public AabbBase {
     }
     cudaStream_t stream_;
     ErrorSink* err_;
+    const HullTable* hulls_ = nullptr;
     DevBuf b_shape_, b_dims_, b_pos_, b_rot_, b_lv_, b_av_, b_cm_, b_sm_, o_mn_, o_mx_;
 };
 

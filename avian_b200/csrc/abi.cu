@@ -5,6 +5,7 @@
 #include <new>
 
 #include "context.hpp"
+#include "hull_math.hpp"
 #include "joint_schedule.hpp"
 
 struct AvnContext {
@@ -20,6 +21,7 @@ struct AvnContext {
     std::unique_ptr<avn::QueriesBase> queries;
     std::unique_ptr<avn::CommBase> comm;
     std::unique_ptr<avn::CcdBase> ccd;
+    avn::HullTable hulls;              // avn_set_convex_hulls; read by aabbs, narrow and contacts
     AvnTimings last{};
 };
 
@@ -94,6 +96,9 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
             return create_fail(AVN_ERR_UNSUPPORTED, "scalar type not available");
         }
         ctx->solver->attach_ccd(ctx->ccd.get(), ctx->contacts.get());
+        ctx->aabbs->attach_hulls(&ctx->hulls);
+        ctx->narrow->attach_hulls(&ctx->hulls);
+        ctx->contacts->attach_hulls(&ctx->hulls);
         *out_ctx = ctx.release();
         return AVN_OK;
     } catch (...) {
@@ -228,6 +233,55 @@ AvnStatus avn_update_aabbs(AvnContext* ctx, const AvnAabbParams* params, AvnColl
 
 AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const AvnNarrowInput* input, AvnRawManifolds* out) {
     return guarded(ctx, [&] { return ctx->narrow->run(params, input, out, ctx->contacts->body_frames()); });
+}
+
+AvnStatus avn_set_convex_hulls(AvnContext* ctx, const AvnConvexHulls* hulls) {
+    return guarded(ctx, [&]() -> AvnStatus {
+        avn::HullTable& t = ctx->hulls;
+        if (!hulls) { t.set = false; return AVN_OK; }
+        const uint32_t H = hulls->hull_count;
+        if (H > AVN_HULL_MAX_COUNT) return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "set_convex_hulls: %u hulls, at most AVN_HULL_MAX_COUNT", H);
+        if (!hulls->vertex_offsets || !hulls->vertices || !hulls->face_offsets || !hulls->loop_offsets || !hulls->loop)
+            return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "set_convex_hulls: vertex_offsets, vertices, face_offsets, loop_offsets and loop are required");
+        const size_t V = hulls->vertex_offsets[H];
+        std::vector<double> vert(3 * V);
+        for (size_t i = 0; i < 3 * V; ++i)
+            vert[i] = ctx->scalar_bits == 64 ? static_cast<const double*>(hulls->vertices)[i] : double(static_cast<const float*>(hulls->vertices)[i]);
+        hm::HullSet set;
+        uint32_t at = 0;
+        if (const char* why = hm::derive_hulls(H, hulls->vertex_offsets, vert.data(), hulls->face_offsets, hulls->loop_offsets, hulls->loop, &set, &at))
+            return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "set_convex_hulls: hull %u: %s", at, why);
+        // the previous table may still be read by work on the stream: let it finish before its buffers are replaced.  Every reader of the
+        // table runs on the context's stream, so the copies go there too (a synchronous cudaMemcpy runs on the legacy default stream, which
+        // a non-blocking stream does not wait for), and the call waits for them before the table is marked set and the host copy is freed
+        cudaError_t e = cudaStreamSynchronize(ctx->stream);
+        auto put = [&](avn::DevBuf& buf, const void* src, size_t bytes) -> const void* {
+            if (e != cudaSuccess) return nullptr;
+            if ((e = buf.ensure(bytes ? bytes : 1)) != cudaSuccess) return nullptr;
+            if (bytes) e = cudaMemcpyAsync(buf.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+            return buf.p;
+        };
+        t.set = false;   // a failed upload leaves no table
+        hm::Table d{};
+        d.count = H;
+        d.vert = static_cast<const double*>(put(t.vert, set.vert.data(), set.vert.size() * sizeof(double)));
+        d.plane = static_cast<const double*>(put(t.plane, set.plane.data(), set.plane.size() * sizeof(double)));
+        d.centre = static_cast<const double*>(put(t.centre, set.centre.data(), set.centre.size() * sizeof(double)));
+        d.radius = static_cast<const double*>(put(t.radius, set.radius.data(), set.radius.size() * sizeof(double)));
+        d.voff = static_cast<const uint32_t*>(put(t.voff, set.voff.data(), set.voff.size() * sizeof(uint32_t)));
+        d.foff = static_cast<const uint32_t*>(put(t.foff, set.foff.data(), set.foff.size() * sizeof(uint32_t)));
+        d.loff = static_cast<const uint32_t*>(put(t.loff, set.loff.data(), set.loff.size() * sizeof(uint32_t)));
+        d.loop = static_cast<const uint32_t*>(put(t.loop, set.loop.data(), set.loop.size() * sizeof(uint32_t)));
+        d.eoff = static_cast<const uint32_t*>(put(t.eoff, set.eoff.data(), set.eoff.size() * sizeof(uint32_t)));
+        d.edge = static_cast<const uint32_t*>(put(t.edge, set.edge.data(), set.edge.size() * sizeof(uint32_t)));
+        const cudaError_t done = cudaStreamSynchronize(ctx->stream);   // also when a copy failed: `set` is freed on return
+        if (e == cudaSuccess) e = done;
+        if (e != cudaSuccess)
+            return ctx->err.fail(e == cudaErrorMemoryAllocation ? AVN_ERR_OUT_OF_MEMORY : AVN_ERR_CUDA, "set_convex_hulls: upload failed: %s", cudaGetErrorString(e));
+        t.dev = d;
+        t.set = true;
+        return AVN_OK;
+    });
 }
 
 AvnStatus avn_contacts_configure(AvnContext* ctx, const AvnContactGraphConfig* config) { return guarded(ctx, [&] { return ctx->contacts->configure(config); }); }
@@ -368,6 +422,8 @@ AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
         if (config && config->count && !(config->flags & AVN_CCD_CAPSULES) && ctx->contacts->has_capsule())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a capsule; capsule times of impact are not implemented");
+        if (config && config->count && ctx->contacts->has_hull())
+            return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a convex hull; hull times of impact are not implemented");
         if (config && config->count && ctx->contacts->body_frames())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: body frames are set (avn_contacts_set_body_frames); swept CCD assumes a collider at its body's origin");
         avn::CcdRows rows;

@@ -4,6 +4,7 @@
 #pragma once
 #include <cstdint>
 
+#include "hull_math.hpp"
 #include "narrow_math.hpp"
 
 namespace avn {
@@ -57,11 +58,18 @@ NM_HD inline bool capsule_row(const NarrowEdgeArgs<S>& a, int e) {
     return a.shape && a.r.live[e] && (a.shape[a.r.c1[e]] == nm::SHAPE_CAPSULE || a.shape[a.r.c2[e]] == nm::SHAPE_CAPSULE);
 }
 
+// A live row that names a convex hull: the device runs it in a kernel of its own (narrow_hull_edges_kernel), see hm::collide.
+template <class S>
+NM_HD inline bool hull_row(const NarrowEdgeArgs<S>& a, int e) {
+    return a.shape && a.r.live[e] && (a.shape[a.r.c1[e]] == hm::SHAPE_CONVEX_HULL || a.shape[a.r.c2[e]] == hm::SHAPE_CONVEX_HULL);
+}
+
 // geometry + match_contacts for every live row (same arithmetic as avh_raw_manifolds + avh_match_raw of the host fixture).  CAPSULES = false:
 // the row holds no capsule (the cuboid / sphere kernel).  FRAMES: the anchors are moved to the bodies' centres of mass by the frames `f`
-// (nm::manifold_points); without it `f` is not read and the row compiles to what it was before body frames existed.
-template <class S, bool CAPSULES = true, bool FRAMES = false>
-NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e, const BodyFrameCols<S>& f = BodyFrameCols<S>{}) {
+// (nm::manifold_points); without it `f` is not read and the row compiles to what it was before body frames existed.  HULLS: the row names a
+// convex hull and runs hm::collide over the hull table `t` (CAPSULES is then not read).
+template <class S, bool CAPSULES = true, bool FRAMES = false, bool HULLS = false>
+NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e, const BodyFrameCols<S>& f = BodyFrameCols<S>{}, const hm::Table* t = nullptr) {
     const EdgeRows<S>& r = a.r;
     if (r.asleep && r.asleep[e]) return;   // update_contacts runs over active_pairs only (narrow_phase/system_param.rs:437)
     if (!r.live[e]) { r.count[e] = 0; r.disjoint[e] = 0; return; }
@@ -85,7 +93,8 @@ NM_HD inline void narrow_edge_row(const NarrowEdgeArgs<S>& a, int e, const BodyF
         const double max_dist = nm::smax(eff_margin, a.tol);
         nm::Contacts pts;
         const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
-        if (nm::collide<CAPSULES>(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts)) {
+        if (HULLS ? hm::collide(*t, ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts)
+                  : nm::collide<CAPSULES>(ta, ldd3(a.dims, ca), pa, qa, tb, ldd3(a.dims, cb), pb, qb, max_dist, normal, pts)) {
             if (FRAMES) np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, pair_frames(f, ba, pa, bb, pb), out);
             else np = nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
         } else

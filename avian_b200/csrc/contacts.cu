@@ -451,11 +451,13 @@ __global__ void report_gather_kernel(GraphRows g, const uint32_t* __restrict__ l
     ob[i] = g.pflags[e] & EV_FLAGS; ob[n + i] = uint8_t(cnt);
 }
 
-// capsules != 0: the shape column holds a capsule, and the rows that name one are left to narrow_capsule_edges_kernel
+// capsules != 0: the shape column holds a capsule, and the rows that name one are left to narrow_capsule_edges_kernel; hulls != 0: the column
+// holds a convex hull, and the rows that name one are left to narrow_hull_edges_kernel
 template <class S>
-__global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh, int capsules) {
+__global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh, int capsules, int hulls) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.r.E) return;
+    if (hulls && hull_row(a, e)) return;
     if (capsules && capsule_row(a, e)) return;
     if (only_fresh) {            // the rows added after the early pass over the existing rows (Contacts::prefetch_inputs)
         if (!fresh[e]) return;
@@ -466,9 +468,10 @@ __global__ void __launch_bounds__(128) narrow_edges_kernel(const __grid_constant
 
 // the rows that name a capsule (launched after narrow_edges_kernel, on the same stream, only when the shape column holds a capsule)
 template <class S>
-__global__ void __launch_bounds__(128) narrow_capsule_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh) {
+__global__ void __launch_bounds__(128) narrow_capsule_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, uint8_t* fresh, int only_fresh, int hulls) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.r.E || !capsule_row(a, e)) return;
+    if (hulls && hull_row(a, e)) return;
     if (only_fresh) {
         if (!fresh[e]) return;
         fresh[e] = 0;
@@ -479,15 +482,30 @@ __global__ void __launch_bounds__(128) narrow_capsule_edges_kernel(const __grid_
 // with body frames (avn_contacts_set_body_frames) these two replace the pair above: the same rows, anchors relative to the centres of mass
 template <class S, bool CAPSULES>
 __global__ void __launch_bounds__(128) narrow_framed_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, const BodyFrameCols<S> f, uint8_t* fresh,
-                                                                  int only_fresh, int capsules) {
+                                                                  int only_fresh, int capsules, int hulls) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.r.E) return;
+    if (hulls && hull_row(a, e)) return;
     if (capsules && capsule_row(a, e) != CAPSULES) return;
     if (only_fresh) {
         if (!fresh[e]) return;
         fresh[e] = 0;
     }
     narrow_edge_row<S, CAPSULES, true>(a, e, f);
+}
+
+// the rows that name a convex hull (launched after the kernels above, on the same stream, only when the shape column holds a hull), with or
+// without body frames
+template <class S, bool FRAMES>
+__global__ void __launch_bounds__(128) narrow_hull_edges_kernel(const __grid_constant__ NarrowEdgeArgs<S> a, const BodyFrameCols<S> f, uint8_t* fresh,
+                                                                int only_fresh, const __grid_constant__ hm::Table t) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.r.E || !hull_row(a, e)) return;
+    if (only_fresh) {
+        if (!fresh[e]) return;
+        fresh[e] = 0;
+    }
+    narrow_edge_row<S, true, FRAMES, true>(a, e, f, &t);
 }
 
 
@@ -1068,16 +1086,27 @@ class Contacts final : public ContactsBase {
         out->dims = in_.dims;
         out->has_capsule = has_capsule_;
     }
+    void attach_hulls(const HullTable* hulls) override { hulls_ = hulls; }
+    bool has_hull() const override { return has_hull_; }
     AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) override {
         if (!in || !in->dims) return AVN_OK;   // step() reports the missing columns
         checked_ = nullptr;
-        if ((flags & AVN_CONTACTS_SHAPES_UNCHANGED) && in_.colliders == in->collider_count && in_.dims) return AVN_OK;   // the column is not copied
+        const uint32_t hull_count = hulls_->count();
+        if ((flags & AVN_CONTACTS_SHAPES_UNCHANGED) && in_.colliders == in->collider_count && in_.dims) {   // the column is not copied
+            if (has_hull_ && max_hull_ >= hull_count)   // the table changed under the kept column
+                return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: the kept shape column names convex hull %u, the hull table holds %u", max_hull_,
+                                  hull_count);
+            return AVN_OK;
+        }
         size_t at = 0;
-        bool capsule = false;
-        if (const char* why = check_shape_column(in->shape, in->dims, in->collider_count, sizeof(S) == 8 ? 64 : 32, &at, &capsule))
+        bool capsule = false, hull = false;
+        uint32_t max_hull = 0;
+        if (const char* why = check_shape_column(in->shape, in->dims, in->collider_count, sizeof(S) == 8 ? 64 : 32, &at, &capsule, &hull_count, &hull, &max_hull))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: collider %zu: %s", at, why);
-        checked_ = in;                  // upload_inputs commits has_capsule_ once this column is on the device
+        checked_ = in;                  // upload_inputs commits has_capsule_ / has_hull_ once this column is on the device
         checked_capsule_ = capsule;
+        checked_hull_ = hull;
+        checked_max_hull_ = max_hull;
         return AVN_OK;
     }
     bool has_capsule() const override { return has_capsule_; }
@@ -1409,7 +1438,11 @@ class Contacts final : public ContactsBase {
         if (!keep_shapes) {
             UPC(i_shape_, in->shape, C, uint8_t, in_.shape);
             UPC(i_dims_, in->dims, 3 * C, S, in_.dims);
-            if (checked_ == in) has_capsule_ = checked_capsule_;   // the flag describes the column now on the device
+            if (checked_ == in) {   // the flags describe the column now on the device
+                has_capsule_ = checked_capsule_;
+                has_hull_ = checked_hull_;
+                max_hull_ = checked_max_hull_;
+            }
         }
         UPC(i_pos_, in->position, 3 * C, S, in_.pos);
         UPC(i_rot_, in->rotation, 4 * C, S, in_.rot);
@@ -1459,11 +1492,16 @@ class Contacts final : public ContactsBase {
         a.thr2 = (0.1 * length_unit) * (0.1 * length_unit);
         a.match = match_contacts ? 1 : 0;
         if (in_.framed) {
-            narrow_framed_edges_kernel<S, false><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
-            if (has_capsule_) narrow_framed_edges_kernel<S, true><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, 1);
+            narrow_framed_edges_kernel<S, false><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0,
+                                                                                 has_hull_ ? 1 : 0);
+            if (has_capsule_)
+                narrow_framed_edges_kernel<S, true><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, 1, has_hull_ ? 1 : 0);
+            if (has_hull_) narrow_hull_edges_kernel<S, true><<<(n + 127) / 128, 128, 0, s>>>(a, in_.frames, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, hulls_->dev);
         } else {
-            narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0);
-            if (has_capsule_) narrow_capsule_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0);
+            narrow_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_capsule_ ? 1 : 0, has_hull_ ? 1 : 0);
+            if (has_capsule_) narrow_capsule_edges_kernel<S><<<(n + 127) / 128, 128, 0, s>>>(a, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, has_hull_ ? 1 : 0);
+            if (has_hull_)
+                narrow_hull_edges_kernel<S, false><<<(n + 127) / 128, 128, 0, s>>>(a, BodyFrameCols<S>{}, fresh_.as<uint8_t>(), only_fresh ? 1 : 0, hulls_->dev);
         }
         AVN_CUDA(cudaGetLastError());
         return AVN_OK;
@@ -1681,6 +1719,11 @@ class Contacts final : public ContactsBase {
     bool has_capsule_ = false;    // the shape column on the device holds a capsule
     const AvnNarrowInput* checked_ = nullptr;   // the input check_shapes last accepted, and whether its column holds a capsule
     bool checked_capsule_ = false;
+    const HullTable* hulls_ = nullptr;
+    bool has_hull_ = false;       // the shape column on the device holds a convex hull; max_hull_: the largest index it names
+    uint32_t max_hull_ = 0;
+    bool checked_hull_ = false;
+    uint32_t checked_max_hull_ = 0;
     bool added_this_step_ = false;
     IslandState isl_{};
     IslandCounters* h_isl_ = nullptr;

@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/avian_b200.h"
+#include "hull_table.hpp"
 
 namespace avn {
 
@@ -54,13 +55,32 @@ struct DevBuf {
 };
 
 // The shape column of a collider set on the host, before anything is copied (a refused call changes nothing): every value at most
-// AVN_SHAPE_CAPSULE, and a capsule's radius and half length not negative.  NULL shape = all cuboids.  Returns NULL or the reason, with the
-// first offending collider in *at; *any_capsule (optional) tells whether the column holds a capsule.
-inline const char* check_shape_column(const uint8_t* shape, const void* dims, size_t count, uint32_t scalar_bits, size_t* at, bool* any_capsule = nullptr) {
+// AVN_SHAPE_CAPSULE (AVN_SHAPE_CONVEX_HULL where hulls are implemented: hull_count != NULL), a capsule's radius and half length not negative,
+// and a hull's index integral and below *hull_count.  NULL shape = all cuboids.  Returns NULL or the reason, with the first offending collider
+// in *at; *any_capsule / *any_hull (optional) tell whether the column holds a capsule / a hull, *max_hull the largest hull index it names.
+inline const char* check_shape_column(const uint8_t* shape, const void* dims, size_t count, uint32_t scalar_bits, size_t* at, bool* any_capsule = nullptr,
+                                      const uint32_t* hull_count = nullptr, bool* any_hull = nullptr, uint32_t* max_hull = nullptr) {
     if (any_capsule) *any_capsule = false;
+    if (any_hull) *any_hull = false;
+    if (max_hull) *max_hull = 0;
     if (!shape) return nullptr;
     for (size_t i = 0; i < count; ++i) {
-        if (shape[i] > AVN_SHAPE_CAPSULE) { *at = i; return "unknown shape (AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE are known)"; }
+        if (shape[i] == AVN_SHAPE_CONVEX_HULL && hull_count) {
+            const double h = scalar_bits == 64 ? static_cast<const double*>(dims)[3 * i] : double(static_cast<const float*>(dims)[3 * i]);
+            if (*hull_count == 0) { *at = i; return "a convex hull collider, and no hull table is set (avn_set_convex_hulls)"; }
+            if (!(h >= 0 && h < double(*hull_count)) || h != double(uint32_t(h))) {
+                *at = i;
+                return "a convex hull's index must be integral, not negative and below the hull table's count";
+            }
+            if (any_hull) *any_hull = true;
+            if (max_hull && uint32_t(h) > *max_hull) *max_hull = uint32_t(h);
+            continue;
+        }
+        if (shape[i] > AVN_SHAPE_CAPSULE) {
+            *at = i;
+            return hull_count ? "unknown shape (AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE, AVN_SHAPE_CAPSULE and AVN_SHAPE_CONVEX_HULL are known)"
+                              : "unknown shape (AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE are known)";
+        }
         if (shape[i] != AVN_SHAPE_CAPSULE) continue;
         if (any_capsule) *any_capsule = true;
         const double r = scalar_bits == 64 ? static_cast<const double*>(dims)[3 * i] : double(static_cast<const float*>(dims)[3 * i]);
@@ -69,6 +89,15 @@ inline const char* check_shape_column(const uint8_t* shape, const void* dims, si
     }
     return nullptr;
 }
+
+// The context's convex hull table (avn_set_convex_hulls) on the device.  dev holds device pointers; count() is 0 while no table is set.  The
+// AABB updater, the narrow phase and the contact store hold a pointer to it.
+struct HullTable {
+    bool set = false;
+    hm::Table dev{};
+    DevBuf vert, plane, centre, radius, voff, foff, loff, loop, eoff, edge;
+    uint32_t count() const { return set ? dev.count : 0; }
+};
 
 // the context's communicator (comm.cu): NCCL bound at run time; a communicator of one needs no NCCL at all
 struct CommBase {
@@ -134,6 +163,7 @@ struct BroadphaseBase {
 struct AabbBase {
     virtual ~AabbBase() {}
     virtual AvnStatus update(const AvnAabbParams* prm, AvnColliderColumns* colliders) = 0;
+    virtual void attach_hulls(const HullTable* hulls) = 0;
 };
 AabbBase* make_aabb_updater(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
@@ -148,6 +178,7 @@ struct NarrowBase {
     virtual ~NarrowBase() {}
     // frames: NULL = a collider at its body's origin, the centre of mass at that origin
     virtual AvnStatus run(const AvnNarrowParams* prm, const AvnNarrowInput* in, AvnRawManifolds* out, const BodyFrames* frames) = 0;
+    virtual void attach_hulls(const HullTable* hulls) = 0;
 };
 NarrowBase* make_narrow(uint32_t scalar_bits, cudaStream_t stream, ErrorSink* err);
 
@@ -219,6 +250,10 @@ struct ContactsBase {
     //      AVN_CCD_CAPSULES, and launches its capsule TOI kernel only when it holds one)
     virtual AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) = 0;
     virtual bool has_capsule() const = 0;
+    // has_hull: the column on the device holds a convex hull (swept CCD refuses it; its rows run in the hull kernels).  The hull table is the
+    // context's (attach_hulls); a step under AVN_CONTACTS_SHAPES_UNCHANGED checks the kept column's largest hull index against it.
+    virtual bool has_hull() const = 0;
+    virtual void attach_hulls(const HullTable* hulls) = 0;
     // ---- body frames (avn_contacts_set_body_frames): checked and copied on the host (NULL clears them); body_frames() = NULL when none are set
     virtual AvnStatus set_body_frames(const AvnBodyFrames* frames) = 0;
     virtual const BodyFrames* body_frames() const = 0;

@@ -1,4 +1,4 @@
-// Contact manifolds for cuboid / sphere / capsule pairs on the device (SURVEY.md 8f "next #1", geometry stage).
+// Contact manifolds for cuboid / sphere / capsule / convex hull pairs on the device (SURVEY.md 8f "next #1", geometry stage).
 // Stands where NarrowPhase::update calls contact_manifolds for every contact pair (narrow_phase/system_param.rs:437-830,
 // collider/parry/contact_query.rs:156-261).  The arithmetic is csrc/narrow_math.hpp — the same header the host fixture compiles — evaluated
 // in double like the fixture and rounded to the column scalar on store, so the device manifolds equal the fixture's bit for bit
@@ -27,12 +27,18 @@ template <class S> __device__ __forceinline__ void st3(S* p, size_t i, nm::V3 v)
 // One thread per pair.  CAPSULES = false (narrow_phase_kernel): the cuboid / sphere pairs, and when `capsules` is set the pairs with a
 // capsule are skipped; CAPSULES = true (narrow_capsule_kernel, launched only for a shape column that holds a capsule): those pairs alone.
 // FRAMES (narrow_framed_kernel, launched instead of the two when body frames are set): anchors relative to the bodies' centres of mass.
-template <class S, bool CAPSULES, bool FRAMES = false>
-__device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules, const BodyFrameCols<S>& f = BodyFrameCols<S>{}) {
+// When `hulls` is set those kernels leave every pair with a convex hull to narrow_hull_kernel (HULLS = true, launched only for a shape column
+// that holds a hull), which runs hm::collide over the context's hull table `t`.
+template <class S, bool CAPSULES, bool FRAMES = false, bool HULLS = false>
+__device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules, const BodyFrameCols<S>& f = BodyFrameCols<S>{}, int hulls = 0,
+                                            const hm::Table* t = nullptr) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.n) return;
     const uint32_t ca = a.c1[k], cb = a.c2[k], ba = a.b1[k], bb = a.b2[k];
-    if (capsules && (a.shape[ca] == nm::SHAPE_CAPSULE || a.shape[cb] == nm::SHAPE_CAPSULE) != CAPSULES) return;
+    if (HULLS || hulls) {
+        if ((a.shape[ca] == hm::SHAPE_CONVEX_HULL || a.shape[cb] == hm::SHAPE_CONVEX_HULL) != HULLS) return;
+    }
+    if (!HULLS && capsules && (a.shape[ca] == nm::SHAPE_CAPSULE || a.shape[cb] == nm::SHAPE_CAPSULE) != CAPSULES) return;
     a.count[k] = 0;
     if (a.amin) {  // the pair is removed when the AABBs no longer overlap (system_param.rs:437-470)
         const nm::V3 mina = ld3(a.amin, ca), maxa = ld3(a.amax, ca), minb = ld3(a.amin, cb), maxb = ld3(a.amax, cb);
@@ -52,7 +58,9 @@ __device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules
     nm::V3 normal;
     nm::Contacts pts;
     const int ta = a.shape ? a.shape[ca] : nm::SHAPE_CUBOID, tb = a.shape ? a.shape[cb] : nm::SHAPE_CUBOID;
-    if (!nm::collide<CAPSULES>(ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts)) return;
+    if (HULLS ? !hm::collide(*t, ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts)
+              : !nm::collide<CAPSULES>(ta, ld3(a.dims, ca), pa, qa, tb, ld3(a.dims, cb), pb, qb, max_dist, normal, pts))
+        return;
     nm::PointOut out[4];
     const int np = FRAMES ? nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, pair_frames(f, ba, pa, bb, pb), out)
                           : nm::manifold_points(pts, normal, pa, pb, rel, w1, w2, a.dt, eff_margin, out);
@@ -67,12 +75,20 @@ __device__ __forceinline__ void narrow_pair(const NarrowArgs<S>& a, int capsules
 }
 
 template <class S>
-__global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant__ NarrowArgs<S> a, int capsules) { narrow_pair<S, false>(a, capsules); }
+__global__ void __launch_bounds__(128) narrow_phase_kernel(const __grid_constant__ NarrowArgs<S> a, int capsules, int hulls) {
+    narrow_pair<S, false>(a, capsules, BodyFrameCols<S>{}, hulls);
+}
 template <class S>
-__global__ void __launch_bounds__(128) narrow_capsule_kernel(const __grid_constant__ NarrowArgs<S> a) { narrow_pair<S, true>(a, 1); }
+__global__ void __launch_bounds__(128) narrow_capsule_kernel(const __grid_constant__ NarrowArgs<S> a, int hulls) {
+    narrow_pair<S, true>(a, 1, BodyFrameCols<S>{}, hulls);
+}
 template <class S, bool CAPSULES>
-__global__ void __launch_bounds__(128) narrow_framed_kernel(const __grid_constant__ NarrowArgs<S> a, const BodyFrameCols<S> f, int capsules) {
-    narrow_pair<S, CAPSULES, true>(a, capsules, f);
+__global__ void __launch_bounds__(128) narrow_framed_kernel(const __grid_constant__ NarrowArgs<S> a, const BodyFrameCols<S> f, int capsules, int hulls) {
+    narrow_pair<S, CAPSULES, true>(a, capsules, f, hulls);
+}
+template <class S, bool FRAMES>
+__global__ void __launch_bounds__(128) narrow_hull_kernel(const __grid_constant__ NarrowArgs<S> a, const BodyFrameCols<S> f, const __grid_constant__ hm::Table t) {
+    narrow_pair<S, true, FRAMES, true>(a, 1, f, 1, &t);
 }
 
 template <class S>
@@ -95,8 +111,9 @@ class Narrow final : public NarrowBase {
             if (in->collider1[k] >= C || in->collider2[k] >= C || in->body1[k] >= B || in->body2[k] >= B)
                 return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: pair %zu indexes past the collider / body columns", k);
         size_t at = 0;
-        bool capsules = false;
-        if (const char* why = check_shape_column(in->shape, in->dims, C, sizeof(S) == 8 ? 64 : 32, &at, &capsules))
+        bool capsules = false, hulls = false;
+        const uint32_t hull_count = hulls_->count();
+        if (const char* why = check_shape_column(in->shape, in->dims, C, sizeof(S) == 8 ? 64 : 32, &at, &capsules, &hull_count, &hulls))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "narrow phase: collider %zu: %s", at, why);
         NarrowArgs<S> a{};
         a.n = int(n);
@@ -138,12 +155,15 @@ class Narrow final : public NarrowBase {
         AVN_CUDA(cudaMemsetAsync(a.anchor2, 0, 12 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.penetration, 0, 4 * n * sizeof(S), stream_));
         AVN_CUDA(cudaMemsetAsync(a.normal_speed, 0, 4 * n * sizeof(S), stream_));
+        const int h = hulls ? 1 : 0;
         if (frames) {
-            narrow_framed_kernel<S, false><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, capsules ? 1 : 0);
-            if (capsules) narrow_framed_kernel<S, true><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, 1);
+            narrow_framed_kernel<S, false><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, capsules ? 1 : 0, h);
+            if (capsules) narrow_framed_kernel<S, true><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, 1, h);
+            if (hulls) narrow_hull_kernel<S, true><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, hulls_->dev);
         } else {
-            narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, capsules ? 1 : 0);
-            if (capsules) narrow_capsule_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a);
+            narrow_phase_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, capsules ? 1 : 0, h);
+            if (capsules) narrow_capsule_kernel<S><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, h);
+            if (hulls) narrow_hull_kernel<S, false><<<unsigned((n + 127) / 128), 128, 0, stream_>>>(a, f, hulls_->dev);
         }
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->point_count, a.count, n, cudaMemcpyDeviceToHost, stream_));
@@ -156,6 +176,7 @@ class Narrow final : public NarrowBase {
         AVN_CUDA(cudaStreamSynchronize(stream_));
         return AVN_OK;
     }
+    void attach_hulls(const HullTable* hulls) override { hulls_ = hulls; }
 
    private:
     template <class T> AvnStatus up(DevBuf& buf, const void* host, size_t count, const T** dev) {
@@ -168,6 +189,7 @@ class Narrow final : public NarrowBase {
     }
     cudaStream_t stream_;
     ErrorSink* err_;
+    const HullTable* hulls_ = nullptr;
     DevBuf i_c1_, i_c2_, i_b1_, i_b2_, i_shape_, i_dims_, i_pos_, i_rot_, i_lv_, i_av_, i_amin_, i_amax_, i_fpos_, i_frot_, i_fcom_;
     DevBuf o_cnt_, o_dis_, o_nrm_, o_a1_, o_a2_, o_pen_, o_ns_;
 };

@@ -325,6 +325,9 @@ AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* b
     if (ccd_active() && contacts->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "upload_resident: swept CCD is configured (avn_ccd_configure) and the contact store's shape column holds a "
                                                "capsule; capsule times of impact are not implemented");
+    if (ccd_active() && contacts->has_hull())
+        return err_->fail(AVN_ERR_UNSUPPORTED, "upload_resident: swept CCD is configured (avn_ccd_configure) and the contact store's shape column holds a "
+                                               "convex hull; hull times of impact are not implemented");
     ContactsBase::AsleepBodies asleep;
     contacts->asleep_bodies(&asleep);
     if (asleep.wake_skipped)
@@ -612,6 +615,9 @@ AvnStatus Solver<S>::run() {
     if (!uploaded_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run before avn_solver_upload");
     if (ccd_contacts_ && ccd_contacts_->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run: swept CCD is configured and the contact store's shape column holds a capsule; capsule "
+                                               "times of impact are not implemented");
+    if (ccd_contacts_ && ccd_contacts_->has_hull())
+        return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run: swept CCD is configured and the contact store's shape column holds a convex hull; hull "
                                                "times of impact are not implemented");
     if (!from_store_ || !ccd_contacts_)
         return err_->fail(AVN_ERR_UNSUPPORTED, "swept CCD is configured: it needs the contact store's ContactGraph (avn_solver_upload_resident), "

@@ -12,7 +12,7 @@ from . import _build, api
 _vp = C.c_void_p
 _lib = None
 
-SHAPE_CUBOID, SHAPE_SPHERE, SHAPE_CAPSULE = 0, 1, 2
+SHAPE_CUBOID, SHAPE_SPHERE, SHAPE_CAPSULE, SHAPE_CONVEX_HULL = 0, 1, 2, 3
 
 
 def _load():
@@ -23,18 +23,18 @@ def _load():
         lib.avh_create.restype = _vp
         lib.avh_destroy.argtypes = [_vp]
         lib.avh_set_shapes.argtypes = [_vp, _vp, _vp, _vp, _vp]
-        lib.avh_update_aabbs.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, C.c_double, _vp, _vp]
+        lib.avh_update_aabbs.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, C.c_double, _vp, _vp, _vp]
         lib.avh_get_order.argtypes = [_vp, _vp]
         lib.avh_get_order.restype = C.c_uint32
         lib.avh_set_order.argtypes = [_vp, _vp]
         lib.avh_existing_pairs.argtypes = [_vp, _vp, C.c_uint64]
         lib.avh_existing_pairs.restype = C.c_uint64
         lib.avh_add_pairs.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64]
-        lib.avh_narrow_phase.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_uint32, C.POINTER(C.c_uint32), _vp, _vp, _vp]
+        lib.avh_narrow_phase.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_uint32, C.POINTER(C.c_uint32), _vp, _vp, _vp, _vp]
         lib.avh_narrow_phase.restype = C.c_uint32
         lib.avh_export_manifolds.argtypes = [_vp, C.c_uint32] + [_vp] * 13
         lib.avh_store_impulses.argtypes = [_vp, C.c_uint32, _vp, _vp, _vp]
-        lib.avh_raw_manifolds.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 12 + [C.c_double, C.c_double] + [_vp] * 12
+        lib.avh_raw_manifolds.argtypes = [C.c_uint32, C.c_uint32] + [_vp] * 12 + [C.c_double, C.c_double] + [_vp] * 13
         lib.avh_active_edges.argtypes = [_vp] * 6
         lib.avh_active_edges.restype = C.c_uint32
         lib.avh_export_edges.argtypes = [_vp] * 7
@@ -45,6 +45,14 @@ def _load():
         lib.avh_rows_narrow.restype = None
         lib.avh_rows_narrow_framed.argtypes = lib.avh_rows_narrow.argtypes + [_vp] * 3
         lib.avh_rows_narrow_framed.restype = None
+        lib.avh_rows_narrow_hulls.argtypes = lib.avh_rows_narrow_framed.argtypes + [_vp]
+        lib.avh_rows_narrow_hulls.restype = None
+        lib.avh_hulls_create.argtypes = [C.c_uint32, _vp, _vp, _vp, _vp, _vp, C.c_char_p, C.c_uint32]
+        lib.avh_hulls_create.restype = _vp
+        lib.avh_hulls_destroy.argtypes = [_vp]
+        lib.avh_hulls_destroy.restype = None
+        lib.avh_hulls_info.argtypes = [_vp] * 7
+        lib.avh_hulls_info.restype = None
         lib.avh_raw_manifolds.restype = None
         lib.avh_remove_colliders.argtypes = [_vp, C.c_uint32, _vp]
         lib.avh_remove_colliders.restype = None
@@ -109,14 +117,68 @@ def body_frame_columns(scalar, frames: dict | None):
     return col("position", 3), col("rotation", 4), col("center_of_mass", 3)
 
 
+class HullTable:
+    """The fixture's convex hull table: avn_set_convex_hulls' checks and derivation (csrc/hull_math.hpp) over an api.ConvexHulls whose vertices
+    are rounded to the column scalar, as the library stores them.  Raises ValueError with the library's reason for a table it refuses."""
+
+    def __init__(self, scalar, hulls: "api.ConvexHulls"):
+        self.lib = _load()
+        self.hulls = hulls
+        self.count = hulls.count
+        v = np.ascontiguousarray(np.asarray(hulls.vertices, dtype=scalar).astype(np.float64))
+        cols = [np.ascontiguousarray(a, dtype=np.uint32) for a in (hulls.vertex_offsets, hulls.face_offsets, hulls.loop_offsets, hulls.loop)]
+        err = C.create_string_buffer(256)
+        self.h = self.lib.avh_hulls_create(self.count, _p(cols[0]), _p(v), _p(cols[1]), _p(cols[2]), _p(cols[3]), err, 256)
+        if not self.h:
+            raise ValueError(err.value.decode())
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.lib.avh_hulls_destroy(self.h)
+            self.h = None
+
+    def derived(self) -> dict:
+        """the derived columns: plane [F,4] (unit outward normal, offset), edge [E,4] (v0, v1, face of v0->v1, face of v1->v0; hull-local),
+        edge_offsets [H+1], centre [H,3] (vertex mean), radius [H]"""
+        counts = np.zeros(4, dtype=np.uint32)
+        self.lib.avh_hulls_info(self.h, _p(counts), None, None, None, None, None)
+        H, _, F, E = (int(x) for x in counts)
+        out = {"plane": np.zeros((F, 4)), "edge": np.zeros((E, 4), dtype=np.uint32), "edge_offsets": np.zeros(H + 1, dtype=np.uint32),
+               "centre": np.zeros((H, 3)), "radius": np.zeros(H)}
+        self.lib.avh_hulls_info(self.h, _p(counts), *(_p(out[k]) for k in ("plane", "edge", "edge_offsets", "centre", "radius")))
+        return out
+
+
+def _hull_table(scalar, hulls) -> "HullTable | None":
+    if hulls is None or isinstance(hulls, HullTable):
+        return hulls
+    return HullTable(scalar, hulls)
+
+
+def check_hull_indices(shape, dims, hulls) -> None:
+    """What avn_update_aabbs / avn_narrow_phase / avn_contacts_step refuse: a hull collider without a table, or an index the table does not hold."""
+    if shape is None:
+        return
+    hull = np.asarray(shape) == SHAPE_CONVEX_HULL
+    if not hull.any():
+        return
+    if hulls is None:
+        raise ValueError("a convex hull collider, and no hull table")
+    idx = np.asarray(dims, dtype=np.float64).reshape(-1, 3)[hull, 0]
+    if not (np.all(idx >= 0) and np.all(idx < hulls.count) and np.all(idx == np.floor(idx))):
+        raise ValueError("a convex hull's index must be integral, not negative and below the hull table's count")
+
+
 def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders: dict, lin_vel: np.ndarray, ang_vel: np.ndarray,
-                  f64_anchors: bool = False, frames: dict | None = None) -> dict:
+                  f64_anchors: bool = False, frames: dict | None = None, hulls=None) -> dict:
     """The geometry stage of the fixture's narrow phase for an explicit pair list (same columns as Context.narrow_phase).
     f64_anchors adds the unrounded anchors (what match_contacts compares on the next step).  frames: the body frames (dict position,
     rotation, center_of_mass=None, [B] rows), as Context.contacts_set_body_frames sets them; the anchors are then relative to the bodies'
-    centres of mass."""
+    centres of mass.  hulls: the convex hull table (api.ConvexHulls or HullTable) the hull colliders index."""
     lib = _load()
     dt_ = np.dtype(scalar)
+    hulls = _hull_table(dt_, hulls)
+    check_hull_indices(colliders.get("shape"), colliders.get("dims"), hulls)
     fp, fr, fc = body_frame_columns(dt_, frames)
     c1, c2, b1, b2 = (np.ascontiguousarray(x, dtype=np.uint32) for x in pairs)
     n = int(c1.shape[0])
@@ -131,7 +193,7 @@ def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders:
     lib.avh_raw_manifolds(32 if dt_ == np.float32 else 64, n, _p(c1), _p(c2), _p(b1), _p(b2), _p(cols["shape"]), _p(cols["dims"]), _p(cols["position"]),
                           _p(cols["rotation"]), _p(lv), _p(av), _p(cols["aabb_min"]), _p(cols["aabb_max"]), float(dt), float(contact_tolerance),
                           *(_p(out[k]) for k in ("point_count", "disjoint", "normal", "anchor1", "anchor2", "penetration", "normal_speed")), _p(a1d), _p(a2d),
-                          _p(fp), _p(fr), _p(fc))
+                          _p(fp), _p(fr), _p(fc), hulls.h if hulls is not None else None)
     if f64_anchors:
         out["anchor1_f64"], out["anchor2_f64"] = a1d, a2d
     return out
@@ -293,8 +355,11 @@ class HostPipeline:
     collider; the AABB update and the narrow phase then take the colliders' world poses (and their velocities) separately."""
 
     def __init__(self, shape_type: np.ndarray, dims: np.ndarray, friction: np.ndarray, restitution: np.ndarray, scalar=np.float32,
-                 collider_body: np.ndarray | None = None):
+                 collider_body: np.ndarray | None = None, hulls=None):
+        """hulls: the convex hull table (api.ConvexHulls or HullTable) that hull colliders index."""
         self.lib = _load()
+        self.hulls = _hull_table(scalar, hulls)
+        check_hull_indices(shape_type, dims, self.hulls)
         self.collider_body = None if collider_body is None else np.ascontiguousarray(collider_body, dtype=np.uint32)
         self.n = int(shape_type.shape[0])
         self.scalar = np.dtype(scalar)
@@ -320,7 +385,7 @@ class HostPipeline:
         if colliders is not None:
             c = {k: np.ascontiguousarray(colliders[k], dtype=self.scalar) for k in c}
         self.lib.avh_update_aabbs(self.h, self.bits, _p(c["position"]), _p(c["rotation"]), _p(c["linear_velocity"]), _p(c["angular_velocity"]), dt,
-                                  _p(mn), _p(mx))
+                                  _p(mn), _p(mx), self.hulls.h if self.hulls is not None else None)
         return mn, mx
 
     def intervals(self, bodies: api.Bodies, aabb_min: np.ndarray, aabb_max: np.ndarray, with_existing: bool = True) -> api.Aabbs:
@@ -361,7 +426,7 @@ class HostPipeline:
             frames = body_frame_columns(self.scalar, {"position": bodies.position, "rotation": bodies.rotation, "center_of_mass": bodies.center_of_mass})
         m = int(self.lib.avh_narrow_phase(self.h, self.bits, _p(kind), _p(pos), _p(rot), _p(bodies.linear_velocity),
                                           _p(bodies.angular_velocity), _p(aabb_min), _p(aabb_max), dt, 1 if match_contacts else 0, C.byref(pts),
-                                          *(_p(f) for f in frames)))
+                                          *(_p(f) for f in frames), self.hulls.h if self.hulls is not None else None))
         return self.export_manifolds(m, int(pts.value))
 
     def export_manifolds(self, m: int | None = None, p: int | None = None) -> api.Manifolds:
@@ -508,7 +573,8 @@ def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, 
                            _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
                            *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
     if st == api.ERR_UNSUPPORTED:
-        raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule and the configuration does not set CCD_CAPSULES")
+        raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule and the configuration does not set CCD_CAPSULES, "
+                                 "or it names a convex hull")
     if st != 0:
         raise ValueError("avh_ccd_solve: invalid configuration")
     return out

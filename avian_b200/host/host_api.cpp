@@ -2,7 +2,7 @@
 // around the GPU hot path, so the hot path can be exercised and benchmarked without Bevy:
 //   * swept collider AABBs        (restates update_aabb for cuboids/spheres/capsules, collider/backend.rs:498-625)
 //   * ContactGraph bookkeeping    (pair set, lowest-free ContactId, contact_graph.rs:521-631; id_pool.rs:43-52)
-//   * a narrow phase for cuboid / sphere / capsule pairs (SAT + face clipping; the reference delegates this arithmetic
+//   * a narrow phase for cuboid / sphere / capsule / convex hull pairs (SAT + face clipping; the reference delegates this arithmetic
 //     to parry3d 0.25, which is not vendored, so this is OUR manifold generator: a fixture, identical for the
 //     oracle and the GPU path, not a parity claim), contact matching (contact_types/mod.rs:426-470),
 //     the status-change loop and ConstraintGraph push/pop colouring (narrow_phase/system_param.rs:136-389,
@@ -23,6 +23,7 @@
 
 #include "../../include/avian_b200.h"
 #include "../csrc/narrow_math.hpp"
+#include "../csrc/hull_math.hpp"
 #include "../csrc/contact_rows.hpp"
 #include "../csrc/query_math.hpp"
 #include "../csrc/ccd_math.hpp"
@@ -155,7 +156,7 @@ static void rows_narrow(uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, ui
                         void* a2, void* pen, void* ns, uint8_t* prev_count, double* prev_a1, double* prev_a2, void* ws_n_in, void* ws_t_in, void* ws_n_out,
                         void* ws_t_out, const uint8_t* shape, const void* dims, const void* pos, const void* rot, const void* lv, const void* av,
                         const void* amin, const void* amax, double dt, double tol, double length_unit, uint32_t match, const void* body_pos = nullptr,
-                        const void* body_rot = nullptr, const void* body_com = nullptr) {
+                        const void* body_rot = nullptr, const void* body_com = nullptr, const hm::HullSet* hulls = nullptr) {
     avn::NarrowEdgeArgs<T> a{};
     a.r.E = int(E);
     a.r.c1 = c1; a.r.c2 = c2; a.r.b1 = b1; a.r.b2 = b2; a.r.live = live; a.r.count = count; a.r.disjoint = disjoint;
@@ -167,10 +168,24 @@ static void rows_narrow(uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, ui
     a.lv = static_cast<const T*>(lv); a.av = static_cast<const T*>(av); a.amin = static_cast<const T*>(amin); a.amax = static_cast<const T*>(amax);
     a.dt = dt; a.tol = tol; a.thr2 = (0.1 * length_unit) * (0.1 * length_unit); a.match = match ? 1 : 0;
     const avn::BodyFrameCols<T> f{static_cast<const T*>(body_pos), static_cast<const T*>(body_rot), static_cast<const T*>(body_com)};
+    const hm::Table t = hulls ? hm::view(*hulls) : hm::Table{};
     for (uint32_t e = 0; e < E; ++e) {
-        if (body_pos) avn::narrow_edge_row<T, true, true>(a, int(e), f);
+        if (hulls && avn::hull_row(a, int(e))) {   // what narrow_hull_edges_kernel runs
+            if (body_pos) avn::narrow_edge_row<T, true, true, true>(a, int(e), f, &t);
+            else avn::narrow_edge_row<T, true, false, true>(a, int(e), f, &t);
+        } else if (body_pos) avn::narrow_edge_row<T, true, true>(a, int(e), f);
         else avn::narrow_edge_row<T>(a, int(e));
     }
+}
+
+// The geometry of one pair with the fixture's dispatch: a pair with a convex hull goes to hm::collide over the table (no table: no contact;
+// the Python wrappers check the indices), every other pair to nm::collide.
+bool collide_any(const hm::HullSet* hulls, int ta, V3 da, V3 pa, Q qa, int tb, V3 db, V3 pb, Q qb, S max_dist, V3& normal, Contacts& pts) {
+    if (ta == hm::SHAPE_CONVEX_HULL || tb == hm::SHAPE_CONVEX_HULL) {
+        pts.clear();
+        return hulls && hm::collide(hm::view(*hulls), ta, da, pa, qa, tb, db, pb, qb, max_dist, normal, pts);
+    }
+    return collide(ta, da, pa, qa, tb, db, pb, qb, max_dist, normal, pts);
 }
 
 // The body frames of a pair over host columns in either scalar (what contact_rows.hpp's pair_frames computes from device columns)
@@ -205,7 +220,8 @@ void avh_set_shapes(AvhPipeline* h, const int32_t* shape_type, const double* dim
 // update_aabb (collider/backend.rs:498-625) for the default configuration: speculative margin = MAX, no collision
 // margin, collider at the body origin.  AABB = merge(aabb(start pose), aabb(end pose)) grown by contact_tolerance.
 void avh_update_aabbs(AvhPipeline* h, uint32_t scalar_bits, const void* position, const void* rotation, const void* linvel, const void* angvel,
-                      double dt, void* out_min, void* out_max) {
+                      double dt, void* out_min, void* out_max, const void* hull_table) {
+    const hm::HullSet* hulls = static_cast<const hm::HullSet*>(hull_table);
     Pipeline& P = *reinterpret_cast<Pipeline*>(h);
     const bool f64 = scalar_bits == 64;
     Col pos{position, f64}, rt{rotation, f64}, lv{linvel, f64}, av{angvel, f64};
@@ -236,6 +252,19 @@ void avh_update_aabbs(AvhPipeline* h, uint32_t scalar_bits, const void* position
                       std::min(lo.z, std::min(ends[0].z, ends[1].z) - sh.he.x)};
                 hi = {std::max(hi.x, std::max(ends[0].x, ends[1].x) + sh.he.x), std::max(hi.y, std::max(ends[0].y, ends[1].y) + sh.he.x),
                       std::max(hi.z, std::max(ends[0].z, ends[1].z) + sh.he.x)};
+                continue;
+            }
+            if (sh.type == hm::SHAPE_CONVEX_HULL && hulls) {   // ConvexPolyhedron::aabb: every vertex moved by the pose (the product above)
+                const Q q = e ? q1 : q0;
+                const V3 b{q.x, q.y, q.z};
+                const uint32_t hi_ = uint32_t(sh.he.x);
+                for (uint32_t k = hulls->voff[hi_]; k < hulls->voff[hi_ + 1]; ++k) {
+                    const V3 v{hulls->vert[3 * k], hulls->vert[3 * k + 1], hulls->vert[3 * k + 2]};
+                    const V3 t = cross(b, v) * 2.0;
+                    const V3 w = ((v + cross(b, t)) + t * q.w) + c;
+                    lo = {std::min(lo.x, w.x), std::min(lo.y, w.y), std::min(lo.z, w.z)};
+                    hi = {std::max(hi.x, w.x), std::max(hi.y, w.y), std::max(hi.z, w.z)};
+                }
                 continue;
             }
             if (sh.type == SHAPE_SPHERE) {
@@ -475,8 +504,9 @@ uint32_t avh_report(AvhPipeline* h, uint32_t scalar_bits, uint32_t events_only, 
 // kind[n] = AvnBodyKind.  Returns the number of exported manifolds; *out_points = number of points.
 uint32_t avh_narrow_phase(AvhPipeline* h, uint32_t scalar_bits, const uint8_t* kind, const void* position, const void* rotation, const void* linvel,
                           const void* angvel, const void* aabb_min, const void* aabb_max, double dt, uint32_t match_contacts, uint32_t* out_points,
-                          const void* body_pos, const void* body_rot, const void* body_com) {
+                          const void* body_pos, const void* body_rot, const void* body_com, const void* hull_table) {
     Pipeline& P = *reinterpret_cast<Pipeline*>(h);
+    const hm::HullSet* hulls = static_cast<const hm::HullSet*>(hull_table);
     const bool f64 = scalar_bits == 64;
     Col pos{position, f64}, rt{rotation, f64}, lv{linvel, f64}, av{angvel, f64}, amin{aabb_min, f64}, amax{aabb_max, f64};
     const S tol = P.contact_tolerance * P.length_unit;
@@ -503,7 +533,7 @@ uint32_t avh_narrow_phase(AvhPipeline* h, uint32_t scalar_bits, const uint8_t* k
         pr.manifolds.clear();
         V3 normal;
         V3 pa = pos.v3(a), pb = pos.v3(b);
-        const bool hit = collide(sa.type, sa.he, pa, rt.q(a), sb.type, sb.he, pb, rt.q(b), max_dist, normal, pts);
+        const bool hit = collide_any(hulls, sa.type, sa.he, pa, rt.q(a), sb.type, sb.he, pb, rt.q(b), max_dist, normal, pts);
         if (hit) {
             PointOut out[4];
             const int np = body_pos ? manifold_points(pts, normal, pa, pb, rel, w1, w2, dt, eff_margin,
@@ -601,7 +631,8 @@ void avh_raw_manifolds(uint32_t scalar_bits, uint32_t pair_count, const uint32_t
                        const uint8_t* shape, const void* dims, const void* position, const void* rotation, const void* linvel, const void* angvel,
                        const void* aabb_min, const void* aabb_max, double dt, double tol, uint8_t* point_count, uint8_t* disjoint, void* normal,
                        void* anchor1, void* anchor2, void* penetration, void* normal_speed, double* anchor1_f64, double* anchor2_f64, const void* body_pos,
-                       const void* body_rot, const void* body_com) {
+                       const void* body_rot, const void* body_com, const void* hull_table) {
+    const hm::HullSet* hulls = static_cast<const hm::HullSet*>(hull_table);
     const bool f64 = scalar_bits == 64;
     Col dm{dims, f64}, pos{position, f64}, rt{rotation, f64}, lv{linvel, f64}, av{angvel, f64}, amin{aabb_min, f64}, amax{aabb_max, f64};
     ColW on{normal, f64}, oa1{anchor1, f64}, oa2{anchor2, f64}, op{penetration, f64}, os{normal_speed, f64};
@@ -626,7 +657,7 @@ void avh_raw_manifolds(uint32_t scalar_bits, uint32_t pair_count, const uint32_t
         V3 nrm;
         Contacts pts;
         int ta = shape ? shape[a] : SHAPE_CUBOID, tb = shape ? shape[b] : SHAPE_CUBOID;
-        if (!collide(ta, dm.v3(a), pa, rt.q(a), tb, dm.v3(b), pb, rt.q(b), max_dist, nrm, pts)) continue;
+        if (!collide_any(hulls, ta, dm.v3(a), pa, rt.q(a), tb, dm.v3(b), pb, rt.q(b), max_dist, nrm, pts)) continue;
         PointOut out[4];
         int np = body_pos ? manifold_points(pts, nrm, pa, pb, rel, w1, w2, dt, eff_margin, host_pair_frames(f64, body_pos, body_rot, body_com, b1[k], pa, b2[k], pb), out)
                           : manifold_points(pts, nrm, pa, pb, rel, w1, w2, dt, eff_margin, out);
@@ -727,7 +758,8 @@ void avh_rows_narrow(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c
         rows_narrow<float>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
                            shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match);
 }
-// avh_rows_narrow with body frames: body_pos [B][3], body_rot [B][4], body_com [B][3] (NULL = 0) in the column scalar
+// avh_rows_narrow with body frames: body_pos [B][3], body_rot [B][4], body_com [B][3] (NULL = 0) in the column scalar.  avh_rows_narrow_hulls:
+// the same with the hull table (avh_hulls_create) as the trailing argument; body_pos NULL = no frames.
 void avh_rows_narrow_framed(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* live, uint8_t* count,
                             uint8_t* disjoint, void* normal, void* a1, void* a2, void* pen, void* ns, uint8_t* prev_count, double* prev_a1, double* prev_a2,
                             void* ws_n_in, void* ws_t_in, void* ws_n_out, void* ws_t_out, const uint8_t* shape, const void* dims, const void* pos,
@@ -739,6 +771,45 @@ void avh_rows_narrow_framed(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint
     else
         rows_narrow<float>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
                            shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match, body_pos, body_rot, body_com);
+}
+void avh_rows_narrow_hulls(uint32_t scalar_bits, uint32_t E, uint32_t* c1, uint32_t* c2, uint32_t* b1, uint32_t* b2, uint8_t* live, uint8_t* count,
+                           uint8_t* disjoint, void* normal, void* a1, void* a2, void* pen, void* ns, uint8_t* prev_count, double* prev_a1, double* prev_a2,
+                           void* ws_n_in, void* ws_t_in, void* ws_n_out, void* ws_t_out, const uint8_t* shape, const void* dims, const void* pos,
+                           const void* rot, const void* lv, const void* av, const void* amin, const void* amax, double dt, double tol, double length_unit,
+                           uint32_t match, const void* body_pos, const void* body_rot, const void* body_com, const void* hull_table) {
+    const hm::HullSet* hulls = static_cast<const hm::HullSet*>(hull_table);
+    if (scalar_bits == 64)
+        rows_narrow<double>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
+                            shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match, body_pos, body_rot, body_com, hulls);
+    else
+        rows_narrow<float>(E, c1, c2, b1, b2, live, count, disjoint, normal, a1, a2, pen, ns, prev_count, prev_a1, prev_a2, ws_n_in, ws_t_in, ws_n_out, ws_t_out,
+                           shape, dims, pos, rot, lv, av, amin, amax, dt, tol, length_unit, match, body_pos, body_rot, body_com, hulls);
+}
+
+// The convex hull table of the fixture: avn_set_convex_hulls' checks and derivation (csrc/hull_math.hpp, the same routine), vertices already
+// widened to double from the column scalar.  Returns the table, or NULL with the reason in err.  The fixture functions take it as their
+// optional trailing argument.
+void* avh_hulls_create(uint32_t hull_count, const uint32_t* vertex_offsets, const double* vertices, const uint32_t* face_offsets, const uint32_t* loop_offsets,
+                       const uint32_t* loop, char* err, uint32_t err_size) {
+    hm::HullSet* s = new hm::HullSet();
+    uint32_t at = 0;
+    if (const char* why = hm::derive_hulls(hull_count, vertex_offsets, vertices, face_offsets, loop_offsets, loop, s, &at)) {
+        snprintf(err, err_size, "hull %u: %s", at, why);
+        delete s;
+        return nullptr;
+    }
+    return s;
+}
+void avh_hulls_destroy(void* hulls) { delete static_cast<hm::HullSet*>(hulls); }
+// table queries the tests read: counts, and the derived columns (plane [F][4], edge [E][4], centre [H][3], radius [H])
+void avh_hulls_info(const void* hulls, uint32_t* counts /*[4]: H, V, F, E*/, double* plane, uint32_t* edge, uint32_t* eoff, double* centre, double* radius) {
+    const hm::HullSet& s = *static_cast<const hm::HullSet*>(hulls);
+    counts[0] = uint32_t(s.radius.size()); counts[1] = uint32_t(s.vert.size() / 3); counts[2] = uint32_t(s.plane.size() / 4); counts[3] = uint32_t(s.edge.size() / 4);
+    if (plane) std::copy(s.plane.begin(), s.plane.end(), plane);
+    if (edge) std::copy(s.edge.begin(), s.edge.end(), edge);
+    if (eoff) std::copy(s.eoff.begin(), s.eoff.end(), eoff);
+    if (centre) std::copy(s.centre.begin(), s.centre.end(), centre);
+    if (radius) std::copy(s.radius.begin(), s.radius.end(), radius);
 }
 
 uint32_t avh_pair_count(AvhPipeline* h) { return uint32_t(reinterpret_cast<Pipeline*>(h)->active.size()); }
@@ -1325,7 +1396,7 @@ extern "C" {
 
 // solve_swept_ccd over the given contact rows.  Velocities: the SolverBody velocities after the substeps; delta_position / delta_rotation
 // ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration (an
-// unknown cfg->flags bit included) and AVN_ERR_UNSUPPORTED for a live row that names a capsule without AVN_CCD_CAPSULES.  The geometry is
+// unknown cfg->flags bit included) and AVN_ERR_UNSUPPORTED for a live row that names a capsule without AVN_CCD_CAPSULES, or a convex hull.  The geometry is
 // the CAPS = true instance either way: with no capsule in a pair it is the device's CAPS = false TOI, bit for bit.
 int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position, const void* rotation,
                   const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation, const uint8_t* shape, const void* dims,
@@ -1337,6 +1408,10 @@ int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t 
     if (cfg->count && shape && !(cfg->flags & AVN_CCD_CAPSULES))
         for (uint32_t r = 0; r < rows; ++r)
             if ((!live || live[r]) && (shape[c1[r]] == SHAPE_CAPSULE || shape[c2[r]] == SHAPE_CAPSULE)) return AVN_ERR_UNSUPPORTED;
+    // convex hulls have no times of impact: a configuration with a row that names one is refused, flag or not, as the device refuses it
+    if (cfg->count && shape)
+        for (uint32_t r = 0; r < rows; ++r)
+            if ((!live || live[r]) && (shape[c1[r]] == hm::SHAPE_CONVEX_HULL || shape[c2[r]] == hm::SHAPE_CONVEX_HULL)) return AVN_ERR_UNSUPPORTED;
     if (scalar_bits == 64)
         return ccd_solve<double>(dt, length_unit, body_count, kind, static_cast<const double*>(position), static_cast<const double*>(rotation),
                                  static_cast<const double*>(com), static_cast<const double*>(linvel), static_cast<const double*>(angvel),

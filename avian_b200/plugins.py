@@ -209,9 +209,9 @@ class World:
             if ccd is not None:
                 raise ValueError("swept CCD assumes a collider at its body's origin: a scene with a collider table cannot use it")
             self.pipeline = HostPipeline(scene.collider_shape, scene.collider_dims, scene.collider_friction, scene.collider_restitution, scalar=self.scalar,
-                                         collider_body=scene.collider_body)
+                                         collider_body=scene.collider_body, hulls=scene.hulls)
         else:
-            self.pipeline = HostPipeline(scene.shape_type, scene.dims, scene.friction, scene.restitution, scalar=self.scalar)
+            self.pipeline = HostPipeline(scene.shape_type, scene.dims, scene.friction, scene.restitution, scalar=self.scalar, hulls=scene.hulls)
         self.collider_pose: dict | None = None   # a collider table: the colliders' world poses of the current step
         integ = plugins.get("IntegratorPlugin")
         cfg = getattr(plugins.get("SolverPlugin"), "config", None) or SolverConfig()
@@ -344,6 +344,8 @@ class DeviceGraphWorld(World):
     def __init__(self, scene: Scene, plugins: PhysicsPlugins, ctx: "api.Context", sleeping: dict | None = None, **kw):
         super().__init__(scene, plugins, **kw)
         self.ctx = ctx
+        if scene.hulls is not None:
+            ctx.set_convex_hulls(scene.hulls)
         n = int(scene.bodies.count)
         self.n = n
         nc = int(scene.collider_body.shape[0]) if scene.compound else n

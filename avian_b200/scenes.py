@@ -32,6 +32,8 @@ class Scene:
     collider_dims: np.ndarray | None = None          # float64[C,3]
     collider_friction: np.ndarray | None = None      # float64[C]
     collider_restitution: np.ndarray | None = None   # float64[C]
+    # optional convex hull table (api.ConvexHulls): colliders of shape SHAPE_CONVEX_HULL name a hull by index in dims[0]
+    hulls: api.ConvexHulls | None = None
 
     @property
     def compound(self) -> bool:
@@ -76,6 +78,29 @@ def _capsule_mass(radius: np.ndarray, half_length: np.ndarray, density: float = 
     iy = m_cyl * r * r / 2.0 + m_sph * 2.0 * r * r / 5.0
     ix = m_cyl * (L * L / 12.0 + r * r / 4.0) + m_sph * (2.0 * r * r / 5.0 + L * L / 4.0 + 3.0 * L * r / 8.0)
     return m_cyl + m_sph, np.stack([ix, iy, ix], axis=1)
+
+
+def hull_mass(vertices, faces, density: float = 1.0):
+    """mass, centre of mass and inertia tensor (about the centre of mass, 3x3) of a solid convex polyhedron: a sum of tetrahedra from the vertex
+    mean over the fan triangles of every face, each with the canonical tetrahedron covariance.  PARITY UNPINNED: the reference takes hull mass
+    properties from bevy_heavy / parry, which are not vendored."""
+    v = np.asarray(vertices, dtype=np.float64)
+    ref = v.mean(axis=0)
+    c0 = np.array([[2.0, 1.0, 1.0], [1.0, 2.0, 1.0], [1.0, 1.0, 2.0]]) / 120.0
+    vol, first, cov = 0.0, np.zeros(3), np.zeros((3, 3))
+    for f in faces:
+        f = [int(i) for i in f]
+        for k in range(1, len(f) - 1):
+            A = np.stack([v[f[0]] - ref, v[f[k]] - ref, v[f[k + 1]] - ref], axis=1)
+            det = float(np.linalg.det(A))
+            vol += det / 6.0
+            first += det / 24.0 * A.sum(axis=1)
+            cov += det * (A @ c0 @ A.T)
+    m = density * vol
+    com_rel = first / vol
+    cov_c = density * cov - m * np.outer(com_rel, com_rel)
+    inertia = np.trace(cov_c) * np.eye(3) - cov_c
+    return m, ref + com_rel, inertia
 
 
 def _assemble(name, pos, rot, kind, he, shape_type, scalar, friction=0.5, restitution=0.0, linvel=None, angvel=None, density=1.0, **extra) -> Scene:
@@ -517,3 +542,226 @@ def spherical_chain(links: int = 100, scalar=np.float32) -> Scene:
                    joint_disabled_body_pairs=dis)
     # a kinematic body keeps its collider mass (SolverBodyInertia::new keeps inv_mass, dominance 128)
     return sc
+
+
+# ---- convex hulls (DESIGN.md §7k) ------------------------------------------------------------------------------------------------------
+
+def _polygon_faces(points, simplices, equations, tol: float = 1e-9):
+    """Qhull's triangles merged into polygon faces: triangles on the same plane become one loop of their vertices, counter-clockwise seen from
+    outside (ordered by angle about the face centre)."""
+    faces, used = [], np.zeros(len(simplices), dtype=bool)
+    for i in range(len(simplices)):
+        if used[i]:
+            continue
+        same = np.nonzero(np.all(np.abs(equations - equations[i]) < tol, axis=1) & ~used)[0]
+        used[same] = True
+        idx = np.unique(simplices[same].ravel())
+        n = equations[i, :3]
+        c = points[idx].mean(axis=0)
+        u = points[idx[0]] - c
+        u /= np.linalg.norm(u)
+        w = np.cross(n, u)
+        ang = np.arctan2((points[idx] - c) @ w, (points[idx] - c) @ u)
+        faces.append([int(k) for k in idx[np.argsort(ang)]])
+    return faces
+
+
+def convex_hull_of(points):
+    """(vertices, faces) of the convex hull of a point cloud: scipy's Qhull with coplanar triangles merged, vertices renumbered to those on the hull"""
+    from scipy.spatial import ConvexHull
+    pts = np.asarray(points, dtype=np.float64)
+    h = ConvexHull(pts)
+    keep = np.unique(h.simplices.ravel())
+    remap = {int(k): i for i, k in enumerate(keep)}
+    faces = _polygon_faces(pts, h.simplices, h.equations)
+    return pts[keep], [[remap[k] for k in f] for f in faces]
+
+
+def regular_solids(scale: float = 0.3):
+    """tetrahedron, octahedron and icosahedron of circumradius `scale`, and a 32-sided prism (radius scale, half height scale / 2)"""
+    t = np.array([[1, 1, 1], [1, -1, -1], [-1, 1, -1], [-1, -1, 1]], dtype=np.float64) / np.sqrt(3.0)
+    o = np.array([[1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1]], dtype=np.float64)
+    g = (1 + np.sqrt(5.0)) / 2
+    ico = np.array([[0, s1, s2 * g] for s1 in (-1, 1) for s2 in (-1, 1)] + [[s1, s2 * g, 0] for s1 in (-1, 1) for s2 in (-1, 1)]
+                   + [[s2 * g, 0, s1] for s1 in (-1, 1) for s2 in (-1, 1)], dtype=np.float64)
+    ico /= np.linalg.norm(ico[0])
+    out = [convex_hull_of(x * scale) for x in (t, o, ico)]
+    k = 32
+    a = 2 * np.pi * np.arange(k) / k
+    ring = np.stack([np.cos(a) * scale, np.zeros(k), np.sin(a) * scale], axis=1)
+    v = np.concatenate([ring + [0, -scale / 2, 0], ring + [0, scale / 2, 0]])
+    faces = [list(range(k)), list(range(2 * k - 1, k - 1, -1))]   # bottom seen from below, top seen from above
+    faces += [[i, (i + 1) % k, k + (i + 1) % k, k + i][::-1] for i in range(k)]
+    out.append((v, _orient(v, faces)))
+    return out
+
+
+def _orient(v, faces):
+    """every loop counter-clockwise seen from outside (reversed where its Newell normal points at the vertex mean)"""
+    c = v.mean(axis=0)
+    res = []
+    for f in faces:
+        p = v[f]
+        n = np.cross(p - p.mean(axis=0), np.roll(p, -1, axis=0) - p.mean(axis=0)).sum(axis=0)
+        res.append(list(f) if n @ (p.mean(axis=0) - c) > 0 else list(f)[::-1])
+    return res
+
+
+def _centred(v, faces):
+    """the polyhedron moved so its centre of mass is the origin (the body's origin), with its mass properties"""
+    m, com, inertia = hull_mass(v, faces)
+    v = np.asarray(v, dtype=np.float64) - com
+    return v, faces, m, inertia
+
+
+def hull_pile(n: int, seed: int = 13, layers: int = 4, scalar=np.float32, kinds: int = 24) -> Scene:
+    """A seeded pile of n dynamic bodies on a static ground cuboid (body 0): mostly convex hulls - `kinds` random hulls (Qhull over 10-18
+    seeded points in a ball of radius 0.2-0.35, coplanar triangles merged into polygons), the regular tetrahedron, octahedron and icosahedron
+    and a 32-sided prism - plus some cuboids, spheres and capsules, on a jittered grid that starts without overlaps.  Every hull is moved so its
+    centre of mass is its origin; mass properties by hull_mass."""
+    rng = np.random.default_rng(seed)
+    polys = [convex_hull_of(rng.normal(size=(int(rng.integers(10, 19)), 3)) * rng.uniform(0.2, 0.35) / 2.0) for _ in range(kinds)]
+    polys += regular_solids(0.3)
+    table = [_centred(v, f) for v, f in polys]
+    hulls = api.ConvexHulls.from_polyhedra([(v, f) for v, f, _, _ in table])
+    u = rng.uniform(size=n)
+    shape = np.where(u < 0.7, api.SHAPE_CONVEX_HULL, np.where(u < 0.8, SHAPE_CUBOID, np.where(u < 0.9, SHAPE_SPHERE, SHAPE_CAPSULE)))
+    he = np.zeros((n, 3))
+    hull = shape == api.SHAPE_CONVEX_HULL
+    idx = rng.integers(0, len(table), size=n)
+    he[hull, 0] = idx[hull]
+    box, sph, cap = shape == SHAPE_CUBOID, shape == SHAPE_SPHERE, shape == SHAPE_CAPSULE
+    he[box] = rng.uniform(0.15, 0.3, size=(box.sum(), 3))
+    he[sph] = rng.uniform(0.15, 0.3, size=sph.sum())[:, None]
+    he[cap, 0] = rng.uniform(0.1, 0.2, size=cap.sum())
+    he[cap, 1] = rng.uniform(0.1, 0.3, size=cap.sum())
+    q = rng.normal(size=(n, 4))
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    pitch = 1.2
+    side = int(np.ceil(np.sqrt(n / layers)))
+    k = np.arange(n)
+    layer, cell = k // (side * side), k % (side * side)
+    pos = np.stack([(cell // side) * pitch, 0.8 + layer * pitch, (cell % side) * pitch], axis=1) + rng.uniform(-0.05, 0.05, size=(n, 3))
+    order = np.lexsort((pos[:, 2], pos[:, 1], pos[:, 0]))
+    pos, q, he, shape = pos[order], q[order], he[order], shape[order]
+    extent = side * pitch
+    pos = np.concatenate([[[extent * 0.5, -0.5, extent * 0.5]], pos])
+    he = np.concatenate([[[extent * 0.5 + 10.0, 0.5, extent * 0.5 + 10.0]], he])
+    rot = np.concatenate([[[0.0, 0.0, 0.0, 1.0]], q])
+    kind = np.concatenate([[api.BODY_STATIC], np.full(n, api.BODY_DYNAMIC)])
+    shape = np.concatenate([[SHAPE_CUBOID], shape])
+    sc = _assemble(f"hull_pile_{n}", pos, rot, kind, np.where((shape == api.SHAPE_CONVEX_HULL)[:, None], 0.5, he), shape, scalar, hulls=hulls)
+    sc.dims = np.ascontiguousarray(he)
+    _set_hull_mass(sc, table)
+    return _own_velocities(sc)
+
+
+def _own_velocities(sc: Scene) -> Scene:
+    """_assemble hands a float64 scene one zero array for both velocity columns: give the angular velocity its own"""
+    sc.bodies.angular_velocity = sc.bodies.angular_velocity.copy()
+    return sc
+
+
+def _set_hull_mass(sc: Scene, table) -> None:
+    """the hull bodies' inverse mass and inverse inertia (upper triangle xx, xy, xz, yy, yz, zz) from the table's mass properties"""
+    s = sc.bodies.inverse_mass.dtype
+    for b in np.nonzero((sc.shape_type == api.SHAPE_CONVEX_HULL) & (sc.bodies.kind == api.BODY_DYNAMIC))[0]:
+        _, _, m, inertia = table[int(sc.dims[b, 0])]
+        inv = np.linalg.inv(inertia)
+        sc.bodies.inverse_mass[b] = s.type(1.0 / m)
+        sc.bodies.inverse_inertia_local[b] = np.array([inv[0, 0], inv[0, 1], inv[0, 2], inv[1, 1], inv[1, 2], inv[2, 2]]).astype(s)
+
+
+def _box_points(he):
+    return np.array([[(1 if m & 1 else -1) * he[0], (1 if m & 2 else -1) * he[1], (1 if m & 4 else -1) * he[2]] for m in range(8)], dtype=np.float64)
+
+
+def _decomposed_scene(name, bodies_parts, ground_extent, at, yaw, scalar) -> Scene:
+    """A compound scene from bodies given as convex decompositions: bodies_parts[i] = [(vertices, faces, position)] in the body's design
+    frame, the ground cuboid as body 0.  Each part's vertices are centred on its centre of mass and the part sits at that point (its local
+    position), like parry's Compound of a convex decomposition.  Every body's origin is its centre of mass; mass properties: hull_mass per
+    part, moved by the parallel-axis theorem (PARITY UNPINNED)."""
+    polys, cb, lp, cd = [], [], [], []
+    pos, rot, inv_m, inv_i = [], [], [], []
+    for i, parts in enumerate(bodies_parts):
+        props = []
+        for v, f, p in parts:
+            m, com, inertia = hull_mass(np.asarray(v, dtype=np.float64) + p, f)
+            props.append((m, com, inertia, np.asarray(v, dtype=np.float64) + p - com, f))
+        M = sum(x[0] for x in props)
+        c = sum(x[0] * x[1] for x in props) / M
+        I = np.zeros((3, 3))
+        for m, com, inertia, v, f in props:
+            d = com - c
+            I += inertia + m * (d @ d * np.eye(3) - np.outer(d, d))
+            cb.append(i + 1)
+            lp.append(com - c)
+            cd.append([float(len(polys)), 0.0, 0.0])
+            polys.append((v, f))
+        q = _quat_axis_angle((0, 1, 0), yaw[i])
+        pos.append(at[i])
+        rot.append(q)
+        Iinv = np.linalg.inv(I)
+        inv_m.append(1.0 / M)
+        inv_i.append([Iinv[0, 0], Iinv[0, 1], Iinv[0, 2], Iinv[1, 1], Iinv[1, 2], Iinv[2, 2]])
+    n = len(bodies_parts)
+    B, s = n + 1, np.dtype(scalar)
+    g = np.asarray(ground_extent, dtype=np.float64)
+    kind = np.concatenate([[api.BODY_STATIC], np.full(n, api.BODY_DYNAMIC)]).astype(np.uint8)
+    P = np.concatenate([[[g[0], -0.5, g[2]]], np.array(pos).reshape(-1, 3)])
+    R = np.concatenate([[[0.0, 0.0, 0.0, 1.0]], np.array(rot).reshape(-1, 4)])
+    z3 = np.zeros((B, 3))
+    bodies = api.Bodies(kind=kind, position=np.ascontiguousarray(P, dtype=s), rotation=np.ascontiguousarray(R, dtype=s),
+                        linear_velocity=np.ascontiguousarray(z3, dtype=s), angular_velocity=np.ascontiguousarray(z3, dtype=s),
+                        inverse_mass=np.ascontiguousarray(np.concatenate([[0.0], inv_m]), dtype=s),
+                        inverse_inertia_local=np.ascontiguousarray(np.concatenate([np.zeros((1, 6)), np.array(inv_i).reshape(-1, 6)]), dtype=s),
+                        center_of_mass=np.zeros((B, 3), dtype=s))
+    C_ = len(cb) + 1
+    ground_dims = [g[0] + 10.0, 0.5, g[2] + 10.0]
+    cshape = np.concatenate([[SHAPE_CUBOID], np.full(C_ - 1, api.SHAPE_CONVEX_HULL)]).astype(np.int32)
+    cdims = np.concatenate([[ground_dims], np.array(cd).reshape(-1, 3)])
+    return Scene(name, bodies, np.full(B, SHAPE_CUBOID, np.int32), np.tile(ground_dims, (B, 1)), np.full(B, 0.5), np.zeros(B),
+                 collider_body=np.concatenate([[0], cb]).astype(np.int32), local_position=np.concatenate([np.zeros((1, 3)), np.array(lp).reshape(-1, 3)]),
+                 local_rotation=np.tile([0.0, 0.0, 0.0, 1.0], (C_, 1)), collider_shape=cshape, collider_dims=np.ascontiguousarray(cdims),
+                 collider_friction=np.full(C_, 0.5), collider_restitution=np.zeros(C_), hulls=api.ConvexHulls.from_polyhedra(polys))
+
+
+def decomposed_l_block(upright_x: float = -0.4, scalar=np.float64) -> Scene:
+    """One L-block given as a convex decomposition of two hull parts (a foot of half extents 0.5 x 0.1 x 0.2 and an upright of 0.1 x 0.6 x 0.2
+    standing on it at x = upright_x) resting on the ground: it stays up while its centre of mass is over the foot (upright_x = -0.4) and tips
+    when the upright hangs past the foot's end (upright_x = -1.05)."""
+    foot = (_box_points([0.5, 0.1, 0.2]), _CUBE_LOOPS, np.array([0.0, 0.1, 0.0]))
+    upright = (_box_points([0.1, 0.6, 0.2]), _CUBE_LOOPS, np.array([upright_x, 0.8, 0.0]))
+    # the body origin is the centre of mass: place it so the foot rests 1 mm above the ground
+    m1, m2 = 0.5 * 0.1 * 0.2, 0.1 * 0.6 * 0.2
+    c = (m1 * foot[2] + m2 * upright[2]) / (m1 + m2)
+    return _decomposed_scene("decomposed_l_block", [[foot, upright]], [5.0, 0.0, 5.0], [c + [0.0, 0.001, 0.0]], [0.0], scalar)
+
+
+_CUBE_LOOPS = [[1, 3, 7, 5], [0, 4, 6, 2], [2, 6, 7, 3], [0, 1, 5, 4], [4, 5, 7, 6], [0, 2, 3, 1]]
+
+
+def decomposed_pile(n: int, seed: int = 17, layers: int = 4, scalar=np.float32) -> Scene:
+    """A seeded pile of n dynamic bodies, each a convex decomposition of 2-4 hull parts (seeded Qhull rocks of 8-14 points, side by side along
+    a bent chain so the bodies are concave), at random yaws on a jittered grid over a static ground cuboid; like the compounds of parry's
+    convex_decomposition.  See _decomposed_scene for the frames and mass properties."""
+    rng = np.random.default_rng(seed)
+    pitch = 1.8
+    side = int(np.ceil(np.sqrt(n / layers)))
+    bodies, at, yaw = [], [], []
+    for i in range(n):
+        k = int(rng.integers(2, 5))
+        parts, p, d = [], np.zeros(3), np.array([1.0, 0.0, 0.0])
+        for j in range(k):
+            v, f = convex_hull_of(rng.normal(size=(int(rng.integers(8, 15)), 3)) * rng.uniform(0.12, 0.18))
+            parts.append((v - v.mean(axis=0), f, p.copy()))
+            ang = rng.uniform(-1.2, 1.2)
+            d = np.array([d[0] * np.cos(ang) - d[1] * np.sin(ang), d[0] * np.sin(ang) + d[1] * np.cos(ang), 0.0])
+            p = p + d * 0.3
+        centre = np.mean([x[2] for x in parts], axis=0)
+        bodies.append([(v, f, q - centre) for v, f, q in parts])
+        layer, cell = i // (side * side), i % (side * side)
+        at.append(np.array([(cell // side) * pitch, 1.0 + layer * pitch, (cell % side) * pitch]) + rng.uniform(-0.05, 0.05, 3))
+        yaw.append(rng.uniform(-np.pi, np.pi))
+    extent = side * pitch
+    return _decomposed_scene(f"decomposed_pile_{n}", bodies, [extent * 0.5, 0.0, extent * 0.5], at, yaw, scalar)

@@ -372,8 +372,40 @@ AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
 /* ---- collider AABBs (SURVEY.md 8f "next #2"): update_aabb for the shapes the device knows ------------------------------- */
 /* AVN_SHAPE_CAPSULE: Collider::capsule(radius, length), dims = [radius, length / 2, unused]; the segment runs from (0, -length/2, 0) to
  * (0, +length/2, 0) in the collider frame.  The AABB update, the narrow phase, the contact store, the spatial queries (colliders and query
- * shapes), move and slide (obstacles and characters) and swept CCD (with AVN_CCD_CAPSULES) take capsules. */
-typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2 } AvnShape;
+ * shapes), move and slide (obstacles and characters) and swept CCD (with AVN_CCD_CAPSULES) take capsules.
+ * AVN_SHAPE_CONVEX_HULL: Collider::convex_hull / the parts of Collider::convex_decomposition, dims = [hull index, unused, unused] into the
+ * context's hull table (avn_set_convex_hulls).  The index is stored in the column scalar: integral, non-negative and below the table's hull
+ * count.  The AABB update, the narrow phase and the contact store take hulls; the spatial queries, move and slide refuse them, and swept CCD
+ * returns AVN_ERR_UNSUPPORTED while the contact store holds one. */
+typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2, AVN_SHAPE_CONVEX_HULL = 3 } AvnShape;
+
+/* ---- convex hulls: the table AVN_SHAPE_CONVEX_HULL colliders index (parry's ConvexPolyhedron: points, faces as vertex loops) ---------- */
+#define AVN_HULL_MAX_VERTICES 64u        /* per hull; the device kernels' fixed buffers are sized from these three */
+#define AVN_HULL_MAX_FACES 128u          /* per hull */
+#define AVN_HULL_MAX_FACE_VERTICES 32u   /* per face loop */
+#define AVN_HULL_MAX_COUNT (1u << 24)    /* hulls per table: every index is exact in an f32 dims column */
+/* The relative tolerance of the table checks: a face is planar, and a hull convex, when no vertex lies more than
+ * AVN_HULL_REL_TOL * size above a face plane (size = the diagonal of the hull's local vertex box); a face's area must exceed
+ * (AVN_HULL_REL_TOL * size)^2, and the vertex mean must lie more than AVN_HULL_REL_TOL * size below every face plane. */
+#define AVN_HULL_REL_TOL 1e-6
+typedef struct AvnConvexHulls {
+    uint32_t hull_count, _pad;
+    const uint32_t* vertex_offsets;    /* [hull_count + 1] CSR into vertices */
+    const void* vertices;              /* [V][3] column scalar, hull-local and already scaled (Collider::shape_scaled) */
+    const uint32_t* face_offsets;      /* [hull_count + 1] CSR into the faces (loop_offsets' rows) */
+    const uint32_t* loop_offsets;      /* [F + 1] CSR into loop */
+    const uint32_t* loop;              /* [L] hull-local vertex indices, each face counter-clockwise seen from outside */
+} AvnConvexHulls;
+/* Checks the table on the host and, when it is accepted, derives in double (face normals by Newell's method, plane offsets, the unique
+ * edges with the two faces each separates, each hull's vertex mean and bounding radius) and uploads it; every later avn_update_aabbs,
+ * avn_narrow_phase and avn_contacts_step of the context reads it.  NULL clears the table.  AVN_ERR_INVALID_ARGUMENT, before anything is
+ * stored (a refused call changes nothing), for: missing columns, more than AVN_HULL_MAX_COUNT hulls, decreasing offsets, a vertex index out
+ * of range, more than AVN_HULL_MAX_VERTICES vertices, AVN_HULL_MAX_FACES faces or AVN_HULL_MAX_FACE_VERTICES vertices on one face, a face
+ * loop of fewer than 3 or with a repeated vertex, two coincident vertices, an open or non-manifold surface (every directed edge once and its
+ * reverse once, V - E + F = 2), a zero-area, non-planar or inward-wound face, and a non-convex hull (tolerances: AVN_HULL_REL_TOL).
+ * A shape column that names a hull while no table is set, or an index at or past the hull count, is AVN_ERR_INVALID_ARGUMENT from
+ * avn_update_aabbs, avn_narrow_phase and avn_contacts_step, before anything is copied. */
+AvnStatus avn_set_convex_hulls(AvnContext* ctx, const AvnConvexHulls* hulls);
 
 typedef struct AvnAabbParams {
     double dt;                         /* Time::delta (full step, collider/backend.rs:536) */
@@ -401,7 +433,8 @@ typedef struct AvnColliderColumns {
  * Replaces update_aabb::<Collider> (src/collision/collider/backend.rs:498-625) for cuboid, sphere and capsule colliders: swept AABB from the
  * current pose to the pose after dt (rotation advanced by Quat::from_scaled_axis + fast_renormalize, translation clamped to the
  * speculative margin), grown by contact_tolerance + collision margin.  AVN_ERR_INVALID_ARGUMENT, before anything is computed, for a shape
- * above AVN_SHAPE_CAPSULE or a capsule with a negative radius or half length (avn_narrow_phase and avn_contacts_step check the same).
+ * above AVN_SHAPE_CONVEX_HULL, a capsule with a negative radius or half length, or a hull index the table does not hold (avn_narrow_phase
+ * and avn_contacts_step check the same).  A hull's AABB is parry's ConvexPolyhedron::aabb: every vertex moved by the pose, min / max.
  */
 AvnStatus avn_update_aabbs(AvnContext* ctx, const AvnAabbParams* params, AvnColliderColumns* colliders);
 
