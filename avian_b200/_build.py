@@ -17,7 +17,7 @@ CUDA_LIB = LIB_DIR / "libavian_b200.so"
 HOST_LIB = LIB_DIR / "libavian_host.so"
 
 CUDA_SOURCES = ["abi.cu", "comm.cu", "solver_host.cu", "broadphase.cu", "aabb.cu", "narrow.cu", "contacts.cu", "queries.cu", "ccd.cu"]
-CUDA_HEADERS = ["avn_math.cuh", "solver_dev.cuh", "joints_dev.cuh", "solver_kernels.cuh", "context.hpp", "joint_schedule.hpp", "broadphase_cells.cuh", "narrow_math.hpp", "hull_table.hpp", "hull_math.hpp", "contact_rows.hpp", "query_math.hpp", "ccd_math.hpp", "move_math.hpp"]
+CUDA_HEADERS = ["avn_math.cuh", "solver_dev.cuh", "joints_dev.cuh", "solver_kernels.cuh", "context.hpp", "joint_schedule.hpp", "broadphase_cells.cuh", "narrow_math.hpp", "hull_table.hpp", "shape_column.hpp", "hull_math.hpp", "contact_rows.hpp", "query_math.hpp", "hull_query_math.hpp", "ccd_math.hpp", "move_math.hpp"]
 # -fmad=false: the reference (Rust) never contracts a*b+c; parity at 1e-5 on contact dynamics needs the same
 # rounding.  Division and sqrt stay IEEE (nvcc defaults -prec-div=true -prec-sqrt=true).
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper)
@@ -45,13 +45,13 @@ def find_nvcc() -> str | None:
 
 # headers each translation unit depends on (anything not listed: every header)
 _UNIT_HEADERS = {
-    "comm.cu": ["context.hpp", "hull_table.hpp"],
-    "aabb.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp"],
-    "broadphase.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "broadphase_cells.cuh", "device_prims.cuh"],
-    "narrow.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp"],
-    "contacts.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp", "device_prims.cuh"],
-    "queries.cu": ["context.hpp", "hull_table.hpp", "narrow_math.hpp", "query_math.hpp", "move_math.hpp", "device_prims.cuh"],
-    "ccd.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "narrow_math.hpp", "query_math.hpp", "ccd_math.hpp", "device_prims.cuh"],
+    "comm.cu": ["context.hpp", "hull_table.hpp", "shape_column.hpp"],
+    "aabb.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp"],
+    "broadphase.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "broadphase_cells.cuh", "device_prims.cuh"],
+    "narrow.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp"],
+    "contacts.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp", "device_prims.cuh"],
+    "queries.cu": ["context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "query_math.hpp", "hull_query_math.hpp", "move_math.hpp", "device_prims.cuh"],
+    "ccd.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "query_math.hpp", "ccd_math.hpp", "device_prims.cuh"],
 }
 
 
@@ -110,8 +110,8 @@ def build_variant(name: str, defines: list[str]) -> Path:
 def build_host(force: bool = False) -> Path:
     src = ROOT / "host"
     deps = [p for p in src.glob("*.[ch]pp")] + [REPO / "include" / "avian_b200.h", ROOT / "csrc" / "narrow_math.hpp", ROOT / "csrc" / "contact_rows.hpp",
-            ROOT / "csrc" / "query_math.hpp", ROOT / "csrc" / "ccd_math.hpp", ROOT / "csrc" / "move_math.hpp", ROOT / "csrc" / "hull_math.hpp",
-            ROOT / "csrc" / "hull_table.hpp"]
+            ROOT / "csrc" / "query_math.hpp", ROOT / "csrc" / "ccd_math.hpp", ROOT / "csrc" / "move_math.hpp", ROOT / "csrc" / "hull_math.hpp", ROOT / "csrc" / "hull_query_math.hpp",
+            ROOT / "csrc" / "hull_table.hpp", ROOT / "csrc" / "shape_column.hpp"]
     if not force and _newer(HOST_LIB, deps):
         return HOST_LIB
     cxx = os.environ.get("CXX") or shutil.which("g++")

@@ -1148,8 +1148,10 @@ class Context:
         self._check(self.lib.avn_contacts_set_body_frames(self.handle, C.byref(f)))
 
     def set_convex_hulls(self, hulls: "ConvexHulls | None") -> None:
-        """avn_set_convex_hulls: the hull table every later update_aabbs / narrow_phase / contacts_step reads (None clears it).  Raises
-        AvianError (AVN_ERR_INVALID_ARGUMENT) for a table the library refuses; a refused call changes nothing."""
+        """avn_set_convex_hulls: the hull table every later update_aabbs / narrow_phase / contacts_step, query_update, spatial query and
+        move_and_slide reads (None clears it).  Replacing or clearing it makes every query and move_and_slide against a tree that holds a
+        hull refuse until the next query_update.  Raises AvianError (AVN_ERR_INVALID_ARGUMENT) for a table the library refuses; a refused
+        call changes nothing."""
         if hulls is None:
             self._check(self.lib.avn_set_convex_hulls(self.handle, None))
             return

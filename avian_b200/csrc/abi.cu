@@ -21,7 +21,7 @@ struct AvnContext {
     std::unique_ptr<avn::QueriesBase> queries;
     std::unique_ptr<avn::CommBase> comm;
     std::unique_ptr<avn::CcdBase> ccd;
-    avn::HullTable hulls;              // avn_set_convex_hulls; read by aabbs, narrow and contacts
+    avn::HullTable hulls;              // avn_set_convex_hulls; read by aabbs, narrow, contacts and queries
     AvnTimings last{};
 };
 
@@ -99,6 +99,7 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
         ctx->aabbs->attach_hulls(&ctx->hulls);
         ctx->narrow->attach_hulls(&ctx->hulls);
         ctx->contacts->attach_hulls(&ctx->hulls);
+        ctx->queries->attach_hulls(&ctx->hulls);
         *out_ctx = ctx.release();
         return AVN_OK;
     } catch (...) {
@@ -238,7 +239,7 @@ AvnStatus avn_narrow_phase(AvnContext* ctx, const AvnNarrowParams* params, const
 AvnStatus avn_set_convex_hulls(AvnContext* ctx, const AvnConvexHulls* hulls) {
     return guarded(ctx, [&]() -> AvnStatus {
         avn::HullTable& t = ctx->hulls;
-        if (!hulls) { t.set = false; return AVN_OK; }
+        if (!hulls) { t.set = false; ++t.generation; return AVN_OK; }
         const uint32_t H = hulls->hull_count;
         if (H > AVN_HULL_MAX_COUNT) return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "set_convex_hulls: %u hulls, at most AVN_HULL_MAX_COUNT", H);
         if (!hulls->vertex_offsets || !hulls->vertices || !hulls->face_offsets || !hulls->loop_offsets || !hulls->loop)
@@ -262,6 +263,7 @@ AvnStatus avn_set_convex_hulls(AvnContext* ctx, const AvnConvexHulls* hulls) {
             return buf.p;
         };
         t.set = false;   // a failed upload leaves no table
+        ++t.generation;
         hm::Table d{};
         d.count = H;
         d.vert = static_cast<const double*>(put(t.vert, set.vert.data(), set.vert.size() * sizeof(double)));

@@ -173,6 +173,22 @@ NM_HD inline Hull table_hull(const Table& t, uint32_t h, V3 c, Q q) {
     return H;
 }
 
+// table_hull posed by a given rotation matrix (the spatial queries pose every shape through qm::rot_mat, the normalised rotation)
+NM_HD inline Hull table_hull_at(const Table& t, uint32_t h, V3 c, const M3& r) {
+    Hull H;
+    const uint32_t v0 = t.voff[h], f0 = t.foff[h], e0 = t.eoff[h];
+    H.v = t.vert + 3 * size_t(v0);
+    H.pl = t.plane + 4 * size_t(f0);
+    H.loff = t.loff + f0;
+    H.loop = t.loop;
+    H.edge = t.edge + 4 * size_t(e0);
+    H.nv = int(t.voff[h + 1] - v0); H.nf = int(t.foff[h + 1] - f0); H.ne = int(t.eoff[h + 1] - e0);
+    H.r = r; H.c = c;
+    H.mid = c + xf(r, V3{t.centre[3 * h], t.centre[3 * h + 1], t.centre[3 * h + 2]});
+    H.radius = t.radius[h];
+    return H;
+}
+
 // A cuboid as a hull: vertex m = (+-he.x, +-he.y, +-he.z) with the sign of bit 0 / 1 / 2 of m; faces +x, -x, +y, -y, +z, -z.
 struct BoxHull {
     double v[24], pl[24];

@@ -19,14 +19,16 @@
 //   * the closest sweep hit is the lowest (t, collider index), not the first hit in tree order (the cast_shape rule).
 //   * intersections are visited in ascending collider index, not tree order (plane pruning and Gauss-Seidel depend on the order).
 //   * the reported hit distance is the TOI; the reference's MoveHitData::collision_distance is the requested movement length (:777).
-// Capsules (DESIGN.md §7j): the loop is a template over CAPS.  CAPS = true compiles the capsule casts of query_math.hpp and the capsule pairs of
-// nm::collide into the sweep and the intersections; CAPS = false is the cuboid / sphere loop as it was before capsule characters, for trees
-// and batches without a capsule (queries.cu picks the instance on the host).  The host fixture runs CAPS = true, which gives the same bits on
-// cuboids and spheres.
+// Capsules and hulls (DESIGN.md §7j, §7l): the loop is a template over the shape level G.  G = 1 compiles the capsule casts of query_math.hpp
+// and the capsule pairs of nm::collide into the sweep and the intersections; G = 0 is the cuboid / sphere loop as it was before capsule
+// characters.  G = 2 adds convex hulls: the casts of hull_query_math.hpp and hm::collide for the pairs with a hull, with the scene's hull
+// table (sc.hulls()).  queries.cu picks the instance on the host; the host fixture runs G = 2, which gives the G = 1 bits on cuboids, spheres
+// and capsules.
 #pragma once
 #include <cmath>
 #include <cstdint>
 
+#include "hull_query_math.hpp"
 #include "narrow_math.hpp"
 #include "query_math.hpp"
 
@@ -132,6 +134,25 @@ NM_COLD inline bool contact_plane(int sa, V3 ha, V3 pa, Q qa, int sb, V3 hb, V3 
     normal = T3<float>{float(-n.x), float(-n.y), float(-n.z)};
     return true;
 }
+// the same for the hull instance: a pair with a convex hull goes through hm::collide (either order), every other pair through
+// nm::collide<true>
+template <class T>
+NM_COLD inline bool contact_plane_hulls(const hm::Table& ht, int sa, V3 ha, V3 pa, Q qa, int sb, V3 hb, V3 pb, Q qb, double prediction, T3<float>& normal,
+                                        T& penetration) {
+    V3 n;
+    nm::Contacts pts;
+    const bool hit = sa == hm::SHAPE_CONVEX_HULL || sb == hm::SHAPE_CONVEX_HULL ? hm::collide(ht, sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts)
+                                                                                 : nm::collide<true>(sa, ha, pa, qa, sb, hb, pb, qb, prediction, n, pts);
+    if (!hit || pts.n == 0) return false;
+    T best = T(nm::dot(pts.p[0].a - pts.p[0].b, n));
+    for (int k = 1; k < pts.n; ++k) {
+        const T p = T(nm::dot(pts.p[k].a - pts.p[k].b, n));
+        if (!(p < best)) best = p;
+    }
+    penetration = best;
+    normal = T3<float>{float(-n.x), float(-n.y), float(-n.z)};
+    return true;
+}
 
 // a configured plane as a Dir (Dir::new on its f32 value); the ABI refuses zero and non-finite planes
 template <class T> NM_HD inline T3<float> plane_dir(T3<T> p) { const T3<float> f = narrow(p); return divs(f, std::sqrt(dot(f, f))); }
@@ -140,19 +161,20 @@ template <class T> NM_HD inline T3<float> plane_dir(T3<T> p) { const T3<float> f
 struct Body { int shape; V3 he; Q q; };
 
 // the character's tight AABB at pos, rounded to T, grown by `grow` (Aabb::grow)
-template <bool CAPS, class T>
-NM_HD inline void grown_aabb(const Body& b, T3<T> pos, T grow, T lo[3], T hi[3]) {
+template <int G, class T, class Scene>
+NM_HD inline void grown_aabb(const Scene& sc, const Body& b, T3<T> pos, T grow, T lo[3], T hi[3]) {
     V3 mn, mx;
-    qm::collider_aabb<CAPS>(b.shape, b.he, to_v3(pos), b.q, mn, mx);
+    if constexpr (G == 2) qh::collider_aabb(sc.hulls(), b.shape, b.he, to_v3(pos), b.q, mn, mx);
+    else qm::collider_aabb<G == 1>(b.shape, b.he, to_v3(pos), b.q, mn, mx);
     lo[0] = T(mn.x) - grow; lo[1] = T(mn.y) - grow; lo[2] = T(mn.z) - grow;
     hi[0] = T(mx.x) + grow; hi[1] = T(mx.y) + grow; hi[2] = T(mx.z) + grow;
 }
 
 // every intersection plane at pos with prediction distance `pred`, in ascending collider index: fn(normal, penetration)
-template <class T, bool CAPS, class Scene, class Fn>
+template <class T, int G, class Scene, class Fn>
 NM_HD inline void intersections(const Scene& sc, const Body& b, T3<T> pos, T pred, Fn fn) {
     T lo[3], hi[3];
-    grown_aabb<CAPS>(b, pos, pred, lo, hi);
+    grown_aabb<G>(sc, b, pos, pred, lo, hi);
     const V3 p = to_v3(pos);
     sc.candidates(lo, hi, [&](uint32_t c) {
         int s;
@@ -161,13 +183,16 @@ NM_HD inline void intersections(const Scene& sc, const Body& b, T3<T> pos, T pre
         sc.collider(c, s, he, cp, cq);
         T3<float> n;
         T pen;
-        if (contact_plane<T, CAPS>(b.shape, b.he, p, b.q, s, he, cp, cq, double(pred), n, pen)) fn(n, pen);
+        bool hit;
+        if constexpr (G == 2) hit = contact_plane_hulls<T>(sc.hulls(), b.shape, b.he, p, b.q, s, he, cp, cq, double(pred), n, pen);
+        else hit = contact_plane<T, G == 1>(b.shape, b.he, p, b.q, s, he, cp, cq, double(pred), n, pen);
+        if (hit) fn(n, pen);
     });
 }
 
 // depenetrate + depenetrate_intersections (:868-897, :982-1009): Gauss-Seidel over the (normal, penetration + skin) list.  The list is
 // kept when it has at most MOVE_WINDOW entries; a longer one is evaluated again, in the same order, in every iteration.
-template <bool CAPS, class T, class Scene>
+template <int G, class T, class Scene>
 NM_HD inline T3<T> depenetrate(const Scene& sc, const Config<T>& cfg, const Body& b, T3<T> pos) {
     T3<T> fixup{0, 0, 0};
     if (cfg.depenetration_iterations == 0) return fixup;
@@ -177,7 +202,7 @@ NM_HD inline T3<T> depenetrate(const Scene& sc, const Config<T>& cfg, const Body
     T3<float> ln[MOVE_WINDOW];
     T ld[MOVE_WINDOW];
     uint32_t count = 0;
-    intersections<T, CAPS>(sc, b, pos, skin, [&](T3<float> n, T pen) {
+    intersections<T, G>(sc, b, pos, skin, [&](T3<float> n, T pen) {
         if (count < uint32_t(MOVE_WINDOW)) { ln[count] = n; ld[count] = pen + skin; }
         ++count;
     });
@@ -196,7 +221,7 @@ NM_ROLLED
         if (kept) {
             for (uint32_t k = 0; k < count; ++k) relax(ln[k], ld[k]);
         } else {
-            intersections<T, CAPS>(sc, b, pos, skin, [&](T3<float> n, T pen) { relax(n, pen + skin); });
+            intersections<T, G>(sc, b, pos, skin, [&](T3<float> n, T pen) { relax(n, pen + skin); });
         }
         if (total < target) break;
     }
@@ -206,12 +231,12 @@ NM_ROLLED
 // MoveAndSlide::move_and_slide (:464-609) with an on_hit that accepts every hit.  pos / vel: in, out.  init: the configured planes
 // (MoveAndSlideConfig::planes) as f32 Dirs, n_init <= max_planes.  hits.sweep(iteration, collider, safe distance, toi, point1, normal1) is
 // called for every iteration that hit something.
-template <bool CAPS = false, class T, class Scene, class Hits>
+template <int G = 0, class T, class Scene, class Hits>
 NM_HD inline void move_and_slide(const Scene& sc, const Config<T>& cfg, const Body& b, T3<T>& pos, T3<T>& vel, const T3<float>* init, int n_init,
                                  Hits& hits) {
     T time_left = cfg.dt;
     const T skin = cfg.length_unit * cfg.skin_width;
-    pos = add(pos, depenetrate<CAPS>(sc, cfg, b, pos));
+    pos = add(pos, depenetrate<G>(sc, cfg, b, pos));
     T3<float> planes[MAX_PLANES + 1];
 NM_ROLLED
     for (uint32_t it = 0; it < cfg.iterations; ++it) {
@@ -237,7 +262,8 @@ NM_ROLLED
         Q cq;
         sc.collider(c, cs, che, cp, cq);
         qm::ShapeContact hc;
-        qm::cast_output<CAPS>(b.shape, b.he, p, b.q, d, qm::CAST_IGNORE_ORIGIN_PENETRATION, cs, che, cp, cq, toi, axis, hc);
+        if constexpr (G == 2) qh::cast_output(sc.hulls(), b.shape, b.he, p, b.q, d, qm::CAST_IGNORE_ORIGIN_PENETRATION, cs, che, cp, cq, toi, axis, hc);
+        else qm::cast_output<G == 1>(b.shape, b.he, p, b.q, d, qm::CAST_IGNORE_ORIGIN_PENETRATION, cs, che, cp, cq, toi, axis, hc);
         const T3<T> normal1 = from_v3<T>(hc.n1);
         const T hit_distance = T(toi);
         // pull_back (:789-793)
@@ -251,7 +277,7 @@ NM_ROLLED
         for (int k = 0; k < n_init; ++k) planes[np++] = init[k];
         planes[np++] = narrow(normal1);
         const T3<T> v = vel;
-        intersections<T, CAPS>(sc, b, pos, skin * T(2), [&](T3<float> n, T) {
+        intersections<T, G>(sc, b, pos, skin * T(2), [&](T3<float> n, T) {
             for (int k = 0; k < np; ++k) {
                 if (T(dot(n, planes[k])) >= cfg.plane_similarity_dot_threshold) {
                     // similar: keep the more blocking normal
@@ -264,7 +290,7 @@ NM_ROLLED
         });
         vel = project_velocity(vel, planes, np);
     }
-    pos = add(pos, depenetrate<CAPS>(sc, cfg, b, pos));
+    pos = add(pos, depenetrate<G>(sc, cfg, b, pos));
 }
 
 }  // namespace mv
@@ -273,10 +299,12 @@ NM_ROLLED
 #include "../../include/avian_b200.h"
 namespace mv {
 // NULL when the call is usable; the reason otherwise.  collider_count: the colliders of the scene (the tree's, the host's)
-// capsules: whether AVN_SHAPE_CAPSULE characters are accepted; saw_capsule (optional): set when the batch holds one
+// capsules: whether AVN_SHAPE_CAPSULE characters are accepted; saw_capsule (optional): set when the batch holds one.  hull_count / saw_hull:
+// hull characters, as qm::check_colliders takes hull colliders
 inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, bool f64, uint32_t collider_count, bool capsules = false,
-                              bool* saw_capsule = nullptr) {
+                              bool* saw_capsule = nullptr, const uint32_t* hull_count = nullptr, bool* saw_hull = nullptr) {
     if (saw_capsule) *saw_capsule = false;
+    if (saw_hull) *saw_hull = false;
     if (!cfg) return "config is required";
     if (!b) return "batch is required";
     const double vals[6] = {cfg->delta_time, cfg->length_unit, cfg->skin_width, cfg->max_depenetration_error, cfg->penetration_rejection_threshold,
@@ -289,6 +317,7 @@ inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, b
     if (b->count == 0) return nullptr;
     if (!b->shape || !b->dims || !b->position || !b->rotation || !b->velocity) return "batch: shape, dims, position, rotation and velocity are required";
     for (uint32_t i = 0; i < b->count; ++i) {
+        if (hull_count && b->shape[i] == AVN_SHAPE_CONVEX_HULL) continue;   // its index: below
         if (!capsules && b->shape[i] > AVN_SHAPE_SPHERE) return "batch: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
         if (b->shape[i] > AVN_SHAPE_CAPSULE) return "batch: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
         for (int k = 0; k < qm::shape_dims_read(b->shape[i]); ++k) {
@@ -297,6 +326,9 @@ inline const char* check_move(const AvnMoveConfig* cfg, const AvnMoveBatch* b, b
         }
         if (saw_capsule && b->shape[i] == AVN_SHAPE_CAPSULE) *saw_capsule = true;
     }
+    size_t at;
+    if (hull_count)
+        if (const char* why = avn::check_shape_column(b->shape, b->dims, b->count, f64 ? 64 : 32, &at, nullptr, hull_count, saw_hull)) return why;
     if (const char* why = qm::check_exclusions(b->count, b->exclude_count, b->exclude_offsets, b->exclude)) return why;
     if (b->plane_offsets) {
         if (b->plane_offsets[0] != 0) return "batch: plane_offsets must start at 0";

@@ -19,9 +19,10 @@
 // hit; project_point (570-615) prunes on the squared point-box distance; point and shape intersections (628-683, 744-826) use the same CSR
 // pattern.  Their geometry is the shape-cast part of query_math.hpp.
 // Move and slide (character_controller/move_and_slide.rs): q_move runs csrc/move_math.hpp's loop per character over this tree (TreeScene).
-// Capsules (DESIGN.md §7j): every kernel that evaluates a collider's or a query's shape has a CAPS instance of its own, launched when the tree
-// holds a capsule (remembered across AVN_QUERY_SHAPES_UNCHANGED updates) or the batch does; the CAPS = false instances compile the cuboid /
-// sphere code they had before capsules were queried.
+// Capsules and convex hulls (DESIGN.md §7j, §7l): every kernel that evaluates a collider's or a query's shape is a template over the shape
+// level G: 0 = cuboids and spheres, 1 = + capsules, 2 = + convex hulls (csrc/hull_query_math.hpp, over the context's hull table, which the
+// tree carries).  The host launches the lowest level that covers the tree (remembered across AVN_QUERY_SHAPES_UNCHANGED updates) and the
+// batch; the G = 0 and G = 1 instances compile the code they had before hulls were queried.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -30,6 +31,7 @@
 
 #include "context.hpp"
 #include "device_prims.cuh"
+#include "hull_query_math.hpp"
 #include "query_math.hpp"
 #include "move_math.hpp"
 
@@ -54,6 +56,7 @@ struct Tree {
     const NodeBox* nodes;                            // [2m - 1]: internal nodes [0, m - 1), leaf k at m - 1 + k; root = 0
     const int2* child;                               // [m - 1]
     const uint32_t* leaf;                            // [m] sorted position -> collider
+    hm::Table hulls;                                 // the context's hull table (count 0: none); read by the G = 2 instances only
 };
 
 template <class S>
@@ -68,6 +71,50 @@ template <class S> __device__ __forceinline__ nm::Q ldq(const S* p, size_t i) {
     return {double(p[4 * i]), double(p[4 * i + 1]), double(p[4 * i + 2]), double(p[4 * i + 3])};
 }
 
+// the geometry of shape level G (0: cuboid / sphere, 1: + capsule, 2: + convex hull over the tree's table)
+template <int G, class S>
+__device__ __forceinline__ void g_aabb(const Tree<S>& t, int shape, nm::V3 he, nm::V3 p, nm::Q q, nm::V3& mn, nm::V3& mx) {
+    if constexpr (G == 2) qh::collider_aabb(t.hulls, shape, he, p, q, mn, mx);
+    else qm::collider_aabb<G == 1>(shape, he, p, q, mn, mx);
+}
+template <int G, class S>
+__device__ __forceinline__ bool g_ray(const Tree<S>& t, int shape, nm::V3 he, nm::V3 p, nm::Q q, nm::V3 o, nm::V3 d, double maxd, bool solid, double& th, nm::V3& nh) {
+    if constexpr (G == 2) return qh::ray_collider(t.hulls, shape, he, p, q, o, d, maxd, solid, th, nh);
+    else return qm::ray_collider<G == 1>(shape, he, p, q, o, d, maxd, solid, th, nh);
+}
+template <int G, class S>
+__device__ __forceinline__ nm::V3 g_half_size(const Tree<S>& t, int shape, nm::V3 he, const nm::M3& r) {
+    if constexpr (G == 2) return qh::half_size(t.hulls, shape, he, r);
+    else return qm::half_size<G == 1>(shape, he, r);
+}
+template <int G, class S>
+__device__ __forceinline__ bool g_cast(const Tree<S>& t, int sa, nm::V3 ha, nm::V3 ca, nm::Q qa, nm::V3 d, double maxd, uint32_t flags, int sb, nm::V3 hb, nm::V3 cb,
+                                       nm::Q qb, double& th, int& axis) {
+    if constexpr (G == 2) return qh::cast_collider(t.hulls, sa, ha, ca, qa, d, maxd, flags, sb, hb, cb, qb, th, axis);
+    else return qm::cast_collider<G == 1>(sa, ha, ca, qa, d, maxd, flags, sb, hb, cb, qb, th, axis);
+}
+template <int G, class S>
+__device__ __forceinline__ void g_cast_output(const Tree<S>& t, int sa, nm::V3 ha, nm::V3 ca, nm::Q qa, nm::V3 d, uint32_t flags, int sb, nm::V3 hb, nm::V3 cb, nm::Q qb,
+                                              double th, int axis, qm::ShapeContact& h) {
+    if constexpr (G == 2) qh::cast_output(t.hulls, sa, ha, ca, qa, d, flags, sb, hb, cb, qb, th, axis, h);
+    else qm::cast_output<G == 1>(sa, ha, ca, qa, d, flags, sb, hb, cb, qb, th, axis, h);
+}
+template <int G, class S>
+__device__ __forceinline__ double g_project(const Tree<S>& t, int shape, nm::V3 he, nm::V3 c, nm::Q q, nm::V3 p, bool solid, nm::V3& proj, bool& inside) {
+    if constexpr (G == 2) return qh::project_point(t.hulls, shape, he, c, q, p, solid, proj, inside);
+    else return qm::project_point<G == 1>(shape, he, c, q, p, solid, proj, inside);
+}
+template <int G, class S>
+__device__ __forceinline__ bool g_contains(const Tree<S>& t, int shape, nm::V3 he, nm::V3 c, nm::Q q, nm::V3 p) {
+    if constexpr (G == 2) return qh::contains_point(t.hulls, shape, he, c, q, p);
+    else return qm::contains_point<G == 1>(shape, he, c, q, p);
+}
+template <int G, class S>
+__device__ __forceinline__ bool g_intersect(const Tree<S>& t, int sa, nm::V3 ha, nm::V3 ca, nm::Q qa, int sb, nm::V3 hb, nm::V3 cb, nm::Q qb) {
+    if constexpr (G == 2) return qh::shapes_intersect(t.hulls, sa, ha, ca, qa, sb, hb, cb, qb);
+    else return qm::shapes_intersect<G == 1>(sa, ha, ca, qa, sb, hb, cb, qb);
+}
+
 __device__ __forceinline__ uint32_t f_ord(float f) { const uint32_t u = __float_as_uint(f); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
 __device__ __forceinline__ float f_unord(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
 
@@ -80,7 +127,7 @@ __device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t* p, uint32_t v) {
 __device__ __forceinline__ float f32_clamped(double x) { return float(fmin(fmax(x, -double(FLT_MAX)), double(FLT_MAX))); }
 
 // 1. per collider: validity, tight AABB (rounded to S), f32 culling box, centre; scene bounds of the centres
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(256) q_prepare(const __grid_constant__ Tree<S> t, S* __restrict__ tmn, S* __restrict__ tmx, NodeBox* __restrict__ cbox,
                                                  float4* __restrict__ centre, uint8_t* __restrict__ valid, int* __restrict__ m, uint32_t* __restrict__ sb) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -92,13 +139,21 @@ __global__ void __launch_bounds__(256) q_prepare(const __grid_constant__ Tree<S>
         ok = qm::collider_valid(he, p, q);
         if (ok) {
             nm::V3 mn, mx;
-            qm::collider_aabb<CAPS>(t.shape[i], he, p, q, mn, mx);
+            g_aabb<G>(t, t.shape[i], he, p, q, mn, mx);
             tmn[3 * i] = S(mn.x); tmn[3 * i + 1] = S(mn.y); tmn[3 * i + 2] = S(mn.z);
             tmx[3 * i] = S(mx.x); tmx[3 * i + 1] = S(mx.y); tmx[3 * i + 2] = S(mx.z);
             NodeBox b;
-            qm::culling_bounds(mn.x, mx.x, b.lo.x, b.hi.x);
-            qm::culling_bounds(mn.y, mx.y, b.lo.y, b.hi.y);
-            qm::culling_bounds(mn.z, mx.z, b.lo.z, b.hi.z);
+            if constexpr (G == 2) {                      // a hull culls against its bounding ball's box (hull_query_math.hpp)
+                nm::V3 lo, hi;
+                qh::cull_box(t.hulls, t.shape[i], he, p, mn, mx, lo, hi);
+                qm::culling_bounds(lo.x, hi.x, b.lo.x, b.hi.x);
+                qm::culling_bounds(lo.y, hi.y, b.lo.y, b.hi.y);
+                qm::culling_bounds(lo.z, hi.z, b.lo.z, b.hi.z);
+            } else {
+                qm::culling_bounds(mn.x, mx.x, b.lo.x, b.hi.x);
+                qm::culling_bounds(mn.y, mx.y, b.lo.y, b.hi.y);
+                qm::culling_bounds(mn.z, mx.z, b.lo.z, b.hi.z);
+            }
             b.lo.w = b.hi.w = 0.f;
             cbox[i] = b;
             // the f32 centre only places the collider on the Morton curve: clamped, so a finite pose beyond the f32 range keeps finite
@@ -247,11 +302,11 @@ __device__ __forceinline__ RayIn<S> load_ray(const Rays<S>& r, int i) {
     q.ok = qm::ray_finite(q.o, q.d, q.maxd);
     return q;
 }
-template <bool CAPS, class S>
+template <int G, class S>
 __device__ __forceinline__ bool ray_leaf(const Tree<S>& t, const RayIn<S>& q, uint32_t c, double& th, nm::V3& nh) {
     const uint32_t memb = t.memb ? t.memb[c] : 1u;
     if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
-    return qm::ray_collider<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), q.o, q.d, q.maxd, q.solid, th, nh);
+    return g_ray<G>(t, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), q.o, q.d, q.maxd, q.solid, th, nh);
 }
 __device__ __forceinline__ bool ray_visit(const NodeBox& b, nm::V3 o, nm::V3 d, double tclip) {
     return qm::ray_box_entry(&b.lo.x, &b.hi.x, o, d, tclip) != INFINITY;
@@ -287,7 +342,7 @@ __device__ __forceinline__ void traverse_closest(const Tree<S>& t, int m, nm::V3
     }
 }
 
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, int32_t* __restrict__ out_c,
                                                          S* __restrict__ out_t, S* __restrict__ out_n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -300,7 +355,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ 
         traverse_closest(t, *t.m, q.o, q.d, q.maxd, best_t, [&](uint32_t c) {
             double th;
             nm::V3 nh;
-            if (ray_leaf<CAPS>(t, q, c, th, nh) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_n = nh; }
+            if (ray_leaf<G>(t, q, c, th, nh) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_n = nh; }
         });
     const bool hit = best_c != 0xffffffffu;
     out_c[i] = hit ? int32_t(best_c) : -1;
@@ -309,7 +364,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_ray(const __grid_constant__ 
 }
 
 // ray_hits count pass: every hit, and the part of it the ray keeps (max_hits)
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_ray_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, uint32_t* __restrict__ full,
                                                           uint32_t* __restrict__ kept) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -318,7 +373,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_count(const __grid_constant__
     uint32_t cnt = 0;
     if (q.ok)
         traverse(t, *t.m, [&](const NodeBox& b) { return ray_visit(b, q.o, q.d, q.maxd); },
-                 [&](uint32_t c) { double th; nm::V3 nh; if (ray_leaf<CAPS>(t, q, c, th, nh)) ++cnt; });
+                 [&](uint32_t c) { double th; nm::V3 nh; if (ray_leaf<G>(t, q, c, th, nh)) ++cnt; });
     full[i] = cnt;
     const uint32_t mh = r.max_hits ? r.max_hits[i] : 0xffffffffu;
     kept[i] = cnt < mh ? cnt : mh;
@@ -348,7 +403,7 @@ __device__ void sort_segment(uint32_t n, Less less, Swap swp) {
 }
 
 // ray_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their normals
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Rays<S> r, const uint64_t* __restrict__ full_off,
                                                          const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
                                                          uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ out_n) {
@@ -366,7 +421,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ 
              [&](uint32_t c) {
                  double th;
                  nm::V3 nh;
-                 if (ray_leaf<CAPS>(t, q, c, th, nh) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+                 if (ray_leaf<G>(t, q, c, th, nh) && w < n) { ts[w] = th; cs[w] = c; ++w; }
              });
     sort_segment(
         w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
@@ -376,7 +431,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_ray_emit(const __grid_constant__ 
         const uint32_t c = cs[k];
         double th;
         nm::V3 nh{0, 0, 0};
-        ray_leaf<CAPS>(t, q, c, th, nh);    // the same exact test again: the normal of this hit
+        ray_leaf<G>(t, q, c, th, nh);    // the same exact test again: the normal of this hit
         out_c[o + k] = c;
         if (out_t) out_t[o + k] = S(ts[k]);
         if (out_n) { out_n[3 * (o + k)] = S(nh.x); out_n[3 * (o + k) + 1] = S(nh.y); out_n[3 * (o + k) + 2] = S(nh.z); }
@@ -431,8 +486,8 @@ struct ShapeIn {
     float ext[3], lo[3], hi[3];
     bool ok;
 };
-template <bool CAPS, class S>
-__device__ __forceinline__ ShapeIn load_shape(const Shapes<S>& s, int i, bool cast) {
+template <int G, class S>
+__device__ __forceinline__ ShapeIn load_shape(const Tree<S>& t, const Shapes<S>& s, int i, bool cast) {
     ShapeIn q;
     q.shape = s.shape[i];
     q.he = ld3(s.dims, i);
@@ -446,7 +501,7 @@ __device__ __forceinline__ ShapeIn load_shape(const Shapes<S>& s, int i, bool ca
     q.nx = s.xoff ? s.xoff[i + 1] - s.xoff[i] : 0u;
     q.ok = cast ? qm::cast_finite(q.he, q.c, q.q, q.d, q.maxd) : qm::collider_valid(q.he, q.c, q.q);
     if (q.ok) {
-        const nm::V3 e = qm::half_size<CAPS>(q.shape, q.he, qm::rot_mat(q.q));
+        const nm::V3 e = g_half_size<G>(t, q.shape, q.he, qm::rot_mat(q.q));
         for (int k = 0; k < 3; ++k) {
             float l, h;
             qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, h);
@@ -503,16 +558,16 @@ __device__ __forceinline__ void traverse_nearest(const Tree<S>& t, int m, const 
     }
 }
 
-template <bool CAPS, class S>
+template <int G, class S>
 __device__ __forceinline__ bool cast_leaf(const Tree<S>& t, const ShapeIn& q, uint32_t c, double& th, int& axis) {
     const uint32_t memb = t.memb ? t.memb[c] : 1u;
     if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return false;
-    return qm::cast_collider<CAPS>(q.shape, q.he, q.c, q.q, q.d, q.maxd, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+    return g_cast<G>(t, q.shape, q.he, q.c, q.q, q.d, q.maxd, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
 }
-template <bool CAPS, class S>
+template <int G, class S>
 __device__ __forceinline__ void cast_store(const Tree<S>& t, const ShapeIn& q, uint32_t c, double th, int axis, size_t o, S* p1, S* p2, S* n1, S* n2) {
     qm::ShapeContact h;
-    qm::cast_output<CAPS>(q.shape, q.he, q.c, q.q, q.d, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis, h);
+    g_cast_output<G>(t, q.shape, q.he, q.c, q.q, q.d, q.flags, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis, h);
     const nm::V3 v[4] = {h.p1, h.p2, h.n1, h.n2};
     S* dst[4] = {p1, p2, n1, n2};
     for (int k = 0; k < 4; ++k)
@@ -521,12 +576,12 @@ __device__ __forceinline__ void cast_store(const Tree<S>& t, const ShapeIn& q, u
 __device__ __forceinline__ bool cast_visit(const NodeBox& b, const ShapeIn& q) { return grown_entry(b, q.ext, q.c, q.d, q.maxd) != INFINITY; }
 
 // cast_shape: the lexicographic minimum of (t, collider)
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_cast_shape(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, int32_t* __restrict__ out_c,
                                                            S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2, S* __restrict__ n1, S* __restrict__ n2) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape<CAPS>(s, i, true);
+    const ShapeIn q = load_shape<G>(t, s, i, true);
     double best_t = INFINITY;
     uint32_t best_c = 0xffffffffu;
     int best_axis = -1;
@@ -535,43 +590,43 @@ __global__ void __launch_bounds__(Q_THREADS) q_cast_shape(const __grid_constant_
                                [&](uint32_t c) {
                                    double th;
                                    int ax;
-                                   if (cast_leaf<CAPS>(t, q, c, th, ax) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_axis = ax; }
+                                   if (cast_leaf<G>(t, q, c, th, ax) && qm::hit_before(th, c, best_t, best_c)) { best_t = th; best_c = c; best_axis = ax; }
                                });
     const bool hit = best_c != 0xffffffffu;
     out_c[i] = hit ? int32_t(best_c) : -1;
     out_t[i] = hit ? S(best_t) : S(0);
     if (hit) {
-        cast_store<CAPS>(t, q, best_c, best_t, best_axis, size_t(i), p1, p2, n1, n2);
+        cast_store<G>(t, q, best_c, best_t, best_axis, size_t(i), p1, p2, n1, n2);
     } else {
         for (int k = 0; k < 3; ++k) p1[3 * i + k] = p2[3 * i + k] = n1[3 * i + k] = n2[3 * i + k] = S(0);
     }
 }
 
 // shape_hits count pass: every hit, and the part of it the query keeps (max_hits)
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_count(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ full,
                                                             uint32_t* __restrict__ kept) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape<CAPS>(s, i, true);
+    const ShapeIn q = load_shape<G>(t, s, i, true);
     uint32_t cnt = 0;
     if (q.ok)
         traverse(t, *t.m, [&](const NodeBox& b) { return cast_visit(b, q); },
-                 [&](uint32_t c) { double th; int ax; if (cast_leaf<CAPS>(t, q, c, th, ax)) ++cnt; });
+                 [&](uint32_t c) { double th; int ax; if (cast_leaf<G>(t, q, c, th, ax)) ++cnt; });
     full[i] = cnt;
     const uint32_t mh = s.max_hits ? s.max_hits[i] : 0xffffffffu;
     kept[i] = cnt < mh ? cnt : mh;
 }
 
 // shape_hits emit pass: all hits into the scratch segment, sorted by (t, collider), the first `kept` written out with their contacts
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, const uint64_t* __restrict__ full_off,
                                                            const uint64_t* __restrict__ kept_off, double* __restrict__ tmp_t, uint32_t* __restrict__ tmp_c,
                                                            uint32_t* __restrict__ out_c, S* __restrict__ out_t, S* __restrict__ p1, S* __restrict__ p2,
                                                            S* __restrict__ n1, S* __restrict__ n2) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape<CAPS>(s, i, true);
+    const ShapeIn q = load_shape<G>(t, s, i, true);
     if (!q.ok) return;
     const uint64_t base = full_off[i];
     const uint32_t n = uint32_t(full_off[i + 1] - base), keep = uint32_t(kept_off[i + 1] - kept_off[i]);
@@ -583,7 +638,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant_
              [&](uint32_t c) {
                  double th;
                  int ax;
-                 if (cast_leaf<CAPS>(t, q, c, th, ax) && w < n) { ts[w] = th; cs[w] = c; ++w; }
+                 if (cast_leaf<G>(t, q, c, th, ax) && w < n) { ts[w] = th; cs[w] = c; ++w; }
              });
     sort_segment(
         w, [&](uint32_t a, uint32_t b) { return qm::hit_before(ts[a], cs[a], ts[b], cs[b]); },
@@ -593,15 +648,15 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_emit(const __grid_constant_
         const uint32_t c = cs[k];
         double th = 0;
         int ax = -1;
-        cast_leaf<CAPS>(t, q, c, th, ax);    // the same exact test again: the axis of this hit
+        cast_leaf<G>(t, q, c, th, ax);    // the same exact test again: the axis of this hit
         out_c[o + k] = c;
         if (out_t) out_t[o + k] = S(ts[k]);
-        cast_store<CAPS>(t, q, c, ts[k], ax, size_t(o + k), p1, p2, n1, n2);
+        cast_store<G>(t, q, c, ts[k], ax, size_t(o + k), p1, p2, n1, n2);
     }
 }
 
 // project_point: the lexicographic minimum of (distance, collider); a node is pruned when its squared distance exceeds the best so far
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, int32_t* __restrict__ out_c,
                                                               S* __restrict__ out_p, uint8_t* __restrict__ out_in) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -622,7 +677,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_consta
                                     if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
                                     nm::V3 pr;
                                     bool in;
-                                    const double dd = qm::project_point<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p, solid, pr, in);
+                                    const double dd = g_project<G>(t, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p, solid, pr, in);
                                     if (qm::hit_before(dd, c, best_d, best_c)) { best_d = dd; best_c = c; best_p = pr; best_in = in; bound = dd * dd; }
                                 });
     const bool hit = best_c != 0xffffffffu;
@@ -632,7 +687,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_project_point(const __grid_consta
 }
 
 // point_intersections: count, then emit + sort ascending by collider
-template <class S, bool EMIT, bool CAPS>
+template <class S, bool EMIT, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Points<S> pts, uint32_t* __restrict__ counts,
                                                             const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -648,7 +703,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant
                  [&](uint32_t c) {
                      const uint32_t memb = t.memb ? t.memb[c] : 1u;
                      if (!qm::passes_filter(memb, mask, xs, nx, c)) return;
-                     if (!qm::contains_point<CAPS>(t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p)) return;
+                     if (!g_contains<G>(t, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), p)) return;
                      if (EMIT) seg[w] = c;
                      ++w;
                  });
@@ -657,12 +712,12 @@ __global__ void __launch_bounds__(Q_THREADS) q_point_isect(const __grid_constant
 }
 
 // shape_intersections: count, then emit + sort ascending by collider
-template <class S, bool EMIT, bool CAPS>
+template <class S, bool EMIT, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant__ Tree<S> t, const __grid_constant__ Shapes<S> s, uint32_t* __restrict__ counts,
                                                             const uint64_t* __restrict__ off, uint32_t* __restrict__ out_c) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= s.n) return;
-    const ShapeIn q = load_shape<CAPS>(s, i, false);
+    const ShapeIn q = load_shape<G>(t, s, i, false);
     uint32_t w = 0;
     uint32_t* seg = EMIT ? out_c + off[i] : nullptr;
     if (q.ok)
@@ -671,7 +726,7 @@ __global__ void __launch_bounds__(Q_THREADS) q_shape_isect(const __grid_constant
                  [&](uint32_t c) {
                      const uint32_t memb = t.memb ? t.memb[c] : 1u;
                      if (!qm::passes_filter(memb, q.mask, q.xs, q.nx, c)) return;
-                     if (!qm::shapes_intersect<CAPS>(q.shape, q.he, q.c, q.q, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c))) return;
+                     if (!g_intersect<G>(t, q.shape, q.he, q.c, q.q, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c))) return;
                      if (EMIT) seg[w] = c;
                      ++w;
                  });
@@ -689,13 +744,13 @@ struct Movers {
 };
 
 // the cast leaf of a move, out of line: the shape-cast geometry is instanced once in the move kernel, not at each inlined call site
-template <bool CAPS, class S>
+template <int G, class S>
 __device__ __noinline__ bool move_cast_leaf(const Tree<S>& t, uint32_t c, int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& th, int& axis) {
-    return qm::cast_collider<CAPS>(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
+    return g_cast<G>(t, shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, t.shape[c], ld3(t.dims, c), ld3(t.pos, c), ldq(t.rot, c), th, axis);
 }
 
 // the scene of move_math.hpp over the tree, with one character's filter
-template <class S, bool CAPS>
+template <class S, int G>
 struct TreeScene {
     const Tree<S>& t;
     int m;
@@ -710,10 +765,11 @@ struct TreeScene {
     __device__ void collider(uint32_t c, int& s, nm::V3& he, nm::V3& p, nm::Q& q) const {
         s = t.shape[c]; he = ld3(t.dims, c); p = ld3(t.pos, c); q = ldq(t.rot, c);
     }
+    __device__ const hm::Table& hulls() const { return t.hulls; }
     // the closest filtered cast: nearest-first over the node boxes grown by the shape's half size (as q_cast_shape)
     __device__ bool cast(int shape, nm::V3 he, nm::V3 ctr, nm::Q q, nm::V3 d, double maxd, double& t_out, uint32_t& c_out, int& axis_out) const {
         float ext[3];
-        const nm::V3 e = qm::half_size<CAPS>(shape, he, qm::rot_mat(q));
+        const nm::V3 e = g_half_size<G>(t, shape, he, qm::rot_mat(q));
         for (int k = 0; k < 3; ++k) {
             float l;
             qm::culling_bounds(-nm::comp(e, k), nm::comp(e, k), l, ext[k]);
@@ -726,7 +782,7 @@ struct TreeScene {
                                    if (!pass(c)) return;
                                    double th;
                                    int ax;
-                                   if (move_cast_leaf<CAPS>(t, c, shape, he, ctr, q, d, maxd, th, ax) && qm::hit_before(th, c, best_t, best_c)) {
+                                   if (move_cast_leaf<G>(t, c, shape, he, ctr, q, d, maxd, th, ax) && qm::hit_before(th, c, best_t, best_c)) {
                                        best_t = th; best_c = c; best_axis = ax;
                                    }
                                });
@@ -782,7 +838,7 @@ struct MoveHits {
     }
 };
 
-template <class S, bool CAPS>
+template <class S, int G>
 __global__ void __launch_bounds__(Q_THREADS) q_move(const __grid_constant__ Tree<S> t, const __grid_constant__ Movers<S> mb, const __grid_constant__ mv::Config<S> cfg,
                                                      S* __restrict__ out_pos, S* __restrict__ out_vel, int32_t* __restrict__ hc, S* __restrict__ hd,
                                                      S* __restrict__ ht, S* __restrict__ hp, S* __restrict__ hn) {
@@ -807,9 +863,9 @@ __global__ void __launch_bounds__(Q_THREADS) q_move(const __grid_constant__ Tree
         if (mb.poff)
             for (uint32_t k = mb.poff[i]; k < mb.poff[i + 1]; ++k)
                 init[ni++] = mv::plane_dir(mv::T3<S>{mb.planes[3 * k], mb.planes[3 * k + 1], mb.planes[3 * k + 2]});
-        const TreeScene<S, CAPS> sc{t, *t.m, mb.mask ? mb.mask[i] : 0xffffffffu, mb.xoff ? mb.xoff[i + 1] - mb.xoff[i] : 0u,
+        const TreeScene<S, G> sc{t, *t.m, mb.mask ? mb.mask[i] : 0xffffffffu, mb.xoff ? mb.xoff[i + 1] - mb.xoff[i] : 0u,
                               mb.xoff ? mb.xs + mb.xoff[i] : nullptr, mb.ignored};
-        mv::move_and_slide<CAPS>(sc, cfg, b, pos, vel, init, ni, hits);
+        mv::move_and_slide<G>(sc, cfg, b, pos, vel, init, ni, hits);
     }
     out_pos[3 * i] = pos.x; out_pos[3 * i + 1] = pos.y; out_pos[3 * i + 2] = pos.z;
     out_vel[3 * i] = vel.x; out_vel[3 * i + 1] = vel.y; out_vel[3 * i + 2] = vel.z;
@@ -822,15 +878,24 @@ class Queries final : public QueriesBase {
 
     AvnStatus update(const AvnQueryColliders* c, uint32_t flags) override {
         const bool keep_shapes = (flags & AVN_QUERY_SHAPES_UNCHANGED) != 0;
-        bool saw_capsule = false;
-        if (const char* why = qm::check_colliders(c, !keep_shapes, sizeof(S) == 8, true, &saw_capsule))
+        bool saw_capsule = false, saw_hull = false;
+        uint32_t max_hull = 0;
+        const uint32_t hc = hull_count();   // the kept column's check below reads it too
+        if (const char* why = qm::check_colliders(c, !keep_shapes, sizeof(S) == 8, true, &saw_capsule, &hc, &saw_hull, &max_hull))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: %s", why);
         if (keep_shapes && (!built_ || c->count != uint32_t(n_)))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: AVN_QUERY_SHAPES_UNCHANGED needs a previous update of the same count");
+        if (keep_shapes && hull_ && max_hull_ >= hc)   // the kept column's hulls against the current table
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_update: the kept shape column names convex hull %u, and the hull table holds %u", max_hull_, hc);
         const int n = int(c->count);
         built_ = false;
         n_ = n;
-        if (!keep_shapes) caps_ = saw_capsule;   // AVN_QUERY_SHAPES_UNCHANGED keeps the shape column, and with it whether it holds a capsule
+        if (!keep_shapes) {                      // AVN_QUERY_SHAPES_UNCHANGED keeps the shape column, and with it whether it holds a capsule or a hull
+            caps_ = saw_capsule;
+            hull_ = saw_hull;
+            max_hull_ = max_hull;
+        }
+        gen_ = hulls_ ? hulls_->generation : 0;  // the hull bounds below are built from this table
         const size_t nn = size_t(std::max(n, 1));
         AVN_CUDA(pos_.ensure(3 * nn * sizeof(S)));
         AVN_CUDA(rot_.ensure(4 * nn * sizeof(S)));
@@ -869,8 +934,9 @@ class Queries final : public QueriesBase {
         const Tree<S> t = tree();
         if (n > 0) {
             const unsigned g = unsigned((n + 255) / 256);
-            if (caps_) q_prepare<S, true><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
-            else q_prepare<S, false><<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
+            const int lv = level(false, false);
+            auto prepare = lv == 2 ? q_prepare<S, 2> : lv == 1 ? q_prepare<S, 1> : q_prepare<S, 0>;
+            prepare<<<g, 256, 0, stream_>>>(t, tmn_.as<S>(), tmx_.as<S>(), cbox_.as<NodeBox>(), centre_.as<float4>(), valid_.as<uint8_t>(), d_m, sb);
             q_codes<<<g, 256, 0, stream_>>>(n, centre_.as<float4>(), valid_.as<uint8_t>(), sb, k0_.as<uint32_t>(), v0_.as<uint32_t>());
             uint32_t *ka = k0_.as<uint32_t>(), *kb = k1_.as<uint32_t>(), *va = v0_.as<uint32_t>(), *vb = v1_.as<uint32_t>();
             for (int pass = 0; pass < 4; ++pass) {
@@ -907,8 +973,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
         AVN_CUDA(on_.ensure(3 * size_t(n) * sizeof(S)));
         const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
-        if (caps_) q_cast_ray<S, true><<<g, Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
-        else q_cast_ray<S, false><<<g, Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
+        const int lv = level(false, false);
+        auto cast = lv == 2 ? q_cast_ray<S, 2> : lv == 1 ? q_cast_ray<S, 1> : q_cast_ray<S, 0>;
+        cast<<<g, Q_THREADS, 0, stream_>>>(tree(), rays_, oc_.as<int32_t>(), ot_.as<S>(), on_.as<S>());
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
         AVN_CUDA(cudaMemcpyAsync(out->distance, ot_.p, size_t(n) * sizeof(S), cudaMemcpyDeviceToHost, stream_));
@@ -928,9 +995,10 @@ class Queries final : public QueriesBase {
         AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
         const Tree<S> t = tree();
         const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
+        const int lv = level(false, false);
         if (n > 0) {
-            if (caps_) q_ray_count<S, true><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
-            else q_ray_count<S, false><<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
+            auto count = lv == 2 ? q_ray_count<S, 2> : lv == 1 ? q_ray_count<S, 1> : q_ray_count<S, 0>;
+            count<<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_.as<uint32_t>(), kept_.as<uint32_t>());
         }
         uint64_t tot[2];
         if ((st = scan(full_.as<uint32_t>(), n, full_off_.as<uint64_t>())) != AVN_OK) return st;
@@ -948,7 +1016,7 @@ class Queries final : public QueriesBase {
         AVN_CUDA(ot_.ensure(nk * sizeof(S)));
         AVN_CUDA(on_.ensure(3 * nk * sizeof(S)));
         if (n > 0 && tot[1] > 0) {
-            auto emit = caps_ ? q_ray_emit<S, true> : q_ray_emit<S, false>;
+            auto emit = lv == 2 ? q_ray_emit<S, 2> : lv == 1 ? q_ray_emit<S, 1> : q_ray_emit<S, 0>;
             emit<<<g, Q_THREADS, 0, stream_>>>(t, rays_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
                                                oc_.as<uint32_t>(), ot_.as<S>(), on_.as<S>());
             AVN_CUDA(cudaGetLastError());
@@ -958,6 +1026,7 @@ class Queries final : public QueriesBase {
 
     AvnStatus aabb_intersections(uint32_t count, const void* mn, const void* mx, AvnHitList* out) override {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_aabb_intersections before any avn_query_update");
+        if (AvnStatus st = stale("avn_query_aabb_intersections")) return st;
         if (count && (!mn || !mx)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_query_aabb_intersections: min and max are required");
         AvnStatus st = list_out(out, "avn_query_aabb_intersections");
         if (st != AVN_OK) return st;
@@ -999,7 +1068,8 @@ class Queries final : public QueriesBase {
         AVN_CUDA(oc_.ensure(size_t(n) * 4));
         AVN_CUDA(ot_.ensure(size_t(n) * sizeof(S)));
         for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * size_t(n) * sizeof(S)));
-        auto cast = caps_ || shapes_caps_ ? q_cast_shape<S, true> : q_cast_shape<S, false>;
+        const int lv = level(shapes_caps_, shapes_hull_);
+        auto cast = lv == 2 ? q_cast_shape<S, 2> : lv == 1 ? q_cast_shape<S, 1> : q_cast_shape<S, 0>;
         cast<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), shapes_, oc_.as<int32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(),
                                                                                  on1_.as<S>(), on2_.as<S>());
         AVN_CUDA(cudaGetLastError());
@@ -1024,9 +1094,9 @@ class Queries final : public QueriesBase {
         AVN_CUDA(kept_off_.ensure(size_t(n + 1) * 8));
         const Tree<S> t = tree();
         const unsigned g = unsigned((n + Q_THREADS - 1) / Q_THREADS);
-        const bool caps = caps_ || shapes_caps_;
+        const int lv = level(shapes_caps_, shapes_hull_);
         if (n > 0) {
-            auto count = caps ? q_shape_count<S, true> : q_shape_count<S, false>;
+            auto count = lv == 2 ? q_shape_count<S, 2> : lv == 1 ? q_shape_count<S, 1> : q_shape_count<S, 0>;
             count<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_.as<uint32_t>(), kept_.as<uint32_t>());
         }
         uint64_t tot[2];
@@ -1045,7 +1115,7 @@ class Queries final : public QueriesBase {
         AVN_CUDA(ot_.ensure(nk * sizeof(S)));
         for (DevBuf* b : {&op1_, &op2_, &on1_, &on2_}) AVN_CUDA(b->ensure(3 * nk * sizeof(S)));
         if (n > 0 && tot[1] > 0) {
-            auto emit = caps ? q_shape_emit<S, true> : q_shape_emit<S, false>;
+            auto emit = lv == 2 ? q_shape_emit<S, 2> : lv == 1 ? q_shape_emit<S, 1> : q_shape_emit<S, 0>;
             emit<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, full_off_.as<uint64_t>(), kept_off_.as<uint64_t>(), tmp_t_.as<double>(), tmp_c_.as<uint32_t>(),
                                                oc_.as<uint32_t>(), ot_.as<S>(), op1_.as<S>(), op2_.as<S>(), on1_.as<S>(), on2_.as<S>());
             AVN_CUDA(cudaGetLastError());
@@ -1074,7 +1144,8 @@ class Queries final : public QueriesBase {
         AVN_CUDA(oc_.ensure(size_t(n) * 4));
         AVN_CUDA(op1_.ensure(3 * size_t(n) * sizeof(S)));
         AVN_CUDA(oin_.ensure(size_t(n)));
-        auto project = caps_ ? q_project_point<S, true> : q_project_point<S, false>;
+        const int lv = level(false, false);
+        auto project = lv == 2 ? q_project_point<S, 2> : lv == 1 ? q_project_point<S, 1> : q_project_point<S, 0>;
         project<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), points_, oc_.as<int32_t>(), op1_.as<S>(), oin_.as<uint8_t>());
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaMemcpyAsync(out->collider, oc_.p, size_t(n) * 4, cudaMemcpyDeviceToHost, stream_));
@@ -1089,9 +1160,12 @@ class Queries final : public QueriesBase {
         if (st != AVN_OK) return st;
         if ((st = list_out(out, "avn_query_point_intersections")) != AVN_OK) return st;
         const int n = int(p->count);
+        const int lv = level(false, false);
         return intersections(n, out, "avn_query_point_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
-            if (counts) (caps_ ? q_point_isect<S, false, true> : q_point_isect<S, false, false>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, counts, nullptr, nullptr);
-            else (caps_ ? q_point_isect<S, true, true> : q_point_isect<S, true, false>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, nullptr, off, oc);
+            if (counts)
+                (lv == 2 ? q_point_isect<S, false, 2> : lv == 1 ? q_point_isect<S, false, 1> : q_point_isect<S, false, 0>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, counts, nullptr, nullptr);
+            else
+                (lv == 2 ? q_point_isect<S, true, 2> : lv == 1 ? q_point_isect<S, true, 1> : q_point_isect<S, true, 0>)<<<g, Q_THREADS, 0, stream_>>>(t, points_, nullptr, off, oc);
         });
     }
 
@@ -1100,17 +1174,21 @@ class Queries final : public QueriesBase {
         if (st != AVN_OK) return st;
         if ((st = list_out(out, "avn_query_shape_intersections")) != AVN_OK) return st;
         const int n = int(s->count);
-        const bool caps = caps_ || shapes_caps_;
+        const int lv = level(shapes_caps_, shapes_hull_);
         return intersections(n, out, "avn_query_shape_intersections", [&](const Tree<S>& t, unsigned g, uint32_t* counts, const uint64_t* off, uint32_t* oc) {
-            if (counts) (caps ? q_shape_isect<S, false, true> : q_shape_isect<S, false, false>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, counts, nullptr, nullptr);
-            else (caps ? q_shape_isect<S, true, true> : q_shape_isect<S, true, false>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, nullptr, off, oc);
+            if (counts)
+                (lv == 2 ? q_shape_isect<S, false, 2> : lv == 1 ? q_shape_isect<S, false, 1> : q_shape_isect<S, false, 0>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, counts, nullptr, nullptr);
+            else
+                (lv == 2 ? q_shape_isect<S, true, 2> : lv == 1 ? q_shape_isect<S, true, 1> : q_shape_isect<S, true, 0>)<<<g, Q_THREADS, 0, stream_>>>(t, shapes_, nullptr, off, oc);
         });
     }
 
     AvnStatus move_and_slide(const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) override {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide before any avn_query_update");
-        bool batch_caps = false;
-        if (const char* why = mv::check_move(cfg, b, sizeof(S) == 8, uint32_t(n_), true, &batch_caps))
+        if (AvnStatus st = stale("avn_move_and_slide")) return st;
+        bool batch_caps = false, batch_hull = false;
+        const uint32_t hull_n = hull_count();
+        if (const char* why = mv::check_move(cfg, b, sizeof(S) == 8, uint32_t(n_), true, &batch_caps, &hull_n, &batch_hull))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: %s", why);
         if (!out || (b->count && (!out->position || !out->velocity)))
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_move_and_slide: position and velocity outputs are required");
@@ -1150,7 +1228,8 @@ class Queries final : public QueriesBase {
             AVN_CUDA(cudaEventCreate(&ev_[1]));
         }
         AVN_CUDA(cudaEventRecord(ev_[0], stream_));
-        auto move = caps_ || batch_caps ? q_move<S, true> : q_move<S, false>;
+        const int lv = level(batch_caps, batch_hull);
+        auto move = lv == 2 ? q_move<S, 2> : lv == 1 ? q_move<S, 1> : q_move<S, 0>;
         move<<<unsigned((n + Q_THREADS - 1) / Q_THREADS), Q_THREADS, 0, stream_>>>(tree(), mb, mv::config_of<S>(cfg), op1_.as<S>(), op2_.as<S>(), hc, hd, ht, hp, hn);
         AVN_CUDA(cudaGetLastError());
         AVN_CUDA(cudaEventRecord(ev_[1], stream_));
@@ -1165,6 +1244,8 @@ class Queries final : public QueriesBase {
         AVN_CUDA(cudaEventElapsedTime(&out->kernel_ms, ev_[0], ev_[1]));
         return AVN_OK;
     }
+
+    void attach_hulls(const HullTable* hulls) override { hulls_ = hulls; }
 
     ~Queries() override {
         for (cudaEvent_t e : ev_)
@@ -1201,7 +1282,10 @@ class Queries final : public QueriesBase {
     // validate on the host, then upload the shape columns into shapes_ (cast: the cast-only columns too)
     AvnStatus shapes_in(const AvnShapeBatch* s, bool cast, const char* what) {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
-        if (const char* why = qm::check_shapes(s, cast, sizeof(S) == 8, true, &shapes_caps_)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
+        if (AvnStatus st = stale(what)) return st;
+        const uint32_t hc = hull_count();
+        if (const char* why = qm::check_shapes(s, cast, sizeof(S) == 8, true, &shapes_caps_, &hc, &shapes_hull_))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
         const size_t n = s->count;
         shapes_ = Shapes<S>{};
         shapes_.n = int(n);
@@ -1226,6 +1310,7 @@ class Queries final : public QueriesBase {
     }
     AvnStatus points_in(const AvnPointBatch* p, const char* what) {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
+        if (AvnStatus st = stale(what)) return st;
         if (const char* why = qm::check_points(p)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
         const size_t n = p->count;
         points_ = Points<S>{};
@@ -1250,12 +1335,23 @@ class Queries final : public QueriesBase {
         t.memb = has_memb_ ? memb_.as<uint32_t>() : nullptr;
         t.tmn = tmn_.as<S>(); t.tmx = tmx_.as<S>();
         t.nodes = nodes_.as<NodeBox>(); t.child = child_.as<int2>(); t.leaf = v0_.as<uint32_t>();
+        t.hulls = hulls_ && hulls_->set ? hulls_->dev : hm::Table{};
         return t;
+    }
+    uint32_t hull_count() const { return hulls_ ? hulls_->count() : 0u; }
+    // the instance that covers the tree and the batch: 2 with a hull, 1 with a capsule, else 0
+    int level(bool batch_caps, bool batch_hull) const { return hull_ || batch_hull ? 2 : (caps_ || batch_caps ? 1 : 0); }
+    // a tree holding a hull was bounded with the table of its update: refused once avn_set_convex_hulls has replaced that table
+    AvnStatus stale(const char* what) {
+        if (hull_ && (!hulls_ || hulls_->generation != gen_))
+            return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: the convex hull table was replaced after the avn_query_update whose tree holds a hull: update again", what);
+        return AVN_OK;
     }
 
     // validate on the host, then upload the ray columns into rays_
     AvnStatus rays_in(const AvnRayBatch* r, const char* what) {
         if (!built_) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s before any avn_query_update", what);
+        if (AvnStatus st = stale(what)) return st;
         if (const char* why = qm::check_rays(r)) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: %s", what, why);
         if (r->count >= 0x7fffffffu) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "%s: too many rays", what);
         const size_t n = r->count;
@@ -1318,6 +1414,11 @@ class Queries final : public QueriesBase {
     bool built_ = false, has_memb_ = false;
     bool caps_ = false;                              // the tree's shape column holds a capsule
     bool shapes_caps_ = false;                       // the last shape batch holds a capsule
+    bool hull_ = false;                              // the tree's shape column holds a convex hull
+    bool shapes_hull_ = false;                       // the last shape batch holds a convex hull
+    uint32_t max_hull_ = 0;                          // the largest hull index of the tree's shape column
+    uint64_t gen_ = 0;                               // the hull table generation the tree was built with
+    const HullTable* hulls_ = nullptr;               // the context's table (attach_hulls)
     int n_ = 0;
     Rays<S> rays_{};
     Shapes<S> shapes_{};

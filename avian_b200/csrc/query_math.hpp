@@ -878,6 +878,7 @@ NM_HD inline S point_box_d2(const float* lo, const float* hi, V3 p) {
 
 // ---- host-side validation shared by the ABI (before any upload) and the host fixture --------------------------------------------------
 #include "../../include/avian_b200.h"
+#include "shape_column.hpp"
 namespace qm {
 // NULL when the batch is usable; the reason otherwise
 inline const char* check_rays(const AvnRayBatch* r) {
@@ -894,9 +895,14 @@ inline const char* check_rays(const AvnRayBatch* r) {
 }
 // the dims a shape reads: a cuboid's three half extents, a sphere's radius, a capsule's radius and half length
 inline int shape_dims_read(uint8_t shape) { return shape == AVN_SHAPE_SPHERE ? 1 : (shape == AVN_SHAPE_CAPSULE ? 2 : 3); }
-// capsules: whether AVN_SHAPE_CAPSULE is accepted; saw_capsule (optional): set when the column holds one
-inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_required, bool f64, bool capsules = false, bool* saw_capsule = nullptr) {
+// capsules: whether AVN_SHAPE_CAPSULE is accepted; saw_capsule (optional): set when the column holds one.  hull_count (the hull instances'
+// callers): AVN_SHAPE_CONVEX_HULL is accepted too, its index checked by avn::check_shape_column against *hull_count (0: no table);
+// saw_hull / max_hull (optional): whether the column holds a hull, and the largest index it names.
+inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_required, bool f64, bool capsules = false, bool* saw_capsule = nullptr,
+                                   const uint32_t* hull_count = nullptr, bool* saw_hull = nullptr, uint32_t* max_hull = nullptr) {
     if (saw_capsule) *saw_capsule = false;
+    if (saw_hull) *saw_hull = false;
+    if (max_hull) *max_hull = 0;
     if (!c) return "colliders are required";
     if (c->count >= 0x80000000u) return "colliders: at most 2^31 - 1";
     if (c->count == 0) return nullptr;
@@ -904,6 +910,7 @@ inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_requi
     if (shapes_required) {
         if (!c->shape || !c->dims) return "colliders: shape and dims are required";
         for (uint32_t i = 0; i < c->count; ++i) {
+            if (hull_count && c->shape[i] == AVN_SHAPE_CONVEX_HULL) continue;   // its index: below
             if (!capsules && c->shape[i] > AVN_SHAPE_SPHERE) return "colliders: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
             if (c->shape[i] > AVN_SHAPE_CAPSULE) return "colliders: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
             for (int k = 0; k < shape_dims_read(c->shape[i]); ++k) {
@@ -912,6 +919,10 @@ inline const char* check_colliders(const AvnQueryColliders* c, bool shapes_requi
             }
             if (saw_capsule && c->shape[i] == AVN_SHAPE_CAPSULE) *saw_capsule = true;
         }
+        size_t at;
+        if (hull_count)
+            if (const char* why = avn::check_shape_column(c->shape, c->dims, c->count, f64 ? 64 : 32, &at, nullptr, hull_count, saw_hull, max_hull))
+                return why;
     }
     return nullptr;
 }
@@ -924,18 +935,21 @@ inline const char* check_exclusions(uint32_t count, uint32_t exclude_count, cons
     if (offsets[count] > exclude_count) return "exclude_offsets run past exclude_count";
     return nullptr;
 }
-// cast: the batch feeds a shape cast (direction and max_distance required, target_distance must be 0)
-inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64, bool capsules = false, bool* saw_capsule = nullptr) {
+// cast: the batch feeds a shape cast (direction and max_distance required, target_distance must be 0); hull_count / saw_hull: as check_colliders
+inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64, bool capsules = false, bool* saw_capsule = nullptr,
+                                const uint32_t* hull_count = nullptr, bool* saw_hull = nullptr) {
     if (saw_capsule) *saw_capsule = false;
+    if (saw_hull) *saw_hull = false;
     if (!s) return "shape batch is required";
     if (s->count >= 0x7fffffffu) return "shapes: too many shapes";
     if (s->count == 0) return nullptr;
     if (!s->shape || !s->dims || !s->position || !s->rotation) return "shapes: shape, dims, position and rotation are required";
     if (cast && (!s->direction || !s->max_distance)) return "shapes: direction and max_distance are required for a cast";
     for (uint32_t i = 0; i < s->count; ++i) {
-        if (!capsules && s->shape[i] > AVN_SHAPE_SPHERE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
-        if (s->shape[i] > AVN_SHAPE_CAPSULE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
-        for (int k = 0; k < shape_dims_read(s->shape[i]); ++k) {
+        const bool hull = hull_count && s->shape[i] == AVN_SHAPE_CONVEX_HULL;   // its index: below
+        if (!hull && !capsules && s->shape[i] > AVN_SHAPE_SPHERE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID and AVN_SHAPE_SPHERE)";
+        if (!hull && s->shape[i] > AVN_SHAPE_CAPSULE) return "shapes: unknown shape (only AVN_SHAPE_CUBOID, AVN_SHAPE_SPHERE and AVN_SHAPE_CAPSULE)";
+        for (int k = 0; !hull && k < shape_dims_read(s->shape[i]); ++k) {
             const double v = f64 ? static_cast<const double*>(s->dims)[3 * size_t(i) + k] : static_cast<const float*>(s->dims)[3 * size_t(i) + k];
             if (v < 0) return "shapes: negative half extent, radius or half length";
         }
@@ -945,6 +959,9 @@ inline const char* check_shapes(const AvnShapeBatch* s, bool cast, bool f64, boo
             if (td != 0) return "shapes: target_distance must be 0 (a cast with a target distance is not supported)";
         }
     }
+    size_t at;
+    if (hull_count)
+        if (const char* why = avn::check_shape_column(s->shape, s->dims, s->count, f64 ? 64 : 32, &at, nullptr, hull_count, saw_hull)) return why;
     if (const char* why = check_exclusions(s->count, s->exclude_count, s->exclude_offsets, s->exclude)) return why;
     return nullptr;
 }

@@ -87,10 +87,17 @@ def _load():
             f.restype = C.c_int
         lib.avh_move_and_slide.argtypes = [C.c_uint32, P(api.AvnQueryColliders), P(api.AvnMoveConfig), P(api.AvnMoveBatch), P(api.AvnMoveResult)]
         lib.avh_move_and_slide.restype = C.c_int
+        for name in ("query_cast_ray", "query_ray_hits", "query_aabb_intersections", "query_cast_shape", "query_shape_hits", "query_project_point",
+                     "query_point_intersections", "query_shape_intersections", "move_and_slide"):   # the same with the hull table
+            f = getattr(lib, f"avh_{name}_hulls")
+            f.argtypes = getattr(lib, f"avh_{name}").argtypes + [_vp]
+            f.restype = C.c_int
         lib.avh_move_project_velocity.argtypes = [C.c_uint32, _vp, _vp, C.c_uint32, _vp]
         lib.avh_move_project_velocity.restype = None
         lib.avh_move_contact.argtypes = [C.c_uint32, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_double, _vp, _vp]
         lib.avh_move_contact.restype = C.c_int
+        lib.avh_move_contact_hulls.argtypes = lib.avh_move_contact.argtypes + [_vp]
+        lib.avh_move_contact_hulls.restype = C.c_int
         lib.avh_ccd_solve.argtypes = [C.c_uint32, C.c_double, C.c_double, C.c_uint32] + [_vp] * 10 + [C.c_uint32] + [_vp] * 5 + [P(api.AvnCcdConfig)] + [_vp] * 5
         lib.avh_ccd_solve.restype = C.c_int
         lib.avh_ccd_pair_toi.argtypes = [C.c_uint32, C.c_int, _vp, _vp, C.c_double, C.c_double, C.c_double]
@@ -199,131 +206,148 @@ def raw_manifolds(scalar, dt: float, contact_tolerance: float, pairs, colliders:
     return out
 
 
-# ---- spatial queries by brute force over every collider (csrc/query_math.hpp): what the device tree must reproduce bit for bit.
-# capsules=True accepts capsule colliders and query shapes (characters for move_and_slide); without it a capsule is refused as an unknown
-# shape.  The device accepts capsules with no flag.
+# ---- spatial queries by brute force over every collider (csrc/query_math.hpp, csrc/hull_query_math.hpp): what the device tree must reproduce
+# bit for bit.  capsules=True accepts capsule colliders and query shapes (characters for move_and_slide); without it a capsule is refused as an
+# unknown shape.  hulls=<HullTable or api.ConvexHulls> accepts convex hulls that index it, and capsules with them; without it a hull is
+# refused as an unknown shape.  The device accepts capsules with no flag, and hulls with the context's table.
 def _query_check(lib, st: int) -> None:
     if st != api.OK:
         raise api.AvianError(st, lib.avh_query_error().decode())
 
 
 CAPSULE_BIT = 0x100   # OR-ed into scalar_bits: the brute force accepts capsule colliders, query shapes and characters
+HULL_BIT = 0x200      # OR-ed into scalar_bits: convex hulls too, with the table of the avh_*_hulls entry points
 
 
-def _bits(dt, capsules: bool) -> int:
-    return (32 if dt == np.float32 else 64) | (CAPSULE_BIT if capsules else 0)
+def _bits(dt, capsules: bool, hulls=None) -> int:
+    return (32 if dt == np.float32 else 64) | (CAPSULE_BIT if capsules else 0) | (HULL_BIT if hulls is not None else 0)
 
 
-def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False) -> dict:
+def _call(lib, name: str, dt, capsules: bool, hulls, *args) -> int:
+    """avh_<name>, or avh_<name>_hulls with the table when hulls is given"""
+    if hulls is None:
+        return getattr(lib, f"avh_{name}")(_bits(dt, capsules), *args)
+    return getattr(lib, f"avh_{name}_hulls")(_bits(dt, capsules, hulls), *args, hulls.h)
+
+
+def query_cast_ray(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False, hulls=None) -> dict:
     """The closest hit of every ray (same output as Context.cast_ray)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     r, keep_r = rays.as_struct(dt)
     n = rays.count
     out = {"collider": np.zeros(n, dtype=np.int32), "distance": np.zeros(n, dtype=dt), "normal": np.zeros((n, 3), dtype=dt)}
     o = api.AvnRayClosest(*(_p(out[k]) for k in ("collider", "distance", "normal")))
-    _query_check(lib, lib.avh_query_cast_ray(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(o)))
+    _query_check(lib, _call(lib, "query_cast_ray", dt, capsules, hulls, C.byref(c), C.byref(r), C.byref(o)))
     return out
 
 
-def query_ray_hits(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False) -> dict:
+def query_ray_hits(scalar, colliders: "api.QueryColliders", rays: "api.Rays", capsules: bool = False, hulls=None) -> dict:
     """Every ray's max_hits nearest hits in (t, collider) order as CSR (same output as Context.ray_hits)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     r, keep_r = rays.as_struct(dt)
     h, out = api.hit_list(rays.count, 0, dt, True)
-    st = lib.avh_query_ray_hits(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(h))
+    st = _call(lib, "query_ray_hits", dt, capsules, hulls, C.byref(c), C.byref(r), C.byref(h))
     if st == api.ERR_CAPACITY:
         h, out = api.hit_list(rays.count, int(h.count), dt, True)
-        st = lib.avh_query_ray_hits(_bits(dt, capsules), C.byref(c), C.byref(r), C.byref(h))
+        st = _call(lib, "query_ray_hits", dt, capsules, hulls, C.byref(c), C.byref(r), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
 
 
-def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, aabb_max, capsules: bool = False) -> dict:
+def query_aabb_intersections(scalar, colliders: "api.QueryColliders", aabb_min, aabb_max, capsules: bool = False, hulls=None) -> dict:
     """Per query box the colliders whose tight AABB it touches, ascending (same output as Context.aabb_intersections)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     mn = np.ascontiguousarray(aabb_min, dtype=dt).reshape(-1, 3)
     mx = np.ascontiguousarray(aabb_max, dtype=dt).reshape(-1, 3)
-    n, bits = int(mn.shape[0]), _bits(dt, capsules)
+    n = int(mn.shape[0])
     h, out = api.hit_list(n, 0, dt, False)
-    st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
+    st = _call(lib, "query_aabb_intersections", dt, capsules, hulls, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
     if st == api.ERR_CAPACITY:
         h, out = api.hit_list(n, int(h.count), dt, False)
-        st = lib.avh_query_aabb_intersections(bits, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
+        st = _call(lib, "query_aabb_intersections", dt, capsules, hulls, C.byref(c), n, _p(mn), _p(mx), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
 
 
-def query_cast_shape(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
+def query_cast_shape(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False, hulls=None) -> dict:
     """The closest hit of every cast (same output as Context.cast_shape)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     s, keep_s = shapes.as_struct(dt)
     o, out = api.shape_closest(shapes.count, dt)
-    _query_check(lib, lib.avh_query_cast_shape(_bits(dt, capsules), C.byref(c), C.byref(s), C.byref(o)))
+    _query_check(lib, _call(lib, "query_cast_shape", dt, capsules, hulls, C.byref(c), C.byref(s), C.byref(o)))
     return out
 
 
-def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
+def query_shape_hits(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False, hulls=None) -> dict:
     """Every cast's max_hits nearest hits in (t, collider) order as CSR (same output as Context.shape_hits)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     s, keep_s = shapes.as_struct(dt)
-    bits = _bits(dt, capsules)
     h, out = api.shape_hit_list(shapes.count, 0, dt)
-    st = lib.avh_query_shape_hits(bits, C.byref(c), C.byref(s), C.byref(h))
+    st = _call(lib, "query_shape_hits", dt, capsules, hulls, C.byref(c), C.byref(s), C.byref(h))
     if st == api.ERR_CAPACITY:
         h, out = api.shape_hit_list(shapes.count, int(h.count), dt)
-        st = lib.avh_query_shape_hits(bits, C.byref(c), C.byref(s), C.byref(h))
+        st = _call(lib, "query_shape_hits", dt, capsules, hulls, C.byref(c), C.byref(s), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
 
 
-def query_project_point(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False) -> dict:
+def query_project_point(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False, hulls=None) -> dict:
     """The closest collider of every point and the projection onto it (same output as Context.project_point)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     p, keep_p = points.as_struct(dt)
     o, out = api.point_projection(points.count, dt)
-    _query_check(lib, lib.avh_query_project_point(_bits(dt, capsules), C.byref(c), C.byref(p), C.byref(o)))
+    _query_check(lib, _call(lib, "query_project_point", dt, capsules, hulls, C.byref(c), C.byref(p), C.byref(o)))
     return out
 
 
-def _query_list(fn, scalar, colliders, batch, capsules: bool) -> dict:
+def _query_list(fn, scalar, colliders, batch, capsules: bool, hulls=None) -> dict:
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     b, keep_b = batch.as_struct(dt)
-    bits, n = _bits(dt, capsules), batch.count
+    n = batch.count
     h, out = api.hit_list(n, 0, dt, False)
-    st = getattr(lib, fn)(bits, C.byref(c), C.byref(b), C.byref(h))
+    st = _call(lib, fn, dt, capsules, hulls, C.byref(c), C.byref(b), C.byref(h))
     if st == api.ERR_CAPACITY:
         h, out = api.hit_list(n, int(h.count), dt, False)
-        st = getattr(lib, fn)(bits, C.byref(c), C.byref(b), C.byref(h))
+        st = _call(lib, fn, dt, capsules, hulls, C.byref(c), C.byref(b), C.byref(h))
     _query_check(lib, st)
     return api.hit_list_result(h, out)
 
 
-def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False) -> dict:
+def query_point_intersections(scalar, colliders: "api.QueryColliders", points: "api.Points", capsules: bool = False, hulls=None) -> dict:
     """Per point the colliders containing it, ascending (same output as Context.point_intersections)."""
-    return _query_list("avh_query_point_intersections", scalar, colliders, points, capsules)
+    return _query_list("query_point_intersections", scalar, colliders, points, capsules, hulls)
 
 
-def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False) -> dict:
+def query_shape_intersections(scalar, colliders: "api.QueryColliders", shapes: "api.ShapeQueries", capsules: bool = False, hulls=None) -> dict:
     """Per query shape the colliders it intersects, ascending (same output as Context.shape_intersections)."""
-    return _query_list("avh_query_shape_intersections", scalar, colliders, shapes, capsules)
+    return _query_list("query_shape_intersections", scalar, colliders, shapes, capsules, hulls)
 
 
 # ---- move and slide by brute force over every collider (csrc/move_math.hpp): what the device kernel must reproduce bit for bit
-def move_and_slide(scalar, colliders: "api.QueryColliders", config: "api.MoveConfig", batch: "api.MoveBatch", capsules: bool = False) -> dict:
+def move_and_slide(scalar, colliders: "api.QueryColliders", config: "api.MoveConfig", batch: "api.MoveBatch", capsules: bool = False,
+                   hulls=None) -> dict:
     """MoveAndSlide::move_and_slide for every character (same output as Context.move_and_slide; kernel_ms is 0)."""
     lib, dt = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt, hulls)
     c, keep_c = colliders.as_struct(dt)
     m, keep_m = config.as_struct()
     b, keep_b = batch.as_struct(dt)
     o, out = api.move_result(batch.count, config.move_and_slide_iterations, dt)
-    _query_check(lib, lib.avh_move_and_slide(_bits(dt, capsules), C.byref(c), C.byref(m), C.byref(b), C.byref(o)))
+    _query_check(lib, _call(lib, "move_and_slide", dt, capsules, hulls, C.byref(c), C.byref(m), C.byref(b), C.byref(o)))
     out["kernel_ms"] = 0.0
     return out
 
@@ -338,14 +362,20 @@ def project_velocity(scalar, v, normals) -> np.ndarray:
     return out
 
 
-def move_contact(scalar, shape_a: int, dims_a, pos_a, rot_a, shape_b: int, dims_b, pos_b, rot_b, prediction: float):
-    """One intersection of a move: (f32 plane normal, deepest penetration) of character a against collider b, or None."""
+def move_contact(scalar, shape_a: int, dims_a, pos_a, rot_a, shape_b: int, dims_b, pos_b, rot_b, prediction: float, hulls=None):
+    """One intersection of a move: (f32 plane normal, deepest penetration) of character a against collider b, or None.  hulls: the table
+    that hull shapes index (the hull instance's contact planes)."""
     lib = _load()
     d = lambda a, k: np.ascontiguousarray(a, dtype=np.float64).reshape(k)
     cols = [d(dims_a, 3), d(pos_a, 3), d(rot_a, 4), d(dims_b, 3), d(pos_b, 3), d(rot_b, 4)]
     n, pen = np.zeros(3, dtype=np.float32), np.zeros(1, dtype=np.float64)
-    hit = lib.avh_move_contact(32 if np.dtype(scalar) == np.float32 else 64, int(shape_a), _p(cols[0]), _p(cols[1]), _p(cols[2]), int(shape_b),
-                               _p(cols[3]), _p(cols[4]), _p(cols[5]), float(prediction), _p(n), _p(pen))
+    args = (32 if np.dtype(scalar) == np.float32 else 64, int(shape_a), _p(cols[0]), _p(cols[1]), _p(cols[2]), int(shape_b),
+            _p(cols[3]), _p(cols[4]), _p(cols[5]), float(prediction), _p(n), _p(pen))
+    if hulls is None:
+        hit = lib.avh_move_contact(*args)
+    else:
+        table = _hull_table(np.dtype(scalar), hulls)   # held for the call: the table is freed with it
+        hit = lib.avh_move_contact_hulls(*args, table.h)
     return (n, float(pen[0])) if hit else None
 
 

@@ -24,6 +24,7 @@
 #include "../../include/avian_b200.h"
 #include "../csrc/narrow_math.hpp"
 #include "../csrc/hull_math.hpp"
+#include "../csrc/hull_query_math.hpp"
 #include "../csrc/contact_rows.hpp"
 #include "../csrc/query_math.hpp"
 #include "../csrc/ccd_math.hpp"
@@ -819,12 +820,21 @@ uint32_t avh_pair_count(AvhPipeline* h) { return uint32_t(reinterpret_cast<Pipel
 // ---- spatial queries, brute force over every collider (the checker of csrc/queries.cu; same header, same conventions) ----------------
 // Arguments are the ABI structs of avn_query_*; the colliders are passed with every call.  Returns an AvnStatus; avh_query_error() says why.
 // scalar_bits: 32 or 64 selects the column type; OR-ed with AVH_CAPSULES (0x100) it also accepts capsule colliders, query shapes and
-// characters.  Without that bit a capsule is refused as an unknown shape, as it was before capsules were queried.  The geometry is always
-// the CAPS = true instance of csrc/query_math.hpp, which gives the CAPS = false bits on cuboids and spheres.
+// characters.  Without that bit a capsule is refused as an unknown shape, as it was before capsules were queried.  OR-ed with AVH_HULLS
+// (0x200) it accepts capsules and convex hulls, whose indices the hull table of the avh_*_hulls variants (avh_hulls_create) must hold;
+// without it a hull is refused as an unknown shape.  The geometry is always csrc/hull_query_math.hpp's, which gives the CAPS = true bits of
+// csrc/query_math.hpp on cuboids, spheres and capsules, and those give the CAPS = false bits on cuboids and spheres.
 namespace {
-constexpr uint32_t AVH_CAPSULES = 0x100u;
+constexpr uint32_t AVH_CAPSULES = 0x100u, AVH_HULLS = 0x200u;
 bool bits_f64(uint32_t scalar_bits) { return (scalar_bits & 0xffu) == 64; }
-bool bits_caps(uint32_t scalar_bits) { return (scalar_bits & AVH_CAPSULES) != 0; }
+bool bits_hulls(uint32_t scalar_bits) { return (scalar_bits & AVH_HULLS) != 0; }
+bool bits_caps(uint32_t scalar_bits) { return (scalar_bits & (AVH_CAPSULES | AVH_HULLS)) != 0; }
+uint32_t hull_count(const hm::HullSet* h) { return h ? uint32_t(h->radius.size()) : 0u; }
+// the collider column check of the brute force: capsules with AVH_CAPSULES, hulls too with AVH_HULLS
+const char* check_query_colliders(uint32_t bits, const AvnQueryColliders* c, const hm::HullSet* h) {
+    const uint32_t hc = hull_count(h);
+    return qm::check_colliders(c, true, bits_f64(bits), bits_caps(bits), nullptr, bits_hulls(bits) ? &hc : nullptr);
+}
 thread_local char g_query_error[256];
 int query_fail(AvnStatus st, const char* why) {
     snprintf(g_query_error, sizeof g_query_error, "%s", why);
@@ -834,7 +844,9 @@ int query_fail(AvnStatus st, const char* why) {
 struct QueryScene {
     const AvnQueryColliders* c; bool f64;
     Col dims, pos, rot;
-    QueryScene(const AvnQueryColliders* cc, bool f) : c(cc), f64(f), dims{cc->dims, f}, pos{cc->position, f}, rot{cc->rotation, f} {}
+    hm::Table t;   // the hull table (count 0: none; the checks refuse a hull without one)
+    QueryScene(const AvnQueryColliders* cc, bool f, const hm::HullSet* h = nullptr)
+        : c(cc), f64(f), dims{cc->dims, f}, pos{cc->position, f}, rot{cc->rotation, f}, t(h ? hm::view(*h) : hm::Table{}) {}
     bool valid(uint32_t i) const { return qm::collider_valid(dims.v3(i), pos.v3(i), rot.q(i)); }
     uint32_t memb(uint32_t i) const { return c->memberships ? c->memberships[i] : 1u; }
 };
@@ -860,7 +872,7 @@ void all_hits(const QueryScene& sc, const RayView& v, std::vector<RayHit>& out) 
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
         RayHit h{0, c, V3{0, 0, 0}};
-        if (qm::ray_collider<true>(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), v.o, v.d, v.maxd, v.solid, h.t, h.n)) out.push_back(h);
+        if (qh::ray_collider(sc.t, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), v.o, v.d, v.maxd, v.solid, h.t, h.n)) out.push_back(h);
     }
     std::sort(out.begin(), out.end(), [](const RayHit& a, const RayHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
 }
@@ -869,30 +881,25 @@ void query_aabbs(const QueryScene& sc, uint32_t n, const T* mn, const T* mx, std
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c)) continue;
         V3 a, b;
-        qm::collider_aabb<true>(sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), a, b);
+        qh::collider_aabb(sc.t, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), a, b);
         const T tmn[3] = {T(a.x), T(a.y), T(a.z)}, tmx[3] = {T(b.x), T(b.y), T(b.z)};
         for (uint32_t i = 0; i < n; ++i)
             if (qm::aabb_overlap(mn + 3 * size_t(i), mx + 3 * size_t(i), tmn, tmx)) per[i].push_back(c);
     }
 }
 
-int query_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r) {
-    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+int query_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, const hm::HullSet* h) {
+    if (const char* why = check_query_colliders(scalar_bits, c, h)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     if (r)
         if (const char* why = qm::check_rays(r)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
 }
-}  // namespace
 
-extern "C" {
-
-const char* avh_query_error() { return g_query_error; }
-
-int avh_query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out) {
-    if (int st = query_inputs(scalar_bits, c, r)) return st;
+int query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out, const hm::HullSet* hs) {
+    if (int st = query_inputs(scalar_bits, c, r, hs)) return st;
     if (!out || (r->count && (!out->collider || !out->distance || !out->normal))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     ColW ot{out->distance, f64}, on{out->normal, f64};
     std::vector<RayHit> hits;
     for (uint32_t i = 0; i < r->count; ++i) {
@@ -904,11 +911,11 @@ int avh_query_cast_ray(uint32_t scalar_bits, const AvnQueryColliders* c, const A
     return AVN_OK;
 }
 
-int avh_query_ray_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out) {
-    if (int st = query_inputs(scalar_bits, c, r)) return st;
+int query_ray_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out, const hm::HullSet* hs) {
+    if (int st = query_inputs(scalar_bits, c, r, hs)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     std::vector<std::vector<RayHit>> per(r->count);
     uint64_t total = 0;
     for (uint32_t i = 0; i < r->count; ++i) {
@@ -934,11 +941,12 @@ int avh_query_ray_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const A
     return AVN_OK;
 }
 
-int avh_query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, uint32_t n, const void* mn, const void* mx, AvnHitList* out) {
-    if (int st = query_inputs(scalar_bits, c, nullptr)) return st;
+int query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, uint32_t n, const void* mn, const void* mx, AvnHitList* out,
+                             const hm::HullSet* hs) {
+    if (int st = query_inputs(scalar_bits, c, nullptr, hs)) return st;
     if (n && (!mn || !mx)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "min and max are required");
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
-    const QueryScene sc(c, bits_f64(scalar_bits));
+    const QueryScene sc(c, bits_f64(scalar_bits), hs);
     std::vector<std::vector<uint32_t>> per(n);
     if (bits_f64(scalar_bits)) query_aabbs(sc, n, static_cast<const double*>(mn), static_cast<const double*>(mx), per);
     else query_aabbs(sc, n, static_cast<const float*>(mn), static_cast<const float*>(mx), per);
@@ -953,6 +961,28 @@ int avh_query_aabb_intersections(uint32_t scalar_bits, const AvnQueryColliders* 
     }
     out->offsets[n] = k;
     return AVN_OK;
+}
+}  // namespace
+
+// The brute force's entry points: avh_query_* as before, and avh_query_*_hulls with the fixture's hull table (avh_hulls_create, or NULL) as
+// the trailing argument, which AVH_HULLS in scalar_bits enables.  Callers that pass the old argument lists keep reading the same functions.
+extern "C" {
+
+const char* avh_query_error() { return g_query_error; }
+
+int avh_query_cast_ray(uint32_t bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out) { return query_cast_ray(bits, c, r, out, nullptr); }
+int avh_query_cast_ray_hulls(uint32_t bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnRayClosest* out, const void* h) {
+    return query_cast_ray(bits, c, r, out, static_cast<const hm::HullSet*>(h));
+}
+int avh_query_ray_hits(uint32_t bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out) { return query_ray_hits(bits, c, r, out, nullptr); }
+int avh_query_ray_hits_hulls(uint32_t bits, const AvnQueryColliders* c, const AvnRayBatch* r, AvnHitList* out, const void* h) {
+    return query_ray_hits(bits, c, r, out, static_cast<const hm::HullSet*>(h));
+}
+int avh_query_aabb_intersections(uint32_t bits, const AvnQueryColliders* c, uint32_t n, const void* mn, const void* mx, AvnHitList* out) {
+    return query_aabb_intersections(bits, c, n, mn, mx, out, nullptr);
+}
+int avh_query_aabb_intersections_hulls(uint32_t bits, const AvnQueryColliders* c, uint32_t n, const void* mn, const void* mx, AvnHitList* out, const void* h) {
+    return query_aabb_intersections(bits, c, n, mn, mx, out, static_cast<const hm::HullSet*>(h));
 }
 
 }  // extern "C"
@@ -984,23 +1014,25 @@ void all_cast_hits(const QueryScene& sc, const ShapeView& v, std::vector<CastHit
     for (uint32_t c = 0; c < sc.c->count; ++c) {
         if (!sc.valid(c) || !qm::passes_filter(sc.memb(c), v.mask, v.xs, v.nx, c)) continue;
         CastHit h{0, c, -1};
-        if (qm::cast_collider<true>(v.shape, v.he, v.c, v.q, v.d, v.maxd, v.flags, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), h.t, h.axis))
+        if (qh::cast_collider(sc.t, v.shape, v.he, v.c, v.q, v.d, v.maxd, v.flags, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), h.t, h.axis))
             out.push_back(h);
     }
     std::sort(out.begin(), out.end(), [](const CastHit& a, const CastHit& b) { return qm::hit_before(a.t, a.c, b.t, b.c); });
 }
 qm::ShapeContact cast_contact_of(const QueryScene& sc, const ShapeView& v, const CastHit& h) {
     qm::ShapeContact k;
-    qm::cast_output<true>(v.shape, v.he, v.c, v.q, v.d, v.flags, sc.c->shape[h.c], sc.dims.v3(h.c), sc.pos.v3(h.c), sc.rot.q(h.c), h.t, h.axis, k);
+    qh::cast_output(sc.t, v.shape, v.he, v.c, v.q, v.d, v.flags, sc.c->shape[h.c], sc.dims.v3(h.c), sc.pos.v3(h.c), sc.rot.q(h.c), h.t, h.axis, k);
     return k;
 }
-int shape_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, bool cast) {
-    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
-    if (const char* why = qm::check_shapes(s, cast, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+int shape_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, bool cast, const hm::HullSet* h) {
+    if (const char* why = check_query_colliders(scalar_bits, c, h)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    const uint32_t hc = hull_count(h);
+    if (const char* why = qm::check_shapes(s, cast, bits_f64(scalar_bits), bits_caps(scalar_bits), nullptr, bits_hulls(scalar_bits) ? &hc : nullptr))
+        return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
 }
-int point_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p) {
-    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+int point_inputs(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, const hm::HullSet* h) {
+    if (const char* why = check_query_colliders(scalar_bits, c, h)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     if (const char* why = qm::check_points(p)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
     return AVN_OK;
 }
@@ -1017,16 +1049,13 @@ int write_list(AvnHitList* out, const std::vector<std::vector<uint32_t>>& per) {
     out->offsets[per.size()] = k;
     return AVN_OK;
 }
-}  // namespace
 
-extern "C" {
-
-int avh_query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeClosest* out) {
-    if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
+int query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeClosest* out, const hm::HullSet* hs) {
+    if (int st = shape_inputs(scalar_bits, c, s, true, hs)) return st;
     if (!out || (s->count && (!out->collider || !out->distance || !out->point1 || !out->point2 || !out->normal1 || !out->normal2)))
         return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     ColW ot{out->distance, f64}, p1{out->point1, f64}, p2{out->point2, f64}, n1{out->normal1, f64}, n2{out->normal2, f64};
     std::vector<CastHit> hits;
     for (uint32_t i = 0; i < s->count; ++i) {
@@ -1041,11 +1070,11 @@ int avh_query_cast_shape(uint32_t scalar_bits, const AvnQueryColliders* c, const
     return AVN_OK;
 }
 
-int avh_query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeHitList* out) {
-    if (int st = shape_inputs(scalar_bits, c, s, true)) return st;
+int query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnShapeHitList* out, const hm::HullSet* hs) {
+    if (int st = shape_inputs(scalar_bits, c, s, true, hs)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     std::vector<std::vector<CastHit>> per(s->count);
     uint64_t total = 0;
     for (uint32_t i = 0; i < s->count; ++i) {
@@ -1076,11 +1105,11 @@ int avh_query_shape_hits(uint32_t scalar_bits, const AvnQueryColliders* c, const
     return AVN_OK;
 }
 
-int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnPointProjection* out) {
-    if (int st = point_inputs(scalar_bits, c, p)) return st;
+int query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnPointProjection* out, const hm::HullSet* hs) {
+    if (int st = point_inputs(scalar_bits, c, p, hs)) return st;
     if (!out || (p->count && (!out->collider || !out->point || !out->is_inside))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "outputs are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     Col pc{p->point, f64};
     ColW op{out->point, f64};
     for (uint32_t i = 0; i < p->count; ++i) {
@@ -1098,7 +1127,7 @@ int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, co
                 if (!sc.valid(col) || !qm::passes_filter(sc.memb(col), mask, xs, nx, col)) continue;
                 V3 pr;
                 bool in;
-                const S d = qm::project_point<true>(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x, solid, pr, in);
+                const S d = qh::project_point(sc.t, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x, solid, pr, in);
                 if (qm::hit_before(d, col, best_d, best_c)) { best_d = d; best_c = col; best_p = pr; best_in = in; }
             }
         const bool hit = best_c != 0xffffffffu;
@@ -1109,11 +1138,11 @@ int avh_query_project_point(uint32_t scalar_bits, const AvnQueryColliders* c, co
     return AVN_OK;
 }
 
-int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnHitList* out) {
-    if (int st = point_inputs(scalar_bits, c, p)) return st;
+int query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnPointBatch* p, AvnHitList* out, const hm::HullSet* hs) {
+    if (int st = point_inputs(scalar_bits, c, p, hs)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     Col pc{p->point, f64};
     std::vector<std::vector<uint32_t>> per(p->count);
     for (uint32_t i = 0; i < p->count; ++i) {
@@ -1124,28 +1153,43 @@ int avh_query_point_intersections(uint32_t scalar_bits, const AvnQueryColliders*
         const uint32_t nx = p->exclude_offsets ? p->exclude_offsets[i + 1] - p->exclude_offsets[i] : 0u;
         for (uint32_t col = 0; col < c->count; ++col)
             if (sc.valid(col) && qm::passes_filter(sc.memb(col), mask, xs, nx, col) &&
-                qm::contains_point<true>(c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x))
+                qh::contains_point(sc.t, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col), x))
                 per[i].push_back(col);
     }
     return write_list(out, per);
 }
 
-int avh_query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnHitList* out) {
-    if (int st = shape_inputs(scalar_bits, c, s, false)) return st;
+int query_shape_intersections(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnShapeBatch* s, AvnHitList* out, const hm::HullSet* hs) {
+    if (int st = shape_inputs(scalar_bits, c, s, false, hs)) return st;
     if (!out || !out->offsets || (out->capacity && !out->collider)) return query_fail(AVN_ERR_INVALID_ARGUMENT, "offsets and collider are required");
     const bool f64 = bits_f64(scalar_bits);
-    const QueryScene sc(c, f64);
+    const QueryScene sc(c, f64, hs);
     std::vector<std::vector<uint32_t>> per(s->count);
     for (uint32_t i = 0; i < s->count; ++i) {
         const ShapeView v = shape_at(s, f64, i, false);
         if (!v.ok) continue;
         for (uint32_t col = 0; col < c->count; ++col)
             if (sc.valid(col) && qm::passes_filter(sc.memb(col), v.mask, v.xs, v.nx, col) &&
-                qm::shapes_intersect<true>(v.shape, v.he, v.c, v.q, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col)))
+                qh::shapes_intersect(sc.t, v.shape, v.he, v.c, v.q, c->shape[col], sc.dims.v3(col), sc.pos.v3(col), sc.rot.q(col)))
                 per[i].push_back(col);
     }
     return write_list(out, per);
 }
+}  // namespace
+
+extern "C" {
+
+#define AVH_QUERY_PAIR(name, Batch, Out)                                                                                              \
+    int avh_query_##name(uint32_t bits, const AvnQueryColliders* c, const Batch* b, Out* out) { return query_##name(bits, c, b, out, nullptr); } \
+    int avh_query_##name##_hulls(uint32_t bits, const AvnQueryColliders* c, const Batch* b, Out* out, const void* h) {                   \
+        return query_##name(bits, c, b, out, static_cast<const hm::HullSet*>(h));                                                     \
+    }
+AVH_QUERY_PAIR(cast_shape, AvnShapeBatch, AvnShapeClosest)
+AVH_QUERY_PAIR(shape_hits, AvnShapeBatch, AvnShapeHitList)
+AVH_QUERY_PAIR(project_point, AvnPointBatch, AvnPointProjection)
+AVH_QUERY_PAIR(point_intersections, AvnPointBatch, AvnHitList)
+AVH_QUERY_PAIR(shape_intersections, AvnShapeBatch, AvnHitList)
+#undef AVH_QUERY_PAIR
 
 }  // extern "C"
 
@@ -1161,6 +1205,7 @@ struct HostMoveScene {
 
     bool pass(uint32_t c) const { return qm::passes_filter(sc.memb(c), mask, xs, nx, c) && !(ignored && ignored[c]); }
     void collider(uint32_t c, int& s, V3& he, V3& p, Q& q) const { s = sc.c->shape[c]; he = sc.dims.v3(c); p = sc.pos.v3(c); q = sc.rot.q(c); }
+    const hm::Table& hulls() const { return sc.t; }
     bool cast(int shape, V3 he, V3 ctr, Q q, V3 d, double maxd, double& t_out, uint32_t& c_out, int& axis_out) const {
         double best_t = INFINITY;
         uint32_t best_c = 0xffffffffu;
@@ -1169,7 +1214,7 @@ struct HostMoveScene {
             if (!valid[c] || !pass(c)) continue;
             double th;
             int ax;
-            if (qm::cast_collider<true>(shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), th, ax) &&
+            if (qh::cast_collider(sc.t, shape, he, ctr, q, d, maxd, qm::CAST_IGNORE_ORIGIN_PENETRATION, sc.c->shape[c], sc.dims.v3(c), sc.pos.v3(c), sc.rot.q(c), th, ax) &&
                 qm::hit_before(th, c, best_t, best_c)) {
                 best_t = th; best_c = c; best_axis = ax;
             }
@@ -1200,8 +1245,8 @@ struct HostMoveHits {
 };
 
 template <class T>
-void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) {
-    const QueryScene sc(c, sizeof(T) == 8);
+void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out, const hm::HullSet* hs) {
+    const QueryScene sc(c, sizeof(T) == 8, hs);
     const uint32_t C = c->count;
     std::vector<uint8_t> valid(C);
     std::vector<T> tmn(3 * size_t(C)), tmx(3 * size_t(C));
@@ -1209,7 +1254,7 @@ void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMov
         valid[k] = sc.valid(k);
         if (!valid[k]) continue;
         V3 a, e;
-        qm::collider_aabb<true>(c->shape[k], sc.dims.v3(k), sc.pos.v3(k), sc.rot.q(k), a, e);
+        qh::collider_aabb(sc.t, c->shape[k], sc.dims.v3(k), sc.pos.v3(k), sc.rot.q(k), a, e);
         tmn[3 * k] = T(a.x); tmn[3 * k + 1] = T(a.y); tmn[3 * k + 2] = T(a.z);
         tmx[3 * k] = T(e.x); tmx[3 * k + 1] = T(e.y); tmx[3 * k + 2] = T(e.z);
     }
@@ -1237,25 +1282,35 @@ void move_all(const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMov
             const HostMoveScene<T> ms{sc, valid.data(), tmn.data(), tmx.data(), b->mask ? b->mask[i] : 0xffffffffu,
                                       b->exclude_offsets ? b->exclude_offsets[i + 1] - b->exclude_offsets[i] : 0u,
                                       b->exclude_offsets ? b->exclude + b->exclude_offsets[i] : nullptr, cfg->ignored};
-            mv::move_and_slide<true>(ms, mc, bd, p, v, init, ni, hits);
+            mv::move_and_slide<2>(ms, mc, bd, p, v, init, ni, hits);
         }
         opos[3 * i] = p.x; opos[3 * i + 1] = p.y; opos[3 * i + 2] = p.z;
         ovel[3 * i] = v.x; ovel[3 * i + 1] = v.y; ovel[3 * i + 2] = v.z;
     }
 }
+int move_and_slide_all(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out, const hm::HullSet* hs) {
+    if (const char* why = check_query_colliders(scalar_bits, c, hs)) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    const uint32_t hc = hull_count(hs);
+    if (const char* why = mv::check_move(cfg, b, bits_f64(scalar_bits), c->count, bits_caps(scalar_bits), nullptr, bits_hulls(scalar_bits) ? &hc : nullptr))
+        return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
+    if (!out || (b->count && (!out->position || !out->velocity))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "position and velocity outputs are required");
+    out->kernel_ms = 0.f;
+    if (bits_f64(scalar_bits)) move_all<double>(c, cfg, b, out, hs);
+    else move_all<float>(c, cfg, b, out, hs);
+    return AVN_OK;
+}
 }  // namespace
 
 extern "C" {
 
-// MoveAndSlide::move_and_slide for every character of the batch against every collider: the same output as avn_move_and_slide
+// MoveAndSlide::move_and_slide for every character of the batch against every collider: the same output as avn_move_and_slide.
+// avh_move_and_slide_hulls: the same with the hull table (AVH_HULLS).
 int avh_move_and_slide(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out) {
-    if (const char* why = qm::check_colliders(c, true, bits_f64(scalar_bits), bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
-    if (const char* why = mv::check_move(cfg, b, bits_f64(scalar_bits), c->count, bits_caps(scalar_bits))) return query_fail(AVN_ERR_INVALID_ARGUMENT, why);
-    if (!out || (b->count && (!out->position || !out->velocity))) return query_fail(AVN_ERR_INVALID_ARGUMENT, "position and velocity outputs are required");
-    out->kernel_ms = 0.f;
-    if (bits_f64(scalar_bits)) move_all<double>(c, cfg, b, out);
-    else move_all<float>(c, cfg, b, out);
-    return AVN_OK;
+    return move_and_slide_all(scalar_bits, c, cfg, b, out, nullptr);
+}
+int avh_move_and_slide_hulls(uint32_t scalar_bits, const AvnQueryColliders* c, const AvnMoveConfig* cfg, const AvnMoveBatch* b, AvnMoveResult* out,
+                             const void* hull_table) {
+    return move_and_slide_all(scalar_bits, c, cfg, b, out, static_cast<const hm::HullSet*>(hull_table));
 }
 
 // test infrastructure: the shared project_velocity (velocity_project.rs:122-324) on one velocity, normals as f32 Dirs
@@ -1290,6 +1345,27 @@ int avh_move_contact(uint32_t scalar_bits, int sa, const double* ha, const doubl
     } else {
         float pen = 0;
         hit = mv::contact_plane<float, true>(sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        *penetration = pen;
+    }
+    normal[0] = n.x; normal[1] = n.y; normal[2] = n.z;
+    return hit ? 1 : 0;
+}
+// the same through the hull instance's contact planes (mv::contact_plane_hulls) with the fixture's hull table
+int avh_move_contact_hulls(uint32_t scalar_bits, int sa, const double* ha, const double* pa, const double* qa, int sb, const double* hb, const double* pb,
+                           const double* qb, double prediction, float* normal, double* penetration, const void* hull_table) {
+    if (!hull_table) return 0;   // no table: no contact plane, as the other *_hulls variants refuse
+    const hm::Table t = hm::view(*static_cast<const hm::HullSet*>(hull_table));
+    const V3 A{ha[0], ha[1], ha[2]}, PA{pa[0], pa[1], pa[2]}, B{hb[0], hb[1], hb[2]}, PB{pb[0], pb[1], pb[2]};
+    const Q QA{qa[0], qa[1], qa[2], qa[3]}, QB{qb[0], qb[1], qb[2], qb[3]};
+    mv::T3<float> n{0, 0, 0};
+    bool hit;
+    if (scalar_bits == 64) {
+        double pen = 0;
+        hit = mv::contact_plane_hulls<double>(t, sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
+        *penetration = pen;
+    } else {
+        float pen = 0;
+        hit = mv::contact_plane_hulls<float>(t, sa, A, PA, QA, sb, B, PB, QB, prediction, n, pen);
         *penetration = pen;
     }
     normal[0] = n.x; normal[1] = n.y; normal[2] = n.z;

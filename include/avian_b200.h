@@ -375,8 +375,8 @@ AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
  * shapes), move and slide (obstacles and characters) and swept CCD (with AVN_CCD_CAPSULES) take capsules.
  * AVN_SHAPE_CONVEX_HULL: Collider::convex_hull / the parts of Collider::convex_decomposition, dims = [hull index, unused, unused] into the
  * context's hull table (avn_set_convex_hulls).  The index is stored in the column scalar: integral, non-negative and below the table's hull
- * count.  The AABB update, the narrow phase and the contact store take hulls; the spatial queries, move and slide refuse them, and swept CCD
- * returns AVN_ERR_UNSUPPORTED while the contact store holds one. */
+ * count.  The AABB update, the narrow phase, the contact store, the spatial queries (colliders and query shapes) and move and slide (obstacles
+ * and characters) take hulls; swept CCD returns AVN_ERR_UNSUPPORTED while the contact store holds one. */
 typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2, AVN_SHAPE_CONVEX_HULL = 3 } AvnShape;
 
 /* ---- convex hulls: the table AVN_SHAPE_CONVEX_HULL colliders index (parry's ConvexPolyhedron: points, faces as vertex loops) ---------- */
@@ -693,7 +693,7 @@ AvnStatus avn_islands_wake(AvnContext* ctx, const uint8_t* wake, AvnIslandsWake*
 AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uint8_t* row_asleep, uint32_t body_count, uint8_t* body_asleep);
 
 /* ---- spatial queries (SpatialQueryPlugin, src/lib.rs:839; spatial_query/pipeline.rs): a collider tree rebuilt on the device by every
- *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid, sphere and capsule colliders.
+ *      avn_query_update, then batched ray casts and AABB intersection tests against it.  Cuboid, sphere, capsule and convex hull colliders.
  *      The per-shape arithmetic is this repository's own (avian_b200/csrc/query_math.hpp, shared with the host fixture; parry3d is not
  *      vendored), so results equal the host brute force over every collider bit for bit, independent of the tree.  Conventions:
  *        - a ray is origin + t * direction, t in units of |direction| (pass a unit Dir3); a hit counts when 0 <= t <= max_distance;
@@ -702,6 +702,12 @@ AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uin
  *          component that is exactly 0 leaves its axis unconstrained when the origin is inside that slab and misses otherwise;
  *        - capsule: tight AABB = the posed segment ends' min / max grown by the radius; normal = unit(hit - closest segment point); a
  *          radius-0 capsule is a closed segment (avian_b200/csrc/query_math.hpp, DESIGN.md §7j);
+ *        - convex hull (avian_b200/csrc/hull_query_math.hpp, DESIGN.md §7l): tight AABB = the posed vertices' min / max; the ray test,
+ *          containment and projection from inside use the table's face planes; normal = the posed face normal of the entering face (largest
+ *          entering parameter, ties to the lowest face); the index is checked against the context's hull table (avn_set_convex_hulls) as
+ *          avn_contacts_step checks it, a hull without a table is refused, and under AVN_QUERY_SHAPES_UNCHANGED the kept column's largest index
+ *          is checked against the current table.  Replacing the table (avn_set_convex_hulls) makes every query and avn_move_and_slide against
+ *          a tree that holds a hull fail with AVN_ERR_INVALID_ARGUMENT until the next avn_query_update;
  *        - filter (SpatialQueryFilter::test, query_filter.rs:97-101): (memberships & mask) != 0 and not in the ray's excluded list;
  *        - AABB test: inclusive compares (Aabb::intersects) against the collider's tight AABB (compute_aabb) rounded to the column scalar,
  *          no filter, as pipeline.rs:709-729;
@@ -711,7 +717,7 @@ AvnStatus avn_contacts_download_sleeping(AvnContext* ctx, uint32_t capacity, uin
  *      Stated deviations: the closest hit is the lexicographic minimum of (t, collider index), where the reference takes the first in tree
  *      order; ray_hits keeps the max_hits NEAREST hits sorted by (t, collider index) — RayHits::iter_sorted order — where the reference keeps
  *      the first max_hits in tree order, unordered (pipeline.rs:213-216); the two sets are equal when a ray has no more than max_hits hits.
- *      Shape casts, point projection and point / shape intersections (cuboid, sphere and capsule query shapes) are further down, with their own
+ *      Shape casts, point projection and point / shape intersections (cuboid, sphere, capsule and hull query shapes) are further down, with their own
  *      conventions.  Not covered: target_distance != 0, other shapes, predicates and the *_callback early exits, several GPUs. ------------- */
 typedef struct AvnQueryColliders {
     uint32_t count;
@@ -877,7 +883,8 @@ AvnStatus avn_query_shape_intersections(AvnContext* ctx, const AvnShapeBatch* sh
  *      Stated deviations: on_hit cannot run on the device — every hit is accepted and nothing edits the normal, position or velocity; the
  *      closest sweep hit is the lowest (t, collider index), not the first in tree order; intersections are visited in ascending collider
  *      index, not tree order; hit_toi reports the TOI, where MoveHitData::collision_distance is the requested movement length (:777);
- *      characters are cuboids, spheres and capsules (capsule conventions: avian_b200/csrc/query_math.hpp, DESIGN.md §7j). ------------- */
+ *      characters are cuboids, spheres, capsules and convex hulls (capsule conventions: avian_b200/csrc/query_math.hpp, DESIGN.md §7j; hulls:
+ *      avian_b200/csrc/hull_query_math.hpp, DESIGN.md §7l, their indices checked against the context's hull table). ------------- */
 #define AVN_MOVE_MAX_PLANES 32
 
 /* MoveAndSlideConfig, one per call.  The reference's defaults: skin_width 0.01, max_depenetration_error 0.0001,
