@@ -51,7 +51,7 @@ _UNIT_HEADERS = {
     "narrow.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp"],
     "contacts.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "contact_rows.hpp", "device_prims.cuh"],
     "queries.cu": ["context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "query_math.hpp", "hull_query_math.hpp", "move_math.hpp", "device_prims.cuh"],
-    "ccd.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "query_math.hpp", "ccd_math.hpp", "device_prims.cuh"],
+    "ccd.cu": ["avn_math.cuh", "context.hpp", "hull_table.hpp", "shape_column.hpp", "narrow_math.hpp", "hull_math.hpp", "query_math.hpp", "hull_query_math.hpp", "ccd_math.hpp", "device_prims.cuh"],
 }
 
 

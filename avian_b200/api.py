@@ -449,11 +449,13 @@ class AvnCcdResult(C.Structure):
 
 SWEEP_LINEAR, SWEEP_NON_LINEAR = 0, 1
 CCD_CAPSULES = 0x1   # AvnCcdConfig.flags: capsule colliders take part in swept CCD
+CCD_HULLS = 0x4      # AvnCcdConfig.flags: convex hull colliders take part in swept CCD
 
 
 def ccd_config(body, collider, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
                prediction_distance: float = float("inf"), flags: int = 0) -> tuple["AvnCcdConfig", tuple]:
-    """An AvnCcdConfig over numpy copies of the columns (returned alongside: they must outlive the struct's use).  flags: CCD_CAPSULES or 0."""
+    """An AvnCcdConfig over numpy copies of the columns (returned alongside: they must outlive the struct's use).  flags: CCD_CAPSULES and
+    CCD_HULLS bits, or 0."""
     cols = (np.ascontiguousarray(body, dtype=np.int32), np.ascontiguousarray(collider, dtype=np.uint32),
             None if mode is None else np.ascontiguousarray(mode, dtype=np.uint8),
             None if include_dynamic is None else np.ascontiguousarray(include_dynamic, dtype=np.uint8),
@@ -1229,15 +1231,17 @@ class Context:
 
     # ---- swept CCD (include/avian_b200.h avn_ccd_*): solve_swept_ccd inside the device-resident solver stage
     def ccd_configure(self, body=None, collider=None, mode=None, include_dynamic=None, linear_threshold=None, angular_threshold=None,
-                      prediction_distance: float = float("inf"), capsules: bool = False) -> None:
+                      prediction_distance: float = float("inf"), capsules: bool = False, hulls: bool = False) -> None:
         """avn_ccd_configure: the SweptCcd bodies in query order and their own colliders; body=None clears the configuration.  capsules=True
-        sets AVN_CCD_CAPSULES: capsule colliders are swept (without it a contact store that holds one is refused)."""
+        sets AVN_CCD_CAPSULES: capsule colliders are swept (without it a contact store that holds one is refused).  hulls=True sets
+        AVN_CCD_HULLS: convex hull colliders are swept over the context's hull table (set_convex_hulls); without it a contact store that holds
+        one is refused.  A solver_run after set_convex_hulls has replaced the table fails until the next contacts_step."""
         if body is None or len(body) == 0:
             self._check(self.lib.avn_ccd_configure(self.handle, None))
             self._ccd_n = 0
             return
         cfg, cols = ccd_config(body, collider, mode, include_dynamic, linear_threshold, angular_threshold, prediction_distance,
-                               CCD_CAPSULES if capsules else 0)
+                               (CCD_CAPSULES if capsules else 0) | (CCD_HULLS if hulls else 0))
         self._check(self.lib.avn_ccd_configure(self.handle, C.byref(cfg)))
         self._ccd_n = int(cfg.count)
 

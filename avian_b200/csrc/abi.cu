@@ -21,7 +21,7 @@ struct AvnContext {
     std::unique_ptr<avn::QueriesBase> queries;
     std::unique_ptr<avn::CommBase> comm;
     std::unique_ptr<avn::CcdBase> ccd;
-    avn::HullTable hulls;              // avn_set_convex_hulls; read by aabbs, narrow, contacts and queries
+    avn::HullTable hulls;              // avn_set_convex_hulls; read by aabbs, narrow, contacts, queries and ccd
     AvnTimings last{};
 };
 
@@ -100,6 +100,7 @@ AvnStatus avn_create(const AvnConfig* config, AvnContext** out_ctx) {
         ctx->narrow->attach_hulls(&ctx->hulls);
         ctx->contacts->attach_hulls(&ctx->hulls);
         ctx->queries->attach_hulls(&ctx->hulls);
+        ctx->ccd->attach_hulls(&ctx->hulls);
         *out_ctx = ctx.release();
         return AVN_OK;
     } catch (...) {
@@ -416,15 +417,16 @@ AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const
 // swept CCD (ccd.cu): solve_swept_ccd inside avn_solver_run
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config) {
     return guarded(ctx, [&] {
-        if (config && config->count && (config->flags & ~AVN_CCD_CAPSULES))
-            return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "ccd_configure: unknown flags 0x%x (only AVN_CCD_CAPSULES)", config->flags & ~AVN_CCD_CAPSULES);
+        const uint32_t known = AVN_CCD_CAPSULES | AVN_CCD_HULLS;
+        if (config && config->count && (config->flags & ~known))
+            return ctx->err.fail(AVN_ERR_INVALID_ARGUMENT, "ccd_configure: unknown flags 0x%x (only AVN_CCD_CAPSULES and AVN_CCD_HULLS)", config->flags & ~known);
         avn::ContactsBase::AsleepBodies asleep;
         ctx->contacts->asleep_bodies(&asleep);
         if (asleep.body_asleep && config && config->count)
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: sleeping is applied on this context (avn_islands_apply); sleeping bodies are not swept against");
         if (config && config->count && !(config->flags & AVN_CCD_CAPSULES) && ctx->contacts->has_capsule())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a capsule; capsule times of impact are not implemented");
-        if (config && config->count && ctx->contacts->has_hull())
+        if (config && config->count && !(config->flags & AVN_CCD_HULLS) && ctx->contacts->has_hull())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: the contact store's shape column holds a convex hull; hull times of impact are not implemented");
         if (config && config->count && ctx->contacts->body_frames())
             return ctx->err.fail(AVN_ERR_UNSUPPORTED, "ccd_configure: body frames are set (avn_contacts_set_body_frames); swept CCD assumes a collider at its body's origin");

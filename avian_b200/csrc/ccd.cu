@@ -6,9 +6,9 @@
 //      filters of its slot and is appended to the candidate list (atomic counter: the results below do not depend on the list's order).
 //   2. TOI: one thread per candidate (the grid is sized for every row, the threads past the device-side count leave), so a warp does only
 //      real TOI work.  Per slot the smallest accepted TOI (ordered bits, atomicMin), then among the candidates that reached it the lowest
-//      ContactId — the stated tie deviation.  The CAPS = true instance, which also sweeps capsules, runs instead of the cuboid / sphere one
-//      only when the contact store's shape column holds a capsule (AVN_CCD_CAPSULES lets such a store through); the other kernels read no
-//      geometry.
+//      ContactId — the stated tie deviation.  The instance is the lowest shape level that covers the contact store's shape column: G = 2
+//      (convex hulls, with the context's hull table) when it holds a hull, G = 1 (capsules) when it holds a capsule, else G = 0 (cuboids
+//      and spheres); AVN_CCD_HULLS / AVN_CCD_CAPSULES let such a store through.  The other kernels read no geometry.
 //   3. apply: per slot with a hit, one record for body 1 and one for body 2 when it has a SolverBody, record index = 2 * slot + side.  A
 //      stable radix sort by body keeps every body's records in slot order; one thread per body replays them: the last delta_position wins
 //      and the delta_rotation compositions happen in order — the reference's sequential loop, bit for bit.
@@ -94,8 +94,8 @@ __global__ void __launch_bounds__(CCD_BLOCK) ccd_candidates_kernel(CcdDev<S> d) 
 }
 
 // 2. the TOI of every candidate (compute_ccd_toi, ccd/mod.rs:692-780) and the per-slot minimum
-template <class S, bool CAPS>
-__global__ void __launch_bounds__(CCD_BLOCK) ccd_toi_kernel(CcdDev<S> d) {
+template <class S, int G>
+__global__ void __launch_bounds__(CCD_BLOCK) ccd_toi_kernel(CcdDev<S> d, hm::Table hulls) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= *d.cand_count) return;
     const uint32_t c = d.cand[i], e = c & CAND_ROW;
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(CCD_BLOCK) ccd_toi_kernel(CcdDev<S> d) {
     const int k = d.slot_of_collider[own];
     const uint32_t body1 = uint32_t(d.body[k]), body2 = side ? d.b1[e] : d.b2[e];
     const ccd::Motion A = motion(d, body1, own), Bm = motion(d, body2, other);
-    const S t = ccd::pair_toi<S, CAPS>((c & CAND_LINEAR) ? ccd::MODE_LINEAR : ccd::MODE_NON_LINEAR, A, Bm, d.dt, d.eps, d.prediction);
+    const S t = ccd::pair_toi<S, G>((c & CAND_LINEAR) ? ccd::MODE_LINEAR : ccd::MODE_NON_LINEAR, A, Bm, d.dt, d.eps, d.prediction, &hulls);
     d.cand_toi[i] = t;
     if (t > S(0) && t < d.dt) {
         atomicAdd(&d.nhit[k], 1u);
@@ -182,7 +182,7 @@ class Ccd final : public CcdBase {
         if (!cfg || cfg->count == 0) {
             K_ = 0;
             ran_ = false;
-            capsules_ = false;
+            capsules_ = hulls_flag_ = false;
             return AVN_OK;
         }
         if (!cfg->body || !cfg->collider) return err_->fail(AVN_ERR_INVALID_ARGUMENT, "ccd: body and collider are required");
@@ -234,11 +234,17 @@ class Ccd final : public CcdBase {
         n_bodies_ = int(rows.bodies);
         prediction_ = cfg->prediction_distance;
         capsules_ = (cfg->flags & AVN_CCD_CAPSULES) != 0;
+        hulls_flag_ = (cfg->flags & AVN_CCD_HULLS) != 0;
         return AVN_OK;
     }
 
     bool active() const override { return K_ > 0; }
     bool capsules() const override { return capsules_; }
+    bool hulls() const override { return hulls_flag_; }
+    void attach_hulls(const HullTable* hulls) override { table_ = hulls; }
+    bool table_changed(const CcdRows& rows) const override {
+        return rows.has_hull && rows.dims && rows.rows > 0 && (!table_ || !table_->set || table_->generation != rows.hull_generation);
+    }
 
     AvnStatus run(const CcdSolverState& st, const CcdRows& rows, uint32_t* launches) override {
         CcdDev<S> d{};
@@ -272,8 +278,9 @@ class Ccd final : public CcdBase {
         if (d.rows > 0) {
             const int g_rows = (d.rows + CCD_BLOCK - 1) / CCD_BLOCK, g_cand = int((cand_cap + CCD_BLOCK - 1) / CCD_BLOCK);
             ccd_candidates_kernel<S><<<g_rows, CCD_BLOCK, 0, stream_>>>(d);
-            if (rows.has_capsule) ccd_toi_kernel<S, true><<<g_cand, CCD_BLOCK, 0, stream_>>>(d);
-            else ccd_toi_kernel<S, false><<<g_cand, CCD_BLOCK, 0, stream_>>>(d);
+            if (rows.has_hull) ccd_toi_kernel<S, 2><<<g_cand, CCD_BLOCK, 0, stream_>>>(d, table_->dev);
+            else if (rows.has_capsule) ccd_toi_kernel<S, 1><<<g_cand, CCD_BLOCK, 0, stream_>>>(d, hm::Table{});
+            else ccd_toi_kernel<S, 0><<<g_cand, CCD_BLOCK, 0, stream_>>>(d, hm::Table{});
             ccd_tie_kernel<S><<<g_cand, CCD_BLOCK, 0, stream_>>>(d);
             n_launch += 3;
         }
@@ -330,7 +337,8 @@ class Ccd final : public CcdBase {
     cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
     int K_ = 0, n_colliders_ = 0, n_bodies_ = 0;
     double prediction_ = INFINITY;
-    bool ran_ = false, capsules_ = false;
+    bool ran_ = false, capsules_ = false, hulls_flag_ = false;
+    const HullTable* table_ = nullptr;
     DevBuf body_, coll_, mode_, inc_, lt_, at_, slot_c_, slot_b_, best_, best_row_, ncand_, nhit_, out_min_, out_body_, out_contact_, m_, k0_, k1_, v0_, v1_,
         hist_, count_, cand_, cand_toi_;
 };

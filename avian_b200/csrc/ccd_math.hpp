@@ -1,4 +1,4 @@
-// Swept continuous collision detection (solve_swept_ccd, dynamics/ccd/mod.rs:523-780) for cuboid / sphere / capsule colliders: the pair time of impact,
+// Swept continuous collision detection (solve_swept_ccd, dynamics/ccd/mod.rs:523-780) for cuboid / sphere / capsule / convex hull colliders: the pair time of impact,
 // the per-pair filters and the delta arithmetic, written once for the host fixture (g++, -ffp-contract=off) and for the device pass
 // (csrc/ccd.cu, nvcc -fmad=false): the same expressions in the same order, so both evaluate to the same bits.
 //
@@ -19,17 +19,26 @@
 //     The iterates do not depend on t_max, so evaluating every candidate against dt and keeping the minimum equals the reference's
 //     sequential scan with a shrinking bound.
 //   * eps = CCD_EPS_PER_LENGTH_UNIT * PhysicsLengthUnit.
-//   * Capsules (the CAPS = true instances; DESIGN.md §7e): dims = [radius, half length, ·], the segment along the collider's local y
-//     (rot_mat(q(t)).c[1], as qm::capsule_of).  Linear mode: qm::cast_toi<true>'s exact capsule casts.  Non-linear mode: capsule_distance
-//     (point-segment, nm::segment_closest, or 0 when qm::segment_meets_box and else nm::segment_box_closest, less the radii; the swapped
-//     orders negate n), and R = |(|lc.x|, |lc.y| + half length, |lc.z|)| + radius.  Every capsule branch is out of line and comes first,
-//     so with no capsule in the pair the TOI is the CAPS = false one, bit for bit.
+//   * Shape level G (DESIGN.md §7e): G = 0 cuboids and spheres, G = 1 adds capsules, G = 2 adds convex hulls over the hull table (the
+//     table pointer of the G = 2 entry points; the lower levels take none).  Every branch of a level is out of line and comes first, so a
+//     pair without the level's shape evaluates exactly as at the level below, bit for bit.
+//   * Capsules (G >= 1): dims = [radius, half length, ·], the segment along the collider's local y (rot_mat(q(t)).c[1], as qm::capsule_of).
+//     Linear mode: qm::cast_toi<true>'s exact capsule casts.  Non-linear mode: capsule_distance (point-segment, nm::segment_closest, or 0
+//     when qm::segment_meets_box and else nm::segment_box_closest, less the radii; the swapped orders negate n), and
+//     R = |(|lc.x|, |lc.y| + half length, |lc.z|)| + radius.
+//   * Convex hulls (G = 2): dims = [hull index, ·, ·], posed by hm::table_hull_at with pose_at's rotation matrix.  Linear mode: qh::cast_toi
+//     (the exact hull casts of the spatial queries).  Non-linear mode: hull_distance (0 when qh::poly_intersect, else hm::hull_hull_closest
+//     for a hull and a hull or a cuboid as hm::box_hull; 0 when qh::point_near_hull, else sqrt(hm::point_hull_closest) less the radius for
+//     a sphere; 0 when qh::segment_near_hull, else the distance of qh::segment_closest_point to the hull less the radius for a capsule; the
+//     swapped orders negate n), and R = max_k |v_k - lc| over the hull-local vertices + AVN_HULL_REL_TOL x the local vertex-box diagonal:
+//     the face planes, which the distance reads, can stand out of the vertex hull by that tolerance.
 //   * sin / cos of from_scaled_axis come from ccd_sincos below (Cody-Waite reduction, Taylor polynomials, no libm), so the host and the
 //     device round identically in f64 too; otherwise the expression tree is avn_math.cuh's q_from_scaled_axis and qmul.
 #pragma once
 #include <cmath>
 #include <cstdint>
 
+#include "hull_query_math.hpp"
 #include "query_math.hpp"
 
 namespace ccd {
@@ -112,10 +121,29 @@ struct Motion {
     V3 v, w;     // linear / angular velocity
 };
 
-// farthest point of the shape from its centre of mass (a capsule: the farther end of its segment, plus the radius)
-template <bool CAPS = false>
-NM_HD inline S motion_radius(const Motion& m) {
-    if (CAPS && m.shape == nm::SHAPE_CAPSULE) return nm::len(V3{fabs(m.lc.x), fabs(m.lc.y) + m.he.y, fabs(m.lc.z)}) + m.he.x;
+// a hull's farthest vertex from the centre of mass, plus the table's tolerance (see the header comment)
+NM_COLD inline S hull_motion_radius(const hm::Table& t, const Motion& m) {
+    const uint32_t h = qh::hull_index(m.he), v0 = t.voff[h], nv = t.voff[h + 1] - v0;
+    const double* v = t.vert + 3 * size_t(v0);
+    V3 lo{v[0], v[1], v[2]}, hi = lo;
+    S r2 = 0;
+NM_ROLLED
+    for (uint32_t k = 0; k < nv; ++k) {
+        const V3 p{v[3 * k], v[3 * k + 1], v[3 * k + 2]}, e = p - m.lc;
+        r2 = nm::smax(r2, nm::dot(e, e));
+        lo = V3{nm::smin(lo.x, p.x), nm::smin(lo.y, p.y), nm::smin(lo.z, p.z)};
+        hi = V3{nm::smax(hi.x, p.x), nm::smax(hi.y, p.y), nm::smax(hi.z, p.z)};
+    }
+    return sqrt(r2) + hm::REL_TOL * nm::len(hi - lo);
+}
+
+// farthest point of the shape from its centre of mass (a capsule: the farther end of its segment, plus the radius; a hull:
+// hull_motion_radius with the table ht, G = 2 only)
+template <int G = 0>
+NM_HD inline S motion_radius(const Motion& m, const hm::Table* ht = nullptr) {
+    if constexpr (G == 2)
+        if (m.shape == hm::SHAPE_CONVEX_HULL) return hull_motion_radius(*ht, m);
+    if (G >= 1 && m.shape == nm::SHAPE_CAPSULE) return nm::len(V3{fabs(m.lc.x), fabs(m.lc.y) + m.he.y, fabs(m.lc.z)}) + m.he.x;
     if (m.shape == nm::SHAPE_SPHERE) return nm::len(m.lc) + m.he.x;
     const V3 e{fabs(m.lc.x) + m.he.x, fabs(m.lc.y) + m.he.y, fabs(m.lc.z) + m.he.z};
     return nm::len(e);
@@ -162,11 +190,42 @@ NM_COLD inline S capsule_distance(int sa, V3 ha, V3 ca, const nm::M3& ra, int sb
     return nm::smax(l - radii, 0);
 }
 
+// shape_distance of a pair with at least one hull H (A when A is one) and the other shape O (see the header comment)
+NM_COLD inline S hull_distance(const hm::Table& t, int sa, V3 ha, V3 ca, const nm::M3& ra, int sb, V3 hb, V3 cb, const nm::M3& rb, V3& n) {
+    n = V3{0, 1, 0};
+    const bool a_hull = sa == hm::SHAPE_CONVEX_HULL;
+    const int so = a_hull ? sb : sa;
+    if (qh::is_poly(so)) {
+        hm::BoxHull ba, bb;
+        const hm::Hull A = qh::polytope(t, ba, sa, ha, ca, ra), B = qh::polytope(t, bb, sb, hb, cb, rb);
+        if (qh::poly_intersect(A, B)) return 0;
+        V3 on_a, on_b;
+        const S l = hm::hull_hull_closest(A, B, on_a, on_b);
+        if (l > 0) n = (on_b - on_a) * (1 / l);
+        return nm::smax(l, 0);
+    }
+    const hm::Hull H = hm::table_hull_at(t, qh::hull_index(a_hull ? ha : hb), a_hull ? ca : cb, a_hull ? ra : rb);
+    const V3 ho = a_hull ? hb : ha, co = a_hull ? cb : ca;
+    V3 x = co;   // the point of O nearest the hull: the sphere's centre, or the capsule segment's point nearest it
+    if (so == nm::SHAPE_SPHERE) {
+        if (qh::point_near_hull(H, co, ho.x)) return 0;
+    } else {
+        const V3 u = (a_hull ? rb : ra).c[1];
+        if (qh::segment_near_hull(H, co, u, ho.y, ho.x)) return 0;
+        x = qh::segment_closest_point(H, co, u, ho.y);
+    }
+    V3 on;
+    const S l = sqrt(hm::point_hull_closest(H, x, on));
+    if (l > 0) n = (a_hull ? x - on : on - x) * (1 / l);
+    return nm::smax(l - ho.x, 0);
+}
+
 // Distance between the closed shapes A and B (0 when they overlap or touch) and the unit direction n from A to B.  Out of line and rolled,
-// like nm::box_box_closest which it calls.  CAPS: pairs with a capsule go to capsule_distance (the CAPS = false instance has no such branch).
-template <bool CAPS = false>
+// like nm::box_box_closest which it calls.  G >= 1: pairs with a capsule go to capsule_distance (the G = 0 instance has no such branch);
+// pairs with a hull never come here (nonlinear_toi sends them to hull_distance).
+template <int G = 0>
 NM_COLD inline S shape_distance(int sa, V3 ha, V3 ca, const nm::M3& ra, int sb, V3 hb, V3 cb, const nm::M3& rb, V3& n) {
-    if (CAPS && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) return capsule_distance(sa, ha, ca, ra, sb, hb, cb, rb, n);
+    if (G >= 1 && (sa == nm::SHAPE_CAPSULE || sb == nm::SHAPE_CAPSULE)) return capsule_distance(sa, ha, ca, ra, sb, hb, cb, rb, n);
     n = V3{0, 1, 0};
     if (sa == nm::SHAPE_SPHERE && sb == nm::SHAPE_SPHERE) {
         const V3 e = cb - ca;
@@ -200,11 +259,11 @@ NM_ROLLED
 }
 
 // conservative advancement on [0, t_max]; see the header comment.  *iterations (optional): the distance evaluations it took; a hit reported
-// with CCD_MAX_ITERATIONS of them stopped at the cap, before reaching eps
-template <bool CAPS = false>
-NM_HD inline bool nonlinear_toi(const Motion& A, const Motion& B, S t_max, S eps, S& toi, int* iterations = nullptr) {
+// with CCD_MAX_ITERATIONS of them stopped at the cap, before reaching eps.  ht: the hull table (G = 2)
+template <int G = 0>
+NM_HD inline bool nonlinear_toi(const Motion& A, const Motion& B, S t_max, S eps, S& toi, int* iterations = nullptr, const hm::Table* ht = nullptr) {
     const V3 rel = B.v - A.v;
-    const S spin = nm::len(A.w) * motion_radius<CAPS>(A) + nm::len(B.w) * motion_radius<CAPS>(B);
+    const S spin = nm::len(A.w) * motion_radius<G>(A, ht) + nm::len(B.w) * motion_radius<G>(B, ht);
     S t = 0;
 NM_ROLLED
     for (int it = 0; it < CCD_MAX_ITERATIONS; ++it) {
@@ -212,7 +271,12 @@ NM_ROLLED
         nm::M3 ra, rb;
         pose_at(A, t, ca, ra);
         pose_at(B, t, cb, rb);
-        const S d = shape_distance<CAPS>(A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n);
+        S d;
+        if constexpr (G == 2)
+            d = A.shape == hm::SHAPE_CONVEX_HULL || B.shape == hm::SHAPE_CONVEX_HULL ? hull_distance(*ht, A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n)
+                                                                                     : shape_distance<1>(A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n);
+        else
+            d = shape_distance<G>(A.shape, A.he, ca, ra, B.shape, B.he, cb, rb, n);
         if (iterations) *iterations = it + 1;
         if (d != d) return false;
         if (d <= eps) { toi = t; return true; }
@@ -225,26 +289,28 @@ NM_ROLLED
     return true;
 }
 
-// shape 1 moving with v1 - v2 against shape 2 at rest (qm::cast_toi)
-template <bool CAPS = false>
-NM_HD inline bool linear_toi(const Motion& A, const Motion& B, S t_max, S& toi) {
+// shape 1 moving with v1 - v2 against shape 2 at rest (qm::cast_toi; qh::cast_toi with the hull table at G = 2)
+template <int G = 0>
+NM_HD inline bool linear_toi(const Motion& A, const Motion& B, S t_max, S& toi, const hm::Table* ht = nullptr) {
     int axis;
-    return qm::cast_toi<CAPS>(A.shape, A.he, A.p, A.q, A.v - B.v, t_max, B.shape, B.he, B.p, B.q, toi, axis);
+    if constexpr (G == 2) return qh::cast_toi(*ht, A.shape, A.he, A.p, A.q, A.v - B.v, t_max, B.shape, B.he, B.p, B.q, toi, axis);
+    else return qm::cast_toi<G == 1>(A.shape, A.he, A.p, A.q, A.v - B.v, t_max, B.shape, B.he, B.p, B.q, toi, axis);
 }
 
 // compute_ccd_toi (ccd/mod.rs:692-780) against the bound dt: the TOI rounded to T, with the reference's fallback when it is exactly 0 (shape 2
 // replaced by a ball of radius prediction_distance at body 2's pose); T(-1) when the shapes never come within reach on [0, dt].  The caller
-// accepts the value when 0 < toi < min_toi.  CAPS: capsules take part (the CAPS = false instance treats every shape as a cuboid or a sphere).
-template <class T, bool CAPS = false> NM_HD inline T pair_toi(int mode, const Motion& A, const Motion& B, T dt, S eps, S prediction_distance) {
+// accepts the value when 0 < toi < min_toi.  G: the shape level (G = 0 treats every shape as a cuboid or a sphere); ht: the hull table (G = 2).
+template <class T, int G = 0>
+NM_HD inline T pair_toi(int mode, const Motion& A, const Motion& B, T dt, S eps, S prediction_distance, const hm::Table* ht = nullptr) {
     S t = 0;
-    const bool hit = mode == MODE_LINEAR ? linear_toi<CAPS>(A, B, S(dt), t) : nonlinear_toi<CAPS>(A, B, S(dt), eps, t);
+    const bool hit = mode == MODE_LINEAR ? linear_toi<G>(A, B, S(dt), t, ht) : nonlinear_toi<G>(A, B, S(dt), eps, t, nullptr, ht);
     if (!hit) return T(-1);
     const T tt = static_cast<T>(t);
     if (tt != T(0)) return tt;
     Motion ball = B;
     ball.shape = nm::SHAPE_SPHERE;
     ball.he = V3{prediction_distance, 0, 0};
-    const bool hit2 = mode == MODE_LINEAR ? linear_toi<CAPS>(A, ball, S(dt), t) : nonlinear_toi<CAPS>(A, ball, S(dt), eps, t);
+    const bool hit2 = mode == MODE_LINEAR ? linear_toi<G>(A, ball, S(dt), t, ht) : nonlinear_toi<G>(A, ball, S(dt), eps, t, nullptr, ht);
     return hit2 ? static_cast<T>(t) : T(-1);
 }
 

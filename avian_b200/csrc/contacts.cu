@@ -894,6 +894,7 @@ class Contacts final : public ContactsBase {
         if (in->body_count > n_bodies_ || in->collider_count > n_colliders_)
             return err_->fail(AVN_ERR_INVALID_ARGUMENT, "contacts_step: %u bodies / %u colliders exceed the configured %u / %u", in->body_count, in->collider_count,
                               n_bodies_, n_colliders_);
+        hull_generation_ = hulls_->generation;   // the table this step's hull kernels read (swept CCD checks it)
         const uint64_t n_new64 = np ? np->count : 0;
         if (n_new64 > 0x7fffffffull - hw_) return err_->fail(AVN_ERR_CAPACITY, "contacts_step: too many contact pairs");
         const uint32_t n_new = uint32_t(n_new64);
@@ -1085,6 +1086,8 @@ class Contacts final : public ContactsBase {
         out->shape = in_.shape;
         out->dims = in_.dims;
         out->has_capsule = has_capsule_;
+        out->has_hull = has_hull_;
+        out->hull_generation = hull_generation_;
     }
     void attach_hulls(const HullTable* hulls) override { hulls_ = hulls; }
     bool has_hull() const override { return has_hull_; }
@@ -1720,6 +1723,7 @@ class Contacts final : public ContactsBase {
     const AvnNarrowInput* checked_ = nullptr;   // the input check_shapes last accepted, and whether its column holds a capsule
     bool checked_capsule_ = false;
     const HullTable* hulls_ = nullptr;
+    uint64_t hull_generation_ = 0;
     bool has_hull_ = false;       // the shape column on the device holds a convex hull; max_hull_: the largest index it names
     uint32_t max_hull_ = 0;
     bool checked_hull_ = false;

@@ -56,10 +56,10 @@ struct DevBuf {
 };
 
 // The context's convex hull table (avn_set_convex_hulls) on the device.  dev holds device pointers; count() is 0 while no table is set.  The
-// AABB updater, the narrow phase, the contact store and the query tree hold a pointer to it.
+// AABB updater, the narrow phase, the contact store, the query tree and swept CCD hold a pointer to it.
 struct HullTable {
     bool set = false;
-    uint64_t generation = 0;   // incremented by every avn_set_convex_hulls that changes the table; the query tree checks it
+    uint64_t generation = 0;   // incremented by every avn_set_convex_hulls that changes the table; the query tree and swept CCD check it
     hm::Table dev{};
     DevBuf vert, plane, centre, radius, voff, foff, loff, loop, eoff, edge;
     uint32_t count() const { return set ? dev.count : 0; }
@@ -218,8 +218,9 @@ struct ContactsBase {
     //      AVN_CCD_CAPSULES, and launches its capsule TOI kernel only when it holds one)
     virtual AvnStatus check_shapes(const AvnNarrowInput* in, uint32_t flags) = 0;
     virtual bool has_capsule() const = 0;
-    // has_hull: the column on the device holds a convex hull (swept CCD refuses it; its rows run in the hull kernels).  The hull table is the
-    // context's (attach_hulls); a step under AVN_CONTACTS_SHAPES_UNCHANGED checks the kept column's largest hull index against it.
+    // has_hull: the column on the device holds a convex hull (swept CCD refuses it unless configured with AVN_CCD_HULLS; its rows run in the
+    // hull kernels).  The hull table is the context's (attach_hulls); a step under AVN_CONTACTS_SHAPES_UNCHANGED checks the kept column's
+    // largest hull index against it, and every step records the table's generation for swept CCD (CcdRows::hull_generation).
     virtual bool has_hull() const = 0;
     virtual void attach_hulls(const HullTable* hulls) = 0;
     // ---- body frames (avn_contacts_set_body_frames): checked and copied on the host (NULL clears them); body_frames() = NULL when none are set
@@ -237,6 +238,8 @@ struct CcdRows {
     const uint8_t* shape = nullptr;    // [C] of the last avn_contacts_step (NULL = cuboid)
     const void* dims = nullptr;        // [C][3]
     bool has_capsule = false;          // the shape column holds a capsule
+    bool has_hull = false;             // the shape column holds a convex hull
+    uint64_t hull_generation = 0;      // HullTable::generation at the last avn_contacts_step (the table its hull kernels read)
 };
 struct CcdSolverState {
     int B = 0;
@@ -251,6 +254,11 @@ struct CcdBase {
     virtual AvnStatus configure(const AvnCcdConfig* cfg, const CcdRows& rows) = 0;
     virtual bool active() const = 0;
     virtual bool capsules() const = 0;   // configured with AVN_CCD_CAPSULES
+    virtual bool hulls() const = 0;      // configured with AVN_CCD_HULLS
+    // the context's hull table, which the hull TOI kernel reads; table_changed: the pass would run that kernel and the table is no longer
+    // the one the last contact step used (avn_set_convex_hulls since)
+    virtual void attach_hulls(const HullTable* hulls) = 0;
+    virtual bool table_changed(const CcdRows& rows) const = 0;
     // enqueued on the context's stream; adds its kernel launches to *launches
     virtual AvnStatus run(const CcdSolverState& st, const CcdRows& rows, uint32_t* launches) = 0;
     virtual AvnStatus download(AvnCcdResult* out) = 0;

@@ -325,7 +325,7 @@ AvnStatus Solver<S>::upload_resident(const AvnStepParams* prm, AvnBodyColumns* b
     if (ccd_active() && contacts->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "upload_resident: swept CCD is configured (avn_ccd_configure) and the contact store's shape column holds a "
                                                "capsule; capsule times of impact are not implemented");
-    if (ccd_active() && contacts->has_hull())
+    if (ccd_active() && contacts->has_hull() && !ccd_->hulls())
         return err_->fail(AVN_ERR_UNSUPPORTED, "upload_resident: swept CCD is configured (avn_ccd_configure) and the contact store's shape column holds a "
                                                "convex hull; hull times of impact are not implemented");
     ContactsBase::AsleepBodies asleep;
@@ -616,16 +616,19 @@ AvnStatus Solver<S>::run() {
     if (ccd_contacts_ && ccd_contacts_->has_capsule() && !ccd_->capsules())
         return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run: swept CCD is configured and the contact store's shape column holds a capsule; capsule "
                                                "times of impact are not implemented");
-    if (ccd_contacts_ && ccd_contacts_->has_hull())
+    if (ccd_contacts_ && ccd_contacts_->has_hull() && !ccd_->hulls())
         return err_->fail(AVN_ERR_UNSUPPORTED, "avn_solver_run: swept CCD is configured and the contact store's shape column holds a convex hull; hull "
                                                "times of impact are not implemented");
     if (!from_store_ || !ccd_contacts_)
         return err_->fail(AVN_ERR_UNSUPPORTED, "swept CCD is configured: it needs the contact store's ContactGraph (avn_solver_upload_resident), "
                                                "not host manifolds");
-    AvnStatus st = launch_range(0, uint32_t(dev_.substeps), AVN_RUN_PREPARE);
-    if (st != AVN_OK) return st;
     CcdRows rows;
     ccd_contacts_->ccd_rows(&rows);
+    if (ccd_->table_changed(rows))
+        return err_->fail(AVN_ERR_INVALID_ARGUMENT, "avn_solver_run: swept CCD would read the convex hull table, which avn_set_convex_hulls replaced after the last "
+                                                    "avn_contacts_step: step the contacts again");
+    AvnStatus st = launch_range(0, uint32_t(dev_.substeps), AVN_RUN_PREPARE);
+    if (st != AVN_OK) return st;
     CcdSolverState s;
     s.B = dev_.B; s.dt = double(dev_.dt); s.length_unit = length_unit_;
     s.kind = dev_.kind; s.position = dev_.position; s.rotation = dev_.rotation; s.com = dev_.com; s.vel = dev_.vel; s.dlt = dev_.dlt;

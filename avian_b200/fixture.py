@@ -104,6 +104,14 @@ def _load():
         lib.avh_ccd_pair_toi.restype = C.c_double
         lib.avh_ccd_nonlinear_toi.argtypes = [_vp, _vp, C.c_double, C.c_double, P(C.c_double), P(C.c_int)]
         lib.avh_ccd_nonlinear_toi.restype = C.c_int
+        lib.avh_ccd_solve_hulls.argtypes = lib.avh_ccd_solve.argtypes + [_vp]
+        lib.avh_ccd_solve_hulls.restype = C.c_int
+        lib.avh_ccd_pair_toi_hulls.argtypes = lib.avh_ccd_pair_toi.argtypes + [_vp]
+        lib.avh_ccd_pair_toi_hulls.restype = C.c_double
+        lib.avh_ccd_nonlinear_toi_hulls.argtypes = lib.avh_ccd_nonlinear_toi.argtypes + [_vp]
+        lib.avh_ccd_nonlinear_toi_hulls.restype = C.c_int
+        lib.avh_ccd_motion_radius.argtypes = [_vp, _vp]
+        lib.avh_ccd_motion_radius.restype = C.c_double
         lib.avh_ccd_apply_record.argtypes = [C.c_uint32, C.c_double, _vp, _vp, _vp, _vp]
         lib.avh_ccd_apply_record.restype = None
         _lib = lib
@@ -554,20 +562,36 @@ def ccd_motion(shape: int, dims, position, rotation, linear_velocity=(0, 0, 0), 
                            np.asarray(com, float).reshape(3), np.asarray(linear_velocity, float).reshape(3), np.asarray(angular_velocity, float).reshape(3)])
 
 
-def ccd_pair_toi(scalar, mode: int, a: np.ndarray, b: np.ndarray, dt: float, eps: float = 1e-4, prediction_distance: float = float("inf")) -> float:
-    """compute_ccd_toi of one pair against the bound dt, rounded to the column scalar (-1 = no hit)."""
+def ccd_pair_toi(scalar, mode: int, a: np.ndarray, b: np.ndarray, dt: float, eps: float = 1e-4, prediction_distance: float = float("inf"),
+                 hulls=None) -> float:
+    """compute_ccd_toi of one pair against the bound dt, rounded to the column scalar (-1 = no hit).  hulls: the hull table (HullTable or
+    api.ConvexHulls) that convex hull motions (shape 3, dims[0] = index) index; the shape level then includes hulls."""
     a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
-    return _load().avh_ccd_pair_toi(32 if np.dtype(scalar) == np.float32 else 64, int(mode), a.ctypes.data, b.ctypes.data, float(dt), float(eps),
-                                    float(prediction_distance))
+    bits = 32 if np.dtype(scalar) == np.float32 else 64
+    args = (bits, int(mode), a.ctypes.data, b.ctypes.data, float(dt), float(eps), float(prediction_distance))
+    if hulls is None:
+        return _load().avh_ccd_pair_toi(*args)
+    table = _hull_table(scalar, hulls)   # held until the call returns: the table is freed with it
+    return _load().avh_ccd_pair_toi_hulls(*args, table.h)
 
 
-def ccd_nonlinear_toi(a: np.ndarray, b: np.ndarray, t_max: float, eps: float = 1e-4, iterations: bool = False):
-    """The raw conservative-advancement TOI in double, or None; with iterations=True, (TOI or None, distance evaluations)."""
+def ccd_nonlinear_toi(a: np.ndarray, b: np.ndarray, t_max: float, eps: float = 1e-4, iterations: bool = False, hulls=None):
+    """The raw conservative-advancement TOI in double, or None; with iterations=True, (TOI or None, distance evaluations).  hulls: as
+    ccd_pair_toi (a table built from api.ConvexHulls keeps the vertices in double)."""
     a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
     t, its = C.c_double(), C.c_int(0)
-    hit = _load().avh_ccd_nonlinear_toi(a.ctypes.data, b.ctypes.data, float(t_max), float(eps), C.byref(t), C.byref(its))
+    args = (a.ctypes.data, b.ctypes.data, float(t_max), float(eps), C.byref(t), C.byref(its))
+    table = _hull_table(np.float64, hulls)
+    hit = _load().avh_ccd_nonlinear_toi(*args) if table is None else _load().avh_ccd_nonlinear_toi_hulls(*args, table.h)
     out = t.value if hit else None
     return (out, its.value) if iterations else out
+
+
+def ccd_motion_radius(a: np.ndarray, hulls=None) -> float:
+    """The spin bound R of one motion (its farthest point from the centre of mass, csrc/ccd_math.hpp motion_radius)."""
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    table = _hull_table(np.float64, hulls)
+    return _load().avh_ccd_motion_radius(a.ctypes.data, None if table is None else table.h)
 
 
 def ccd_apply_record(scalar, m: float, v, w, dp, dq):
@@ -578,12 +602,15 @@ def ccd_apply_record(scalar, m: float, v, w, dp, dq):
     return dp, dq
 
 
-def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, rows: dict, cfg: dict, delta_position=None, delta_rotation=None) -> dict:
+def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, rows: dict, cfg: dict, delta_position=None, delta_rotation=None,
+              hulls=None) -> dict:
     """solve_swept_ccd over the contact rows (dict c1, c2, b1, b2, live) by the reference's sequential loop.  bodies: dict kind, position,
     rotation, linear_velocity, angular_velocity (SolverBody velocities after the substeps), center_of_mass (optional).  cfg: the keyword
-    arguments of api.ccd_config, plus capsules=True for api.CCD_CAPSULES (as Context.ccd_configure takes it).  delta_position /
-    delta_rotation are updated in place when given.  Returns what Context.ccd_download returns."""
+    arguments of api.ccd_config, plus capsules=True for api.CCD_CAPSULES and hulls=True for api.CCD_HULLS (as Context.ccd_configure takes
+    them).  hulls: the hull table (HullTable or api.ConvexHulls) the hull colliders index.  delta_position / delta_rotation are updated in
+    place when given.  Returns what Context.ccd_download returns."""
     lib, dt_ = _load(), np.dtype(scalar)
+    hulls = _hull_table(dt_, hulls)
     col = lambda a, t=dt_: None if a is None else np.ascontiguousarray(a, dtype=t)
     kind = col(bodies.get("kind"), np.uint8)
     pos, rot, com, lv, av = (col(bodies.get(k)) for k in ("position", "rotation", "center_of_mass", "linear_velocity", "angular_velocity"))
@@ -592,19 +619,21 @@ def ccd_solve(scalar, dt: float, length_unit: float, bodies: dict, shape, dims, 
     c1, c2, b1, b2 = (col(rows[k], np.uint32) for k in ("c1", "c2", "b1", "b2"))
     live = col(rows["live"], np.uint8)
     cfg = dict(cfg)
-    cfg["flags"] = cfg.get("flags", 0) | (api.CCD_CAPSULES if cfg.pop("capsules", False) else 0)
+    cfg["flags"] = cfg.get("flags", 0) | (api.CCD_CAPSULES if cfg.pop("capsules", False) else 0) | (api.CCD_HULLS if cfg.pop("hulls", False) else 0)
     conf, keep = api.ccd_config(**cfg)
     n = int(conf.count)
     out = {"min_toi": np.zeros(n, dtype=dt_), "hit_body": np.zeros(n, dtype=np.int32), "hit_contact": np.zeros(n, dtype=np.int32),
            "candidates": np.zeros(n, dtype=np.uint32), "hits": np.zeros(n, dtype=np.uint32)}
     for a in (delta_position, delta_rotation):
         assert a is None or (a.dtype == dt_ and a.flags["C_CONTIGUOUS"])
-    st = lib.avh_ccd_solve(32 if dt_ == np.float32 else 64, float(dt), float(length_unit), B, _p(kind), _p(pos), _p(rot), _p(com), _p(lv), _p(av),
-                           _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
-                           *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
+    args = (32 if dt_ == np.float32 else 64, float(dt), float(length_unit), B, _p(kind), _p(pos), _p(rot), _p(com), _p(lv), _p(av),
+            _p(delta_position), _p(delta_rotation), _p(sh), _p(dm), int(c1.shape[0]), _p(c1), _p(c2), _p(b1), _p(b2), _p(live), C.byref(conf),
+            *(_p(out[k]) for k in ("min_toi", "hit_body", "hit_contact", "candidates", "hits")))
+    st = lib.avh_ccd_solve(*args) if hulls is None else lib.avh_ccd_solve_hulls(*args, hulls.h)
     if st == api.ERR_UNSUPPORTED:
         raise api.AvianError(st, "avh_ccd_solve: a contact row names a capsule and the configuration does not set CCD_CAPSULES, "
-                                 "or it names a convex hull")
+                                 "or a convex hull and it does not set CCD_HULLS")
     if st != 0:
-        raise ValueError("avh_ccd_solve: invalid configuration")
+        raise ValueError("avh_ccd_solve: invalid configuration (an unknown flag bit included), or a contact row names a convex hull the hull "
+                         "table does not hold")
     return out

@@ -1394,7 +1394,8 @@ ccd::Motion ccd_motion(const T* shape_dims, const uint8_t* shape, uint32_t c, co
 template <class T>
 int ccd_solve(double dt_d, double length_unit, uint32_t B, const uint8_t* kind, const T* pos, const T* rot, const T* com, const T* lv, const T* av, T* dpos,
               T* drot, const uint8_t* shape, const T* dims, uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2,
-              const uint8_t* live, const AvnCcdConfig* cfg, T* out_min, int32_t* out_body, int32_t* out_contact, uint32_t* out_cand, uint32_t* out_hits) {
+              const uint8_t* live, const AvnCcdConfig* cfg, T* out_min, int32_t* out_body, int32_t* out_contact, uint32_t* out_cand, uint32_t* out_hits,
+              const hm::Table* ht) {
     const T dt = T(dt_d);
     const S eps = ccd::CCD_EPS_PER_LENGTH_UNIT * length_unit;
     auto kind_of = [&](uint32_t b) { return kind ? kind[b] : uint8_t(AVN_BODY_DYNAMIC); };
@@ -1431,8 +1432,8 @@ int ccd_solve(double dt_d, double length_unit, uint32_t B, const uint8_t* kind, 
                 const int mode = (mode_of(k) == ccd::MODE_LINEAR && (it == slot_of_body.end() || mode_of(it->second) == ccd::MODE_LINEAR)) ? ccd::MODE_LINEAR
                                                                                                                                       : ccd::MODE_NON_LINEAR;
                 ++cand;
-                const T t = ccd::pair_toi<T, true>(mode, ccd_motion(dims, shape, own, pos, rot, com, v1, w1, body1),
-                                             ccd_motion(dims, shape, other, pos, rot, com, v2, w2, body2), dt, eps, cfg->prediction_distance);
+                const ccd::Motion A = ccd_motion(dims, shape, own, pos, rot, com, v1, w1, body1), Bm = ccd_motion(dims, shape, other, pos, rot, com, v2, w2, body2);
+                const T t = ht ? ccd::pair_toi<T, 2>(mode, A, Bm, dt, eps, cfg->prediction_distance, ht) : ccd::pair_toi<T, 1>(mode, A, Bm, dt, eps, cfg->prediction_distance);
                 if (t > T(0) && t < dt) ++hits;
                 if (t > T(0) && t < min_toi) { min_toi = t; hit = int32_t(body2); hit_row = int32_t(e); }
             }
@@ -1466,53 +1467,108 @@ ccd::Motion motion_from(const double* m) {   // shape, he[3], p[3], q[4], local 
     return r;
 }
 
+// avh_ccd_solve(_hulls): the refusals, then the loop (G = 2 with the table under AVN_CCD_HULLS, else G = 1)
+int ccd_solve_any(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position, const void* rotation,
+                  const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation, const uint8_t* shape, const void* dims,
+                  uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2, const uint8_t* live, const AvnCcdConfig* cfg,
+                  void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates, uint32_t* hits, const hm::HullSet* hulls) {
+    if (!cfg || (cfg->count && (!cfg->body || !cfg->collider))) return -1;
+    if (cfg->count && (cfg->flags & ~(AVN_CCD_CAPSULES | AVN_CCD_HULLS))) return AVN_ERR_INVALID_ARGUMENT;
+    // without AVN_CCD_CAPSULES a configuration with a row that names a capsule is refused, as the device refuses it
+    if (cfg->count && shape && !(cfg->flags & AVN_CCD_CAPSULES))
+        for (uint32_t r = 0; r < rows; ++r)
+            if ((!live || live[r]) && (shape[c1[r]] == SHAPE_CAPSULE || shape[c2[r]] == SHAPE_CAPSULE)) return AVN_ERR_UNSUPPORTED;
+    // the same for convex hulls without AVN_CCD_HULLS; with it, a row naming a hull the table does not hold (or no table) is refused, as the
+    // contact step refuses the column
+    const bool sweep_hulls = (cfg->flags & AVN_CCD_HULLS) != 0;
+    if (cfg->count && shape)
+        for (uint32_t r = 0; r < rows; ++r) {
+            if (live && !live[r]) continue;
+            for (const uint32_t c : {c1[r], c2[r]}) {
+                if (shape[c] != hm::SHAPE_CONVEX_HULL) continue;
+                if (!sweep_hulls) return AVN_ERR_UNSUPPORTED;
+                const double h = scalar_bits == 64 ? static_cast<const double*>(dims)[3 * size_t(c)] : double(static_cast<const float*>(dims)[3 * size_t(c)]);
+                if (!hulls || !(h >= 0 && h < double(hull_count(hulls))) || h != double(uint32_t(h))) return AVN_ERR_INVALID_ARGUMENT;
+            }
+        }
+    hm::Table t{};
+    if (hulls) t = hm::view(*hulls);
+    const hm::Table* ht = sweep_hulls && hulls ? &t : nullptr;
+    if (scalar_bits == 64)
+        return ccd_solve<double>(dt, length_unit, body_count, kind, static_cast<const double*>(position), static_cast<const double*>(rotation),
+                                 static_cast<const double*>(com), static_cast<const double*>(linvel), static_cast<const double*>(angvel),
+                                 static_cast<double*>(delta_position), static_cast<double*>(delta_rotation), shape, static_cast<const double*>(dims), rows, c1, c2,
+                                 b1, b2, live, cfg, static_cast<double*>(min_toi), hit_body, hit_contact, candidates, hits, ht);
+    return ccd_solve<float>(dt, length_unit, body_count, kind, static_cast<const float*>(position), static_cast<const float*>(rotation),
+                            static_cast<const float*>(com), static_cast<const float*>(linvel), static_cast<const float*>(angvel),
+                            static_cast<float*>(delta_position), static_cast<float*>(delta_rotation), shape, static_cast<const float*>(dims), rows, c1, c2, b1,
+                            b2, live, cfg, static_cast<float*>(min_toi), hit_body, hit_contact, candidates, hits, ht);
+}
+
 }  // namespace
 
 extern "C" {
 
 // solve_swept_ccd over the given contact rows.  Velocities: the SolverBody velocities after the substeps; delta_position / delta_rotation
-// ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration (an
-// unknown cfg->flags bit included) and AVN_ERR_UNSUPPORTED for a live row that names a capsule without AVN_CCD_CAPSULES, or a convex hull.  The geometry is
-// the CAPS = true instance either way: with no capsule in a pair it is the device's CAPS = false TOI, bit for bit.
+// ([B][3] / [B][4], in/out, may be NULL): the substeps' deltas, onto which the pass writes.  Returns -1 for an invalid configuration,
+// AVN_ERR_INVALID_ARGUMENT for an unknown cfg->flags bit, and AVN_ERR_UNSUPPORTED for a live row that names a capsule without
+// AVN_CCD_CAPSULES or a convex hull without AVN_CCD_HULLS.  The geometry is the G = 1 instance: with no capsule in a pair it is the device's
+// G = 0 TOI, bit for bit.
 int avh_ccd_solve(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position, const void* rotation,
                   const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation, const uint8_t* shape, const void* dims,
                   uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2, const uint8_t* live, const AvnCcdConfig* cfg,
                   void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates, uint32_t* hits) {
-    if (!cfg || (cfg->count && (!cfg->body || !cfg->collider))) return -1;
-    if (cfg->count && (cfg->flags & ~AVN_CCD_CAPSULES)) return AVN_ERR_INVALID_ARGUMENT;
-    // without AVN_CCD_CAPSULES a configuration with a row that names a capsule is refused, as the device refuses it
-    if (cfg->count && shape && !(cfg->flags & AVN_CCD_CAPSULES))
-        for (uint32_t r = 0; r < rows; ++r)
-            if ((!live || live[r]) && (shape[c1[r]] == SHAPE_CAPSULE || shape[c2[r]] == SHAPE_CAPSULE)) return AVN_ERR_UNSUPPORTED;
-    // convex hulls have no times of impact: a configuration with a row that names one is refused, flag or not, as the device refuses it
-    if (cfg->count && shape)
-        for (uint32_t r = 0; r < rows; ++r)
-            if ((!live || live[r]) && (shape[c1[r]] == hm::SHAPE_CONVEX_HULL || shape[c2[r]] == hm::SHAPE_CONVEX_HULL)) return AVN_ERR_UNSUPPORTED;
-    if (scalar_bits == 64)
-        return ccd_solve<double>(dt, length_unit, body_count, kind, static_cast<const double*>(position), static_cast<const double*>(rotation),
-                                 static_cast<const double*>(com), static_cast<const double*>(linvel), static_cast<const double*>(angvel),
-                                 static_cast<double*>(delta_position), static_cast<double*>(delta_rotation), shape, static_cast<const double*>(dims), rows, c1, c2,
-                                 b1, b2, live, cfg, static_cast<double*>(min_toi), hit_body, hit_contact, candidates, hits);
-    return ccd_solve<float>(dt, length_unit, body_count, kind, static_cast<const float*>(position), static_cast<const float*>(rotation),
-                            static_cast<const float*>(com), static_cast<const float*>(linvel), static_cast<const float*>(angvel),
-                            static_cast<float*>(delta_position), static_cast<float*>(delta_rotation), shape, static_cast<const float*>(dims), rows, c1, c2, b1,
-                            b2, live, cfg, static_cast<float*>(min_toi), hit_body, hit_contact, candidates, hits);
+    return ccd_solve_any(scalar_bits, dt, length_unit, body_count, kind, position, rotation, com, linvel, angvel, delta_position, delta_rotation, shape, dims,
+                         rows, c1, c2, b1, b2, live, cfg, min_toi, hit_body, hit_contact, candidates, hits, nullptr);
+}
+// The same with the fixture's hull table (avh_hulls_create, may be NULL).  Under AVN_CCD_HULLS with a table the geometry is the G = 2
+// instance, which gives the G = 1 bits on pairs without a hull; a live row naming a hull the table does not hold is AVN_ERR_INVALID_ARGUMENT.
+int avh_ccd_solve_hulls(uint32_t scalar_bits, double dt, double length_unit, uint32_t body_count, const uint8_t* kind, const void* position,
+                        const void* rotation, const void* com, const void* linvel, const void* angvel, void* delta_position, void* delta_rotation,
+                        const uint8_t* shape, const void* dims, uint32_t rows, const uint32_t* c1, const uint32_t* c2, const uint32_t* b1, const uint32_t* b2,
+                        const uint8_t* live, const AvnCcdConfig* cfg, void* min_toi, int32_t* hit_body, int32_t* hit_contact, uint32_t* candidates,
+                        uint32_t* hits, const void* hull_table) {
+    return ccd_solve_any(scalar_bits, dt, length_unit, body_count, kind, position, rotation, com, linvel, angvel, delta_position, delta_rotation, shape, dims,
+                         rows, c1, c2, b1, b2, live, cfg, min_toi, hit_body, hit_contact, candidates, hits, static_cast<const hm::HullSet*>(hull_table));
 }
 
 // One pair's compute_ccd_toi against the bound dt (ccd::pair_toi, fallback included), rounded to the column scalar and returned as a double;
 // -1 = no hit.  Motions: 20 doubles each (shape, half extents / radius / capsule radius and half length, position, rotation, local com,
 // linear and angular velocity).  Capsules (shape 2) are accepted.
 double avh_ccd_pair_toi(uint32_t scalar_bits, int mode, const double* a, const double* b, double dt, double eps, double prediction_distance) {
-    if (scalar_bits == 64) return ccd::pair_toi<double, true>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance);
-    return double(ccd::pair_toi<float, true>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance));
+    if (scalar_bits == 64) return ccd::pair_toi<double, 1>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance);
+    return double(ccd::pair_toi<float, 1>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance));
+}
+// The same at G = 2 with the fixture's hull table (convex hulls, shape 3, dims[0] = the hull index); NULL table: avh_ccd_pair_toi
+double avh_ccd_pair_toi_hulls(uint32_t scalar_bits, int mode, const double* a, const double* b, double dt, double eps, double prediction_distance,
+                              const void* hull_table) {
+    if (!hull_table) return avh_ccd_pair_toi(scalar_bits, mode, a, b, dt, eps, prediction_distance);
+    const hm::Table t = hm::view(*static_cast<const hm::HullSet*>(hull_table));
+    if (scalar_bits == 64) return ccd::pair_toi<double, 2>(mode, motion_from(a), motion_from(b), dt, eps, prediction_distance, &t);
+    return double(ccd::pair_toi<float, 2>(mode, motion_from(a), motion_from(b), float(dt), eps, prediction_distance, &t));
 }
 
 // The raw non-linear TOI in double (no rounding, no fallback): 1 and *toi on a hit, 0 otherwise; *iterations = distance evaluations.
 int avh_ccd_nonlinear_toi(const double* a, const double* b, double t_max, double eps, double* toi, int* iterations) {
     double t = 0;
-    const bool hit = ccd::nonlinear_toi<true>(motion_from(a), motion_from(b), t_max, eps, t, iterations);
+    const bool hit = ccd::nonlinear_toi<1>(motion_from(a), motion_from(b), t_max, eps, t, iterations);
     *toi = t;
     return hit ? 1 : 0;
+}
+// The same at G = 2 with the fixture's hull table; NULL table: avh_ccd_nonlinear_toi
+int avh_ccd_nonlinear_toi_hulls(const double* a, const double* b, double t_max, double eps, double* toi, int* iterations, const void* hull_table) {
+    if (!hull_table) return avh_ccd_nonlinear_toi(a, b, t_max, eps, toi, iterations);
+    const hm::Table t = hm::view(*static_cast<const hm::HullSet*>(hull_table));
+    double tt = 0;
+    const bool hit = ccd::nonlinear_toi<2>(motion_from(a), motion_from(b), t_max, eps, tt, iterations, &t);
+    *toi = tt;
+    return hit ? 1 : 0;
+}
+// test infrastructure: ccd::motion_radius of one motion (G = 2 with the table, G = 1 without)
+double avh_ccd_motion_radius(const double* m, const void* hull_table) {
+    if (!hull_table) return ccd::motion_radius<1>(motion_from(m));
+    const hm::Table t = hm::view(*static_cast<const hm::HullSet*>(hull_table));
+    return ccd::motion_radius<2>(motion_from(m), &t);
 }
 
 // Quat::from_scaled_axis and the delta write of one record, in the column scalar (tests)

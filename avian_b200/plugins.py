@@ -193,7 +193,7 @@ class World:
     def __init__(self, scene: Scene, plugins: PhysicsPlugins, dt: float = 1.0 / 60.0, substeps: int = 6, solver_iterations: int = 1,
                  ccd: dict | None = None, sensor=None, events_enabled=None):
         """ccd: the SweptCcd bodies — the keyword arguments of api.Context.ccd_configure (body, collider, mode, include_dynamic,
-        linear_threshold, angular_threshold, prediction_distance, capsules).  The solver plugin must run solve_swept_ccd (a `step_ccd` method).
+        linear_threshold, angular_threshold, prediction_distance, capsules, hulls).  The solver plugin must run solve_swept_ccd (a `step_ccd` method).
         sensor / events_enabled: optional per-collider columns (Sensor, CollisionEventsEnabled).  After every step `events` holds the
         (started, ended) lists of api.Context.contacts_events (DeviceGraphWorld: when either column is given)."""
         self.scene = scene

@@ -376,7 +376,7 @@ AvnStatus avn_broadphase_download(AvnContext* ctx, AvnPairList* out_pairs);
  * AVN_SHAPE_CONVEX_HULL: Collider::convex_hull / the parts of Collider::convex_decomposition, dims = [hull index, unused, unused] into the
  * context's hull table (avn_set_convex_hulls).  The index is stored in the column scalar: integral, non-negative and below the table's hull
  * count.  The AABB update, the narrow phase, the contact store, the spatial queries (colliders and query shapes) and move and slide (obstacles
- * and characters) take hulls; swept CCD returns AVN_ERR_UNSUPPORTED while the contact store holds one. */
+ * and characters) and swept CCD (with AVN_CCD_HULLS) take hulls. */
 typedef enum AvnShape { AVN_SHAPE_CUBOID = 0, AVN_SHAPE_SPHERE = 1, AVN_SHAPE_CAPSULE = 2, AVN_SHAPE_CONVEX_HULL = 3 } AvnShape;
 
 /* ---- convex hulls: the table AVN_SHAPE_CONVEX_HULL colliders index (parry's ConvexPolyhedron: points, faces as vertex loops) ---------- */
@@ -950,8 +950,9 @@ AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const
  *      order of the configured list, so a body hit by several CCD bodies ends with the last one's delta_position.
  *      Assumptions, as the narrow phase makes them: a collider sits at its body's origin and its pose is the body's pose before the step; the
  *      body columns and the collider rows of the contact pipeline (avn_contacts_configure / avn_contacts_step) describe the same bodies.
- *      Geometry: cuboid and sphere colliders, and capsules with AVN_CCD_CAPSULES; conventions in avian_b200/csrc/ccd_math.hpp (linear: the
- *      shape casts of the spatial queries; non-linear: conservative advancement to eps = 1e-4 * length_unit, at most 64 iterations).
+ *      Geometry: cuboid and sphere colliders, capsules with AVN_CCD_CAPSULES and convex hulls with AVN_CCD_HULLS; conventions in
+ *      avian_b200/csrc/ccd_math.hpp (linear: the shape casts of the spatial queries; non-linear: conservative advancement to
+ *      eps = 1e-4 * length_unit, at most 64 iterations).
  *      Stated deviation: equal TOIs go to the lowest ContactId, where the reference keeps the first in ContactGraph adjacency order.
  *      Runs inside avn_solver_run when the upload came from the contact store (avn_solver_upload_resident): the step becomes
  *      prepare + substeps -> CCD pass -> restitution + finalize.  While CCD is configured, avn_solver_run_range,
@@ -959,6 +960,7 @@ AvnStatus avn_move_and_slide(AvnContext* ctx, const AvnMoveConfig* config, const
 typedef enum AvnSweepMode { AVN_SWEEP_LINEAR = 0, AVN_SWEEP_NON_LINEAR = 1 } AvnSweepMode;
 
 #define AVN_CCD_CAPSULES 0x1u           /* AvnCcdConfig.flags: capsule colliders take part (see avn_ccd_configure) */
+#define AVN_CCD_HULLS 0x4u              /* AvnCcdConfig.flags: convex hull colliders take part (see avn_ccd_configure) */
 
 typedef struct AvnCcdConfig {
     uint32_t count;                    /* SweptCcd bodies, in query order */
@@ -983,10 +985,15 @@ typedef struct AvnCcdResult {          /* per configured body, the last step's p
 } AvnCcdResult;
 
 /* Persists across steps; NULL or count == 0 clears it.  Needs avn_contacts_configure first (bodies and colliders are checked against its counts).
- * Refused with AVN_ERR_INVALID_ARGUMENT: a flag bit other than AVN_CCD_CAPSULES, bodies or colliders out of range, a body listed twice, NaN
- * thresholds, an unknown mode.  Capsules: without AVN_CCD_CAPSULES, a contact store whose shape column holds a capsule is refused with
- * AVN_ERR_UNSUPPORTED here, and so are avn_solver_upload_resident and avn_solver_run once a later avn_contacts_step brings one in.  With it,
- * capsules are swept like the other shapes (exact capsule casts in Linear mode, exact capsule distances in NonLinear mode). */
+ * Refused with AVN_ERR_INVALID_ARGUMENT: a flag bit other than AVN_CCD_CAPSULES and AVN_CCD_HULLS, bodies or colliders out of range, a body
+ * listed twice, NaN thresholds, an unknown mode.  Capsules: without AVN_CCD_CAPSULES, a contact store whose shape column holds a capsule is
+ * refused with AVN_ERR_UNSUPPORTED here, and so are avn_solver_upload_resident and avn_solver_run once a later avn_contacts_step brings one
+ * in.  With it, capsules are swept like the other shapes (exact capsule casts in Linear mode, exact capsule distances in NonLinear mode).
+ * Convex hulls: the same with AVN_CCD_HULLS, independently of AVN_CCD_CAPSULES (a store holding both shapes needs both bits).  With it, hulls
+ * are swept with the exact hull casts of the spatial queries (Linear) and exact hull distances (NonLinear) over the context's hull table.
+ * The pass reads the table the last avn_contacts_step used: once avn_set_convex_hulls has replaced it, avn_solver_run returns
+ * AVN_ERR_INVALID_ARGUMENT before launching anything while the store holds a hull, until the next avn_contacts_step.  Body frames stay
+ * refused whatever the flags. */
 AvnStatus avn_ccd_configure(AvnContext* ctx, const AvnCcdConfig* config);
 /* The results of the last step that ran the pass (AVN_ERR_INVALID_ARGUMENT before any). */
 AvnStatus avn_ccd_download(AvnContext* ctx, AvnCcdResult* out);
